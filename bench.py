@@ -2,6 +2,7 @@
 """bench.py — the measured headline of this repository.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--mnk M_N_K] [--acc fp32|fp16] [--impl ours|reference]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 Metric (BASELINE.json): HGEMM TFLOP/s, offline mode (back-to-back calls), per (M,N,K). One "step" is ONE
@@ -12,11 +13,15 @@ GEMM of the workload shape through the C ABI (libb200_hgemm.so). Default workloa
 What is timed
   value   K steps with operands resident in HBM, CUDA events on the launching (legacy default) stream, bracketed
           by barrier + device synchronize, MAX over ranks; FLOPs = 2*M*N*K per step per rank (unpadded).
-          Successive steps rotate over operand sets whose total size exceeds the 126 MB L2 several times.
+          Successive steps rotate over operand sets whose total size exceeds the 50 MB L2 several times.
+          --dump-outputs DIR writes C of the last timed step as DIR/c.npy (float32; above 4M elements, a fixed seeded
+          sample of its rows, indices in DIR/c_rows.npy as float64). Operands are seeded, so two builds of the project
+          run with the same arguments can be compared output for output.
   e2e     the same GEMM through b200_hgemm_host(): pinned HOST buffers, H2D of A and B + kernel + D2H of C inside
           the timed region every step.
   roofline  achieved = 2MNK / (average kernel duration from the same CUDA events); peak = measured cuBLAS bf16
-          burst TFLOP/s from MEASURED_PEAKS.json (fallback 1590, said so in `peak_source`).
+          burst TFLOP/s from MEASURED_PEAKS.json (fallback: the H100 SXM data sheet's dense fp16 989 TFLOP/s and
+          3.35 TB/s, said so in `peak_source`).
   cpu_baseline  the reference's CPU path, verbatim: torch.matmul(a.float(), b.float()).half() on the host cores
           (zero_one_correctness_check.py:87-90), a bounded ~10 s sample of the same shape, rank 0, N=1 only.
   --impl reference   times that same CPU path as the whole job (the reference has no other CPU implementation
@@ -50,8 +55,9 @@ sys.path.insert(0, str(REPO))
 
 import torch  # noqa: E402
 
-L2_BYTES = 126 * 1024 * 1024
-FALLBACK_TFLOPS, FALLBACK_HBM = 1590.0, 6650.0
+L2_BYTES = 50 * 1024 * 1024
+FALLBACK_TFLOPS, FALLBACK_HBM = 989.0, 3350.0
+DUMP_MAX_ELEMS = 1 << 22          # --dump-outputs: larger outputs are row-sampled to this many elements
 
 
 def parse_args():
@@ -68,6 +74,8 @@ def parse_args():
     p.add_argument("--sweep", type=str, default="grid", help="'grid' (1001 shapes), 'none', or a comma list of M_N_K")
     p.add_argument("--sweep_ms", type=float, default=25.0, help="sampling budget per shape of the sweep leg")
     p.add_argument("--cpu_threads", type=int, default=0, help="threads of the CPU arms (0 = half the host's logical CPUs)")
+    p.add_argument("--dump-outputs", dest="dump_outputs", type=str, default=None,
+                   help="directory: write C of the last timed step there as .npy (float32, seeded row sample if large)")
     return p.parse_args()
 
 
@@ -80,7 +88,7 @@ def peaks():
                     float(d.get("bf16_tflops_sustained", 0.0)) or None)
         except Exception:
             pass
-    return FALLBACK_TFLOPS, FALLBACK_HBM, "fallback (B200_PROFILING.md)", 1400.0
+    return FALLBACK_TFLOPS, FALLBACK_HBM, "fallback (NVIDIA H100 SXM data sheet, dense fp16, 700 W)", None
 
 
 class ClockSampler:
@@ -202,6 +210,21 @@ def cpu_baseline(m, n, k, seconds: float, threads: int) -> dict:
     return {"value": tf, "unit": "TFLOP/s", "cores": cores, "host_cpus": os.cpu_count(),
             "kind": "reference",
             "sample": f"{reps} x torch.matmul(a.cpu().float(), b.cpu().float()).half() at {m}x{n}x{k} in {el:.1f} s on {cores} threads"}
+
+
+def dump_outputs(out_dir: str, c: torch.Tensor) -> None:
+    """C as the caller receives it, as float32; above DUMP_MAX_ELEMS a fixed seeded sample of whole rows."""
+    import numpy as np
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    m, n = c.shape
+    host = c.float().cpu().numpy()
+    if m * n > DUMP_MAX_ELEMS:
+        rows = np.sort(np.random.default_rng(0).choice(m, size=max(1, DUMP_MAX_ELEMS // n), replace=False))
+        host = host[rows]
+        np.save(d / "c_rows.npy", rows.astype(np.float64))
+    np.save(d / "c.npy", np.ascontiguousarray(host, dtype=np.float32))
 
 
 def run_reference(args, m, n, k, rank, world):
@@ -357,7 +380,7 @@ def main():
     from cuda_l2_b200 import capi
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the HGEMM path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: the HGEMM path has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -411,6 +434,8 @@ def main():
     barrier()
     launches = capi.launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None      # the clock record of the region `value` is computed from
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, sets[(args.steps - 1) % nsets][2])
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     if dist is not None:
         lt = torch.tensor([launches], device="cuda", dtype=torch.int64)
@@ -495,7 +520,7 @@ def main():
             "dtype": "f16 x f16 -> " + ("f32" if args.acc == "fp32" else "f16") + " accumulate -> f16",
             "data": "synthetic N(0,1) fp16",
             "config": {"workload": f"{args.mnk} --acc_precise {args.acc} --mode offline", "parallelism": f"1 GEMM per GPU x {world}",
-                       "l2_policy": f"rotating {nsets} operand sets ({nsets * set_bytes >> 20} MiB > 126 MiB L2)",
+                       "l2_policy": f"rotating {nsets} operand sets ({nsets * set_bytes >> 20} MiB > 50 MiB L2)",
                        "kernel_config": {"tile": f"{128 * cfg['cta_group'] * cfg.get('m_rep', 1)}x{cfg['bn']}x64", "stages": cfg["stages"],
                                          "cta_group": cfg["cta_group"], "cluster": f"{cfg['cluster_m']}x{cfg['cluster_n']}", "group_m": group_m,
                                          "split_k": splits}},

@@ -1,6 +1,6 @@
-"""In-tree builds of the native pieces (nvcc cross-compiles sm_100a without a GPU).
+"""In-tree builds of the native pieces (nvcc cross-compiles sm_90a without a GPU).
 
-Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored, shipped to the GPU box by gpurun):
+Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
 
 * ``libb200_hgemm.so``  — the C-ABI product library (include/b200_hgemm.h)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
@@ -21,14 +21,14 @@ REPO = PKG_DIR.parent
 CSRC = PKG_DIR / "csrc"
 LIB_DIR = PKG_DIR / "lib"
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fno-gnu-unique"]
 
 
 def nvcc_path() -> str:
     cand = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not Path(cand).exists():
-        raise RuntimeError("nvcc not found: the B200 HGEMM library cannot be built")
+        raise RuntimeError("nvcc not found: the HGEMM library cannot be built")
     return cand
 
 
@@ -48,6 +48,12 @@ def _run(cmd: list[str], verbose: bool) -> None:
         raise RuntimeError(f"build step failed ({r.returncode}): {' '.join(cmd)}")
     if verbose and r.stdout.strip():
         print(r.stdout)
+    elif "warning" in r.stdout.lower():
+        sys.stderr.write(r.stdout)   # compiler warnings are always shown
+    # C7510: ptxas serialised the wgmma pipeline (a function call or a non-inlined boundary inside the MMA loop). The
+    # kernels are still correct but lose the overlap of consecutive wgmma groups, so such a build is refused.
+    if "C7510" in r.stdout:
+        raise RuntimeError(f"ptxas serialised wgmma (warning C7510) in: {' '.join(cmd)}")
 
 
 def _headers() -> list[Path]:
@@ -104,29 +110,9 @@ def build_variant(name: str, defines: list[str], verbose: bool = False, force: b
     return out
 
 
-def build_trace(verbose: bool = False, force: bool = False) -> Path:
-    """Per-CTA phase timestamps (-DB200_HGEMM_TRACE): libb200_hgemm_trace.so + dev_check_trace."""
-    return build_variant("trace", ["B200_HGEMM_TRACE"], verbose, force)
-
-
-def build_early_tma(verbose: bool = False, force: bool = False) -> Path:
-    """First TMA ring issued before the set-up barrier (-DB200_HGEMM_EARLY_TMA=1): the fixed-cost experiment."""
-    return build_variant("early", ["B200_HGEMM_EARLY_TMA=1"], verbose, force)
-
-
-def build_split_setup(verbose: bool = False, force: bool = False) -> Path:
-    """TMEM allocation behind the first set-up barrier, producer not waiting for it (-DB200_HGEMM_SPLIT_SETUP=1)."""
-    return build_variant("split", ["B200_HGEMM_SPLIT_SETUP=1"], verbose, force)
-
-
 def build_no_k_decomp(verbose: bool = False, force: bool = False) -> Path:
     """Kernels without split-K / stream-K code (-DB200_HGEMM_NO_K_DECOMP=1): what does that code cost the plain path?"""
     return build_variant("plain", ["B200_HGEMM_NO_K_DECOMP=1"], verbose, force)
-
-
-def build_wait_hint(ns: int = 2000, verbose: bool = False, force: bool = False) -> Path:
-    """mbarrier.try_wait with a suspend-time hint (-DB200_HGEMM_WAIT_HINT_NS): the polling-power experiment."""
-    return build_variant("hint", [f"B200_HGEMM_WAIT_HINT_NS={ns}"], verbose, force)
 
 
 def build_all(verbose: bool = False, force: bool = False) -> dict[str, Path]:

@@ -4,7 +4,7 @@ This is the Python face of the drop-in boundary: the same entry points the torch
 (``pybind/hgemm_b200_fp32.cc`` / ``hgemm_b200_fp16.cc``) wraps, reachable without a JIT build.  Tensors
 are torch CUDA tensors used purely as device-memory handles (``data_ptr()``); all arithmetic happens in
 ``libb200_hgemm.so``.  There is no CPU or PyTorch fallback: if the library is missing or the device is
-not a B200, these functions raise.
+not an H100, these functions raise.
 """
 from __future__ import annotations
 
@@ -46,6 +46,7 @@ def hgemm_lib() -> ctypes.CDLL:
         lib.b200_hgemm_config_info.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
         lib.b200_hgemm_config_cluster.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(i)]
         lib.b200_hgemm_config_m_rep.argtypes = [i]
+        lib.b200_hgemm_config_stages_requested.argtypes = [i]
         lib.b200_hgemm_select_config.argtypes = [i, i, i, i]
         lib.b200_hgemm_select.argtypes = [i, i, i, i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
         lib.b200_hgemm_run_config.argtypes = [i, i, vp, vp, vp, i, i, i, i, i, i, vp]
@@ -83,7 +84,7 @@ def exported_symbols() -> dict[str, list[str]]:
     return {
         "libb200_hgemm.so": [
             "b200_hgemm_f32acc", "b200_hgemm_f16acc", "b200_hgemm_num_configs", "b200_hgemm_config_info",
-            "b200_hgemm_config_cluster", "b200_hgemm_config_m_rep",
+            "b200_hgemm_config_cluster", "b200_hgemm_config_m_rep", "b200_hgemm_config_stages_requested",
             "b200_hgemm_select_config", "b200_hgemm_select", "b200_hgemm_run_config", "b200_hgemm_host", "b200_hgemm_launch_count",
             "b200_hgemm_strerror", "b200_hgemm_schedule_units", "b200_hgemm_prewarm", "b200_hgemm_release",
             "b200_bgemm_f32acc", "b200_bgemm_run_config",
@@ -190,6 +191,7 @@ def configs() -> list[dict]:
         cm, cn = ctypes.c_int(), ctypes.c_int()
         lib.b200_hgemm_config_cluster(cid, ctypes.byref(cm), ctypes.byref(cn))
         out.append({"id": cid, "bn": bn.value, "stages": st.value, "cta_group": cg.value,
+                    "stages_requested": lib.b200_hgemm_config_stages_requested(cid),
                     "cluster_m": cm.value, "cluster_n": cn.value, "m_rep": lib.b200_hgemm_config_m_rep(cid)})
     return out
 
@@ -209,7 +211,7 @@ def select(acc: str | int, m: int, n: int, k: int) -> tuple[int, int, int]:
 STREAMK_TAIL, STREAMK_TAIL_PLUS_WAVE = 100, 101      # `splits` codes of b200_hgemm_run_config
 
 
-def schedule(config_id: int, m: int, n: int, k: int, splits: int = 1, num_sms: int = 148) -> dict:
+def schedule(config_id: int, m: int, n: int, k: int, splits: int = 1, num_sms: int = 132) -> dict:
     """Host-side view of the kernel's schedule (no GPU needed; the kernel walks the same code).
 
     Returns ``{"workers": W, "sk_tiles": S, "units": [[(tile, kb0, kb1, contributors), ...] per worker]}``."""

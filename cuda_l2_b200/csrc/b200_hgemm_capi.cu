@@ -14,6 +14,9 @@
 namespace {
 
 std::atomic<unsigned long long> g_launches{0};
+// the ring depth a configuration runs with (its requested depth, capped by shared memory)
+template <class Cfg>
+constexpr int ring_depth() { return Cfg::STAGES; }
 constexpr int kBf16Acc32 = 0xB32;   // internal selector of run(): bf16 operands, fp32 accumulation
 
 template <bool kAccF32, bool kBf16 = false>
@@ -94,7 +97,7 @@ int b200_hgemm_config_info(int config_id, int* bn, int* stages, int* cta_group) 
 #define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)  \
   case ID:                             \
     if (bn) *bn = BN;                  \
-    if (stages) *stages = STAGES;      \
+    if (stages) *stages = ring_depth<b200::Config<BN, STAGES, CG, true, CM, CN, MR>>();   \
     if (cta_group) *cta_group = CG;    \
     return 0;
     B200_HGEMM_CONFIGS(B200_CASE)
@@ -126,6 +129,18 @@ int b200_hgemm_schedule_units(int config_id, int M, int N, int K, int splits, in
   case ID:                                                                                                          \
     return schedule_units<b200::Config<BN, STAGES, CG, true, CM, CN, MR>>(M, N, K, splits, num_sms, worker, units, \
                                                                           max_units, num_workers, sk_tiles, contributors);
+    B200_HGEMM_CONFIGS(B200_CASE)
+#undef B200_CASE
+    default:
+      return b200::host::kBadConfig;
+  }
+}
+
+int b200_hgemm_config_stages_requested(int config_id) {
+  switch (config_id) {
+#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR) \
+  case ID:                                        \
+    return STAGES;
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE
     default:
@@ -308,35 +323,6 @@ int b200_hgemm_release(void) {
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : int(e);
 }
-
-#ifdef B200_HGEMM_TRACE
-// Developer-only entry points of libb200_hgemm_trace.so (see kTraceSlots in hgemm_sm100.cuh); not part of the C ABI.
-static unsigned long long* g_trace_dev = nullptr;
-static int g_trace_ctas = 0;
-int b200_hgemm_trace_slots(void) { return b200::kTraceSlots; }
-int b200_hgemm_trace_arm(int max_ctas) {   // zero the buffer and point the kernels at it (max_ctas <= 0: disarm)
-  unsigned long long* none = nullptr;
-  if (max_ctas <= 0) return int(cudaMemcpyToSymbol(b200::g_trace_buf, &none, sizeof(none)));
-  const size_t bytes = size_t(max_ctas) * b200::kTraceSlots * 2 * sizeof(unsigned long long);
-  if (max_ctas > g_trace_ctas) {
-    if (g_trace_dev) cudaFree(g_trace_dev);
-    g_trace_dev = nullptr; g_trace_ctas = 0;
-    cudaError_t e = cudaMalloc(&g_trace_dev, bytes);
-    if (e != cudaSuccess) return int(e);
-    g_trace_ctas = max_ctas;
-  }
-  cudaError_t e = cudaMemset(g_trace_dev, 0, bytes);
-  if (e != cudaSuccess) return int(e);
-  return int(cudaMemcpyToSymbol(b200::g_trace_buf, &g_trace_dev, sizeof(g_trace_dev)));
-}
-int b200_hgemm_trace_read(unsigned long long* out, int ctas) {
-  if (!g_trace_dev || ctas > g_trace_ctas) return b200::host::kBadShape;
-  cudaError_t e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) return int(e);
-  return int(cudaMemcpy(out, g_trace_dev, size_t(ctas) * b200::kTraceSlots * 2 * sizeof(unsigned long long),
-                        cudaMemcpyDeviceToHost));
-}
-#endif
 
 unsigned long long b200_hgemm_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 

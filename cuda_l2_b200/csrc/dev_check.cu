@@ -8,7 +8,6 @@
 //   dev_check wall  <acc_bits> <M> <N> <K> [seconds [tune_warm tune_bench]]  the harness's protocol (one baseline/ours pair at a time,
 //                                                     fresh operands per iteration, zero-filled output) vs 6 library baselines
 //   dev_check wallgrid <acc_bits> <part> <nparts> [seconds tune_warm tune_bench limit]   `wall` over a share of the grid
-//   dev_check_trace trace <acc_bits> <cfg|-1> <M> <N> <K> [gm splits cold]   per-CTA phase timestamps of one launch (trace build only)
 //   dev_check grid  <acc_bits> [part nparts budget_ms min_gflop max_gflop [wall]]  time every config on the whole shape grid (CSV);
 //                                                     "wall": rank by the harness metric instead of CUDA-event time
 //
@@ -397,22 +396,22 @@ static int do_grid(int acc, int part, int nparts, double budget_ms, double min_g
       const int nm = (p.M + 128 * cg * cm * mr - 1) / (128 * cg * cm * mr);
       const int nn = (p.N + bn * cn - 1) / (bn * cn);
       std::vector<std::pair<int, int>> cands = {{0, 1}};   // (group_m, splits)
-      if (nm * nn > 148 / (cg * cm * cn) && nm > 1 && nn > 1) {
+      if (nm * nn > 132 / (cg * cm * cn) && nm > 1 && nn > 1) {
         cands = {{1, 1}, {4, 1}, {8, 1}, {16, 1}};
         if (nm >= 32) cands.push_back({32, 1});
       }
       const int nkb = (p.K + 63) / 64;
-      if (plain && cg == 1 && nm * nn * 2 <= 148 && nkb >= 4)
+      if (plain && cg == 1 && nm * nn * 2 <= 132 && nkb >= 4)
         for (int sp : {2, 3, 4, 6, 8, 12, 16, 24, 32})
-          if (sp <= 148 / (nm * nn) && sp <= nkb) cands.push_back({0, sp});
-      if (plain && cg == 1 && nkb >= 8 && nm * nn <= 148)
+          if (sp <= 132 / (nm * nn) && sp <= nkb) cands.push_back({0, sp});
+      if (plain && cg == 1 && nkb >= 8 && nm * nn <= 132)
         for (int cs : {2, 4, 8})
-          if (nm * nn * cs <= 296 && nkb >= 2 * cs) cands.push_back({0, -cs});   // cluster (DSMEM) split-K
+          if (nm * nn * cs <= 2 * 132 && nkb >= 2 * cs) cands.push_back({0, -cs});   // cluster (DSMEM) split-K
       // stream-K (splits code 100: the partial last wave, 101: that plus one full wave) where the tile count leaves
       // more than 5 % of the last wave empty
       // (round 2: in the harness's synchronised-call metric stream-K won 41 of the 51 tensor-bound shapes it was tuned
       //  into, also where the last wave is nearly full, so it is a candidate wherever the tile count is not a wave multiple)
-      const int workers = 148 / cg;
+      const int workers = 132 / cg;
       if (plain && (nm * nn) % workers != 0 && nkb >= 8) {
         const std::vector<int> sk_gms = (nm * nn > workers && nm > 1 && nn > 1) ? std::vector<int>{4, 16} : std::vector<int>{0};
         for (int g : sk_gms) {
@@ -516,79 +515,6 @@ static int do_grid(int acc, int part, int nparts, double budget_ms, double min_g
 }
 
 
-#ifdef B200_HGEMM_TRACE
-// trace (dev_check_trace only, linked against libb200_hgemm_trace.so): where one launch spends its time, from
-// per-CTA timestamps written by the instrumented kernel (slots documented next to kTraceSlots in hgemm_sm100.cuh).
-extern "C" int b200_hgemm_trace_slots(void);
-extern "C" int b200_hgemm_trace_arm(int max_ctas);
-extern "C" int b200_hgemm_trace_read(unsigned long long* out, int ctas);
-
-// cold != 0: before the traced launch, other work (a cuBLAS GEMM on other operands, 512 MB of memset) evicts this
-// kernel's instructions, descriptors and operands from the caches and the TLBs — the state every call of the
-// harness's rotation starts from, as opposed to the back-to-back state of `dev_check time`.
-static int do_trace(int acc, int cfg, int M, int N, int K, int gm, int splits, int cold) {
-  Problem p; alloc_random(p, M, N, K);
-  for (int i = 0; i < 3; ++i) if (run_ours(acc, cfg, p, gm, splits)) { printf("TRACE launch failed\n"); return 1; }
-  CK(cudaDeviceSynchronize());
-  if (cold) {
-    Problem other; alloc_random(other, 2048, 2048, 2048);
-    void* scratch; const size_t bytes = size_t(512) << 20;
-    CK(cudaMalloc(&scratch, bytes));
-    for (int i = 0; i < 2; ++i) { cublas_tn(other, other.Cref); CK(cudaMemsetAsync(scratch, i, bytes)); }
-    CK(cudaDeviceSynchronize());
-    cudaFree(scratch);
-    other.release();
-  }
-  const int kMaxCtas = 320, S = b200_hgemm_trace_slots();
-  if (b200_hgemm_trace_arm(kMaxCtas)) { printf("TRACE arm failed\n"); return 1; }
-  if (run_ours(acc, cfg, p, gm, splits)) { printf("TRACE launch failed\n"); return 1; }
-  std::vector<unsigned long long> buf(size_t(kMaxCtas) * S * 2);
-  if (b200_hgemm_trace_read(buf.data(), kMaxCtas)) { printf("TRACE read failed\n"); return 1; }
-  b200_hgemm_trace_arm(0);
-  auto gt = [&](int cta, int slot) { return double(buf[(size_t(cta) * S + slot) * 2]); };          // ns
-  auto ck = [&](int cta, int slot) { return double(buf[(size_t(cta) * S + slot) * 2 + 1]); };      // SM cycles
-  int ctas = 0;
-  double t0 = 1e300, t_end = 0;
-  for (int c = 0; c < kMaxCtas; ++c) if (gt(c, 0) > 0) { ctas = c + 1; t0 = std::min(t0, gt(c, 0)); t_end = std::max(t_end, gt(c, 8)); }
-  if (!ctas) { printf("TRACE: no CTA wrote a timestamp\n"); return 1; }
-  struct Row { const char* name; std::vector<double> v; };
-  std::vector<Row> rows = {{"entry after first CTA [us]", {}}, {"setup (entry -> barrier) [us]", {}},
-                           {"entry -> first TMA issued [us]", {}}, {"entry -> first stage landed [us]", {}},
-                           {"main loop: first stage landed -> last accumulator complete [us]", {}},
-                           {"MMA issue: cycles per k-block", {}}, {"MMA issue: ns per k-block", {}},
-                           {"producer finished before last accumulator by [us]", {}},
-                           {"tail: last accumulator complete -> epilogue drained [us]", {}},
-                           {"teardown: epilogue drained -> after last barrier [us]", {}},
-                           {"CTA lifetime [us]", {}}, {"k-blocks issued", {}}, {"units", {}}};
-  for (int c = 0; c < ctas; ++c) {
-    if (gt(c, 0) == 0) continue;
-    rows[0].v.push_back((gt(c, 0) - t0) * 1e-3);
-    rows[1].v.push_back((gt(c, 1) - gt(c, 0)) * 1e-3);
-    if (gt(c, 2) > 0) rows[2].v.push_back((gt(c, 2) - gt(c, 0)) * 1e-3);
-    if (gt(c, 4) > 0) {   // leader CTAs only (the MMA issuer)
-      rows[3].v.push_back((gt(c, 4) - gt(c, 0)) * 1e-3);
-      if (gt(c, 10) > 0) rows[4].v.push_back((gt(c, 10) - gt(c, 4)) * 1e-3);
-      const double kb = gt(c, 9);
-      if (kb > 0) { rows[5].v.push_back((ck(c, 5) - ck(c, 4)) / kb); rows[6].v.push_back((gt(c, 5) - gt(c, 4)) / kb); }
-      rows[11].v.push_back(kb); rows[12].v.push_back(gt(c, 11));
-    }
-    if (gt(c, 3) > 0 && gt(c, 10) > 0) rows[7].v.push_back((gt(c, 10) - gt(c, 3)) * 1e-3);
-    if (gt(c, 7) > 0 && gt(c, 10) > 0) rows[8].v.push_back((gt(c, 7) - gt(c, 10)) * 1e-3);
-    if (gt(c, 7) > 0) rows[9].v.push_back((gt(c, 8) - gt(c, 7)) * 1e-3);
-    rows[10].v.push_back((gt(c, 8) - gt(c, 0)) * 1e-3);
-  }
-  int sel = cfg < 0 ? b200_hgemm_select_config(acc, M, N, K) : cfg;
-  printf("TRACE acc=%d cfg=%d(%d) gm=%d splits=%d %s %dx%dx%d  ctas=%d  first entry -> last exit %.2f us\n", acc, cfg, sel, gm, splits,
-         cold ? "COLD" : "warm", M, N, K, ctas, (t_end - t0) * 1e-3);
-  for (auto& r : rows) {
-    if (r.v.empty()) continue;
-    std::sort(r.v.begin(), r.v.end());
-    printf("  %-72s min %10.2f  median %10.2f  max %10.2f  (n=%zu)\n", r.name, r.v.front(), r.v[r.v.size() / 2], r.v.back(), r.v.size());
-  }
-  p.release();
-  return 0;
-}
-#endif
 
 // wall: the harness's measurement PROTOCOL in C++ (reference benchmarking_offline.py:119-161, benchmarking_utils.py:12-69;
 // eval_one_file.sh:71-135), one (baseline, ours) pair at a time as the reference runs one pair per process:
@@ -786,11 +712,6 @@ int main(int argc, char** argv) {
                       argc > 8 ? atoi(argv[8]) : 0, argc > 9 ? atoi(argv[9]) : 1);
   if (mode == "sweep" && argc >= 6)
     return do_sweep(atoi(argv[2]), atoi(argv[3]), atoi(argv[4]), atoi(argv[5]), argc > 6 ? atoi(argv[6]) : 20);
-#ifdef B200_HGEMM_TRACE
-  if (mode == "trace" && argc >= 7)
-    return do_trace(atoi(argv[2]), atoi(argv[3]), atoi(argv[4]), atoi(argv[5]), atoi(argv[6]), argc > 7 ? atoi(argv[7]) : 0,
-                    argc > 8 ? atoi(argv[8]) : 1, argc > 9 ? atoi(argv[9]) : 0);
-#endif
   if (mode == "probe") { probe_cluster_addresses<<<4, 32>>>(); CK(cudaDeviceSynchronize()); return 0; }
   if (mode == "wall" && argc >= 6)
     return do_wall(atoi(argv[2]), atoi(argv[3]), atoi(argv[4]), atoi(argv[5]), argc > 6 ? atof(argv[6]) : 1.0,

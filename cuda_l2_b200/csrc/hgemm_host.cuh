@@ -1,4 +1,4 @@
-// Host side of the B200 HGEMM: tensor-map construction (cached), one-time kernel attribute setup,
+// Host side of the H100 HGEMM: tensor-map construction (cached), one-time kernel attribute setup,
 // and the cluster launch. Shared by the C-ABI library (b200_hgemm_capi.cu) and by the per-shape
 // translation units under kernels/b200_*/ that the reference-style JIT harness compiles.
 #pragma once
@@ -12,7 +12,7 @@
 #include <deque>
 #include <mutex>
 
-#include "hgemm_sm100.cuh"
+#include "hgemm_sm90.cuh"
 
 namespace b200 {
 namespace host {
@@ -25,7 +25,7 @@ enum Status : int {
   kEncodeFailed = -4,
   kNullPointer = -5,
   kBadConfig = -6,
-  kNotBlackwell = -7,
+  kNotHopper = -7,
   kNoScratch = -8,       // internal: no split-K scratch for this (device, stream) and none can be allocated now (stream capture)
   // > 0: a cudaError_t from the launch
 };
@@ -39,7 +39,7 @@ inline const char* status_string(int s) {
     case kEncodeFailed: return "cuTensorMapEncodeTiled failed";
     case kNullPointer: return "null operand pointer";
     case kBadConfig: return "unknown kernel configuration id";
-    case kNotBlackwell: return "device is not compute capability 10.x (sm_100a build)";
+    case kNotHopper: return "device is not compute capability 9.0 (sm_90a build)";
     case kNoScratch: return "split-K scratch unavailable (allocate it outside stream capture with b200_hgemm_prewarm)";
     default: return s > 0 ? cudaGetErrorString(static_cast<cudaError_t>(s)) : "unknown error";
   }
@@ -401,13 +401,13 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   int st = validate(A, Bt, C, M, N, K);
   if (st != kOk) return st;
   const DeviceInfo& di = device_info();
-  if (di.cc_major != 10) return kNotBlackwell;
+  if (di.cc_major != 9) return kNotHopper;
 
   LaunchArgs a{};
   MapCache& cache = map_cache();
   if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, kBlockK, Cfg::BF16)) != kOk) return st;
   if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, kBlockK, Cfg::BF16)) != kOk) return st;
-  if ((st = cache.get(C, M, N, 32, &a.mc, Cfg::EPI_N, Cfg::BF16)) != kOk) return st;
+  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, Cfg::BF16)) != kOk) return st;
 
   constexpr bool kCanSplit = Cfg::SPLIT_K && (MODES & ((1u << kWorkspaceSplitK) | (1u << kClusterSplitK)));
   constexpr bool kCanStream = Cfg::STREAM_K && (MODES & (1u << kStreamK));
@@ -443,7 +443,7 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   if (cache_hints_enabled()) {
     const size_t a_bytes = size_t(M) * K * 2, b_bytes = size_t(N) * K * 2;
     const int n_tiles = (N + Cfg::BN - 1) / Cfg::BN, m_tiles = (M + Cfg::TILE_M - 1) / Cfg::TILE_M;
-    constexpr size_t kL2Keep = size_t(48) << 20, kStream = size_t(96) << 20;
+    constexpr size_t kL2Keep = size_t(20) << 20, kStream = size_t(40) << 20;   // against the 50 MB L2
     if (a_bytes >= kStream && b_bytes <= kL2Keep && n_tiles <= 4) { a.hint_a = ptx::kL2EvictFirst; a.hint_b = ptx::kL2EvictLast; }
     else if (b_bytes >= kStream && a_bytes <= kL2Keep && m_tiles <= 4) { a.hint_b = ptx::kL2EvictFirst; a.hint_a = ptx::kL2EvictLast; }
   }

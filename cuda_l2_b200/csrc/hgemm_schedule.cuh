@@ -11,7 +11,7 @@
 //                   the tail of one tile, whole tiles, the head of another tile, then its data-parallel tiles.
 //                   A unit that starts at k-block 0 OWNS its tile: it adds the partial sums of the units holding the
 //                   rest of the tile's k-range (they belong to the next workers, always as their FIRST unit, so they
-//                   never wait on anybody) and writes C. See streamk_* in hgemm_sm100.cuh.
+//                   never wait on anybody) and writes C. See streamk_* in hgemm_sm90.cuh.
 #pragma once
 #include <cuda_runtime.h>
 

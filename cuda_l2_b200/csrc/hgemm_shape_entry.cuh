@@ -3,6 +3,8 @@
 // torch binding links against (pybind/b200_raw_api.h). The reference does the equivalent with a
 // hand-picked tile/stage/swizzle inside each per-shape .cu (kernels/a100_F32F16F16F32/4096_4096_4096.cu:292-310).
 #pragma once
+// STAGES is the configuration table's requested ring depth (Config caps it at what fits in shared memory, see
+// b200_hgemm_config_info); CTA_GROUP == 2 is the CTA pair, a 2-CTA cluster that multicasts its shared B tile.
 #include "hgemm_host.cuh"
 
 // The K-modes a per-shape translation unit needs compiled: its own (from the tuned split code) and the plain fallback.

@@ -11,7 +11,7 @@ the nearest grid shape — so deployment is a plain operator:
 * :class:`B200Linear`: ``y = x @ W^T (+ b)`` for any leading dimensions; :func:`replace_linear_modules` swaps the
   eligible ``nn.Linear`` layers of a model in place.
 
-There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-B200 device
+There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernel on explicitly
 transposed copies, so a fine-tuning loop works, at the price of two transposes per layer.
 """
@@ -36,7 +36,7 @@ def _check_operands(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str) -> tuple[
     if acc not in ("fp32", "fp16"):
         raise capi.B200HgemmError(f"acc must be 'fp32' or 'fp16', got {acc!r}")
     if a.dtype == torch.bfloat16 and acc != "fp32":
-        raise capi.B200HgemmError("bf16 operands accumulate in fp32 only (tcgen05 kind::f16 has no bf16 accumulator)")
+        raise capi.B200HgemmError("bf16 operands accumulate in fp32 only (wgmma has no bf16 accumulator)")
     m, k = a.shape
     n, k2 = b_kmajor.shape
     if k2 != k:
@@ -62,7 +62,7 @@ def _hgemm_cuda(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> t
 
 @torch.library.impl(f"{_LIB}::hgemm", "CPU")
 def _hgemm_cpu(a, b_kmajor, acc="fp32"):
-    raise capi.B200HgemmError("cuda_l2_b200::hgemm has no CPU implementation (and no fallback): move the tensors to a B200")
+    raise capi.B200HgemmError("cuda_l2_b200::hgemm has no CPU implementation (and no fallback): move the tensors to an H100")
 
 
 @torch.library.register_fake(f"{_LIB}::hgemm")
@@ -92,7 +92,7 @@ torch.library.register_autograd(f"{_LIB}::hgemm", _hgemm_backward, setup_context
 
 
 def hgemm(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
-    """``a`` [M,K] @ ``b_kmajor`` [N,K]^T -> [M,N] through the B200 kernel (see the module docstring)."""
+    """``a`` [M,K] @ ``b_kmajor`` [N,K]^T -> [M,N] through the H100 kernel (see the module docstring)."""
     return torch.ops.cuda_l2_b200.hgemm(a, b_kmajor, acc)
 
 
@@ -101,7 +101,7 @@ def linear_supported(in_features: int, out_features: int, dtype: torch.dtype) ->
 
 
 class B200Linear(nn.Module):
-    """``nn.Linear`` whose matmul runs on the B200 HGEMM kernel. The weight keeps ``nn.Linear``'s layout
+    """``nn.Linear`` whose matmul runs on the H100 HGEMM kernel. The weight keeps ``nn.Linear``'s layout
     ``[out_features, in_features]`` — which IS the kernel's K-major B operand — so swapping a layer copies nothing."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True, device=None,

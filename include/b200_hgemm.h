@@ -1,4 +1,4 @@
-/* b200_hgemm.h — C ABI of the B200-native HGEMM hot path (libb200_hgemm.so).
+/* b200_hgemm.h — C ABI of the H100-native HGEMM hot path (libb200_hgemm.so).
  *
  * This is the drop-in boundary for the one path this repository accelerates:
  *     C[M,N] (fp16) = A[M,K] (fp16) x B[K,N] (fp16), fp32 or fp16 accumulation.
@@ -51,8 +51,12 @@ int b200_bgemm_run_config(int config_id, const void* A, const void* B_kmajor, vo
  * kernels/<dev>/<M>_<N>_<K>.cu (e.g. a100_F32F16F16F32/4096_4096_4096.cu:185-200,305-309). Here the
  * per-shape choice is a table lookup; these calls expose it for the tuner and the tests. */
 int b200_hgemm_num_configs(void);
-/* BN = tile N, stages = smem ring depth, cta_group = 1 (128xBN per SM) or 2 (256xBN per SM pair). */
+/* BN = tile N, stages = the shared-memory ring depth the kernel runs with, cta_group = 1 (128xBN per CTA) or 2
+ * (a 2-CTA cluster of 256xBN sharing its B tile). */
 int b200_hgemm_config_info(int config_id, int* bn, int* stages, int* cta_group);
+/* The ring depth the configuration table requests; the kernel caps it at what fits in shared memory (the value
+ * config_info reports). The per-shape sources under kernels/ name this value. Negative status for an unknown id. */
+int b200_hgemm_config_stages_requested(int config_id);
 /* TMA-multicast cluster shape of a configuration (1 x 1 = none): cluster_m x cluster_n single-CTA groups work on
  * adjacent tiles; A tiles are shared along N, B tiles along M. */
 int b200_hgemm_config_cluster(int config_id, int* cluster_m, int* cluster_n);

@@ -136,7 +136,7 @@ void oracle_hgemm_f32acc_fast(const uint16_t* A, const uint16_t* Bt, uint16_t* C
 }
 
 /* ---- F16F16F16F16: the accumulator is re-rounded to fp16 after every `chunk` products ----------
- * (chunk = 16 models one m16n8k16 / tcgen05 K=16 step: products summed wide, accumulator stored in
+ * (chunk = 16 models one m16n8k16 / wgmma K=16 step: products summed wide, accumulator stored in
  * fp16). The hardware's exact internal order is not specified by the reference or by NVIDIA; on
  * the 0/1 domain with |sum| < 2048 every order is exact. */
 void oracle_hgemm_f16acc(const uint16_t* A, const uint16_t* Bt, uint16_t* C, int M, int N, int K, int chunk) {

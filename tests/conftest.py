@@ -11,7 +11,7 @@ GOLDEN = REPO / "tests" / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine with one)")
 
 
 def load_zero_one_cases():

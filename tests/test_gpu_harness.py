@@ -1,4 +1,4 @@
-"""The reference-style harness end to end on the B200: JIT-build hgemm_lib for one shape (torch extension with the
+"""The reference-style harness end to end on the H100: JIT-build hgemm_lib for one shape (torch extension with the
 reference's 15 exported names), run the 0/1 exactness procedure against every baseline, time one sample."""
 import json
 import subprocess

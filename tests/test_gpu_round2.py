@@ -1,4 +1,4 @@
-"""Round-2 parity tests on the B200: the top of the shape grid at full size through the reference's procedure, the
+"""Round-2 parity tests on the H100: the top of the shape grid at full size through the reference's procedure, the
 fp16-accumulate path against the oracle's fp16 model, the bf16 variant, concurrent / captured split-K launches, and
 the deployable operator."""
 import numpy as np
@@ -18,8 +18,8 @@ def dev(x: np.ndarray) -> torch.Tensor:
 
 
 @pytest.fixture(scope="module", autouse=True)
-def _need_b200(built_libs):
-    assert torch.cuda.is_available() and torch.cuda.get_device_capability()[0] == 10
+def _need_h100(built_libs):
+    assert torch.cuda.is_available() and torch.cuda.get_device_capability() == (9, 0)
     before = capi.launch_count()
     yield
     assert capi.launch_count() > before, "no kernel of libb200_hgemm.so was launched"
@@ -30,7 +30,7 @@ def _need_b200(built_libs):
 def test_top_of_the_grid_passes_the_reference_check_procedure(acc, mnk):
     """The 12288/16384 class at FULL size through the harness's 0/1 procedure — {0,0,1} operand density because
     max(M,N,K) > 8192 (zero_one_correctness_check.py:65-73), CPU fp32 truth, |truth| > 2047 masked, guard bands,
-    == 0 rule — with the dispatcher's own choice for the shape (512x256 pair tiles, L2 hints, split-K) in the kernel slot."""
+    == 0 rule — with the dispatcher's own choice for the shape (512-row pair tiles, L2 hints, split-K) in the kernel slot."""
     name = f"cuda_l2_b200_{acc}"
 
     def kernel(a, b, b_col_major, c):

@@ -1,5 +1,5 @@
 """The reference's defense.py properties on the real kernel (SURVEY §8(f) item 2). Runs after the parity tests: it is
-the newest GPU test and the only one that has not been on a B200 yet."""
+the newest GPU test."""
 import pytest
 import torch
 

@@ -33,7 +33,7 @@ def load(path: Path):
 def label(name: str) -> str:
     stem = name[len("cuda_l2_b200_"):-len(".csv")]
     acc, rest = stem.split("_speedup_", 1)
-    return f"B200 {acc} {rest.replace('_', ' ')}"
+    return f"H100 {acc} {rest.replace('_', ' ')}"
 
 
 def svg(groups, path: Path):
@@ -43,7 +43,7 @@ def svg(groups, path: Path):
     y = lambda v: top + h - h * v / vmax
     parts = [f'<svg xmlns="http://www.w3.org/2000/svg" width="{width}" height="{top + h + 90}" font-family="sans-serif" font-size="11">',
              f'<rect width="100%" height="100%" fill="white"/>',
-             f'<text x="{left}" y="20" font-size="14" font-weight="bold">Mean speed-up of the B200 kernels over each baseline (all shapes of the file)</text>']
+             f'<text x="{left}" y="20" font-size="14" font-weight="bold">Mean speed-up of the H100 kernels over each baseline (all shapes of the file)</text>']
     t = 0.0
     while t <= vmax:
         parts.append(f'<line x1="{left}" x2="{width - 10}" y1="{y(t):.1f}" y2="{y(t):.1f}" stroke="{"#444" if abs(t - 1.0) < 1e-9 else "#ddd"}"/>')
@@ -73,7 +73,7 @@ def main():
     files = sorted((REPO / "eval_results").glob("cuda_l2_b200_*_speedup_*.csv"))
     files = [f for f in files if not f.name.endswith("_absolute.csv")]
     groups = [load(f) for f in files]
-    lines = ["# B200 results in the reference's format", "",
+    lines = ["# H100 results in the reference's format", "",
              "Mean speed-up over each baseline (the reference's README figure), per results file; `won` = shapes at or above",
              "1.0 against cuBLASLt-auto-tuning-max (the harder of its two layouts). Files tagged `harness_sample` / `server` come",
              "from the real `eval_one_file.sh` flow or the harness's Python loop on a stratified sample (see DESIGN.md §6).", "",
@@ -81,9 +81,9 @@ def main():
     for g in groups:
         cells = [f"{g[c][0]:.3f}" + (f" ({g[c][1]})" if g[c][1] != g["shapes"] else "") if g[c][0] else "-" for c in COLS]
         lines.append(f"| `{g['file']}` | {g['shapes']} | " + " | ".join(cells) + f" | {g['won']} / {g['n_auto']} = {100.0 * g['won'] / max(g['n_auto'], 1):.1f} % |")
-    lines += ["", "![speed-up summary](../assets/speedup_summary_b200.svg)", ""]
+    lines += ["", "![speed-up summary](speedup_summary.svg)", ""]
     (REPO / "eval_results" / "SUMMARY.md").write_text("\n".join(lines))
-    svg(groups, REPO / "assets" / "speedup_summary_b200.svg")
+    svg(groups, REPO / "eval_results" / "speedup_summary.svg")   # next to the tables it summarises (git-ignored)
     print("\n".join(lines))
     return 0
 

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""SASS evidence that libb200_hgemm.so is a Blackwell-native kernel family (B200_PROFILING.md, "What proves a
-Blackwell-native kernel"): counts of tcgen05 / TMEM / TMA mnemonics, and of the legacy tensor-core paths that must be 0.
+"""SASS evidence that libb200_hgemm.so is a Hopper-native kernel family: counts of wgmma (HGMMA), TMA and cluster
+mnemonics, of the wgmma waits (one WARPGROUP.DEPBAR per HGMMA would mean ptxas serialised the pipeline), and of the
+legacy tensor-core paths that must be 0.
 
-    python tools/sass_summary.py > profiles/sass_summary.txt      # no GPU needed (cuobjdump reads the cubin)
+    python tools/sass_summary.py      # no GPU needed (cuobjdump reads the cubin)
 """
 import collections
 import re
@@ -12,8 +13,8 @@ from pathlib import Path
 
 REPO = Path(__file__).resolve().parent.parent
 LIB = REPO / "cuda_l2_b200" / "lib" / "libb200_hgemm.so"
-WANT = ["UTCHMMA", "UTCHMMA.2CTA", "LDTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "UTCATOMSWS", "SYNCS", "UCGABAR", "ACQBULK", "PREEXIT",
-        "HMMA", "HGMMA", "LDGSTS"]
+WANT = ["HGMMA", "WARPGROUP.DEPBAR", "WARPGROUP.ARRIVE", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "UCGABAR", "USETMAXREG",
+        "ACQBULK", "HMMA", "LDGSTS"]
 
 
 def main():
@@ -35,7 +36,8 @@ def main():
         match = lambda k: k == w or k.startswith(w + ".") or k.startswith(w + "_")
         exact = sum(v for k, v in ops.items() if match(k))
         variants = sorted(k for k in ops if match(k))
-        note = {"HMMA": "   <- legacy mma.sync path: must be 0", "HGMMA": "   <- Hopper wgmma: must be 0",
+        note = {"HMMA": "   <- legacy mma.sync path: must be 0", "HGMMA": "   <- Hopper wgmma",
+                "WARPGROUP.DEPBAR": "   <- wgmma waits: about two per kernel, not one per HGMMA",
                 "LDGSTS": "   <- cp.async (not used: every bulk load is TMA)"}.get(w, "")
         print(f"{w:14s} {exact:6d}   {' '.join(variants[:8])}{note}")
     return 0

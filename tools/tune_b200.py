@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Turn `dev_check grid` measurements into the dispatcher's tuned table.
 
-    # on the B200 (8 parts can run on 8 GPUs, or sequentially on one):
+    # on the GPU (8 parts can run on 8 GPUs, or sequentially on one):
     cuda_l2_b200/lib/dev_check grid 32 0 1 > gpurun_out/grid_fp32.csv
     cuda_l2_b200/lib/dev_check grid 16 0 1 > gpurun_out/grid_fp16.csv
     # (append `3.0 0 1e30 wall` to rank candidates by the harness's own wall-clock metric instead of event time)
@@ -18,6 +18,7 @@ loses by more than 1.5 % (noise guard).
 """
 from __future__ import annotations
 
+import os
 import re
 import sys
 from collections import defaultdict
@@ -129,7 +130,8 @@ def main(argv):
             if acc in e and e[acc][3] == e[acc][3]:      # measured in this run (kept entries carry NaN)
                 wins[acc][1] += 1
                 wins[acc][0] += e[acc][3] <= e[acc][4]
-    text = ("// GENERATED by tools/tune_b200.py — per-shape winners measured on a B200. Do not edit by hand.\n"
+    gpu = os.environ.get("TUNE_GPU_NAME", "the GPU the grid files were measured on")
+    text = (f"// GENERATED by tools/tune_b200.py — per-shape winners measured on {gpu}. Do not edit by hand.\n"
             "// {M, N, K, cfg/group_m/splits (fp32 acc), cfg/group_m/splits (fp16 acc)}; sorted by (M, N, K).\n"
             "static const TunedEntry kTuned[] = {\n" + "\n".join(rows) + "\n"
             "    {0, 0, 0, -1, 0, 1, -1, 0, 1},   // sentinel so the array is never empty\n};\n"

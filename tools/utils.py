@@ -1,13 +1,13 @@
 """JIT-build glue of the harness — same public surface as the reference's ``tools/utils.py``
 (``extract_bm_bk_bn``, ``get_build_sources``, ``get_build_cuda_cflags``, ``build_from_sources``,
-``as_col_major``; reference tools/utils.py:8-115), written for ``--device_type b200``.
+``as_col_major``; reference tools/utils.py:8-115), written for ``--device_type b200`` (the H100 kernel family's name in the harness).
 
-Differences that matter on a B200:
+Differences that matter here:
 
 * the five sources of one ``hgemm_lib`` build are torch-free ``.cu`` files plus ONE ``.cc`` that holds every
   ``torch::Tensor`` wrapper, so a per-shape rebuild is a few seconds of nvcc instead of minutes;
 * ``CUTLASS_DIR`` is not needed (the b200 kernels are hand-written PTX, not CuTe templates);
-* the arch flag is pinned to ``-gencode arch=compute_100a,code=sm_100a`` (plain ``sm_100`` rejects tcgen05);
+* the arch flag is pinned to ``-gencode arch=compute_90a,code=sm_90a`` (plain ``sm_90`` rejects wgmma and setmaxnreg);
 * nothing here touches the GPU, so ``compile.py`` can pre-build on a machine without one.
 """
 from __future__ import annotations
@@ -22,7 +22,7 @@ PROJECT_DIR = Path(__file__).resolve().parent.parent
 
 DEVICE_TYPES = ("b200",)
 ACC_DIRS = {"fp16": "F16F16F16F16", "fp32": "F32F16F16F32"}
-SM100A_GENCODE = "-gencode=arch=compute_100a,code=sm_100a"
+SM90A_GENCODE = "-gencode=arch=compute_90a,code=sm_90a"
 
 _TILE_TOKEN = re.compile(r"(BM|BN|BK)=Int<(\d+)>")
 
@@ -68,12 +68,12 @@ def get_build_sources(mnk, acc_precise, device_type):
 
 
 def get_build_cuda_cflags(build_pkg: bool = False):
-    """nvcc flags (reference tools/utils.py:57-92 minus the CUTLASS include paths, plus the sm_100a target)."""
+    """nvcc flags (reference tools/utils.py:57-92 minus the CUTLASS include paths, plus the sm_90a target)."""
     flags = [
         "-O3",
         "-std=c++17",
         "-lineinfo",
-        SM100A_GENCODE,
+        SM90A_GENCODE,
         "-U__CUDA_NO_HALF_OPERATORS__",
         "-U__CUDA_NO_HALF_CONVERSIONS__",
         "-U__CUDA_NO_HALF2_OPERATORS__",
@@ -105,11 +105,11 @@ def build_from_sources(mnk, acc_precise, device_type, base_dir: str, verbose: bo
     if torch.cuda.is_available():
         dev = torch.cuda.current_device()
         print(f"Loading hgemm lib on device: {torch.cuda.get_device_name(dev)} :: "
-              f"{torch.cuda.get_device_capability(dev)} :: sm_100a")
+              f"{torch.cuda.get_device_capability(dev)} :: sm_90a")
     os.makedirs(base_dir, exist_ok=True)
-    # torch appends its own -gencode flags from TORCH_CUDA_ARCH_LIST; make that exactly sm_100a too
+    # torch appends its own -gencode flags from TORCH_CUDA_ARCH_LIST; make that exactly sm_90a too
     prev = os.environ.get("TORCH_CUDA_ARCH_LIST")
-    os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0a"
+    os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"
     try:
         return load(
             name="hgemm_lib",
