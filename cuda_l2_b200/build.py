@@ -90,31 +90,6 @@ def build_dev_check(verbose: bool = False, force: bool = False) -> Path:
     return out
 
 
-def build_variant(name: str, defines: list[str], verbose: bool = False, force: bool = False) -> Path:
-    """Developer build of the library and of dev_check with extra -D flags: libb200_hgemm_<name>.so + dev_check_<name>.
-
-    Not part of build_all(): the product library is always the plain build."""
-    LIB_DIR.mkdir(exist_ok=True)
-    build_baselines(verbose, force)
-    flags = [f"-D{d}" for d in defines]
-    lib = LIB_DIR / f"libb200_hgemm_{name}.so"
-    src = CSRC / "b200_hgemm_capi.cu"
-    if force or _stale(lib, [src] + _headers()):
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, *flags, "--shared", "-o", str(lib), str(src)], verbose)
-    out = LIB_DIR / f"dev_check_{name}"
-    dsrc = CSRC / "dev_check.cu"
-    if force or _stale(out, [dsrc, lib] + _headers()):
-        _run([nvcc_path(), *ARCH_FLAGS, "-std=c++17", "-O3", "-lineinfo", *flags, "-o", str(out), str(dsrc),
-              f"-L{LIB_DIR}", f"-lb200_hgemm_{name}", "-lb200_baselines", "-lcublas", "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN"],
-             verbose)
-    return out
-
-
-def build_no_k_decomp(verbose: bool = False, force: bool = False) -> Path:
-    """Kernels without split-K / stream-K code (-DB200_HGEMM_NO_K_DECOMP=1): what does that code cost the plain path?"""
-    return build_variant("plain", ["B200_HGEMM_NO_K_DECOMP=1"], verbose, force)
-
-
 def build_all(verbose: bool = False, force: bool = False) -> dict[str, Path]:
     out = {"capi": build_capi(verbose, force)}
     if (CSRC / "b200_baselines_capi.cu").exists():

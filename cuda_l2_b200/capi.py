@@ -52,7 +52,7 @@ def hgemm_lib() -> ctypes.CDLL:
         lib.b200_hgemm_run_config.argtypes = [i, i, vp, vp, vp, i, i, i, i, i, i, vp]
         lib.b200_hgemm_host.argtypes = [i, vp, vp, vp, i, i, i]
         ip = ctypes.POINTER(i)
-        lib.b200_hgemm_schedule_units.argtypes = [i, i, i, i, i, i, i, ip, i, ip, ip, ip]
+        lib.b200_hgemm_schedule_units.argtypes = [i, i, i, i, i, i, i, ip, i, ip, ip, ip, ip]
         lib.b200_hgemm_schedule_units.restype = i
         lib.b200_hgemm_prewarm.argtypes = [vp]
         lib.b200_hgemm_release.argtypes = []
@@ -209,29 +209,31 @@ def select(acc: str | int, m: int, n: int, k: int) -> tuple[int, int, int]:
 
 
 STREAMK_TAIL, STREAMK_TAIL_PLUS_WAVE = 100, 101      # `splits` codes of b200_hgemm_run_config
+KMODES = ("plain", "split-k", "cluster-split-k", "stream-k")   # the K-modes b200_hgemm_schedule_units reports, in order
 
 
 def schedule(config_id: int, m: int, n: int, k: int, splits: int = 1, num_sms: int = 132) -> dict:
     """Host-side view of the kernel's schedule (no GPU needed; the kernel walks the same code).
 
-    Returns ``{"workers": W, "sk_tiles": S, "units": [[(tile, kb0, kb1, contributors), ...] per worker]}``."""
+    Returns ``{"workers": W, "sk_tiles": S, "mode": one of KMODES,
+    "units": [[(tile, kb0, kb1, contributors), ...] per worker]}``."""
     lib = hgemm_lib()
-    nw, sk = ctypes.c_int(), ctypes.c_int()
+    nw, sk, mode = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
     cap = 64
     buf, contrib = (ctypes.c_int * (3 * cap))(), (ctypes.c_int * cap)()
     st = lib.b200_hgemm_schedule_units(config_id, m, n, k, splits, num_sms, 0, buf, cap, ctypes.byref(nw),
-                                       ctypes.byref(sk), contrib)
+                                       ctypes.byref(sk), ctypes.byref(mode), contrib)
     _check(min(st, 0), "b200_hgemm_schedule_units")
     units = []
     for w in range(nw.value):
-        cnt = lib.b200_hgemm_schedule_units(config_id, m, n, k, splits, num_sms, w, buf, cap, None, None, contrib)
+        cnt = lib.b200_hgemm_schedule_units(config_id, m, n, k, splits, num_sms, w, buf, cap, None, None, None, contrib)
         _check(min(cnt, 0), "b200_hgemm_schedule_units")
         if cnt > cap:
             cap = cnt
             buf, contrib = (ctypes.c_int * (3 * cap))(), (ctypes.c_int * cap)()
-            cnt = lib.b200_hgemm_schedule_units(config_id, m, n, k, splits, num_sms, w, buf, cap, None, None, contrib)
+            cnt = lib.b200_hgemm_schedule_units(config_id, m, n, k, splits, num_sms, w, buf, cap, None, None, None, contrib)
         units.append([(buf[3 * j], buf[3 * j + 1], buf[3 * j + 2], contrib[j]) for j in range(cnt)])
-    return {"workers": nw.value, "sk_tiles": sk.value, "units": units}
+    return {"workers": nw.value, "sk_tiles": sk.value, "mode": KMODES[mode.value], "units": units}
 
 
 def prewarm(stream: int | None = None) -> None:

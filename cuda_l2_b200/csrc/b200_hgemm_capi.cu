@@ -14,9 +14,6 @@
 namespace {
 
 std::atomic<unsigned long long> g_launches{0};
-// the ring depth a configuration runs with (its requested depth, capped by shared memory)
-template <class Cfg>
-constexpr int ring_depth() { return Cfg::STAGES; }
 constexpr int kBf16Acc32 = 0xB32;   // internal selector of run(): bf16 operands, fp32 accumulation
 
 template <bool kAccF32, bool kBf16 = false>
@@ -40,11 +37,14 @@ int run_config(int id, const void* A, const void* Bt, void* C, int M, int N, int
 
 template <class Cfg>
 int schedule_units(int M, int N, int K, int splits, int num_sms, int worker, int* units, int max_units,
-                   int* num_workers, int* sk_tiles, int* contributors) {
+                   int* num_workers, int* sk_tiles, int* mode, int* contributors) {
   using namespace b200;
-  const host::Plan p = host::make_plan<Cfg>(M, N, K, num_sms / Cfg::CLUSTER_CTAS, splits);
+  // every K-mode compiled, every cluster resident: the launcher's plan on a device of num_sms SMs
+  const int max_workers = num_sms / Cfg::CLUSTER_CTAS;
+  const host::Plan p = host::plan<Cfg>(M, N, K, splits, max_workers, [=] { return max_workers; });
   if (num_workers) *num_workers = p.workers;
   if (sk_tiles) *sk_tiles = p.sk_tiles;
+  if (mode) *mode = p.mode;
   if (worker < 0 || worker >= p.workers) return host::kBadShape;
   WorkIter it(worker, p.workers, p.num_tiles, p.nkb, p.splits, p.sk_tiles);
   WorkUnit u;
@@ -60,6 +60,8 @@ int schedule_units(int M, int N, int K, int splits, int num_sms, int worker, int
   }
   return n;
 }
+
+const b200::ConfigDesc* config_desc(int id) { return id >= 0 && id < b200::kNumConfigs ? &b200::kConfigs[id] : nullptr; }
 
 int run(int acc_bits, int id, const void* A, const void* Bt, void* C, int M, int N, int K, int group_m,
         int max_ctas, int splits, void* stream) {
@@ -93,42 +95,30 @@ extern "C" {
 int b200_hgemm_num_configs(void) { return b200::kNumConfigs; }
 
 int b200_hgemm_config_info(int config_id, int* bn, int* stages, int* cta_group) {
-  switch (config_id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)  \
-  case ID:                             \
-    if (bn) *bn = BN;                  \
-    if (stages) *stages = ring_depth<b200::Config<BN, STAGES, CG, true, CM, CN, MR>>();   \
-    if (cta_group) *cta_group = CG;    \
-    return 0;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      return b200::host::kBadConfig;
-  }
+  const b200::ConfigDesc* c = config_desc(config_id);
+  if (!c) return b200::host::kBadConfig;
+  if (bn) *bn = c->bn;
+  if (stages) *stages = c->stages;
+  if (cta_group) *cta_group = c->cta_group;
+  return 0;
 }
 
 int b200_hgemm_config_cluster(int config_id, int* cluster_m, int* cluster_n) {
-  switch (config_id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR) \
-  case ID:                                    \
-    if (cluster_m) *cluster_m = CM;           \
-    if (cluster_n) *cluster_n = CN;           \
-    return 0;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      return b200::host::kBadConfig;
-  }
+  const b200::ConfigDesc* c = config_desc(config_id);
+  if (!c) return b200::host::kBadConfig;
+  if (cluster_m) *cluster_m = c->cluster_m;
+  if (cluster_n) *cluster_n = c->cluster_n;
+  return 0;
 }
 
 int b200_hgemm_schedule_units(int config_id, int M, int N, int K, int splits, int num_sms, int worker, int* units,
-                              int max_units, int* num_workers, int* sk_tiles, int* contributors) {
+                              int max_units, int* num_workers, int* sk_tiles, int* mode, int* contributors) {
   if (M <= 0 || N <= 0 || K <= 0 || num_sms <= 0) return b200::host::kBadShape;
   switch (config_id) {
 #define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                   \
   case ID:                                                                                                          \
     return schedule_units<b200::Config<BN, STAGES, CG, true, CM, CN, MR>>(M, N, K, splits, num_sms, worker, units, \
-                                                                          max_units, num_workers, sk_tiles, contributors);
+                                                                          max_units, num_workers, sk_tiles, mode, contributors);
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE
     default:
@@ -137,27 +127,13 @@ int b200_hgemm_schedule_units(int config_id, int M, int N, int K, int splits, in
 }
 
 int b200_hgemm_config_stages_requested(int config_id) {
-  switch (config_id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR) \
-  case ID:                                        \
-    return STAGES;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      return b200::host::kBadConfig;
-  }
+  const b200::ConfigDesc* c = config_desc(config_id);
+  return c ? c->stages_requested : b200::host::kBadConfig;
 }
 
 int b200_hgemm_config_m_rep(int config_id) {
-  switch (config_id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR) \
-  case ID:                                        \
-    return MR;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      return b200::host::kBadConfig;
-  }
+  const b200::ConfigDesc* c = config_desc(config_id);
+  return c ? c->m_rep : b200::host::kBadConfig;
 }
 
 int b200_hgemm_select_config(int acc_bits, int M, int N, int K) {

@@ -46,4 +46,21 @@
 
 namespace b200 {
 constexpr int kNumConfigs = 31;
+
+// What the host needs to know about a configuration, as Config<> derives it: tile and ring shape, cluster layout, and
+// which K-decompositions its kernels carry. The accumulator and operand type change none of these.
+struct ConfigDesc {
+  int bn, stages, stages_requested, cta_group, cluster_m, cluster_n, m_rep;
+  bool split_k, stream_k;
+};
+template <class Cfg>
+constexpr ConfigDesc describe(int stages_requested) {
+  return ConfigDesc{Cfg::BN, Cfg::STAGES, stages_requested, Cfg::CTA_GROUP, Cfg::CLUSTER_M, Cfg::CLUSTER_N, Cfg::M_REP,
+                    Cfg::SPLIT_K, Cfg::STREAM_K};
 }
+constexpr ConfigDesc kConfigs[kNumConfigs] = {
+#define B200_DESC(ID, BN, STAGES, CG, CM, CN, MR) describe<Config<BN, STAGES, CG, true, CM, CN, MR>>(STAGES),
+    B200_HGEMM_CONFIGS(B200_DESC)
+#undef B200_DESC
+};
+}  // namespace b200

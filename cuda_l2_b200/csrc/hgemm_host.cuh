@@ -206,70 +206,109 @@ inline void release_scratch() {
   cudaSetDevice(cur);
 }
 
-// Largest usable split factor for this problem/config: units must fit the SMs (one CTA per unit), every
-// split must own at least one k-block, and the partial tiles must fit the workspace.
-template <class Cfg>
-int clamp_splits(int splits, int M, int N, int K, int num_sms) {
-  if (splits <= 1 || Cfg::CTA_GROUP != 1) return 1;
-  const int tiles = ((M + kBlockM - 1) / kBlockM) * ((N + Cfg::BN - 1) / Cfg::BN);   // CTA_GROUP == 1: callers exclude M_REP > 1
-  const int nkb = (K + kBlockK - 1) / kBlockK;
-  if (tiles > kMaxSplitTiles) return 1;
-  splits = std::min(splits, std::min(num_sms / tiles, std::min(nkb, 32)));   // <= 32: the slices of all partials must fit the pipeline smem
-  while (splits > 1 && (splits - 1) * ((nkb + splits - 1) / splits) >= nkb) --splits;   // no empty split
-  while (splits > 1 && size_t(tiles) * splits * kBlockM * Cfg::BN * sizeof(float) > kSplitKWsBytes) --splits;
-  return std::max(splits, 1);
-}
-
-// `splits` values with a special meaning (besides > 1: workspace split-K, -2/-4/-8: cluster split-K)
+// `splits` codes with a special meaning (besides > 1: workspace split-K, -2/-4/-8: cluster split-K)
 constexpr int kStreamKTail = 100;           // stream-K over the tiles of the partial last wave
 constexpr int kStreamKTailPlusWave = 101;   // ... plus one full wave, so that every worker's slice is longer than a tile
 constexpr int kMinStreamKSlice = 4;         // k-blocks; shorter slices are all pipeline fill and fix-up
 
-// What a launch will run: how many workers (CTAs, CTA pairs or clusters), which K-decomposition.
+// What a `splits` code asks for: a K-mode and its factor, which is the split count (workspace split-K), the cluster
+// size (cluster split-K) or the code itself (stream-K: kStreamKTail or kStreamKTailPlusWave). 1, 0 and -1 ask for none.
+struct KRequest { KMode mode; int factor; };
+constexpr KRequest decode_splits(int splits) {
+  return (splits == kStreamKTail || splits == kStreamKTailPlusWave) ? KRequest{kStreamK, splits}
+         : splits > 1                                               ? KRequest{kWorkspaceSplitK, splits}
+         : splits < -1                                              ? KRequest{kClusterSplitK, -splits}
+                                                                    : KRequest{kPlain, 1};
+}
+
+// Does the call site have this configuration's kernel for this mode? MODES: bit mask of the K-modes it compiles. The
+// K-decompositions are wired for single CTAs and CTA pairs without multicast, BN >= 64, 128 rows per CTA (split-K:
+// single CTAs only); the plain schedule is always available.
+template <class Cfg, unsigned MODES>
+constexpr bool has_mode(KMode m) {
+  return ((MODES >> m) & 1u) && (m == kPlain || (m == kStreamK ? Cfg::STREAM_K : Cfg::SPLIT_K));
+}
+
+// What a launch will run: its K-mode, how many workers (CTAs, CTA pairs or clusters), how K is divided.
 struct Plan {
+  KMode mode;
   int num_tiles, nkb;
-  int workers;          // grid = workers * (CTAs per worker)
+  int workers;          // grid = workers * (CTAs per worker); split-K: one CTA per (tile, split)
   int splits;           // > 1: split-K, one worker per (tile, split)
   int cluster_reduce;   // != 0: the splits of a tile form a cluster of this many CTAs and reduce through DSMEM
   int sk_tiles;         // > 0: stream-K over the first sk_tiles tiles
 };
 
-// `workers_avail`: workers the device can hold at once (SMs / CTAs per worker, after max_ctas and cluster occupancy).
-template <class Cfg>
-Plan make_plan(int M, int N, int K, int workers_avail, int splits) {
+// The one place that turns a `splits` request into a schedule. Pure host code: the device comes in as `max_workers`
+// (SMs, or max_ctas, over the CTAs per worker) and `resident_clusters()`, the number of clusters of this configuration
+// the device holds at once — an occupancy query, called only when that number bounds the workers. A request the call
+// site or the configuration cannot run, or that the problem cannot use, runs plain; a factor is clamped to what fits.
+template <class Cfg, unsigned MODES = 0xFu, class ResidentClusters>
+Plan plan(int M, int N, int K, int splits, int max_workers, ResidentClusters&& resident_clusters) {
+  KRequest req = decode_splits(splits);
+  // A per-shape translation unit with a stream-K code compiles the stream-K kernel, but its launches run the plain
+  // schedule: without the workspace split-K kernel, every code > 1 has always run plain there. Running stream-K in
+  // those units changes their results' summation order and their timings, and is left to a change of its own.
+  const bool per_shape_stream_k = req.mode == kStreamK && !((MODES >> kWorkspaceSplitK) & 1u);
+  if (!has_mode<Cfg, MODES>(req.mode) || per_shape_stream_k) req = KRequest{kPlain, 1};
   Plan p{};
   const int num_m_blocks = (M + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M);
   const int num_n_blocks = (N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N);
   p.num_tiles = num_m_blocks * num_n_blocks;
   p.nkb = (K + kBlockK - 1) / kBlockK;
-  p.workers = std::max(workers_avail, 1);
-  const bool plain = Cfg::STREAM_K;   // no multicast cluster, BN >= 64, 128 rows per CTA: the K-decompositions are wired for these
-  int sk_mode = 0;
-  if (splits == kStreamKTail || splits == kStreamKTailPlusWave) { sk_mode = splits; splits = 1; }
-  if (!plain) splits = 1;
-  if (splits < -1) {
-    int cs = -splits;
-    if (Cfg::CTA_GROUP == 1 && (cs == 2 || cs == 4 || cs == 8)) {
+  p.splits = 1;
+  // Clusters must fit inside a GPC, so fewer than SMs / cluster size may be resident at once. Larger clusters are
+  // always sized to what fits; CTA pairs only for stream-K, whose owners wait for contributors that must therefore be
+  // running (for the plain schedule a pair that starts late is merely late).
+  if (Cfg::CLUSTER_CTAS > 2 || (Cfg::CLUSTER_CTAS == 2 && req.mode == kStreamK))
+    max_workers = std::min(max_workers, resident_clusters());
+  p.workers = std::max(max_workers, 1);
+  if (req.mode == kClusterSplitK) {
+    int cs = req.factor;
+    if (cs == 2 || cs == 4 || cs == 8) {
       // every CTA of the cluster must own at least one k-block: halve the cluster until no k-range is empty
       while (cs > 1 && (cs - 1) * ((p.nkb + cs - 1) / cs) >= p.nkb) cs /= 2;
-      if (cs > 1) p.cluster_reduce = cs;
+      if (cs > 1) {
+        p.mode = kClusterSplitK;
+        p.splits = p.cluster_reduce = cs;
+        p.workers = p.num_tiles * cs;   // one cluster per tile, one CTA per k-range
+        return p;
+      }
     }
-    splits = 1;
-  }
-  p.splits = clamp_splits<Cfg>(splits, M, N, K, p.workers);
-  if (p.cluster_reduce) {
-    p.workers = p.num_tiles * p.cluster_reduce;   // one cluster per tile, one CTA per k-range
-    p.splits = p.cluster_reduce;
-  } else if (p.splits > 1) {
-    p.workers = p.num_tiles * p.splits;           // exactly one CTA per (tile, split) unit
-  } else {
-    if (sk_mode && plain && p.num_tiles % p.workers != 0 && p.workers * Cfg::CTA_GROUP <= kMaxStreamKSlots) {
-      int sk = p.num_tiles % p.workers;
-      if (sk_mode == kStreamKTailPlusWave && p.num_tiles > p.workers) sk += p.workers;
-      if (sk * p.nkb / p.workers >= kMinStreamKSlice) p.sk_tiles = sk;
+  } else if (req.mode == kWorkspaceSplitK && p.num_tiles <= kMaxSplitTiles) {
+    // units must fit the SMs (one CTA per unit), every split must own at least one k-block, and the partial tiles
+    // must fit the workspace; <= 32: the slices of all partials must fit the pipeline smem
+    int s = std::min(req.factor, std::min(p.workers / p.num_tiles, std::min(p.nkb, 32)));
+    while (s > 1 && (s - 1) * ((p.nkb + s - 1) / s) >= p.nkb) --s;   // no empty split
+    while (s > 1 && size_t(p.num_tiles) * s * kBlockM * Cfg::BN * sizeof(float) > kSplitKWsBytes) --s;
+    if (s > 1) {
+      p.mode = kWorkspaceSplitK;
+      p.splits = s;
+      p.workers = p.num_tiles * s;      // exactly one CTA per (tile, split) unit
+      return p;
     }
-    if (!p.sk_tiles && p.workers > p.num_tiles) p.workers = p.num_tiles;
+  } else if (req.mode == kStreamK && p.num_tiles % p.workers != 0 && p.workers * Cfg::CTA_GROUP <= kMaxStreamKSlots) {
+    int sk = p.num_tiles % p.workers;
+    if (req.factor == kStreamKTailPlusWave && p.num_tiles > p.workers) sk += p.workers;
+    if (sk * p.nkb / p.workers >= kMinStreamKSlice) {
+      p.mode = kStreamK;
+      p.sk_tiles = sk;
+      return p;
+    }
   }
+  p.workers = std::min(p.workers, p.num_tiles);
+  return p;
+}
+
+// The same launch on the plain schedule, when a workspace split-K or stream-K plan cannot run (no scratch, or the
+// device refuses the co-resident grid). It keeps the plan's worker bound: CTA pairs planned for stream-K stay within
+// the resident clusters.
+inline Plan undivided(Plan p) {
+  p.mode = kPlain;
+  p.splits = 1;
+  p.cluster_reduce = 0;
+  p.sk_tiles = 0;
+  p.workers = std::min(p.workers, p.num_tiles);
   return p;
 }
 
@@ -392,9 +431,9 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
 }
 
 // group_m <= 0 selects the default rasterisation width. max_ctas <= 0 means "all SMs". `splits`: 1 none, > 1 workspace
-// split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K — each clamped to what the problem and
-// the configuration allow. MODES: bit mask of the K-modes this call site may need (a per-shape translation unit
-// names its one mode and so compiles two kernels instead of four; the plain mode is always available as fallback).
+// split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
+// mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
+// kernels instead of four; the plain mode is always available as fallback).
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
            int group_m = 0, int max_ctas = 0, int splits = 1) {
@@ -409,28 +448,15 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, kBlockK, Cfg::BF16)) != kOk) return st;
   if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, Cfg::BF16)) != kOk) return st;
 
-  constexpr bool kCanSplit = Cfg::SPLIT_K && (MODES & ((1u << kWorkspaceSplitK) | (1u << kClusterSplitK)));
-  constexpr bool kCanStream = Cfg::STREAM_K && (MODES & (1u << kStreamK));
-  const bool wants_stream_k = (splits == kStreamKTail || splits == kStreamKTailPlusWave);
-  if ((wants_stream_k && !kCanStream) || (!wants_stream_k && splits != 1 && !kCanSplit)) splits = 1;
-  if (splits > 1 && !(MODES & (1u << kWorkspaceSplitK))) splits = 1;
-  if (splits < -1 && !(MODES & (1u << kClusterSplitK))) splits = 1;
-
-  int workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
-  // Clusters must fit inside a GPC, so fewer than SMs / cluster size may be resident at once. Larger clusters are
-  // always sized to what fits; CTA pairs only when stream-K is requested, whose owners wait for contributors
-  // that must therefore be running (for the plain schedule a pair that starts late is merely late).
-  if (Cfg::CLUSTER_CTAS > 2 || (Cfg::CLUSTER_CTAS == 2 && wants_stream_k && splits != 1)) {
-    workers = std::min(workers, max_resident_clusters<Cfg>(di));
-  }
-  a.plan = make_plan<Cfg>(M, N, K, workers, splits);
-  if ((a.plan.splits > 1 && !a.plan.cluster_reduce) || a.plan.sk_tiles) {
+  const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
+  a.plan = plan<Cfg, MODES>(M, N, K, splits, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
+  if (a.plan.mode == kWorkspaceSplitK || a.plan.mode == kStreamK) {
     SplitKScratch* sk = nullptr;
     if (splitk_scratch(di.dev, stream, &sk) == kOk) {
       a.ws = sk->ws; a.ctr = sk->ctr;
     } else {
-      cudaGetLastError();
-      a.plan = make_plan<Cfg>(M, N, K, workers, 1);   // no scratch (allocation failed, or first use inside a stream capture): run undivided
+      cudaGetLastError();   // no scratch (allocation failed, or first use inside a stream capture): run undivided
+      a.plan = undivided(a.plan);
     }
   }
   a.M = M; a.N = N; a.K = K;
@@ -448,20 +474,25 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
     else if (b_bytes >= kStream && a_bytes <= kL2Keep && m_tiles <= 4) { a.hint_b = ptx::kL2EvictFirst; a.hint_a = ptx::kL2EvictLast; }
   }
   // a co-resident mode the device cannot hold (refused before anything ran) falls back to the undivided schedule
-  auto undivided = [&](int err) {
+  auto or_undivided = [&](int err) {
     if (err != int(cudaErrorCooperativeLaunchTooLarge) && err != int(cudaErrorLaunchOutOfResources)) return err;
     cudaGetLastError();
-    a.plan = make_plan<Cfg>(M, N, K, workers, 1);
+    a.plan = undivided(a.plan);
     return launch_mode<Cfg, kPlain>(di, a);
   };
-  if constexpr (kCanStream) {
-    if (a.plan.sk_tiles > 0) return undivided(launch_mode<Cfg, kStreamK>(di, a));
-  }
-  if constexpr (Cfg::SPLIT_K && (MODES & (1u << kClusterSplitK))) {
-    if (a.plan.cluster_reduce) return launch_mode<Cfg, kClusterSplitK>(di, a);
-  }
-  if constexpr (Cfg::SPLIT_K && (MODES & (1u << kWorkspaceSplitK))) {
-    if (a.plan.splits > 1) return undivided(launch_mode<Cfg, kWorkspaceSplitK>(di, a));
+  // plan() only picks a mode for which has_mode holds; the `if constexpr` keeps the others from being instantiated
+  switch (a.plan.mode) {
+    case kStreamK:
+      if constexpr (has_mode<Cfg, MODES>(kStreamK)) return or_undivided(launch_mode<Cfg, kStreamK>(di, a));
+      break;
+    case kClusterSplitK:
+      if constexpr (has_mode<Cfg, MODES>(kClusterSplitK)) return launch_mode<Cfg, kClusterSplitK>(di, a);
+      break;
+    case kWorkspaceSplitK:
+      if constexpr (has_mode<Cfg, MODES>(kWorkspaceSplitK)) return or_undivided(launch_mode<Cfg, kWorkspaceSplitK>(di, a));
+      break;
+    case kPlain:
+      break;
   }
   return launch_mode<Cfg, kPlain>(di, a);
 }

@@ -8,10 +8,8 @@
 #include "hgemm_host.cuh"
 
 // The K-modes a per-shape translation unit needs compiled: its own (from the tuned split code) and the plain fallback.
-#define B200_HGEMM_SHAPE_MODES(SPLITS)                                                                  \
-  ((1u << b200::kPlain) | ((SPLITS) >= 100 ? (1u << b200::kStreamK)                                     \
-                           : (SPLITS) > 1  ? (1u << b200::kWorkspaceSplitK)                              \
-                           : (SPLITS) < -1 ? (1u << b200::kClusterSplitK) : 0u))
+#define B200_HGEMM_SHAPE_MODES(SPLITS) \
+  ((1u << b200::kPlain) | (1u << b200::host::decode_splits(SPLITS).mode))
 
 #define B200_HGEMM_SHAPE_ENTRY(ACC_F32, BN, STAGES, CTA_GROUP, CLUSTER_M, CLUSTER_N, GROUP_M, SPLITS)                                       \
   extern "C" int b200_hgemm_shape_entry(const void* A, const void* B_kmajor, void* C, int M, int N, int K,    \

@@ -54,10 +54,6 @@ constexpr int kSmemLimit = 232448;   // 227 KB of dynamic shared memory per bloc
 // every launch — carries none of the three other epilogues.
 enum KMode : int { kPlain = 0, kWorkspaceSplitK = 1, kClusterSplitK = 2, kStreamK = 3 };
 
-#ifndef B200_HGEMM_NO_K_DECOMP
-#define B200_HGEMM_NO_K_DECOMP 0     // experiment: kernels without split-K / stream-K code
-#endif
-
 template <int BN_, int STAGES_, int CTA_GROUP_, bool ACC_F32_, int CLUSTER_M_ = 1, int CLUSTER_N_ = 1, int M_REP_ = 1, bool BF16_ = false>
 struct Config {
   static constexpr int BN = BN_;               // tile N (= wgmma N)
@@ -91,8 +87,8 @@ struct Config {
   static constexpr int EPI_ROWS = 16;                        // rows of one warp's share of a 64-row wgmma tile
   static constexpr int NUM_THREADS = kNumThreads;
   // which K-decompositions this configuration's kernel carries
-  static constexpr bool SPLIT_K = !B200_HGEMM_NO_K_DECOMP && CTA_GROUP_ * CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
-  static constexpr bool STREAM_K = !B200_HGEMM_NO_K_DECOMP && CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
+  static constexpr bool STREAM_K = CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
+  static constexpr bool SPLIT_K = STREAM_K && CTA_GROUP_ == 1;
   static constexpr int EPI_BYTES = 8 * EPI_ROWS * 64 * 2;    // 8 consumer warps x one staging buffer (sized for EPI_N = 64)
   static constexpr int BAR_BYTES = 256;
   // STAGES_ is the requested ring depth; on sm_90 every CTA of a pair holds the whole B tile, so the depth is capped

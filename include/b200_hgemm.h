@@ -79,12 +79,14 @@ int b200_hgemm_run_config(int acc_bits, int config_id, const void* A, const void
                           int M, int N, int K, int group_m, int max_ctas, int splits, void* stream);
 
 /* Host-only view of the kernel's schedule (no device needed): the work units worker `worker` runs, in order, on a
- * device with num_sms SMs, as triples (tile, first k-block, end k-block) written to units[3 * max_units]. Also
- * reports the number of workers (CTAs, CTA pairs or clusters) of the launch, the stream-K tile count, and per unit
- * the number of contributor units an owner unit waits for (NULL to skip). Returns the worker's unit count
- * (possibly > max_units) or a negative status. The same code walks the schedule inside the kernel. */
+ * device with num_sms SMs, as triples (tile, first k-block, end k-block) written to units[3 * max_units]. The plan
+ * is the one b200_hgemm_run_config makes for this `splits` request. Also reports the number of workers (CTAs, CTA
+ * pairs or clusters) of the launch, the stream-K tile count, the K-mode the request runs in (0 plain, 1 workspace
+ * split-K, 2 cluster split-K, 3 stream-K), and per unit the number of contributor units an owner unit waits for
+ * (each NULL to skip). Returns the worker's unit count (possibly > max_units) or a negative status. The same code
+ * walks the schedule inside the kernel. */
 int b200_hgemm_schedule_units(int config_id, int M, int N, int K, int splits, int num_sms, int worker, int* units,
-                              int max_units, int* num_workers, int* sk_tiles, int* contributors);
+                              int max_units, int* num_workers, int* sk_tiles, int* mode, int* contributors);
 
 /* End-to-end form with HOST buffers (pageable or pinned): copies A and B_kmajor to the device,
  * runs the GEMM and copies C back, synchronising before it returns. This is the call bench.py

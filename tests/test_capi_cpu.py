@@ -179,6 +179,88 @@ def test_stream_k_fills_the_partial_wave_and_balances_the_workers(built_libs):
     assert _check_schedule(cfgs[3], 512, 8192, 128, capi.STREAMK_TAIL)["sk_tiles"] == 0
 
 
+def test_schedule_names_the_k_mode_a_request_runs_in(built_libs):
+    cfgs = capi.configs()
+    s = _check_schedule(cfgs[3], 512, 8192, 8192, capi.STREAMK_TAIL)
+    assert s["mode"] == "stream-k"
+    # 512 x 512 with 128 x 128 tiles: 16 tiles, 64 k-blocks
+    s = _check_schedule(cfgs[1], 512, 512, 4096, -4)
+    assert s["mode"] == "cluster-split-k" and s["workers"] == 16 * 4 and s["sk_tiles"] == 0
+    s = _check_schedule(cfgs[1], 512, 512, 4096, 4)
+    assert s["mode"] == "split-k" and s["workers"] == 16 * 4 and s["sk_tiles"] == 0
+    # split-K needs single CTAs; stream-K no multicast cluster, no 32-wide tiles and no 256-row CTAs
+    assert _check_schedule(cfgs[3], 512, 512, 4096, 4)["mode"] == "plain"
+    for cid in (18, 12, 26):
+        assert _check_schedule(cfgs[cid], 512, 8192, 8192, capi.STREAMK_TAIL)["mode"] == "plain"
+    # 4 k-blocks cannot feed an 8-CTA cluster: the cluster is halved to 4 CTAs, one k-block each
+    s = _check_schedule(cfgs[1], 512, 512, 256, -8)
+    assert s["mode"] == "cluster-split-k" and s["workers"] == 16 * 4
+    assert all(len(u) == 1 and u[0][2] - u[0][1] == 1 for u in s["units"])
+
+
+PER_SHAPE_PLANS = r"""
+#include <cstdio>
+#include "cuda_l2_b200/csrc/hgemm_shape_entry.cuh"
+using namespace b200;
+using host::Plan;
+static bool same(const Plan& a, const Plan& b) {
+  return a.mode == b.mode && a.num_tiles == b.num_tiles && a.nkb == b.nkb && a.workers == b.workers &&
+         a.splits == b.splits && a.cluster_reduce == b.cluster_reduce && a.sk_tiles == b.sk_tiles;
+}
+static int bad = 0, lib_stream_k = 0, lib_split = 0;
+template <unsigned MODES, class Cfg>
+static void check(int code) {
+  const int dims[] = {64, 200, 512, 1024, 4096, 8192}, ks[] = {64, 256, 4096, 8192}, sms[] = {132, 100, 16};
+  for (int m : dims) for (int n : dims) for (int k : ks) for (int s : sms) {
+    const int w = s / Cfg::CLUSTER_CTAS;
+    auto all = [=] { return w; };
+    const Plan lib = host::plan<Cfg>(m, n, k, code, w, all), plain = host::plan<Cfg>(m, n, k, 1, w, all);
+    // a per-shape unit plans as the library does, except that its stream-K codes run plain
+    const Plan want = host::decode_splits(code).mode == kStreamK ? plain : lib;
+    if (!same(host::plan<Cfg, MODES>(m, n, k, code, w, all), want)) { ++bad; std::printf("per-shape %d %d %d %d %d\n", code, m, n, k, s); }
+    // without scratch, or refused, a co-resident launch runs as the plain request would (every cluster resident here)
+    if ((lib.mode == kWorkspaceSplitK || lib.mode == kStreamK) && !same(host::undivided(lib), plain)) { ++bad; std::printf("undivided %d %d %d %d %d\n", code, m, n, k, s); }
+    lib_stream_k += lib.mode == kStreamK;
+    lib_split += lib.mode == kWorkspaceSplitK || lib.mode == kClusterSplitK;
+  }
+}
+#define CHECK(CFG, CODE) check<B200_HGEMM_SHAPE_MODES(CODE), CFG>(CODE)
+int main() {
+  using Pair = Config<256, 6, 2, true>;
+  using Single = Config<128, 6, 1, true>;
+  using Multicast = Config<64, 8, 1, true, 1, 2>;
+  CHECK(Pair, 1); CHECK(Pair, 100); CHECK(Pair, 101); CHECK(Pair, -4);
+  CHECK(Single, 1); CHECK(Single, 4); CHECK(Single, -2); CHECK(Single, -8); CHECK(Single, 100); CHECK(Single, 101);
+  CHECK(Multicast, 100);
+  // a CTA pair planned for stream-K within 40 resident clusters keeps that bound when it runs undivided
+  const Plan sk = host::plan<Pair>(512, 8192, 8192, host::kStreamKTail, 66, [] { return 40; });
+  const Plan u = host::undivided(sk);
+  if (sk.mode != kStreamK || u.mode != kPlain || u.workers != 40 || u.sk_tiles != 0) { ++bad; std::printf("bound\n"); }
+  std::printf("library stream-K plans %d, split-K plans %d\n", lib_stream_k, lib_split);
+  return bad != 0 || lib_stream_k == 0 || lib_split == 0;
+}
+"""
+
+
+def test_per_shape_units_plan_like_the_library_but_run_stream_k_codes_plain(tmp_path):
+    """The per-shape translation units compile a subset of the K-modes (B200_HGEMM_SHAPE_MODES). Their plans, checked
+    by a host program built from the same headers: those of the library, except that a stream-K code runs plain there,
+    as it always has. Also: the undivided fallback of a divided plan."""
+    import shutil
+    import subprocess
+    from pathlib import Path
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    if not Path(nvcc).exists():
+        pytest.skip("nvcc not available")
+    src, exe = tmp_path / "plans.cu", tmp_path / "plans"
+    src.write_text(PER_SHAPE_PLANS)
+    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O1", f"-I{REPO}", str(src),
+                        "-o", str(exe)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-1500:]
+    r = subprocess.run([str(exe)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stdout[-1500:]
+
+
 def test_schedule_is_a_partition_for_random_problems(built_libs):
     """Randomised version of the coverage test: odd sizes, short and long K, restricted SM counts, every mode."""
     import random
