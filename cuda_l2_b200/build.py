@@ -61,11 +61,21 @@ def _headers() -> list[Path]:
 
 
 def build_capi(verbose: bool = False, force: bool = False) -> Path:
+    """The 16-bit kernels (b200_hgemm_capi.cu) and the e4m3 ones (b200_fp8_capi.cu) compile in parallel, then link
+    into one library."""
     LIB_DIR.mkdir(exist_ok=True)
     out = LIB_DIR / "libb200_hgemm.so"
-    src = CSRC / "b200_hgemm_capi.cu"
-    if force or _stale(out, [src] + _headers()):
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), str(src)], verbose)
+    srcs = [CSRC / "b200_hgemm_capi.cu", CSRC / "b200_fp8_capi.cu"]
+    if force or _stale(out, srcs + _headers()):
+        objs = [LIB_DIR / (src.stem + ".o") for src in srcs]
+        from concurrent.futures import ThreadPoolExecutor
+        with ThreadPoolExecutor(len(srcs)) as pool:
+            for f in [pool.submit(_run, [nvcc_path(), *ARCH_FLAGS, *COMMON, "-c", "-o", str(obj), str(src)], verbose)
+                      for src, obj in zip(srcs, objs)]:
+                f.result()
+        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs)], verbose)
+        for obj in objs:
+            obj.unlink()
     return out
 
 

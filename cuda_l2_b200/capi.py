@@ -42,6 +42,11 @@ def hgemm_lib() -> ctypes.CDLL:
         lib.b200_bgemm_f32acc.argtypes = [vp, vp, vp, vp, i, i, i, vp]
         lib.b200_bgemm_f32acc.restype = i
         lib.b200_bgemm_run_config.argtypes = [i, vp, vp, vp, i, i, i, i, i, i, vp]
+        lib.b200_fp8gemm.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, vp]
+        lib.b200_fp8gemm.restype = i
+        lib.b200_fp8gemm_run_config.argtypes = [i, i, vp, vp, vp, vp, vp, i, i, i, i, i, i, vp]
+        lib.b200_fp8gemm_run_config.restype = i
+        lib.b200_fp8gemm_select.argtypes = [i, i, i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
         lib.b200_hgemm_num_configs.restype = i
         lib.b200_hgemm_config_info.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
         lib.b200_hgemm_config_cluster.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(i)]
@@ -87,7 +92,7 @@ def exported_symbols() -> dict[str, list[str]]:
             "b200_hgemm_config_cluster", "b200_hgemm_config_m_rep", "b200_hgemm_config_stages_requested",
             "b200_hgemm_select_config", "b200_hgemm_select", "b200_hgemm_run_config", "b200_hgemm_host", "b200_hgemm_launch_count",
             "b200_hgemm_strerror", "b200_hgemm_schedule_units", "b200_hgemm_prewarm", "b200_hgemm_release",
-            "b200_bgemm_f32acc", "b200_bgemm_run_config",
+            "b200_bgemm_f32acc", "b200_bgemm_run_config", "b200_fp8gemm", "b200_fp8gemm_run_config", "b200_fp8gemm_select",
         ],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
@@ -162,6 +167,48 @@ def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = No
     else:
         st = lib.b200_hgemm_run_config(bits, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m, 0, splits, stream)
     _check(st, "b200 gemm")
+
+
+def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config_id: int | None = None,
+             group_m: int = 0, splits: int = 1) -> None:
+    """c[M,N] = (a[M,K] @ b_kmajor[N,K]^T) * scale_a * scale_b with ``float8_e4m3fn`` operands, fp32 accumulation and
+    one rounding to ``c``'s dtype (fp16 or bf16). ``scale_a`` / ``scale_b`` are one-element fp32 CUDA tensors, read when
+    the kernel runs. ``config_id`` pins one kernel configuration (tests; ``splits`` as in b200_hgemm_run_config);
+    default is the dispatcher."""
+    import torch
+
+    if a.dtype != torch.float8_e4m3fn or b_kmajor.dtype != torch.float8_e4m3fn:
+        raise B200HgemmError(f"a and b_kmajor must be torch.float8_e4m3fn, got {a.dtype}, {b_kmajor.dtype}")
+    if c.dtype not in (torch.half, torch.bfloat16):
+        raise B200HgemmError(f"c must be fp16 or bf16, got {c.dtype}")
+    for name, t in (("scale_a", scale_a), ("scale_b", scale_b)):
+        if t.dtype != torch.float32 or t.numel() != 1 or not t.is_cuda:
+            raise B200HgemmError(f"{name} must be a one-element fp32 CUDA tensor, got {t.dtype} {tuple(t.shape)} on {t.device}")
+    for name, t in (("a", a), ("b_kmajor", b_kmajor), ("c", c)):
+        if not t.is_cuda or not t.is_contiguous():
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    if a.dim() != 2 or b_kmajor.dim() != 2 or c.dim() != 2:
+        raise B200HgemmError(f"2-D operands expected: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
+    (m, k), (n, k2) = a.shape, b_kmajor.shape
+    if k2 != k or tuple(c.shape) != (m, n):
+        raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
+    lib = hgemm_lib()
+    out_bf16 = int(c.dtype == torch.bfloat16)
+    if config_id is None:
+        st = lib.b200_fp8gemm(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), scale_b.data_ptr(),
+                              out_bf16, m, n, k, stream)
+    else:
+        st = lib.b200_fp8gemm_run_config(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(),
+                                         scale_a.data_ptr(), scale_b.data_ptr(), m, n, k, group_m, 0, splits, stream)
+    _check(st, "b200_fp8gemm")
+
+
+def fp8_select(m: int, n: int, k: int) -> tuple[int, int, int]:
+    """(config id, rasterisation group, split-K factor) the dispatcher uses for an e4m3 problem."""
+    cid, gm, sp = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    _check(hgemm_lib().b200_fp8gemm_select(m, n, k, ctypes.byref(cid), ctypes.byref(gm), ctypes.byref(sp)),
+           "b200_fp8gemm_select")
+    return cid.value, gm.value, sp.value
 
 
 def hgemm_config(a, b_col_major, c, config_id: int, acc: str | int = "fp32", group_m: int = 0, max_ctas: int = 0,

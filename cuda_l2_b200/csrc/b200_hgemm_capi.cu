@@ -90,6 +90,11 @@ HostCtx& host_ctx(int dev) {
 
 }  // namespace
 
+namespace b200 {
+// One launch counter for the whole library: the e4m3 entry points (b200_fp8_capi.cu) count theirs here too.
+__attribute__((visibility("hidden"))) void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
+}  // namespace b200
+
 extern "C" {
 
 int b200_hgemm_num_configs(void) { return b200::kNumConfigs; }

@@ -27,6 +27,7 @@ enum Status : int {
   kBadConfig = -6,
   kNotHopper = -7,
   kNoScratch = -8,       // internal: no split-K scratch for this (device, stream) and none can be allocated now (stream capture)
+  kBadFp8K = -9,         // e4m3 operands: K % 16 == 0 (16-byte TMA strides at one byte per element)
   // > 0: a cudaError_t from the launch
 };
 
@@ -41,6 +42,7 @@ inline const char* status_string(int s) {
     case kBadConfig: return "unknown kernel configuration id";
     case kNotHopper: return "device is not compute capability 9.0 (sm_90a build)";
     case kNoScratch: return "split-K scratch unavailable (allocate it outside stream capture with b200_hgemm_prewarm)";
+    case kBadFp8K: return "e4m3 operands need K % 16 == 0 (16-byte row strides at one byte per element)";
     default: return s > 0 ? cudaGetErrorString(static_cast<cudaError_t>(s)) : "unknown error";
   }
 }
@@ -62,18 +64,24 @@ inline EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// Row-major fp16 matrix [rows, cols] (cols contiguous) -> 2-D tiled map, 128B swizzle,
-// box = {box_cols (64 or 32) columns, box_rows}. Out-of-bounds elements read as zero / are not written.
+// Element type of a tensor map. e4m3 is encoded as UINT8: TMA only moves the bytes, wgmma interprets them.
+enum class Elem : int { kF16 = 0, kBF16 = 1, kE4M3 = 2 };
+constexpr int elem_bytes(Elem e) { return e == Elem::kE4M3 ? 1 : 2; }
+template <class Cfg> constexpr Elem operand_elem() { return Cfg::E4M3 ? Elem::kE4M3 : Cfg::BF16 ? Elem::kBF16 : Elem::kF16; }
+template <class Cfg> constexpr Elem output_elem() { return Cfg::BF16 ? Elem::kBF16 : Elem::kF16; }
+
+// Row-major matrix [rows, cols] (cols contiguous) -> 2-D tiled map, box = {box_cols columns, box_rows}, swizzled over the
+// box's inner extent in bytes (128 or 64). Out-of-bounds elements read as zero / are not written.
 inline int encode_2d(CUtensorMap* map, const void* ptr, int rows, int cols, int box_rows, int box_cols = kBlockK,
-                     bool bf16 = false) {
+                     Elem elem = Elem::kF16) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return kNoDriver;
   cuuint64_t dims[2] = {cuuint64_t(cols), cuuint64_t(rows)};
-  cuuint64_t strides[1] = {cuuint64_t(cols) * 2};
+  cuuint64_t strides[1] = {cuuint64_t(cols) * elem_bytes(elem)};
   cuuint32_t box[2] = {cuuint32_t(box_cols), cuuint32_t(box_rows)};
   cuuint32_t estr[2] = {1, 1};
-  // the swizzle span equals the box's inner extent: 64 fp16 = 128 B, 32 fp16 = 64 B
-  const CUtensorMapSwizzle swz = box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  // the swizzle span equals the box's inner extent: 64 fp16 or 128 e4m3 = 128 B, 32 fp16 = 64 B
+  const CUtensorMapSwizzle swz = box_cols * elem_bytes(elem) == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   // experiment hook: B200_HGEMM_L2_PROMOTION = 0 (none) | 1 (64 B) | 2 (128 B) | 3 (256 B, the default)
   static const CUtensorMapL2promotion promo = [] {
     const char* e = std::getenv("B200_HGEMM_L2_PROMOTION");
@@ -81,17 +89,20 @@ inline int encode_2d(CUtensorMap* map, const void* ptr, int rows, int cols, int 
     return v == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : v == 1 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B
          : v == 2 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
   }();
-  CUresult r = fn(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  const CUtensorMapDataType dt = elem == Elem::kE4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                               : elem == Elem::kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUresult r = fn(map, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? kOk : kEncodeFailed;
 }
 
 // Small direct-mapped cache of encoded maps: benchmark loops re-present the same few pointers
-// (the caching allocator recycles them), and an encode costs about a microsecond of host time.
+// (the caching allocator recycles them), and an encode costs about a microsecond of host time. The key carries the
+// element type: an e4m3 and an fp16 map of the same pointer and dimensions differ.
 struct MapKey {
-  const void* ptr; int rows, cols, box_rows, box_cols; bool bf16;
+  const void* ptr; int rows, cols, box_rows, box_cols; Elem elem;
   bool operator==(const MapKey& o) const {
-    return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows && box_cols == o.box_cols && bf16 == o.bf16;
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows && box_cols == o.box_cols && elem == o.elem;
   }
 };
 struct MapCache {
@@ -101,14 +112,14 @@ struct MapCache {
   bool valid[kSlots];
   MapCache() { std::memset(valid, 0, sizeof(valid)); }
   // Copies the map out: two operands of one call may share a slot, so a pointer into the cache would alias.
-  int get(const void* ptr, int rows, int cols, int box_rows, CUtensorMap* out, int box_cols = kBlockK, bool bf16 = false) {
-    MapKey k{ptr, rows, cols, box_rows, box_cols, bf16};
+  int get(const void* ptr, int rows, int cols, int box_rows, CUtensorMap* out, int box_cols = kBlockK, Elem elem = Elem::kF16) {
+    MapKey k{ptr, rows, cols, box_rows, box_cols, elem};
     uint64_t h = (reinterpret_cast<uint64_t>(ptr) >> 8) * 0x9E3779B97F4A7C15ull;
     h ^= uint64_t(uint32_t(rows)) * 0xC2B2AE3D27D4EB4Full + uint64_t(uint32_t(cols)) * 0x165667B19E3779F9ull +
          uint64_t(box_rows) * 131u + uint64_t(box_cols);
     int slot = int((h >> 32) % kSlots);
     if (!(valid[slot] && keys[slot] == k)) {
-      int st = encode_2d(&maps[slot], ptr, rows, cols, box_rows, box_cols, bf16);
+      int st = encode_2d(&maps[slot], ptr, rows, cols, box_rows, box_cols, elem);
       if (st != kOk) { valid[slot] = false; return st; }
       keys[slot] = k;
       valid[slot] = true;
@@ -144,6 +155,20 @@ inline int validate(const void* A, const void* Bt, const void* C, int M, int N, 
   if ((K % 8) || (N % 8)) return kBadAlignment;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
     return kBadAlignment;
+  return kOk;
+}
+
+// e4m3 operands: one byte per element, so K % 16 == 0 keeps the A / Bt row strides at 16 bytes; C is 16-bit as before.
+// The two per-tensor scales are fp32 values in device memory.
+inline int validate_fp8(const void* A, const void* Bt, const void* C, const float* scale_a, const float* scale_b, int M,
+                        int N, int K) {
+  if (!A || !Bt || !C || !scale_a || !scale_b) return kNullPointer;
+  if (M <= 0 || N <= 0 || K <= 0) return kBadShape;
+  if (K % 16) return kBadFp8K;
+  if (N % 8) return kBadAlignment;
+  if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
+    return kBadAlignment;
+  if ((reinterpret_cast<uintptr_t>(scale_a) | reinterpret_cast<uintptr_t>(scale_b)) & 3) return kBadAlignment;
   return kOk;
 }
 
@@ -255,7 +280,7 @@ Plan plan(int M, int N, int K, int splits, int max_workers, ResidentClusters&& r
   const int num_m_blocks = (M + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M);
   const int num_n_blocks = (N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N);
   p.num_tiles = num_m_blocks * num_n_blocks;
-  p.nkb = (K + kBlockK - 1) / kBlockK;
+  p.nkb = (K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
   p.splits = 1;
   // Clusters must fit inside a GPC, so fewer than SMs / cluster size may be resident at once. Larger clusters are
   // always sized to what fits; CTA pairs only for stream-K, whose owners wait for contributors that must therefore be
@@ -362,6 +387,7 @@ struct LaunchArgs {
   Plan plan;
   float* ws; unsigned* ctr; __half* c;
   uint64_t hint_a, hint_b;
+  Scales scales;
   cudaStream_t stream;
 };
 
@@ -419,13 +445,13 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   cfg.attrs = attr;
   cfg.numAttrs = na;
   cudaError_t e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                                     a.plan.splits, a.plan.sk_tiles, a.ws, a.ctr, a.c, a.hint_a, a.hint_b);
+                                     a.plan.splits, a.plan.sk_tiles, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
   if (e != cudaSuccess && coop && pdl && e != cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
     coop_pdl_ok = false;               // the pair of attributes is not accepted here: cooperative only, from now on
     cfg.numAttrs = na - 1;
     e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                           a.plan.splits, a.plan.sk_tiles, a.ws, a.ctr, a.c, a.hint_a, a.hint_b);
+                           a.plan.splits, a.plan.sk_tiles, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
   }
   return e == cudaSuccess ? kOk : int(e);
 }
@@ -433,20 +459,21 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
 // group_m <= 0 selects the default rasterisation width. max_ctas <= 0 means "all SMs". `splits`: 1 none, > 1 workspace
 // split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
 // mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
-// kernels instead of four; the plain mode is always available as fallback).
+// kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor scales of an
+// e4m3 configuration (device pointers), unused otherwise.
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
-           int group_m = 0, int max_ctas = 0, int splits = 1) {
-  int st = validate(A, Bt, C, M, N, K);
+           int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}) {
+  int st = Cfg::E4M3 ? validate_fp8(A, Bt, C, scales.a, scales.b, M, N, K) : validate(A, Bt, C, M, N, K);
   if (st != kOk) return st;
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
 
   LaunchArgs a{};
   MapCache& cache = map_cache();
-  if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, kBlockK, Cfg::BF16)) != kOk) return st;
-  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, kBlockK, Cfg::BF16)) != kOk) return st;
-  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, Cfg::BF16)) != kOk) return st;
+  if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, operand_elem<Cfg>())) != kOk) return st;
+  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, operand_elem<Cfg>())) != kOk) return st;
+  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output_elem<Cfg>())) != kOk) return st;
 
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = plan<Cfg, MODES>(M, N, K, splits, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
@@ -462,12 +489,13 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   a.M = M; a.N = N; a.K = K;
   a.group_m = group_m > 0 ? group_m : (Cfg::CTA_GROUP == 2 ? 8 : 16);
   a.c = static_cast<__half*>(C);
+  a.scales = scales;
   a.stream = stream;
   // L2 eviction priorities: when one operand is streamed (about) once while the other is re-read by every tile row
   // or column and is small enough to live in L2, keep the small one and let the streamed one go first.
   a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
   if (cache_hints_enabled()) {
-    const size_t a_bytes = size_t(M) * K * 2, b_bytes = size_t(N) * K * 2;
+    const size_t a_bytes = size_t(M) * K * Cfg::OP_BYTES, b_bytes = size_t(N) * K * Cfg::OP_BYTES;
     const int n_tiles = (N + Cfg::BN - 1) / Cfg::BN, m_tiles = (M + Cfg::TILE_M - 1) / Cfg::TILE_M;
     constexpr size_t kL2Keep = size_t(20) << 20, kStream = size_t(40) << 20;   // against the 50 MB L2
     if (a_bytes >= kStream && b_bytes <= kL2Keep && n_tiles <= 4) { a.hint_a = ptx::kL2EvictFirst; a.hint_b = ptx::kL2EvictLast; }

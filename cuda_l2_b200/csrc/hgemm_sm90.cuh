@@ -1,5 +1,6 @@
 // H100 (sm_90a) HGEMM:  C[M,N] (fp16) = A[M,K] (fp16, K-contiguous) * Bt[N,K]^T (fp16, K-contiguous)
-// with fp32 (F32F16F16F32) or fp16 (F16F16F16F16) accumulation in registers.
+// with fp32 (F32F16F16F32) or fp16 (F16F16F16F16) accumulation in registers. The same pipeline also runs bf16 operands
+// (bf16 out) and e4m3 operands with per-tensor scales (fp16 or bf16 out), both with fp32 accumulation.
 //
 // Replaces, for this repository's device type, the per-shape kernels the reference ships
 // (reference: kernels/a100_F32F16F16F32/4096_4096_4096.cu:22-177 mainloop+epilogue, :179-279 launcher;
@@ -41,8 +42,9 @@
 
 namespace b200 {
 
+constexpr int kBlockKBytes = 128;    // one k-block = one 128-byte swizzle row: 64 16-bit or 128 8-bit elements
 constexpr int kBlockK = 64;          // 64 fp16 = 128 B = one swizzle row
-constexpr int kWgmmaK = 16;          // K per wgmma.mma_async (16-bit operands)
+constexpr int kWgmmaK = 16;          // K per wgmma.mma_async (16-bit operands; k32 = the same 32 bytes for 8-bit ones)
 constexpr int kBlockM = 128;         // rows per CTA (per 128-row block: two consumer warpgroups x 64 rows)
 constexpr int kNumThreads = 384;     // warpgroup 0: producer (warp 0 issues), warpgroups 1-2: MMA + epilogue
 constexpr int kEpiWarp0 = 4;         // first consumer warp
@@ -54,7 +56,8 @@ constexpr int kSmemLimit = 232448;   // 227 KB of dynamic shared memory per bloc
 // every launch — carries none of the three other epilogues.
 enum KMode : int { kPlain = 0, kWorkspaceSplitK = 1, kClusterSplitK = 2, kStreamK = 3 };
 
-template <int BN_, int STAGES_, int CTA_GROUP_, bool ACC_F32_, int CLUSTER_M_ = 1, int CLUSTER_N_ = 1, int M_REP_ = 1, bool BF16_ = false>
+template <int BN_, int STAGES_, int CTA_GROUP_, bool ACC_F32_, int CLUSTER_M_ = 1, int CLUSTER_N_ = 1, int M_REP_ = 1, bool BF16_ = false,
+          bool E4M3_ = false>
 struct Config {
   static constexpr int BN = BN_;               // tile N (= wgmma N)
   static constexpr int CTA_GROUP = CTA_GROUP_; // 1: one CTA per 128-row tile; 2: a pair of CTAs sharing the B tile
@@ -63,6 +66,13 @@ struct Config {
   // wgmma type and the epilogue's convert differ. bf16 products accumulate in fp32 only.
   static constexpr bool BF16 = BF16_;
   static_assert(!BF16_ || ACC_F32_, "bf16 operands accumulate in fp32");
+  // e4m3 operands (float8_e4m3fn): the operand type is then separate from the output type, which BF16 names (fp16 or
+  // bf16). The k-block stays 128 bytes, now 128 elements; stage sizes, descriptors and the wgmma count per k-block are
+  // unchanged. The per-tensor scales multiply the finished fp32 sum once, just before the one rounding to the output.
+  static constexpr bool E4M3 = E4M3_;
+  static_assert(!E4M3_ || ACC_F32_, "e4m3 operands accumulate in fp32");
+  static constexpr int OP_BYTES = E4M3_ ? 1 : 2;             // bytes per operand element
+  static constexpr int BLOCK_K = kBlockKBytes / OP_BYTES;    // operand elements per k-block
   // Multicast cluster: CLUSTER_M x CLUSTER_N groups (single CTAs or CTA pairs) work on a block of adjacent tiles.
   // On sm_90 a CTA pair is two CTAs along M that multicast B between them, so the cluster is MCAST_M x CLUSTER_N
   // CTAs, cluster rank = mi + MCAST_M * cn with mi = cm * CTA_GROUP + (position inside the pair).
@@ -110,6 +120,17 @@ struct Config {
 };
 
 constexpr int kMaxSplitTiles = 256;   // split-K is only used when tiles * splits <= #SMs
+
+// Per-tensor scales of an e4m3 launch: one fp32 value each, in device memory (null for the 16-bit operand types).
+struct Scales { const float* a; const float* b; };
+
+// The factor applied to the finished fp32 sum before it is rounded to the output type: fp32(scale_a * scale_b) for e4m3
+// operands, read where it is used (after the grid dependency wait, so a preceding kernel may have just written it).
+template <class Cfg>
+__device__ __forceinline__ float output_scale(const Scales& s) {
+  if constexpr (Cfg::E4M3) return __fmul_rn(*s.a, *s.b);
+  else return 1.f;
+}
 
 // Where an accumulator register lands in the 64-row tile of its warpgroup: packed pair p (two adjacent columns) of
 // warp w, lane l sits at row 16w + l/4 + 8(p%2), columns 8(p/2) + 2(l%4) + {0,1} (wgmma_sm90.cuh).
@@ -163,13 +184,13 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
 //   phase 1  every split writes its 128 x BN fp32 partial tile to the workspace slot (tile, split);
 //   barrier  a per-tile arrival counter in global memory (release/acquire at gpu scope);
 //   phase 2  split s sums a contiguous 1/splits slice of the tile's rows over ALL partials in the fixed
-//            order s' = 0..splits-1 (deterministic), rounds once to fp16 and stores to C.
+//            order s' = 0..splits-1 (deterministic), scales it (e4m3), rounds once to fp16 and stores to C.
 // The last split to finish phase 2 zeroes both counters, so the next launch on the stream starts clean.
 template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void splitk_epilogue(const Reg (&d)[NR], int e, int row_base, int lane, int tile, int split,
                                                 int splits, int m_base, int n0, int M, int N, float* __restrict__ ws,
                                                 unsigned* __restrict__ ctr, __half* __restrict__ C,
-                                                uint32_t red_smem, uint32_t red_bar) {
+                                                uint32_t red_smem, uint32_t red_bar, const Scales& scales) {
   using namespace ptx;
   constexpr int BN = Cfg::BN;
   float* slot = ws + (size_t(tile) * splits + split) * (kBlockM * BN);
@@ -208,6 +229,7 @@ __device__ __forceinline__ void splitk_epilogue(const Reg (&d)[NR], int e, int r
         bulk_load_1d(red_smem + uint32_t(sp) * slice_bytes, tile_ws + size_t(sp) * (kBlockM * BN), slice_bytes, red_bar);
     }
     mbar_wait(red_bar, 0);
+    const float scale = output_scale<Cfg>(scales);
     constexpr int V = BN / 4;      // float4 per row
     for (int i = e; i < (r1 - r0) * V; i += kConsumerThreads) {
       const int r = r0 + i / V, c4 = i % V;
@@ -217,6 +239,10 @@ __device__ __forceinline__ void splitk_epilogue(const Reg (&d)[NR], int e, int r
       for (int sp = 0; sp < splits; ++sp) {   // fixed order: deterministic
         const float4 p = ld_shared_v4f(red_smem + uint32_t(sp) * slice_bytes + uint32_t(i) * 16u);
         acc.x += p.x; acc.y += p.y; acc.z += p.z; acc.w += p.w;
+      }
+      if constexpr (Cfg::E4M3) {
+        acc.x = __fmul_rn(acc.x, scale); acc.y = __fmul_rn(acc.y, scale);
+        acc.z = __fmul_rn(acc.z, scale); acc.w = __fmul_rn(acc.w, scale);
       }
       uint2 out;
       out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
@@ -255,10 +281,12 @@ __device__ __forceinline__ void cluster_splitk_park(const Reg (&d)[NR], int row_
 
 template <class Cfg>
 __device__ __forceinline__ void cluster_splitk_reduce(int e, int split, int splits, int m_base, int n0, int M, int N,
-                                                      uint32_t part_smem, __half* __restrict__ C) {
+                                                      uint32_t part_smem, __half* __restrict__ C,
+                                                      const Scales& scales) {
   using namespace ptx;
   constexpr int BN = Cfg::BN;
   constexpr int V = BN / 4;
+  const float scale = output_scale<Cfg>(scales);
   const int rows_per = kBlockM / splits;            // splits is 2, 4 or 8
   const int r0 = split * rows_per;
   uint32_t peer[8];
@@ -276,6 +304,10 @@ __device__ __forceinline__ void cluster_splitk_reduce(int e, int split, int spli
         const float4 v = ld_dsmem_v4f(peer[p] + off);
         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
       }
+    }
+    if constexpr (Cfg::E4M3) {
+      acc.x = __fmul_rn(acc.x, scale); acc.y = __fmul_rn(acc.y, scale);
+      acc.z = __fmul_rn(acc.z, scale); acc.w = __fmul_rn(acc.w, scale);
     }
     uint2 out;
     out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
@@ -323,7 +355,8 @@ __device__ __forceinline__ void streamk_contribute(const Reg (&d)[NR], int t, in
 }
 
 // Owner: the partials of `n` contributors (slots slot0, slot0 + slot_stride, ... — increasing k) added to the own
-// accumulator in fp32 in that fixed order; fp16 accumulators are widened, summed and rounded once. The flags are
+// accumulator in fp32 in that fixed order; fp16 accumulators are widened, summed and rounded once. The images are
+// unscaled: an e4m3 owner's plain epilogue applies the scales to the finished sum. The flags are
 // lowered afterwards (this warp is their only reader, and the next writer is a later launch).
 template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void streamk_own(Reg (&d)[NR], int t, int ew, int lane, const uint4* __restrict__ ws,
@@ -380,8 +413,8 @@ __device__ __forceinline__ void streamk_own(Reg (&d)[NR], int t, int ew, int lan
 
 template <class Cfg, int KMODE = kPlain>
 __global__ void __launch_bounds__(kNumThreads, 1)
-hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {64, A_BOX_ROWS}
-                const __grid_constant__ CUtensorMap tmap_b,   // Bt [N,K]  box {64, B_BOX_ROWS}
+hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {BLOCK_K, A_BOX_ROWS}
+                const __grid_constant__ CUtensorMap tmap_b,   // Bt [N,K]  box {BLOCK_K, B_BOX_ROWS}
                 const __grid_constant__ CUtensorMap tmap_c,   // C  [M,N]  box {EPI_N, EPI_ROWS}
                 int M, int N, int K, int group_m,
                 int splits_arg,                   // split-K factor (modes kWorkspaceSplitK / kClusterSplitK: one unit per CTA)
@@ -390,7 +423,8 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
                 unsigned* __restrict__ splitk_ctr,   // [2][kMaxSplitTiles] split-K arrive / done counters, then the
                                                      // stream-K flags; all zero between launches
                 __half* __restrict__ c_raw,       // C base pointer, used by the split-K reductions' direct stores
-                uint64_t hint_a, uint64_t hint_b  /* L2 eviction priority of the A / B loads (ptx::kL2Evict*) */) {
+                uint64_t hint_a, uint64_t hint_b, // L2 eviction priority of the A / B loads (ptx::kL2Evict*)
+                Scales scales                     /* e4m3: the per-tensor scales (not read by the 16-bit kernels) */) {
   constexpr int BN = Cfg::BN;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int EM = Cfg::MCAST_M;
@@ -427,7 +461,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   const int num_m_blocks = (M + Cfg::CTA_M * EM - 1) / (Cfg::CTA_M * EM);
   const int num_n_blocks = (N + BN * CN - 1) / (BN * CN);
   const int num_tiles = num_m_blocks * num_n_blocks;
-  const int num_k_blocks = (K + kBlockK - 1) / kBlockK;
+  const int num_k_blocks = (K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
   const int num_workers = gridDim.x / Cfg::CLUSTER_CTAS;   // clusters (or single CTAs)
   const int worker = blockIdx.x / Cfg::CLUSTER_CTAS;
   // A work unit is (tile, k-block range), see hgemm_schedule.cuh. splits == 1: whole tiles walked persistently
@@ -488,10 +522,10 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
             mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);   // the whole stage lands here, from this CTA and its peers
             const uint32_t dst_a = smem_a + stage * Cfg::A_STAGE_BYTES + a_slice;
             const uint32_t dst_b = smem_b + stage * Cfg::B_STAGE_BYTES + b_slice;
-            if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * kBlockK, m0, mask_a, hint_a);
-            else tma_load_2d_hint(dst_a, &tmap_a, full, kb * kBlockK, m0, hint_a);
-            if constexpr (EM > 1) tma_load_2d_mcast_hint(dst_b, &tmap_b, full, kb * kBlockK, n0, mask_b, hint_b);
-            else tma_load_2d_hint(dst_b, &tmap_b, full, kb * kBlockK, n0, hint_b);
+            if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, mask_a, hint_a);
+            else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, hint_a);
+            if constexpr (EM > 1) tma_load_2d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, mask_b, hint_b);
+            else tma_load_2d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, hint_b);
           }
           __syncwarp();
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -509,7 +543,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   } else {
     setmaxnreg_inc<kConsumerRegs>();
     // ===== consumers: warpgroup wg owns rows [wg * 64 * MR, (wg + 1) * 64 * MR) of the CTA's tile =====
-    using W = Wgmma<BN, Cfg::ACC_F32, Cfg::BF16>;
+    using W = Wgmma<BN, Cfg::ACC_F32, Cfg::BF16 && !Cfg::E4M3, Cfg::E4M3>;
     using Reg = typename W::Reg;
     constexpr int NR = W::kRegs;
     const int wg = warp / 4 - 1;
@@ -554,7 +588,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {   // four wgmmas of 32 bytes of K each, for every operand type
 #pragma unroll
           for (int r = 0; r < MR; ++r)
             W::mma(da + uint64_t(r * ((64 * kBlockK * 2) >> 4) + 2 * k), db + uint64_t(2 * k), acc[r],
@@ -602,8 +636,19 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         ck_m_base = m_cta; ck_n0 = n0; ck_split = worker - tile * splits;   // the reduction runs after the cluster barrier below
       } else if constexpr (KMODE == kWorkspaceSplitK) {
         splitk_epilogue<Cfg>(acc[0], t, wg * 64 + wq * 16, lane, tile, worker - tile * splits, splits, m_cta, n0, M, N,
-                             splitk_ws, splitk_ctr, c_raw, smem_a, bar_splitk);
+                             splitk_ws, splitk_ctr, c_raw, smem_a, bar_splitk, scales);
       } else {
+        if constexpr (Cfg::E4M3) {
+          // the finished sums are scaled in place, right before the epilogue rounds them: the scale is read per unit,
+          // after the main loop, and is dead before the epilogue's own temporaries are live
+          const float scale = output_scale<Cfg>(scales);
+#pragma unroll
+          for (int r = 0; r < MR; ++r)
+#pragma unroll
+            for (int i = 0; i < NR; ++i) acc[r][i] = __fmul_rn(acc[r][i], scale);
+#pragma unroll
+          for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
+        }
 #pragma unroll
         for (int r = 0; r < MR; ++r) {
           const int row0 = m_cta + (wg * MR + r) * 64 + wq * 16;
@@ -618,7 +663,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
     __syncwarp();
     if constexpr (KMODE == kClusterSplitK) {
       cluster_sync_all();   // every split's partial tile is parked in its CTA's shared memory
-      cluster_splitk_reduce<Cfg>(t, ck_split, splits, ck_m_base, ck_n0, M, N, smem_a, c_raw);
+      cluster_splitk_reduce<Cfg>(t, ck_split, splits, ck_m_base, ck_n0, M, N, smem_a, c_raw, scales);
       __syncwarp();
       cluster_sync_all();   // no CTA leaves (and frees its smem) while a peer may still be reading it
     } else if constexpr (Cfg::CLUSTER_CTAS > 1) {

@@ -10,10 +10,15 @@ the nearest grid shape — so deployment is a plain operator:
   operands (bf16 always accumulates in fp32); ``acc`` = "fp32" | "fp16".
 * :class:`B200Linear`: ``y = x @ W^T (+ b)`` for any leading dimensions; :func:`replace_linear_modules` swaps the
   eligible ``nn.Linear`` layers of a model in place.
+* ``torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)``: ``float8_e4m3fn`` operands in the same
+  layout, per-tensor fp32 scales as one-element CUDA tensors, ``(a @ b_kmajor^T) * scale_a * scale_b`` rounded once to
+  ``out_dtype`` (fp16 or bf16) — ``torch._scaled_mm`` with per-tensor scales and fast accumulation.
+* :class:`B200Fp8Linear`: inference-only FP8 version of an ``nn.Linear`` (weight quantised once, activation per call).
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernel on explicitly
-transposed copies, so a fine-tuning loop works, at the price of two transposes per layer.
+transposed copies, so a fine-tuning loop works, at the price of two transposes per layer. The FP8 operator has no
+gradient: a backward through it raises.
 """
 from __future__ import annotations
 
@@ -157,4 +162,118 @@ def replace_linear_modules(model: nn.Module, acc: str = "fp32", skip: tuple[str,
     return done
 
 
-__all__ = ["hgemm", "B200Linear", "replace_linear_modules", "linear_supported"]
+# ------------------------------------------------------------------------------------------ FP8 (e4m3), inference only
+E4M3_MAX = 448.0   # largest finite float8_e4m3fn value
+_OUT_DTYPES = (torch.float16, torch.bfloat16)
+
+torch.library.define(f"{_LIB}::fp8_gemm",
+                     "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor")
+
+
+def _check_fp8_operands(a, b_kmajor, scale_a, scale_b, out_dtype) -> tuple[int, int, int]:
+    if a.dim() != 2 or b_kmajor.dim() != 2:
+        raise capi.B200HgemmError(f"fp8_gemm wants 2-D operands, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}")
+    if a.dtype != torch.float8_e4m3fn or b_kmajor.dtype != torch.float8_e4m3fn:
+        raise capi.B200HgemmError(f"fp8_gemm wants float8_e4m3fn operands, got {a.dtype} and {b_kmajor.dtype}")
+    if out_dtype not in _OUT_DTYPES:
+        raise capi.B200HgemmError(f"out_dtype must be torch.float16 or torch.bfloat16, got {out_dtype}")
+    for name, t in (("scale_a", scale_a), ("scale_b", scale_b)):
+        if t.dtype != torch.float32 or t.numel() != 1:
+            raise capi.B200HgemmError(f"{name} must be a one-element float32 tensor, got {t.dtype} {tuple(t.shape)}")
+    m, k = a.shape
+    n, k2 = b_kmajor.shape
+    if k2 != k:
+        raise capi.B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} (K-major: [N, K])")
+    if k % 16 or n % 8:
+        raise capi.B200HgemmError(f"fp8_gemm needs K % 16 == 0 and N % 8 == 0 (16-byte TMA strides), got N={n}, K={k}")
+    return m, n, k
+
+
+@torch.library.impl(f"{_LIB}::fp8_gemm", "CUDA")
+def _fp8_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype):
+    m, n, _ = _check_fp8_operands(a, b_kmajor, scale_a, scale_b, out_dtype)
+    a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
+    c = torch.empty((m, n), dtype=out_dtype, device=a.device)
+    if m == 0:
+        return c
+    with torch.cuda.device(a.device):
+        capi.fp8_gemm(a, b_kmajor, c, scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous(),
+                      stream=torch.cuda.current_stream(a.device).cuda_stream)
+    return c
+
+
+@torch.library.impl(f"{_LIB}::fp8_gemm", "CPU")
+def _fp8_gemm_cpu(a, b_kmajor, scale_a, scale_b, out_dtype):
+    raise capi.B200HgemmError("cuda_l2_b200::fp8_gemm has no CPU implementation (and no fallback): move the tensors to an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::fp8_gemm")
+def _fp8_gemm_fake(a, b_kmajor, scale_a, scale_b, out_dtype):
+    m, n, _ = _check_fp8_operands(a, b_kmajor, scale_a, scale_b, out_dtype)
+    return a.new_empty((m, n), dtype=out_dtype)
+
+
+def _fp8_gemm_no_backward(ctx, grad_c):
+    raise capi.B200HgemmError("cuda_l2_b200::fp8_gemm is inference only: it has no gradient (train with the fp16 / bf16 "
+                              "operator and quantise afterwards)")
+
+
+# No gradient formula: without this, autograd would only warn and hand back no gradient for the inputs.
+torch.library.register_autograd(f"{_LIB}::fp8_gemm", _fp8_gemm_no_backward)
+
+
+def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
+             out_dtype: torch.dtype = torch.float16) -> torch.Tensor:
+    """(``a`` [M,K] @ ``b_kmajor`` [N,K]^T) * scale_a * scale_b -> [M,N] ``out_dtype``, e4m3 operands (see the module docstring)."""
+    return torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)
+
+
+def quantize_e4m3(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per-tensor quantisation on x's device: scale = amax(|x|) / 448 (a one-element fp32 tensor), q = e4m3(x / scale).
+    Torch ops only, no host synchronisation."""
+    scale = (x.abs().amax().float() / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny).reshape(1)
+    q = (x.float() / scale).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return q, scale
+
+
+class B200Fp8Linear(nn.Module):
+    """Inference-only FP8 ``nn.Linear``: the weight is quantised once to e4m3 with a per-tensor scale (buffers
+    ``weight_fp8`` / ``weight_scale``); every call quantises the activation per tensor on the device and runs
+    ``cuda_l2_b200::fp8_gemm``, then adds the bias (shared with the source layer). No ``.item()`` and no host
+    synchronisation, so the forward can be captured in a CUDA graph. Needs in_features % 16 == 0, out_features % 8 == 0."""
+
+    @classmethod
+    def from_linear(cls, lin: nn.Linear, out_dtype: torch.dtype | None = None) -> "B200Fp8Linear":
+        out_dtype = out_dtype or lin.weight.dtype
+        if out_dtype not in _OUT_DTYPES or lin.in_features % 16 or lin.out_features % 8:
+            raise capi.B200HgemmError(f"cannot convert {lin} to FP8: needs in_features % 16 == 0, out_features % 8 == 0 "
+                                      f"and an fp16 / bf16 output type (got {out_dtype})")
+        new = cls.__new__(cls)
+        nn.Module.__init__(new)
+        new.in_features, new.out_features, new.out_dtype = lin.in_features, lin.out_features, out_dtype
+        with torch.no_grad():
+            w_q, w_scale = quantize_e4m3(lin.weight)
+        new.register_buffer("weight_fp8", w_q)
+        new.register_buffer("weight_scale", w_scale)
+        new.bias = lin.bias                                  # shared with the source layer
+        return new
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        lead = x.shape[:-1]
+        x2 = x.reshape(-1, self.in_features)
+        if x2.shape[0] == 0:
+            y = x2.new_empty((0, self.out_features), dtype=self.out_dtype)
+        else:
+            x_q, x_scale = quantize_e4m3(x2)
+            y = torch.ops.cuda_l2_b200.fp8_gemm(x_q, self.weight_fp8, x_scale, self.weight_scale, self.out_dtype)
+        if self.bias is not None:
+            y = y + self.bias
+        return y.view(*lead, self.out_features)
+
+    def extra_repr(self) -> str:
+        return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
+                f"out_dtype={self.out_dtype}")
+
+
+__all__ = ["hgemm", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
+           "B200Fp8Linear"]

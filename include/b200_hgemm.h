@@ -47,6 +47,25 @@ int b200_bgemm_f32acc(const void* A, const void* B_rowmajor, const void* B_kmajo
 int b200_bgemm_run_config(int config_id, const void* A, const void* B_kmajor, void* C,
                           int M, int N, int K, int group_m, int max_ctas, int splits, void* stream);
 
+/* FP8 variant (no reference kernel exists for it): A [M,K] and B_kmajor [N,K] hold float8_e4m3fn values (one byte
+ * each, K contiguous); C [M,N] is fp16 (out_bf16 = 0) or bf16 (out_bf16 = 1), row-major, fully overwritten:
+ *     C = RN_out( (sum_k A[m,k] * B_kmajor[n,k]) * fp32(scale_a * scale_b) )
+ * The sum is accumulated by the tensor core in fp32 (one accumulator per element, the equivalent of fast accumulation:
+ * Hopper's FP8 MMA keeps fewer than 23 mantissa bits in its running sum); the scale is applied once, to the finished sum,
+ * right before the one rounding to the output type, in every K-mode. scale_a and scale_b point to one fp32 value each in
+ * DEVICE memory (4-byte aligned) and are read when the kernel runs, after the stream's preceding work: a graph replay
+ * sees their current contents. The same as torch._scaled_mm(A, B_kmajor.t(), scale_a, scale_b, out_dtype) with
+ * per-tensor scales. Requires K % 16 == 0 (16-byte row strides; status -9 otherwise), N % 8 == 0 and 16-byte aligned A,
+ * B_kmajor and C. The dispatcher takes the fp32-accumulate table's choice for (M, N, K / 2), the fp16 problem that moves
+ * the same bytes per k-block. b200_fp8gemm_run_config is b200_hgemm_run_config for this data type (same `splits`
+ * codes); b200_fp8gemm_select reports the dispatcher's choice. */
+int b200_fp8gemm(const void* A, const void* B_kmajor, void* C, const void* scale_a, const void* scale_b, int out_bf16,
+                 int M, int N, int K, void* stream);
+int b200_fp8gemm_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
+                            const void* scale_a, const void* scale_b, int M, int N, int K, int group_m, int max_ctas,
+                            int splits, void* stream);
+int b200_fp8gemm_select(int M, int N, int K, int* config_id, int* group_m, int* splits);
+
 /* The reference fixes tile/stage/swizzle per (M,N,K) at compile time inside each
  * kernels/<dev>/<M>_<N>_<K>.cu (e.g. a100_F32F16F16F32/4096_4096_4096.cu:185-200,305-309). Here the
  * per-shape choice is a table lookup; these calls expose it for the tuner and the tests. */

@@ -1,0 +1,257 @@
+"""FP8 (e4m3) GEMM on the H100: bit-exact against the oracle on small-integer operands (every configuration, both output
+types, ragged shapes, every K-mode, both kinds of scale), scales read at run time (stream order, graph replay), guard
+bands, random data at production sizes, and the B200Fp8Linear module.
+
+Exactness. Hopper's FP8 wgmma keeps fewer bits in its running sum than fp32 does (public reports: about 14). On small
+integers every partial sum is an integer far below that (|c| <= 2047 here; the tests assert it of their data), so the
+kernel, the oracle and torch must agree bit for bit there, in every summation order and K-mode.
+
+Tolerance on N(0,1) data (per-tensor amax / 448 quantisation, the truth being the fp32 product of the quantised
+operands, scaled): err = max |C - truth| / rms(truth). Measured on an H100 80GB HBM3, two seeds per case:
+  4096^3            fp16 out 0.0227-0.0235   bf16 out 0.0284-0.0306
+  2048x11008x4096   fp16 out 0.0234-0.0251   bf16 out 0.0312
+  16x4096x4096      fp16 out 0.0127-0.0168   bf16 out 0.0176-0.0196
+The output rounding alone accounts for 0.002 (fp16) and 0.016 (bf16) of that; torch._scaled_mm without fast
+accumulation reached 0.0024 (fp16) there, so the rest is the FP8 tensor core's reduced-precision sum. At all three
+shapes the kernel's output was bit-identical to torch._scaled_mm(use_fast_accum=True). RANDOM_TOL = 0.05 is the largest
+measured figure (0.0312) with margin; the kernel must also stay within 2 x RANDOM_TOL of _scaled_mm's fast path.
+B200Fp8Linear against the fp16 / bf16 nn.Linear it came from (1024 -> 512, N(0,1) input): 0.150-0.176 measured, bound
+0.25 — e4m3 quantisation of both operands, not the GEMM, dominates that.
+"""
+import numpy as np
+import pytest
+import torch
+
+from oracle import fp8 as fp8_oracle
+from cuda_l2_b200 import capi
+
+pytestmark = pytest.mark.gpu
+
+E4 = torch.float8_e4m3fn
+POW2, NON_POW2 = (0.5, 4.0), (0.3, 1.7)
+RANDOM_TOL = 0.05   # max |C - truth| / rms(truth) on N(0,1) data; measured up to 0.0312 (module docstring)
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _device():
+    if not torch.cuda.is_available() or torch.cuda.get_device_capability(0)[0] != 9:
+        pytest.skip("needs an H100 (compute capability 9.0)")
+    torch.cuda.set_device(0)
+
+
+def small_ints(shape, lim, seed):
+    g = torch.Generator().manual_seed(seed)
+    return (torch.randint(0, 2 * lim + 1, shape, generator=g) - lim).float().to(E4)
+
+
+def scale_tensors(pair):
+    return (torch.tensor([pair[0]], dtype=torch.float32, device="cuda"),
+            torch.tensor([pair[1]], dtype=torch.float32, device="cuda"))
+
+
+def codes(t):
+    return t.cpu().view(torch.uint8).numpy()
+
+
+def bits(c):
+    return c.view(torch.int16).cpu().numpy().view(np.uint16)
+
+
+def want_bits(a, bt, pair, out_dtype):
+    # the exact domain: every sum a small integer
+    assert float((a.float() @ bt.float().t()).abs().max()) <= 2047
+    return fp8_oracle.fp8gemm_f32acc(codes(a), codes(bt), pair[0], pair[1], out_dtype == torch.bfloat16)
+
+
+def run(a, bt, pair, out_dtype, **kw):
+    c = torch.full((a.shape[0], bt.shape[0]), float("nan"), dtype=out_dtype, device="cuda")
+    sa, sb = scale_tensors(pair)
+    capi.fp8_gemm(a.cuda(), bt.cuda(), c, sa, sb, **kw)
+    torch.cuda.synchronize()
+    return c
+
+
+def test_every_configuration_both_outputs_bit_exact():
+    m, n = 520, 392                                  # off tile multiples in M and N
+    before = capi.launch_count()
+    launches = 0
+    for out_dtype, k in ((torch.float16, 400), (torch.bfloat16, 240)):   # K off the 128-element k-block
+        a, bt = small_ints((m, k), 1, 1), small_ints((n, k), 1, 2)
+        want = {p: want_bits(a, bt, p, out_dtype) for p in (POW2, NON_POW2)}
+        for cfg in capi.configs():
+            pair = (POW2, NON_POW2)[(cfg["id"] + (out_dtype == torch.bfloat16)) % 2]
+            got = bits(run(a, bt, pair, out_dtype, config_id=cfg["id"]))
+            launches += 1
+            assert np.array_equal(got, want[pair]), (cfg, out_dtype, pair)
+    assert capi.launch_count() - before == launches
+
+
+@pytest.mark.parametrize("out_dtype", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("mnk", [(200, 328, 144), (1, 8, 16), (129, 136, 272), (16, 4096, 1024), (1000, 1032, 1040)])
+def test_dispatched_ragged_shapes_bit_exact(mnk, out_dtype):
+    m, n, k = mnk
+    a, bt = small_ints((m, k), 1, m + k), small_ints((n, k), 1, n + 3 * k)
+    for pair in (POW2, NON_POW2):
+        assert np.array_equal(bits(run(a, bt, pair, out_dtype)), want_bits(a, bt, pair, out_dtype)), (mnk, pair)
+
+
+# (config, M, N, K, splits code, K-mode the planner must choose). The planner sees an e4m3 problem (M, N, K) as the fp16
+# problem (M, N, K / 2): both have K / 128 k-blocks of 128 bytes, which is what capi.schedule is asked about.
+K_MODES = [
+    (1, 512, 512, 8192, 1, "plain"),
+    (1, 512, 512, 8192, 4, "split-k"),
+    (1, 512, 512, 8192, 16, "split-k"),
+    (1, 512, 512, 8192, -2, "cluster-split-k"),
+    (1, 512, 512, 8192, -4, "cluster-split-k"),
+    (1, 512, 512, 8192, -8, "cluster-split-k"),
+    (1, 512, 512, 8192, 100, "stream-k"),
+    (4, 1280, 1792, 1024, 101, "stream-k"),               # CTA pairs: 70 tiles on 66 workers
+]
+
+
+@pytest.mark.parametrize("cfg,m,n,k,splits,mode", K_MODES)
+def test_every_k_mode_bit_exact(cfg, m, n, k, splits, mode):
+    assert capi.schedule(cfg, m, n, k // 2, splits)["mode"] == mode
+    a, bt = small_ints((m, k), 1, 10 + splits), small_ints((n, k), 1, 20 + splits)
+    for out_dtype, pair in ((torch.float16, POW2), (torch.bfloat16, NON_POW2)):
+        got = bits(run(a, bt, pair, out_dtype, config_id=cfg, splits=splits))
+        assert np.array_equal(got, want_bits(a, bt, pair, out_dtype)), (cfg, splits, out_dtype)
+
+
+def test_scale_written_just_before_the_gemm_is_the_one_used():
+    from cuda_l2_b200 import ops
+    m, n, k = 256, 256, 512
+    a, bt = small_ints((m, k), 1, 5).cuda(), small_ints((n, k), 1, 6).cuda()
+    sa, sb = scale_tensors((1.0, 0.5))
+    ops.fp8_gemm(a, bt, sa, sb, torch.float16)
+    for v in (4.0, 0.3, 0.125):
+        sa.fill_(v)                                          # a torch kernel, same stream, right before the GEMM
+        y = ops.fp8_gemm(a, bt, sa, sb, torch.float16)
+        assert np.array_equal(bits(y), want_bits(a, bt, (v, 0.5), torch.float16)), v
+
+
+def test_graph_replay_reads_the_current_scales():
+    from cuda_l2_b200 import ops
+    m, n, k = 512, 512, 8192                                 # dispatched with a K-decomposition
+    a, bt = small_ints((m, k), 1, 7).cuda(), small_ints((n, k), 1, 8).cuda()
+    sa, sb = scale_tensors((1.0, 1.0))
+    s = torch.cuda.Stream()
+    capi.prewarm(s.cuda_stream)
+    with torch.cuda.stream(s):
+        ops.fp8_gemm(a, bt, sa, sb, torch.bfloat16)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, stream=s):
+        y = ops.fp8_gemm(a, bt, sa, sb, torch.bfloat16)
+    for pair in ((0.5, 2.0), NON_POW2, (0.25, 0.25)):
+        sa.fill_(pair[0]); sb.fill_(pair[1])
+        g.replay()
+        torch.cuda.synchronize()
+        assert np.array_equal(bits(y), want_bits(a, bt, pair, torch.bfloat16)), pair
+
+
+def test_unprewarmed_capture_runs_undivided():
+    m, n, k = 512, 512, 8192
+    a, bt = small_ints((m, k), 1, 9).cuda(), small_ints((n, k), 1, 10).cuda()
+    sa, sb = scale_tensors(POW2)
+    c = torch.empty((m, n), dtype=torch.float16, device="cuda")
+    s = torch.cuda.Stream()                                  # a stream that has never run a split-K launch
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, stream=s):
+        capi.fp8_gemm(a, bt, c, sa, sb, stream=s.cuda_stream, config_id=1, splits=4)
+    c.fill_(float("nan"))
+    g.replay()
+    torch.cuda.synchronize()
+    assert np.array_equal(bits(c), want_bits(a, bt, POW2, torch.float16))
+
+
+@pytest.mark.parametrize("cfg,splits", [(1, 1), (3, 1), (26, 1), (14, 1), (1, 4), (1, -4), (1, 100), (30, 1)])
+def test_guard_bands(cfg, splits):
+    m, n, k = 200, 328, 4096
+    a, bt = small_ints((m, k), 1, 11).cuda(), small_ints((n, k), 1, 12).cuda()
+    sa, sb = scale_tensors(POW2)
+    pad = 4096
+    buf = torch.full((m * n + 2 * pad,), -7.0, dtype=torch.float16, device="cuda")
+    c = buf[pad:pad + m * n].view(m, n)
+    c.fill_(float("nan"))
+    capi.fp8_gemm(a, bt, c, sa, sb, config_id=cfg, splits=splits)
+    torch.cuda.synchronize()
+    assert np.array_equal(bits(c), want_bits(a, bt, POW2, torch.float16))
+    assert bool((buf[:pad] == -7).all()) and bool((buf[pad + m * n:] == -7).all())
+
+
+def quantised_randn(shape, seed):
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    x = torch.randn(shape, device="cuda", generator=g)
+    s = (x.abs().amax() / 448).reshape(1)
+    return (x / s).to(E4), s
+
+
+def scaled_mm(a, bt, sa, sb, out_dtype, fast):
+    return torch._scaled_mm(a, bt.t(), scale_a=sa.reshape(()), scale_b=sb.reshape(()), out_dtype=out_dtype,
+                            use_fast_accum=fast)
+
+
+@pytest.mark.parametrize("mnk", [(4096, 4096, 4096), (2048, 11008, 4096), (16, 4096, 4096)])
+@pytest.mark.parametrize("out_dtype", [torch.float16, torch.bfloat16])
+def test_random_data_within_the_measured_tolerance(mnk, out_dtype):
+    from cuda_l2_b200 import ops
+    m, n, k = mnk
+    a, sa = quantised_randn((m, k), 1)
+    bt, sb = quantised_randn((n, k), 2)
+    y = ops.fp8_gemm(a, bt, sa, sb, out_dtype).float()
+    prev = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        truth = (a.float() @ bt.float().t()) * (sa * sb)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev
+    rms = truth.pow(2).mean().sqrt()
+    err = float((y - truth).abs().max() / rms)
+    fast = scaled_mm(a, bt, sa, sb, out_dtype, True).float()
+    err_fast = float((fast - truth).abs().max() / rms)
+    assert err <= RANDOM_TOL, (mnk, out_dtype, err, err_fast)
+    assert float((y - fast).abs().max() / rms) <= 2 * RANDOM_TOL, (mnk, out_dtype, err, err_fast)
+
+
+@pytest.mark.parametrize("bias", [True, False])
+@pytest.mark.parametrize("lead", [(64,), (4, 33)])
+def test_fp8_linear_agrees_with_its_fp16_source(bias, lead):
+    from torch import nn
+
+    from cuda_l2_b200 import ops
+    torch.manual_seed(3)
+    lin = nn.Linear(1024, 512, bias=bias, dtype=torch.float16, device="cuda")
+    m = ops.B200Fp8Linear.from_linear(lin)
+    x = torch.randn(*lead, 1024, dtype=torch.float16, device="cuda")
+    with torch.no_grad():
+        y, ref = m(x), lin(x)
+    assert y.shape == ref.shape and y.dtype == torch.float16
+    rel = float((y.float() - ref.float()).abs().max() / ref.float().pow(2).mean().sqrt())
+    assert rel <= 0.25, rel          # measured 0.150-0.176 (module docstring): e4m3 keeps 3 mantissa bits
+
+
+def test_fp8_linear_captures_in_a_graph_and_has_no_backward():
+    from torch import nn
+
+    from cuda_l2_b200 import ops
+    lin = nn.Linear(512, 256, dtype=torch.bfloat16, device="cuda")
+    m = ops.B200Fp8Linear.from_linear(lin)
+    x = torch.randn(128, 512, dtype=torch.bfloat16, device="cuda")
+    s = torch.cuda.Stream()
+    capi.prewarm(s.cuda_stream)
+    with torch.no_grad():
+        with torch.cuda.stream(s):
+            m(x)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=s):
+            y = m(x)
+        for seed in (1, 2):
+            x.copy_(torch.randn(128, 512, generator=torch.Generator(device="cuda").manual_seed(seed), device="cuda"))
+            g.replay()
+            torch.cuda.synchronize()
+            assert torch.equal(y, m(x))
+    xg = torch.randn(8, 512, dtype=torch.bfloat16, device="cuda", requires_grad=True)
+    with pytest.raises(Exception, match="inference only"):
+        m(xg).sum().backward()
