@@ -10,6 +10,7 @@ from __future__ import annotations
 
 import ctypes
 from pathlib import Path
+from typing import NamedTuple
 
 LIB_DIR = Path(__file__).resolve().parent / "lib"
 _hgemm = None
@@ -137,6 +138,66 @@ def hgemm(a, b_col_major, c, acc: str | int = "fp32", stream: int | None = None)
     _check(fn(a.data_ptr(), None, b_col_major.data_ptr(), c.data_ptr(), m, n, k, stream), "b200_hgemm")
 
 
+class GemmType(NamedTuple):
+    """A data-type variant of the kernel family (include/b200_hgemm.h)."""
+    k_align: int    # K % k_align == 0: 16-byte operand rows
+    scale: object   # dtype of the per-tensor scales the variant takes (e4m3 operands: float32), None if it takes none
+
+    def fits(self, n: int, k: int) -> bool:
+        """Whether an [M,K] x [N,K] problem meets the 16-byte row rule (TMA strides) of this variant."""
+        return n % 8 == 0 and k % self.k_align == 0
+
+
+_GEMM_TYPES: dict = {}   # (operand dtype, output dtype, accumulator bits) -> GemmType, filled on first use
+
+
+def gemm_type(operand, output, acc: str | int = "fp32") -> GemmType | None:
+    """The variant with these operand and output dtypes and accumulator, or None: the kernel family has none."""
+    if not _GEMM_TYPES:
+        import torch
+        h, b, e, f = torch.float16, torch.bfloat16, torch.float8_e4m3fn, torch.float32
+        _GEMM_TYPES.update({(h, h, 32): GemmType(8, None), (h, h, 16): GemmType(8, None), (b, b, 32): GemmType(8, None),
+                            (e, h, 32): GemmType(16, f), (e, b, 32): GemmType(16, f)})
+    return _GEMM_TYPES.get((operand, output, ACC_BITS.get(acc)))
+
+
+def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tuple = ()) -> tuple[int, int, int]:
+    """(M, N, K) of a[M,K] @ b_kmajor[N,K]^T -> ``out_dtype``, by the rules of the variant the dtypes and ``acc`` name:
+    2-D operands of one dtype, a shared K, 16-byte rows, one-element fp32 scales exactly for a scaled variant.
+    Checks shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
+    try:
+        (m, k), (n, k2) = a.shape, b_kmajor.shape
+    except ValueError:
+        raise B200HgemmError(f"2-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
+    dtype = a.dtype
+    t = gemm_type(dtype, out_dtype, acc) if b_kmajor.dtype == dtype else None
+    if t is None:
+        raise B200HgemmError(f"no kernel for {dtype} x {b_kmajor.dtype} -> {out_dtype} with acc={acc!r} (fp16 with "
+                             "fp32 or fp16 accumulation, bf16 with fp32, e4m3 -> fp16 / bf16 with fp32)")
+    if len(scales) != (0 if t.scale is None else 2):
+        raise B200HgemmError(f"{dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
+    for name, s in zip(("scale_a", "scale_b"), scales):
+        if s.dtype != t.scale or s.numel() != 1:
+            raise B200HgemmError(f"{name} must be a one-element {t.scale} tensor, got {s.dtype} {tuple(s.shape)}")
+    if k2 != k:
+        raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} (K-major: [N, K])")
+    if not t.fits(n, k):
+        raise B200HgemmError(f"{dtype} operands need N % 8 == 0 and K % {t.k_align} == 0 (16-byte TMA strides), "
+                             f"got N={n}, K={k}")
+    return m, n, k
+
+
+def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = ()) -> tuple[int, int, int]:
+    """check_operands for c = a @ b_kmajor^T, all of them (scales included) contiguous CUDA tensors, c of shape [M,N]."""
+    for name, x in zip(("a", "b_kmajor", "c", "scale_a", "scale_b"), (a, b_kmajor, c, *scales)):
+        if not x.is_cuda or not x.is_contiguous():
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    m, n, k = check_operands(a, b_kmajor, c.dtype, acc, scales)
+    if c.shape != (m, n):
+        raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
+    return m, n, k
+
+
 def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = None, config_id: int | None = None,
                 group_m: int = 0, splits: int = 1) -> None:
     """c[M,N] = a[M,K] @ b_kmajor[N,K]^T with the operands' dtype deciding the kernel family: fp16 (fp32 or fp16
@@ -144,19 +205,10 @@ def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = No
     ``config_id`` pins one kernel configuration (tests); default is the dispatcher."""
     import torch
 
-    if a.dtype not in (torch.half, torch.bfloat16) or b_kmajor.dtype != a.dtype or c.dtype != a.dtype:
-        raise B200HgemmError(f"operands must all be fp16 or all bf16, got {a.dtype}, {b_kmajor.dtype}, {c.dtype}")
-    for name, t in (("a", a), ("b_kmajor", b_kmajor), ("c", c)):
-        if not t.is_cuda or not t.is_contiguous():
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
-    (m, k), (n, k2) = a.shape, b_kmajor.shape
-    if k2 != k or tuple(c.shape) != (m, n):
-        raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
+    m, n, k = _kmajor_operands(a, b_kmajor, c, acc)
     lib = hgemm_lib()
     bits = ACC_BITS[acc]
     if a.dtype == torch.bfloat16:
-        if bits != 32:
-            raise B200HgemmError("bf16 operands accumulate in fp32 only")
         if config_id is None:
             st = lib.b200_bgemm_f32acc(a.data_ptr(), None, b_kmajor.data_ptr(), c.data_ptr(), m, n, k, stream)
         else:
@@ -177,21 +229,7 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     default is the dispatcher."""
     import torch
 
-    if a.dtype != torch.float8_e4m3fn or b_kmajor.dtype != torch.float8_e4m3fn:
-        raise B200HgemmError(f"a and b_kmajor must be torch.float8_e4m3fn, got {a.dtype}, {b_kmajor.dtype}")
-    if c.dtype not in (torch.half, torch.bfloat16):
-        raise B200HgemmError(f"c must be fp16 or bf16, got {c.dtype}")
-    for name, t in (("scale_a", scale_a), ("scale_b", scale_b)):
-        if t.dtype != torch.float32 or t.numel() != 1 or not t.is_cuda:
-            raise B200HgemmError(f"{name} must be a one-element fp32 CUDA tensor, got {t.dtype} {tuple(t.shape)} on {t.device}")
-    for name, t in (("a", a), ("b_kmajor", b_kmajor), ("c", c)):
-        if not t.is_cuda or not t.is_contiguous():
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
-    if a.dim() != 2 or b_kmajor.dim() != 2 or c.dim() != 2:
-        raise B200HgemmError(f"2-D operands expected: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
-    (m, k), (n, k2) = a.shape, b_kmajor.shape
-    if k2 != k or tuple(c.shape) != (m, n):
-        raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
+    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b))
     lib = hgemm_lib()
     out_bf16 = int(c.dtype == torch.bfloat16)
     if config_id is None:

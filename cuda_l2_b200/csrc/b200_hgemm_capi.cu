@@ -1,8 +1,8 @@
-// libb200_hgemm.so — C-ABI entry points declared in include/b200_hgemm.h.
-// Holds every kernel configuration and the per-shape dispatcher. No torch, no CUTLASS, no cuBLAS.
+// libb200_hgemm.so — C-ABI entry points declared in include/b200_hgemm.h: the 16-bit variants (fp16 with fp32 or fp16
+// accumulation, bf16), the configuration table and schedule queries, the host-buffer entry and resource management.
+// The e4m3 variants are in b200_fp8_capi.cu. No torch, no CUTLASS, no cuBLAS.
 #include "../../include/b200_hgemm.h"
 
-#include <atomic>
 #include <cstdlib>
 #include <map>
 #include <memory>
@@ -13,27 +13,7 @@
 
 namespace {
 
-std::atomic<unsigned long long> g_launches{0};
-constexpr int kBf16Acc32 = 0xB32;   // internal selector of run(): bf16 operands, fp32 accumulation
-
-template <bool kAccF32, bool kBf16 = false>
-int run_config(int id, const void* A, const void* Bt, void* C, int M, int N, int K, int group_m, int max_ctas,
-               int splits, cudaStream_t s) {
-  using namespace b200;
-  int st;
-  switch (id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                      \
-  case ID:                                                                                         \
-    st = host::launch<Config<BN, STAGES, CG, kAccF32, CM, CN, MR, kBf16>>(A, Bt, C, M, N, K, s, group_m, max_ctas, splits); \
-    break;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      return host::kBadConfig;
-  }
-  if (st == host::kOk) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return st;
-}
+using b200::host::GemmType;
 
 template <class Cfg>
 int schedule_units(int M, int N, int K, int splits, int num_sms, int worker, int* units, int max_units,
@@ -63,14 +43,8 @@ int schedule_units(int M, int N, int K, int splits, int num_sms, int worker, int
 
 const b200::ConfigDesc* config_desc(int id) { return id >= 0 && id < b200::kNumConfigs ? &b200::kConfigs[id] : nullptr; }
 
-int run(int acc_bits, int id, const void* A, const void* Bt, void* C, int M, int N, int K, int group_m,
-        int max_ctas, int splits, void* stream) {
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (acc_bits == 32) return run_config<true>(id, A, Bt, C, M, N, K, group_m, max_ctas, splits, s);
-  if (acc_bits == 16) return run_config<false>(id, A, Bt, C, M, N, K, group_m, max_ctas, splits, s);
-  if (acc_bits == kBf16Acc32) return run_config<true, true>(id, A, Bt, C, M, N, K, group_m, max_ctas, splits, s);
-  return b200::host::kBadConfig;
-}
+// The fp16 variant with `acc_bits` (32 or 16) of accumulation.
+GemmType fp16_type(int acc_bits) { return acc_bits == 32 ? GemmType::kF16Acc32 : GemmType::kF16Acc16; }
 
 constexpr int kHostBlocks = 8;   // at most this many row blocks in the pipelined host entry
 struct HostCtx {
@@ -89,11 +63,6 @@ HostCtx& host_ctx(int dev) {
 }
 
 }  // namespace
-
-namespace b200 {
-// One launch counter for the whole library: the e4m3 entry points (b200_fp8_capi.cu) count theirs here too.
-__attribute__((visibility("hidden"))) void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
-}  // namespace b200
 
 extern "C" {
 
@@ -144,13 +113,13 @@ int b200_hgemm_config_m_rep(int config_id) {
 int b200_hgemm_select_config(int acc_bits, int M, int N, int K) {
   if (acc_bits != 32 && acc_bits != 16) return b200::host::kBadConfig;
   if (M <= 0 || N <= 0 || K <= 0) return b200::host::kBadShape;
-  return b200::dispatch::select(acc_bits, M, N, K).config_id;
+  return b200::dispatch::select(fp16_type(acc_bits), M, N, K).config_id;
 }
 
 int b200_hgemm_select(int acc_bits, int M, int N, int K, int* config_id, int* group_m, int* splits) {
   if (acc_bits != 32 && acc_bits != 16) return b200::host::kBadConfig;
   if (M <= 0 || N <= 0 || K <= 0) return b200::host::kBadShape;
-  const b200::dispatch::Choice ch = b200::dispatch::select(acc_bits, M, N, K);
+  const b200::dispatch::Choice ch = b200::dispatch::select(fp16_type(acc_bits), M, N, K);
   if (config_id) *config_id = ch.config_id;
   if (group_m) *group_m = ch.group_m;
   if (splits) *splits = ch.splits;
@@ -159,37 +128,31 @@ int b200_hgemm_select(int acc_bits, int M, int N, int K, int* config_id, int* gr
 
 int b200_hgemm_run_config(int acc_bits, int config_id, const void* A, const void* B_kmajor, void* C, int M,
                           int N, int K, int group_m, int max_ctas, int splits, void* stream) {
-  return run(acc_bits, config_id, A, B_kmajor, C, M, N, K, group_m, max_ctas, splits, stream);
+  if (acc_bits == 32)
+    return b200::run_config<GemmType::kF16Acc32>(config_id, A, B_kmajor, C, {}, M, N, K, group_m, max_ctas, splits, stream);
+  if (acc_bits == 16)
+    return b200::run_config<GemmType::kF16Acc16>(config_id, A, B_kmajor, C, {}, M, N, K, group_m, max_ctas, splits, stream);
+  return b200::host::kBadConfig;
 }
 
 int b200_hgemm_f32acc(const void* A, const void* /*B_rowmajor*/, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
-  int st = b200::host::validate(A, B_kmajor, C, M, N, K);
-  if (st) return st;
-  const b200::dispatch::Choice ch = b200::dispatch::select(32, M, N, K);
-  return run(32, ch.config_id, A, B_kmajor, C, M, N, K, ch.group_m, 0, ch.splits, stream);
+  return b200::dispatch::gemm<GemmType::kF16Acc32>(A, B_kmajor, C, {}, M, N, K, stream);
 }
 
 int b200_hgemm_f16acc(const void* A, const void* /*B_rowmajor*/, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
-  int st = b200::host::validate(A, B_kmajor, C, M, N, K);
-  if (st) return st;
-  const b200::dispatch::Choice ch = b200::dispatch::select(16, M, N, K);
-  return run(16, ch.config_id, A, B_kmajor, C, M, N, K, ch.group_m, 0, ch.splits, stream);
+  return b200::dispatch::gemm<GemmType::kF16Acc16>(A, B_kmajor, C, {}, M, N, K, stream);
 }
 
 int b200_bgemm_f32acc(const void* A, const void* /*B_rowmajor*/, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
-  int st = b200::host::validate(A, B_kmajor, C, M, N, K);
-  if (st) return st;
-  // same data movement and the same MMA rate as the fp16 / fp32-accumulate kernel: its tuned table applies
-  const b200::dispatch::Choice ch = b200::dispatch::select(32, M, N, K);
-  return run(kBf16Acc32, ch.config_id, A, B_kmajor, C, M, N, K, ch.group_m, 0, ch.splits, stream);
+  return b200::dispatch::gemm<GemmType::kBF16>(A, B_kmajor, C, {}, M, N, K, stream);
 }
 
 int b200_bgemm_run_config(int config_id, const void* A, const void* B_kmajor, void* C, int M, int N, int K,
                           int group_m, int max_ctas, int splits, void* stream) {
-  return run(kBf16Acc32, config_id, A, B_kmajor, C, M, N, K, group_m, max_ctas, splits, stream);
+  return b200::run_config<GemmType::kBF16>(config_id, A, B_kmajor, C, {}, M, N, K, group_m, max_ctas, splits, stream);
 }
 
 int b200_hgemm_host(int acc_bits, const void* hA, const void* hB_kmajor, void* hC, int M, int N, int K) {
@@ -305,7 +268,7 @@ int b200_hgemm_release(void) {
   return e == cudaSuccess ? 0 : int(e);
 }
 
-unsigned long long b200_hgemm_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
+unsigned long long b200_hgemm_launch_count(void) { return b200::g_launches.load(std::memory_order_relaxed); }
 
 const char* b200_hgemm_strerror(int status) { return b200::host::status_string(status); }
 

@@ -9,6 +9,8 @@
 // 29 / 30: four CTA pairs in a 2 x 2 multicast cluster (8 CTAs: both operands fetched from L2 once per two pairs).
 // CLUSTER_M x CLUSTER_N > 1: TMA-multicast clusters of groups (single CTAs or CTA pairs): A shared along N, B along M.
 #pragma once
+#include <atomic>
+
 #include "hgemm_host.cuh"
 
 #define B200_HGEMM_CONFIGS(X) \
@@ -63,4 +65,31 @@ constexpr ConfigDesc kConfigs[kNumConfigs] = {
     B200_HGEMM_CONFIGS(B200_DESC)
 #undef B200_DESC
 };
+
+// Kernel launches the library has issued (b200_hgemm_launch_count). One counter for every translation unit of the
+// library; hidden, so that no other shared object's copy is bound to it.
+__attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_launches{0};
+
+// Launch configuration `id` of variant T. An instantiation compiles the kernels of all configurations for T, so each
+// translation unit of the library instantiates only the variants it exports.
+template <host::GemmType T>
+int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, int M, int N, int K, int group_m,
+               int max_ctas, int splits, void* stream) {
+  constexpr host::GemmTypeTraits t = host::traits(T);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int st;
+  switch (id) {
+#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                    \
+  case ID:                                                                                                       \
+    st = host::launch<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16(), t.e4m3()>>(A, Bt, C, M, N, K, s, group_m, \
+                                                                                         max_ctas, splits, scales); \
+    break;
+    B200_HGEMM_CONFIGS(B200_CASE)
+#undef B200_CASE
+    default:
+      return host::kBadConfig;
+  }
+  if (st == host::kOk) g_launches.fetch_add(1, std::memory_order_relaxed);
+  return st;
+}
 }  // namespace b200

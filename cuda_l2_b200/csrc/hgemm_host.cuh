@@ -67,8 +67,34 @@ inline EncodeTiledFn encode_fn() {
 // Element type of a tensor map. e4m3 is encoded as UINT8: TMA only moves the bytes, wgmma interprets them.
 enum class Elem : int { kF16 = 0, kBF16 = 1, kE4M3 = 2 };
 constexpr int elem_bytes(Elem e) { return e == Elem::kE4M3 ? 1 : 2; }
-template <class Cfg> constexpr Elem operand_elem() { return Cfg::E4M3 ? Elem::kE4M3 : Cfg::BF16 ? Elem::kBF16 : Elem::kF16; }
-template <class Cfg> constexpr Elem output_elem() { return Cfg::BF16 ? Elem::kBF16 : Elem::kF16; }
+
+// The data-type variants of the kernel family. Everything the host does differently per variant (which kernels it
+// instantiates, the argument rules, the tuned-table entry) reads the variant's row of kGemmTypes.
+enum class GemmType : int { kF16Acc32, kF16Acc16, kBF16, kE4M3F16, kE4M3BF16 };
+struct GemmTypeTraits {
+  Elem operand, output;
+  bool acc_f32;       // fp32 accumulation (fp16 otherwise); the dispatcher reads that accumulator's tuned entry ...
+  int table_k_div;    // ... at K / table_k_div: the 16-bit problem that moves as many bytes per k-block
+  bool scaled;        // takes per-tensor fp32 scales in device memory
+  // the Config<> flags: BF16 names the output type, E4M3 the operand type
+  constexpr bool bf16() const { return output == Elem::kBF16; }
+  constexpr bool e4m3() const { return operand == Elem::kE4M3; }
+};
+constexpr GemmTypeTraits kGemmTypes[] = {
+    {Elem::kF16, Elem::kF16, true, 1, false},      // kF16Acc32
+    {Elem::kF16, Elem::kF16, false, 1, false},     // kF16Acc16
+    {Elem::kBF16, Elem::kBF16, true, 1, false},    // kBF16
+    {Elem::kE4M3, Elem::kF16, true, 2, true},      // kE4M3F16
+    {Elem::kE4M3, Elem::kBF16, true, 2, true},     // kE4M3BF16
+};
+constexpr const GemmTypeTraits& traits(GemmType t) { return kGemmTypes[int(t)]; }
+
+// The variant whose Config<> flags Cfg carries (a Config that names none does not compile: the index runs past the rows).
+template <class Cfg>
+constexpr GemmType gemm_type(int t = 0) {
+  const GemmTypeTraits& x = kGemmTypes[t];
+  return x.acc_f32 == Cfg::ACC_F32 && x.bf16() == Cfg::BF16 && x.e4m3() == Cfg::E4M3 ? GemmType(t) : gemm_type<Cfg>(t + 1);
+}
 
 // Row-major matrix [rows, cols] (cols contiguous) -> 2-D tiled map, box = {box_cols columns, box_rows}, swizzled over the
 // box's inner extent in bytes (128 or 64). Out-of-bounds elements read as zero / are not written.
@@ -149,26 +175,19 @@ inline const DeviceInfo& device_info() {
   return info;
 }
 
-inline int validate(const void* A, const void* Bt, const void* C, int M, int N, int K) {
-  if (!A || !Bt || !C) return kNullPointer;
+// The argument rules of a variant, checked before anything touches the device. TMA wants 16-byte row strides: A / Bt
+// rows hold K operand elements (K % 8 == 0 at two bytes, K % 16 == 0 at one byte), C rows N 16-bit elements. The scales
+// of a scaled variant are fp32 values in device memory.
+inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K) {
+  const GemmTypeTraits& t = traits(type);
+  if (!A || !Bt || !C || (t.scaled && (!scales.a || !scales.b))) return kNullPointer;
   if (M <= 0 || N <= 0 || K <= 0) return kBadShape;
-  if ((K % 8) || (N % 8)) return kBadAlignment;
-  if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
-    return kBadAlignment;
-  return kOk;
-}
-
-// e4m3 operands: one byte per element, so K % 16 == 0 keeps the A / Bt row strides at 16 bytes; C is 16-bit as before.
-// The two per-tensor scales are fp32 values in device memory.
-inline int validate_fp8(const void* A, const void* Bt, const void* C, const float* scale_a, const float* scale_b, int M,
-                        int N, int K) {
-  if (!A || !Bt || !C || !scale_a || !scale_b) return kNullPointer;
-  if (M <= 0 || N <= 0 || K <= 0) return kBadShape;
-  if (K % 16) return kBadFp8K;
+  if (K % (16 / elem_bytes(t.operand))) return t.e4m3() ? kBadFp8K : kBadAlignment;
   if (N % 8) return kBadAlignment;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
     return kBadAlignment;
-  if ((reinterpret_cast<uintptr_t>(scale_a) | reinterpret_cast<uintptr_t>(scale_b)) & 3) return kBadAlignment;
+  if (t.scaled && ((reinterpret_cast<uintptr_t>(scales.a) | reinterpret_cast<uintptr_t>(scales.b)) & 3))
+    return kBadAlignment;
   return kOk;
 }
 
@@ -459,21 +478,23 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
 // group_m <= 0 selects the default rasterisation width. max_ctas <= 0 means "all SMs". `splits`: 1 none, > 1 workspace
 // split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
 // mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
-// kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor scales of an
-// e4m3 configuration (device pointers), unused otherwise.
+// kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor scales of a
+// scaled variant (device pointers), unused otherwise.
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
            int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}) {
-  int st = Cfg::E4M3 ? validate_fp8(A, Bt, C, scales.a, scales.b, M, N, K) : validate(A, Bt, C, M, N, K);
+  constexpr GemmType kType = gemm_type<Cfg>();
+  int st = validate(kType, A, Bt, C, scales, M, N, K);
   if (st != kOk) return st;
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
 
   LaunchArgs a{};
   MapCache& cache = map_cache();
-  if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, operand_elem<Cfg>())) != kOk) return st;
-  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, operand_elem<Cfg>())) != kOk) return st;
-  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output_elem<Cfg>())) != kOk) return st;
+  const Elem operand = traits(kType).operand, output = traits(kType).output;
+  if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, operand)) != kOk) return st;
+  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, operand)) != kOk) return st;
+  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk) return st;
 
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = plan<Cfg, MODES>(M, N, K, splits, max_workers, [&] { return max_resident_clusters<Cfg>(di); });

@@ -28,32 +28,13 @@ from torch import nn
 from . import capi
 
 _LIB = "cuda_l2_b200"
-_DTYPES = (torch.float16, torch.bfloat16)
 
 torch.library.define(f"{_LIB}::hgemm", "(Tensor a, Tensor b_kmajor, str acc='fp32') -> Tensor")
 
 
-def _check_operands(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str) -> tuple[int, int, int]:
-    if a.dim() != 2 or b_kmajor.dim() != 2:
-        raise capi.B200HgemmError(f"hgemm wants 2-D operands, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}")
-    if a.dtype not in _DTYPES or b_kmajor.dtype != a.dtype:
-        raise capi.B200HgemmError(f"hgemm wants matching fp16 or bf16 operands, got {a.dtype} and {b_kmajor.dtype}")
-    if acc not in ("fp32", "fp16"):
-        raise capi.B200HgemmError(f"acc must be 'fp32' or 'fp16', got {acc!r}")
-    if a.dtype == torch.bfloat16 and acc != "fp32":
-        raise capi.B200HgemmError("bf16 operands accumulate in fp32 only (wgmma has no bf16 accumulator)")
-    m, k = a.shape
-    n, k2 = b_kmajor.shape
-    if k2 != k:
-        raise capi.B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} (K-major: [N, K])")
-    if n % 8 or k % 8:
-        raise capi.B200HgemmError(f"N and K must be multiples of 8 (16-byte TMA strides), got N={n}, K={k}")
-    return m, n, k
-
-
 @torch.library.impl(f"{_LIB}::hgemm", "CUDA")
 def _hgemm_cuda(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
-    m, n, k = _check_operands(a, b_kmajor, acc)
+    m, n, k = capi.check_operands(a, b_kmajor, a.dtype, acc)
     a = a.contiguous()
     b_kmajor = b_kmajor.contiguous()
     c = torch.empty((m, n), dtype=a.dtype, device=a.device)
@@ -72,7 +53,7 @@ def _hgemm_cpu(a, b_kmajor, acc="fp32"):
 
 @torch.library.register_fake(f"{_LIB}::hgemm")
 def _hgemm_fake(a, b_kmajor, acc="fp32"):
-    m, n, _ = _check_operands(a, b_kmajor, acc)
+    m, n, _ = capi.check_operands(a, b_kmajor, a.dtype, acc)
     return a.new_empty((m, n))
 
 
@@ -102,7 +83,8 @@ def hgemm(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.T
 
 
 def linear_supported(in_features: int, out_features: int, dtype: torch.dtype) -> bool:
-    return dtype in _DTYPES and in_features % 8 == 0 and out_features % 8 == 0
+    t = capi.gemm_type(dtype, dtype)
+    return t is not None and t.fits(out_features, in_features)
 
 
 class B200Linear(nn.Module):
@@ -164,34 +146,14 @@ def replace_linear_modules(model: nn.Module, acc: str = "fp32", skip: tuple[str,
 
 # ------------------------------------------------------------------------------------------ FP8 (e4m3), inference only
 E4M3_MAX = 448.0   # largest finite float8_e4m3fn value
-_OUT_DTYPES = (torch.float16, torch.bfloat16)
 
 torch.library.define(f"{_LIB}::fp8_gemm",
                      "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor")
 
 
-def _check_fp8_operands(a, b_kmajor, scale_a, scale_b, out_dtype) -> tuple[int, int, int]:
-    if a.dim() != 2 or b_kmajor.dim() != 2:
-        raise capi.B200HgemmError(f"fp8_gemm wants 2-D operands, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}")
-    if a.dtype != torch.float8_e4m3fn or b_kmajor.dtype != torch.float8_e4m3fn:
-        raise capi.B200HgemmError(f"fp8_gemm wants float8_e4m3fn operands, got {a.dtype} and {b_kmajor.dtype}")
-    if out_dtype not in _OUT_DTYPES:
-        raise capi.B200HgemmError(f"out_dtype must be torch.float16 or torch.bfloat16, got {out_dtype}")
-    for name, t in (("scale_a", scale_a), ("scale_b", scale_b)):
-        if t.dtype != torch.float32 or t.numel() != 1:
-            raise capi.B200HgemmError(f"{name} must be a one-element float32 tensor, got {t.dtype} {tuple(t.shape)}")
-    m, k = a.shape
-    n, k2 = b_kmajor.shape
-    if k2 != k:
-        raise capi.B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} (K-major: [N, K])")
-    if k % 16 or n % 8:
-        raise capi.B200HgemmError(f"fp8_gemm needs K % 16 == 0 and N % 8 == 0 (16-byte TMA strides), got N={n}, K={k}")
-    return m, n, k
-
-
 @torch.library.impl(f"{_LIB}::fp8_gemm", "CUDA")
 def _fp8_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype):
-    m, n, _ = _check_fp8_operands(a, b_kmajor, scale_a, scale_b, out_dtype)
+    m, n, _ = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
     a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
     c = torch.empty((m, n), dtype=out_dtype, device=a.device)
     if m == 0:
@@ -209,7 +171,7 @@ def _fp8_gemm_cpu(a, b_kmajor, scale_a, scale_b, out_dtype):
 
 @torch.library.register_fake(f"{_LIB}::fp8_gemm")
 def _fp8_gemm_fake(a, b_kmajor, scale_a, scale_b, out_dtype):
-    m, n, _ = _check_fp8_operands(a, b_kmajor, scale_a, scale_b, out_dtype)
+    m, n, _ = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
     return a.new_empty((m, n), dtype=out_dtype)
 
 
@@ -245,7 +207,8 @@ class B200Fp8Linear(nn.Module):
     @classmethod
     def from_linear(cls, lin: nn.Linear, out_dtype: torch.dtype | None = None) -> "B200Fp8Linear":
         out_dtype = out_dtype or lin.weight.dtype
-        if out_dtype not in _OUT_DTYPES or lin.in_features % 16 or lin.out_features % 8:
+        t = capi.gemm_type(torch.float8_e4m3fn, out_dtype)
+        if t is None or not t.fits(lin.out_features, lin.in_features):
             raise capi.B200HgemmError(f"cannot convert {lin} to FP8: needs in_features % 16 == 0, out_features % 8 == 0 "
                                       f"and an fp16 / bf16 output type (got {out_dtype})")
         new = cls.__new__(cls)

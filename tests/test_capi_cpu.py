@@ -57,6 +57,7 @@ def test_argument_validation_happens_before_any_cuda_call(built_libs):
     assert lib.b200_hgemm_f32acc(p + 2, None, p, p, 64, 64, 64, None) == -2             # misaligned A
     assert lib.b200_hgemm_run_config(32, 99, p, p, p, 64, 64, 64, 0, 0, 1, None) == -6     # unknown config
     assert lib.b200_hgemm_run_config(8, 0, p, p, p, 64, 64, 64, 0, 0, 1, None) == -6       # unknown accumulator
+    assert lib.b200_hgemm_run_config(0xB32, 0, p, p, p, 64, 64, 64, 0, 0, 1, None) == -6   # bf16 has its own entry
     assert "16-byte" in capi.strerror(-2)
     assert capi.launch_count() == 0
 
