@@ -57,9 +57,13 @@ __device__ __forceinline__ void fence_mbar_init() {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// arrive on a barrier that lives in (possibly) another CTA of the cluster
+// Arrive on a barrier that lives in (possibly) another CTA of the cluster. The only caller is a consumer's stage
+// release: the arrive reports that this warp's wgmma reads of the stage have finished (wgmma.wait_group has already
+// waited for them) and publishes no data, and the peer producer's refill is an async-proxy TMA write issued only after
+// it sees the phase flip. So the arrive needs no cluster-scope release: the default (.release.cta) form compiles to a
+// bare SYNCS.ARRIVE, while .release.cluster would put a MEMBAR.ALL.GPU on every k-block of every consumer warp.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar)
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar)
                : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """SASS evidence that libb200_hgemm.so is a Hopper-native kernel family: counts of wgmma (HGMMA for 16-bit operands,
-QGMMA for e4m3), TMA and cluster mnemonics, of the wgmma waits (one WARPGROUP.DEPBAR per HGMMA would mean ptxas serialised the pipeline), and of the
+QGMMA for e4m3), TMA and cluster mnemonics, of the wgmma waits (one WARPGROUP.DEPBAR per HGMMA would mean ptxas serialised the pipeline), of
+GPU-scope memory barriers inside the consumer k-loop (one there runs every k-block of every consumer warp), and of the
 legacy tensor-core paths that must be 0.
 
     python tools/sass_summary.py      # no GPU needed (cuobjdump reads the cubin)
@@ -15,6 +16,33 @@ REPO = Path(__file__).resolve().parent.parent
 LIB = REPO / "cuda_l2_b200" / "lib" / "libb200_hgemm.so"
 WANT = ["HGMMA", "QGMMA", "WARPGROUP.DEPBAR", "WARPGROUP.ARRIVE", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "UCGABAR", "USETMAXREG",
         "ACQBULK", "HMMA", "LDGSTS"]
+INSN = re.compile(r"^\s+/\*([0-9a-f]+)\*/\s+((?:@!?U?P\d+\s+)?([A-Z][A-Za-z0-9_.]*)[^;]*)", re.M)
+
+
+def sass_by_kernel(sass: str) -> dict[str, list[tuple[int, str, str]]]:
+    """(address, mnemonic, instruction text) of every instruction of every kernel in `cuobjdump -sass` output."""
+    parts = re.split(r"\n\s+Function : (\S+)\n", sass)
+    return {name: [(int(m.group(1), 16), m.group(3), m.group(2)) for m in INSN.finditer(body)]
+            for name, body in zip(parts[1::2], parts[2::2])}
+
+
+def k_loop(insns: list[tuple[int, str, str]]) -> list[tuple[int, str, str]]:
+    """The consumer k-loop: the shortest range from a backward branch's target to the branch that holds a wgmma
+    (HGMMA / QGMMA). It runs once per k-block, from the full-barrier wait to the stage release; empty if there is none."""
+    index = {addr: i for i, (addr, _, _) in enumerate(insns)}
+    best = []
+    for i, (addr, op, text) in enumerate(insns):
+        m = re.search(r"\bBRA(?:\.\S+)?\s+0x([0-9a-f]+)", text) if op.startswith("BRA") else None
+        if not m or int(m.group(1), 16) >= addr or int(m.group(1), 16) not in index:
+            continue
+        body = insns[index[int(m.group(1), 16)]:i + 1]
+        if any(o.startswith(("HGMMA", "QGMMA")) for _, o, _ in body) and (not best or len(body) < len(best)):
+            best = body
+    return best
+
+
+def k_loop_gpu_membars(insns: list[tuple[int, str, str]]) -> int:
+    return sum(1 for _, op, _ in k_loop(insns) if op.startswith("MEMBAR") and op.endswith(".GPU"))
 
 
 def operand_kind(func: str) -> str:
@@ -48,6 +76,10 @@ def main():
                 "WARPGROUP.DEPBAR": "   <- wgmma waits: about two per kernel, not one per HGMMA",
                 "LDGSTS": "   <- cp.async (not used: every bulk load is TMA)"}.get(w, "")
         print(f"{w:14s} {exact:6d}   {' '.join(variants[:8])}{note}")
+        if w == "WARPGROUP.DEPBAR":
+            per_kernel = collections.Counter(k_loop_gpu_membars(insns) for insns in sass_by_kernel(sass).values())
+            print(f"{'MEMBAR.*.GPU':14s} {sum(n * c for n, c in per_kernel.items()):6d}   in the consumer k-loop, per kernel: " +
+                  ", ".join(f"{n} in {c} kernels" for n, c in sorted(per_kernel.items())) + "   <- must be 0")
     return 0
 
 
