@@ -47,6 +47,10 @@ def hgemm_lib() -> ctypes.CDLL:
         lib.b200_fp8gemm.restype = i
         lib.b200_fp8gemm_run_config.argtypes = [i, i, vp, vp, vp, vp, vp, i, i, i, i, i, i, vp]
         lib.b200_fp8gemm_run_config.restype = i
+        lib.b200_fp8gemm_rowwise.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, vp]
+        lib.b200_fp8gemm_rowwise.restype = i
+        lib.b200_fp8gemm_rowwise_run_config.argtypes = [i, i, vp, vp, vp, vp, vp, i, i, i, i, i, i, vp]
+        lib.b200_fp8gemm_rowwise_run_config.restype = i
         lib.b200_fp8gemm_select.argtypes = [i, i, i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
         lib.b200_hgemm_num_configs.restype = i
         lib.b200_hgemm_config_info.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
@@ -94,6 +98,7 @@ def exported_symbols() -> dict[str, list[str]]:
             "b200_hgemm_select_config", "b200_hgemm_select", "b200_hgemm_run_config", "b200_hgemm_host", "b200_hgemm_launch_count",
             "b200_hgemm_strerror", "b200_hgemm_schedule_units", "b200_hgemm_prewarm", "b200_hgemm_release",
             "b200_bgemm_f32acc", "b200_bgemm_run_config", "b200_fp8gemm", "b200_fp8gemm_run_config", "b200_fp8gemm_select",
+            "b200_fp8gemm_rowwise", "b200_fp8gemm_rowwise_run_config",
         ],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
@@ -141,7 +146,7 @@ def hgemm(a, b_col_major, c, acc: str | int = "fp32", stream: int | None = None)
 class GemmType(NamedTuple):
     """A data-type variant of the kernel family (include/b200_hgemm.h)."""
     k_align: int    # K % k_align == 0: 16-byte operand rows
-    scale: object   # dtype of the per-tensor scales the variant takes (e4m3 operands: float32), None if it takes none
+    scale: object   # dtype of the scales the variant takes (e4m3 operands: float32), None if it takes none
 
     def fits(self, n: int, k: int) -> bool:
         """Whether an [M,K] x [N,K] problem meets the 16-byte row rule (TMA strides) of this variant."""
@@ -161,10 +166,26 @@ def gemm_type(operand, output, acc: str | int = "fp32") -> GemmType | None:
     return _GEMM_TYPES.get((operand, output, ACC_BITS.get(acc)))
 
 
+def scale_granularity(m: int, n: int, scale_a, scale_b) -> str:
+    """torch._scaled_mm's rule for the scales of an [M,K] x [N,K] e4m3 product: two one-element fp32 tensors are
+    ``"tensor"`` scales; ``scale_a`` [M,1] with ``scale_b`` [1,N], both fp32, are ``"rowwise"`` scales (one per row of A,
+    one per output column). Anything else, a mix of the two included, raises B200HgemmError."""
+    import torch
+
+    sa, sb = tuple(scale_a.shape), tuple(scale_b.shape)
+    if scale_a.dtype == torch.float32 and scale_b.dtype == torch.float32:
+        if scale_a.numel() == 1 and scale_b.numel() == 1:
+            return "tensor"
+        if sa == (m, 1) and sb == (1, n):
+            return "rowwise"
+    raise B200HgemmError(f"scales must be fp32 and either both one-element (per tensor) or scale_a [{m}, 1] with "
+                         f"scale_b [1, {n}] (rowwise), got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
+
+
 def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tuple = ()) -> tuple[int, int, int]:
     """(M, N, K) of a[M,K] @ b_kmajor[N,K]^T -> ``out_dtype``, by the rules of the variant the dtypes and ``acc`` name:
-    2-D operands of one dtype, a shared K, 16-byte rows, one-element fp32 scales exactly for a scaled variant.
-    Checks shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
+    2-D operands of one dtype, a shared K, 16-byte rows, two scales exactly for a scaled variant, per tensor or rowwise
+    (:func:`scale_granularity`). Checks shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
     try:
         (m, k), (n, k2) = a.shape, b_kmajor.shape
     except ValueError:
@@ -176,9 +197,8 @@ def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tupl
                              "fp32 or fp16 accumulation, bf16 with fp32, e4m3 -> fp16 / bf16 with fp32)")
     if len(scales) != (0 if t.scale is None else 2):
         raise B200HgemmError(f"{dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
-    for name, s in zip(("scale_a", "scale_b"), scales):
-        if s.dtype != t.scale or s.numel() != 1:
-            raise B200HgemmError(f"{name} must be a one-element {t.scale} tensor, got {s.dtype} {tuple(s.shape)}")
+    if scales:
+        scale_granularity(m, n, *scales)
     if k2 != k:
         raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} (K-major: [N, K])")
     if not t.fits(n, k):
@@ -223,22 +243,26 @@ def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = No
 
 def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config_id: int | None = None,
              group_m: int = 0, splits: int = 1) -> None:
-    """c[M,N] = (a[M,K] @ b_kmajor[N,K]^T) * scale_a * scale_b with ``float8_e4m3fn`` operands, fp32 accumulation and
-    one rounding to ``c``'s dtype (fp16 or bf16). ``scale_a`` / ``scale_b`` are one-element fp32 CUDA tensors, read when
-    the kernel runs. ``config_id`` pins one kernel configuration (tests; ``splits`` as in b200_hgemm_run_config);
-    default is the dispatcher."""
+    """c[M,N] = (a[M,K] @ b_kmajor[N,K]^T) scaled, with ``float8_e4m3fn`` operands, fp32 accumulation and one rounding
+    to ``c``'s dtype (fp16 or bf16). ``scale_a`` / ``scale_b`` are fp32 CUDA tensors, read when the kernel runs: one
+    element each (per tensor: ``* scale_a * scale_b``), or ``scale_a`` [M,1] and ``scale_b`` [1,N], 16-byte aligned
+    (rowwise: ``* scale_b[n]``, then ``* scale_a[m]``). ``config_id`` pins one kernel configuration (tests; ``splits`` as
+    in b200_hgemm_run_config); default is the dispatcher."""
     import torch
 
     m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b))
     lib = hgemm_lib()
     out_bf16 = int(c.dtype == torch.bfloat16)
+    rowwise = scale_granularity(m, n, scale_a, scale_b) == "rowwise"
     if config_id is None:
-        st = lib.b200_fp8gemm(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), scale_b.data_ptr(),
-                              out_bf16, m, n, k, stream)
+        fn = lib.b200_fp8gemm_rowwise if rowwise else lib.b200_fp8gemm
+        st = fn(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), scale_b.data_ptr(), out_bf16,
+                m, n, k, stream)
     else:
-        st = lib.b200_fp8gemm_run_config(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(),
-                                         scale_a.data_ptr(), scale_b.data_ptr(), m, n, k, group_m, 0, splits, stream)
-    _check(st, "b200_fp8gemm")
+        fn = lib.b200_fp8gemm_rowwise_run_config if rowwise else lib.b200_fp8gemm_run_config
+        st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(),
+                scale_b.data_ptr(), m, n, k, group_m, 0, splits, stream)
+    _check(st, "b200_fp8gemm_rowwise" if rowwise else "b200_fp8gemm")
 
 
 def fp8_select(m: int, n: int, k: int) -> tuple[int, int, int]:

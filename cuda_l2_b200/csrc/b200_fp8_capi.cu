@@ -1,6 +1,7 @@
-// libb200_hgemm.so, e4m3 part: C[M,N] (fp16 or bf16) = (A[M,K] (e4m3) * Bt[N,K]^T (e4m3)) * scale_a * scale_b, fp32
-// accumulation, per-tensor fp32 scales in device memory. A translation unit of its own so that its 92 kernels compile in
-// parallel with the 16-bit ones (b200_hgemm_capi.cu); both are linked into the one library.
+// libb200_hgemm.so, e4m3 part: C[M,N] (fp16 or bf16) = (A[M,K] (e4m3) * Bt[N,K]^T (e4m3)) scaled, fp32 accumulation,
+// per-tensor or rowwise (per-row of A x per-row of Bt) fp32 scales in device memory. A translation unit of its own so
+// that its 92 kernels compile in parallel with the 16-bit ones (b200_hgemm_capi.cu); both are linked into the one
+// library. Both scale granularities run the same 92 kernels: the granularity travels in Scales.
 #include "../../include/b200_hgemm.h"
 
 #include "hgemm_configs.cuh"
@@ -8,17 +9,44 @@
 
 using b200::host::GemmType;
 
-extern "C" {
+namespace {
 
-int b200_fp8gemm_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
-                            const void* scale_a, const void* scale_b, int M, int N, int K, int group_m, int max_ctas,
-                            int splits, void* stream) {
-  const b200::Scales sc{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
+b200::Scales scales_of(const void* scale_a, const void* scale_b, bool rowwise) {
+  return b200::Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b), rowwise};
+}
+
+int fp8_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C, b200::Scales sc, int M,
+                   int N, int K, int group_m, int max_ctas, int splits, void* stream) {
   if (out_bf16 == 0)
     return b200::run_config<GemmType::kE4M3F16>(config_id, A, B_kmajor, C, sc, M, N, K, group_m, max_ctas, splits, stream);
   if (out_bf16 == 1)
     return b200::run_config<GemmType::kE4M3BF16>(config_id, A, B_kmajor, C, sc, M, N, K, group_m, max_ctas, splits, stream);
   return b200::host::kBadConfig;
+}
+
+int fp8_gemm(const void* A, const void* B_kmajor, void* C, b200::Scales sc, int out_bf16, int M, int N, int K,
+             void* stream) {
+  if (out_bf16 == 0) return b200::dispatch::gemm<GemmType::kE4M3F16>(A, B_kmajor, C, sc, M, N, K, stream);
+  if (out_bf16 == 1) return b200::dispatch::gemm<GemmType::kE4M3BF16>(A, B_kmajor, C, sc, M, N, K, stream);
+  return b200::host::kBadConfig;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200_fp8gemm_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
+                            const void* scale_a, const void* scale_b, int M, int N, int K, int group_m, int max_ctas,
+                            int splits, void* stream) {
+  return fp8_run_config(config_id, out_bf16, A, B_kmajor, C, scales_of(scale_a, scale_b, false), M, N, K, group_m,
+                        max_ctas, splits, stream);
+}
+
+int b200_fp8gemm_rowwise_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
+                                    const void* scale_a, const void* scale_b, int M, int N, int K, int group_m,
+                                    int max_ctas, int splits, void* stream) {
+  return fp8_run_config(config_id, out_bf16, A, B_kmajor, C, scales_of(scale_a, scale_b, true), M, N, K, group_m,
+                        max_ctas, splits, stream);
 }
 
 int b200_fp8gemm_select(int M, int N, int K, int* config_id, int* group_m, int* splits) {
@@ -32,10 +60,12 @@ int b200_fp8gemm_select(int M, int N, int K, int* config_id, int* group_m, int* 
 
 int b200_fp8gemm(const void* A, const void* B_kmajor, void* C, const void* scale_a, const void* scale_b, int out_bf16,
                  int M, int N, int K, void* stream) {
-  const b200::Scales sc{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
-  if (out_bf16 == 0) return b200::dispatch::gemm<GemmType::kE4M3F16>(A, B_kmajor, C, sc, M, N, K, stream);
-  if (out_bf16 == 1) return b200::dispatch::gemm<GemmType::kE4M3BF16>(A, B_kmajor, C, sc, M, N, K, stream);
-  return b200::host::kBadConfig;
+  return fp8_gemm(A, B_kmajor, C, scales_of(scale_a, scale_b, false), out_bf16, M, N, K, stream);
+}
+
+int b200_fp8gemm_rowwise(const void* A, const void* B_kmajor, void* C, const void* scale_a, const void* scale_b,
+                         int out_bf16, int M, int N, int K, void* stream) {
+  return fp8_gemm(A, B_kmajor, C, scales_of(scale_a, scale_b, true), out_bf16, M, N, K, stream);
 }
 
 }  // extern "C"

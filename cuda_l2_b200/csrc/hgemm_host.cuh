@@ -177,7 +177,8 @@ inline const DeviceInfo& device_info() {
 
 // The argument rules of a variant, checked before anything touches the device. TMA wants 16-byte row strides: A / Bt
 // rows hold K operand elements (K % 8 == 0 at two bytes, K % 16 == 0 at one byte), C rows N 16-bit elements. The scales
-// of a scaled variant are fp32 values in device memory.
+// of a scaled variant are fp32 values in device memory: 4-byte aligned per tensor, 16-byte aligned vectors (M and N
+// values) rowwise, where the split-K reductions read the column scales as float4.
 inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K) {
   const GemmTypeTraits& t = traits(type);
   if (!A || !Bt || !C || (t.scaled && (!scales.a || !scales.b))) return kNullPointer;
@@ -186,7 +187,7 @@ inline int validate(GemmType type, const void* A, const void* Bt, const void* C,
   if (N % 8) return kBadAlignment;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
     return kBadAlignment;
-  if (t.scaled && ((reinterpret_cast<uintptr_t>(scales.a) | reinterpret_cast<uintptr_t>(scales.b)) & 3))
+  if (t.scaled && ((reinterpret_cast<uintptr_t>(scales.a) | reinterpret_cast<uintptr_t>(scales.b)) & (scales.rowwise ? 15 : 3)))
     return kBadAlignment;
   return kOk;
 }
@@ -478,8 +479,8 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
 // group_m <= 0 selects the default rasterisation width. max_ctas <= 0 means "all SMs". `splits`: 1 none, > 1 workspace
 // split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
 // mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
-// kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor scales of a
-// scaled variant (device pointers), unused otherwise.
+// kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor or rowwise scales
+// of a scaled variant (device pointers), unused otherwise.
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
            int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}) {

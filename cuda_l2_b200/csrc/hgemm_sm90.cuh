@@ -1,6 +1,6 @@
 // H100 (sm_90a) HGEMM:  C[M,N] (fp16) = A[M,K] (fp16, K-contiguous) * Bt[N,K]^T (fp16, K-contiguous)
 // with fp32 (F32F16F16F32) or fp16 (F16F16F16F16) accumulation in registers. The same pipeline also runs bf16 operands
-// (bf16 out) and e4m3 operands with per-tensor scales (fp16 or bf16 out), both with fp32 accumulation.
+// (bf16 out) and e4m3 operands with per-tensor or rowwise scales (fp16 or bf16 out), both with fp32 accumulation.
 //
 // Replaces, for this repository's device type, the per-shape kernels the reference ships
 // (reference: kernels/a100_F32F16F16F32/4096_4096_4096.cu:22-177 mainloop+epilogue, :179-279 launcher;
@@ -121,16 +121,41 @@ struct Config {
 
 constexpr int kMaxSplitTiles = 256;   // split-K is only used when tiles * splits <= #SMs
 
-// Per-tensor scales of an e4m3 launch: one fp32 value each, in device memory (null for the 16-bit operand types).
-struct Scales { const float* a; const float* b; };
+// Scales of an e4m3 launch, in device memory (null for the 16-bit operand types). Per tensor: one fp32 value each.
+// Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
+// 16-byte aligned; C[m,n] = RN_out(fp32(fp32(acc * b[n]) * a[m])). The granularity is a run-time property of the
+// same kernels.
+struct Scales { const float* a; const float* b; bool rowwise = false; };
 
-// The factor applied to the finished fp32 sum before it is rounded to the output type: fp32(scale_a * scale_b) for e4m3
-// operands, read where it is used (after the grid dependency wait, so a preceding kernel may have just written it).
+// The uniform factor applied to the finished fp32 sum before it is rounded to the output type: fp32(scale_a * scale_b)
+// for per-tensor e4m3 scales, read where it is used (after the grid dependency wait, so a preceding kernel may have just
+// written it). Rowwise launches scale per element instead (scale_quad, the plain epilogue) and do not read it.
 template <class Cfg>
 __device__ __forceinline__ float output_scale(const Scales& s) {
-  if constexpr (Cfg::E4M3) return __fmul_rn(*s.a, *s.b);
+  if constexpr (Cfg::E4M3) return s.rowwise ? 1.f : __fmul_rn(*s.a, *s.b);
   else return 1.f;
 }
+
+// One finished float4 of the split-K reductions, output row gm, columns gn .. gn+3 (gn % 4 == 0, in bounds), scaled
+// before its rounding: by the uniform factor, or (rowwise) by b[gn..gn+3] (one 16-byte load) and then a[gm].
+template <class Cfg>
+__device__ __forceinline__ void scale_quad(float4& acc, float scale, const Scales& s, int gm, int gn) {
+  if constexpr (Cfg::E4M3) {
+    if (s.rowwise) {
+      const float sa = s.a[gm];
+      const float4 sb = *reinterpret_cast<const float4*>(s.b + gn);
+      acc.x = __fmul_rn(__fmul_rn(acc.x, sb.x), sa); acc.y = __fmul_rn(__fmul_rn(acc.y, sb.y), sa);
+      acc.z = __fmul_rn(__fmul_rn(acc.z, sb.z), sa); acc.w = __fmul_rn(__fmul_rn(acc.w, sb.w), sa);
+    } else {
+      acc.x = __fmul_rn(acc.x, scale); acc.y = __fmul_rn(acc.y, scale);
+      acc.z = __fmul_rn(acc.z, scale); acc.w = __fmul_rn(acc.w, scale);
+    }
+  }
+}
+
+// The rowwise scales one thread's share of a 64-row block needs in the plain epilogue: its two row scales (rows
+// l/4 and l/4 + 8 of its warp's 16, 0 past M) and the column-scale vector, read one float2 per column pair where used.
+struct RowwiseEpi { float sa_lo, sa_hi; const float* sb; };
 
 // Where an accumulator register lands in the 64-row tile of its warpgroup: packed pair p (two adjacent columns) of
 // warp w, lane l sits at row 16w + l/4 + 8(p%2), columns 8(p/2) + 2(l%4) + {0,1} (wgmma_sm90.cuh).
@@ -154,21 +179,46 @@ __device__ __forceinline__ uint32_t acc_packed(const Reg (&d)[NR], int p) {
   else return d[p];   // fp16 accumulators are already the output format
 }
 
-// registers -> swizzled staging buffer -> TMA store of one EPI_ROWS x EPI_N chunk of this warp
+// registers -> swizzled staging buffer -> TMA store of one EPI_ROWS x EPI_N chunk of this warp. With rowwise e4m3 scales
+// (`rw` non-null) each fp32 pair is scaled by its column scales, then its row scale, right before the rounding. The
+// column scales of a chunk are loaded here, after the previous chunk's store wait, one float2 (one column pair) per
+// lane, and reach the lanes that need them by shuffle: two registers per thread instead of the chunk's 16, which the
+// 128 accumulators of a BN = 256 (or M_REP = 2) tile leave no room for.
 template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chunk, uint32_t epi_buf, int lane,
-                                                     const CUtensorMap* tmap_c, int col0, int row0, int M, int N) {
+                                                     const CUtensorMap* tmap_c, int col0, int row0, int M, int N,
+                                                     const RowwiseEpi* rw = nullptr) {
   using namespace ptx;
   constexpr int EN = Cfg::EPI_N;
   constexpr int PER_CHUNK = EN / 4;   // packed pairs of one chunk per thread
   // the previous store from this warp's staging buffer must have finished reading it
   if (lane == 0) tma_store_wait_read<0>();
   __syncwarp();
+  [[maybe_unused]] float2 sb_lane = make_float2(0.f, 0.f);   // rowwise: chunk columns 2 lane, 2 lane + 1
+  [[maybe_unused]] float sbx = 0.f, sby = 0.f;                 // rowwise: the column scales of pairs q, q + 1 (q even)
+  if constexpr (Cfg::E4M3) {
+    const int n = col0 + 2 * lane;   // even, and N % 8 == 0: n < N covers n + 1
+    if (rw && 2 * lane < EN && n < N) sb_lane = *reinterpret_cast<const float2*>(rw->sb + n);
+  }
 #pragma unroll
   for (int q = 0; q < PER_CHUNK; ++q) {
     uint32_t off = uint32_t(frag_row(lane, q) * (EN * 2) + frag_col(lane, q) * 2);
     // 128-byte rows use the 128B swizzle (16-byte chunk ^= row % 8), 64-byte rows the 64B one (chunk ^= (row / 2) % 4)
     off ^= (EN == 64 ? ((off >> 7) & 7u) : ((off >> 7) & 3u)) << 4;
+    if constexpr (Cfg::E4M3) {
+      if (rw) {   // warp-uniform
+        if ((q & 1) == 0) {   // pairs q and q + 1 share their columns (rows l/4 and l/4 + 8)
+          const int src = frag_col(lane, q) / 2;   // the lane holding them
+          sbx = __shfl_sync(0xffffffffu, sb_lane.x, src);
+          sby = __shfl_sync(0xffffffffu, sb_lane.y, src);
+        }
+        const float sa = (q & 1) ? rw->sa_hi : rw->sa_lo;
+        const float2 v = acc_pair<Cfg>(d, chunk * PER_CHUNK + q);
+        st_shared_b32(epi_buf + off, pack_out_x2_rn<Cfg::BF16>(__fmul_rn(__fmul_rn(v.x, sbx), sa),
+                                                               __fmul_rn(__fmul_rn(v.y, sby), sa)));
+        continue;
+      }
+    }
     st_shared_b32(epi_buf + off, acc_packed<Cfg>(d, chunk * PER_CHUNK + q));
   }
   fence_proxy_async_smem();
@@ -240,10 +290,7 @@ __device__ __forceinline__ void splitk_epilogue(const Reg (&d)[NR], int e, int r
         const float4 p = ld_shared_v4f(red_smem + uint32_t(sp) * slice_bytes + uint32_t(i) * 16u);
         acc.x += p.x; acc.y += p.y; acc.z += p.z; acc.w += p.w;
       }
-      if constexpr (Cfg::E4M3) {
-        acc.x = __fmul_rn(acc.x, scale); acc.y = __fmul_rn(acc.y, scale);
-        acc.z = __fmul_rn(acc.z, scale); acc.w = __fmul_rn(acc.w, scale);
-      }
+      scale_quad<Cfg>(acc, scale, scales, gm, gn);
       uint2 out;
       out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
       out.y = pack_out_x2_rn<Cfg::BF16>(acc.z, acc.w);
@@ -305,10 +352,7 @@ __device__ __forceinline__ void cluster_splitk_reduce(int e, int split, int spli
         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
       }
     }
-    if constexpr (Cfg::E4M3) {
-      acc.x = __fmul_rn(acc.x, scale); acc.y = __fmul_rn(acc.y, scale);
-      acc.z = __fmul_rn(acc.z, scale); acc.w = __fmul_rn(acc.w, scale);
-    }
+    scale_quad<Cfg>(acc, scale, scales, gm, gn);
     uint2 out;
     out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
     out.y = pack_out_x2_rn<Cfg::BF16>(acc.z, acc.w);
@@ -639,6 +683,19 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
                              splitk_ws, splitk_ctr, c_raw, smem_a, bar_splitk, scales);
       } else {
         if constexpr (Cfg::E4M3) {
+          if (scales.rowwise) {
+            // each element gets its own factor, applied as it is packed for the store (epilogue_store_chunk)
+#pragma unroll
+            for (int r = 0; r < MR; ++r) {
+              const int row0 = m_cta + (wg * MR + r) * 64 + wq * 16;
+              const int ra = row0 + (lane >> 2), rb = ra + 8;   // frag_row of the even / odd pairs
+              const RowwiseEpi rw{ra < M ? scales.a[ra] : 0.f, rb < M ? scales.a[rb] : 0.f, scales.b};
+#pragma unroll
+              for (int j = 0; j < Cfg::EPI_CHUNKS; ++j)
+                epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, row0, M, N, &rw);
+            }
+            continue;   // the unit is done
+          }
           // the finished sums are scaled in place, right before the epilogue rounds them: the scale is read per unit,
           // after the main loop, and is dead before the epilogue's own temporaries are live
           const float scale = output_scale<Cfg>(scales);

@@ -12,8 +12,10 @@ the nearest grid shape — so deployment is a plain operator:
   eligible ``nn.Linear`` layers of a model in place.
 * ``torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)``: ``float8_e4m3fn`` operands in the same
   layout, per-tensor fp32 scales as one-element CUDA tensors, ``(a @ b_kmajor^T) * scale_a * scale_b`` rounded once to
-  ``out_dtype`` (fp16 or bf16) — ``torch._scaled_mm`` with per-tensor scales and fast accumulation.
-* :class:`B200Fp8Linear`: inference-only FP8 version of an ``nn.Linear`` (weight quantised once, activation per call).
+  ``out_dtype`` (fp16 or bf16) — ``torch._scaled_mm`` with per-tensor scales and fast accumulation. Rowwise scales
+  follow ``torch._scaled_mm``'s shapes, ``scale_a`` [M,1] and ``scale_b`` [1,N]: ``((a @ b_kmajor^T) * scale_b) * scale_a``.
+* :class:`B200Fp8Linear`: inference-only FP8 version of an ``nn.Linear`` (weight quantised once, activation per call;
+  per tensor or rowwise).
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernel on explicitly
@@ -151,6 +153,12 @@ torch.library.define(f"{_LIB}::fp8_gemm",
                      "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor")
 
 
+def _rowwise_scale_arg(s: torch.Tensor) -> torch.Tensor:
+    """A rowwise scale vector as the kernel reads it: contiguous and 16-byte aligned (a fresh copy if it is not)."""
+    s = s.contiguous()
+    return s if s.data_ptr() % 16 == 0 else s.clone()
+
+
 @torch.library.impl(f"{_LIB}::fp8_gemm", "CUDA")
 def _fp8_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype):
     m, n, _ = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
@@ -158,9 +166,12 @@ def _fp8_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype):
     c = torch.empty((m, n), dtype=out_dtype, device=a.device)
     if m == 0:
         return c
+    if capi.scale_granularity(m, n, scale_a, scale_b) == "rowwise":
+        scale_a, scale_b = _rowwise_scale_arg(scale_a), _rowwise_scale_arg(scale_b)
+    else:
+        scale_a, scale_b = scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous()
     with torch.cuda.device(a.device):
-        capi.fp8_gemm(a, b_kmajor, c, scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous(),
-                      stream=torch.cuda.current_stream(a.device).cuda_stream)
+        capi.fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream=torch.cuda.current_stream(a.device).cuda_stream)
     return c
 
 
@@ -186,7 +197,8 @@ torch.library.register_autograd(f"{_LIB}::fp8_gemm", _fp8_gemm_no_backward)
 
 def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
              out_dtype: torch.dtype = torch.float16) -> torch.Tensor:
-    """(``a`` [M,K] @ ``b_kmajor`` [N,K]^T) * scale_a * scale_b -> [M,N] ``out_dtype``, e4m3 operands (see the module docstring)."""
+    """(``a`` [M,K] @ ``b_kmajor`` [N,K]^T), scaled, -> [M,N] ``out_dtype``, e4m3 operands (see the module docstring).
+    Per-tensor scales: one element each. Rowwise scales: ``scale_a`` [M,1], ``scale_b`` [1,N]."""
     return torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)
 
 
@@ -198,24 +210,46 @@ def quantize_e4m3(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
     return q, scale
 
 
+def quantize_e4m3_rowwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per-row quantisation of a 2-D ``x`` [rows, cols] on its device: scale[r] = amax(|x[r]|) / 448 (an fp32
+    [rows, 1] tensor), q = e4m3(x / scale). One outlier row no longer squeezes every other row into e4m3's few low
+    codes. Torch ops only, no host synchronisation."""
+    scale = (x.abs().amax(dim=1, keepdim=True).float() / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
+    q = (x.float() / scale).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return q, scale
+
+
+FP8_GRANULARITIES = ("tensor", "rowwise")
+
+
 class B200Fp8Linear(nn.Module):
-    """Inference-only FP8 ``nn.Linear``: the weight is quantised once to e4m3 with a per-tensor scale (buffers
-    ``weight_fp8`` / ``weight_scale``); every call quantises the activation per tensor on the device and runs
-    ``cuda_l2_b200::fp8_gemm``, then adds the bias (shared with the source layer). No ``.item()`` and no host
-    synchronisation, so the forward can be captured in a CUDA graph. Needs in_features % 16 == 0, out_features % 8 == 0."""
+    """Inference-only FP8 ``nn.Linear``: the weight is quantised once to e4m3 (buffers ``weight_fp8`` / ``weight_scale``);
+    every call quantises the activation on the device and runs ``cuda_l2_b200::fp8_gemm``, then adds the bias (shared
+    with the source layer). ``granularity="tensor"``: one scale for the weight (``weight_scale`` [1]) and one per call
+    for the activation. ``"rowwise"``: one scale per output channel (``weight_scale`` [1, out_features], the layout of
+    common FP8 checkpoints) and one per activation row (token). No ``.item()`` and no host synchronisation, so the
+    forward can be captured in a CUDA graph. Needs in_features % 16 == 0, out_features % 8 == 0."""
 
     @classmethod
-    def from_linear(cls, lin: nn.Linear, out_dtype: torch.dtype | None = None) -> "B200Fp8Linear":
+    def from_linear(cls, lin: nn.Linear, out_dtype: torch.dtype | None = None,
+                    granularity: str = "tensor") -> "B200Fp8Linear":
         out_dtype = out_dtype or lin.weight.dtype
         t = capi.gemm_type(torch.float8_e4m3fn, out_dtype)
         if t is None or not t.fits(lin.out_features, lin.in_features):
             raise capi.B200HgemmError(f"cannot convert {lin} to FP8: needs in_features % 16 == 0, out_features % 8 == 0 "
                                       f"and an fp16 / bf16 output type (got {out_dtype})")
+        if granularity not in FP8_GRANULARITIES:
+            raise capi.B200HgemmError(f"granularity must be one of {FP8_GRANULARITIES}, got {granularity!r}")
         new = cls.__new__(cls)
         nn.Module.__init__(new)
         new.in_features, new.out_features, new.out_dtype = lin.in_features, lin.out_features, out_dtype
+        new.granularity = granularity
         with torch.no_grad():
-            w_q, w_scale = quantize_e4m3(lin.weight)
+            if granularity == "rowwise":
+                w_q, w_scale = quantize_e4m3_rowwise(lin.weight)
+                w_scale = w_scale.reshape(1, lin.out_features)   # [1, N]: the column scales of the product
+            else:
+                w_q, w_scale = quantize_e4m3(lin.weight)
         new.register_buffer("weight_fp8", w_q)
         new.register_buffer("weight_scale", w_scale)
         new.bias = lin.bias                                  # shared with the source layer
@@ -227,7 +261,8 @@ class B200Fp8Linear(nn.Module):
         if x2.shape[0] == 0:
             y = x2.new_empty((0, self.out_features), dtype=self.out_dtype)
         else:
-            x_q, x_scale = quantize_e4m3(x2)
+            quantize = quantize_e4m3_rowwise if self.granularity == "rowwise" else quantize_e4m3
+            x_q, x_scale = quantize(x2)
             y = torch.ops.cuda_l2_b200.fp8_gemm(x_q, self.weight_fp8, x_scale, self.weight_scale, self.out_dtype)
         if self.bias is not None:
             y = y + self.bias
@@ -235,8 +270,8 @@ class B200Fp8Linear(nn.Module):
 
     def extra_repr(self) -> str:
         return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
-                f"out_dtype={self.out_dtype}")
+                f"out_dtype={self.out_dtype}, granularity={self.granularity}")
 
 
 __all__ = ["hgemm", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
-           "B200Fp8Linear"]
+           "quantize_e4m3_rowwise", "B200Fp8Linear"]

@@ -66,6 +66,20 @@ int b200_fp8gemm_run_config(int config_id, int out_bf16, const void* A, const vo
                             int splits, void* stream);
 int b200_fp8gemm_select(int M, int N, int K, int* config_id, int* group_m, int* splits);
 
+/* FP8 with rowwise scales (per token x per output channel): the same operands, output, kernels and dispatcher choice as
+ * b200_fp8gemm, but scale_a points to M fp32 values (one per row of A) and scale_b to N fp32 values (one per row of
+ * B_kmajor, i.e. per output column), both in DEVICE memory and 16-byte aligned (status -2 otherwise, -5 if NULL):
+ *     C[m,n] = RN_out( fp32( fp32(acc[m,n] * scale_b[n]) * scale_a[m] ) ),   acc[m,n] = sum_k A[m,k] * B_kmajor[n,k]
+ * The column scale is applied first, then the row scale, each product rounded to fp32, then the one rounding to the
+ * output type, in every K-mode. The vectors are read when the kernel runs (a graph replay sees their current contents).
+ * The same as torch._scaled_mm(A, B_kmajor.t(), scale_a[M,1], scale_b[1,N], out_dtype) with rowwise scales.
+ * b200_fp8gemm_rowwise_run_config is b200_fp8gemm_run_config for these scales (same `splits` codes). */
+int b200_fp8gemm_rowwise(const void* A, const void* B_kmajor, void* C, const void* scale_a, const void* scale_b,
+                         int out_bf16, int M, int N, int K, void* stream);
+int b200_fp8gemm_rowwise_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
+                                    const void* scale_a, const void* scale_b, int M, int N, int K, int group_m,
+                                    int max_ctas, int splits, void* stream);
+
 /* The reference fixes tile/stage/swizzle per (M,N,K) at compile time inside each
  * kernels/<dev>/<M>_<N>_<K>.cu (e.g. a100_F32F16F16F32/4096_4096_4096.cu:185-200,305-309). Here the
  * per-shape choice is a table lookup; these calls expose it for the tuner and the tests. */

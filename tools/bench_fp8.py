@@ -3,9 +3,11 @@
 
     python tools/bench_fp8.py [--steps K] [--warmup W] [--mnk M_N_K]
 
-Shapes: --mnk (default 4096_4096_4096), 4096^3 and 2048x11008x4096. Per shape, four legs with the same rules:
+Shapes: --mnk (default 4096_4096_4096), 4096^3 and 2048x11008x4096. Per shape, six legs with the same rules:
 b200_fp8gemm (e4m3 operands quantised per tensor from N(0,1) data, fp16 out, the dispatcher's choice),
-torch._scaled_mm with fast accumulation on and off (same operands and scales), and b200_hgemm_f32acc on the fp16 data.
+torch._scaled_mm with fast accumulation on and off (same operands and scales), b200_hgemm_f32acc on the fp16 data, and
+two bf16-out legs on the same data quantised per row (scales [M,1] and [1,N]): b200_fp8gemm_rowwise and
+torch._scaled_mm with rowwise scales and fast accumulation.
 Each leg: warm-up, then K back-to-back calls between two CUDA events on the legacy default stream, rotating over seeded
 operand sets whose fp16 footprint exceeds the 50 MB L2 four times. TFLOP/s = 2MNK per call. Prints one JSON line with
 the card's name and enforced power limit (figures are only comparable at the same limit). Writes nothing.
@@ -51,7 +53,11 @@ def time_shape(m: int, n: int, k: int, steps: int, warmup: int, gen: torch.Gener
         bt = torch.randn((n, k), device="cuda", generator=gen).half()
         qa, sa = ops.quantize_e4m3(a)
         qb, sb = ops.quantize_e4m3(bt)
-        sets.append(dict(a=a, bt=bt, qa=qa, qb=qb, sa=sa, sb=sb, c=torch.empty((m, n), dtype=torch.half, device="cuda")))
+        qa_r, sa_r = ops.quantize_e4m3_rowwise(a)
+        qb_r, sb_r = ops.quantize_e4m3_rowwise(bt)
+        sets.append(dict(a=a, bt=bt, qa=qa, qb=qb, sa=sa, sb=sb, c=torch.empty((m, n), dtype=torch.half, device="cuda"),
+                         qa_r=qa_r, qb_r=qb_r, sa_r=sa_r, sb_r=sb_r.reshape(1, n),
+                         c_bf16=torch.empty((m, n), dtype=torch.bfloat16, device="cuda")))
 
     def ours_fp8(st):
         capi.fp8_gemm(st["qa"], st["qb"], st["c"], st["sa"], st["sb"])
@@ -63,8 +69,16 @@ def time_shape(m: int, n: int, k: int, steps: int, warmup: int, gen: torch.Gener
         return lambda st: torch._scaled_mm(st["qa"], st["qb"].t(), scale_a=st["sa"].reshape(()),
                                            scale_b=st["sb"].reshape(()), out_dtype=torch.half, use_fast_accum=fast)
 
+    def ours_rowwise(st):
+        capi.fp8_gemm(st["qa_r"], st["qb_r"], st["c_bf16"], st["sa_r"], st["sb_r"])
+
+    def scaled_rowwise(st):
+        return torch._scaled_mm(st["qa_r"], st["qb_r"].t(), scale_a=st["sa_r"], scale_b=st["sb_r"],
+                                out_dtype=torch.bfloat16, use_fast_accum=True)
+
     legs = {"ours_e4m3": ours_fp8, "scaled_mm_fast_accum": scaled(True), "scaled_mm_no_fast_accum": scaled(False),
-            "ours_fp16_fp32acc": ours_fp16}
+            "ours_fp16_fp32acc": ours_fp16, "ours_e4m3_rowwise_bf16": ours_rowwise,
+            "scaled_mm_rowwise_fast_accum_bf16": scaled_rowwise}
     row = {}
     for name, fn in legs.items():
         for i in range(max(warmup, 3)):
