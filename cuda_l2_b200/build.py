@@ -3,6 +3,7 @@
 Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
 
 * ``libb200_hgemm.so``  — the C-ABI product library (include/b200_hgemm.h)
+* ``libb200_fp8block.so`` — the block-scaled FP8 GEMM (include/b200_fp8_block.h)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -79,6 +80,16 @@ def build_capi(verbose: bool = False, force: bool = False) -> Path:
     return out
 
 
+def build_fp8block(verbose: bool = False, force: bool = False) -> Path:
+    """The block-scaled e4m3 kernels: a library of their own, so that libb200_hgemm.so's device code is unaffected."""
+    LIB_DIR.mkdir(exist_ok=True)
+    out = LIB_DIR / "libb200_fp8block.so"
+    src = CSRC / "b200_fp8_block_capi.cu"
+    if force or _stale(out, [src] + _headers()):
+        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), str(src)], verbose)
+    return out
+
+
 def build_baselines(verbose: bool = False, force: bool = False) -> Path:
     LIB_DIR.mkdir(exist_ok=True)
     out = LIB_DIR / "libb200_baselines.so"
@@ -101,7 +112,10 @@ def build_dev_check(verbose: bool = False, force: bool = False) -> Path:
 
 
 def build_all(verbose: bool = False, force: bool = False) -> dict[str, Path]:
-    out = {"capi": build_capi(verbose, force)}
+    from concurrent.futures import ThreadPoolExecutor
+    with ThreadPoolExecutor(2) as pool:   # the block-scaled library compiles next to the product library's two units
+        block = pool.submit(build_fp8block, verbose, force)
+        out = {"capi": build_capi(verbose, force), "fp8block": block.result()}
     if (CSRC / "b200_baselines_capi.cu").exists():
         out["baselines"] = build_baselines(verbose, force)
     out["dev_check"] = build_dev_check(verbose, force)

@@ -15,6 +15,7 @@ from typing import NamedTuple
 LIB_DIR = Path(__file__).resolve().parent / "lib"
 _hgemm = None
 _baselines = None
+_fp8block = None
 
 ACC_BITS = {"fp32": 32, "fp16": 16, 32: 32, 16: 16}
 
@@ -73,6 +74,25 @@ def hgemm_lib() -> ctypes.CDLL:
     return _hgemm
 
 
+def fp8block_lib() -> ctypes.CDLL:
+    """libb200_fp8block.so: the block-scaled e4m3 GEMM (include/b200_fp8_block.h)."""
+    global _fp8block
+    if _fp8block is None:
+        lib = _load("libb200_fp8block.so")
+        vp, i, ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
+        lib.b200_fp8gemm_blockwise.argtypes = [vp, vp, vp, vp, i, vp, i, i, i, i, vp]
+        lib.b200_fp8gemm_blockwise.restype = i
+        lib.b200_fp8gemm_blockwise_run_config.argtypes = [i, i, vp, vp, vp, vp, i, vp, i, i, i, i, i, i, vp]
+        lib.b200_fp8gemm_blockwise_run_config.restype = i
+        lib.b200_fp8gemm_blockwise_select.argtypes = [i, i, i, ip, ip, ip]
+        lib.b200_fp8gemm_blockwise_select.restype = i
+        lib.b200_fp8block_launch_count.restype = ctypes.c_ulonglong
+        lib.b200_fp8block_strerror.argtypes = [i]
+        lib.b200_fp8block_strerror.restype = ctypes.c_char_p
+        _fp8block = lib
+    return _fp8block
+
+
 def baselines_lib() -> ctypes.CDLL:
     global _baselines
     if _baselines is None:
@@ -99,6 +119,10 @@ def exported_symbols() -> dict[str, list[str]]:
             "b200_hgemm_strerror", "b200_hgemm_schedule_units", "b200_hgemm_prewarm", "b200_hgemm_release",
             "b200_bgemm_f32acc", "b200_bgemm_run_config", "b200_fp8gemm", "b200_fp8gemm_run_config", "b200_fp8gemm_select",
             "b200_fp8gemm_rowwise", "b200_fp8gemm_rowwise_run_config",
+        ],
+        "libb200_fp8block.so": [
+            "b200_fp8gemm_blockwise", "b200_fp8gemm_blockwise_run_config", "b200_fp8gemm_blockwise_select",
+            "b200_fp8block_launch_count", "b200_fp8block_strerror",
         ],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
@@ -166,10 +190,20 @@ def gemm_type(operand, output, acc: str | int = "fp32") -> GemmType | None:
     return _GEMM_TYPES.get((operand, output, ACC_BITS.get(acc)))
 
 
-def scale_granularity(m: int, n: int, scale_a, scale_b) -> str:
+BLOCK = 128   # block scales: one per (row of A, 128 k) and one per 128 x 128 block of Bt
+
+
+def num_k_blocks(k: int) -> int:
+    """ceil(K / 128): the scale blocks along K of a block-scaled product."""
+    return -(-k // BLOCK)
+
+
+def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None) -> str:
     """torch._scaled_mm's rule for the scales of an [M,K] x [N,K] e4m3 product: two one-element fp32 tensors are
     ``"tensor"`` scales; ``scale_a`` [M,1] with ``scale_b`` [1,N], both fp32, are ``"rowwise"`` scales (one per row of A,
-    one per output column). Anything else, a mix of the two included, raises B200HgemmError."""
+    one per output column); ``scale_a`` [M, nkb] with ``scale_b`` [ceil(N/128), nkb], nkb = ceil(K/128), both fp32, are
+    ``"blockwise"`` scales (one per row of A and 128 k, one per 128 x 128 block of Bt). Without ``k``, any nkb the two
+    agree on is accepted. Anything else, a mix of them included, raises B200HgemmError."""
     import torch
 
     sa, sb = tuple(scale_a.shape), tuple(scale_b.shape)
@@ -178,8 +212,25 @@ def scale_granularity(m: int, n: int, scale_a, scale_b) -> str:
             return "tensor"
         if sa == (m, 1) and sb == (1, n):
             return "rowwise"
-    raise B200HgemmError(f"scales must be fp32 and either both one-element (per tensor) or scale_a [{m}, 1] with "
-                         f"scale_b [1, {n}] (rowwise), got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
+        nkb = num_k_blocks(k) if k is not None else (sa[1] if len(sa) == 2 else -1)
+        if sa == (m, nkb) and sb == (-(-n // BLOCK), nkb):
+            return "blockwise"
+    raise B200HgemmError(f"scales must be fp32 and either both one-element (per tensor), scale_a [{m}, 1] with "
+                         f"scale_b [1, {n}] (rowwise), or scale_a [{m}, ceil(K/128)] with scale_b [ceil({n}/128), "
+                         f"ceil(K/128)] (blockwise), got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
+
+
+def blockwise_ld_a(scale_a) -> int | None:
+    """The row stride ld_a with which the kernel can read a blockwise ``scale_a`` [M, nkb] in place: M-major (strides
+    (1, ld_a), torch's ``[nkb, ld_a]`` buffer viewed as ``buf[:, :M].t()``), ld_a >= M, ld_a % 4 == 0, 16-byte aligned,
+    and nkb * ld_a floats readable in its storage (one k-block: ld_a = M rounded up to 4). None if the tensor is not
+    laid out that way."""
+    m, nkb = scale_a.shape
+    ld = scale_a.stride(1) if nkb > 1 else -(-m // 4) * 4     # one k-block: the stride is never stepped
+    if (m > 1 and scale_a.stride(0) != 1) or ld < m or ld % 4 or scale_a.data_ptr() % 16:
+        return None
+    readable = scale_a.untyped_storage().nbytes() // 4 - scale_a.storage_offset()
+    return ld if nkb * ld <= readable else None
 
 
 def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tuple = ()) -> tuple[int, int, int]:
@@ -198,7 +249,7 @@ def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tupl
     if len(scales) != (0 if t.scale is None else 2):
         raise B200HgemmError(f"{dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
     if scales:
-        scale_granularity(m, n, *scales)
+        scale_granularity(m, n, *scales, k=k)
     if k2 != k:
         raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} (K-major: [N, K])")
     if not t.fits(n, k):
@@ -207,10 +258,12 @@ def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tupl
     return m, n, k
 
 
-def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = ()) -> tuple[int, int, int]:
-    """check_operands for c = a @ b_kmajor^T, all of them (scales included) contiguous CUDA tensors, c of shape [M,N]."""
+def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = (), strided_scale_a: bool = False
+                     ) -> tuple[int, int, int]:
+    """check_operands for c = a @ b_kmajor^T, all of them (scales included) contiguous CUDA tensors, c of shape [M,N].
+    ``strided_scale_a``: scale_a need not be contiguous (blockwise scales are read M-major)."""
     for name, x in zip(("a", "b_kmajor", "c", "scale_a", "scale_b"), (a, b_kmajor, c, *scales)):
-        if not x.is_cuda or not x.is_contiguous():
+        if not x.is_cuda or not (x.is_contiguous() or (strided_scale_a and name == "scale_a")):
             raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
     m, n, k = check_operands(a, b_kmajor, c.dtype, acc, scales)
     if c.shape != (m, n):
@@ -246,14 +299,35 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     """c[M,N] = (a[M,K] @ b_kmajor[N,K]^T) scaled, with ``float8_e4m3fn`` operands, fp32 accumulation and one rounding
     to ``c``'s dtype (fp16 or bf16). ``scale_a`` / ``scale_b`` are fp32 CUDA tensors, read when the kernel runs: one
     element each (per tensor: ``* scale_a * scale_b``), or ``scale_a`` [M,1] and ``scale_b`` [1,N], 16-byte aligned
-    (rowwise: ``* scale_b[n]``, then ``* scale_a[m]``). ``config_id`` pins one kernel configuration (tests; ``splits`` as
-    in b200_hgemm_run_config); default is the dispatcher."""
+    (rowwise: ``* scale_b[n]``, then ``* scale_a[m]``), or blockwise scales (include/b200_fp8_block.h): ``scale_a``
+    [M, ceil(K/128)] M-major (strides (1, ld_a), see :func:`blockwise_ld_a`), ``scale_b`` [ceil(N/128), ceil(K/128)]
+    contiguous, run by libb200_fp8block.so. ``config_id`` pins one kernel configuration (tests; ``splits`` as in
+    b200_hgemm_run_config); default is the dispatcher."""
     import torch
 
-    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b))
-    lib = hgemm_lib()
+    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b), strided_scale_a=True)
     out_bf16 = int(c.dtype == torch.bfloat16)
-    rowwise = scale_granularity(m, n, scale_a, scale_b) == "rowwise"
+    granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
+    if granularity == "blockwise":
+        ld_a = blockwise_ld_a(scale_a)
+        if ld_a is None:
+            raise B200HgemmError(f"blockwise scale_a must be M-major with a row stride ld_a >= M, ld_a % 4 == 0, 16-byte "
+                                 f"aligned, ceil(K/128) * ld_a floats readable; got strides {tuple(scale_a.stride())}")
+        blk = fp8block_lib()
+        if config_id is None:
+            st = blk.b200_fp8gemm_blockwise(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a,
+                                            scale_b.data_ptr(), out_bf16, m, n, k, stream)
+        else:
+            st = blk.b200_fp8gemm_blockwise_run_config(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(),
+                                                       c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr(), m, n,
+                                                       k, group_m, 0, splits, stream)
+        if st != 0:
+            raise B200HgemmError(f"b200_fp8gemm_blockwise failed: status {st} ({blk.b200_fp8block_strerror(st).decode()})")
+        return
+    if not scale_a.is_contiguous():
+        raise B200HgemmError("scale_a must be a contiguous CUDA tensor")
+    lib = hgemm_lib()
+    rowwise = granularity == "rowwise"
     if config_id is None:
         fn = lib.b200_fp8gemm_rowwise if rowwise else lib.b200_fp8gemm
         st = fn(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), scale_b.data_ptr(), out_bf16,
@@ -271,6 +345,20 @@ def fp8_select(m: int, n: int, k: int) -> tuple[int, int, int]:
     _check(hgemm_lib().b200_fp8gemm_select(m, n, k, ctypes.byref(cid), ctypes.byref(gm), ctypes.byref(sp)),
            "b200_fp8gemm_select")
     return cid.value, gm.value, sp.value
+
+
+def fp8_blockwise_select(m: int, n: int, k: int) -> tuple[int, int, int]:
+    """(config id, rasterisation group, splits code) the block-scaled dispatcher uses (b200_fp8gemm_blockwise_select)."""
+    cid, gm, sp = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    lib = fp8block_lib()
+    st = lib.b200_fp8gemm_blockwise_select(m, n, k, ctypes.byref(cid), ctypes.byref(gm), ctypes.byref(sp))
+    if st != 0:
+        raise B200HgemmError(f"b200_fp8gemm_blockwise_select failed: status {st}")
+    return cid.value, gm.value, sp.value
+
+
+def fp8block_launch_count() -> int:
+    return int(fp8block_lib().b200_fp8block_launch_count())
 
 
 def hgemm_config(a, b_col_major, c, config_id: int, acc: str | int = "fp32", group_m: int = 0, max_ctas: int = 0,

@@ -1,0 +1,134 @@
+// libb200_fp8block.so: the block-scaled e4m3 GEMM (include/b200_fp8_block.h). The kernels are the family's pipeline
+// with BlockScaled<> configurations (hgemm_sm90.cuh): every k-block's sum is promoted into a second fp32 accumulator
+// with its scales. A library of its own, so that libb200_hgemm.so's device code stays as it is.
+#include "../../include/b200_fp8_block.h"
+
+#include "hgemm_configs.cuh"
+#include "hgemm_dispatch.cuh"
+
+using b200::host::GemmType;
+
+namespace b200 {
+namespace block {
+
+// Two accumulator sets (the running sum and the k-block's wgmma target) fit the registers for M_REP * BN <= 128.
+constexpr bool eligible(int id) { return kConfigs[id].m_rep * kConfigs[id].bn <= 128; }
+
+// The block-scaled stand-in of configuration `id`: the same CTA group and cluster, M_REP = 1, BN = min(BN, 128).
+constexpr int sibling(int id) {
+  const ConfigDesc& c = kConfigs[id];
+  const int bn = c.bn < 128 ? c.bn : 128;
+  for (int j = 0; j < kNumConfigs; ++j) {
+    const ConfigDesc& d = kConfigs[j];
+    if (d.cta_group == c.cta_group && d.cluster_m == c.cluster_m && d.cluster_n == c.cluster_n && d.m_rep == 1 &&
+        d.bn == bn)
+      return j;
+  }
+  return -1;
+}
+constexpr bool every_config_has_an_eligible_sibling() {
+  for (int id = 0; id < kNumConfigs; ++id) {
+    const int s = sibling(id);
+    if (s < 0 || !eligible(s) || (eligible(id) && s != id)) return false;
+  }
+  return true;
+}
+static_assert(every_config_has_an_eligible_sibling(), "the configuration table lost a block-scaled sibling");
+
+// The dispatcher's `splits` code for the sibling: workspace split-K becomes cluster split-K of the largest of 8/4/2
+// not above it, stream-K the plain schedule; only configurations with split-K kernels keep a split.
+constexpr int sibling_splits(int id, int splits) {
+  if (!kConfigs[id].split_k) return 1;
+  const host::KRequest r = host::decode_splits(splits);
+  if (r.mode == kWorkspaceSplitK) return r.factor >= 8 ? -8 : r.factor >= 4 ? -4 : -2;
+  if (r.mode == kClusterSplitK) return splits;
+  return 1;
+}
+
+// Workspace split-K and stream-K are not compiled for this variant: plan() runs such requests plain.
+constexpr unsigned kModes = (1u << kPlain) | (1u << kClusterSplitK);
+
+// Kernel launches of this library (b200_fp8block_launch_count).
+__attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_block_launches{0};
+
+template <GemmType T>
+int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, int ld_a, int M, int N, int K,
+               int group_m, int max_ctas, int splits, cudaStream_t s) {
+  constexpr host::GemmTypeTraits t = host::traits(T);
+  static_assert(t.block && t.e4m3() && t.acc_f32, "block-scaled e4m3 variants only");
+  int st = host::kBadConfig;
+  switch (id) {
+#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
+  case ID:                                                                                                     \
+    if constexpr (eligible(ID))                                                                                \
+      st = host::launch<BlockScaled<Config<BN, STAGES, CG, true, CM, CN, MR, t.bf16(), true>>, kModes>(         \
+          A, Bt, C, M, N, K, s, group_m, max_ctas, splits, scales, ld_a);                                           \
+    break;
+    B200_HGEMM_CONFIGS(B200_CASE)
+#undef B200_CASE
+    default:
+      break;
+  }
+  if (st == host::kOk) g_block_launches.fetch_add(1, std::memory_order_relaxed);
+  return st;
+}
+
+dispatch::Choice select(int M, int N, int K) {
+  dispatch::Choice ch = dispatch::select(GemmType::kE4M3F16Block, M, N, K);
+  ch.config_id = sibling(ch.config_id);
+  ch.splits = sibling_splits(ch.config_id, ch.splits);
+  return ch;
+}
+
+Scales scales_of(const void* scale_a, const void* scale_b) {
+  return Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
+}
+
+int run(int config_id, int out_bf16, const void* A, const void* Bt, void* C, Scales sc, int ld_a, int M, int N, int K,
+        int group_m, int max_ctas, int splits, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (out_bf16 == 0)
+    return run_config<GemmType::kE4M3F16Block>(config_id, A, Bt, C, sc, ld_a, M, N, K, group_m, max_ctas, splits, s);
+  if (out_bf16 == 1)
+    return run_config<GemmType::kE4M3BF16Block>(config_id, A, Bt, C, sc, ld_a, M, N, K, group_m, max_ctas, splits, s);
+  return host::kBadConfig;
+}
+
+}  // namespace block
+}  // namespace b200
+
+extern "C" {
+
+int b200_fp8gemm_blockwise(const void* A, const void* B_kmajor, void* C, const void* scale_a, int ld_a,
+                           const void* scale_b, int out_bf16, int M, int N, int K, void* stream) {
+  using namespace b200;
+  if (out_bf16 != 0 && out_bf16 != 1) return host::kBadConfig;
+  const Scales sc = block::scales_of(scale_a, scale_b);
+  if (const int st = host::validate(GemmType::kE4M3F16Block, A, B_kmajor, C, sc, M, N, K, ld_a)) return st;
+  const dispatch::Choice ch = block::select(M, N, K);
+  return block::run(ch.config_id, out_bf16, A, B_kmajor, C, sc, ld_a, M, N, K, ch.group_m, 0, ch.splits, stream);
+}
+
+int b200_fp8gemm_blockwise_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
+                                      const void* scale_a, int ld_a, const void* scale_b, int M, int N, int K,
+                                      int group_m, int max_ctas, int splits, void* stream) {
+  return b200::block::run(config_id, out_bf16, A, B_kmajor, C, b200::block::scales_of(scale_a, scale_b), ld_a, M,
+                          N, K, group_m, max_ctas, splits, stream);
+}
+
+int b200_fp8gemm_blockwise_select(int M, int N, int K, int* config_id, int* group_m, int* splits) {
+  if (M <= 0 || N <= 0 || K <= 0) return b200::host::kBadShape;
+  const b200::dispatch::Choice ch = b200::block::select(M, N, K);
+  if (config_id) *config_id = ch.config_id;
+  if (group_m) *group_m = ch.group_m;
+  if (splits) *splits = ch.splits;
+  return 0;
+}
+
+unsigned long long b200_fp8block_launch_count(void) {
+  return b200::block::g_block_launches.load(std::memory_order_relaxed);
+}
+
+const char* b200_fp8block_strerror(int status) { return b200::host::status_string(status); }
+
+}  // extern "C"

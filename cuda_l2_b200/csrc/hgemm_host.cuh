@@ -28,6 +28,7 @@ enum Status : int {
   kNotHopper = -7,
   kNoScratch = -8,       // internal: no split-K scratch for this (device, stream) and none can be allocated now (stream capture)
   kBadFp8K = -9,         // e4m3 operands: K % 16 == 0 (16-byte TMA strides at one byte per element)
+  kBadScaleLd = -10,     // block scales: the row stride of A's scales must be >= M and a multiple of 4
   // > 0: a cudaError_t from the launch
 };
 
@@ -43,6 +44,7 @@ inline const char* status_string(int s) {
     case kNotHopper: return "device is not compute capability 9.0 (sm_90a build)";
     case kNoScratch: return "split-K scratch unavailable (allocate it outside stream capture with b200_hgemm_prewarm)";
     case kBadFp8K: return "e4m3 operands need K % 16 == 0 (16-byte row strides at one byte per element)";
+    case kBadScaleLd: return "block scales need ld_a >= M and ld_a % 4 == 0 (16-byte aligned k-block rows of A's scales)";
     default: return s > 0 ? cudaGetErrorString(static_cast<cudaError_t>(s)) : "unknown error";
   }
 }
@@ -70,12 +72,13 @@ constexpr int elem_bytes(Elem e) { return e == Elem::kE4M3 ? 1 : 2; }
 
 // The data-type variants of the kernel family. Everything the host does differently per variant (which kernels it
 // instantiates, the argument rules, the tuned-table entry) reads the variant's row of kGemmTypes.
-enum class GemmType : int { kF16Acc32, kF16Acc16, kBF16, kE4M3F16, kE4M3BF16 };
+enum class GemmType : int { kF16Acc32, kF16Acc16, kBF16, kE4M3F16, kE4M3BF16, kE4M3F16Block, kE4M3BF16Block };
 struct GemmTypeTraits {
   Elem operand, output;
   bool acc_f32;       // fp32 accumulation (fp16 otherwise); the dispatcher reads that accumulator's tuned entry ...
   int table_k_div;    // ... at K / table_k_div: the 16-bit problem that moves as many bytes per k-block
-  bool scaled;        // takes per-tensor fp32 scales in device memory
+  bool scaled;        // takes fp32 scales in device memory (per tensor or rowwise, see Scales) ...
+  bool block = false; // ... or block scales (BlockScaled<> kernels, a library of their own)
   // the Config<> flags: BF16 names the output type, E4M3 the operand type
   constexpr bool bf16() const { return output == Elem::kBF16; }
   constexpr bool e4m3() const { return operand == Elem::kE4M3; }
@@ -86,6 +89,8 @@ constexpr GemmTypeTraits kGemmTypes[] = {
     {Elem::kBF16, Elem::kBF16, true, 1, false},    // kBF16
     {Elem::kE4M3, Elem::kF16, true, 2, true},      // kE4M3F16
     {Elem::kE4M3, Elem::kBF16, true, 2, true},     // kE4M3BF16
+    {Elem::kE4M3, Elem::kF16, true, 2, true, true},    // kE4M3F16Block
+    {Elem::kE4M3, Elem::kBF16, true, 2, true, true},   // kE4M3BF16Block
 };
 constexpr const GemmTypeTraits& traits(GemmType t) { return kGemmTypes[int(t)]; }
 
@@ -93,7 +98,8 @@ constexpr const GemmTypeTraits& traits(GemmType t) { return kGemmTypes[int(t)]; 
 template <class Cfg>
 constexpr GemmType gemm_type(int t = 0) {
   const GemmTypeTraits& x = kGemmTypes[t];
-  return x.acc_f32 == Cfg::ACC_F32 && x.bf16() == Cfg::BF16 && x.e4m3() == Cfg::E4M3 ? GemmType(t) : gemm_type<Cfg>(t + 1);
+  return x.acc_f32 == Cfg::ACC_F32 && x.bf16() == Cfg::BF16 && x.e4m3() == Cfg::E4M3 && x.block == block_scaled<Cfg>()
+             ? GemmType(t) : gemm_type<Cfg>(t + 1);
 }
 
 // Row-major matrix [rows, cols] (cols contiguous) -> 2-D tiled map, box = {box_cols columns, box_rows}, swizzled over the
@@ -178,8 +184,10 @@ inline const DeviceInfo& device_info() {
 // The argument rules of a variant, checked before anything touches the device. TMA wants 16-byte row strides: A / Bt
 // rows hold K operand elements (K % 8 == 0 at two bytes, K % 16 == 0 at one byte), C rows N 16-bit elements. The scales
 // of a scaled variant are fp32 values in device memory: 4-byte aligned per tensor, 16-byte aligned vectors (M and N
-// values) rowwise, where the split-K reductions read the column scales as float4.
-inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K) {
+// values) rowwise, where the split-K reductions read the column scales as float4. Block scales: `a` 16-byte aligned (one
+// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned.
+inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K,
+                    int ld_a = 0) {
   const GemmTypeTraits& t = traits(type);
   if (!A || !Bt || !C || (t.scaled && (!scales.a || !scales.b))) return kNullPointer;
   if (M <= 0 || N <= 0 || K <= 0) return kBadShape;
@@ -187,6 +195,11 @@ inline int validate(GemmType type, const void* A, const void* Bt, const void* C,
   if (N % 8) return kBadAlignment;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
     return kBadAlignment;
+  if (t.block) {
+    if ((reinterpret_cast<uintptr_t>(scales.a) & 15) || (reinterpret_cast<uintptr_t>(scales.b) & 3)) return kBadAlignment;
+    if (ld_a < M || ld_a % 4) return kBadScaleLd;
+    return kOk;
+  }
   if (t.scaled && ((reinterpret_cast<uintptr_t>(scales.a) | reinterpret_cast<uintptr_t>(scales.b)) & (scales.rowwise ? 15 : 3)))
     return kBadAlignment;
   return kOk;
@@ -408,6 +421,7 @@ struct LaunchArgs {
   float* ws; unsigned* ctr; __half* c;
   uint64_t hint_a, hint_b;
   Scales scales;
+  int ld_a;             // block scales: the row stride of scales.a
   cudaStream_t stream;
 };
 
@@ -464,14 +478,15 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
+  const int aux = block_scaled<Cfg>() ? a.ld_a : a.plan.sk_tiles;   // the kernel's aux_arg
   cudaError_t e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                                     a.plan.splits, a.plan.sk_tiles, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
+                                     a.plan.splits, aux, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
   if (e != cudaSuccess && coop && pdl && e != cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
     coop_pdl_ok = false;               // the pair of attributes is not accepted here: cooperative only, from now on
     cfg.numAttrs = na - 1;
     e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                           a.plan.splits, a.plan.sk_tiles, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
+                           a.plan.splits, aux, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
   }
   return e == cudaSuccess ? kOk : int(e);
 }
@@ -480,12 +495,12 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
 // split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
 // mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
 // kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor or rowwise scales
-// of a scaled variant (device pointers), unused otherwise.
+// of a scaled variant (device pointers), unused otherwise; `ld_a`: the row stride of block scales.
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
-           int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}) {
+           int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0) {
   constexpr GemmType kType = gemm_type<Cfg>();
-  int st = validate(kType, A, Bt, C, scales, M, N, K);
+  int st = validate(kType, A, Bt, C, scales, M, N, K, ld_a);
   if (st != kOk) return st;
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
@@ -512,6 +527,7 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   a.group_m = group_m > 0 ? group_m : (Cfg::CTA_GROUP == 2 ? 8 : 16);
   a.c = static_cast<__half*>(C);
   a.scales = scales;
+  a.ld_a = ld_a;
   a.stream = stream;
   // L2 eviction priorities: when one operand is streamed (about) once while the other is re-read by every tile row
   // or column and is small enough to live in L2, keep the small one and let the streamed one go first.

@@ -121,18 +121,47 @@ struct Config {
 
 constexpr int kMaxSplitTiles = 256;   // split-K is only used when tiles * splits <= #SMs
 
+// Block-scaled e4m3 (the layout of DeepSeek-V3-style FP8 checkpoints): one fp32 scale per (row of A, 128-element
+// k-block) and one per 128 x 128 block of Bt. Every k-block's wgmma sum is scaled and added into a separate fp32
+// accumulator, so the kernel holds two accumulator sets: only tiles with M_REP * BN <= 128 qualify, and a BN <= 128 tile
+// lies inside one 128-column scale block of Bt. Each ring stage carries its k-block's scales next to the operands:
+// CTA_M values of A's scales (one 1-D bulk copy, counted in the stage's transaction bytes) and the tile's one value of
+// Bt's (written by the producer before its arrive), 16 bytes of padding keeping the next stage's slice aligned.
+// A wrapper, so that the Config<> instantiations of the other variants, and with them their kernels' names, stay as
+// they are; block_scaled<Cfg>() reads the flag, false for a plain Config.
+template <class Base>
+struct BlockScaled : Base {
+  static constexpr bool BLOCK_SCALED = true;
+  static_assert(Base::E4M3 && Base::M_REP * Base::BN <= 128, "block scales: e4m3, and room for two accumulator sets");
+  static constexpr int SCALE_STAGE_BYTES = Base::CTA_M * 4 + 16;
+  static constexpr int MAX_STAGES =
+      (kSmemLimit - 1024 - Base::EPI_BYTES - Base::BAR_BYTES) / (Base::STAGE_BYTES + SCALE_STAGE_BYTES);
+  static constexpr int STAGES = Base::STAGES < MAX_STAGES ? Base::STAGES : MAX_STAGES;
+  static constexpr int SMEM_BYTES = Base::SMEM_BYTES + STAGES * SCALE_STAGE_BYTES - (Base::STAGES - STAGES) * Base::STAGE_BYTES;
+  static_assert(STAGES >= 2 && SMEM_BYTES <= kSmemLimit, "block-scaled ring does not fit");
+};
+template <class Cfg, class = void>
+struct BlockScaledFlag { static constexpr bool value = false; };
+template <class Cfg>
+struct BlockScaledFlag<Cfg, decltype(void(Cfg::BLOCK_SCALED))> { static constexpr bool value = Cfg::BLOCK_SCALED; };
+template <class Cfg>
+__host__ __device__ constexpr bool block_scaled() { return BlockScaledFlag<Cfg>::value; }
+
 // Scales of an e4m3 launch, in device memory (null for the 16-bit operand types). Per tensor: one fp32 value each.
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
 // 16-byte aligned; C[m,n] = RN_out(fp32(fp32(acc * b[n]) * a[m])). The granularity is a run-time property of the
-// same kernels.
+// same kernels. Block-scaled kernels (BlockScaled<>): value (m, kb) of `a` at a[kb * ld_a + m] (16-byte aligned,
+// ld_a % 4 == 0), `b` row-major [ceil(N/128), ceil(K/128)]. ld_a travels in the kernel's aux_arg, not here: a member
+// added to this struct, even in its padding, changes the code ptxas emits for the other e4m3 kernels.
 struct Scales { const float* a; const float* b; bool rowwise = false; };
 
 // The uniform factor applied to the finished fp32 sum before it is rounded to the output type: fp32(scale_a * scale_b)
 // for per-tensor e4m3 scales, read where it is used (after the grid dependency wait, so a preceding kernel may have just
-// written it). Rowwise launches scale per element instead (scale_quad, the plain epilogue) and do not read it.
+// written it). Rowwise launches scale per element instead (scale_quad, the plain epilogue) and do not read it; block-
+// scaled sums are scaled in the main loop, so their epilogues only round.
 template <class Cfg>
 __device__ __forceinline__ float output_scale(const Scales& s) {
-  if constexpr (Cfg::E4M3) return s.rowwise ? 1.f : __fmul_rn(*s.a, *s.b);
+  if constexpr (Cfg::E4M3 && !block_scaled<Cfg>()) return s.rowwise ? 1.f : __fmul_rn(*s.a, *s.b);
   else return 1.f;
 }
 
@@ -140,7 +169,7 @@ __device__ __forceinline__ float output_scale(const Scales& s) {
 // before its rounding: by the uniform factor, or (rowwise) by b[gn..gn+3] (one 16-byte load) and then a[gm].
 template <class Cfg>
 __device__ __forceinline__ void scale_quad(float4& acc, float scale, const Scales& s, int gm, int gn) {
-  if constexpr (Cfg::E4M3) {
+  if constexpr (Cfg::E4M3 && !block_scaled<Cfg>()) {
     if (s.rowwise) {
       const float sa = s.a[gm];
       const float4 sb = *reinterpret_cast<const float4*>(s.b + gn);
@@ -462,7 +491,8 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
                 const __grid_constant__ CUtensorMap tmap_c,   // C  [M,N]  box {EPI_N, EPI_ROWS}
                 int M, int N, int K, int group_m,
                 int splits_arg,                   // split-K factor (modes kWorkspaceSplitK / kClusterSplitK: one unit per CTA)
-                int sk_tiles_arg,                 // mode kStreamK: the first sk_tiles tiles are cut along K across all workers
+                int aux_arg,                      // mode kStreamK: sk_tiles, the first tiles, cut along K across all
+                                                  // workers; block-scaled kernels (no stream-K): ld_a of scales.a
                 float* __restrict__ splitk_ws,    // [units][128][BN] fp32 partial tiles (workspace split-K) / stream-K slots
                 unsigned* __restrict__ splitk_ctr,   // [2][kMaxSplitTiles] split-K arrive / done counters, then the
                                                      // stream-K flags; all zero between launches
@@ -480,7 +510,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   static_assert(!kSplit || (kBlockM + 32) * BN * 4 <= STAGES * Cfg::STAGE_BYTES, "split-K partials must fit the pipeline smem");
   // the schedule parameters a mode does not use are constants for it
   const int splits = kSplit ? splits_arg : 1;
-  const int sk_tiles = (KMODE == kStreamK) ? sk_tiles_arg : 0;
+  const int sk_tiles = (KMODE == kStreamK) ? aux_arg : 0;
   using namespace ptx;
 
   extern __shared__ uint8_t smem_raw[];
@@ -492,6 +522,10 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   const uint32_t bar_full = smem_bar;                        // [STAGES]
   const uint32_t bar_empty = bar_full + 8 * STAGES;          // [STAGES]
   const uint32_t bar_splitk = bar_empty + 8 * STAGES;        // split-K: bulk loads of the partial slices
+  constexpr bool kBlock = block_scaled<Cfg>();
+  static_assert(!kBlock || KMODE == kPlain || KMODE == kClusterSplitK, "block scales: plain and cluster split-K only");
+  [[maybe_unused]] const int ld_a = kBlock ? aux_arg : 0;
+  [[maybe_unused]] const uint32_t smem_scales = smem_bar + Cfg::BAR_BYTES;   // block scales: [STAGES] scale stages
 
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x) >> 5, 0);
   const int lane = threadIdx.x & 31;
@@ -559,11 +593,31 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         const TileCoord tc = tile_coord(u.tile, num_m_blocks, num_n_blocks, group_m);
         const int m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M + cn * Cfg::A_BOX_ROWS;
         const int n0 = (tc.n_blk * CN + cn) * BN + mi * Cfg::B_BOX_ROWS;
+        // block scales: this CTA's own rows of A's scales (never multicast; none past ld_a, so a padding CTA loads
+        // none) and the row of Bt's scales that holds the tile (none for a tile past N)
+        [[maybe_unused]] const int sa_m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M;
+        [[maybe_unused]] const int sa_rows = kBlock ? max(0, min(Cfg::CTA_M, ld_a - sa_m0)) : 0;
+        [[maybe_unused]] const int sb_n0 = (tc.n_blk * CN + cn) * BN;
+        [[maybe_unused]] const float* sb_row = (kBlock && sb_n0 < N) ? scales.b + size_t(sb_n0 / 128) * num_k_blocks : nullptr;
+        [[maybe_unused]] float sb_chunk = 0.f;   // lane j: Bt's scale of k-block kb0 + 32 i + j
         for (int kb = u.kb0; kb < u.kb1; ++kb) {
           mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+          [[maybe_unused]] float sb_kb = 0.f;
+          if constexpr (kBlock) {   // one global load per lane and 32 k-blocks, handed to the issuing lane by shuffle
+            if (((kb - u.kb0) & 31) == 0) sb_chunk = (sb_row && kb + lane < u.kb1) ? sb_row[kb + lane] : 0.f;
+            sb_kb = __shfl_sync(0xffffffffu, sb_chunk, (kb - u.kb0) & 31);
+          }
           if (elect_one()) {
             const uint32_t full = bar_full + 8 * stage;
-            mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);   // the whole stage lands here, from this CTA and its peers
+            if constexpr (kBlock) {
+              const uint32_t sc = smem_scales + stage * Cfg::SCALE_STAGE_BYTES;
+              st_shared_f32(sc + Cfg::CTA_M * 4, sb_kb);   // published to the consumers by the arrive below
+              mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES + uint32_t(sa_rows) * 4u);
+              if (sa_rows > 0)
+                bulk_load_1d(sc, scales.a + size_t(kb) * ld_a + sa_m0, uint32_t(sa_rows) * 4u, full);
+            } else {
+              mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);   // the whole stage lands here, from this CTA and its peers
+            }
             const uint32_t dst_a = smem_a + stage * Cfg::A_STAGE_BYTES + a_slice;
             const uint32_t dst_b = smem_b + stage * Cfg::B_STAGE_BYTES + b_slice;
             if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, mask_a, hint_a);
@@ -622,6 +676,41 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
     WorkIter work(worker, num_workers, num_tiles, num_k_blocks, splits, sk_tiles);
     WorkUnit u;
     while (work.next(u)) {
+      if constexpr (kBlock) {
+        // ---- block-scaled main loop: each k-block's wgmma group sums into `part` (its first wgmma overwrites it),
+        // is retired, and is promoted into acc with fp32(sa[m] * sb): acc = p * s on the unit's first k-block (keeps
+        // the sign of zero), fmaf(p, s, acc) after it. The warpgroup's tensor-core work pauses during the promotion;
+        // the other consumer warpgroup, out of phase with it, keeps the tensor core busy.
+        static_assert(MR == 1 && Cfg::ACC_F32, "one 64-row block of fp32 accumulators per warpgroup");
+        Reg part[NR];
+        const uint32_t sa_off = uint32_t(wg * 64 + wq * 16 + (lane >> 2)) * 4u;   // row l/4 of the warp's 16; +8: +32 B
+        for (int kb = u.kb0; kb < u.kb1; ++kb) {
+          mbar_wait(bar_full + 8 * stage, phase);
+          const uint64_t da = make_smem_desc(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg) * (64 * kBlockK * 2));
+          const uint64_t db = make_smem_desc(smem_b + stage * Cfg::B_STAGE_BYTES);
+          reg_fence(part);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kBlockK / kWgmmaK; ++k) W::mma(da + uint64_t(2 * k), db + uint64_t(2 * k), part, k > 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(part);
+          const uint32_t sc = smem_scales + stage * Cfg::SCALE_STAGE_BYTES;
+          const float sb = ld_shared_f32(sc + Cfg::CTA_M * 4);
+          const float s_lo = __fmul_rn(ld_shared_f32(sc + sa_off), sb);
+          const float s_hi = __fmul_rn(ld_shared_f32(sc + sa_off + 32u), sb);
+          release(stage);   // operands read by the retired group, scales in registers
+          if (kb == u.kb0) {
+#pragma unroll
+            for (int i = 0; i < NR; ++i) acc[0][i] = __fmul_rn(part[i], (i & 2) ? s_hi : s_lo);
+          } else {
+#pragma unroll
+            for (int i = 0; i < NR; ++i) acc[0][i] = __fmaf_rn(part[i], (i & 2) ? s_hi : s_lo, acc[0][i]);
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        reg_fence(acc[0]);
+      } else {
       // ---- main loop: one wgmma group per k-block, the previous one retired before its stage is released
       int prev = -1;
       for (int kb = u.kb0; kb < u.kb1; ++kb) {
@@ -654,6 +743,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
 #pragma unroll
       for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
       release(prev);
+      }
 
       // ---- epilogue of the unit
       const int tile = u.tile;
@@ -682,7 +772,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         splitk_epilogue<Cfg>(acc[0], t, wg * 64 + wq * 16, lane, tile, worker - tile * splits, splits, m_cta, n0, M, N,
                              splitk_ws, splitk_ctr, c_raw, smem_a, bar_splitk, scales);
       } else {
-        if constexpr (Cfg::E4M3) {
+        if constexpr (Cfg::E4M3 && !kBlock) {   // block-scaled sums are already scaled: the epilogue only rounds
           if (scales.rowwise) {
             // each element gets its own factor, applied as it is packed for the store (epilogue_store_chunk)
 #pragma unroll

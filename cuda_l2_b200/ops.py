@@ -14,8 +14,11 @@ the nearest grid shape — so deployment is a plain operator:
   layout, per-tensor fp32 scales as one-element CUDA tensors, ``(a @ b_kmajor^T) * scale_a * scale_b`` rounded once to
   ``out_dtype`` (fp16 or bf16) — ``torch._scaled_mm`` with per-tensor scales and fast accumulation. Rowwise scales
   follow ``torch._scaled_mm``'s shapes, ``scale_a`` [M,1] and ``scale_b`` [1,N]: ``((a @ b_kmajor^T) * scale_b) * scale_a``.
+  Blockwise scales (DeepSeek-V3-style checkpoints): ``scale_a`` [M, ceil(K/128)] (one per token and 128 input
+  channels), ``scale_b`` [ceil(N/128), ceil(K/128)] (one per 128 x 128 weight block); every 128-wide k-block's sum is
+  scaled and accumulated in fp32 (include/b200_fp8_block.h).
 * :class:`B200Fp8Linear`: inference-only FP8 version of an ``nn.Linear`` (weight quantised once, activation per call;
-  per tensor or rowwise).
+  per tensor, rowwise or blockwise), or of a checkpoint's e4m3 weight and block scales (:meth:`B200Fp8Linear.from_fp8`).
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernel on explicitly
@@ -159,14 +162,28 @@ def _rowwise_scale_arg(s: torch.Tensor) -> torch.Tensor:
     return s if s.data_ptr() % 16 == 0 else s.clone()
 
 
+def _m_major(s: torch.Tensor) -> torch.Tensor:
+    """A blockwise ``scale_a`` [M, nkb] as the kernel reads it: M-major with a row stride ld_a = M rounded up to 4
+    (``buf[:, :M].t()`` of an [nkb, ld_a] buffer), a device copy unless it is already laid out so."""
+    if capi.blockwise_ld_a(s) is not None:
+        return s
+    m, nkb = s.shape
+    buf = torch.empty((nkb, -(-m // 4) * 4), dtype=s.dtype, device=s.device)
+    buf[:, :m].copy_(s.t())
+    return buf[:, :m].t()
+
+
 @torch.library.impl(f"{_LIB}::fp8_gemm", "CUDA")
 def _fp8_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype):
-    m, n, _ = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
+    m, n, k = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
     a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
     c = torch.empty((m, n), dtype=out_dtype, device=a.device)
     if m == 0:
         return c
-    if capi.scale_granularity(m, n, scale_a, scale_b) == "rowwise":
+    granularity = capi.scale_granularity(m, n, scale_a, scale_b, k=k)
+    if granularity == "blockwise":
+        scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
+    elif granularity == "rowwise":
         scale_a, scale_b = _rowwise_scale_arg(scale_a), _rowwise_scale_arg(scale_b)
     else:
         scale_a, scale_b = scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous()
@@ -198,7 +215,8 @@ torch.library.register_autograd(f"{_LIB}::fp8_gemm", _fp8_gemm_no_backward)
 def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
              out_dtype: torch.dtype = torch.float16) -> torch.Tensor:
     """(``a`` [M,K] @ ``b_kmajor`` [N,K]^T), scaled, -> [M,N] ``out_dtype``, e4m3 operands (see the module docstring).
-    Per-tensor scales: one element each. Rowwise scales: ``scale_a`` [M,1], ``scale_b`` [1,N]."""
+    Per-tensor scales: one element each. Rowwise scales: ``scale_a`` [M,1], ``scale_b`` [1,N]. Blockwise scales:
+    ``scale_a`` [M, ceil(K/128)] in any layout, ``scale_b`` [ceil(N/128), ceil(K/128)]."""
     return torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)
 
 
@@ -219,7 +237,33 @@ def quantize_e4m3_rowwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
     return q, scale
 
 
-FP8_GRANULARITIES = ("tensor", "rowwise")
+def quantize_e4m3_blockwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per 1 x 128 block quantisation of activations ``x`` [M, K] on its device: scale[m, kb] = amax(|x[m, 128 kb :
+    128 kb + 128]|) / 448, q = e4m3(x / scale). The scale comes back as the M-major [M, ceil(K/128)] view the kernel
+    reads in place (strides (1, ld_a), ld_a = M rounded up to 4). Torch ops only, no host synchronisation."""
+    m, k = x.shape
+    nkb = capi.num_k_blocks(k)
+    xb = nn.functional.pad(x.float(), (0, nkb * capi.BLOCK - k)).view(m, nkb, capi.BLOCK)
+    scale = (xb.abs().amax(dim=2) / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
+    q = (xb / scale[:, :, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(m, nkb * capi.BLOCK)
+    buf = torch.empty((nkb, -(-m // 4) * 4), dtype=torch.float32, device=x.device)
+    buf[:, :m].copy_(scale.t())
+    return q[:, :k].contiguous(), buf[:, :m].t()
+
+
+def quantize_e4m3_block128x128(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per 128 x 128 block quantisation of a weight ``w`` [N, K] on its device (the layout of DeepSeek-V3-style
+    checkpoints' ``weight_scale_inv``): scale [ceil(N/128), ceil(K/128)] = amax(|block|) / 448, q = e4m3(w / scale).
+    Torch ops only, no host synchronisation."""
+    n, k = w.shape
+    nnb, nkb, b = -(-n // capi.BLOCK), capi.num_k_blocks(k), capi.BLOCK
+    wb = nn.functional.pad(w.float(), (0, nkb * b - k, 0, nnb * b - n)).view(nnb, b, nkb, b)
+    scale = (wb.abs().amax(dim=(1, 3)) / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
+    q = (wb / scale[:, None, :, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(nnb * b, nkb * b)
+    return q[:n, :k].contiguous(), scale.contiguous()
+
+
+FP8_GRANULARITIES = ("tensor", "rowwise", "blockwise")
 
 
 class B200Fp8Linear(nn.Module):
@@ -227,17 +271,23 @@ class B200Fp8Linear(nn.Module):
     every call quantises the activation on the device and runs ``cuda_l2_b200::fp8_gemm``, then adds the bias (shared
     with the source layer). ``granularity="tensor"``: one scale for the weight (``weight_scale`` [1]) and one per call
     for the activation. ``"rowwise"``: one scale per output channel (``weight_scale`` [1, out_features], the layout of
-    common FP8 checkpoints) and one per activation row (token). No ``.item()`` and no host synchronisation, so the
+    common FP8 checkpoints) and one per activation row (token). ``"blockwise"``: one scale per 128 x 128 weight block
+    (``weight_scale`` [ceil(out/128), ceil(in/128)], DeepSeek-V3-style checkpoints, loadable as they are with
+    :meth:`from_fp8`) and one per token and 128 input channels. No ``.item()`` and no host synchronisation, so the
     forward can be captured in a CUDA graph. Needs in_features % 16 == 0, out_features % 8 == 0."""
+
+    @staticmethod
+    def _check_fits(in_features: int, out_features: int, out_dtype: torch.dtype, what) -> None:
+        t = capi.gemm_type(torch.float8_e4m3fn, out_dtype)
+        if t is None or not t.fits(out_features, in_features):
+            raise capi.B200HgemmError(f"cannot convert {what} to FP8: needs in_features % 16 == 0, out_features % 8 == 0 "
+                                      f"and an fp16 / bf16 output type (got {out_dtype})")
 
     @classmethod
     def from_linear(cls, lin: nn.Linear, out_dtype: torch.dtype | None = None,
                     granularity: str = "tensor") -> "B200Fp8Linear":
         out_dtype = out_dtype or lin.weight.dtype
-        t = capi.gemm_type(torch.float8_e4m3fn, out_dtype)
-        if t is None or not t.fits(lin.out_features, lin.in_features):
-            raise capi.B200HgemmError(f"cannot convert {lin} to FP8: needs in_features % 16 == 0, out_features % 8 == 0 "
-                                      f"and an fp16 / bf16 output type (got {out_dtype})")
+        cls._check_fits(lin.in_features, lin.out_features, out_dtype, lin)
         if granularity not in FP8_GRANULARITIES:
             raise capi.B200HgemmError(f"granularity must be one of {FP8_GRANULARITIES}, got {granularity!r}")
         new = cls.__new__(cls)
@@ -248,11 +298,33 @@ class B200Fp8Linear(nn.Module):
             if granularity == "rowwise":
                 w_q, w_scale = quantize_e4m3_rowwise(lin.weight)
                 w_scale = w_scale.reshape(1, lin.out_features)   # [1, N]: the column scales of the product
+            elif granularity == "blockwise":
+                w_q, w_scale = quantize_e4m3_block128x128(lin.weight)
             else:
                 w_q, w_scale = quantize_e4m3(lin.weight)
         new.register_buffer("weight_fp8", w_q)
         new.register_buffer("weight_scale", w_scale)
         new.bias = lin.bias                                  # shared with the source layer
+        return new
+
+    @classmethod
+    def from_fp8(cls, weight_fp8: torch.Tensor, weight_scale: torch.Tensor, bias: torch.Tensor | None = None,
+                 out_dtype: torch.dtype = torch.bfloat16) -> "B200Fp8Linear":
+        """A blockwise layer from a checkpoint's e4m3 weight [out, in] and its fp32 128 x 128 block scales
+        [ceil(out/128), ceil(in/128)] (``weight_scale_inv``), taken as they are: no re-quantisation."""
+        out_features, in_features = weight_fp8.shape
+        cls._check_fits(in_features, out_features, out_dtype, f"a [{out_features}, {in_features}] weight")
+        want = (-(-out_features // capi.BLOCK), capi.num_k_blocks(in_features))
+        if weight_fp8.dtype != torch.float8_e4m3fn or weight_scale.dtype != torch.float32 or tuple(weight_scale.shape) != want:
+            raise capi.B200HgemmError(f"from_fp8 needs a float8_e4m3fn weight and fp32 block scales of shape {list(want)}, "
+                                      f"got {weight_fp8.dtype} and {weight_scale.dtype} {list(weight_scale.shape)}")
+        new = cls.__new__(cls)
+        nn.Module.__init__(new)
+        new.in_features, new.out_features, new.out_dtype = in_features, out_features, out_dtype
+        new.granularity = "blockwise"
+        new.register_buffer("weight_fp8", weight_fp8.contiguous())
+        new.register_buffer("weight_scale", weight_scale.contiguous())
+        new.bias = bias
         return new
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
@@ -261,7 +333,8 @@ class B200Fp8Linear(nn.Module):
         if x2.shape[0] == 0:
             y = x2.new_empty((0, self.out_features), dtype=self.out_dtype)
         else:
-            quantize = quantize_e4m3_rowwise if self.granularity == "rowwise" else quantize_e4m3
+            quantize = {"rowwise": quantize_e4m3_rowwise, "blockwise": quantize_e4m3_blockwise}.get(self.granularity,
+                                                                                                 quantize_e4m3)
             x_q, x_scale = quantize(x2)
             y = torch.ops.cuda_l2_b200.fp8_gemm(x_q, self.weight_fp8, x_scale, self.weight_scale, self.out_dtype)
         if self.bias is not None:
@@ -274,4 +347,4 @@ class B200Fp8Linear(nn.Module):
 
 
 __all__ = ["hgemm", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
-           "quantize_e4m3_rowwise", "B200Fp8Linear"]
+           "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear"]

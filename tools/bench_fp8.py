@@ -7,7 +7,9 @@ Shapes: --mnk (default 4096_4096_4096), 4096^3 and 2048x11008x4096. Per shape, s
 b200_fp8gemm (e4m3 operands quantised per tensor from N(0,1) data, fp16 out, the dispatcher's choice),
 torch._scaled_mm with fast accumulation on and off (same operands and scales), b200_hgemm_f32acc on the fp16 data, and
 two bf16-out legs on the same data quantised per row (scales [M,1] and [1,N]): b200_fp8gemm_rowwise and
-torch._scaled_mm with rowwise scales and fast accumulation.
+torch._scaled_mm with rowwise scales and fast accumulation, and two bf16-out legs on the same data quantised per block
+(1 x 128 for a, 128 x 128 for bt): b200_fp8gemm_blockwise (libb200_fp8block.so) and torch._scaled_mm with blockwise
+scales, the latter reported as {"skipped": reason} where torch refuses it.
 Each leg: warm-up, then K back-to-back calls between two CUDA events on the legacy default stream, rotating over seeded
 operand sets whose fp16 footprint exceeds the 50 MB L2 four times. TFLOP/s = 2MNK per call. Prints one JSON line with
 the card's name and enforced power limit (figures are only comparable at the same limit). Writes nothing.
@@ -55,9 +57,12 @@ def time_shape(m: int, n: int, k: int, steps: int, warmup: int, gen: torch.Gener
         qb, sb = ops.quantize_e4m3(bt)
         qa_r, sa_r = ops.quantize_e4m3_rowwise(a)
         qb_r, sb_r = ops.quantize_e4m3_rowwise(bt)
+        qa_b, sa_b = ops.quantize_e4m3_blockwise(a)
+        qb_b, sb_b = ops.quantize_e4m3_block128x128(bt)
         sets.append(dict(a=a, bt=bt, qa=qa, qb=qb, sa=sa, sb=sb, c=torch.empty((m, n), dtype=torch.half, device="cuda"),
                          qa_r=qa_r, qb_r=qb_r, sa_r=sa_r, sb_r=sb_r.reshape(1, n),
-                         c_bf16=torch.empty((m, n), dtype=torch.bfloat16, device="cuda")))
+                         c_bf16=torch.empty((m, n), dtype=torch.bfloat16, device="cuda"),
+                         qa_b=qa_b, qb_b=qb_b, sa_b=sa_b, sb_b=sb_b))
 
     def ours_fp8(st):
         capi.fp8_gemm(st["qa"], st["qb"], st["c"], st["sa"], st["sb"])
@@ -76,11 +81,26 @@ def time_shape(m: int, n: int, k: int, steps: int, warmup: int, gen: torch.Gener
         return torch._scaled_mm(st["qa_r"], st["qb_r"].t(), scale_a=st["sa_r"], scale_b=st["sb_r"],
                                 out_dtype=torch.bfloat16, use_fast_accum=True)
 
+    def ours_blockwise(st):
+        capi.fp8_gemm(st["qa_b"], st["qb_b"], st["c_bf16"], st["sa_b"], st["sb_b"])
+
+    def scaled_blockwise(st):
+        return torch._scaled_mm(st["qa_b"], st["qb_b"].t(), scale_a=st["sa_b"], scale_b=st["sb_b"].t(),
+                                out_dtype=torch.bfloat16)
+
     legs = {"ours_e4m3": ours_fp8, "scaled_mm_fast_accum": scaled(True), "scaled_mm_no_fast_accum": scaled(False),
             "ours_fp16_fp32acc": ours_fp16, "ours_e4m3_rowwise_bf16": ours_rowwise,
-            "scaled_mm_rowwise_fast_accum_bf16": scaled_rowwise}
+            "scaled_mm_rowwise_fast_accum_bf16": scaled_rowwise, "ours_e4m3_blockwise_bf16": ours_blockwise,
+            "scaled_mm_blockwise_bf16": scaled_blockwise}
     row = {}
     for name, fn in legs.items():
+        if name == "scaled_mm_blockwise_bf16":
+            try:
+                fn(sets[0])
+                torch.cuda.synchronize()
+            except (RuntimeError, NotImplementedError, ValueError) as e:
+                row[name] = {"skipped": str(e).splitlines()[0]}
+                continue
         for i in range(max(warmup, 3)):
             fn(sets[i % nsets])
         torch.cuda.synchronize()
@@ -94,6 +114,8 @@ def time_shape(m: int, n: int, k: int, steps: int, warmup: int, gen: torch.Gener
         row[name] = {"tflops": 2.0 * m * n * k / (ms * 1e-3) * 1e-12, "ms_per_call": ms}
     cfg_id, group_m, splits = capi.fp8_select(m, n, k)
     row["ours_e4m3"]["dispatch"] = {"config": cfg_id, "group_m": group_m, "splits": splits}
+    cfg_id, group_m, splits = capi.fp8_blockwise_select(m, n, k)
+    row["ours_e4m3_blockwise_bf16"]["dispatch"] = {"config": cfg_id, "group_m": group_m, "splits": splits}
     return row
 
 
