@@ -272,10 +272,11 @@ def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = (), strided
 
 
 def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = None, config_id: int | None = None,
-                group_m: int = 0, splits: int = 1) -> None:
+                group_m: int = 0, splits: int = 1, max_ctas: int = 0) -> None:
     """c[M,N] = a[M,K] @ b_kmajor[N,K]^T with the operands' dtype deciding the kernel family: fp16 (fp32 or fp16
     accumulation) or bf16 (fp32 accumulation). ``b_kmajor`` is shaped as stored, [N,K] — an ``nn.Linear`` weight.
-    ``config_id`` pins one kernel configuration (tests); default is the dispatcher."""
+    ``config_id`` pins one kernel configuration (tests); default is the dispatcher. ``max_ctas`` (with ``config_id``)
+    caps the CTAs of the launch, 0 meaning all SMs, so that each worker runs several tiles."""
     import torch
 
     m, n, k = _kmajor_operands(a, b_kmajor, c, acc)
@@ -285,24 +286,26 @@ def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = No
         if config_id is None:
             st = lib.b200_bgemm_f32acc(a.data_ptr(), None, b_kmajor.data_ptr(), c.data_ptr(), m, n, k, stream)
         else:
-            st = lib.b200_bgemm_run_config(config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m, 0, splits, stream)
+            st = lib.b200_bgemm_run_config(config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m,
+                                           max_ctas, splits, stream)
     elif config_id is None:
         fn = lib.b200_hgemm_f32acc if bits == 32 else lib.b200_hgemm_f16acc
         st = fn(a.data_ptr(), None, b_kmajor.data_ptr(), c.data_ptr(), m, n, k, stream)
     else:
-        st = lib.b200_hgemm_run_config(bits, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m, 0, splits, stream)
+        st = lib.b200_hgemm_run_config(bits, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m,
+                                       max_ctas, splits, stream)
     _check(st, "b200 gemm")
 
 
 def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config_id: int | None = None,
-             group_m: int = 0, splits: int = 1) -> None:
+             group_m: int = 0, splits: int = 1, max_ctas: int = 0) -> None:
     """c[M,N] = (a[M,K] @ b_kmajor[N,K]^T) scaled, with ``float8_e4m3fn`` operands, fp32 accumulation and one rounding
     to ``c``'s dtype (fp16 or bf16). ``scale_a`` / ``scale_b`` are fp32 CUDA tensors, read when the kernel runs: one
     element each (per tensor: ``* scale_a * scale_b``), or ``scale_a`` [M,1] and ``scale_b`` [1,N], 16-byte aligned
     (rowwise: ``* scale_b[n]``, then ``* scale_a[m]``), or blockwise scales (include/b200_fp8_block.h): ``scale_a``
     [M, ceil(K/128)] M-major (strides (1, ld_a), see :func:`blockwise_ld_a`), ``scale_b`` [ceil(N/128), ceil(K/128)]
     contiguous, run by libb200_fp8block.so. ``config_id`` pins one kernel configuration (tests; ``splits`` as in
-    b200_hgemm_run_config); default is the dispatcher."""
+    b200_hgemm_run_config; ``max_ctas`` as in :func:`gemm_kmajor`); default is the dispatcher."""
     import torch
 
     m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b), strided_scale_a=True)
@@ -320,7 +323,7 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
         else:
             st = blk.b200_fp8gemm_blockwise_run_config(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(),
                                                        c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr(), m, n,
-                                                       k, group_m, 0, splits, stream)
+                                                       k, group_m, max_ctas, splits, stream)
         if st != 0:
             raise B200HgemmError(f"b200_fp8gemm_blockwise failed: status {st} ({blk.b200_fp8block_strerror(st).decode()})")
         return
@@ -335,7 +338,7 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     else:
         fn = lib.b200_fp8gemm_rowwise_run_config if rowwise else lib.b200_fp8gemm_run_config
         st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(),
-                scale_b.data_ptr(), m, n, k, group_m, 0, splits, stream)
+                scale_b.data_ptr(), m, n, k, group_m, max_ctas, splits, stream)
     _check(st, "b200_fp8gemm_rowwise" if rowwise else "b200_fp8gemm")
 
 

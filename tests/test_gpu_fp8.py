@@ -24,6 +24,7 @@ import torch
 
 from oracle import fp8 as fp8_oracle
 from cuda_l2_b200 import capi
+from test_gpu_exact_range import KMODE_CASES, case8, e4m3_refs, run8
 
 pytestmark = pytest.mark.gpu
 
@@ -106,7 +107,8 @@ K_MODES = [
     (1, 512, 512, 8192, -8, "cluster-split-k"),
     (1, 512, 512, 8192, 100, "stream-k"),
     (4, 1280, 1792, 1024, 101, "stream-k"),               # CTA pairs: 70 tiles on 66 workers
-]
+] + [(cfg, m, n, 2 * k, sp, mode) for cfg, m, n, k, sp, mode in KMODE_CASES]
+# ^ workspace split-K 4/16/64 and cluster split-K -2/-4/-8 on configurations 0, 1, 2, 5, stream-K 100/101 on 0-6
 
 
 @pytest.mark.parametrize("cfg,m,n,k,splits,mode", K_MODES)
@@ -116,6 +118,10 @@ def test_every_k_mode_bit_exact(cfg, m, n, k, splits, mode):
     for out_dtype, pair in ((torch.float16, POW2), (torch.bfloat16, NON_POW2)):
         got = bits(run(a, bt, pair, out_dtype, config_id=cfg, splits=splits))
         assert np.array_equal(got, want_bits(a, bt, pair, out_dtype)), (cfg, splits, out_dtype)
+    # the full output range (exact_domain.py): ties, subnormals and overflow reach every reduction site
+    da, dbt, _, _ = case8(m, n, k)
+    for out_dtype, sa, sb, want in e4m3_refs(m, n, k)["tensor"]:
+        assert np.array_equal(run8(da, dbt, sa, sb, out_dtype, config_id=cfg, splits=splits), want), (cfg, splits, out_dtype)
 
 
 def test_scale_written_just_before_the_gemm_is_the_one_used():

@@ -29,6 +29,7 @@ import torch
 
 from cuda_l2_b200 import capi
 from fp8_rowwise_ref import fp8gemm_f32acc_rowwise
+from test_gpu_exact_range import case8, e4m3_refs, run8
 from test_gpu_fp8 import K_MODES, small_ints
 
 pytestmark = pytest.mark.gpu
@@ -99,6 +100,10 @@ def test_every_k_mode_bit_exact(cfg, m, n, k, splits, mode):
         sa, sb = vectors(m, n, 60 + splits, pow2)
         got = bits(run(a, bt, sa, sb, out_dtype, config_id=cfg, splits=splits))
         assert np.array_equal(got, want_bits(a, bt, sa, sb, out_dtype)), (cfg, splits, out_dtype)
+    # the full output range (exact_domain.py): ties, subnormals and overflow reach every reduction site
+    da, dbt, _, _ = case8(m, n, k)
+    for out_dtype, sa, sb, want in e4m3_refs(m, n, k)["rowwise"]:
+        assert np.array_equal(run8(da, dbt, sa, sb, out_dtype, config_id=cfg, splits=splits), want), (cfg, splits, out_dtype)
 
 
 @pytest.mark.parametrize("out_dtype", [torch.float16, torch.bfloat16])
