@@ -4,6 +4,7 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
 
 * ``libb200_hgemm.so``  — the C-ABI product library (include/b200_hgemm.h)
 * ``libb200_fp8block.so`` — the block-scaled FP8 GEMM (include/b200_fp8_block.h)
+* ``libb200_batched.so`` — the batched fp16 / bf16 GEMM (include/b200_batched.h)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -90,6 +91,29 @@ def build_fp8block(verbose: bool = False, force: bool = False) -> Path:
     return out
 
 
+BATCHED_VARIANTS = (0, 1, 2)   # fp16 with fp32 accumulation, fp16 with fp16 accumulation, bf16 (the GemmType index)
+
+
+def build_batched(verbose: bool = False, force: bool = False) -> Path:
+    """The batched 16-bit kernels: a library of their own, so that libb200_hgemm.so's device code is unaffected. One
+    source, compiled once per data type in parallel (31 kernels each), then linked."""
+    LIB_DIR.mkdir(exist_ok=True)
+    out = LIB_DIR / "libb200_batched.so"
+    src = CSRC / "b200_batched_capi.cu"
+    if force or _stale(out, [src] + _headers()):
+        objs = [LIB_DIR / f"b200_batched_{v}.o" for v in BATCHED_VARIANTS]
+        from concurrent.futures import ThreadPoolExecutor
+        with ThreadPoolExecutor(len(objs)) as pool:
+            for f in [pool.submit(_run, [nvcc_path(), *ARCH_FLAGS, *COMMON, f"-DB200_BATCHED_VARIANT={v}", "-c", "-o",
+                                         str(obj), str(src)], verbose)
+                      for v, obj in zip(BATCHED_VARIANTS, objs)]:
+                f.result()
+        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs)], verbose)
+        for obj in objs:
+            obj.unlink()
+    return out
+
+
 def build_baselines(verbose: bool = False, force: bool = False) -> Path:
     LIB_DIR.mkdir(exist_ok=True)
     out = LIB_DIR / "libb200_baselines.so"
@@ -113,9 +137,10 @@ def build_dev_check(verbose: bool = False, force: bool = False) -> Path:
 
 def build_all(verbose: bool = False, force: bool = False) -> dict[str, Path]:
     from concurrent.futures import ThreadPoolExecutor
-    with ThreadPoolExecutor(2) as pool:   # the block-scaled library compiles next to the product library's two units
+    with ThreadPoolExecutor(3) as pool:   # the block-scaled and batched libraries compile next to the product library
         block = pool.submit(build_fp8block, verbose, force)
-        out = {"capi": build_capi(verbose, force), "fp8block": block.result()}
+        batched = pool.submit(build_batched, verbose, force)
+        out = {"capi": build_capi(verbose, force), "fp8block": block.result(), "batched": batched.result()}
     if (CSRC / "b200_baselines_capi.cu").exists():
         out["baselines"] = build_baselines(verbose, force)
     out["dev_check"] = build_dev_check(verbose, force)

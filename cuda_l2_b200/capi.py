@@ -16,6 +16,7 @@ LIB_DIR = Path(__file__).resolve().parent / "lib"
 _hgemm = None
 _baselines = None
 _fp8block = None
+_batched = None
 
 ACC_BITS = {"fp32": 32, "fp16": 16, 32: 32, 16: 16}
 
@@ -93,6 +94,27 @@ def fp8block_lib() -> ctypes.CDLL:
     return _fp8block
 
 
+def batched_lib() -> ctypes.CDLL:
+    """libb200_batched.so: the batched fp16 / bf16 GEMM (include/b200_batched.h)."""
+    global _batched
+    if _batched is None:
+        lib = _load("libb200_batched.so")
+        vp, i, ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
+        lib.b200_batched_gemm.argtypes = [i, vp, vp, vp, vp, i, i, i, i, vp]
+        lib.b200_batched_gemm.restype = i
+        lib.b200_batched_gemm_run_config.argtypes = [i, i, vp, vp, vp, vp, i, i, i, i, i, i, vp]
+        lib.b200_batched_gemm_run_config.restype = i
+        lib.b200_batched_select.argtypes = [i, i, i, i, i, ip, ip]
+        lib.b200_batched_select.restype = i
+        lib.b200_batched_schedule_units.argtypes = [i, i, i, i, i, ip, i, i, ip, i, ip]
+        lib.b200_batched_schedule_units.restype = i
+        lib.b200_batched_launch_count.restype = ctypes.c_ulonglong
+        lib.b200_batched_strerror.argtypes = [i]
+        lib.b200_batched_strerror.restype = ctypes.c_char_p
+        _batched = lib
+    return _batched
+
+
 def baselines_lib() -> ctypes.CDLL:
     global _baselines
     if _baselines is None:
@@ -123,6 +145,10 @@ def exported_symbols() -> dict[str, list[str]]:
         "libb200_fp8block.so": [
             "b200_fp8gemm_blockwise", "b200_fp8gemm_blockwise_run_config", "b200_fp8gemm_blockwise_select",
             "b200_fp8block_launch_count", "b200_fp8block_strerror",
+        ],
+        "libb200_batched.so": [
+            "b200_batched_gemm", "b200_batched_gemm_run_config", "b200_batched_select", "b200_batched_schedule_units",
+            "b200_batched_launch_count", "b200_batched_strerror",
         ],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
@@ -362,6 +388,102 @@ def fp8_blockwise_select(m: int, n: int, k: int) -> tuple[int, int, int]:
 
 def fp8block_launch_count() -> int:
     return int(fp8block_lib().b200_fp8block_launch_count())
+
+
+# ------------------------------------------------------------------------------------------ batched (libb200_batched.so)
+def batched_variant(dtype, acc: str | int = "fp32") -> int | None:
+    """The ``variant`` argument of include/b200_batched.h (the GemmType index): 0 fp16 with fp32 accumulation, 1 fp16
+    with fp16 accumulation, 2 bf16; None for any other combination."""
+    import torch
+
+    return {(torch.float16, 32): 0, (torch.float16, 16): 1, (torch.bfloat16, 32): 2}.get((dtype, ACC_BITS.get(acc)))
+
+
+def check_batched_operands(a, b_kmajor, acc: str | int = "fp32", masked_m=None) -> tuple[int, int, int, int]:
+    """(B, M, N, K) of a[B,M,K] @ b_kmajor[B,N,K]^T per batch, by the rules of the 16-bit variant the dtype and ``acc``
+    name (the 2-D rules per matrix, :meth:`GemmType.fits`); ``masked_m``, if given, is an int32 tensor of B elements.
+    Checks shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
+    import torch
+
+    try:
+        (bsz, m, k), (bsz2, n, k2) = a.shape, b_kmajor.shape
+    except ValueError:
+        raise B200HgemmError(f"3-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
+    t = gemm_type(a.dtype, a.dtype, acc) if b_kmajor.dtype == a.dtype else None
+    if t is None or t.scale is not None:
+        raise B200HgemmError(f"no batched kernel for {a.dtype} x {b_kmajor.dtype} with acc={acc!r} (fp16 with fp32 or "
+                             "fp16 accumulation, bf16 with fp32)")
+    if bsz2 != bsz or k2 != k:
+        raise B200HgemmError(f"batch counts or inner dimensions differ: a {tuple(a.shape)}, b_kmajor "
+                             f"{tuple(b_kmajor.shape)} (K-major: [B, N, K])")
+    if not t.fits(n, k):
+        raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % {t.k_align} == 0 (16-byte TMA strides), "
+                             f"got N={n}, K={k}")
+    if masked_m is not None and (masked_m.dtype != torch.int32 or tuple(masked_m.shape) != (bsz,)):
+        raise B200HgemmError(f"masked_m must be an int32 tensor of shape [{bsz}], got {masked_m.dtype} "
+                             f"{tuple(masked_m.shape)}")
+    return bsz, m, n, k
+
+
+def gemm_batched(a, b_kmajor, c, acc: str | int = "fp32", masked_m=None, stream: int | None = None,
+                 config_id: int | None = None, group_m: int = 0, max_ctas: int = 0) -> None:
+    """c[b] = a[b] @ b_kmajor[b]^T for every b, fp16 (fp32 or fp16 accumulation) or bf16 operands, all three contiguous
+    CUDA tensors ([B,M,K], [B,N,K], [B,M,N]). ``masked_m``: an optional int32 CUDA tensor [B], read by the kernel when
+    it runs: only rows [0, clamp(masked_m[b], 0, M)) of c[b] are computed (include/b200_batched.h). ``config_id``
+    pins one kernel configuration (tests), ``max_ctas`` caps the CTAs (0: all SMs); default is the dispatcher."""
+    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("masked_m", masked_m)):
+        if x is not None and (not x.is_cuda or not x.is_contiguous()):
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    bsz, m, n, k = check_batched_operands(a, b_kmajor, acc, masked_m)
+    if c.dtype != a.dtype or tuple(c.shape) != (bsz, m, n):
+        raise B200HgemmError(f"c must be {a.dtype} [{bsz}, {m}, {n}], got {c.dtype} {tuple(c.shape)}")
+    lib = batched_lib()
+    variant = batched_variant(a.dtype, acc)
+    mm = None if masked_m is None else masked_m.data_ptr()
+    if config_id is None:
+        st = lib.b200_batched_gemm(variant, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), mm, bsz, m, n, k, stream)
+    else:
+        st = lib.b200_batched_gemm_run_config(variant, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), mm,
+                                              bsz, m, n, k, group_m, max_ctas, stream)
+    if st != 0:
+        raise B200HgemmError(f"b200_batched_gemm failed: status {st} ({lib.b200_batched_strerror(st).decode()})")
+
+
+def batched_select(variant: int, b: int, m: int, n: int, k: int) -> tuple[int, int]:
+    """(config id, rasterisation group) the batched dispatcher uses (b200_batched_select)."""
+    cid, gm = ctypes.c_int(), ctypes.c_int()
+    st = batched_lib().b200_batched_select(variant, b, m, n, k, ctypes.byref(cid), ctypes.byref(gm))
+    if st != 0:
+        raise B200HgemmError(f"b200_batched_select failed: status {st}")
+    return cid.value, gm.value
+
+
+def batched_schedule(config_id: int, b: int, m: int, n: int, k: int, masked_m=None, num_sms: int = 132) -> dict:
+    """Host-side view of a batched launch's schedule (no GPU needed; the kernel walks the same code), with the
+    launcher's default rasterisation. ``masked_m``: per-batch row counts (a sequence of ints) or None (dense).
+
+    Returns ``{"workers": W, "units": [[(batch, m_block, n_block), ...] per worker]}``; blocks are cluster blocks."""
+    lib = batched_lib()
+    counts = None if masked_m is None else (ctypes.c_int * b)(*masked_m)
+    nw = ctypes.c_int()
+    cap = 256
+    buf = (ctypes.c_int * (3 * cap))()
+    st = lib.b200_batched_schedule_units(config_id, b, m, n, k, counts, num_sms, 0, buf, cap, ctypes.byref(nw))
+    if st < 0:
+        raise B200HgemmError(f"b200_batched_schedule_units failed: status {st}")
+    units = []
+    for w in range(nw.value):
+        cnt = lib.b200_batched_schedule_units(config_id, b, m, n, k, counts, num_sms, w, buf, cap, None)
+        if cnt > cap:
+            cap = cnt
+            buf = (ctypes.c_int * (3 * cap))()
+            cnt = lib.b200_batched_schedule_units(config_id, b, m, n, k, counts, num_sms, w, buf, cap, None)
+        units.append([(buf[3 * j], buf[3 * j + 1], buf[3 * j + 2]) for j in range(cnt)])
+    return {"workers": nw.value, "units": units}
+
+
+def batched_launch_count() -> int:
+    return int(batched_lib().b200_batched_launch_count())
 
 
 def hgemm_config(a, b_col_major, c, config_id: int, acc: str | int = "fp32", group_m: int = 0, max_ctas: int = 0,

@@ -103,15 +103,18 @@ constexpr GemmType gemm_type(int t = 0) {
 }
 
 // Row-major matrix [rows, cols] (cols contiguous) -> 2-D tiled map, box = {box_cols columns, box_rows}, swizzled over the
-// box's inner extent in bytes (128 or 64). Out-of-bounds elements read as zero / are not written.
+// box's inner extent in bytes (128 or 64). Out-of-bounds elements read as zero / are not written. batches > 0: a
+// contiguous batch of such matrices [batches, rows, cols] -> 3-D map {cols, rows, batches}, box depth 1, so that the
+// bounds of each matrix hold for every box (batches == 1 is still a 3-D map: the batched kernels issue 3-D copies).
 inline int encode_2d(CUtensorMap* map, const void* ptr, int rows, int cols, int box_rows, int box_cols = kBlockK,
-                     Elem elem = Elem::kF16) {
+                     Elem elem = Elem::kF16, int batches = 0) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return kNoDriver;
-  cuuint64_t dims[2] = {cuuint64_t(cols), cuuint64_t(rows)};
-  cuuint64_t strides[1] = {cuuint64_t(cols) * elem_bytes(elem)};
-  cuuint32_t box[2] = {cuuint32_t(box_cols), cuuint32_t(box_rows)};
-  cuuint32_t estr[2] = {1, 1};
+  const cuuint32_t rank = batches > 0 ? 3 : 2;
+  cuuint64_t dims[3] = {cuuint64_t(cols), cuuint64_t(rows), cuuint64_t(batches)};
+  cuuint64_t strides[2] = {cuuint64_t(cols) * elem_bytes(elem), cuuint64_t(rows) * cuuint64_t(cols) * elem_bytes(elem)};
+  cuuint32_t box[3] = {cuuint32_t(box_cols), cuuint32_t(box_rows), 1};
+  cuuint32_t estr[3] = {1, 1, 1};
   // the swizzle span equals the box's inner extent: 64 fp16 or 128 e4m3 = 128 B, 32 fp16 = 64 B
   const CUtensorMapSwizzle swz = box_cols * elem_bytes(elem) == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   // experiment hook: B200_HGEMM_L2_PROMOTION = 0 (none) | 1 (64 B) | 2 (128 B) | 3 (256 B, the default)
@@ -123,18 +126,20 @@ inline int encode_2d(CUtensorMap* map, const void* ptr, int rows, int cols, int 
   }();
   const CUtensorMapDataType dt = elem == Elem::kE4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                : elem == Elem::kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUresult r = fn(map, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = fn(map, dt, rank, const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? kOk : kEncodeFailed;
 }
 
 // Small direct-mapped cache of encoded maps: benchmark loops re-present the same few pointers
 // (the caching allocator recycles them), and an encode costs about a microsecond of host time. The key carries the
-// element type: an e4m3 and an fp16 map of the same pointer and dimensions differ.
+// element type: an e4m3 and an fp16 map of the same pointer and dimensions differ; and the batch count (0: a 2-D map),
+// so one cache serves both ranks.
 struct MapKey {
-  const void* ptr; int rows, cols, box_rows, box_cols; Elem elem;
+  const void* ptr; int rows, cols, box_rows, box_cols; Elem elem; int batches;
   bool operator==(const MapKey& o) const {
-    return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows && box_cols == o.box_cols && elem == o.elem;
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows && box_cols == o.box_cols &&
+           elem == o.elem && batches == o.batches;
   }
 };
 struct MapCache {
@@ -144,14 +149,15 @@ struct MapCache {
   bool valid[kSlots];
   MapCache() { std::memset(valid, 0, sizeof(valid)); }
   // Copies the map out: two operands of one call may share a slot, so a pointer into the cache would alias.
-  int get(const void* ptr, int rows, int cols, int box_rows, CUtensorMap* out, int box_cols = kBlockK, Elem elem = Elem::kF16) {
-    MapKey k{ptr, rows, cols, box_rows, box_cols, elem};
+  int get(const void* ptr, int rows, int cols, int box_rows, CUtensorMap* out, int box_cols = kBlockK, Elem elem = Elem::kF16,
+          int batches = 0) {
+    MapKey k{ptr, rows, cols, box_rows, box_cols, elem, batches};
     uint64_t h = (reinterpret_cast<uint64_t>(ptr) >> 8) * 0x9E3779B97F4A7C15ull;
     h ^= uint64_t(uint32_t(rows)) * 0xC2B2AE3D27D4EB4Full + uint64_t(uint32_t(cols)) * 0x165667B19E3779F9ull +
-         uint64_t(box_rows) * 131u + uint64_t(box_cols);
+         uint64_t(box_rows) * 131u + uint64_t(box_cols) + uint64_t(uint32_t(batches)) * 0x27D4EB2F165667C5ull;
     int slot = int((h >> 32) % kSlots);
     if (!(valid[slot] && keys[slot] == k)) {
-      int st = encode_2d(&maps[slot], ptr, rows, cols, box_rows, box_cols, elem);
+      int st = encode_2d(&maps[slot], ptr, rows, cols, box_rows, box_cols, elem, batches);
       if (st != kOk) { valid[slot] = false; return st; }
       keys[slot] = k;
       valid[slot] = true;
@@ -185,12 +191,14 @@ inline const DeviceInfo& device_info() {
 // rows hold K operand elements (K % 8 == 0 at two bytes, K % 16 == 0 at one byte), C rows N 16-bit elements. The scales
 // of a scaled variant are fp32 values in device memory: 4-byte aligned per tensor, 16-byte aligned vectors (M and N
 // values) rowwise, where the split-K reductions read the column scales as float4. Block scales: `a` 16-byte aligned (one
-// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned.
+// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned. Batched launches: batches >= 1 matrices,
+// whose tiles (`tiles` per matrix) number at most INT_MAX in all, and row counts `masked_m` (optional) 4-byte aligned.
 inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K,
-                    int ld_a = 0) {
+                    int ld_a = 0, int batches = 1, long long tiles = 1, const int* masked_m = nullptr) {
   const GemmTypeTraits& t = traits(type);
   if (!A || !Bt || !C || (t.scaled && (!scales.a || !scales.b))) return kNullPointer;
-  if (M <= 0 || N <= 0 || K <= 0) return kBadShape;
+  if (M <= 0 || N <= 0 || K <= 0 || batches < 1 || batches * tiles > 0x7fffffffLL) return kBadShape;
+  if (reinterpret_cast<uintptr_t>(masked_m) & 3) return kBadAlignment;
   if (K % (16 / elem_bytes(t.operand))) return t.e4m3() ? kBadFp8K : kBadAlignment;
   if (N % 8) return kBadAlignment;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
@@ -422,6 +430,8 @@ struct LaunchArgs {
   uint64_t hint_a, hint_b;
   Scales scales;
   int ld_a;             // block scales: the row stride of scales.a
+  int batches;          // batched kernels: the batch count ...
+  const int* masked_m;  // ... and the row counts per batch (null: dense)
   cudaStream_t stream;
 };
 
@@ -479,14 +489,17 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   cfg.attrs = attr;
   cfg.numAttrs = na;
   const int aux = block_scaled<Cfg>() ? a.ld_a : a.plan.sk_tiles;   // the kernel's aux_arg
+  // batched kernels (plain only) take the batch count as splits_arg and the row counts as splitk_ctr
+  const int splits_arg = batched<Cfg>() ? a.batches : a.plan.splits;
+  unsigned* ctr = batched<Cfg>() ? reinterpret_cast<unsigned*>(const_cast<int*>(a.masked_m)) : a.ctr;
   cudaError_t e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                                     a.plan.splits, aux, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
+                                     splits_arg, aux, a.ws, ctr, a.c, a.hint_a, a.hint_b, a.scales);
   if (e != cudaSuccess && coop && pdl && e != cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
     coop_pdl_ok = false;               // the pair of attributes is not accepted here: cooperative only, from now on
     cfg.numAttrs = na - 1;
     e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                           a.plan.splits, aux, a.ws, a.ctr, a.c, a.hint_a, a.hint_b, a.scales);
+                           splits_arg, aux, a.ws, ctr, a.c, a.hint_a, a.hint_b, a.scales);
   }
   return e == cudaSuccess ? kOk : int(e);
 }
@@ -560,6 +573,60 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
     case kPlain:
       break;
   }
+  return launch_mode<Cfg, kPlain>(di, a);
+}
+
+// Tiles (cluster blocks) of one M x N matrix of a batched launch.
+template <class Cfg>
+constexpr long long batch_tiles(int M, int N) {
+  return (long long)((M + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M)) *
+         ((N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N));
+}
+
+// The schedule of a batched launch: plain (there is no other for this variant, so it needs no scratch and is always
+// safe to capture in a graph), workers bounded by the dense tile list. With row counts the kernel's list is shorter,
+// and the workers without a tile leave at once.
+template <class Cfg, class ResidentClusters>
+Plan batched_plan(int batches, int M, int N, int K, int max_workers, ResidentClusters&& resident_clusters) {
+  Plan p{};
+  p.mode = kPlain;
+  p.splits = 1;
+  p.num_tiles = int(batches * batch_tiles<Cfg>(M, N));   // validate() bounds it
+  p.nkb = (K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
+  if (Cfg::CLUSTER_CTAS > 2) max_workers = std::min(max_workers, resident_clusters());
+  p.workers = std::min(std::max(max_workers, 1), p.num_tiles);
+  return p;
+}
+
+// C[b] = A[b] Bt[b]^T for b < batches, A [batches, M, K], Bt [batches, N, K], C [batches, M, N], all contiguous;
+// masked_m (device memory, optional): only rows [0, clamp(masked_m[b], 0, M)) of C[b] are computed, and no 16-row
+// store box starting at or past that count is written. No L2 eviction hints: which operand is re-read depends on the
+// batch as much as on the shapes.
+template <class Cfg>
+int launch_batched(const void* A, const void* Bt, void* C, const int* masked_m, int batches, int M, int N, int K,
+                   cudaStream_t stream, int group_m = 0, int max_ctas = 0) {
+  static_assert(batched<Cfg>(), "a Batched<> configuration");
+  constexpr GemmType kType = gemm_type<Cfg>();
+  int st = validate(kType, A, Bt, C, Scales{nullptr, nullptr}, M, N, K, 0, batches, batch_tiles<Cfg>(M, N), masked_m);
+  if (st != kOk) return st;
+  const DeviceInfo& di = device_info();
+  if (di.cc_major != 9) return kNotHopper;
+
+  LaunchArgs a{};
+  MapCache& cache = map_cache();
+  const Elem elem = traits(kType).operand;
+  if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem, batches)) != kOk) return st;
+  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, batches)) != kOk) return st;
+  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, elem, batches)) != kOk) return st;
+  const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
+  a.plan = batched_plan<Cfg>(batches, M, N, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
+  a.M = M; a.N = N; a.K = K;
+  a.group_m = group_m > 0 ? group_m : (Cfg::CTA_GROUP == 2 ? 8 : 16);
+  a.c = static_cast<__half*>(C);
+  a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
+  a.batches = batches;
+  a.masked_m = masked_m;
+  a.stream = stream;
   return launch_mode<Cfg, kPlain>(di, a);
 }
 

@@ -14,6 +14,7 @@
 //                   never wait on anybody) and writes C. See streamk_* in hgemm_sm90.cuh.
 #pragma once
 #include <cuda_runtime.h>
+#include <type_traits>
 
 namespace b200 {
 
@@ -91,6 +92,70 @@ struct WorkIter {
     }
     return false;
   }
+};
+
+// Batched launches (C[b] = A[b] Bt[b]^T for b < num_batches, plain schedule): one flat list of tiles, batch 0's first,
+// each batch's own tiles in the grouped rasterisation of tile_coord. With per-batch row counts (`counts`, the masked
+// form) batch b holds only the cluster blocks that start below clamp(counts[b], 0, M), so the list holds only tiles
+// with work in them and the persistent workers stay balanced. Every role builds its own cursor, sums the list
+// (total()), and then locates its tiles, whose indices only increase, so the cursor only moves forward: no shared
+// memory and no bound on the batch count. The host walks the same code over a host copy of the counts.
+struct BatchTile {
+  int batch;
+  int rows;        // valid rows of the batch: stores of boxes that start at or past them are skipped
+  TileCoord tc;    // cluster block inside the batch
+};
+
+struct BatchCursor {
+  const int* counts;   // valid rows per batch, clamped to [0, M]; null: every batch has M
+  int num_batches, M, block_rows, n_blocks, group_m;
+  int batch, first, m_blocks;   // the current batch: its tiles are [first, first + m_blocks * n_blocks)
+
+  __host__ __device__ BatchCursor(const int* counts_, int num_batches_, int M_, int block_rows_, int n_blocks_,
+                                  int group_m_)
+      : counts(counts_), num_batches(num_batches_), M(M_), block_rows(block_rows_), n_blocks(n_blocks_),
+        group_m(group_m_), batch(0), first(0), m_blocks(blocks_of(0)) {}
+
+  __host__ __device__ __forceinline__ int rows_of(int b) const {
+    if (!counts) return M;
+    const int r = counts[b];
+    return r < 0 ? 0 : r < M ? r : M;
+  }
+  __host__ __device__ __forceinline__ int blocks_of(int b) const {
+    return b < num_batches ? (rows_of(b) + block_rows - 1) / block_rows : 0;
+  }
+  // the length of the list
+  __host__ __device__ __forceinline__ int total() const {
+    if (!counts) return num_batches * m_blocks * n_blocks;
+    int blocks = 0;
+    for (int b = 0; b < num_batches; ++b) blocks += blocks_of(b);
+    return blocks * n_blocks;
+  }
+  // tile t < total() of the list; t must not be smaller than at the previous call
+  __host__ __device__ __forceinline__ BatchTile locate(int t) {
+    if (!counts) {   // every batch has the same tiles
+      const int per = m_blocks * n_blocks;
+      batch = t / per;
+      first = batch * per;
+    } else {
+      while (t >= first + m_blocks * n_blocks) {
+        first += m_blocks * n_blocks;
+        m_blocks = blocks_of(++batch);
+      }
+    }
+    BatchTile r;
+    r.batch = batch;
+    r.rows = rows_of(batch);
+    r.tc = tile_coord(t - first, m_blocks, n_blocks, group_m);
+    return r;
+  }
+};
+
+// What the kernels of the other variants hold in place of a BatchCursor: nothing.
+struct NoBatches {
+  __host__ __device__ NoBatches(const int*, int, int, int, int, int) {}
+  __host__ __device__ int total() const { return 0; }
+  __host__ __device__ BatchTile locate(int) { return BatchTile{}; }
 };
 
 // Owner side of a stream-K tile: the unit (tile, 0, kb1 < nkb) of worker w is completed by the first units of

@@ -147,6 +147,24 @@ struct BlockScaledFlag<Cfg, decltype(void(Cfg::BLOCK_SCALED))> { static constexp
 template <class Cfg>
 __host__ __device__ constexpr bool block_scaled() { return BlockScaledFlag<Cfg>::value; }
 
+// Batched 16-bit GEMM, C[b] = A[b] Bt[b]^T (libb200_batched.so): A, Bt and C are 3-D tensor maps whose third
+// coordinate is the batch, so a tile's loads are zero-filled and its stores clipped at its own matrix's edge, and a
+// cluster block never crosses a batch (multicast is kept). The flat tile list of BatchCursor (hgemm_schedule.cuh),
+// plain schedule only. A plain launch reads neither splits_arg nor splitk_ctr, so these carry the batch count and the
+// optional per-batch row counts (int32, device memory, read after the grid dependency wait). A wrapper, like
+// BlockScaled<>, so that the other kernels and their names stay as they are.
+template <class Base>
+struct Batched : Base {
+  static constexpr bool BATCHED = true;
+  static_assert(!Base::E4M3, "batched: 16-bit operands");
+};
+template <class Cfg, class = void>
+struct BatchedFlag { static constexpr bool value = false; };
+template <class Cfg>
+struct BatchedFlag<Cfg, decltype(void(Cfg::BATCHED))> { static constexpr bool value = Cfg::BATCHED; };
+template <class Cfg>
+__host__ __device__ constexpr bool batched() { return BatchedFlag<Cfg>::value; }
+
 // Scales of an e4m3 launch, in device memory (null for the 16-bit operand types). Per tensor: one fp32 value each.
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
 // 16-byte aligned; C[m,n] = RN_out(fp32(fp32(acc * b[n]) * a[m])). The granularity is a run-time property of the
@@ -216,7 +234,7 @@ __device__ __forceinline__ uint32_t acc_packed(const Reg (&d)[NR], int p) {
 template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chunk, uint32_t epi_buf, int lane,
                                                      const CUtensorMap* tmap_c, int col0, int row0, int M, int N,
-                                                     const RowwiseEpi* rw = nullptr) {
+                                                     const RowwiseEpi* rw = nullptr, int batch = 0) {
   using namespace ptx;
   constexpr int EN = Cfg::EPI_N;
   constexpr int PER_CHUNK = EN / 4;   // packed pairs of one chunk per thread
@@ -253,8 +271,10 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
   fence_proxy_async_smem();
   __syncwarp();
   if (lane == 0) {
-    if (row0 < M && col0 < N)   // rows/cols past the edge are clipped by the tensor map
-      tma_store_2d(tmap_c, epi_buf, col0, row0);
+    if (row0 < M && col0 < N) {   // rows/cols past the edge are clipped by the tensor map
+      if constexpr (batched<Cfg>()) tma_store_3d(tmap_c, epi_buf, col0, row0, batch);
+      else tma_store_2d(tmap_c, epi_buf, col0, row0);
+    }
     tma_store_commit();
   }
 }
@@ -490,12 +510,14 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
                 const __grid_constant__ CUtensorMap tmap_b,   // Bt [N,K]  box {BLOCK_K, B_BOX_ROWS}
                 const __grid_constant__ CUtensorMap tmap_c,   // C  [M,N]  box {EPI_N, EPI_ROWS}
                 int M, int N, int K, int group_m,
-                int splits_arg,                   // split-K factor (modes kWorkspaceSplitK / kClusterSplitK: one unit per CTA)
+                int splits_arg,                   // split-K factor (modes kWorkspaceSplitK / kClusterSplitK: one unit per CTA);
+                                                  // batched kernels (plain only): the batch count
                 int aux_arg,                      // mode kStreamK: sk_tiles, the first tiles, cut along K across all
                                                   // workers; block-scaled kernels (no stream-K): ld_a of scales.a
                 float* __restrict__ splitk_ws,    // [units][128][BN] fp32 partial tiles (workspace split-K) / stream-K slots
                 unsigned* __restrict__ splitk_ctr,   // [2][kMaxSplitTiles] split-K arrive / done counters, then the
-                                                     // stream-K flags; all zero between launches
+                                                     // stream-K flags; all zero between launches. Batched kernels:
+                                                     // the int32 row counts per batch, or null (dense)
                 __half* __restrict__ c_raw,       // C base pointer, used by the split-K reductions' direct stores
                 uint64_t hint_a, uint64_t hint_b, // L2 eviction priority of the A / B loads (ptx::kL2Evict*)
                 Scales scales                     /* e4m3: the per-tensor scales (not read by the 16-bit kernels) */) {
@@ -526,6 +548,12 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   static_assert(!kBlock || KMODE == kPlain || KMODE == kClusterSplitK, "block scales: plain and cluster split-K only");
   [[maybe_unused]] const int ld_a = kBlock ? aux_arg : 0;
   [[maybe_unused]] const uint32_t smem_scales = smem_bar + Cfg::BAR_BYTES;   // block scales: [STAGES] scale stages
+  constexpr bool kBatched = batched<Cfg>();
+  static_assert(!kBatched || KMODE == kPlain, "batched: plain schedule only");
+  [[maybe_unused]] const int num_batches = kBatched ? splits_arg : 1;
+  [[maybe_unused]] const int* masked_m = kBatched ? reinterpret_cast<const int*>(splitk_ctr) : nullptr;
+  // the tile list of a batched launch; an empty stand-in for the other kernels, so that their code is as it was
+  using Cursor = std::conditional_t<kBatched, BatchCursor, NoBatches>;
 
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x) >> 5, 0);
   const int lane = threadIdx.x & 31;
@@ -587,10 +615,14 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       const uint32_t a_slice = uint32_t(cn) * (Cfg::A_BOX_ROWS * kBlockK * 2);
       const uint32_t b_slice = uint32_t(mi) * (Cfg::B_BOX_ROWS * kBlockK * 2);
       int stage = 0; uint32_t phase = 0;
-      WorkIter work(worker, num_workers, num_tiles, num_k_blocks, splits, sk_tiles);
+      // batched: the list of (batch, cluster block) tiles, summed over the row counts (read after the dependency wait)
+      [[maybe_unused]] Cursor batches(masked_m, num_batches, M, Cfg::CTA_M * EM, num_n_blocks, group_m);
+      WorkIter work(worker, num_workers, kBatched ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
       WorkUnit u;
       while (work.next(u)) {
-        const TileCoord tc = tile_coord(u.tile, num_m_blocks, num_n_blocks, group_m);
+        [[maybe_unused]] BatchTile bt{0, M, TileCoord{0, 0}};
+        if constexpr (kBatched) bt = batches.locate(u.tile);
+        const TileCoord tc = kBatched ? bt.tc : tile_coord(u.tile, num_m_blocks, num_n_blocks, group_m);
         const int m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M + cn * Cfg::A_BOX_ROWS;
         const int n0 = (tc.n_blk * CN + cn) * BN + mi * Cfg::B_BOX_ROWS;
         // block scales: this CTA's own rows of A's scales (never multicast; none past ld_a, so a padding CTA loads
@@ -620,10 +652,18 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
             }
             const uint32_t dst_a = smem_a + stage * Cfg::A_STAGE_BYTES + a_slice;
             const uint32_t dst_b = smem_b + stage * Cfg::B_STAGE_BYTES + b_slice;
+            if constexpr (kBatched) {
+              const int b = bt.batch;
+              if constexpr (CN > 1) tma_load_3d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, b, mask_a, hint_a);
+              else tma_load_3d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, b, hint_a);
+              if constexpr (EM > 1) tma_load_3d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, b, mask_b, hint_b);
+              else tma_load_3d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, b, hint_b);
+            } else {
             if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, mask_a, hint_a);
             else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, hint_a);
             if constexpr (EM > 1) tma_load_2d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, mask_b, hint_b);
             else tma_load_2d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, hint_b);
+            }
           }
           __syncwarp();
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -673,7 +713,8 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       }
     };
     int stage = 0; uint32_t phase = 0;
-    WorkIter work(worker, num_workers, num_tiles, num_k_blocks, splits, sk_tiles);
+    [[maybe_unused]] Cursor batches(masked_m, num_batches, M, Cfg::CTA_M * EM, num_n_blocks, group_m);
+    WorkIter work(worker, num_workers, kBatched ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
     WorkUnit u;
     while (work.next(u)) {
       if constexpr (kBlock) {
@@ -747,7 +788,9 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
 
       // ---- epilogue of the unit
       const int tile = u.tile;
-      const TileCoord tc = tile_coord(tile, num_m_blocks, num_n_blocks, group_m);
+      [[maybe_unused]] BatchTile bt{0, M, TileCoord{0, 0}};
+      if constexpr (kBatched) bt = batches.locate(tile);   // its boxes are stored only where they start below bt.rows
+      const TileCoord tc = kBatched ? bt.tc : tile_coord(tile, num_m_blocks, num_n_blocks, group_m);
       const int m_cta = (tc.m_blk * EM + mi) * Cfg::CTA_M;
       const int n0 = (tc.n_blk * CN + cn) * BN;
       [[maybe_unused]] uint4* ws4 = reinterpret_cast<uint4*>(splitk_ws);
@@ -801,7 +844,8 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
           const int row0 = m_cta + (wg * MR + r) * 64 + wq * 16;
 #pragma unroll
           for (int j = 0; j < Cfg::EPI_CHUNKS; ++j)
-            epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, row0, M, N);
+            epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, row0, kBatched ? bt.rows : M,
+                                      N, nullptr, bt.batch);
         }
       }
     }

@@ -130,6 +130,25 @@ __device__ __forceinline__ void tma_load_2d_mcast_hint(uint32_t smem_dst, const 
       : "memory");
 }
 
+// 3-D versions for batched operands: coordinate c2 is the matrix of the batch (box depth 1), so TMA clips and zero-fills
+// rows at each matrix's own edge instead of reading into the next one
+__device__ __forceinline__ void tma_load_3d_hint(uint32_t smem_dst, const void* tmap, uint32_t bar,
+                                                 int32_t c0, int32_t c1, int32_t c2, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_3d_mcast_hint(uint32_t smem_dst, const void* tmap, uint32_t bar,
+                                                       int32_t c0, int32_t c1, int32_t c2, uint16_t mask, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6, %7;"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(mask), "l"(hint)
+      : "memory");
+}
+
 // 1-D bulk copy global -> this CTA's smem (bytes % 16 == 0, both addresses 16-byte aligned)
 __device__ __forceinline__ void bulk_load_1d(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -139,6 +158,11 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t smem_dst, const void* gsrc
 __device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1, int32_t c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() {

@@ -8,6 +8,11 @@ the nearest grid shape — so deployment is a plain operator:
 * ``torch.ops.cuda_l2_b200.hgemm(a, b_kmajor, acc)``: ``a`` [M,K] times B given K-major as ``b_kmajor`` [N,K]
   (exactly the layout of an ``nn.Linear`` weight: ``[out_features, in_features]``), returns [M,N]. fp16 or bf16
   operands (bf16 always accumulates in fp32); ``acc`` = "fp32" | "fp16".
+* ``torch.ops.cuda_l2_b200.hgemm_batched(a, b_kmajor, acc, masked_m=None)``: ``a`` [B,M,K] times ``b_kmajor``
+  [B,N,K] per batch, returns [B,M,N] — ``torch.bmm(a, b_kmajor.transpose(1, 2))`` in one launch (per-head attention
+  products, per-expert projections). ``masked_m``, an int32 CUDA tensor [B] read by the kernel (no host
+  synchronisation), limits batch b to its first ``masked_m[b]`` rows: the layout of an MoE layer's experts, whose token
+  counts live on the GPU. Inference only in that form; the dense form has a gradient.
 * :class:`B200Linear`: ``y = x @ W^T (+ b)`` for any leading dimensions; :func:`replace_linear_modules` swaps the
   eligible ``nn.Linear`` layers of a model in place.
 * ``torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)``: ``float8_e4m3fn`` operands in the same
@@ -85,6 +90,70 @@ torch.library.register_autograd(f"{_LIB}::hgemm", _hgemm_backward, setup_context
 def hgemm(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
     """``a`` [M,K] @ ``b_kmajor`` [N,K]^T -> [M,N] through the H100 kernel (see the module docstring)."""
     return torch.ops.cuda_l2_b200.hgemm(a, b_kmajor, acc)
+
+
+# ------------------------------------------------------------------------------------------ batched (libb200_batched.so)
+torch.library.define(f"{_LIB}::hgemm_batched",
+                     "(Tensor a, Tensor b_kmajor, str acc='fp32', Tensor? masked_m=None) -> Tensor")
+
+
+@torch.library.impl(f"{_LIB}::hgemm_batched", "CUDA")
+def _hgemm_batched_cuda(a, b_kmajor, acc="fp32", masked_m=None):
+    bsz, m, n, _ = capi.check_batched_operands(a, b_kmajor, acc, masked_m)
+    a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
+    c = torch.empty((bsz, m, n), dtype=a.dtype, device=a.device)
+    if bsz == 0 or m == 0:
+        return c
+    if masked_m is not None:
+        masked_m = masked_m.contiguous()
+    with torch.cuda.device(a.device):
+        capi.gemm_batched(a, b_kmajor, c, acc, masked_m=masked_m, stream=torch.cuda.current_stream(a.device).cuda_stream)
+    return c
+
+
+@torch.library.impl(f"{_LIB}::hgemm_batched", "CPU")
+def _hgemm_batched_cpu(a, b_kmajor, acc="fp32", masked_m=None):
+    raise capi.B200HgemmError("cuda_l2_b200::hgemm_batched has no CPU implementation (and no fallback): move the tensors "
+                              "to an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::hgemm_batched")
+def _hgemm_batched_fake(a, b_kmajor, acc="fp32", masked_m=None):
+    bsz, m, n, _ = capi.check_batched_operands(a, b_kmajor, acc, masked_m)
+    return a.new_empty((bsz, m, n))
+
+
+def _hgemm_batched_backward(ctx, grad_c):
+    if ctx.masked:
+        raise capi.B200HgemmError("cuda_l2_b200::hgemm_batched with masked_m is inference only: it has no gradient")
+    a, b_kmajor = ctx.saved_tensors
+    grad_a = grad_b = None
+    g = grad_c.contiguous()
+    # per batch, as _hgemm_backward: dA = dC Bt (B operand Bt^T, K-major in N), dBt = dC^T A (reduction over M)
+    if ctx.needs_input_grad[0]:
+        grad_a = torch.ops.cuda_l2_b200.hgemm_batched(g, b_kmajor.transpose(1, 2).contiguous(), "fp32")
+    if ctx.needs_input_grad[1]:
+        grad_b = torch.ops.cuda_l2_b200.hgemm_batched(g.transpose(1, 2).contiguous(), a.transpose(1, 2).contiguous(),
+                                                      "fp32")
+    return grad_a, grad_b, None, None
+
+
+def _hgemm_batched_setup_context(ctx, inputs, output):
+    a, b_kmajor, _, masked_m = inputs
+    ctx.masked = masked_m is not None
+    ctx.save_for_backward(a, b_kmajor)
+
+
+torch.library.register_autograd(f"{_LIB}::hgemm_batched", _hgemm_batched_backward,
+                                setup_context=_hgemm_batched_setup_context)
+
+
+def hgemm_batched(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32",
+                  masked_m: torch.Tensor | None = None) -> torch.Tensor:
+    """``a`` [B,M,K] @ ``b_kmajor`` [B,N,K]^T per batch -> [B,M,N] (``torch.bmm(a, b_kmajor.transpose(1, 2))``) through
+    the H100 kernel (see the module docstring). ``masked_m``: optional int32 CUDA tensor [B]; only rows
+    [0, clamp(masked_m[b], 0, M)) of batch b are computed, the rest of the result is unspecified."""
+    return torch.ops.cuda_l2_b200.hgemm_batched(a, b_kmajor, acc, masked_m)
 
 
 def linear_supported(in_features: int, out_features: int, dtype: torch.dtype) -> bool:
@@ -346,5 +415,5 @@ class B200Fp8Linear(nn.Module):
                 f"out_dtype={self.out_dtype}, granularity={self.granularity}")
 
 
-__all__ = ["hgemm", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
+__all__ = ["hgemm", "hgemm_batched", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear"]
