@@ -5,6 +5,7 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
 * ``libb200_hgemm.so``  — the C-ABI product library (include/b200_hgemm.h)
 * ``libb200_fp8block.so`` — the block-scaled FP8 GEMM (include/b200_fp8_block.h)
 * ``libb200_batched.so`` — the batched fp16 / bf16 GEMM (include/b200_batched.h)
+* ``libb200_grouped.so`` — the grouped fp16 / bf16 GEMM over contiguous row groups (include/b200_grouped.h)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -114,6 +115,30 @@ def build_batched(verbose: bool = False, force: bool = False) -> Path:
     return out
 
 
+GROUPED_VARIANTS = BATCHED_VARIANTS
+
+
+def build_grouped(verbose: bool = False, force: bool = False) -> Path:
+    """The grouped 16-bit kernels over contiguous row groups: a library of their own, so that the device code of
+    libb200_hgemm.so and libb200_batched.so is unaffected. One source, compiled once per data type in parallel (31
+    kernels each), then linked."""
+    LIB_DIR.mkdir(exist_ok=True)
+    out = LIB_DIR / "libb200_grouped.so"
+    src = CSRC / "b200_grouped_capi.cu"
+    if force or _stale(out, [src] + _headers()):
+        objs = [LIB_DIR / f"b200_grouped_{v}.o" for v in GROUPED_VARIANTS]
+        from concurrent.futures import ThreadPoolExecutor
+        with ThreadPoolExecutor(len(objs)) as pool:
+            for f in [pool.submit(_run, [nvcc_path(), *ARCH_FLAGS, *COMMON, f"-DB200_GROUPED_VARIANT={v}", "-c", "-o",
+                                         str(obj), str(src)], verbose)
+                      for v, obj in zip(GROUPED_VARIANTS, objs)]:
+                f.result()
+        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs)], verbose)
+        for obj in objs:
+            obj.unlink()
+    return out
+
+
 def build_baselines(verbose: bool = False, force: bool = False) -> Path:
     LIB_DIR.mkdir(exist_ok=True)
     out = LIB_DIR / "libb200_baselines.so"
@@ -137,10 +162,12 @@ def build_dev_check(verbose: bool = False, force: bool = False) -> Path:
 
 def build_all(verbose: bool = False, force: bool = False) -> dict[str, Path]:
     from concurrent.futures import ThreadPoolExecutor
-    with ThreadPoolExecutor(3) as pool:   # the block-scaled and batched libraries compile next to the product library
+    with ThreadPoolExecutor(4) as pool:   # the block-scaled, batched and grouped libraries compile next to the product library
         block = pool.submit(build_fp8block, verbose, force)
         batched = pool.submit(build_batched, verbose, force)
-        out = {"capi": build_capi(verbose, force), "fp8block": block.result(), "batched": batched.result()}
+        grouped = pool.submit(build_grouped, verbose, force)
+        out = {"capi": build_capi(verbose, force), "fp8block": block.result(), "batched": batched.result(),
+               "grouped": grouped.result()}
     if (CSRC / "b200_baselines_capi.cu").exists():
         out["baselines"] = build_baselines(verbose, force)
     out["dev_check"] = build_dev_check(verbose, force)

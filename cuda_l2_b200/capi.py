@@ -17,6 +17,7 @@ _hgemm = None
 _baselines = None
 _fp8block = None
 _batched = None
+_grouped = None
 
 ACC_BITS = {"fp32": 32, "fp16": 16, 32: 32, 16: 16}
 
@@ -115,6 +116,27 @@ def batched_lib() -> ctypes.CDLL:
     return _batched
 
 
+def grouped_lib() -> ctypes.CDLL:
+    """libb200_grouped.so: the grouped fp16 / bf16 GEMM over contiguous row groups (include/b200_grouped.h)."""
+    global _grouped
+    if _grouped is None:
+        lib = _load("libb200_grouped.so")
+        vp, i, ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
+        lib.b200_grouped_gemm.argtypes = [i, vp, vp, vp, vp, i, i, i, i, vp]
+        lib.b200_grouped_gemm.restype = i
+        lib.b200_grouped_gemm_run_config.argtypes = [i, i, vp, vp, vp, vp, i, i, i, i, i, i, vp]
+        lib.b200_grouped_gemm_run_config.restype = i
+        lib.b200_grouped_select.argtypes = [i, i, i, i, i, ip, ip]
+        lib.b200_grouped_select.restype = i
+        lib.b200_grouped_schedule_units.argtypes = [i, i, i, i, i, ip, i, i, ip, i, ip]
+        lib.b200_grouped_schedule_units.restype = i
+        lib.b200_grouped_launch_count.restype = ctypes.c_ulonglong
+        lib.b200_grouped_strerror.argtypes = [i]
+        lib.b200_grouped_strerror.restype = ctypes.c_char_p
+        _grouped = lib
+    return _grouped
+
+
 def baselines_lib() -> ctypes.CDLL:
     global _baselines
     if _baselines is None:
@@ -149,6 +171,10 @@ def exported_symbols() -> dict[str, list[str]]:
         "libb200_batched.so": [
             "b200_batched_gemm", "b200_batched_gemm_run_config", "b200_batched_select", "b200_batched_schedule_units",
             "b200_batched_launch_count", "b200_batched_strerror",
+        ],
+        "libb200_grouped.so": [
+            "b200_grouped_gemm", "b200_grouped_gemm_run_config", "b200_grouped_select", "b200_grouped_schedule_units",
+            "b200_grouped_launch_count", "b200_grouped_strerror",
         ],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
@@ -484,6 +510,98 @@ def batched_schedule(config_id: int, b: int, m: int, n: int, k: int, masked_m=No
 
 def batched_launch_count() -> int:
     return int(batched_lib().b200_batched_launch_count())
+
+
+# ------------------------------------------------------------------------------------------ grouped (libb200_grouped.so)
+def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32") -> tuple[int, int, int, int]:
+    """(G, T, N, K) of the grouped product a[T,K] by b_kmajor[G,N,K] with the int32 group ends ``offs`` [G]
+    (``torch._grouped_mm(a, b_kmajor.transpose(-2, -1), offs=offs)``), by the rules of the 16-bit variant the dtype and
+    ``acc`` name (the 2-D rules, :meth:`GemmType.fits`). Checks shapes and dtypes only (meta tensors pass);
+    B200HgemmError otherwise."""
+    import torch
+
+    try:
+        (t, k), (g, n, k2) = a.shape, b_kmajor.shape
+    except ValueError:
+        raise B200HgemmError(f"a [T, K] and b_kmajor [G, N, K] expected, got {tuple(a.shape)} and "
+                             f"{tuple(b_kmajor.shape)}") from None
+    gt = gemm_type(a.dtype, a.dtype, acc) if b_kmajor.dtype == a.dtype else None
+    if gt is None or gt.scale is not None:
+        raise B200HgemmError(f"no grouped kernel for {a.dtype} x {b_kmajor.dtype} with acc={acc!r} (fp16 with fp32 or "
+                             "fp16 accumulation, bf16 with fp32)")
+    if k2 != k:
+        raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} "
+                             "(K-major: [G, N, K])")
+    if not gt.fits(n, k):
+        raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % {gt.k_align} == 0 (16-byte TMA strides), "
+                             f"got N={n}, K={k}")
+    if offs.dtype != torch.int32 or tuple(offs.shape) != (g,):
+        raise B200HgemmError(f"offs must be an int32 tensor of shape [{g}], got {offs.dtype} {tuple(offs.shape)}")
+    return g, t, n, k
+
+
+def gemm_grouped(a, b_kmajor, c, offs, acc: str | int = "fp32", config_id: int | None = None, group_m: int = 0,
+                 max_ctas: int = 0, stream: int | None = None) -> None:
+    """c[start_g:end_g] = a[start_g:end_g] @ b_kmajor[g]^T for every group g, fp16 (fp32 or fp16 accumulation) or bf16
+    operands, all contiguous CUDA tensors ([T,K], [G,N,K], [T,N]). ``offs``: an int32 CUDA tensor [G] of cumulative
+    group ends, read by the kernel when it runs (clamped as include/b200_grouped.h describes); rows of c at or past the
+    last group's end are not written. ``config_id`` pins one kernel configuration (tests), ``max_ctas`` caps the CTAs
+    (0: all SMs); default is the dispatcher."""
+    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("offs", offs)):
+        if not x.is_cuda or not x.is_contiguous():
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    g, t, n, k = check_grouped_operands(a, b_kmajor, offs, acc)
+    if c.dtype != a.dtype or tuple(c.shape) != (t, n):
+        raise B200HgemmError(f"c must be {a.dtype} [{t}, {n}], got {c.dtype} {tuple(c.shape)}")
+    lib = grouped_lib()
+    variant = batched_variant(a.dtype, acc)
+    if config_id is None:
+        st = lib.b200_grouped_gemm(variant, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), offs.data_ptr(), g, t, n, k,
+                                   stream)
+    else:
+        st = lib.b200_grouped_gemm_run_config(variant, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(),
+                                              offs.data_ptr(), g, t, n, k, group_m, max_ctas, stream)
+    if st != 0:
+        raise B200HgemmError(f"b200_grouped_gemm failed: status {st} ({lib.b200_grouped_strerror(st).decode()})")
+
+
+def grouped_select(variant: int, g: int, t: int, n: int, k: int) -> tuple[int, int]:
+    """(config id, rasterisation group) the grouped dispatcher uses (b200_grouped_select)."""
+    cid, gm = ctypes.c_int(), ctypes.c_int()
+    st = grouped_lib().b200_grouped_select(variant, g, t, n, k, ctypes.byref(cid), ctypes.byref(gm))
+    if st != 0:
+        raise B200HgemmError(f"b200_grouped_select failed: status {st}")
+    return cid.value, gm.value
+
+
+def grouped_schedule(config_id: int, t: int, n: int, k: int, offs, num_sms: int = 132) -> dict:
+    """Host-side view of a grouped launch's schedule (no GPU needed; the kernel walks the same code), with the
+    launcher's default rasterisation. ``offs``: the cumulative group ends (a sequence of ints, G of them).
+
+    Returns ``{"workers": W, "units": [[(group, m_block, n_block), ...] per worker]}``; blocks are cluster blocks, and
+    m-blocks count from the group's first row."""
+    lib = grouped_lib()
+    g = len(offs)
+    ends = (ctypes.c_int * g)(*offs)
+    nw = ctypes.c_int()
+    cap = 256
+    buf = (ctypes.c_int * (3 * cap))()
+    st = lib.b200_grouped_schedule_units(config_id, g, t, n, k, ends, num_sms, 0, buf, cap, ctypes.byref(nw))
+    if st < 0:
+        raise B200HgemmError(f"b200_grouped_schedule_units failed: status {st}")
+    units = []
+    for w in range(nw.value):
+        cnt = lib.b200_grouped_schedule_units(config_id, g, t, n, k, ends, num_sms, w, buf, cap, None)
+        if cnt > cap:
+            cap = cnt
+            buf = (ctypes.c_int * (3 * cap))()
+            cnt = lib.b200_grouped_schedule_units(config_id, g, t, n, k, ends, num_sms, w, buf, cap, None)
+        units.append([(buf[3 * j], buf[3 * j + 1], buf[3 * j + 2]) for j in range(cnt)])
+    return {"workers": nw.value, "units": units}
+
+
+def grouped_launch_count() -> int:
+    return int(grouped_lib().b200_grouped_launch_count())
 
 
 def hgemm_config(a, b_col_major, c, config_id: int, acc: str | int = "fp32", group_m: int = 0, max_ctas: int = 0,

@@ -74,13 +74,8 @@ int run(int variant, int config_id, const void* A, const void* Bt, void* C, cons
   }
 }
 
-// The 2-D entry of (B * M, N, K) has about the batched problem's tile count; it is taken if its pair / cluster fits one
-// M x N matrix, and the 2-D choice for one matrix otherwise. A heuristic: no batched shape has been tuned.
 dispatch::Choice select(int variant, int B, int M, int N, int K) {
-  const GemmType T = GemmType(variant);
-  const int rows = int(std::min<long long>((long long)B * M, INT_MAX));
-  const dispatch::Choice ch = dispatch::select(T, rows, N, K);
-  return dispatch::usable(ch, M, N) ? ch : dispatch::select(T, M, N, K);
+  return dispatch::select_batched(GemmType(variant), B, M, N, K);
 }
 
 template <class Cfg>

@@ -193,6 +193,7 @@ inline const DeviceInfo& device_info() {
 // values) rowwise, where the split-K reductions read the column scales as float4. Block scales: `a` 16-byte aligned (one
 // bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned. Batched launches: batches >= 1 matrices,
 // whose tiles (`tiles` per matrix) number at most INT_MAX in all, and row counts `masked_m` (optional) 4-byte aligned.
+// Grouped launches (validate_grouped) pass their offsets as `masked_m` and the worst-case tile list as `tiles`.
 inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K,
                     int ld_a = 0, int batches = 1, long long tiles = 1, const int* masked_m = nullptr) {
   const GemmTypeTraits& t = traits(type);
@@ -431,7 +432,7 @@ struct LaunchArgs {
   Scales scales;
   int ld_a;             // block scales: the row stride of scales.a
   int batches;          // batched kernels: the batch count ...
-  const int* masked_m;  // ... and the row counts per batch (null: dense)
+  const int* masked_m;  // ... and the row counts per batch (null: dense); grouped kernels: G and the offsets
   cudaStream_t stream;
 };
 
@@ -489,9 +490,11 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   cfg.attrs = attr;
   cfg.numAttrs = na;
   const int aux = block_scaled<Cfg>() ? a.ld_a : a.plan.sk_tiles;   // the kernel's aux_arg
-  // batched kernels (plain only) take the batch count as splits_arg and the row counts as splitk_ctr
-  const int splits_arg = batched<Cfg>() ? a.batches : a.plan.splits;
-  unsigned* ctr = batched<Cfg>() ? reinterpret_cast<unsigned*>(const_cast<int*>(a.masked_m)) : a.ctr;
+  // batched kernels (plain only) take the batch count as splits_arg and the row counts as splitk_ctr; grouped kernels
+  // the group count and the offsets
+  constexpr bool kTileList = batched<Cfg>() || grouped<Cfg>();
+  const int splits_arg = kTileList ? a.batches : a.plan.splits;
+  unsigned* ctr = kTileList ? reinterpret_cast<unsigned*>(const_cast<int*>(a.masked_m)) : a.ctr;
   cudaError_t e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
                                      splits_arg, aux, a.ws, ctr, a.c, a.hint_a, a.hint_b, a.scales);
   if (e != cudaSuccess && coop && pdl && e != cudaErrorCooperativeLaunchTooLarge) {
@@ -626,6 +629,71 @@ int launch_batched(const void* A, const void* Bt, void* C, const int* masked_m, 
   a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
   a.batches = batches;
   a.masked_m = masked_m;
+  a.stream = stream;
+  return launch_mode<Cfg, kPlain>(di, a);
+}
+
+// The longest tile list a grouped launch over T rows and G groups can have: every group adds at most one partial
+// cluster row block to the ceil(T / block_rows) of the rows themselves.
+template <class Cfg>
+constexpr long long grouped_worst_tiles(int groups, int T, int N) {
+  return (((long long)T + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M) + groups) *
+         (((long long)N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N));
+}
+
+// The argument rules of a grouped launch: those of a 2-D [T, K] x [N, K] call (T == 0 is an empty problem and valid),
+// G >= 1 groups whose offsets (G int32 values, device memory) are non-null and 4-byte aligned, and a worst-case tile
+// list (`worst_tiles`, grouped_worst_tiles) of at most INT_MAX tiles.
+inline int validate_grouped(GemmType type, const void* A, const void* Bt, const void* C, const int* offs, int groups,
+                            int T, int N, int K, long long worst_tiles) {
+  if (!A || !Bt || !C || !offs) return kNullPointer;
+  if (T < 0 || groups < 1) return kBadShape;
+  return validate(type, A, Bt, C, Scales{nullptr, nullptr}, T > 0 ? T : 1, N, K, 0, 1, worst_tiles, offs);
+}
+
+// The schedule of a grouped launch: plain, like the batched one, with the workers bounded by the worst-case tile list
+// (the real one is only known on the device, where the workers without a tile leave at once).
+template <class Cfg, class ResidentClusters>
+Plan grouped_plan(int groups, int T, int N, int K, int max_workers, ResidentClusters&& resident_clusters) {
+  Plan p{};
+  p.mode = kPlain;
+  p.splits = 1;
+  p.num_tiles = int(grouped_worst_tiles<Cfg>(groups, T, N));   // validate_grouped() bounds it
+  p.nkb = (K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
+  if (Cfg::CLUSTER_CTAS > 2) max_workers = std::min(max_workers, resident_clusters());
+  p.workers = std::min(std::max(max_workers, 1), p.num_tiles);
+  return p;
+}
+
+// C[start_g : end_g] = A[start_g : end_g] Bt[g]^T for g < groups: A [T, K], Bt [groups, N, K], C [T, N], contiguous.
+// offs (device memory, read by the kernel only): the cumulative group ends, end_g = clamp(offs[g], start_g, T) with
+// start_0 = 0 and start_g = end_{g-1}. Every row of C below end_{groups-1} is written once, by its own group; no other
+// is written. T == 0 launches nothing. No L2 eviction hints, as for the batched launches.
+template <class Cfg>
+int launch_grouped(const void* A, const void* Bt, void* C, const int* offs, int groups, int T, int N, int K,
+                   cudaStream_t stream, int group_m = 0, int max_ctas = 0) {
+  static_assert(grouped<Cfg>(), "a Grouped<> configuration");
+  constexpr GemmType kType = gemm_type<Cfg>();
+  const long long worst = groups > 0 && T >= 0 ? grouped_worst_tiles<Cfg>(groups, T, N) : 1;
+  int st = validate_grouped(kType, A, Bt, C, offs, groups, T, N, K, worst);
+  if (st != kOk || T == 0) return st;
+  const DeviceInfo& di = device_info();
+  if (di.cc_major != 9) return kNotHopper;
+
+  LaunchArgs a{};
+  MapCache& cache = map_cache();
+  const Elem elem = traits(kType).operand;
+  if ((st = cache.get(A, T, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem)) != kOk) return st;
+  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, groups)) != kOk) return st;
+  if ((st = cache.get(C, T, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, elem)) != kOk) return st;
+  const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
+  a.plan = grouped_plan<Cfg>(groups, T, N, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
+  a.M = T; a.N = N; a.K = K;
+  a.group_m = group_m > 0 ? group_m : (Cfg::CTA_GROUP == 2 ? 8 : 16);
+  a.c = static_cast<__half*>(C);
+  a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
+  a.batches = groups;
+  a.masked_m = offs;
   a.stream = stream;
   return launch_mode<Cfg, kPlain>(di, a);
 }

@@ -151,6 +151,57 @@ struct BatchCursor {
   }
 };
 
+// Grouped launches (the contiguous MoE layout: C[start_g : end_g] = A[start_g : end_g] Bt[g]^T for g < num_groups,
+// plain schedule): group g owns rows [start_g, end_g) of A and C, with start_0 = 0, start_g = end_{g-1} and
+// end_g = clamp(offs[g], start_g, T), so decreasing, negative or too-large offsets give empty or shortened groups and
+// no group reaches past T. The list is BatchCursor's, over the cluster blocks of each group's own rows: group g holds
+// ceil((end_g - start_g) / block_rows) * n_blocks tiles in tile_coord's rasterisation. The same constructor and
+// interface, so the kernel walks either cursor with the same code; locate() returns the group as `batch` and its row
+// count as `rows`, and leaves the group's first row in `start`.
+struct GroupCursor {
+  const int* offs;   // cumulative ends of the groups (torch._grouped_mm's offs)
+  int num_groups, T, block_rows, n_blocks, group_m;
+  int group, first, m_blocks, start, end;   // the current group: rows [start, end), tiles [first, first + m_blocks * n_blocks)
+
+  __host__ __device__ GroupCursor(const int* offs_, int num_groups_, int T_, int block_rows_, int n_blocks_,
+                                  int group_m_)
+      : offs(offs_), num_groups(num_groups_), T(T_), block_rows(block_rows_), n_blocks(n_blocks_), group_m(group_m_),
+        group(0), first(0), start(0) {
+    end = end_of(0, 0);
+    m_blocks = (end - start + block_rows - 1) / block_rows;
+  }
+
+  __host__ __device__ __forceinline__ int end_of(int g, int s) const {
+    if (g >= num_groups) return s;
+    const int e = offs[g];
+    return e < s ? s : e < T ? e : T;
+  }
+  // the length of the list
+  __host__ __device__ __forceinline__ int total() const {
+    int blocks = 0, s = 0;
+    for (int g = 0; g < num_groups; ++g) {
+      const int e = end_of(g, s);
+      blocks += (e - s + block_rows - 1) / block_rows;
+      s = e;
+    }
+    return blocks * n_blocks;
+  }
+  // tile t < total() of the list; t must not be smaller than at the previous call
+  __host__ __device__ __forceinline__ BatchTile locate(int t) {
+    while (t >= first + m_blocks * n_blocks) {
+      first += m_blocks * n_blocks;
+      start = end;
+      end = end_of(++group, start);
+      m_blocks = (end - start + block_rows - 1) / block_rows;
+    }
+    BatchTile r;
+    r.batch = group;
+    r.rows = end - start;
+    r.tc = tile_coord(t - first, m_blocks, n_blocks, group_m);
+    return r;
+  }
+};
+
 // What the kernels of the other variants hold in place of a BatchCursor: nothing.
 struct NoBatches {
   __host__ __device__ NoBatches(const int*, int, int, int, int, int) {}

@@ -165,6 +165,25 @@ struct BatchedFlag<Cfg, decltype(void(Cfg::BATCHED))> { static constexpr bool va
 template <class Cfg>
 __host__ __device__ constexpr bool batched() { return BatchedFlag<Cfg>::value; }
 
+// Grouped 16-bit GEMM over contiguous row groups, C[start_g : end_g] = A[start_g : end_g] Bt[g]^T (the MoE prefill
+// layout, libb200_grouped.so): A [T, K] and C [T, N] are 2-D tensor maps, Bt [G, N, K] the batched 3-D map. The flat
+// tile list of GroupCursor (hgemm_schedule.cuh), plain schedule only; a cluster block never crosses a group, so
+// multicast is kept. splits_arg carries the group count and splitk_ctr the int32 offsets (device memory, read after
+// the grid dependency wait). A group starts at any row, so the rows of a box past the group's end belong to the next
+// group: they are multiplied but never stored. A 16-row store box wholly inside the group is a TMA store; one that
+// straddles the group's end stores only the group's rows, with 16-byte generic stores from the staging buffer.
+template <class Base>
+struct Grouped : Base {
+  static constexpr bool GROUPED = true;
+  static_assert(!Base::E4M3, "grouped: 16-bit operands");
+};
+template <class Cfg, class = void>
+struct GroupedFlag { static constexpr bool value = false; };
+template <class Cfg>
+struct GroupedFlag<Cfg, decltype(void(Cfg::GROUPED))> { static constexpr bool value = Cfg::GROUPED; };
+template <class Cfg>
+__host__ __device__ constexpr bool grouped() { return GroupedFlag<Cfg>::value; }
+
 // Scales of an e4m3 launch, in device memory (null for the 16-bit operand types). Per tensor: one fp32 value each.
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
 // 16-byte aligned; C[m,n] = RN_out(fp32(fp32(acc * b[n]) * a[m])). The granularity is a run-time property of the
@@ -226,7 +245,9 @@ __device__ __forceinline__ uint32_t acc_packed(const Reg (&d)[NR], int p) {
   else return d[p];   // fp16 accumulators are already the output format
 }
 
-// registers -> swizzled staging buffer -> TMA store of one EPI_ROWS x EPI_N chunk of this warp. With rowwise e4m3 scales
+// registers -> swizzled staging buffer -> TMA store of one EPI_ROWS x EPI_N chunk of this warp. Grouped kernels: M is
+// the end row of the tile's group, and a box that straddles it is copied out row by row instead (c_raw: C [., N]).
+// With rowwise e4m3 scales
 // (`rw` non-null) each fp32 pair is scaled by its column scales, then its row scale, right before the rounding. The
 // column scales of a chunk are loaded here, after the previous chunk's store wait, one float2 (one column pair) per
 // lane, and reach the lanes that need them by shuffle: two registers per thread instead of the chunk's 16, which the
@@ -234,7 +255,8 @@ __device__ __forceinline__ uint32_t acc_packed(const Reg (&d)[NR], int p) {
 template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chunk, uint32_t epi_buf, int lane,
                                                      const CUtensorMap* tmap_c, int col0, int row0, int M, int N,
-                                                     const RowwiseEpi* rw = nullptr, int batch = 0) {
+                                                     const RowwiseEpi* rw = nullptr, int batch = 0,
+                                                     __half* __restrict__ c_raw = nullptr) {
   using namespace ptx;
   constexpr int EN = Cfg::EPI_N;
   constexpr int PER_CHUNK = EN / 4;   // packed pairs of one chunk per thread
@@ -270,6 +292,24 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
   }
   fence_proxy_async_smem();
   __syncwarp();
+  if constexpr (grouped<Cfg>()) {
+    // A box that straddles the group's end (warp-uniform): the rows past it belong to the next group, which another
+    // CTA is storing, so only the rows below M leave, one 16-byte chunk per lane and step, read through the same
+    // swizzle. N % 8 == 0: a chunk is wholly inside or wholly outside the columns. A box at or past M stores nothing.
+    if (row0 + Cfg::EPI_ROWS > M) {
+      constexpr int CPR = EN * 2 / 16;   // 16-byte chunks per staged row
+#pragma unroll 1
+      for (int i = lane; i < Cfg::EPI_ROWS * CPR; i += 32) {
+        const int r = i / CPR, c = i % CPR;
+        if (row0 + r < M && col0 + 8 * c < N) {
+          uint32_t off = uint32_t(r * (EN * 2) + c * 16);
+          off ^= (EN == 64 ? ((off >> 7) & 7u) : ((off >> 7) & 3u)) << 4;
+          *reinterpret_cast<uint4*>(c_raw + size_t(row0 + r) * N + col0 + 8 * c) = ld_shared_v4_b32(epi_buf + off);
+        }
+      }
+      return;
+    }
+  }
   if (lane == 0) {
     if (row0 < M && col0 < N) {   // rows/cols past the edge are clipped by the tensor map
       if constexpr (batched<Cfg>()) tma_store_3d(tmap_c, epi_buf, col0, row0, batch);
@@ -511,13 +551,14 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
                 const __grid_constant__ CUtensorMap tmap_c,   // C  [M,N]  box {EPI_N, EPI_ROWS}
                 int M, int N, int K, int group_m,
                 int splits_arg,                   // split-K factor (modes kWorkspaceSplitK / kClusterSplitK: one unit per CTA);
-                                                  // batched kernels (plain only): the batch count
+                                                  // batched kernels (plain only): the batch count; grouped: G
                 int aux_arg,                      // mode kStreamK: sk_tiles, the first tiles, cut along K across all
                                                   // workers; block-scaled kernels (no stream-K): ld_a of scales.a
                 float* __restrict__ splitk_ws,    // [units][128][BN] fp32 partial tiles (workspace split-K) / stream-K slots
                 unsigned* __restrict__ splitk_ctr,   // [2][kMaxSplitTiles] split-K arrive / done counters, then the
                                                      // stream-K flags; all zero between launches. Batched kernels:
-                                                     // the int32 row counts per batch, or null (dense)
+                                                     // the int32 row counts per batch, or null (dense);
+                                                     // grouped: the G int32 offsets (cumulative group ends)
                 __half* __restrict__ c_raw,       // C base pointer, used by the split-K reductions' direct stores
                 uint64_t hint_a, uint64_t hint_b, // L2 eviction priority of the A / B loads (ptx::kL2Evict*)
                 Scales scales                     /* e4m3: the per-tensor scales (not read by the 16-bit kernels) */) {
@@ -549,11 +590,15 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   [[maybe_unused]] const int ld_a = kBlock ? aux_arg : 0;
   [[maybe_unused]] const uint32_t smem_scales = smem_bar + Cfg::BAR_BYTES;   // block scales: [STAGES] scale stages
   constexpr bool kBatched = batched<Cfg>();
-  static_assert(!kBatched || KMODE == kPlain, "batched: plain schedule only");
-  [[maybe_unused]] const int num_batches = kBatched ? splits_arg : 1;
-  [[maybe_unused]] const int* masked_m = kBatched ? reinterpret_cast<const int*>(splitk_ctr) : nullptr;
-  // the tile list of a batched launch; an empty stand-in for the other kernels, so that their code is as it was
-  using Cursor = std::conditional_t<kBatched, BatchCursor, NoBatches>;
+  constexpr bool kGrouped = grouped<Cfg>();
+  constexpr bool kTileList = kBatched || kGrouped;   // the schedule walks a cursor's flat tile list
+  static_assert(!kTileList || KMODE == kPlain, "batched / grouped: plain schedule only");
+  // grouped kernels: the group count and the offsets, in the same places (M is then T, the rows of A and C)
+  [[maybe_unused]] const int num_batches = kTileList ? splits_arg : 1;
+  [[maybe_unused]] const int* masked_m = kTileList ? reinterpret_cast<const int*>(splitk_ctr) : nullptr;
+  // the tile list of a batched or grouped launch; an empty stand-in for the other kernels, so that their code is as
+  // it was
+  using Cursor = std::conditional_t<kBatched, BatchCursor, std::conditional_t<kGrouped, GroupCursor, NoBatches>>;
 
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x) >> 5, 0);
   const int lane = threadIdx.x & 31;
@@ -617,12 +662,12 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       int stage = 0; uint32_t phase = 0;
       // batched: the list of (batch, cluster block) tiles, summed over the row counts (read after the dependency wait)
       [[maybe_unused]] Cursor batches(masked_m, num_batches, M, Cfg::CTA_M * EM, num_n_blocks, group_m);
-      WorkIter work(worker, num_workers, kBatched ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
+      WorkIter work(worker, num_workers, kTileList ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
       WorkUnit u;
       while (work.next(u)) {
         [[maybe_unused]] BatchTile bt{0, M, TileCoord{0, 0}};
-        if constexpr (kBatched) bt = batches.locate(u.tile);
-        const TileCoord tc = kBatched ? bt.tc : tile_coord(u.tile, num_m_blocks, num_n_blocks, group_m);
+        if constexpr (kTileList) bt = batches.locate(u.tile);
+        const TileCoord tc = kTileList ? bt.tc : tile_coord(u.tile, num_m_blocks, num_n_blocks, group_m);
         const int m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M + cn * Cfg::A_BOX_ROWS;
         const int n0 = (tc.n_blk * CN + cn) * BN + mi * Cfg::B_BOX_ROWS;
         // block scales: this CTA's own rows of A's scales (never multicast; none past ld_a, so a padding CTA loads
@@ -658,6 +703,12 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
               else tma_load_3d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, b, hint_a);
               if constexpr (EM > 1) tma_load_3d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, b, mask_b, hint_b);
               else tma_load_3d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, b, hint_b);
+            } else if constexpr (kGrouped) {   // A rows from the group's first row on (rows past T read as zero)
+              const int ma = batches.start + m0, g = bt.batch;
+              if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, ma, mask_a, hint_a);
+              else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, ma, hint_a);
+              if constexpr (EM > 1) tma_load_3d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, g, mask_b, hint_b);
+              else tma_load_3d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, g, hint_b);
             } else {
             if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, mask_a, hint_a);
             else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, hint_a);
@@ -714,7 +765,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
     };
     int stage = 0; uint32_t phase = 0;
     [[maybe_unused]] Cursor batches(masked_m, num_batches, M, Cfg::CTA_M * EM, num_n_blocks, group_m);
-    WorkIter work(worker, num_workers, kBatched ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
+    WorkIter work(worker, num_workers, kTileList ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
     WorkUnit u;
     while (work.next(u)) {
       if constexpr (kBlock) {
@@ -789,8 +840,8 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       // ---- epilogue of the unit
       const int tile = u.tile;
       [[maybe_unused]] BatchTile bt{0, M, TileCoord{0, 0}};
-      if constexpr (kBatched) bt = batches.locate(tile);   // its boxes are stored only where they start below bt.rows
-      const TileCoord tc = kBatched ? bt.tc : tile_coord(tile, num_m_blocks, num_n_blocks, group_m);
+      if constexpr (kTileList) bt = batches.locate(tile);   // its boxes are stored only where they start below bt.rows
+      const TileCoord tc = kTileList ? bt.tc : tile_coord(tile, num_m_blocks, num_n_blocks, group_m);
       const int m_cta = (tc.m_blk * EM + mi) * Cfg::CTA_M;
       const int n0 = (tc.n_blk * CN + cn) * BN;
       [[maybe_unused]] uint4* ws4 = reinterpret_cast<uint4*>(splitk_ws);
@@ -843,9 +894,14 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         for (int r = 0; r < MR; ++r) {
           const int row0 = m_cta + (wg * MR + r) * 64 + wq * 16;
 #pragma unroll
-          for (int j = 0; j < Cfg::EPI_CHUNKS; ++j)
-            epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, row0, kBatched ? bt.rows : M,
-                                      N, nullptr, bt.batch);
+          for (int j = 0; j < Cfg::EPI_CHUNKS; ++j) {
+            if constexpr (kGrouped)   // rows of C from the group's first row on, stored only below the group's end
+              epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, batches.start + row0,
+                                        batches.end, N, nullptr, 0, c_raw);
+            else
+              epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, row0,
+                                        kBatched ? bt.rows : M, N, nullptr, bt.batch);
+          }
         }
       }
     }

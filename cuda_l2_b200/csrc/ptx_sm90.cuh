@@ -255,6 +255,12 @@ __device__ __forceinline__ float4 ld_shared_v4f(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
   return v;
 }
+// 16 raw bytes (packed output elements of an epilogue staging buffer)
+__device__ __forceinline__ uint4 ld_shared_v4_b32(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
 __device__ __forceinline__ uint32_t pack_f16x2_rn(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);   // cvt.rn.f16x2.f32: one rounding per element
   return *reinterpret_cast<uint32_t*>(&h);

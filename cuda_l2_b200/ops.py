@@ -13,6 +13,10 @@ the nearest grid shape — so deployment is a plain operator:
   products, per-expert projections). ``masked_m``, an int32 CUDA tensor [B] read by the kernel (no host
   synchronisation), limits batch b to its first ``masked_m[b]`` rows: the layout of an MoE layer's experts, whose token
   counts live on the GPU. Inference only in that form; the dense form has a gradient.
+* ``torch.ops.cuda_l2_b200.hgemm_grouped(a, b_kmajor, offs, acc)``: ``a`` [T,K] whose rows are sorted into contiguous
+  groups, ``b_kmajor`` [G,N,K] one weight per group, ``offs`` the int32 cumulative group ends on the GPU; returns
+  [T,N] — ``torch._grouped_mm(a, b_kmajor.transpose(-2, -1), offs=offs)`` in one launch, the MoE prefill layout.
+  Inference only.
 * :class:`B200Linear`: ``y = x @ W^T (+ b)`` for any leading dimensions; :func:`replace_linear_modules` swaps the
   eligible ``nn.Linear`` layers of a model in place.
 * ``torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)``: ``float8_e4m3fn`` operands in the same
@@ -154,6 +158,50 @@ def hgemm_batched(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32",
     the H100 kernel (see the module docstring). ``masked_m``: optional int32 CUDA tensor [B]; only rows
     [0, clamp(masked_m[b], 0, M)) of batch b are computed, the rest of the result is unspecified."""
     return torch.ops.cuda_l2_b200.hgemm_batched(a, b_kmajor, acc, masked_m)
+
+
+# ------------------------------------------------------------------------------------------ grouped (libb200_grouped.so)
+torch.library.define(f"{_LIB}::hgemm_grouped", "(Tensor a, Tensor b_kmajor, Tensor offs, str acc='fp32') -> Tensor")
+
+
+@torch.library.impl(f"{_LIB}::hgemm_grouped", "CUDA")
+def _hgemm_grouped_cuda(a, b_kmajor, offs, acc="fp32"):
+    g, t, n, _ = capi.check_grouped_operands(a, b_kmajor, offs, acc)
+    a, b_kmajor, offs = a.contiguous(), b_kmajor.contiguous(), offs.contiguous()
+    c = torch.empty((t, n), dtype=a.dtype, device=a.device)
+    if g == 0 or t == 0:
+        return c
+    with torch.cuda.device(a.device):
+        capi.gemm_grouped(a, b_kmajor, c, offs, acc, stream=torch.cuda.current_stream(a.device).cuda_stream)
+    return c
+
+
+@torch.library.impl(f"{_LIB}::hgemm_grouped", "CPU")
+def _hgemm_grouped_cpu(a, b_kmajor, offs, acc="fp32"):
+    raise capi.B200HgemmError("cuda_l2_b200::hgemm_grouped has no CPU implementation (and no fallback): move the tensors "
+                              "to an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::hgemm_grouped")
+def _hgemm_grouped_fake(a, b_kmajor, offs, acc="fp32"):
+    _, t, n, _ = capi.check_grouped_operands(a, b_kmajor, offs, acc)
+    return a.new_empty((t, n))
+
+
+def _hgemm_grouped_no_backward(ctx, grad_c):
+    raise capi.B200HgemmError("cuda_l2_b200::hgemm_grouped is inference only: it has no gradient (the weight gradient is "
+                              "a grouped product over K, a different kernel)")
+
+
+torch.library.register_autograd(f"{_LIB}::hgemm_grouped", _hgemm_grouped_no_backward)
+
+
+def hgemm_grouped(a: torch.Tensor, b_kmajor: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
+    """``a`` [T,K] by ``b_kmajor`` [G,N,K] over contiguous row groups -> [T,N]: rows [offs[g-1], offs[g]) of the
+    result are those rows of ``a`` times ``b_kmajor[g]^T`` (``torch._grouped_mm(a, b_kmajor.transpose(-2, -1),
+    offs=offs)``), in one launch. ``offs``: int32 CUDA tensor [G] of cumulative group ends, read by the kernel (no host
+    synchronisation) and clamped to [previous end, T]. Rows at or past ``offs[-1]`` are unspecified. Inference only."""
+    return torch.ops.cuda_l2_b200.hgemm_grouped(a, b_kmajor, offs, acc)
 
 
 def linear_supported(in_features: int, out_features: int, dtype: torch.dtype) -> bool:
@@ -415,5 +463,5 @@ class B200Fp8Linear(nn.Module):
                 f"out_dtype={self.out_dtype}, granularity={self.granularity}")
 
 
-__all__ = ["hgemm", "hgemm_batched", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
+__all__ = ["hgemm", "hgemm_batched", "hgemm_grouped", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear"]
