@@ -63,23 +63,28 @@ def _headers() -> list[Path]:
     return sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.inc")) + sorted((REPO / "include").glob("*.h"))
 
 
-def build_capi(verbose: bool = False, force: bool = False) -> Path:
-    """The 16-bit kernels (b200_hgemm_capi.cu) and the e4m3 ones (b200_fp8_capi.cu) compile in parallel, then link
-    into one library."""
+def _compile_and_link(out: Path, objects: list[tuple[Path, list[str]]], verbose: bool, force: bool) -> Path:
+    """Compiles each (source, defines) object in parallel, then links them into the shared library ``out``."""
     LIB_DIR.mkdir(exist_ok=True)
-    out = LIB_DIR / "libb200_hgemm.so"
-    srcs = [CSRC / "b200_hgemm_capi.cu", CSRC / "b200_fp8_capi.cu"]
-    if force or _stale(out, srcs + _headers()):
-        objs = [LIB_DIR / (src.stem + ".o") for src in srcs]
+    if force or _stale(out, [src for src, _ in objects] + _headers()):
+        objs = [LIB_DIR / f"{out.stem}_{i}.o" for i in range(len(objects))]
         from concurrent.futures import ThreadPoolExecutor
-        with ThreadPoolExecutor(len(srcs)) as pool:
-            for f in [pool.submit(_run, [nvcc_path(), *ARCH_FLAGS, *COMMON, "-c", "-o", str(obj), str(src)], verbose)
-                      for src, obj in zip(srcs, objs)]:
+        with ThreadPoolExecutor(len(objects)) as pool:
+            for f in [pool.submit(_run, [nvcc_path(), *ARCH_FLAGS, *COMMON, *defines, "-c", "-o", str(obj), str(src)],
+                                  verbose)
+                      for (src, defines), obj in zip(objects, objs)]:
                 f.result()
         _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs)], verbose)
         for obj in objs:
             obj.unlink()
     return out
+
+
+def build_capi(verbose: bool = False, force: bool = False) -> Path:
+    """The 16-bit kernels (b200_hgemm_capi.cu) and the e4m3 ones (b200_fp8_capi.cu) compile in parallel, then link
+    into one library."""
+    return _compile_and_link(LIB_DIR / "libb200_hgemm.so",
+                             [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], verbose, force)
 
 
 def build_fp8block(verbose: bool = False, force: bool = False) -> Path:
@@ -92,51 +97,21 @@ def build_fp8block(verbose: bool = False, force: bool = False) -> Path:
     return out
 
 
-BATCHED_VARIANTS = (0, 1, 2)   # fp16 with fp32 accumulation, fp16 with fp16 accumulation, bf16 (the GemmType index)
+VARIANTS = (0, 1, 2)   # fp16 with fp32 accumulation, fp16 with fp16 accumulation, bf16 (the GemmType index)
 
 
 def build_batched(verbose: bool = False, force: bool = False) -> Path:
     """The batched 16-bit kernels: a library of their own, so that libb200_hgemm.so's device code is unaffected. One
-    source, compiled once per data type in parallel (31 kernels each), then linked."""
-    LIB_DIR.mkdir(exist_ok=True)
-    out = LIB_DIR / "libb200_batched.so"
-    src = CSRC / "b200_batched_capi.cu"
-    if force or _stale(out, [src] + _headers()):
-        objs = [LIB_DIR / f"b200_batched_{v}.o" for v in BATCHED_VARIANTS]
-        from concurrent.futures import ThreadPoolExecutor
-        with ThreadPoolExecutor(len(objs)) as pool:
-            for f in [pool.submit(_run, [nvcc_path(), *ARCH_FLAGS, *COMMON, f"-DB200_BATCHED_VARIANT={v}", "-c", "-o",
-                                         str(obj), str(src)], verbose)
-                      for v, obj in zip(BATCHED_VARIANTS, objs)]:
-                f.result()
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs)], verbose)
-        for obj in objs:
-            obj.unlink()
-    return out
-
-
-GROUPED_VARIANTS = BATCHED_VARIANTS
+    source, compiled once per data type (31 kernels each)."""
+    return _compile_and_link(LIB_DIR / "libb200_batched.so",
+                             [(CSRC / "b200_batched_capi.cu", [f"-DB200_VARIANT={v}"]) for v in VARIANTS], verbose, force)
 
 
 def build_grouped(verbose: bool = False, force: bool = False) -> Path:
     """The grouped 16-bit kernels over contiguous row groups: a library of their own, so that the device code of
-    libb200_hgemm.so and libb200_batched.so is unaffected. One source, compiled once per data type in parallel (31
-    kernels each), then linked."""
-    LIB_DIR.mkdir(exist_ok=True)
-    out = LIB_DIR / "libb200_grouped.so"
-    src = CSRC / "b200_grouped_capi.cu"
-    if force or _stale(out, [src] + _headers()):
-        objs = [LIB_DIR / f"b200_grouped_{v}.o" for v in GROUPED_VARIANTS]
-        from concurrent.futures import ThreadPoolExecutor
-        with ThreadPoolExecutor(len(objs)) as pool:
-            for f in [pool.submit(_run, [nvcc_path(), *ARCH_FLAGS, *COMMON, f"-DB200_GROUPED_VARIANT={v}", "-c", "-o",
-                                         str(obj), str(src)], verbose)
-                      for v, obj in zip(GROUPED_VARIANTS, objs)]:
-                f.result()
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs)], verbose)
-        for obj in objs:
-            obj.unlink()
-    return out
+    libb200_hgemm.so and libb200_batched.so is unaffected. One source, compiled once per data type (31 kernels each)."""
+    return _compile_and_link(LIB_DIR / "libb200_grouped.so",
+                             [(CSRC / "b200_grouped_capi.cu", [f"-DB200_VARIANT={v}"]) for v in VARIANTS], verbose, force)
 
 
 def build_baselines(verbose: bool = False, force: bool = False) -> Path:

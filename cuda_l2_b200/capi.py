@@ -16,8 +16,7 @@ LIB_DIR = Path(__file__).resolve().parent / "lib"
 _hgemm = None
 _baselines = None
 _fp8block = None
-_batched = None
-_grouped = None
+_tile_list_libs: dict = {}
 
 ACC_BITS = {"fp32": 32, "fp16": 16, 32: 32, 16: 16}
 
@@ -95,46 +94,38 @@ def fp8block_lib() -> ctypes.CDLL:
     return _fp8block
 
 
+# The entry points of a tile-list library (include/b200_batched.h, include/b200_grouped.h), b200_<prefix>_<suffix>, with
+# the same signatures in both: suffix -> (argtypes, restype).
+_vp, _i, _ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
+_TILE_LIST_ABI = {
+    "gemm": ([_i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp], _i),
+    "gemm_run_config": ([_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i),
+    "select": ([_i, _i, _i, _i, _i, _ip, _ip], _i),
+    "schedule_units": ([_i, _i, _i, _i, _i, _ip, _i, _i, _ip, _i, _ip], _i),
+    "launch_count": ([], ctypes.c_ulonglong),
+    "strerror": ([_i], ctypes.c_char_p),
+}
+
+
+def _tile_list_lib(name: str, prefix: str) -> ctypes.CDLL:
+    """The tile-list library ``name``, its entry points named b200_<prefix>_*."""
+    if name not in _tile_list_libs:
+        lib = _load(name)
+        for suffix, (args, res) in _TILE_LIST_ABI.items():
+            fn = getattr(lib, f"b200_{prefix}_{suffix}")
+            fn.argtypes, fn.restype = args, res
+        _tile_list_libs[name] = lib
+    return _tile_list_libs[name]
+
+
 def batched_lib() -> ctypes.CDLL:
     """libb200_batched.so: the batched fp16 / bf16 GEMM (include/b200_batched.h)."""
-    global _batched
-    if _batched is None:
-        lib = _load("libb200_batched.so")
-        vp, i, ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
-        lib.b200_batched_gemm.argtypes = [i, vp, vp, vp, vp, i, i, i, i, vp]
-        lib.b200_batched_gemm.restype = i
-        lib.b200_batched_gemm_run_config.argtypes = [i, i, vp, vp, vp, vp, i, i, i, i, i, i, vp]
-        lib.b200_batched_gemm_run_config.restype = i
-        lib.b200_batched_select.argtypes = [i, i, i, i, i, ip, ip]
-        lib.b200_batched_select.restype = i
-        lib.b200_batched_schedule_units.argtypes = [i, i, i, i, i, ip, i, i, ip, i, ip]
-        lib.b200_batched_schedule_units.restype = i
-        lib.b200_batched_launch_count.restype = ctypes.c_ulonglong
-        lib.b200_batched_strerror.argtypes = [i]
-        lib.b200_batched_strerror.restype = ctypes.c_char_p
-        _batched = lib
-    return _batched
+    return _tile_list_lib("libb200_batched.so", "batched")
 
 
 def grouped_lib() -> ctypes.CDLL:
     """libb200_grouped.so: the grouped fp16 / bf16 GEMM over contiguous row groups (include/b200_grouped.h)."""
-    global _grouped
-    if _grouped is None:
-        lib = _load("libb200_grouped.so")
-        vp, i, ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
-        lib.b200_grouped_gemm.argtypes = [i, vp, vp, vp, vp, i, i, i, i, vp]
-        lib.b200_grouped_gemm.restype = i
-        lib.b200_grouped_gemm_run_config.argtypes = [i, i, vp, vp, vp, vp, i, i, i, i, i, i, vp]
-        lib.b200_grouped_gemm_run_config.restype = i
-        lib.b200_grouped_select.argtypes = [i, i, i, i, i, ip, ip]
-        lib.b200_grouped_select.restype = i
-        lib.b200_grouped_schedule_units.argtypes = [i, i, i, i, i, ip, i, i, ip, i, ip]
-        lib.b200_grouped_schedule_units.restype = i
-        lib.b200_grouped_launch_count.restype = ctypes.c_ulonglong
-        lib.b200_grouped_strerror.argtypes = [i]
-        lib.b200_grouped_strerror.restype = ctypes.c_char_p
-        _grouped = lib
-    return _grouped
+    return _tile_list_lib("libb200_grouped.so", "grouped")
 
 
 def baselines_lib() -> ctypes.CDLL:
@@ -168,14 +159,8 @@ def exported_symbols() -> dict[str, list[str]]:
             "b200_fp8gemm_blockwise", "b200_fp8gemm_blockwise_run_config", "b200_fp8gemm_blockwise_select",
             "b200_fp8block_launch_count", "b200_fp8block_strerror",
         ],
-        "libb200_batched.so": [
-            "b200_batched_gemm", "b200_batched_gemm_run_config", "b200_batched_select", "b200_batched_schedule_units",
-            "b200_batched_launch_count", "b200_batched_strerror",
-        ],
-        "libb200_grouped.so": [
-            "b200_grouped_gemm", "b200_grouped_gemm_run_config", "b200_grouped_select", "b200_grouped_schedule_units",
-            "b200_grouped_launch_count", "b200_grouped_strerror",
-        ],
+        "libb200_batched.so": [f"b200_batched_{suffix}" for suffix in _TILE_LIST_ABI],
+        "libb200_grouped.so": [f"b200_grouped_{suffix}" for suffix in _TILE_LIST_ABI],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
             "b200_bl_lt_autotune", "b200_bl_lt_autotune_info",
@@ -293,21 +278,36 @@ def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tupl
         (m, k), (n, k2) = a.shape, b_kmajor.shape
     except ValueError:
         raise B200HgemmError(f"2-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
-    dtype = a.dtype
-    t = gemm_type(dtype, out_dtype, acc) if b_kmajor.dtype == dtype else None
-    if t is None:
-        raise B200HgemmError(f"no kernel for {dtype} x {b_kmajor.dtype} -> {out_dtype} with acc={acc!r} (fp16 with "
-                             "fp32 or fp16 accumulation, bf16 with fp32, e4m3 -> fp16 / bf16 with fp32)")
+    t = _operand_type(a, b_kmajor, out_dtype, acc)
     if len(scales) != (0 if t.scale is None else 2):
-        raise B200HgemmError(f"{dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
+        raise B200HgemmError(f"{a.dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
     if scales:
         scale_granularity(m, n, *scales, k=k)
-    if k2 != k:
-        raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} (K-major: [N, K])")
-    if not t.fits(n, k):
-        raise B200HgemmError(f"{dtype} operands need N % 8 == 0 and K % {t.k_align} == 0 (16-byte TMA strides), "
-                             f"got N={n}, K={k}")
+    _check_k(a, b_kmajor, t, n, k, k2, "[N, K]")
     return m, n, k
+
+
+def _operand_type(a, b_kmajor, out_dtype, acc: str | int, scaled: bool = True) -> GemmType:
+    """The variant of a @ b_kmajor^T -> ``out_dtype`` with ``acc``: operands of one dtype that name one (``scaled=False``:
+    a 16-bit one). B200HgemmError otherwise."""
+    t = gemm_type(a.dtype, out_dtype, acc) if b_kmajor.dtype == a.dtype else None
+    if t is None or (t.scale is not None and not scaled):
+        kinds = "fp16 with fp32 or fp16 accumulation, bf16 with fp32"
+        if scaled:
+            kinds += ", e4m3 -> fp16 / bf16 with fp32"
+        raise B200HgemmError(f"no kernel for {a.dtype} x {b_kmajor.dtype} -> {out_dtype} with acc={acc!r} ({kinds})")
+    return t
+
+
+def _check_k(a, b_kmajor, t: GemmType, n: int, k: int, k2: int, b_layout: str) -> None:
+    """The rules every product shares: a's K is b_kmajor's (``b_layout``, K-major), and rows of 16 bytes
+    (:meth:`GemmType.fits`). B200HgemmError otherwise."""
+    if k2 != k:
+        raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} "
+                             f"(K-major: {b_layout})")
+    if not t.fits(n, k):
+        raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % {t.k_align} == 0 (16-byte TMA strides), "
+                             f"got N={n}, K={k}")
 
 
 def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = (), strided_scale_a: bool = False
@@ -416,6 +416,26 @@ def fp8block_launch_count() -> int:
     return int(fp8block_lib().b200_fp8block_launch_count())
 
 
+def _tile_list_schedule(schedule_units, *args) -> dict:
+    """Every worker's units from a tile-list library's ``schedule_units`` entry point, called with ``args`` (config id,
+    count, rows, N, K, host list, SMs) and then the worker and its buffer."""
+    nw = ctypes.c_int()
+    cap = 256
+    buf = (ctypes.c_int * (3 * cap))()
+    st = schedule_units(*args, 0, buf, cap, ctypes.byref(nw))
+    if st < 0:
+        raise B200HgemmError(f"{schedule_units.__name__} failed: status {st}")
+    units = []
+    for w in range(nw.value):
+        cnt = schedule_units(*args, w, buf, cap, None)
+        if cnt > cap:
+            cap = cnt
+            buf = (ctypes.c_int * (3 * cap))()
+            cnt = schedule_units(*args, w, buf, cap, None)
+        units.append([(buf[3 * j], buf[3 * j + 1], buf[3 * j + 2]) for j in range(cnt)])
+    return {"workers": nw.value, "units": units}
+
+
 # ------------------------------------------------------------------------------------------ batched (libb200_batched.so)
 def batched_variant(dtype, acc: str | int = "fp32") -> int | None:
     """The ``variant`` argument of include/b200_batched.h (the GemmType index): 0 fp16 with fp32 accumulation, 1 fp16
@@ -435,16 +455,10 @@ def check_batched_operands(a, b_kmajor, acc: str | int = "fp32", masked_m=None) 
         (bsz, m, k), (bsz2, n, k2) = a.shape, b_kmajor.shape
     except ValueError:
         raise B200HgemmError(f"3-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
-    t = gemm_type(a.dtype, a.dtype, acc) if b_kmajor.dtype == a.dtype else None
-    if t is None or t.scale is not None:
-        raise B200HgemmError(f"no batched kernel for {a.dtype} x {b_kmajor.dtype} with acc={acc!r} (fp16 with fp32 or "
-                             "fp16 accumulation, bf16 with fp32)")
-    if bsz2 != bsz or k2 != k:
-        raise B200HgemmError(f"batch counts or inner dimensions differ: a {tuple(a.shape)}, b_kmajor "
-                             f"{tuple(b_kmajor.shape)} (K-major: [B, N, K])")
-    if not t.fits(n, k):
-        raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % {t.k_align} == 0 (16-byte TMA strides), "
-                             f"got N={n}, K={k}")
+    t = _operand_type(a, b_kmajor, a.dtype, acc, scaled=False)
+    if bsz2 != bsz:
+        raise B200HgemmError(f"batch counts differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}")
+    _check_k(a, b_kmajor, t, n, k, k2, "[B, N, K]")
     if masked_m is not None and (masked_m.dtype != torch.int32 or tuple(masked_m.shape) != (bsz,)):
         raise B200HgemmError(f"masked_m must be an int32 tensor of shape [{bsz}], got {masked_m.dtype} "
                              f"{tuple(masked_m.shape)}")
@@ -489,23 +503,8 @@ def batched_schedule(config_id: int, b: int, m: int, n: int, k: int, masked_m=No
     launcher's default rasterisation. ``masked_m``: per-batch row counts (a sequence of ints) or None (dense).
 
     Returns ``{"workers": W, "units": [[(batch, m_block, n_block), ...] per worker]}``; blocks are cluster blocks."""
-    lib = batched_lib()
     counts = None if masked_m is None else (ctypes.c_int * b)(*masked_m)
-    nw = ctypes.c_int()
-    cap = 256
-    buf = (ctypes.c_int * (3 * cap))()
-    st = lib.b200_batched_schedule_units(config_id, b, m, n, k, counts, num_sms, 0, buf, cap, ctypes.byref(nw))
-    if st < 0:
-        raise B200HgemmError(f"b200_batched_schedule_units failed: status {st}")
-    units = []
-    for w in range(nw.value):
-        cnt = lib.b200_batched_schedule_units(config_id, b, m, n, k, counts, num_sms, w, buf, cap, None)
-        if cnt > cap:
-            cap = cnt
-            buf = (ctypes.c_int * (3 * cap))()
-            cnt = lib.b200_batched_schedule_units(config_id, b, m, n, k, counts, num_sms, w, buf, cap, None)
-        units.append([(buf[3 * j], buf[3 * j + 1], buf[3 * j + 2]) for j in range(cnt)])
-    return {"workers": nw.value, "units": units}
+    return _tile_list_schedule(batched_lib().b200_batched_schedule_units, config_id, b, m, n, k, counts, num_sms)
 
 
 def batched_launch_count() -> int:
@@ -525,16 +524,7 @@ def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32") -> tuple[
     except ValueError:
         raise B200HgemmError(f"a [T, K] and b_kmajor [G, N, K] expected, got {tuple(a.shape)} and "
                              f"{tuple(b_kmajor.shape)}") from None
-    gt = gemm_type(a.dtype, a.dtype, acc) if b_kmajor.dtype == a.dtype else None
-    if gt is None or gt.scale is not None:
-        raise B200HgemmError(f"no grouped kernel for {a.dtype} x {b_kmajor.dtype} with acc={acc!r} (fp16 with fp32 or "
-                             "fp16 accumulation, bf16 with fp32)")
-    if k2 != k:
-        raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)} "
-                             "(K-major: [G, N, K])")
-    if not gt.fits(n, k):
-        raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % {gt.k_align} == 0 (16-byte TMA strides), "
-                             f"got N={n}, K={k}")
+    _check_k(a, b_kmajor, _operand_type(a, b_kmajor, a.dtype, acc, scaled=False), n, k, k2, "[G, N, K]")
     if offs.dtype != torch.int32 or tuple(offs.shape) != (g,):
         raise B200HgemmError(f"offs must be an int32 tensor of shape [{g}], got {offs.dtype} {tuple(offs.shape)}")
     return g, t, n, k
@@ -580,24 +570,8 @@ def grouped_schedule(config_id: int, t: int, n: int, k: int, offs, num_sms: int 
 
     Returns ``{"workers": W, "units": [[(group, m_block, n_block), ...] per worker]}``; blocks are cluster blocks, and
     m-blocks count from the group's first row."""
-    lib = grouped_lib()
-    g = len(offs)
-    ends = (ctypes.c_int * g)(*offs)
-    nw = ctypes.c_int()
-    cap = 256
-    buf = (ctypes.c_int * (3 * cap))()
-    st = lib.b200_grouped_schedule_units(config_id, g, t, n, k, ends, num_sms, 0, buf, cap, ctypes.byref(nw))
-    if st < 0:
-        raise B200HgemmError(f"b200_grouped_schedule_units failed: status {st}")
-    units = []
-    for w in range(nw.value):
-        cnt = lib.b200_grouped_schedule_units(config_id, g, t, n, k, ends, num_sms, w, buf, cap, None)
-        if cnt > cap:
-            cap = cnt
-            buf = (ctypes.c_int * (3 * cap))()
-            cnt = lib.b200_grouped_schedule_units(config_id, g, t, n, k, ends, num_sms, w, buf, cap, None)
-        units.append([(buf[3 * j], buf[3 * j + 1], buf[3 * j + 2]) for j in range(cnt)])
-    return {"workers": nw.value, "units": units}
+    ends = (ctypes.c_int * len(offs))(*offs)
+    return _tile_list_schedule(grouped_lib().b200_grouped_schedule_units, config_id, len(offs), t, n, k, ends, num_sms)
 
 
 def grouped_launch_count() -> int:

@@ -92,4 +92,109 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
   if (st == host::kOk) g_launches.fetch_add(1, std::memory_order_relaxed);
   return st;
 }
+
+// The tile-list libraries (libb200_batched.so, libb200_grouped.so): the 16-bit variants 0, 1, 2 (the GemmType index) of
+// every configuration, wrapped in Wrapper (Batched or Grouped), launched by host::launch_list.
+namespace tile_list {
+
+inline bool known_variant(int v) { return v >= 0 && v <= 2; }
+
+// Kernel launches of the library that holds it (b200_batched_launch_count, b200_grouped_launch_count): one counter
+// for the library's objects; hidden, like g_launches.
+__attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_list_launches{0};
+
+template <template <class> class Wrapper, host::GemmType T>
+int run_config(int id, const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
+               int group_m, int max_ctas, cudaStream_t s) {
+  constexpr host::GemmTypeTraits t = host::traits(T);
+  static_assert(!t.e4m3() && !t.scaled, "16-bit variants only");
+  int st;
+  switch (id) {
+#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
+  case ID:                                                                                                     \
+    st = host::launch_list<Wrapper<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16()>>>(                  \
+        A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas);                                               \
+    break;
+    B200_HGEMM_CONFIGS(B200_CASE)
+#undef B200_CASE
+    default:
+      return host::kBadConfig;
+  }
+  if (st == host::kOk && rows > 0) g_list_launches.fetch_add(1, std::memory_order_relaxed);   // rows == 0: no launch
+  return st;
+}
+
+// A library compiles its source once per variant (-DB200_VARIANT = 0, 1, 2), in parallel: each object instantiates
+// its own variant's 31 kernels, and the calls of the other objects' variants link against theirs. Variant 0's object
+// also holds the C entry points.
+#define B200_LIST_RUN(W, T)                                                                                    \
+  int run_config<W, T>(int, const void*, const void*, void*, const int*, int, int, int, int, int, int, cudaStream_t)
+#define B200_LIST_OBJECT(W)                                                                                    \
+  extern template B200_LIST_RUN(W, host::GemmType::kF16Acc32);                                                 \
+  extern template B200_LIST_RUN(W, host::GemmType::kF16Acc16);                                                 \
+  extern template B200_LIST_RUN(W, host::GemmType::kBF16);                                                     \
+  template B200_LIST_RUN(W, host::GemmType(B200_VARIANT))
+
+template <template <class> class Wrapper>
+int run(int variant, int config_id, const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N,
+        int K, int group_m, int max_ctas, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  switch (variant) {
+    case 0:
+      return run_config<Wrapper, host::GemmType::kF16Acc32>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
+                                                            max_ctas, s);
+    case 1:
+      return run_config<Wrapper, host::GemmType::kF16Acc16>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
+                                                            max_ctas, s);
+    case 2:
+      return run_config<Wrapper, host::GemmType::kBF16>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
+                                                        max_ctas, s);
+    default: return host::kBadConfig;
+  }
+}
+
+// Host view of worker `worker`'s tiles, with the launcher's plan on a device of num_sms SMs (every cluster resident)
+// and its default group_m: (index, m_block, n_block) per tile into `units` (at most max_units); returns the count.
+template <class Cfg>
+int schedule_units(int count, int rows, int N, int K, const int* list, int num_sms, int worker, int* units,
+                   int max_units, int* num_workers) {
+  const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
+  if (tiles > 0x7fffffffLL) return host::kBadShape;
+  const int max_workers = num_sms / Cfg::CLUSTER_CTAS;
+  const host::Plan p = host::list_plan<Cfg>(tiles, K, max_workers, [=] { return max_workers; });
+  if (num_workers) *num_workers = p.workers;
+  if (worker < 0 || worker >= p.workers) return host::kBadShape;
+  const int n_blocks = (N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N);
+  typename Cfg::Cursor cursor(list, count, rows, Cfg::TILE_M * Cfg::CLUSTER_M, n_blocks, host::default_group_m<Cfg>());
+  WorkIter it(worker, p.workers, cursor.total(), p.nkb, 1, 0);
+  WorkUnit u;
+  int n = 0;
+  while (it.next(u)) {
+    const BatchTile bt = cursor.locate(u.tile);
+    if (n < max_units && units) {
+      units[3 * n] = bt.batch; units[3 * n + 1] = bt.tc.m_blk; units[3 * n + 2] = bt.tc.n_blk;
+    }
+    ++n;
+  }
+  return n;
+}
+
+// The same for configuration `config_id` (fp32-accumulating fp16: the schedule does not depend on the variant).
+template <template <class> class Wrapper>
+int schedule_config(int config_id, int count, int rows, int N, int K, const int* list, int num_sms, int worker,
+                    int* units, int max_units, int* num_workers) {
+  switch (config_id) {
+#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                 \
+  case ID:                                                                                                      \
+    return schedule_units<Wrapper<Config<BN, STAGES, CG, true, CM, CN, MR>>>(count, rows, N, K, list, num_sms,  \
+                                                                             worker, units, max_units,          \
+                                                                             num_workers);
+    B200_HGEMM_CONFIGS(B200_CASE)
+#undef B200_CASE
+    default:
+      return host::kBadConfig;
+  }
+}
+
+}  // namespace tile_list
 }  // namespace b200

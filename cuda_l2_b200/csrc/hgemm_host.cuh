@@ -191,15 +191,15 @@ inline const DeviceInfo& device_info() {
 // rows hold K operand elements (K % 8 == 0 at two bytes, K % 16 == 0 at one byte), C rows N 16-bit elements. The scales
 // of a scaled variant are fp32 values in device memory: 4-byte aligned per tensor, 16-byte aligned vectors (M and N
 // values) rowwise, where the split-K reductions read the column scales as float4. Block scales: `a` 16-byte aligned (one
-// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned. Batched launches: batches >= 1 matrices,
-// whose tiles (`tiles` per matrix) number at most INT_MAX in all, and row counts `masked_m` (optional) 4-byte aligned.
-// Grouped launches (validate_grouped) pass their offsets as `masked_m` and the worst-case tile list as `tiles`.
+// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned. Tile-list launches (launch_list):
+// batches >= 1 matrices, a tile list of at most INT_MAX `tiles`, and its device array `list` (a batched launch's
+// optional row counts) 4-byte aligned. Grouped launches (validate_grouped) pass their offsets as `list`.
 inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K,
-                    int ld_a = 0, int batches = 1, long long tiles = 1, const int* masked_m = nullptr) {
+                    int ld_a = 0, int batches = 1, long long tiles = 1, const int* list = nullptr) {
   const GemmTypeTraits& t = traits(type);
   if (!A || !Bt || !C || (t.scaled && (!scales.a || !scales.b))) return kNullPointer;
-  if (M <= 0 || N <= 0 || K <= 0 || batches < 1 || batches * tiles > 0x7fffffffLL) return kBadShape;
-  if (reinterpret_cast<uintptr_t>(masked_m) & 3) return kBadAlignment;
+  if (M <= 0 || N <= 0 || K <= 0 || batches < 1 || tiles > 0x7fffffffLL) return kBadShape;
+  if (reinterpret_cast<uintptr_t>(list) & 3) return kBadAlignment;
   if (K % (16 / elem_bytes(t.operand))) return t.e4m3() ? kBadFp8K : kBadAlignment;
   if (N % 8) return kBadAlignment;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
@@ -507,6 +507,10 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   return e == cudaSuccess ? kOk : int(e);
 }
 
+// The rasterisation width (tile_coord's group_m) of a launch that passes group_m <= 0.
+template <class Cfg>
+constexpr int default_group_m() { return Cfg::CTA_GROUP == 2 ? 8 : 16; }
+
 // group_m <= 0 selects the default rasterisation width. max_ctas <= 0 means "all SMs". `splits`: 1 none, > 1 workspace
 // split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
 // mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
@@ -540,7 +544,7 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
     }
   }
   a.M = M; a.N = N; a.K = K;
-  a.group_m = group_m > 0 ? group_m : (Cfg::CTA_GROUP == 2 ? 8 : 16);
+  a.group_m = group_m > 0 ? group_m : default_group_m<Cfg>();
   a.c = static_cast<__half*>(C);
   a.scales = scales;
   a.ld_a = ld_a;
@@ -579,71 +583,24 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   return launch_mode<Cfg, kPlain>(di, a);
 }
 
-// Tiles (cluster blocks) of one M x N matrix of a batched launch.
-template <class Cfg>
-constexpr long long batch_tiles(int M, int N) {
-  return (long long)((M + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M)) *
-         ((N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N));
-}
-
-// The schedule of a batched launch: plain (there is no other for this variant, so it needs no scratch and is always
-// safe to capture in a graph), workers bounded by the dense tile list. With row counts the kernel's list is shorter,
-// and the workers without a tile leave at once.
+// The schedule of a tile-list launch: plain (there is no other for these kernels, so a launch needs no scratch and is
+// always safe to capture in a graph), workers bounded by the cursor's longest list, `max_tiles`. The kernel's list may
+// be shorter (row counts, group offsets), and the workers without a tile leave at once.
 template <class Cfg, class ResidentClusters>
-Plan batched_plan(int batches, int M, int N, int K, int max_workers, ResidentClusters&& resident_clusters) {
+Plan list_plan(long long max_tiles, int K, int max_workers, ResidentClusters&& resident_clusters) {
   Plan p{};
   p.mode = kPlain;
   p.splits = 1;
-  p.num_tiles = int(batches * batch_tiles<Cfg>(M, N));   // validate() bounds it
+  p.num_tiles = int(max_tiles);   // validate() bounds it
   p.nkb = (K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
   if (Cfg::CLUSTER_CTAS > 2) max_workers = std::min(max_workers, resident_clusters());
   p.workers = std::min(std::max(max_workers, 1), p.num_tiles);
   return p;
 }
 
-// C[b] = A[b] Bt[b]^T for b < batches, A [batches, M, K], Bt [batches, N, K], C [batches, M, N], all contiguous;
-// masked_m (device memory, optional): only rows [0, clamp(masked_m[b], 0, M)) of C[b] are computed, and no 16-row
-// store box starting at or past that count is written. No L2 eviction hints: which operand is re-read depends on the
-// batch as much as on the shapes.
-template <class Cfg>
-int launch_batched(const void* A, const void* Bt, void* C, const int* masked_m, int batches, int M, int N, int K,
-                   cudaStream_t stream, int group_m = 0, int max_ctas = 0) {
-  static_assert(batched<Cfg>(), "a Batched<> configuration");
-  constexpr GemmType kType = gemm_type<Cfg>();
-  int st = validate(kType, A, Bt, C, Scales{nullptr, nullptr}, M, N, K, 0, batches, batch_tiles<Cfg>(M, N), masked_m);
-  if (st != kOk) return st;
-  const DeviceInfo& di = device_info();
-  if (di.cc_major != 9) return kNotHopper;
-
-  LaunchArgs a{};
-  MapCache& cache = map_cache();
-  const Elem elem = traits(kType).operand;
-  if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem, batches)) != kOk) return st;
-  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, batches)) != kOk) return st;
-  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, elem, batches)) != kOk) return st;
-  const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
-  a.plan = batched_plan<Cfg>(batches, M, N, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
-  a.M = M; a.N = N; a.K = K;
-  a.group_m = group_m > 0 ? group_m : (Cfg::CTA_GROUP == 2 ? 8 : 16);
-  a.c = static_cast<__half*>(C);
-  a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
-  a.batches = batches;
-  a.masked_m = masked_m;
-  a.stream = stream;
-  return launch_mode<Cfg, kPlain>(di, a);
-}
-
-// The longest tile list a grouped launch over T rows and G groups can have: every group adds at most one partial
-// cluster row block to the ceil(T / block_rows) of the rows themselves.
-template <class Cfg>
-constexpr long long grouped_worst_tiles(int groups, int T, int N) {
-  return (((long long)T + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M) + groups) *
-         (((long long)N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N));
-}
-
 // The argument rules of a grouped launch: those of a 2-D [T, K] x [N, K] call (T == 0 is an empty problem and valid),
 // G >= 1 groups whose offsets (G int32 values, device memory) are non-null and 4-byte aligned, and a worst-case tile
-// list (`worst_tiles`, grouped_worst_tiles) of at most INT_MAX tiles.
+// list (`worst_tiles`, GroupCursor::max_tiles) of at most INT_MAX tiles.
 inline int validate_grouped(GemmType type, const void* A, const void* Bt, const void* C, const int* offs, int groups,
                             int T, int N, int K, long long worst_tiles) {
   if (!A || !Bt || !C || !offs) return kNullPointer;
@@ -651,49 +608,45 @@ inline int validate_grouped(GemmType type, const void* A, const void* Bt, const 
   return validate(type, A, Bt, C, Scales{nullptr, nullptr}, T > 0 ? T : 1, N, K, 0, 1, worst_tiles, offs);
 }
 
-// The schedule of a grouped launch: plain, like the batched one, with the workers bounded by the worst-case tile list
-// (the real one is only known on the device, where the workers without a tile leave at once).
-template <class Cfg, class ResidentClusters>
-Plan grouped_plan(int groups, int T, int N, int K, int max_workers, ResidentClusters&& resident_clusters) {
-  Plan p{};
-  p.mode = kPlain;
-  p.splits = 1;
-  p.num_tiles = int(grouped_worst_tiles<Cfg>(groups, T, N));   // validate_grouped() bounds it
-  p.nkb = (K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
-  if (Cfg::CLUSTER_CTAS > 2) max_workers = std::min(max_workers, resident_clusters());
-  p.workers = std::min(std::max(max_workers, 1), p.num_tiles);
-  return p;
-}
-
-// C[start_g : end_g] = A[start_g : end_g] Bt[g]^T for g < groups: A [T, K], Bt [groups, N, K], C [T, N], contiguous.
-// offs (device memory, read by the kernel only): the cumulative group ends, end_g = clamp(offs[g], start_g, T) with
-// start_0 = 0 and start_g = end_{g-1}. Every row of C below end_{groups-1} is written once, by its own group; no other
-// is written. T == 0 launches nothing. No L2 eviction hints, as for the batched launches.
+// One launch of a Batched<> or Grouped<> configuration, which walks the flat tile list of its Cfg::Cursor over
+// `count` matrices or groups. No L2 eviction hints: which operand is re-read depends on the batch or group as much as
+// on the shapes. rows == 0 launches nothing.
+//   Batched<>: C[b] = A[b] Bt[b]^T for b < count, A [count, rows, K], Bt [count, N, K], C [count, rows, N], all
+//   contiguous; `list` (device memory, optional): only rows [0, clamp(list[b], 0, rows)) of C[b] are computed, and no
+//   16-row store box starting at or past that count is written.
+//   Grouped<>: C[start_g : end_g] = A[start_g : end_g] Bt[g]^T for g < count, A [rows, K], Bt [count, N, K],
+//   C [rows, N], contiguous; `list` (device memory, read by the kernel only): the cumulative group ends,
+//   end_g = clamp(list[g], start_g, rows) with start_0 = 0 and start_g = end_{g-1}. Every row of C below
+//   end_{count-1} is written once, by its own group; no other is written.
 template <class Cfg>
-int launch_grouped(const void* A, const void* Bt, void* C, const int* offs, int groups, int T, int N, int K,
-                   cudaStream_t stream, int group_m = 0, int max_ctas = 0) {
-  static_assert(grouped<Cfg>(), "a Grouped<> configuration");
+int launch_list(const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
+                cudaStream_t stream, int group_m = 0, int max_ctas = 0) {
+  static_assert(batched<Cfg>() || grouped<Cfg>(), "a Batched<> or Grouped<> configuration");
   constexpr GemmType kType = gemm_type<Cfg>();
-  const long long worst = groups > 0 && T >= 0 ? grouped_worst_tiles<Cfg>(groups, T, N) : 1;
-  int st = validate_grouped(kType, A, Bt, C, offs, groups, T, N, K, worst);
-  if (st != kOk || T == 0) return st;
+  const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
+  int st = grouped<Cfg>() ? validate_grouped(kType, A, Bt, C, list, count, rows, N, K, tiles)
+                          : validate(kType, A, Bt, C, Scales{nullptr, nullptr}, rows, N, K, 0, count, tiles, list);
+  if (st != kOk || rows == 0) return st;
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
 
   LaunchArgs a{};
   MapCache& cache = map_cache();
   const Elem elem = traits(kType).operand;
-  if ((st = cache.get(A, T, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem)) != kOk) return st;
-  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, groups)) != kOk) return st;
-  if ((st = cache.get(C, T, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, elem)) != kOk) return st;
+  // Bt is one N x K matrix per batch or group; A and C are one matrix per batch (3-D maps, so that TMA clips each box
+  // at its own matrix's edge), or the rows of all groups (2-D maps)
+  const int depth = batched<Cfg>() ? count : 0;
+  if ((st = cache.get(A, rows, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem, depth)) != kOk) return st;
+  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, count)) != kOk) return st;
+  if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, elem, depth)) != kOk) return st;
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
-  a.plan = grouped_plan<Cfg>(groups, T, N, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
-  a.M = T; a.N = N; a.K = K;
-  a.group_m = group_m > 0 ? group_m : (Cfg::CTA_GROUP == 2 ? 8 : 16);
+  a.plan = list_plan<Cfg>(tiles, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
+  a.M = rows; a.N = N; a.K = K;
+  a.group_m = group_m > 0 ? group_m : default_group_m<Cfg>();
   a.c = static_cast<__half*>(C);
   a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
-  a.batches = groups;
-  a.masked_m = offs;
+  a.batches = count;
+  a.masked_m = list;
   a.stream = stream;
   return launch_mode<Cfg, kPlain>(di, a);
 }

@@ -14,7 +14,6 @@
 //                   never wait on anybody) and writes C. See streamk_* in hgemm_sm90.cuh.
 #pragma once
 #include <cuda_runtime.h>
-#include <type_traits>
 
 namespace b200 {
 
@@ -116,6 +115,14 @@ struct BatchCursor {
       : counts(counts_), num_batches(num_batches_), M(M_), block_rows(block_rows_), n_blocks(n_blocks_),
         group_m(group_m_), batch(0), first(0), m_blocks(blocks_of(0)) {}
 
+  // The longest list of a launch of Cfg over num_batches matrices of M x N (host side: it bounds the workers): the
+  // dense one.
+  template <class Cfg>
+  static constexpr long long max_tiles(int num_batches, int M, int N) {
+    return num_batches * ((long long)((M + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M)) *
+                          ((N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N)));
+  }
+
   __host__ __device__ __forceinline__ int rows_of(int b) const {
     if (!counts) return M;
     const int r = counts[b];
@@ -169,6 +176,15 @@ struct GroupCursor {
         group(0), first(0), start(0) {
     end = end_of(0, 0);
     m_blocks = (end - start + block_rows - 1) / block_rows;
+  }
+
+  // The longest list of a launch of Cfg over T rows in num_groups groups and N columns (host side: it bounds the
+  // workers; the real list is only known on the device): every group adds at most one partial cluster row block to
+  // the ceil(T / block_rows) of the rows themselves.
+  template <class Cfg>
+  static constexpr long long max_tiles(int num_groups, int T, int N) {
+    return (((long long)T + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M) + num_groups) *
+           (((long long)N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N));
   }
 
   __host__ __device__ __forceinline__ int end_of(int g, int s) const {

@@ -99,6 +99,9 @@ struct Config {
   // which K-decompositions this configuration's kernel carries
   static constexpr bool STREAM_K = CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
   static constexpr bool SPLIT_K = STREAM_K && CTA_GROUP_ == 1;
+  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>) override these
+  static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false;
+  using Cursor = NoBatches;   // the flat tile list the kernel walks (hgemm_schedule.cuh): none
   static constexpr int EPI_BYTES = 8 * EPI_ROWS * 64 * 2;    // 8 consumer warps x one staging buffer (sized for EPI_N = 64)
   static constexpr int BAR_BYTES = 256;
   // STAGES_ is the requested ring depth; on sm_90 every CTA of a pair holds the whole B tile, so the depth is capped
@@ -128,7 +131,7 @@ constexpr int kMaxSplitTiles = 256;   // split-K is only used when tiles * split
 // CTA_M values of A's scales (one 1-D bulk copy, counted in the stage's transaction bytes) and the tile's one value of
 // Bt's (written by the producer before its arrive), 16 bytes of padding keeping the next stage's slice aligned.
 // A wrapper, so that the Config<> instantiations of the other variants, and with them their kernels' names, stay as
-// they are; block_scaled<Cfg>() reads the flag, false for a plain Config.
+// they are; block_scaled<Cfg>() reads the flag.
 template <class Base>
 struct BlockScaled : Base {
   static constexpr bool BLOCK_SCALED = true;
@@ -140,12 +143,8 @@ struct BlockScaled : Base {
   static constexpr int SMEM_BYTES = Base::SMEM_BYTES + STAGES * SCALE_STAGE_BYTES - (Base::STAGES - STAGES) * Base::STAGE_BYTES;
   static_assert(STAGES >= 2 && SMEM_BYTES <= kSmemLimit, "block-scaled ring does not fit");
 };
-template <class Cfg, class = void>
-struct BlockScaledFlag { static constexpr bool value = false; };
 template <class Cfg>
-struct BlockScaledFlag<Cfg, decltype(void(Cfg::BLOCK_SCALED))> { static constexpr bool value = Cfg::BLOCK_SCALED; };
-template <class Cfg>
-__host__ __device__ constexpr bool block_scaled() { return BlockScaledFlag<Cfg>::value; }
+__host__ __device__ constexpr bool block_scaled() { return Cfg::BLOCK_SCALED; }
 
 // Batched 16-bit GEMM, C[b] = A[b] Bt[b]^T (libb200_batched.so): A, Bt and C are 3-D tensor maps whose third
 // coordinate is the batch, so a tile's loads are zero-filled and its stores clipped at its own matrix's edge, and a
@@ -156,14 +155,11 @@ __host__ __device__ constexpr bool block_scaled() { return BlockScaledFlag<Cfg>:
 template <class Base>
 struct Batched : Base {
   static constexpr bool BATCHED = true;
+  using Cursor = BatchCursor;
   static_assert(!Base::E4M3, "batched: 16-bit operands");
 };
-template <class Cfg, class = void>
-struct BatchedFlag { static constexpr bool value = false; };
 template <class Cfg>
-struct BatchedFlag<Cfg, decltype(void(Cfg::BATCHED))> { static constexpr bool value = Cfg::BATCHED; };
-template <class Cfg>
-__host__ __device__ constexpr bool batched() { return BatchedFlag<Cfg>::value; }
+__host__ __device__ constexpr bool batched() { return Cfg::BATCHED; }
 
 // Grouped 16-bit GEMM over contiguous row groups, C[start_g : end_g] = A[start_g : end_g] Bt[g]^T (the MoE prefill
 // layout, libb200_grouped.so): A [T, K] and C [T, N] are 2-D tensor maps, Bt [G, N, K] the batched 3-D map. The flat
@@ -175,14 +171,11 @@ __host__ __device__ constexpr bool batched() { return BatchedFlag<Cfg>::value; }
 template <class Base>
 struct Grouped : Base {
   static constexpr bool GROUPED = true;
+  using Cursor = GroupCursor;
   static_assert(!Base::E4M3, "grouped: 16-bit operands");
 };
-template <class Cfg, class = void>
-struct GroupedFlag { static constexpr bool value = false; };
 template <class Cfg>
-struct GroupedFlag<Cfg, decltype(void(Cfg::GROUPED))> { static constexpr bool value = Cfg::GROUPED; };
-template <class Cfg>
-__host__ __device__ constexpr bool grouped() { return GroupedFlag<Cfg>::value; }
+__host__ __device__ constexpr bool grouped() { return Cfg::GROUPED; }
 
 // Scales of an e4m3 launch, in device memory (null for the 16-bit operand types). Per tensor: one fp32 value each.
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
@@ -598,7 +591,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   [[maybe_unused]] const int* masked_m = kTileList ? reinterpret_cast<const int*>(splitk_ctr) : nullptr;
   // the tile list of a batched or grouped launch; an empty stand-in for the other kernels, so that their code is as
   // it was
-  using Cursor = std::conditional_t<kBatched, BatchCursor, std::conditional_t<kGrouped, GroupCursor, NoBatches>>;
+  using Cursor = typename Cfg::Cursor;
 
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x) >> 5, 0);
   const int lane = threadIdx.x & 31;
