@@ -31,6 +31,7 @@ int b200_batched_gemm(int variant, const void* A, const void* B_kmajor, void* C,
   if (const int st = host::validate(GemmType(variant), A, B_kmajor, C, Scales{nullptr, nullptr}, M, N, K, 0, B, 1,
                                     masked_m))
     return st;
+  if (tile_list::fewest_tiles<Batched>(B, M, N) > 0x7fffffffLL) return host::kBadShape;
   const dispatch::Choice ch = dispatch::select_batched(GemmType(variant), B, M, N, K);
   return tile_list::run<Batched>(variant, ch.config_id, A, B_kmajor, C, masked_m, B, M, N, K, ch.group_m, 0, stream);
 }

@@ -23,9 +23,9 @@ B200_LIST_OBJECT(Grouped);
 using b200::host::GemmType;
 
 namespace {
-// The batched rule with B = G matrices of the average group, ceil(T / G) rows.
+// The batched rule with B = G matrices of the average group, ceil(T / G) rows (in 64-bit: T + G - 1 may pass INT_MAX).
 b200::dispatch::Choice select_grouped(int variant, int G, int T, int N, int K) {
-  return b200::dispatch::select_batched(GemmType(variant), G, (T + G - 1) / G, N, K);
+  return b200::dispatch::select_batched(GemmType(variant), G, int((T + (G - 1LL)) / G), N, K);
 }
 }  // namespace
 
@@ -38,6 +38,7 @@ int b200_grouped_gemm(int variant, const void* A, const void* B_kmajor, void* C,
   // the argument rules before the lookup, which wants a valid shape (the tile count is checked with the configuration)
   if (const int st = host::validate_grouped(GemmType(variant), A, B_kmajor, C, offs, G, T, N, K, 1)) return st;
   if (T == 0) return host::kOk;
+  if (tile_list::fewest_tiles<Grouped>(G, T, N) > 0x7fffffffLL) return host::kBadShape;
   const dispatch::Choice ch = select_grouped(variant, G, T, N, K);
   return tile_list::run<Grouped>(variant, ch.config_id, A, B_kmajor, C, offs, G, T, N, K, ch.group_m, 0, stream);
 }

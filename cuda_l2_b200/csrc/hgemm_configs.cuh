@@ -179,6 +179,21 @@ int schedule_units(int count, int rows, int N, int K, const int* list, int num_s
   return n;
 }
 
+// The shortest worst-case tile list (Cursor::max_tiles) of any configuration. When it passes INT_MAX, every
+// configuration refuses the shape, so the dispatched call refuses it before the lookup.
+template <template <class> class Wrapper>
+long long fewest_tiles(int count, int rows, int N) {
+  long long fewest = 0x7fffffffffffffffLL;
+#define B200_TILES(ID, BN, STAGES, CG, CM, CN, MR)                                                               \
+  {                                                                                                             \
+    using W = Wrapper<Config<BN, STAGES, CG, true, CM, CN, MR>>;                                                \
+    fewest = std::min(fewest, W::Cursor::template max_tiles<W>(count, rows, N));                                \
+  }
+  B200_HGEMM_CONFIGS(B200_TILES)
+#undef B200_TILES
+  return fewest;
+}
+
 // The same for configuration `config_id` (fp32-accumulating fp16: the schedule does not depend on the variant).
 template <template <class> class Wrapper>
 int schedule_config(int config_id, int count, int rows, int N, int K, const int* list, int num_sms, int worker,

@@ -116,11 +116,13 @@ struct BatchCursor {
         group_m(group_m_), batch(0), first(0), m_blocks(blocks_of(0)) {}
 
   // The longest list of a launch of Cfg over num_batches matrices of M x N (host side: it bounds the workers): the
-  // dense one.
+  // dense one. 64-bit for M and N up to INT_MAX; a matrix's count is capped at 2^31 first (the launch refuses more than
+  // INT_MAX tiles anyway), so that the product with num_batches cannot overflow.
   template <class Cfg>
   static constexpr long long max_tiles(int num_batches, int M, int N) {
-    return num_batches * ((long long)((M + Cfg::TILE_M * Cfg::CLUSTER_M - 1) / (Cfg::TILE_M * Cfg::CLUSTER_M)) *
-                          ((N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N)));
+    const long long per_matrix = ((M - 1LL + Cfg::TILE_M * Cfg::CLUSTER_M) / (Cfg::TILE_M * Cfg::CLUSTER_M)) *
+                                 ((N - 1LL + Cfg::BN * Cfg::CLUSTER_N) / (Cfg::BN * Cfg::CLUSTER_N));
+    return num_batches * (per_matrix < 0x80000000LL ? per_matrix : 0x80000000LL);
   }
 
   __host__ __device__ __forceinline__ int rows_of(int b) const {
