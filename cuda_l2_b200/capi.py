@@ -16,6 +16,7 @@ LIB_DIR = Path(__file__).resolve().parent / "lib"
 _hgemm = None
 _baselines = None
 _fp8block = None
+_grouped_fp8 = None
 _tile_list_libs: dict = {}
 
 ACC_BITS = {"fp32": 32, "fp16": 16, 32: 32, 16: 16}
@@ -128,6 +129,26 @@ def grouped_lib() -> ctypes.CDLL:
     return _tile_list_lib("libb200_grouped.so", "grouped")
 
 
+def grouped_fp8_lib() -> ctypes.CDLL:
+    """libb200_grouped_fp8.so: the block-scaled e4m3 grouped GEMM over contiguous row groups
+    (include/b200_grouped_fp8.h)."""
+    global _grouped_fp8
+    if _grouped_fp8 is None:
+        lib = _load("libb200_grouped_fp8.so")
+        lib.b200_grouped_fp8_gemm.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp]
+        lib.b200_grouped_fp8_gemm.restype = _i
+        lib.b200_grouped_fp8_gemm_run_config.argtypes = [_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i,
+                                                         _i, _vp]
+        lib.b200_grouped_fp8_gemm_run_config.restype = _i
+        lib.b200_grouped_fp8_select.argtypes = [_i, _i, _i, _i, _ip, _ip]
+        lib.b200_grouped_fp8_select.restype = _i
+        lib.b200_grouped_fp8_launch_count.restype = ctypes.c_ulonglong
+        lib.b200_grouped_fp8_strerror.argtypes = [_i]
+        lib.b200_grouped_fp8_strerror.restype = ctypes.c_char_p
+        _grouped_fp8 = lib
+    return _grouped_fp8
+
+
 def baselines_lib() -> ctypes.CDLL:
     global _baselines
     if _baselines is None:
@@ -161,6 +182,10 @@ def exported_symbols() -> dict[str, list[str]]:
         ],
         "libb200_batched.so": [f"b200_batched_{suffix}" for suffix in _TILE_LIST_ABI],
         "libb200_grouped.so": [f"b200_grouped_{suffix}" for suffix in _TILE_LIST_ABI],
+        "libb200_grouped_fp8.so": [
+            "b200_grouped_fp8_gemm", "b200_grouped_fp8_gemm_run_config", "b200_grouped_fp8_select",
+            "b200_grouped_fp8_launch_count", "b200_grouped_fp8_strerror",
+        ],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
             "b200_bl_lt_autotune", "b200_bl_lt_autotune_info",
@@ -235,23 +260,29 @@ def num_k_blocks(k: int) -> int:
     return -(-k // BLOCK)
 
 
-def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None) -> str:
+def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None, groups: int | None = None) -> str:
     """torch._scaled_mm's rule for the scales of an [M,K] x [N,K] e4m3 product: two one-element fp32 tensors are
     ``"tensor"`` scales; ``scale_a`` [M,1] with ``scale_b`` [1,N], both fp32, are ``"rowwise"`` scales (one per row of A,
     one per output column); ``scale_a`` [M, nkb] with ``scale_b`` [ceil(N/128), nkb], nkb = ceil(K/128), both fp32, are
     ``"blockwise"`` scales (one per row of A and 128 k, one per 128 x 128 block of Bt). Without ``k``, any nkb the two
-    agree on is accepted. Anything else, a mix of them included, raises B200HgemmError."""
+    agree on is accepted. ``groups``: the grouped product of M = T rows by ``groups`` matrices Bt [N,K], whose only
+    scales are blockwise, with ``scale_b`` [groups, ceil(N/128), nkb]. Anything else, a mix of them included, raises
+    B200HgemmError."""
     import torch
 
     sa, sb = tuple(scale_a.shape), tuple(scale_b.shape)
+    lead = () if groups is None else (groups,)
     if scale_a.dtype == torch.float32 and scale_b.dtype == torch.float32:
-        if scale_a.numel() == 1 and scale_b.numel() == 1:
+        if groups is None and scale_a.numel() == 1 and scale_b.numel() == 1:
             return "tensor"
-        if sa == (m, 1) and sb == (1, n):
+        if groups is None and sa == (m, 1) and sb == (1, n):
             return "rowwise"
         nkb = num_k_blocks(k) if k is not None else (sa[1] if len(sa) == 2 else -1)
-        if sa == (m, nkb) and sb == (-(-n // BLOCK), nkb):
+        if sa == (m, nkb) and sb == (*lead, -(-n // BLOCK), nkb):
             return "blockwise"
+    if groups is not None:
+        raise B200HgemmError(f"grouped scales must be fp32 blockwise scales, scale_a [{m}, ceil(K/128)] with scale_b "
+                             f"[{groups}, ceil({n}/128), ceil(K/128)], got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
     raise B200HgemmError(f"scales must be fp32 and either both one-element (per tensor), scale_a [{m}, 1] with "
                          f"scale_b [1, {n}] (rowwise), or scale_a [{m}, ceil(K/128)] with scale_b [ceil({n}/128), "
                          f"ceil(K/128)] (blockwise), got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
@@ -512,11 +543,13 @@ def batched_launch_count() -> int:
 
 
 # ------------------------------------------------------------------------------------------ grouped (libb200_grouped.so)
-def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32") -> tuple[int, int, int, int]:
+def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32", out_dtype=None,
+                           scales: tuple = ()) -> tuple[int, int, int, int]:
     """(G, T, N, K) of the grouped product a[T,K] by b_kmajor[G,N,K] with the int32 group ends ``offs`` [G]
-    (``torch._grouped_mm(a, b_kmajor.transpose(-2, -1), offs=offs)``), by the rules of the 16-bit variant the dtype and
-    ``acc`` name (the 2-D rules, :meth:`GemmType.fits`). Checks shapes and dtypes only (meta tensors pass);
-    B200HgemmError otherwise."""
+    (``torch._grouped_mm(a, b_kmajor.transpose(-2, -1), offs=offs)``), by the rules of the variant the dtypes and ``acc``
+    name (the 2-D rules, :meth:`GemmType.fits`): a 16-bit one with the output dtype of the operands, or e4m3 operands
+    with ``out_dtype`` fp16 / bf16 and two blockwise ``scales`` (:func:`scale_granularity` with ``groups``). Checks
+    shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
     import torch
 
     try:
@@ -524,7 +557,12 @@ def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32") -> tuple[
     except ValueError:
         raise B200HgemmError(f"a [T, K] and b_kmajor [G, N, K] expected, got {tuple(a.shape)} and "
                              f"{tuple(b_kmajor.shape)}") from None
-    _check_k(a, b_kmajor, _operand_type(a, b_kmajor, a.dtype, acc, scaled=False), n, k, k2, "[G, N, K]")
+    typ = _operand_type(a, b_kmajor, a.dtype if out_dtype is None else out_dtype, acc, scaled=bool(scales))
+    if len(scales) != (0 if typ.scale is None else 2):
+        raise B200HgemmError(f"{a.dtype} operands take {'no' if typ.scale is None else 'two'} scales, got {len(scales)}")
+    if scales:
+        scale_granularity(t, n, *scales, k=k, groups=g)
+    _check_k(a, b_kmajor, typ, n, k, k2, "[G, N, K]")
     if offs.dtype != torch.int32 or tuple(offs.shape) != (g,):
         raise B200HgemmError(f"offs must be an int32 tensor of shape [{g}], got {offs.dtype} {tuple(offs.shape)}")
     return g, t, n, k
@@ -576,6 +614,53 @@ def grouped_schedule(config_id: int, t: int, n: int, k: int, offs, num_sms: int 
 
 def grouped_launch_count() -> int:
     return int(grouped_lib().b200_grouped_launch_count())
+
+
+def fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs, config_id: int | None = None, group_m: int = 0,
+                     max_ctas: int = 0, stream: int | None = None) -> None:
+    """c[start_g:end_g] = the block-scaled product of a[start_g:end_g] and b_kmajor[g]^T for every group g, with
+    ``float8_e4m3fn`` operands a [T,K] and b_kmajor [G,N,K] (contiguous CUDA tensors), c [T,N] fp16 or bf16, and block
+    scales read by the kernel when it runs (include/b200_grouped_fp8.h): ``scale_a`` [T, ceil(K/128)] M-major (strides
+    (1, ld_a), see :func:`blockwise_ld_a`: what ``ops.quantize_e4m3_blockwise`` returns), ``scale_b``
+    [G, ceil(N/128), ceil(K/128)] contiguous. ``offs``: an int32 CUDA tensor [G] of cumulative group ends, clamped as
+    for :func:`gemm_grouped`; rows of c at or past the last group's end are not written. ``config_id`` pins one kernel
+    configuration (tests), ``max_ctas`` caps the CTAs (0: all SMs); default is the dispatcher."""
+    import torch
+
+    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("scale_a", scale_a), ("scale_b", scale_b),
+                    ("offs", offs)):
+        if not x.is_cuda or not (x.is_contiguous() or name == "scale_a"):
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    g, t, n, k = check_grouped_operands(a, b_kmajor, offs, "fp32", c.dtype, (scale_a, scale_b))
+    if tuple(c.shape) != (t, n):
+        raise B200HgemmError(f"c must be [{t}, {n}], got {tuple(c.shape)}")
+    ld_a = blockwise_ld_a(scale_a)
+    if ld_a is None:
+        raise B200HgemmError(f"blockwise scale_a must be M-major with a row stride ld_a >= T, ld_a % 4 == 0, 16-byte "
+                             f"aligned, ceil(K/128) * ld_a floats readable; got strides {tuple(scale_a.stride())}")
+    lib = grouped_fp8_lib()
+    out_bf16 = int(c.dtype == torch.bfloat16)
+    args = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr())
+    if config_id is None:
+        st = lib.b200_grouped_fp8_gemm(*args, out_bf16, offs.data_ptr(), g, t, n, k, stream)
+    else:
+        st = lib.b200_grouped_fp8_gemm_run_config(config_id, out_bf16, *args, offs.data_ptr(), g, t, n, k, group_m,
+                                                  max_ctas, stream)
+    if st != 0:
+        raise B200HgemmError(f"b200_grouped_fp8_gemm failed: status {st} ({lib.b200_grouped_fp8_strerror(st).decode()})")
+
+
+def fp8_grouped_select(g: int, t: int, n: int, k: int) -> tuple[int, int]:
+    """(config id, rasterisation group) the block-scaled grouped dispatcher uses (b200_grouped_fp8_select)."""
+    cid, gm = ctypes.c_int(), ctypes.c_int()
+    st = grouped_fp8_lib().b200_grouped_fp8_select(g, t, n, k, ctypes.byref(cid), ctypes.byref(gm))
+    if st != 0:
+        raise B200HgemmError(f"b200_grouped_fp8_select failed: status {st}")
+    return cid.value, gm.value
+
+
+def fp8_grouped_launch_count() -> int:
+    return int(grouped_fp8_lib().b200_grouped_fp8_launch_count())
 
 
 def hgemm_config(a, b_col_major, c, config_id: int, acc: str | int = "fp32", group_m: int = 0, max_ctas: int = 0,

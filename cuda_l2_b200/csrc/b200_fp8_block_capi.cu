@@ -11,30 +11,7 @@ using b200::host::GemmType;
 namespace b200 {
 namespace block {
 
-// Two accumulator sets (the running sum and the k-block's wgmma target) fit the registers for M_REP * BN <= 128.
-constexpr bool eligible(int id) { return kConfigs[id].m_rep * kConfigs[id].bn <= 128; }
-
-// The block-scaled stand-in of configuration `id`: the same CTA group and cluster, M_REP = 1, BN = min(BN, 128).
-constexpr int sibling(int id) {
-  const ConfigDesc& c = kConfigs[id];
-  const int bn = c.bn < 128 ? c.bn : 128;
-  for (int j = 0; j < kNumConfigs; ++j) {
-    const ConfigDesc& d = kConfigs[j];
-    if (d.cta_group == c.cta_group && d.cluster_m == c.cluster_m && d.cluster_n == c.cluster_n && d.m_rep == 1 &&
-        d.bn == bn)
-      return j;
-  }
-  return -1;
-}
-constexpr bool every_config_has_an_eligible_sibling() {
-  for (int id = 0; id < kNumConfigs; ++id) {
-    const int s = sibling(id);
-    if (s < 0 || !eligible(s) || (eligible(id) && s != id)) return false;
-  }
-  return true;
-}
-static_assert(every_config_has_an_eligible_sibling(), "the configuration table lost a block-scaled sibling");
-
+// (eligible() and sibling() are in hgemm_configs.cuh.)
 // The dispatcher's `splits` code for the sibling: workspace split-K becomes cluster split-K of the largest of 8/4/2
 // not above it, stream-K the plain schedule; only configurations with split-K kernels keep a split.
 constexpr int sibling_splits(int id, int splits) {

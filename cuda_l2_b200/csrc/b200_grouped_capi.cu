@@ -22,13 +22,6 @@ B200_LIST_OBJECT(Grouped);
 
 using b200::host::GemmType;
 
-namespace {
-// The batched rule with B = G matrices of the average group, ceil(T / G) rows (in 64-bit: T + G - 1 may pass INT_MAX).
-b200::dispatch::Choice select_grouped(int variant, int G, int T, int N, int K) {
-  return b200::dispatch::select_batched(GemmType(variant), G, int((T + (G - 1LL)) / G), N, K);
-}
-}  // namespace
-
 extern "C" {
 
 int b200_grouped_gemm(int variant, const void* A, const void* B_kmajor, void* C, const int* offs, int G, int T, int N,
@@ -39,7 +32,7 @@ int b200_grouped_gemm(int variant, const void* A, const void* B_kmajor, void* C,
   if (const int st = host::validate_grouped(GemmType(variant), A, B_kmajor, C, offs, G, T, N, K, 1)) return st;
   if (T == 0) return host::kOk;
   if (tile_list::fewest_tiles<Grouped>(G, T, N) > 0x7fffffffLL) return host::kBadShape;
-  const dispatch::Choice ch = select_grouped(variant, G, T, N, K);
+  const dispatch::Choice ch = dispatch::select_grouped(GemmType(variant), G, T, N, K);
   return tile_list::run<Grouped>(variant, ch.config_id, A, B_kmajor, C, offs, G, T, N, K, ch.group_m, 0, stream);
 }
 
@@ -52,7 +45,7 @@ int b200_grouped_gemm_run_config(int variant, int config_id, const void* A, cons
 int b200_grouped_select(int variant, int G, int T, int N, int K, int* config_id, int* group_m) {
   if (!b200::tile_list::known_variant(variant)) return b200::host::kBadConfig;
   if (G <= 0 || T <= 0 || N <= 0 || K <= 0) return b200::host::kBadShape;
-  const b200::dispatch::Choice ch = select_grouped(variant, G, T, N, K);
+  const b200::dispatch::Choice ch = b200::dispatch::select_grouped(GemmType(variant), G, T, N, K);
   if (config_id) *config_id = ch.config_id;
   if (group_m) *group_m = ch.group_m;
   return 0;

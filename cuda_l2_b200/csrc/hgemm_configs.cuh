@@ -66,6 +66,36 @@ constexpr ConfigDesc kConfigs[kNumConfigs] = {
 #undef B200_DESC
 };
 
+// The block-scaled configurations (libb200_fp8block.so, libb200_grouped_fp8.so). Host code: both libraries map the
+// dispatcher's choice through the same rule.
+namespace block {
+
+// Two accumulator sets (the running sum and the k-block's wgmma target) fit the registers for M_REP * BN <= 128.
+constexpr bool eligible(int id) { return kConfigs[id].m_rep * kConfigs[id].bn <= 128; }
+
+// The block-scaled stand-in of configuration `id`: the same CTA group and cluster, M_REP = 1, BN = min(BN, 128).
+constexpr int sibling(int id) {
+  const ConfigDesc& c = kConfigs[id];
+  const int bn = c.bn < 128 ? c.bn : 128;
+  for (int j = 0; j < kNumConfigs; ++j) {
+    const ConfigDesc& d = kConfigs[j];
+    if (d.cta_group == c.cta_group && d.cluster_m == c.cluster_m && d.cluster_n == c.cluster_n && d.m_rep == 1 &&
+        d.bn == bn)
+      return j;
+  }
+  return -1;
+}
+constexpr bool every_config_has_an_eligible_sibling() {
+  for (int id = 0; id < kNumConfigs; ++id) {
+    const int s = sibling(id);
+    if (s < 0 || !eligible(s) || (eligible(id) && s != id)) return false;
+  }
+  return true;
+}
+static_assert(every_config_has_an_eligible_sibling(), "the configuration table lost a block-scaled sibling");
+
+}  // namespace block
+
 // Kernel launches the library has issued (b200_hgemm_launch_count). One counter for every translation unit of the
 // library; hidden, so that no other shared object's copy is bound to it.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_launches{0};
@@ -94,45 +124,56 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
 }
 
 // The tile-list libraries (libb200_batched.so, libb200_grouped.so): the 16-bit variants 0, 1, 2 (the GemmType index) of
-// every configuration, wrapped in Wrapper (Batched or Grouped), launched by host::launch_list.
+// every configuration, wrapped in Wrapper (Batched or Grouped), launched by host::launch_list. libb200_grouped_fp8.so:
+// the block-scaled e4m3 variants 5, 6 of the block-scaled configurations, Wrapper<BlockScaled<...>>, with their scales.
 namespace tile_list {
 
 inline bool known_variant(int v) { return v >= 0 && v <= 2; }
 
-// Kernel launches of the library that holds it (b200_batched_launch_count, b200_grouped_launch_count): one counter
-// for the library's objects; hidden, like g_launches.
+// Kernel launches of the library that holds it (b200_batched_launch_count, b200_grouped_launch_count,
+// b200_grouped_fp8_launch_count): one counter for the library's objects; hidden, like g_launches.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_list_launches{0};
 
+// A configuration without a kernel of variant T (block scales: not block::eligible) returns kBadConfig.
 template <template <class> class Wrapper, host::GemmType T>
 int run_config(int id, const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
-               int group_m, int max_ctas, cudaStream_t s) {
+               int group_m, int max_ctas, cudaStream_t s, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0) {
   constexpr host::GemmTypeTraits t = host::traits(T);
-  static_assert(!t.e4m3() && !t.scaled, "16-bit variants only");
-  int st;
+  static_assert(!t.scaled || t.block, "16-bit or block-scaled variants");
+  int st = host::kBadConfig;
   switch (id) {
 #define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
   case ID:                                                                                                     \
-    st = host::launch_list<Wrapper<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16()>>>(                  \
-        A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas);                                               \
+    if constexpr (!t.block)                                                                                    \
+      st = host::launch_list<Wrapper<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16()>>>(                \
+          A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas);                                             \
+    else if constexpr (block::eligible(ID))                                                                    \
+      st = host::launch_list<Wrapper<BlockScaled<Config<BN, STAGES, CG, true, CM, CN, MR, t.bf16(), true>>>>(  \
+          A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas, scales, ld_a);                               \
     break;
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE
     default:
-      return host::kBadConfig;
+      break;
   }
   if (st == host::kOk && rows > 0) g_list_launches.fetch_add(1, std::memory_order_relaxed);   // rows == 0: no launch
   return st;
 }
 
-// A library compiles its source once per variant (-DB200_VARIANT = 0, 1, 2), in parallel: each object instantiates
-// its own variant's 31 kernels, and the calls of the other objects' variants link against theirs. Variant 0's object
-// also holds the C entry points.
+// A library compiles its source once per variant (-DB200_VARIANT = 0, 1, 2, or 5, 6 for block scales), in parallel:
+// each object instantiates its own variant's kernels, and the calls of the other objects' variants link against
+// theirs. The first variant's object also holds the C entry points.
 #define B200_LIST_RUN(W, T)                                                                                    \
-  int run_config<W, T>(int, const void*, const void*, void*, const int*, int, int, int, int, int, int, cudaStream_t)
+  int run_config<W, T>(int, const void*, const void*, void*, const int*, int, int, int, int, int, int, cudaStream_t, \
+                       Scales, int)
 #define B200_LIST_OBJECT(W)                                                                                    \
   extern template B200_LIST_RUN(W, host::GemmType::kF16Acc32);                                                 \
   extern template B200_LIST_RUN(W, host::GemmType::kF16Acc16);                                                 \
   extern template B200_LIST_RUN(W, host::GemmType::kBF16);                                                     \
+  template B200_LIST_RUN(W, host::GemmType(B200_VARIANT))
+#define B200_BLOCK_LIST_OBJECT(W)                                                                              \
+  extern template B200_LIST_RUN(W, host::GemmType::kE4M3F16Block);                                             \
+  extern template B200_LIST_RUN(W, host::GemmType::kE4M3BF16Block);                                            \
   template B200_LIST_RUN(W, host::GemmType(B200_VARIANT))
 
 template <template <class> class Wrapper>
@@ -179,13 +220,13 @@ int schedule_units(int count, int rows, int N, int K, const int* list, int num_s
   return n;
 }
 
-// The shortest worst-case tile list (Cursor::max_tiles) of any configuration. When it passes INT_MAX, every
-// configuration refuses the shape, so the dispatched call refuses it before the lookup.
+// The shortest worst-case tile list (Cursor::max_tiles) of any configuration (block_only: of any block::eligible one).
+// When it passes INT_MAX, every configuration refuses the shape, so the dispatched call refuses it before the lookup.
 template <template <class> class Wrapper>
-long long fewest_tiles(int count, int rows, int N) {
+long long fewest_tiles(int count, int rows, int N, bool block_only = false) {
   long long fewest = 0x7fffffffffffffffLL;
 #define B200_TILES(ID, BN, STAGES, CG, CM, CN, MR)                                                               \
-  {                                                                                                             \
+  if (!block_only || block::eligible(ID)) {                                                                     \
     using W = Wrapper<Config<BN, STAGES, CG, true, CM, CN, MR>>;                                                \
     fewest = std::min(fewest, W::Cursor::template max_tiles<W>(count, rows, N));                                \
   }

@@ -600,12 +600,14 @@ Plan list_plan(long long max_tiles, int K, int max_workers, ResidentClusters&& r
 
 // The argument rules of a grouped launch: those of a 2-D [T, K] x [N, K] call (T == 0 is an empty problem and valid),
 // G >= 1 groups whose offsets (G int32 values, device memory) are non-null and 4-byte aligned, and a worst-case tile
-// list (`worst_tiles`, GroupCursor::max_tiles) of at most INT_MAX tiles.
+// list (`worst_tiles`, GroupCursor::max_tiles) of at most INT_MAX tiles. Block-scaled e4m3: the block-scale rules with
+// M = T (at least one row: ld_a >= max(T, 1)).
 inline int validate_grouped(GemmType type, const void* A, const void* Bt, const void* C, const int* offs, int groups,
-                            int T, int N, int K, long long worst_tiles) {
+                            int T, int N, int K, long long worst_tiles, Scales scales = Scales{nullptr, nullptr},
+                            int ld_a = 0) {
   if (!A || !Bt || !C || !offs) return kNullPointer;
   if (T < 0 || groups < 1) return kBadShape;
-  return validate(type, A, Bt, C, Scales{nullptr, nullptr}, T > 0 ? T : 1, N, K, 0, 1, worst_tiles, offs);
+  return validate(type, A, Bt, C, scales, T > 0 ? T : 1, N, K, ld_a, 1, worst_tiles, offs);
 }
 
 // One launch of a Batched<> or Grouped<> configuration, which walks the flat tile list of its Cfg::Cursor over
@@ -618,13 +620,16 @@ inline int validate_grouped(GemmType type, const void* A, const void* Bt, const 
 //   C [rows, N], contiguous; `list` (device memory, read by the kernel only): the cumulative group ends,
 //   end_g = clamp(list[g], start_g, rows) with start_0 = 0 and start_g = end_{g-1}. Every row of C below
 //   end_{count-1} is written once, by its own group; no other is written.
+//   Grouped<BlockScaled<>> (e4m3 operands): the same, with the block scales of the 2-D call over M = rows (`scales.a`,
+//   `ld_a`) and one [ceil(N/128), ceil(K/128)] matrix of Bt's scales per group (`scales.b`).
 template <class Cfg>
 int launch_list(const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
-                cudaStream_t stream, int group_m = 0, int max_ctas = 0) {
+                cudaStream_t stream, int group_m = 0, int max_ctas = 0, Scales scales = Scales{nullptr, nullptr},
+                int ld_a = 0) {
   static_assert(batched<Cfg>() || grouped<Cfg>(), "a Batched<> or Grouped<> configuration");
   constexpr GemmType kType = gemm_type<Cfg>();
   const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
-  int st = grouped<Cfg>() ? validate_grouped(kType, A, Bt, C, list, count, rows, N, K, tiles)
+  int st = grouped<Cfg>() ? validate_grouped(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a)
                           : validate(kType, A, Bt, C, Scales{nullptr, nullptr}, rows, N, K, 0, count, tiles, list);
   if (st != kOk || rows == 0) return st;
   const DeviceInfo& di = device_info();
@@ -632,19 +637,21 @@ int launch_list(const void* A, const void* Bt, void* C, const int* list, int cou
 
   LaunchArgs a{};
   MapCache& cache = map_cache();
-  const Elem elem = traits(kType).operand;
+  const Elem elem = traits(kType).operand, output = traits(kType).output;
   // Bt is one N x K matrix per batch or group; A and C are one matrix per batch (3-D maps, so that TMA clips each box
   // at its own matrix's edge), or the rows of all groups (2-D maps)
   const int depth = batched<Cfg>() ? count : 0;
   if ((st = cache.get(A, rows, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem, depth)) != kOk) return st;
   if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, count)) != kOk) return st;
-  if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, elem, depth)) != kOk) return st;
+  if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, depth)) != kOk) return st;
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = list_plan<Cfg>(tiles, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
   a.M = rows; a.N = N; a.K = K;
   a.group_m = group_m > 0 ? group_m : default_group_m<Cfg>();
   a.c = static_cast<__half*>(C);
   a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
+  a.scales = scales;
+  a.ld_a = ld_a;
   a.batches = count;
   a.masked_m = list;
   a.stream = stream;

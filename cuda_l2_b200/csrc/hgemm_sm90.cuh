@@ -136,7 +136,8 @@ template <class Base>
 struct BlockScaled : Base {
   static constexpr bool BLOCK_SCALED = true;
   static_assert(Base::E4M3 && Base::M_REP * Base::BN <= 128, "block scales: e4m3, and room for two accumulator sets");
-  static constexpr int SCALE_STAGE_BYTES = Base::CTA_M * 4 + 16;
+  static constexpr int SA_WINDOW_BYTES = Base::CTA_M * 4;   // A's scales of a stage; Bt's one value follows them
+  static constexpr int SCALE_STAGE_BYTES = SA_WINDOW_BYTES + 16;
   static constexpr int MAX_STAGES =
       (kSmemLimit - 1024 - Base::EPI_BYTES - Base::BAR_BYTES) / (Base::STAGE_BYTES + SCALE_STAGE_BYTES);
   static constexpr int STAGES = Base::STAGES < MAX_STAGES ? Base::STAGES : MAX_STAGES;
@@ -172,7 +173,26 @@ template <class Base>
 struct Grouped : Base {
   static constexpr bool GROUPED = true;
   using Cursor = GroupCursor;
-  static_assert(!Base::E4M3, "grouped: 16-bit operands");
+  static_assert(!Base::E4M3, "grouped: 16-bit operands, or block-scaled e4m3 (Grouped<BlockScaled<...>>)");
+};
+// Grouped block-scaled e4m3 (libb200_grouped_fp8.so): the grouped kernel with BlockScaled<>'s main loop, Bt's scales
+// [G, ceil(N/128), ceil(K/128)] read at the group's own matrix. A CTA's first row r0 = start_g + (its row block) * CTA_M
+// is any row, but the bulk copy of A's scales needs a 16-byte aligned source and size: the stage holds the aligned
+// window [r0 & ~3, min(round_up(r0 + CTA_M, 4), ld_a)), up to CTA_M + 4 values, and the consumers read row i at
+// (start_g & 3) + i (CTA_M % 4 == 0, so the shift is the group's). 16 more bytes per scale stage than BlockScaled<>,
+// whose own layout stays as it is; the ring depth is recomputed with the larger stage.
+template <class Base>
+struct Grouped<BlockScaled<Base>> : BlockScaled<Base> {
+  static constexpr bool GROUPED = true;
+  using Cursor = GroupCursor;
+  static constexpr int SA_WINDOW_BYTES = Base::CTA_M * 4 + 16;
+  static constexpr int SCALE_STAGE_BYTES = SA_WINDOW_BYTES + 16;
+  static constexpr int MAX_STAGES =
+      (kSmemLimit - 1024 - Base::EPI_BYTES - Base::BAR_BYTES) / (Base::STAGE_BYTES + SCALE_STAGE_BYTES);
+  static constexpr int STAGES = Base::STAGES < MAX_STAGES ? Base::STAGES : MAX_STAGES;
+  static constexpr int SMEM_BYTES = Base::SMEM_BYTES + STAGES * SCALE_STAGE_BYTES - (Base::STAGES - STAGES) * Base::STAGE_BYTES;
+  static_assert(STAGES >= 2 && SMEM_BYTES <= kSmemLimit, "grouped block-scaled ring does not fit");
+  static_assert(Base::CTA_M % 4 == 0, "the scale window's shift is the group's");
 };
 template <class Cfg>
 __host__ __device__ constexpr bool grouped() { return Cfg::GROUPED; }
@@ -181,8 +201,9 @@ __host__ __device__ constexpr bool grouped() { return Cfg::GROUPED; }
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
 // 16-byte aligned; C[m,n] = RN_out(fp32(fp32(acc * b[n]) * a[m])). The granularity is a run-time property of the
 // same kernels. Block-scaled kernels (BlockScaled<>): value (m, kb) of `a` at a[kb * ld_a + m] (16-byte aligned,
-// ld_a % 4 == 0), `b` row-major [ceil(N/128), ceil(K/128)]. ld_a travels in the kernel's aux_arg, not here: a member
-// added to this struct, even in its padding, changes the code ptxas emits for the other e4m3 kernels.
+// ld_a % 4 == 0), `b` row-major [ceil(N/128), ceil(K/128)] (grouped: one such matrix per group). ld_a travels in the
+// kernel's aux_arg, not here: a member added to this struct, even in its padding, changes the code ptxas emits for the
+// other e4m3 kernels.
 struct Scales { const float* a; const float* b; bool rowwise = false; };
 
 // The uniform factor applied to the finished fp32 sum before it is rounded to the output type: fp32(scale_a * scale_b)
@@ -665,10 +686,18 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         const int n0 = (tc.n_blk * CN + cn) * BN + mi * Cfg::B_BOX_ROWS;
         // block scales: this CTA's own rows of A's scales (never multicast; none past ld_a, so a padding CTA loads
         // none) and the row of Bt's scales that holds the tile (none for a tile past N)
-        [[maybe_unused]] const int sa_m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M;
-        [[maybe_unused]] const int sa_rows = kBlock ? max(0, min(Cfg::CTA_M, ld_a - sa_m0)) : 0;
+        [[maybe_unused]] int sa_m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M;
+        [[maybe_unused]] int sa_rows = kBlock ? max(0, min(Cfg::CTA_M, ld_a - sa_m0)) : 0;
         [[maybe_unused]] const int sb_n0 = (tc.n_blk * CN + cn) * BN;
         [[maybe_unused]] const float* sb_row = (kBlock && sb_n0 < N) ? scales.b + size_t(sb_n0 / 128) * num_k_blocks : nullptr;
+        if constexpr (kBlock && kGrouped) {
+          // the aligned window around the CTA's rows from the group's first row on (Grouped<BlockScaled<>>), and the
+          // scales of the group's own Bt
+          const int r0 = batches.start + sa_m0;
+          sa_m0 = r0 & ~3;
+          sa_rows = max(0, min(ld_a - sa_m0, ((r0 & 3) + Cfg::CTA_M + 3) & ~3));
+          if (sb_row) sb_row += size_t(bt.batch) * ((N + 127) / 128) * num_k_blocks;
+        }
         [[maybe_unused]] float sb_chunk = 0.f;   // lane j: Bt's scale of k-block kb0 + 32 i + j
         for (int kb = u.kb0; kb < u.kb1; ++kb) {
           mbar_wait(bar_empty + 8 * stage, phase ^ 1);
@@ -681,7 +710,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
             const uint32_t full = bar_full + 8 * stage;
             if constexpr (kBlock) {
               const uint32_t sc = smem_scales + stage * Cfg::SCALE_STAGE_BYTES;
-              st_shared_f32(sc + Cfg::CTA_M * 4, sb_kb);   // published to the consumers by the arrive below
+              st_shared_f32(sc + Cfg::SA_WINDOW_BYTES, sb_kb);   // published to the consumers by the arrive below
               mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES + uint32_t(sa_rows) * 4u);
               if (sa_rows > 0)
                 bulk_load_1d(sc, scales.a + size_t(kb) * ld_a + sa_m0, uint32_t(sa_rows) * 4u, full);
@@ -768,7 +797,13 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         // the other consumer warpgroup, out of phase with it, keeps the tensor core busy.
         static_assert(MR == 1 && Cfg::ACC_F32, "one 64-row block of fp32 accumulators per warpgroup");
         Reg part[NR];
-        const uint32_t sa_off = uint32_t(wg * 64 + wq * 16 + (lane >> 2)) * 4u;   // row l/4 of the warp's 16; +8: +32 B
+        // row l/4 of the warp's 16; +8: +32 B. Grouped: the window starts start_g & 3 rows before the CTA's first row
+        [[maybe_unused]] uint32_t sa_shift = 0;
+        if constexpr (kGrouped) {
+          batches.locate(u.tile);
+          sa_shift = uint32_t(batches.start & 3) * 4u;
+        }
+        const uint32_t sa_off = uint32_t(wg * 64 + wq * 16 + (lane >> 2)) * 4u + sa_shift;
         for (int kb = u.kb0; kb < u.kb1; ++kb) {
           mbar_wait(bar_full + 8 * stage, phase);
           const uint64_t da = make_smem_desc(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg) * (64 * kBlockK * 2));
@@ -781,7 +816,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
           wgmma_wait<0>();
           reg_fence(part);
           const uint32_t sc = smem_scales + stage * Cfg::SCALE_STAGE_BYTES;
-          const float sb = ld_shared_f32(sc + Cfg::CTA_M * 4);
+          const float sb = ld_shared_f32(sc + Cfg::SA_WINDOW_BYTES);
           const float s_lo = __fmul_rn(ld_shared_f32(sc + sa_off), sb);
           const float s_hi = __fmul_rn(ld_shared_f32(sc + sa_off + 32u), sb);
           release(stage);   // operands read by the retired group, scales in registers

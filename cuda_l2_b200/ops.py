@@ -28,6 +28,12 @@ the nearest grid shape — so deployment is a plain operator:
   scaled and accumulated in fp32 (include/b200_fp8_block.h).
 * :class:`B200Fp8Linear`: inference-only FP8 version of an ``nn.Linear`` (weight quantised once, activation per call;
   per tensor, rowwise or blockwise), or of a checkpoint's e4m3 weight and block scales (:meth:`B200Fp8Linear.from_fp8`).
+* ``torch.ops.cuda_l2_b200.fp8_grouped_gemm(a, b_kmajor, scale_a, scale_b, offs, out_dtype)``: the grouped product of
+  ``hgemm_grouped`` with e4m3 operands and block scales, ``scale_a`` [T, ceil(K/128)] (one per token and 128 input
+  channels), ``scale_b`` [G, ceil(N/128), ceil(K/128)] (each expert's ``weight_scale_inv``): the routed experts of an
+  FP8 mixture-of-experts checkpoint in one launch (include/b200_grouped_fp8.h). Inference only.
+* :class:`B200Fp8GroupedLinear`: those experts as a module, from a checkpoint's stacked e4m3 weights and block scales
+  (:meth:`B200Fp8GroupedLinear.from_fp8`) or from a 16-bit stack (:meth:`B200Fp8GroupedLinear.from_weights`).
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernel on explicitly
@@ -371,13 +377,15 @@ def quantize_e4m3_blockwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor
 def quantize_e4m3_block128x128(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
     """Per 128 x 128 block quantisation of a weight ``w`` [N, K] on its device (the layout of DeepSeek-V3-style
     checkpoints' ``weight_scale_inv``): scale [ceil(N/128), ceil(K/128)] = amax(|block|) / 448, q = e4m3(w / scale).
-    Torch ops only, no host synchronisation."""
-    n, k = w.shape
+    A stack of experts' weights [G, N, K] is quantised per expert, with scales [G, ceil(N/128), ceil(K/128)]. Torch ops
+    only, no host synchronisation."""
+    *lead, n, k = w.shape
     nnb, nkb, b = -(-n // capi.BLOCK), capi.num_k_blocks(k), capi.BLOCK
-    wb = nn.functional.pad(w.float(), (0, nkb * b - k, 0, nnb * b - n)).view(nnb, b, nkb, b)
-    scale = (wb.abs().amax(dim=(1, 3)) / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
-    q = (wb / scale[:, None, :, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(nnb * b, nkb * b)
-    return q[:n, :k].contiguous(), scale.contiguous()
+    wb = nn.functional.pad(w.float(), (0, nkb * b - k, 0, nnb * b - n)).view(*lead, nnb, b, nkb, b)
+    scale = (wb.abs().amax(dim=(-3, -1)) / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
+    q = (wb / scale[..., :, None, :, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(*lead, nnb * b,
+                                                                                                      nkb * b)
+    return q[..., :n, :k].contiguous(), scale.contiguous()
 
 
 FP8_GRANULARITIES = ("tensor", "rowwise", "blockwise")
@@ -463,5 +471,109 @@ class B200Fp8Linear(nn.Module):
                 f"out_dtype={self.out_dtype}, granularity={self.granularity}")
 
 
+# ------------------------------------------------------------------------------------------ grouped FP8 (libb200_grouped_fp8.so)
+torch.library.define(f"{_LIB}::fp8_grouped_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, "
+                     "Tensor offs, ScalarType out_dtype) -> Tensor")
+
+
+def _fp8_grouped_check(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
+    return capi.check_grouped_operands(a, b_kmajor, offs, "fp32", out_dtype, (scale_a, scale_b))
+
+
+@torch.library.impl(f"{_LIB}::fp8_grouped_gemm", "CUDA")
+def _fp8_grouped_gemm_cuda(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
+    g, t, n, _ = _fp8_grouped_check(a, b_kmajor, scale_a, scale_b, offs, out_dtype)
+    c = torch.empty((t, n), dtype=out_dtype, device=a.device)
+    if g == 0 or t == 0:
+        return c
+    a, b_kmajor, offs = a.contiguous(), b_kmajor.contiguous(), offs.contiguous()
+    scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
+    with torch.cuda.device(a.device):
+        capi.fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs,
+                              stream=torch.cuda.current_stream(a.device).cuda_stream)
+    return c
+
+
+@torch.library.impl(f"{_LIB}::fp8_grouped_gemm", "CPU")
+def _fp8_grouped_gemm_cpu(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
+    raise capi.B200HgemmError("cuda_l2_b200::fp8_grouped_gemm has no CPU implementation (and no fallback): move the "
+                              "tensors to an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::fp8_grouped_gemm")
+def _fp8_grouped_gemm_fake(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
+    _, t, n, _ = _fp8_grouped_check(a, b_kmajor, scale_a, scale_b, offs, out_dtype)
+    return a.new_empty((t, n), dtype=out_dtype)
+
+
+def _fp8_grouped_gemm_no_backward(ctx, grad_c):
+    raise capi.B200HgemmError("cuda_l2_b200::fp8_grouped_gemm is inference only: it has no gradient")
+
+
+torch.library.register_autograd(f"{_LIB}::fp8_grouped_gemm", _fp8_grouped_gemm_no_backward)
+
+
+def fp8_grouped_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
+                     offs: torch.Tensor, out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """``a`` [T,K] by ``b_kmajor`` [G,N,K], e4m3 operands with block scales, over contiguous row groups -> [T,N]
+    ``out_dtype``: rows [offs[g-1], offs[g]) of the result are the block-scaled product of those rows of ``a`` and
+    ``b_kmajor[g]^T``, in one launch. ``scale_a`` [T, ceil(K/128)] in any layout (the M-major one of
+    :func:`quantize_e4m3_blockwise` is read in place), ``scale_b`` [G, ceil(N/128), ceil(K/128)]. ``offs`` as for
+    :func:`hgemm_grouped`; rows at or past ``offs[-1]`` are unspecified. Inference only."""
+    return torch.ops.cuda_l2_b200.fp8_grouped_gemm(a, b_kmajor, scale_a, scale_b, offs, out_dtype)
+
+
+class B200Fp8GroupedLinear(nn.Module):
+    """Inference-only FP8 experts of a mixture-of-experts layer: G ``nn.Linear`` weights [N, K] without bias, stacked
+    as e4m3 ``weight_fp8`` [G, N, K] with 128 x 128 block scales ``weight_scale`` [G, ceil(N/128), ceil(K/128)]. The
+    forward takes the tokens sorted by expert, ``x`` [T, K], and the int32 cumulative group ends ``offs`` [G] on the
+    GPU, quantises ``x`` per token and 128 input channels on the device and runs ``cuda_l2_b200::fp8_grouped_gemm``:
+    no ``.item()`` and no host synchronisation, so it can be captured in a CUDA graph. Rows at or past ``offs[-1]``
+    of the result are unspecified. Needs K % 16 == 0, N % 8 == 0."""
+
+    @classmethod
+    def from_fp8(cls, weight_fp8: torch.Tensor, weight_scale_inv: torch.Tensor,
+                 out_dtype: torch.dtype = torch.bfloat16) -> "B200Fp8GroupedLinear":
+        """The experts of a checkpoint, taken as they are: the e4m3 weights [G, N, K] and their fp32 128 x 128 block
+        scales [G, ceil(N/128), ceil(K/128)] (each expert's ``weight_scale_inv``, stacked). No re-quantisation."""
+        try:
+            g, n, k = weight_fp8.shape
+        except ValueError:
+            raise capi.B200HgemmError(f"from_fp8 needs a stacked weight [G, N, K], got {list(weight_fp8.shape)}") from None
+        B200Fp8Linear._check_fits(k, n, out_dtype, f"a [{g}, {n}, {k}] weight stack")
+        want = (g, -(-n // capi.BLOCK), capi.num_k_blocks(k))
+        if weight_fp8.dtype != torch.float8_e4m3fn or weight_scale_inv.dtype != torch.float32 or \
+                tuple(weight_scale_inv.shape) != want:
+            raise capi.B200HgemmError(f"from_fp8 needs a float8_e4m3fn weight stack and fp32 block scales of shape "
+                                      f"{list(want)}, got {weight_fp8.dtype} and {weight_scale_inv.dtype} "
+                                      f"{list(weight_scale_inv.shape)}")
+        new = cls()
+        new.num_groups, new.in_features, new.out_features, new.out_dtype = g, k, n, out_dtype
+        new.register_buffer("weight_fp8", weight_fp8.contiguous())
+        new.register_buffer("weight_scale", weight_scale_inv.contiguous())
+        return new
+
+    @classmethod
+    def from_weights(cls, w: torch.Tensor) -> "B200Fp8GroupedLinear":
+        """The experts from a 16-bit weight stack ``w`` [G, N, K], quantised per 128 x 128 block; the output dtype is
+        ``w``'s."""
+        if w.dtype not in (torch.float16, torch.bfloat16) or w.dim() != 3:
+            raise capi.B200HgemmError(f"from_weights needs an fp16 / bf16 weight stack [G, N, K], got {w.dtype} "
+                                      f"{list(w.shape)}")
+        with torch.no_grad():
+            w_q, w_scale = quantize_e4m3_block128x128(w)
+        return cls.from_fp8(w_q, w_scale, w.dtype)
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+        x_q, x_scale = quantize_e4m3_blockwise(x)
+        return torch.ops.cuda_l2_b200.fp8_grouped_gemm(x_q, self.weight_fp8, x_scale, self.weight_scale, offs,
+                                                       self.out_dtype)
+
+    def extra_repr(self) -> str:
+        return (f"num_groups={self.num_groups}, in_features={self.in_features}, out_features={self.out_features}, "
+                f"out_dtype={self.out_dtype}")
+
+
 __all__ = ["hgemm", "hgemm_batched", "hgemm_grouped", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
-           "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear"]
+           "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear",
+           "fp8_grouped_gemm", "B200Fp8GroupedLinear"]
