@@ -7,6 +7,7 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
 * ``libb200_batched.so`` — the batched fp16 / bf16 GEMM (include/b200_batched.h)
 * ``libb200_grouped.so`` — the grouped fp16 / bf16 GEMM over contiguous row groups (include/b200_grouped.h)
 * ``libb200_grouped_fp8.so`` — the block-scaled FP8 grouped GEMM over contiguous row groups (include/b200_grouped_fp8.h)
+* ``libb200_batched_fp8.so`` — the block-scaled FP8 batched GEMM with per-batch row counts (include/b200_batched_fp8.h)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -127,6 +128,15 @@ def build_grouped_fp8(verbose: bool = False, force: bool = False) -> Path:
                              verbose, force)
 
 
+def build_batched_fp8(verbose: bool = False, force: bool = False) -> Path:
+    """The block-scaled e4m3 batched kernels: a library of their own, so that the device code and kernel counts of
+    libb200_batched.so and libb200_fp8block.so are unaffected. One source, compiled once per output type (17 kernels
+    each)."""
+    return _compile_and_link(LIB_DIR / "libb200_batched_fp8.so",
+                             [(CSRC / "b200_batched_fp8_capi.cu", [f"-DB200_VARIANT={v}"]) for v in BLOCK_VARIANTS],
+                             verbose, force)
+
+
 def build_baselines(verbose: bool = False, force: bool = False) -> Path:
     LIB_DIR.mkdir(exist_ok=True)
     out = LIB_DIR / "libb200_baselines.so"
@@ -150,13 +160,14 @@ def build_dev_check(verbose: bool = False, force: bool = False) -> Path:
 
 def build_all(verbose: bool = False, force: bool = False) -> dict[str, Path]:
     from concurrent.futures import ThreadPoolExecutor
-    with ThreadPoolExecutor(5) as pool:   # the block-scaled, batched and grouped libraries compile next to the product library
+    with ThreadPoolExecutor(6) as pool:   # the block-scaled, batched and grouped libraries compile next to the product library
         block = pool.submit(build_fp8block, verbose, force)
         batched = pool.submit(build_batched, verbose, force)
         grouped = pool.submit(build_grouped, verbose, force)
         grouped_fp8 = pool.submit(build_grouped_fp8, verbose, force)
+        batched_fp8 = pool.submit(build_batched_fp8, verbose, force)
         out = {"capi": build_capi(verbose, force), "fp8block": block.result(), "batched": batched.result(),
-               "grouped": grouped.result(), "grouped_fp8": grouped_fp8.result()}
+               "grouped": grouped.result(), "grouped_fp8": grouped_fp8.result(), "batched_fp8": batched_fp8.result()}
     if (CSRC / "b200_baselines_capi.cu").exists():
         out["baselines"] = build_baselines(verbose, force)
     out["dev_check"] = build_dev_check(verbose, force)

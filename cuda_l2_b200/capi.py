@@ -17,6 +17,7 @@ _hgemm = None
 _baselines = None
 _fp8block = None
 _grouped_fp8 = None
+_batched_fp8 = None
 _tile_list_libs: dict = {}
 
 ACC_BITS = {"fp32": 32, "fp16": 16, 32: 32, 16: 16}
@@ -149,6 +150,26 @@ def grouped_fp8_lib() -> ctypes.CDLL:
     return _grouped_fp8
 
 
+def batched_fp8_lib() -> ctypes.CDLL:
+    """libb200_batched_fp8.so: the block-scaled e4m3 batched GEMM with per-batch row counts on the device
+    (include/b200_batched_fp8.h)."""
+    global _batched_fp8
+    if _batched_fp8 is None:
+        lib = _load("libb200_batched_fp8.so")
+        lib.b200_batched_fp8_gemm.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp]
+        lib.b200_batched_fp8_gemm.restype = _i
+        lib.b200_batched_fp8_gemm_run_config.argtypes = [_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i,
+                                                         _i, _vp]
+        lib.b200_batched_fp8_gemm_run_config.restype = _i
+        lib.b200_batched_fp8_select.argtypes = [_i, _i, _i, _i, _ip, _ip]
+        lib.b200_batched_fp8_select.restype = _i
+        lib.b200_batched_fp8_launch_count.restype = ctypes.c_ulonglong
+        lib.b200_batched_fp8_strerror.argtypes = [_i]
+        lib.b200_batched_fp8_strerror.restype = ctypes.c_char_p
+        _batched_fp8 = lib
+    return _batched_fp8
+
+
 def baselines_lib() -> ctypes.CDLL:
     global _baselines
     if _baselines is None:
@@ -185,6 +206,10 @@ def exported_symbols() -> dict[str, list[str]]:
         "libb200_grouped_fp8.so": [
             "b200_grouped_fp8_gemm", "b200_grouped_fp8_gemm_run_config", "b200_grouped_fp8_select",
             "b200_grouped_fp8_launch_count", "b200_grouped_fp8_strerror",
+        ],
+        "libb200_batched_fp8.so": [
+            "b200_batched_fp8_gemm", "b200_batched_fp8_gemm_run_config", "b200_batched_fp8_select",
+            "b200_batched_fp8_launch_count", "b200_batched_fp8_strerror",
         ],
         "libb200_baselines.so": [
             "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
@@ -260,29 +285,37 @@ def num_k_blocks(k: int) -> int:
     return -(-k // BLOCK)
 
 
-def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None, groups: int | None = None) -> str:
+def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None, groups: int | None = None,
+                      batches: int | None = None) -> str:
     """torch._scaled_mm's rule for the scales of an [M,K] x [N,K] e4m3 product: two one-element fp32 tensors are
     ``"tensor"`` scales; ``scale_a`` [M,1] with ``scale_b`` [1,N], both fp32, are ``"rowwise"`` scales (one per row of A,
     one per output column); ``scale_a`` [M, nkb] with ``scale_b`` [ceil(N/128), nkb], nkb = ceil(K/128), both fp32, are
     ``"blockwise"`` scales (one per row of A and 128 k, one per 128 x 128 block of Bt). Without ``k``, any nkb the two
     agree on is accepted. ``groups``: the grouped product of M = T rows by ``groups`` matrices Bt [N,K], whose only
-    scales are blockwise, with ``scale_b`` [groups, ceil(N/128), nkb]. Anything else, a mix of them included, raises
-    B200HgemmError."""
+    scales are blockwise, with ``scale_b`` [groups, ceil(N/128), nkb]. ``batches``: the batched product of ``batches``
+    matrices [M,K] by as many Bt [N,K], whose only scales are blockwise, with ``scale_a`` [batches, M, nkb] and
+    ``scale_b`` [batches, ceil(N/128), nkb]. Anything else, a mix of them included, raises B200HgemmError."""
     import torch
 
     sa, sb = tuple(scale_a.shape), tuple(scale_b.shape)
-    lead = () if groups is None else (groups,)
+    lead_a = () if batches is None else (batches,)
+    lead = lead_a if groups is None else (groups,)
+    plain = groups is None and batches is None
     if scale_a.dtype == torch.float32 and scale_b.dtype == torch.float32:
-        if groups is None and scale_a.numel() == 1 and scale_b.numel() == 1:
+        if plain and scale_a.numel() == 1 and scale_b.numel() == 1:
             return "tensor"
-        if groups is None and sa == (m, 1) and sb == (1, n):
+        if plain and sa == (m, 1) and sb == (1, n):
             return "rowwise"
-        nkb = num_k_blocks(k) if k is not None else (sa[1] if len(sa) == 2 else -1)
-        if sa == (m, nkb) and sb == (*lead, -(-n // BLOCK), nkb):
+        nkb = num_k_blocks(k) if k is not None else (sa[-1] if len(sa) == 2 + len(lead_a) else -1)
+        if sa == (*lead_a, m, nkb) and sb == (*lead, -(-n // BLOCK), nkb):
             return "blockwise"
     if groups is not None:
         raise B200HgemmError(f"grouped scales must be fp32 blockwise scales, scale_a [{m}, ceil(K/128)] with scale_b "
                              f"[{groups}, ceil({n}/128), ceil(K/128)], got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
+    if batches is not None:
+        raise B200HgemmError(f"batched scales must be fp32 blockwise scales, scale_a [{batches}, {m}, ceil(K/128)] with "
+                             f"scale_b [{batches}, ceil({n}/128), ceil(K/128)], got {scale_a.dtype} {sa} and "
+                             f"{scale_b.dtype} {sb}")
     raise B200HgemmError(f"scales must be fp32 and either both one-element (per tensor), scale_a [{m}, 1] with "
                          f"scale_b [1, {n}] (rowwise), or scale_a [{m}, ceil(K/128)] with scale_b [ceil({n}/128), "
                          f"ceil(K/128)] (blockwise), got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
@@ -299,6 +332,24 @@ def blockwise_ld_a(scale_a) -> int | None:
         return None
     readable = scale_a.untyped_storage().nbytes() // 4 - scale_a.storage_offset()
     return ld if nkb * ld <= readable else None
+
+
+def batched_blockwise_ld_a(scale_a) -> int | None:
+    """The row stride ld_a with which the batched kernel can read a blockwise ``scale_a`` [B, M, nkb] in place: one
+    M-major [nkb, ld_a] block per matrix, stacked (strides (nkb * ld_a, 1, ld_a), torch's ``[B, nkb, ld_a]`` buffer
+    viewed as ``buf[:, :, :M].transpose(1, 2)``), ld_a >= M, ld_a % 4 == 0, 16-byte aligned, and B * nkb * ld_a floats
+    readable in its storage. Strides of size-1 dimensions are never stepped and do not count. None if the tensor is not
+    laid out that way."""
+    bsz, m, nkb = scale_a.shape
+    ld = scale_a.stride(2) if nkb > 1 else -(-m // 4) * 4
+    if nkb > 1 and bsz > 1 and scale_a.stride(0) != nkb * ld:
+        return None
+    if nkb == 1 and bsz > 1:   # the batch stride is the only one stepped: it is nkb * ld_a = ld_a
+        ld = scale_a.stride(0)
+    if (m > 1 and scale_a.stride(1) != 1) or ld < m or ld % 4 or scale_a.data_ptr() % 16:
+        return None
+    readable = scale_a.untyped_storage().nbytes() // 4 - scale_a.storage_offset()
+    return ld if bsz * nkb * ld <= readable else None
 
 
 def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tuple = ()) -> tuple[int, int, int]:
@@ -476,19 +527,26 @@ def batched_variant(dtype, acc: str | int = "fp32") -> int | None:
     return {(torch.float16, 32): 0, (torch.float16, 16): 1, (torch.bfloat16, 32): 2}.get((dtype, ACC_BITS.get(acc)))
 
 
-def check_batched_operands(a, b_kmajor, acc: str | int = "fp32", masked_m=None) -> tuple[int, int, int, int]:
-    """(B, M, N, K) of a[B,M,K] @ b_kmajor[B,N,K]^T per batch, by the rules of the 16-bit variant the dtype and ``acc``
-    name (the 2-D rules per matrix, :meth:`GemmType.fits`); ``masked_m``, if given, is an int32 tensor of B elements.
-    Checks shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
+def check_batched_operands(a, b_kmajor, acc: str | int = "fp32", masked_m=None, out_dtype=None,
+                           scales: tuple = ()) -> tuple[int, int, int, int]:
+    """(B, M, N, K) of a[B,M,K] @ b_kmajor[B,N,K]^T per batch, by the rules of the variant the dtypes and ``acc`` name
+    (the 2-D rules per matrix, :meth:`GemmType.fits`): a 16-bit one with the output dtype of the operands, or e4m3
+    operands with ``out_dtype`` fp16 / bf16 and two blockwise ``scales`` (:func:`scale_granularity` with ``batches``).
+    ``masked_m``, if given, is an int32 tensor of B elements. Checks shapes and dtypes only (meta tensors pass);
+    B200HgemmError otherwise."""
     import torch
 
     try:
         (bsz, m, k), (bsz2, n, k2) = a.shape, b_kmajor.shape
     except ValueError:
         raise B200HgemmError(f"3-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
-    t = _operand_type(a, b_kmajor, a.dtype, acc, scaled=False)
+    t = _operand_type(a, b_kmajor, a.dtype if out_dtype is None else out_dtype, acc, scaled=bool(scales))
+    if len(scales) != (0 if t.scale is None else 2):
+        raise B200HgemmError(f"{a.dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
     if bsz2 != bsz:
         raise B200HgemmError(f"batch counts differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}")
+    if scales:
+        scale_granularity(m, n, *scales, k=k, batches=bsz)
     _check_k(a, b_kmajor, t, n, k, k2, "[B, N, K]")
     if masked_m is not None and (masked_m.dtype != torch.int32 or tuple(masked_m.shape) != (bsz,)):
         raise B200HgemmError(f"masked_m must be an int32 tensor of shape [{bsz}], got {masked_m.dtype} "
@@ -661,6 +719,56 @@ def fp8_grouped_select(g: int, t: int, n: int, k: int) -> tuple[int, int]:
 
 def fp8_grouped_launch_count() -> int:
     return int(grouped_fp8_lib().b200_grouped_fp8_launch_count())
+
+
+def fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=None, config_id: int | None = None, group_m: int = 0,
+                     max_ctas: int = 0, stream: int | None = None) -> None:
+    """c[b] = the block-scaled product of a[b] and b_kmajor[b]^T for every b, with ``float8_e4m3fn`` operands a [B,M,K]
+    and b_kmajor [B,N,K] (contiguous CUDA tensors), c [B,M,N] fp16 or bf16, and block scales read by the kernel when
+    it runs (include/b200_batched_fp8.h): ``scale_a`` [B, M, ceil(K/128)] with one M-major block per matrix (strides
+    (nkb * ld_a, 1, ld_a), see :func:`batched_blockwise_ld_a`: what ``ops.quantize_e4m3_blockwise`` of a [B,M,K]
+    tensor returns), ``scale_b`` [B, ceil(N/128), ceil(K/128)] contiguous. ``masked_m``: an optional int32 CUDA tensor
+    [B], read by the kernel: only rows [0, clamp(masked_m[b], 0, M)) of c[b] are computed, as for
+    :func:`gemm_batched`. ``config_id`` pins one kernel configuration (tests), ``max_ctas`` caps the CTAs (0: all SMs);
+    default is the dispatcher."""
+    import torch
+
+    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("scale_a", scale_a), ("scale_b", scale_b),
+                    ("masked_m", masked_m)):
+        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name == "scale_a")):
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    bsz, m, n, k = check_batched_operands(a, b_kmajor, "fp32", masked_m, c.dtype, (scale_a, scale_b))
+    if tuple(c.shape) != (bsz, m, n):
+        raise B200HgemmError(f"c must be [{bsz}, {m}, {n}], got {tuple(c.shape)}")
+    ld_a = batched_blockwise_ld_a(scale_a)
+    if ld_a is None:
+        raise B200HgemmError(f"batched blockwise scale_a must hold one M-major block per matrix, strides "
+                             f"(ceil(K/128) * ld_a, 1, ld_a) with ld_a >= M, ld_a % 4 == 0, 16-byte aligned, "
+                             f"B * ceil(K/128) * ld_a floats readable; got strides {tuple(scale_a.stride())}")
+    lib = batched_fp8_lib()
+    out_bf16 = int(c.dtype == torch.bfloat16)
+    args = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr())
+    mm = None if masked_m is None else masked_m.data_ptr()
+    if config_id is None:
+        st = lib.b200_batched_fp8_gemm(*args, out_bf16, mm, bsz, m, n, k, stream)
+    else:
+        st = lib.b200_batched_fp8_gemm_run_config(config_id, out_bf16, *args, mm, bsz, m, n, k, group_m, max_ctas,
+                                                  stream)
+    if st != 0:
+        raise B200HgemmError(f"b200_batched_fp8_gemm failed: status {st} ({lib.b200_batched_fp8_strerror(st).decode()})")
+
+
+def fp8_batched_select(b: int, m: int, n: int, k: int) -> tuple[int, int]:
+    """(config id, rasterisation group) the block-scaled batched dispatcher uses (b200_batched_fp8_select)."""
+    cid, gm = ctypes.c_int(), ctypes.c_int()
+    st = batched_fp8_lib().b200_batched_fp8_select(b, m, n, k, ctypes.byref(cid), ctypes.byref(gm))
+    if st != 0:
+        raise B200HgemmError(f"b200_batched_fp8_select failed: status {st}")
+    return cid.value, gm.value
+
+
+def fp8_batched_launch_count() -> int:
+    return int(batched_fp8_lib().b200_batched_fp8_launch_count())
 
 
 def hgemm_config(a, b_col_major, c, config_id: int, acc: str | int = "fp32", group_m: int = 0, max_ctas: int = 0,

@@ -66,8 +66,8 @@ constexpr ConfigDesc kConfigs[kNumConfigs] = {
 #undef B200_DESC
 };
 
-// The block-scaled configurations (libb200_fp8block.so, libb200_grouped_fp8.so). Host code: both libraries map the
-// dispatcher's choice through the same rule.
+// The block-scaled configurations (libb200_fp8block.so, libb200_batched_fp8.so, libb200_grouped_fp8.so). Host code:
+// the three libraries map the dispatcher's choice through the same rule.
 namespace block {
 
 // Two accumulator sets (the running sum and the k-block's wgmma target) fit the registers for M_REP * BN <= 128.
@@ -124,14 +124,16 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
 }
 
 // The tile-list libraries (libb200_batched.so, libb200_grouped.so): the 16-bit variants 0, 1, 2 (the GemmType index) of
-// every configuration, wrapped in Wrapper (Batched or Grouped), launched by host::launch_list. libb200_grouped_fp8.so:
-// the block-scaled e4m3 variants 5, 6 of the block-scaled configurations, Wrapper<BlockScaled<...>>, with their scales.
+// every configuration, wrapped in Wrapper (Batched or Grouped), launched by host::launch_list. libb200_batched_fp8.so,
+// libb200_grouped_fp8.so: the block-scaled e4m3 variants 5, 6 of the block-scaled configurations,
+// Wrapper<BlockScaled<...>>, with their scales.
 namespace tile_list {
 
 inline bool known_variant(int v) { return v >= 0 && v <= 2; }
 
 // Kernel launches of the library that holds it (b200_batched_launch_count, b200_grouped_launch_count,
-// b200_grouped_fp8_launch_count): one counter for the library's objects; hidden, like g_launches.
+// b200_batched_fp8_launch_count, b200_grouped_fp8_launch_count): one counter for the library's objects; hidden, like
+// g_launches.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_list_launches{0};
 
 // A configuration without a kernel of variant T (block scales: not block::eligible) returns kBadConfig.
@@ -192,6 +194,23 @@ int run(int variant, int config_id, const void* A, const void* Bt, void* C, cons
                                                         max_ctas, s);
     default: return host::kBadConfig;
   }
+}
+
+// The block-scaled tile-list libraries (libb200_batched_fp8.so, libb200_grouped_fp8.so): configuration `config_id`
+// with fp16 (out_bf16 = 0) or bf16 (1) output, A's and Bt's block scales and ld_a; any other out_bf16 is kBadConfig.
+template <template <class> class Wrapper>
+int run_block(int config_id, int out_bf16, const void* A, const void* Bt, void* C, const void* scale_a, int ld_a,
+              const void* scale_b, const int* list, int count, int rows, int N, int K, int group_m, int max_ctas,
+              void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const Scales sc{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
+  if (out_bf16 == 0)
+    return run_config<Wrapper, host::GemmType::kE4M3F16Block>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
+                                                               max_ctas, s, sc, ld_a);
+  if (out_bf16 == 1)
+    return run_config<Wrapper, host::GemmType::kE4M3BF16Block>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
+                                                                max_ctas, s, sc, ld_a);
+  return host::kBadConfig;
 }
 
 // Host view of worker `worker`'s tiles, with the launcher's plan on a device of num_sms SMs (every cluster resident)

@@ -622,6 +622,9 @@ inline int validate_grouped(GemmType type, const void* A, const void* Bt, const 
 //   end_{count-1} is written once, by its own group; no other is written.
 //   Grouped<BlockScaled<>> (e4m3 operands): the same, with the block scales of the 2-D call over M = rows (`scales.a`,
 //   `ld_a`) and one [ceil(N/128), ceil(K/128)] matrix of Bt's scales per group (`scales.b`).
+//   Batched<BlockScaled<>> (e4m3 operands): the batched product, with one [ceil(K/128), ld_a] block of A's scales per
+//   matrix, stacked (value (b, m, kb) at scales.a[(b * ceil(K/128) + kb) * ld_a + m]), and one [ceil(N/128),
+//   ceil(K/128)] matrix of Bt's scales per batch (`scales.b`).
 template <class Cfg>
 int launch_list(const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
                 cudaStream_t stream, int group_m = 0, int max_ctas = 0, Scales scales = Scales{nullptr, nullptr},
@@ -630,7 +633,7 @@ int launch_list(const void* A, const void* Bt, void* C, const int* list, int cou
   constexpr GemmType kType = gemm_type<Cfg>();
   const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
   int st = grouped<Cfg>() ? validate_grouped(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a)
-                          : validate(kType, A, Bt, C, Scales{nullptr, nullptr}, rows, N, K, 0, count, tiles, list);
+                          : validate(kType, A, Bt, C, scales, rows, N, K, ld_a, count, tiles, list);
   if (st != kOk || rows == 0) return st;
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;

@@ -157,7 +157,16 @@ template <class Base>
 struct Batched : Base {
   static constexpr bool BATCHED = true;
   using Cursor = BatchCursor;
-  static_assert(!Base::E4M3, "batched: 16-bit operands");
+  static_assert(!Base::E4M3, "batched: 16-bit operands, or block-scaled e4m3 (Batched<BlockScaled<...>>)");
+};
+// Batched block-scaled e4m3 (libb200_batched_fp8.so, the MoE decode layout of an FP8 checkpoint): the batched kernel
+// with BlockScaled<>'s main loop. A's scales are one [ceil(K/128), ld_a] block per matrix, stacked, and Bt's one
+// [ceil(N/128), ceil(K/128)] matrix per batch. A CTA's first row inside its matrix is a multiple of CTA_M, so the bulk
+// copy of A's scales is aligned as in 2-D: the scale stage, the ring depth and the shared memory are BlockScaled<>'s.
+template <class Base>
+struct Batched<BlockScaled<Base>> : BlockScaled<Base> {
+  static constexpr bool BATCHED = true;
+  using Cursor = BatchCursor;
 };
 template <class Cfg>
 __host__ __device__ constexpr bool batched() { return Cfg::BATCHED; }
@@ -201,7 +210,8 @@ __host__ __device__ constexpr bool grouped() { return Cfg::GROUPED; }
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
 // 16-byte aligned; C[m,n] = RN_out(fp32(fp32(acc * b[n]) * a[m])). The granularity is a run-time property of the
 // same kernels. Block-scaled kernels (BlockScaled<>): value (m, kb) of `a` at a[kb * ld_a + m] (16-byte aligned,
-// ld_a % 4 == 0), `b` row-major [ceil(N/128), ceil(K/128)] (grouped: one such matrix per group). ld_a travels in the
+// ld_a % 4 == 0; batched: one [nkb, ld_a] block per matrix), `b` row-major [ceil(N/128), ceil(K/128)] (batched /
+// grouped: one such matrix per batch or group). ld_a travels in the
 // kernel's aux_arg, not here: a member added to this struct, even in its padding, changes the code ptxas emits for the
 // other e4m3 kernels.
 struct Scales { const float* a; const float* b; bool rowwise = false; };
@@ -691,11 +701,12 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         [[maybe_unused]] const int sb_n0 = (tc.n_blk * CN + cn) * BN;
         [[maybe_unused]] const float* sb_row = (kBlock && sb_n0 < N) ? scales.b + size_t(sb_n0 / 128) * num_k_blocks : nullptr;
         if constexpr (kBlock && kGrouped) {
-          // the aligned window around the CTA's rows from the group's first row on (Grouped<BlockScaled<>>), and the
-          // scales of the group's own Bt
+          // the aligned window around the CTA's rows from the group's first row on (Grouped<BlockScaled<>>)
           const int r0 = batches.start + sa_m0;
           sa_m0 = r0 & ~3;
           sa_rows = max(0, min(ld_a - sa_m0, ((r0 & 3) + Cfg::CTA_M + 3) & ~3));
+        }
+        if constexpr (kBlock && kTileList) {   // the scales of the batch's or group's own Bt
           if (sb_row) sb_row += size_t(bt.batch) * ((N + 127) / 128) * num_k_blocks;
         }
         [[maybe_unused]] float sb_chunk = 0.f;   // lane j: Bt's scale of k-block kb0 + 32 i + j
@@ -712,8 +723,13 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
               const uint32_t sc = smem_scales + stage * Cfg::SCALE_STAGE_BYTES;
               st_shared_f32(sc + Cfg::SA_WINDOW_BYTES, sb_kb);   // published to the consumers by the arrive below
               mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES + uint32_t(sa_rows) * 4u);
-              if (sa_rows > 0)
-                bulk_load_1d(sc, scales.a + size_t(kb) * ld_a + sa_m0, uint32_t(sa_rows) * 4u, full);
+              if (sa_rows > 0) {
+                if constexpr (kBatched)   // matrix b's [nkb, ld_a] block of A's scales (Batched<BlockScaled<>>)
+                  bulk_load_1d(sc, scales.a + (size_t(bt.batch) * num_k_blocks + kb) * ld_a + sa_m0,
+                               uint32_t(sa_rows) * 4u, full);
+                else
+                  bulk_load_1d(sc, scales.a + size_t(kb) * ld_a + sa_m0, uint32_t(sa_rows) * 4u, full);
+              }
             } else {
               mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);   // the whole stage lands here, from this CTA and its peers
             }

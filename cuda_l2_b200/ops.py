@@ -32,8 +32,13 @@ the nearest grid shape — so deployment is a plain operator:
   ``hgemm_grouped`` with e4m3 operands and block scales, ``scale_a`` [T, ceil(K/128)] (one per token and 128 input
   channels), ``scale_b`` [G, ceil(N/128), ceil(K/128)] (each expert's ``weight_scale_inv``): the routed experts of an
   FP8 mixture-of-experts checkpoint in one launch (include/b200_grouped_fp8.h). Inference only.
+* ``torch.ops.cuda_l2_b200.fp8_batched_gemm(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None)``: the batched
+  product of ``hgemm_batched`` with e4m3 operands and block scales, ``scale_a`` [B, M, ceil(K/128)], ``scale_b``
+  [B, ceil(N/128), ceil(K/128)], and the optional per-batch row counts on the GPU: the same experts in the padded
+  decode layout (include/b200_batched_fp8.h). Inference only.
 * :class:`B200Fp8GroupedLinear`: those experts as a module, from a checkpoint's stacked e4m3 weights and block scales
-  (:meth:`B200Fp8GroupedLinear.from_fp8`) or from a 16-bit stack (:meth:`B200Fp8GroupedLinear.from_weights`).
+  (:meth:`B200Fp8GroupedLinear.from_fp8`) or from a 16-bit stack (:meth:`B200Fp8GroupedLinear.from_weights`);
+  ``forward`` takes the prefill layout, ``forward_masked`` the decode layout.
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernel on explicitly
@@ -363,15 +368,19 @@ def quantize_e4m3_rowwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
 def quantize_e4m3_blockwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
     """Per 1 x 128 block quantisation of activations ``x`` [M, K] on its device: scale[m, kb] = amax(|x[m, 128 kb :
     128 kb + 128]|) / 448, q = e4m3(x / scale). The scale comes back as the M-major [M, ceil(K/128)] view the kernel
-    reads in place (strides (1, ld_a), ld_a = M rounded up to 4). Torch ops only, no host synchronisation."""
-    m, k = x.shape
+    reads in place (strides (1, ld_a), ld_a = M rounded up to 4). A batch ``x`` [B, M, K] is quantised per matrix, the
+    same way: its scale is [B, M, ceil(K/128)], a view of a [B, ceil(K/128), ld_a] buffer that the batched kernel reads
+    in place (strides (ceil(K/128) * ld_a, 1, ld_a)). Torch ops only, no host synchronisation."""
+    if x.dim() not in (2, 3):
+        raise capi.B200HgemmError(f"quantize_e4m3_blockwise takes [M, K] or [B, M, K], got {list(x.shape)}")
+    *lead, m, k = x.shape
     nkb = capi.num_k_blocks(k)
-    xb = nn.functional.pad(x.float(), (0, nkb * capi.BLOCK - k)).view(m, nkb, capi.BLOCK)
-    scale = (xb.abs().amax(dim=2) / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
-    q = (xb / scale[:, :, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(m, nkb * capi.BLOCK)
-    buf = torch.empty((nkb, -(-m // 4) * 4), dtype=torch.float32, device=x.device)
-    buf[:, :m].copy_(scale.t())
-    return q[:, :k].contiguous(), buf[:, :m].t()
+    xb = nn.functional.pad(x.float(), (0, nkb * capi.BLOCK - k)).view(*lead, m, nkb, capi.BLOCK)
+    scale = (xb.abs().amax(dim=-1) / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
+    q = (xb / scale[..., None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(*lead, m, nkb * capi.BLOCK)
+    buf = torch.empty((*lead, nkb, -(-m // 4) * 4), dtype=torch.float32, device=x.device)
+    buf[..., :m].copy_(scale.transpose(-2, -1))
+    return q[..., :k].contiguous(), buf[..., :m].transpose(-2, -1)
 
 
 def quantize_e4m3_block128x128(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
@@ -523,6 +532,72 @@ def fp8_grouped_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Ten
     return torch.ops.cuda_l2_b200.fp8_grouped_gemm(a, b_kmajor, scale_a, scale_b, offs, out_dtype)
 
 
+# ------------------------------------------------------------------------------------------ batched FP8 (libb200_batched_fp8.so)
+torch.library.define(f"{_LIB}::fp8_batched_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, "
+                     "ScalarType out_dtype, Tensor? masked_m=None) -> Tensor")
+
+
+def _fp8_batched_check(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m):
+    return capi.check_batched_operands(a, b_kmajor, "fp32", masked_m, out_dtype, (scale_a, scale_b))
+
+
+def _batched_m_major(s: torch.Tensor) -> torch.Tensor:
+    """A batched blockwise ``scale_a`` [B, M, nkb] as the kernel reads it: one M-major [nkb, ld_a] block per matrix,
+    ld_a = M rounded up to 4 (``buf[:, :, :M].transpose(1, 2)`` of a [B, nkb, ld_a] buffer), a device copy unless it is
+    already laid out so."""
+    if capi.batched_blockwise_ld_a(s) is not None:
+        return s
+    bsz, m, nkb = s.shape
+    buf = torch.empty((bsz, nkb, -(-m // 4) * 4), dtype=s.dtype, device=s.device)
+    buf[:, :, :m].copy_(s.transpose(1, 2))
+    return buf[:, :, :m].transpose(1, 2)
+
+
+@torch.library.impl(f"{_LIB}::fp8_batched_gemm", "CUDA")
+def _fp8_batched_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None):
+    bsz, m, n, _ = _fp8_batched_check(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m)
+    c = torch.empty((bsz, m, n), dtype=out_dtype, device=a.device)
+    if bsz == 0 or m == 0:
+        return c
+    a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
+    scale_a, scale_b = _batched_m_major(scale_a), _rowwise_scale_arg(scale_b)
+    if masked_m is not None:
+        masked_m = masked_m.contiguous()
+    with torch.cuda.device(a.device):
+        capi.fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=masked_m,
+                              stream=torch.cuda.current_stream(a.device).cuda_stream)
+    return c
+
+
+@torch.library.impl(f"{_LIB}::fp8_batched_gemm", "CPU")
+def _fp8_batched_gemm_cpu(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None):
+    raise capi.B200HgemmError("cuda_l2_b200::fp8_batched_gemm has no CPU implementation (and no fallback): move the "
+                              "tensors to an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::fp8_batched_gemm")
+def _fp8_batched_gemm_fake(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None):
+    bsz, m, n, _ = _fp8_batched_check(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m)
+    return a.new_empty((bsz, m, n), dtype=out_dtype)
+
+
+def _fp8_batched_gemm_no_backward(ctx, grad_c):
+    raise capi.B200HgemmError("cuda_l2_b200::fp8_batched_gemm is inference only: it has no gradient")
+
+
+torch.library.register_autograd(f"{_LIB}::fp8_batched_gemm", _fp8_batched_gemm_no_backward)
+
+
+def fp8_batched_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
+                     out_dtype: torch.dtype = torch.bfloat16, masked_m: torch.Tensor | None = None) -> torch.Tensor:
+    """``a`` [B,M,K] by ``b_kmajor`` [B,N,K] per batch, e4m3 operands with block scales -> [B,M,N] ``out_dtype``, in
+    one launch. ``scale_a`` [B, M, ceil(K/128)] in any layout (the one :func:`quantize_e4m3_blockwise` returns for a
+    [B,M,K] input is read in place), ``scale_b`` [B, ceil(N/128), ceil(K/128)]. ``masked_m``: optional int32 CUDA
+    tensor [B], read by the kernel; only rows [0, clamp(masked_m[b], 0, M)) of batch b are computed, the rest of the
+    result is unspecified (the MoE decode layout). Inference only."""
+    return torch.ops.cuda_l2_b200.fp8_batched_gemm(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m)
+
+
 class B200Fp8GroupedLinear(nn.Module):
     """Inference-only FP8 experts of a mixture-of-experts layer: G ``nn.Linear`` weights [N, K] without bias, stacked
     as e4m3 ``weight_fp8`` [G, N, K] with 128 x 128 block scales ``weight_scale`` [G, ceil(N/128), ceil(K/128)]. The
@@ -569,6 +644,16 @@ class B200Fp8GroupedLinear(nn.Module):
         return torch.ops.cuda_l2_b200.fp8_grouped_gemm(x_q, self.weight_fp8, x_scale, self.weight_scale, offs,
                                                        self.out_dtype)
 
+    def forward_masked(self, x: torch.Tensor, masked_m: torch.Tensor) -> torch.Tensor:
+        """The same experts in the padded decode layout: ``x`` [G, M, K], one fixed slot of M tokens per expert, and the
+        int32 token counts ``masked_m`` [G] on the GPU -> [G, M, N]. Rows [0, clamp(masked_m[g], 0, M)) of expert g are
+        computed; the rest of its slot in the result is unspecified. Quantises ``x`` per token and 128 input channels
+        on the device and runs ``cuda_l2_b200::fp8_batched_gemm``: no host synchronisation, so it can be captured in a
+        CUDA graph."""
+        x_q, x_scale = quantize_e4m3_blockwise(x)
+        return torch.ops.cuda_l2_b200.fp8_batched_gemm(x_q, self.weight_fp8, x_scale, self.weight_scale,
+                                                       self.out_dtype, masked_m)
+
     def extra_repr(self) -> str:
         return (f"num_groups={self.num_groups}, in_features={self.in_features}, out_features={self.out_features}, "
                 f"out_dtype={self.out_dtype}")
@@ -576,4 +661,4 @@ class B200Fp8GroupedLinear(nn.Module):
 
 __all__ = ["hgemm", "hgemm_batched", "hgemm_grouped", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear",
-           "fp8_grouped_gemm", "B200Fp8GroupedLinear"]
+           "fp8_grouped_gemm", "fp8_batched_gemm", "B200Fp8GroupedLinear"]
