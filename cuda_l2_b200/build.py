@@ -65,7 +65,8 @@ def _headers() -> list[Path]:
     return sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.inc")) + sorted((REPO / "include").glob("*.h"))
 
 
-def _compile_and_link(out: Path, objects: list[tuple[Path, list[str]]], verbose: bool, force: bool) -> Path:
+def _compile_and_link(out: Path, objects: list[tuple[Path, list[str]]], link_flags: list[str], verbose: bool,
+                      force: bool) -> Path:
     """Compiles each (source, defines) object in parallel, then links them into the shared library ``out``."""
     LIB_DIR.mkdir(exist_ok=True)
     if force or _stale(out, [src for src, _ in objects] + _headers()):
@@ -76,80 +77,44 @@ def _compile_and_link(out: Path, objects: list[tuple[Path, list[str]]], verbose:
                                   verbose)
                       for (src, defines), obj in zip(objects, objs)]:
                 f.result()
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs)], verbose)
+        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), *map(str, objs), *link_flags], verbose)
         for obj in objs:
             obj.unlink()
     return out
 
 
-def build_capi(verbose: bool = False, force: bool = False) -> Path:
-    """The 16-bit kernels (b200_hgemm_capi.cu) and the e4m3 ones (b200_fp8_capi.cu) compile in parallel, then link
-    into one library."""
-    return _compile_and_link(LIB_DIR / "libb200_hgemm.so",
-                             [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], verbose, force)
-
-
-def build_fp8block(verbose: bool = False, force: bool = False) -> Path:
-    """The block-scaled e4m3 kernels: a library of their own, so that libb200_hgemm.so's device code is unaffected."""
-    LIB_DIR.mkdir(exist_ok=True)
-    out = LIB_DIR / "libb200_fp8block.so"
-    src = CSRC / "b200_fp8_block_capi.cu"
-    if force or _stale(out, [src] + _headers()):
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), str(src)], verbose)
-    return out
-
-
 VARIANTS = (0, 1, 2)   # fp16 with fp32 accumulation, fp16 with fp16 accumulation, bf16 (the GemmType index)
-
-
-def build_batched(verbose: bool = False, force: bool = False) -> Path:
-    """The batched 16-bit kernels: a library of their own, so that libb200_hgemm.so's device code is unaffected. One
-    source, compiled once per data type (31 kernels each)."""
-    return _compile_and_link(LIB_DIR / "libb200_batched.so",
-                             [(CSRC / "b200_batched_capi.cu", [f"-DB200_VARIANT={v}"]) for v in VARIANTS], verbose, force)
-
-
-def build_grouped(verbose: bool = False, force: bool = False) -> Path:
-    """The grouped 16-bit kernels over contiguous row groups: a library of their own, so that the device code of
-    libb200_hgemm.so and libb200_batched.so is unaffected. One source, compiled once per data type (31 kernels each)."""
-    return _compile_and_link(LIB_DIR / "libb200_grouped.so",
-                             [(CSRC / "b200_grouped_capi.cu", [f"-DB200_VARIANT={v}"]) for v in VARIANTS], verbose, force)
-
-
 BLOCK_VARIANTS = (5, 6)   # block-scaled e4m3 with fp16 / bf16 output (the GemmType index)
 
 
-def build_grouped_fp8(verbose: bool = False, force: bool = False) -> Path:
-    """The block-scaled e4m3 grouped kernels: a library of their own, so that the device code and kernel counts of
-    libb200_grouped.so and libb200_fp8block.so are unaffected. One source, compiled once per output type (17 kernels
-    each)."""
-    return _compile_and_link(LIB_DIR / "libb200_grouped_fp8.so",
-                             [(CSRC / "b200_grouped_fp8_capi.cu", [f"-DB200_VARIANT={v}"]) for v in BLOCK_VARIANTS],
-                             verbose, force)
+def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, list[str]]]:
+    """One object of ``source`` per variant: each instantiates only that variant's kernels."""
+    return [(CSRC / source, [f"-DB200_VARIANT={v}"]) for v in variants]
 
 
-def build_batched_fp8(verbose: bool = False, force: bool = False) -> Path:
-    """The block-scaled e4m3 batched kernels: a library of their own, so that the device code and kernel counts of
-    libb200_batched.so and libb200_fp8block.so are unaffected. One source, compiled once per output type (17 kernels
-    each)."""
-    return _compile_and_link(LIB_DIR / "libb200_batched_fp8.so",
-                             [(CSRC / "b200_batched_fp8_capi.cu", [f"-DB200_VARIANT={v}"]) for v in BLOCK_VARIANTS],
-                             verbose, force)
+# Every library: key -> (file name, its (source, defines) objects, extra link flags). The libraries other than
+# libb200_hgemm.so hold kernels of their own, so that the device code of the others stays as it is. libb200_hgemm.so
+# compiles its 16-bit kernels (b200_hgemm_capi.cu) and its e4m3 ones (b200_fp8_capi.cu) in parallel; the tile-list
+# libraries compile one source per variant (31 kernels each for the 16-bit variants, 17 for the block-scaled ones).
+LIBRARIES = {
+    "capi": ("libb200_hgemm.so", [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], []),
+    "fp8block": ("libb200_fp8block.so", [(CSRC / "b200_fp8_block_capi.cu", [])], []),
+    "batched": ("libb200_batched.so", _per_variant("b200_batched_capi.cu", VARIANTS), []),
+    "grouped": ("libb200_grouped.so", _per_variant("b200_grouped_capi.cu", VARIANTS), []),
+    "grouped_fp8": ("libb200_grouped_fp8.so", _per_variant("b200_grouped_fp8_capi.cu", BLOCK_VARIANTS), []),
+    "batched_fp8": ("libb200_batched_fp8.so", _per_variant("b200_batched_fp8_capi.cu", BLOCK_VARIANTS), []),
+    "baselines": ("libb200_baselines.so", [(CSRC / "b200_baselines_capi.cu", [])], ["-lcublas", "-lcublasLt"]),
+}
 
 
-def build_baselines(verbose: bool = False, force: bool = False) -> Path:
-    LIB_DIR.mkdir(exist_ok=True)
-    out = LIB_DIR / "libb200_baselines.so"
-    src = CSRC / "b200_baselines_capi.cu"
-    if force or _stale(out, [src] + _headers()):
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON, "--shared", "-o", str(out), str(src), "-lcublas", "-lcublasLt"],
-             verbose)
-    return out
+def build_library(key: str, verbose: bool = False, force: bool = False) -> Path:
+    name, objects, link_flags = LIBRARIES[key]
+    return _compile_and_link(LIB_DIR / name, objects, link_flags, verbose, force)
 
 
 def build_dev_check(verbose: bool = False, force: bool = False) -> Path:
-    lib = build_capi(verbose, force)
-    build_baselines(verbose, force)
+    lib = build_library("capi", verbose, force)
+    build_library("baselines", verbose, force)
     out = LIB_DIR / "dev_check"
     src = CSRC / "dev_check.cu"
     if force or _stale(out, [src, lib] + _headers()):
@@ -159,17 +124,11 @@ def build_dev_check(verbose: bool = False, force: bool = False) -> Path:
 
 
 def build_all(verbose: bool = False, force: bool = False) -> dict[str, Path]:
+    """Every library of LIBRARIES, compiled next to each other, then dev_check."""
     from concurrent.futures import ThreadPoolExecutor
-    with ThreadPoolExecutor(6) as pool:   # the block-scaled, batched and grouped libraries compile next to the product library
-        block = pool.submit(build_fp8block, verbose, force)
-        batched = pool.submit(build_batched, verbose, force)
-        grouped = pool.submit(build_grouped, verbose, force)
-        grouped_fp8 = pool.submit(build_grouped_fp8, verbose, force)
-        batched_fp8 = pool.submit(build_batched_fp8, verbose, force)
-        out = {"capi": build_capi(verbose, force), "fp8block": block.result(), "batched": batched.result(),
-               "grouped": grouped.result(), "grouped_fp8": grouped_fp8.result(), "batched_fp8": batched_fp8.result()}
-    if (CSRC / "b200_baselines_capi.cu").exists():
-        out["baselines"] = build_baselines(verbose, force)
+    with ThreadPoolExecutor(len(LIBRARIES)) as pool:
+        futures = {key: pool.submit(build_library, key, verbose, force) for key in LIBRARIES}
+        out = {key: f.result() for key, f in futures.items()}
     out["dev_check"] = build_dev_check(verbose, force)
     return out
 

@@ -13,12 +13,6 @@ from pathlib import Path
 from typing import NamedTuple
 
 LIB_DIR = Path(__file__).resolve().parent / "lib"
-_hgemm = None
-_baselines = None
-_fp8block = None
-_grouped_fp8 = None
-_batched_fp8 = None
-_tile_list_libs: dict = {}
 
 ACC_BITS = {"fp32": 32, "fp16": 16, 32: 32, 16: 16}
 
@@ -27,77 +21,9 @@ class B200HgemmError(RuntimeError):
     pass
 
 
-def _load(name: str) -> ctypes.CDLL:
-    path = LIB_DIR / name
-    if not path.exists():
-        raise B200HgemmError(
-            f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(or `python cuda_l2_b200/build.py`). There is no fallback path.")
-    return ctypes.CDLL(str(path))
-
-
-def hgemm_lib() -> ctypes.CDLL:
-    global _hgemm
-    if _hgemm is None:
-        lib = _load("libb200_hgemm.so")
-        vp, i = ctypes.c_void_p, ctypes.c_int
-        for fn in ("b200_hgemm_f32acc", "b200_hgemm_f16acc"):
-            getattr(lib, fn).argtypes = [vp, vp, vp, vp, i, i, i, vp]
-            getattr(lib, fn).restype = i
-        lib.b200_bgemm_f32acc.argtypes = [vp, vp, vp, vp, i, i, i, vp]
-        lib.b200_bgemm_f32acc.restype = i
-        lib.b200_bgemm_run_config.argtypes = [i, vp, vp, vp, i, i, i, i, i, i, vp]
-        lib.b200_fp8gemm.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, vp]
-        lib.b200_fp8gemm.restype = i
-        lib.b200_fp8gemm_run_config.argtypes = [i, i, vp, vp, vp, vp, vp, i, i, i, i, i, i, vp]
-        lib.b200_fp8gemm_run_config.restype = i
-        lib.b200_fp8gemm_rowwise.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, vp]
-        lib.b200_fp8gemm_rowwise.restype = i
-        lib.b200_fp8gemm_rowwise_run_config.argtypes = [i, i, vp, vp, vp, vp, vp, i, i, i, i, i, i, vp]
-        lib.b200_fp8gemm_rowwise_run_config.restype = i
-        lib.b200_fp8gemm_select.argtypes = [i, i, i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
-        lib.b200_hgemm_num_configs.restype = i
-        lib.b200_hgemm_config_info.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
-        lib.b200_hgemm_config_cluster.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(i)]
-        lib.b200_hgemm_config_m_rep.argtypes = [i]
-        lib.b200_hgemm_config_stages_requested.argtypes = [i]
-        lib.b200_hgemm_select_config.argtypes = [i, i, i, i]
-        lib.b200_hgemm_select.argtypes = [i, i, i, i, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
-        lib.b200_hgemm_run_config.argtypes = [i, i, vp, vp, vp, i, i, i, i, i, i, vp]
-        lib.b200_hgemm_host.argtypes = [i, vp, vp, vp, i, i, i]
-        ip = ctypes.POINTER(i)
-        lib.b200_hgemm_schedule_units.argtypes = [i, i, i, i, i, i, i, ip, i, ip, ip, ip, ip]
-        lib.b200_hgemm_schedule_units.restype = i
-        lib.b200_hgemm_prewarm.argtypes = [vp]
-        lib.b200_hgemm_release.argtypes = []
-        lib.b200_hgemm_launch_count.restype = ctypes.c_ulonglong
-        lib.b200_hgemm_strerror.argtypes = [i]
-        lib.b200_hgemm_strerror.restype = ctypes.c_char_p
-        _hgemm = lib
-    return _hgemm
-
-
-def fp8block_lib() -> ctypes.CDLL:
-    """libb200_fp8block.so: the block-scaled e4m3 GEMM (include/b200_fp8_block.h)."""
-    global _fp8block
-    if _fp8block is None:
-        lib = _load("libb200_fp8block.so")
-        vp, i, ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
-        lib.b200_fp8gemm_blockwise.argtypes = [vp, vp, vp, vp, i, vp, i, i, i, i, vp]
-        lib.b200_fp8gemm_blockwise.restype = i
-        lib.b200_fp8gemm_blockwise_run_config.argtypes = [i, i, vp, vp, vp, vp, i, vp, i, i, i, i, i, i, vp]
-        lib.b200_fp8gemm_blockwise_run_config.restype = i
-        lib.b200_fp8gemm_blockwise_select.argtypes = [i, i, i, ip, ip, ip]
-        lib.b200_fp8gemm_blockwise_select.restype = i
-        lib.b200_fp8block_launch_count.restype = ctypes.c_ulonglong
-        lib.b200_fp8block_strerror.argtypes = [i]
-        lib.b200_fp8block_strerror.restype = ctypes.c_char_p
-        _fp8block = lib
-    return _fp8block
-
-
-# The entry points of a tile-list library (include/b200_batched.h, include/b200_grouped.h), b200_<prefix>_<suffix>, with
-# the same signatures in both: suffix -> (argtypes, restype).
+# The entry points of a tile-list library, b200_<prefix>_<suffix>, with the same signatures in both libraries of a
+# pair: suffix -> (argtypes, restype). The 16-bit pair (include/b200_batched.h, include/b200_grouped.h) and the
+# block-scaled FP8 pair (include/b200_batched_fp8.h, include/b200_grouped_fp8.h).
 _vp, _i, _ip = ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)
 _TILE_LIST_ABI = {
     "gemm": ([_i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp], _i),
@@ -107,115 +33,132 @@ _TILE_LIST_ABI = {
     "launch_count": ([], ctypes.c_ulonglong),
     "strerror": ([_i], ctypes.c_char_p),
 }
+_FP8_TILE_LIST_ABI = {
+    "gemm": ([_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp], _i),
+    "gemm_run_config": ([_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i),
+    "select": ([_i, _i, _i, _i, _ip, _ip], _i),
+    "launch_count": ([], ctypes.c_ulonglong),
+    "strerror": ([_i], ctypes.c_char_p),
+}
 
 
-def _tile_list_lib(name: str, prefix: str) -> ctypes.CDLL:
-    """The tile-list library ``name``, its entry points named b200_<prefix>_*."""
-    if name not in _tile_list_libs:
-        lib = _load(name)
-        for suffix, (args, res) in _TILE_LIST_ABI.items():
-            fn = getattr(lib, f"b200_{prefix}_{suffix}")
+def _prefixed(prefix: str, abi: dict) -> dict:
+    return {f"b200_{prefix}_{suffix}": sig for suffix, sig in abi.items()}
+
+
+# The C ABI of every library, as its header declares it: file name -> {symbol: (argtypes, restype)}. The loaders apply
+# it, exported_symbols() lists it, and build() checks each library's exports against it.
+_GEMM = ([_vp, _vp, _vp, _vp, _i, _i, _i, _vp], _i)
+_FP8GEMM = ([_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp], _i)
+_FP8GEMM_RUN_CONFIG = ([_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i)
+_BASELINE = ([_i, _i, _vp, _vp, _vp, _i, _i, _i], _i)
+ABI = {
+    "libb200_hgemm.so": {
+        "b200_hgemm_f32acc": _GEMM,
+        "b200_hgemm_f16acc": _GEMM,
+        "b200_bgemm_f32acc": _GEMM,
+        "b200_bgemm_run_config": ([_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i),
+        "b200_fp8gemm": _FP8GEMM,
+        "b200_fp8gemm_run_config": _FP8GEMM_RUN_CONFIG,
+        "b200_fp8gemm_rowwise": _FP8GEMM,
+        "b200_fp8gemm_rowwise_run_config": _FP8GEMM_RUN_CONFIG,
+        "b200_fp8gemm_select": ([_i, _i, _i, _ip, _ip, _ip], _i),
+        "b200_hgemm_num_configs": ([], _i),
+        "b200_hgemm_config_info": ([_i, _ip, _ip, _ip], _i),
+        "b200_hgemm_config_cluster": ([_i, _ip, _ip], _i),
+        "b200_hgemm_config_m_rep": ([_i], _i),
+        "b200_hgemm_config_stages_requested": ([_i], _i),
+        "b200_hgemm_select_config": ([_i, _i, _i, _i], _i),
+        "b200_hgemm_select": ([_i, _i, _i, _i, _ip, _ip, _ip], _i),
+        "b200_hgemm_run_config": ([_i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i),
+        "b200_hgemm_host": ([_i, _vp, _vp, _vp, _i, _i, _i], _i),
+        "b200_hgemm_schedule_units": ([_i, _i, _i, _i, _i, _i, _i, _ip, _i, _ip, _ip, _ip, _ip], _i),
+        "b200_hgemm_prewarm": ([_vp], _i),
+        "b200_hgemm_release": ([], _i),
+        "b200_hgemm_launch_count": ([], ctypes.c_ulonglong),
+        "b200_hgemm_strerror": ([_i], ctypes.c_char_p),
+    },
+    "libb200_fp8block.so": {
+        "b200_fp8gemm_blockwise": ([_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp], _i),
+        "b200_fp8gemm_blockwise_run_config": ([_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp], _i),
+        "b200_fp8gemm_blockwise_select": ([_i, _i, _i, _ip, _ip, _ip], _i),
+        "b200_fp8block_launch_count": ([], ctypes.c_ulonglong),
+        "b200_fp8block_strerror": ([_i], ctypes.c_char_p),
+    },
+    "libb200_batched.so": _prefixed("batched", _TILE_LIST_ABI),
+    "libb200_grouped.so": _prefixed("grouped", _TILE_LIST_ABI),
+    "libb200_grouped_fp8.so": _prefixed("grouped_fp8", _FP8_TILE_LIST_ABI),
+    "libb200_batched_fp8.so": _prefixed("batched_fp8", _FP8_TILE_LIST_ABI),
+    "libb200_baselines.so": {
+        "b200_bl_init": ([_i], _i),
+        "b200_bl_destroy": ([_i], None),
+        "b200_bl_cublas": _BASELINE,
+        "b200_bl_lt_heuristic": _BASELINE,
+        "b200_bl_lt_autotune_find": ([_i, _i, _i, _i, _i, _i, _i], _i),
+        "b200_bl_lt_autotune": _BASELINE,
+        "b200_bl_lt_autotune_info": ([_i, _i, _ip, ctypes.POINTER(ctypes.c_float)], _i),
+    },
+}
+_libs: dict = {}
+
+
+def load(name: str) -> ctypes.CDLL:
+    """The library ``name`` (a key of :data:`ABI`), loaded once with its table's argtypes and restypes applied: a
+    symbol it does not export raises."""
+    if name not in _libs:
+        path = LIB_DIR / name
+        if not path.exists():
+            raise B200HgemmError(
+                f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
+                "(or `python cuda_l2_b200/build.py`). There is no fallback path.")
+        lib = ctypes.CDLL(str(path))
+        for sym, (args, res) in ABI[name].items():
+            fn = getattr(lib, sym)
             fn.argtypes, fn.restype = args, res
-        _tile_list_libs[name] = lib
-    return _tile_list_libs[name]
+        _libs[name] = lib
+    return _libs[name]
+
+
+def hgemm_lib() -> ctypes.CDLL:
+    """libb200_hgemm.so: the 16-bit and per-tensor / rowwise e4m3 GEMMs (include/b200_hgemm.h)."""
+    return load("libb200_hgemm.so")
+
+
+def fp8block_lib() -> ctypes.CDLL:
+    """libb200_fp8block.so: the block-scaled e4m3 GEMM (include/b200_fp8_block.h)."""
+    return load("libb200_fp8block.so")
 
 
 def batched_lib() -> ctypes.CDLL:
     """libb200_batched.so: the batched fp16 / bf16 GEMM (include/b200_batched.h)."""
-    return _tile_list_lib("libb200_batched.so", "batched")
+    return load("libb200_batched.so")
 
 
 def grouped_lib() -> ctypes.CDLL:
     """libb200_grouped.so: the grouped fp16 / bf16 GEMM over contiguous row groups (include/b200_grouped.h)."""
-    return _tile_list_lib("libb200_grouped.so", "grouped")
+    return load("libb200_grouped.so")
 
 
 def grouped_fp8_lib() -> ctypes.CDLL:
     """libb200_grouped_fp8.so: the block-scaled e4m3 grouped GEMM over contiguous row groups
     (include/b200_grouped_fp8.h)."""
-    global _grouped_fp8
-    if _grouped_fp8 is None:
-        lib = _load("libb200_grouped_fp8.so")
-        lib.b200_grouped_fp8_gemm.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp]
-        lib.b200_grouped_fp8_gemm.restype = _i
-        lib.b200_grouped_fp8_gemm_run_config.argtypes = [_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i,
-                                                         _i, _vp]
-        lib.b200_grouped_fp8_gemm_run_config.restype = _i
-        lib.b200_grouped_fp8_select.argtypes = [_i, _i, _i, _i, _ip, _ip]
-        lib.b200_grouped_fp8_select.restype = _i
-        lib.b200_grouped_fp8_launch_count.restype = ctypes.c_ulonglong
-        lib.b200_grouped_fp8_strerror.argtypes = [_i]
-        lib.b200_grouped_fp8_strerror.restype = ctypes.c_char_p
-        _grouped_fp8 = lib
-    return _grouped_fp8
+    return load("libb200_grouped_fp8.so")
 
 
 def batched_fp8_lib() -> ctypes.CDLL:
     """libb200_batched_fp8.so: the block-scaled e4m3 batched GEMM with per-batch row counts on the device
     (include/b200_batched_fp8.h)."""
-    global _batched_fp8
-    if _batched_fp8 is None:
-        lib = _load("libb200_batched_fp8.so")
-        lib.b200_batched_fp8_gemm.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _vp]
-        lib.b200_batched_fp8_gemm.restype = _i
-        lib.b200_batched_fp8_gemm_run_config.argtypes = [_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i,
-                                                         _i, _vp]
-        lib.b200_batched_fp8_gemm_run_config.restype = _i
-        lib.b200_batched_fp8_select.argtypes = [_i, _i, _i, _i, _ip, _ip]
-        lib.b200_batched_fp8_select.restype = _i
-        lib.b200_batched_fp8_launch_count.restype = ctypes.c_ulonglong
-        lib.b200_batched_fp8_strerror.argtypes = [_i]
-        lib.b200_batched_fp8_strerror.restype = ctypes.c_char_p
-        _batched_fp8 = lib
-    return _batched_fp8
+    return load("libb200_batched_fp8.so")
 
 
 def baselines_lib() -> ctypes.CDLL:
-    global _baselines
-    if _baselines is None:
-        lib = _load("libb200_baselines.so")
-        vp, i = ctypes.c_void_p, ctypes.c_int
-        lib.b200_bl_init.argtypes = [i]
-        lib.b200_bl_destroy.argtypes = [i]
-        lib.b200_bl_destroy.restype = None
-        for fn in ("b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune"):
-            getattr(lib, fn).argtypes = [i, i, vp, vp, vp, i, i, i]
-        lib.b200_bl_lt_autotune_find.argtypes = [i, i, i, i, i, i, i]
-        lib.b200_bl_lt_autotune_info.argtypes = [i, i, ctypes.POINTER(i), ctypes.POINTER(ctypes.c_float)]
-        _baselines = lib
-    return _baselines
+    """libb200_baselines.so: the cuBLAS / cuBLASLt comparators (include/b200_baselines.h)."""
+    return load("libb200_baselines.so")
 
 
 def exported_symbols() -> dict[str, list[str]]:
     """Symbols each header declares — used by the CPU tests to check the libraries export all of them."""
-    return {
-        "libb200_hgemm.so": [
-            "b200_hgemm_f32acc", "b200_hgemm_f16acc", "b200_hgemm_num_configs", "b200_hgemm_config_info",
-            "b200_hgemm_config_cluster", "b200_hgemm_config_m_rep", "b200_hgemm_config_stages_requested",
-            "b200_hgemm_select_config", "b200_hgemm_select", "b200_hgemm_run_config", "b200_hgemm_host", "b200_hgemm_launch_count",
-            "b200_hgemm_strerror", "b200_hgemm_schedule_units", "b200_hgemm_prewarm", "b200_hgemm_release",
-            "b200_bgemm_f32acc", "b200_bgemm_run_config", "b200_fp8gemm", "b200_fp8gemm_run_config", "b200_fp8gemm_select",
-            "b200_fp8gemm_rowwise", "b200_fp8gemm_rowwise_run_config",
-        ],
-        "libb200_fp8block.so": [
-            "b200_fp8gemm_blockwise", "b200_fp8gemm_blockwise_run_config", "b200_fp8gemm_blockwise_select",
-            "b200_fp8block_launch_count", "b200_fp8block_strerror",
-        ],
-        "libb200_batched.so": [f"b200_batched_{suffix}" for suffix in _TILE_LIST_ABI],
-        "libb200_grouped.so": [f"b200_grouped_{suffix}" for suffix in _TILE_LIST_ABI],
-        "libb200_grouped_fp8.so": [
-            "b200_grouped_fp8_gemm", "b200_grouped_fp8_gemm_run_config", "b200_grouped_fp8_select",
-            "b200_grouped_fp8_launch_count", "b200_grouped_fp8_strerror",
-        ],
-        "libb200_batched_fp8.so": [
-            "b200_batched_fp8_gemm", "b200_batched_fp8_gemm_run_config", "b200_batched_fp8_select",
-            "b200_batched_fp8_launch_count", "b200_batched_fp8_strerror",
-        ],
-        "libb200_baselines.so": [
-            "b200_bl_init", "b200_bl_destroy", "b200_bl_cublas", "b200_bl_lt_heuristic", "b200_bl_lt_autotune_find",
-            "b200_bl_lt_autotune", "b200_bl_lt_autotune_info",
-        ],
-    }
+    return {name: list(symbols) for name, symbols in ABI.items()}
 
 
 def strerror(status: int) -> str:
@@ -322,34 +265,34 @@ def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None, gr
 
 
 def blockwise_ld_a(scale_a) -> int | None:
-    """The row stride ld_a with which the kernel can read a blockwise ``scale_a`` [M, nkb] in place: M-major (strides
+    """The row stride ld_a with which the kernels can read a blockwise ``scale_a`` [M, nkb] in place: M-major (strides
     (1, ld_a), torch's ``[nkb, ld_a]`` buffer viewed as ``buf[:, :M].t()``), ld_a >= M, ld_a % 4 == 0, 16-byte aligned,
-    and nkb * ld_a floats readable in its storage (one k-block: ld_a = M rounded up to 4). None if the tensor is not
-    laid out that way."""
-    m, nkb = scale_a.shape
-    ld = scale_a.stride(1) if nkb > 1 else -(-m // 4) * 4     # one k-block: the stride is never stepped
-    if (m > 1 and scale_a.stride(0) != 1) or ld < m or ld % 4 or scale_a.data_ptr() % 16:
-        return None
-    readable = scale_a.untyped_storage().nbytes() // 4 - scale_a.storage_offset()
-    return ld if nkb * ld <= readable else None
-
-
-def batched_blockwise_ld_a(scale_a) -> int | None:
-    """The row stride ld_a with which the batched kernel can read a blockwise ``scale_a`` [B, M, nkb] in place: one
-    M-major [nkb, ld_a] block per matrix, stacked (strides (nkb * ld_a, 1, ld_a), torch's ``[B, nkb, ld_a]`` buffer
-    viewed as ``buf[:, :, :M].transpose(1, 2)``), ld_a >= M, ld_a % 4 == 0, 16-byte aligned, and B * nkb * ld_a floats
-    readable in its storage. Strides of size-1 dimensions are never stepped and do not count. None if the tensor is not
-    laid out that way."""
-    bsz, m, nkb = scale_a.shape
-    ld = scale_a.stride(2) if nkb > 1 else -(-m // 4) * 4
-    if nkb > 1 and bsz > 1 and scale_a.stride(0) != nkb * ld:
-        return None
+    and nkb * ld_a floats readable in its storage (one k-block: ld_a = M rounded up to 4). A batched ``scale_a``
+    [B, M, nkb] holds one such block per matrix, stacked (strides (nkb * ld_a, 1, ld_a), torch's ``[B, nkb, ld_a]``
+    buffer viewed as ``buf[:, :, :M].transpose(1, 2)``), B * nkb * ld_a floats readable. Strides of size-1 dimensions
+    are never stepped and do not count. None if the tensor is not laid out that way."""
+    *lead, m, nkb = scale_a.shape
+    bsz, st = (lead[0] if lead else 1), scale_a.stride()
+    ld = st[-1] if nkb > 1 else -(-m // 4) * 4     # one k-block: the k stride is never stepped
     if nkb == 1 and bsz > 1:   # the batch stride is the only one stepped: it is nkb * ld_a = ld_a
-        ld = scale_a.stride(0)
-    if (m > 1 and scale_a.stride(1) != 1) or ld < m or ld % 4 or scale_a.data_ptr() % 16:
+        ld = st[0]
+    if (bsz > 1 and st[0] != nkb * ld) or (m > 1 and st[-2] != 1) or ld < m or ld % 4 or scale_a.data_ptr() % 16:
         return None
     readable = scale_a.untyped_storage().nbytes() // 4 - scale_a.storage_offset()
     return ld if bsz * nkb * ld <= readable else None
+
+
+batched_blockwise_ld_a = blockwise_ld_a   # the batched [B, M, nkb] form, by the name of the batched call
+
+
+def _scale_ld_a(scale_a) -> int:
+    """blockwise_ld_a of a ``scale_a`` the kernel reads in place; B200HgemmError if it cannot."""
+    ld_a = blockwise_ld_a(scale_a)
+    if ld_a is None:
+        raise B200HgemmError(f"blockwise scale_a must hold one M-major [ceil(K/128), ld_a] block per matrix (strides "
+                             f"(1, ld_a), batched (ceil(K/128) * ld_a, 1, ld_a)) with ld_a >= M, ld_a % 4 == 0, 16-byte "
+                             f"aligned, every block readable; got strides {tuple(scale_a.stride())}")
+    return ld_a
 
 
 def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tuple = ()) -> tuple[int, int, int]:
@@ -360,24 +303,24 @@ def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tupl
         (m, k), (n, k2) = a.shape, b_kmajor.shape
     except ValueError:
         raise B200HgemmError(f"2-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
-    t = _operand_type(a, b_kmajor, out_dtype, acc)
-    if len(scales) != (0 if t.scale is None else 2):
-        raise B200HgemmError(f"{a.dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
+    t = _operand_type(a, b_kmajor, out_dtype, acc, scales)
     if scales:
         scale_granularity(m, n, *scales, k=k)
     _check_k(a, b_kmajor, t, n, k, k2, "[N, K]")
     return m, n, k
 
 
-def _operand_type(a, b_kmajor, out_dtype, acc: str | int, scaled: bool = True) -> GemmType:
+def _operand_type(a, b_kmajor, out_dtype, acc: str | int, scales: tuple, scaled: bool = True) -> GemmType:
     """The variant of a @ b_kmajor^T -> ``out_dtype`` with ``acc``: operands of one dtype that name one (``scaled=False``:
-    a 16-bit one). B200HgemmError otherwise."""
+    a 16-bit one), and two ``scales`` exactly if it is scaled. B200HgemmError otherwise."""
     t = gemm_type(a.dtype, out_dtype, acc) if b_kmajor.dtype == a.dtype else None
     if t is None or (t.scale is not None and not scaled):
         kinds = "fp16 with fp32 or fp16 accumulation, bf16 with fp32"
         if scaled:
             kinds += ", e4m3 -> fp16 / bf16 with fp32"
         raise B200HgemmError(f"no kernel for {a.dtype} x {b_kmajor.dtype} -> {out_dtype} with acc={acc!r} ({kinds})")
+    if len(scales) != (0 if t.scale is None else 2):
+        raise B200HgemmError(f"{a.dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
     return t
 
 
@@ -446,10 +389,7 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     out_bf16 = int(c.dtype == torch.bfloat16)
     granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
     if granularity == "blockwise":
-        ld_a = blockwise_ld_a(scale_a)
-        if ld_a is None:
-            raise B200HgemmError(f"blockwise scale_a must be M-major with a row stride ld_a >= M, ld_a % 4 == 0, 16-byte "
-                                 f"aligned, ceil(K/128) * ld_a floats readable; got strides {tuple(scale_a.stride())}")
+        ld_a = _scale_ld_a(scale_a)
         blk = fp8block_lib()
         if config_id is None:
             st = blk.b200_fp8gemm_blockwise(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a,
@@ -476,22 +416,22 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     _check(st, "b200_fp8gemm_rowwise" if rowwise else "b200_fp8gemm")
 
 
+def _select(fn, *args) -> tuple[int, ...]:
+    """A *_select entry point's answer: ``fn`` called with ``args``, then one int out-parameter for each of its
+    remaining arguments, whose values it returns. B200HgemmError on a non-zero status."""
+    outs = [ctypes.c_int() for _ in fn.argtypes[len(args):]]
+    _check(fn(*args, *map(ctypes.byref, outs)), fn.__name__)
+    return tuple(v.value for v in outs)
+
+
 def fp8_select(m: int, n: int, k: int) -> tuple[int, int, int]:
     """(config id, rasterisation group, split-K factor) the dispatcher uses for an e4m3 problem."""
-    cid, gm, sp = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    _check(hgemm_lib().b200_fp8gemm_select(m, n, k, ctypes.byref(cid), ctypes.byref(gm), ctypes.byref(sp)),
-           "b200_fp8gemm_select")
-    return cid.value, gm.value, sp.value
+    return _select(hgemm_lib().b200_fp8gemm_select, m, n, k)
 
 
 def fp8_blockwise_select(m: int, n: int, k: int) -> tuple[int, int, int]:
     """(config id, rasterisation group, splits code) the block-scaled dispatcher uses (b200_fp8gemm_blockwise_select)."""
-    cid, gm, sp = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    lib = fp8block_lib()
-    st = lib.b200_fp8gemm_blockwise_select(m, n, k, ctypes.byref(cid), ctypes.byref(gm), ctypes.byref(sp))
-    if st != 0:
-        raise B200HgemmError(f"b200_fp8gemm_blockwise_select failed: status {st}")
-    return cid.value, gm.value, sp.value
+    return _select(fp8block_lib().b200_fp8gemm_blockwise_select, m, n, k)
 
 
 def fp8block_launch_count() -> int:
@@ -518,6 +458,49 @@ def _tile_list_schedule(schedule_units, *args) -> dict:
     return {"workers": nw.value, "units": units}
 
 
+def _tile_list_gemm(kind: str, a, b_kmajor, c, lst, acc: str | int, scales: tuple, config_id: int | None,
+                    group_m: int, max_ctas: int, stream: int | None) -> None:
+    """The call of a tile-list library: ``kind`` "batched" (``lst``: the optional row counts masked_m) or "grouped"
+    (``lst``: the group ends offs); with two blockwise ``scales`` the block-scaled FP8 library of that kind, with fp16 /
+    bf16 output as ``c``'s dtype. Every tensor is a contiguous CUDA tensor, except that scale_a is read in place
+    (:func:`blockwise_ld_a`). ``config_id`` pins one kernel configuration; default is the dispatcher."""
+    import torch
+
+    list_name = "masked_m" if kind == "batched" else "offs"
+    for name, x in zip(("a", "b_kmajor", "c", *("scale_a", "scale_b")[:len(scales)], list_name),
+                       (a, b_kmajor, c, *scales, lst)):
+        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name == "scale_a")):
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    out_dtype = c.dtype if scales else None
+    if kind == "batched":
+        count, rows, n, k = check_batched_operands(a, b_kmajor, acc, lst, out_dtype, scales)
+        c_shape = (count, rows, n)
+    else:
+        count, rows, n, k = check_grouped_operands(a, b_kmajor, lst, acc, out_dtype, scales)
+        c_shape = (rows, n)
+    want = c.dtype if scales else a.dtype
+    if c.dtype != want or tuple(c.shape) != c_shape:
+        raise B200HgemmError(f"c must be {want} {list(c_shape)}, got {c.dtype} {tuple(c.shape)}")
+    ptrs = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr())
+    if scales:   # the FP8 entry points take the scales after the operands, and the output selector after them
+        selector = int(c.dtype == torch.bfloat16)
+        ptrs += (scales[0].data_ptr(), _scale_ld_a(scales[0]), scales[1].data_ptr())
+    else:        # the 16-bit ones take the variant first
+        selector = batched_variant(a.dtype, acc)
+    prefix = f"{kind}_fp8" if scales else kind
+    lib = load(f"libb200_{prefix}.so")
+    problem = (None if lst is None else lst.data_ptr(), count, rows, n, k)
+    if config_id is None:
+        args = (*ptrs, selector) if scales else (selector, *ptrs)
+        st = getattr(lib, f"b200_{prefix}_gemm")(*args, *problem, stream)
+    else:
+        head = (config_id, selector) if scales else (selector, config_id)
+        st = getattr(lib, f"b200_{prefix}_gemm_run_config")(*head, *ptrs, *problem, group_m, max_ctas, stream)
+    if st != 0:
+        raise B200HgemmError(f"b200_{prefix}_gemm failed: status {st} "
+                             f"({getattr(lib, f'b200_{prefix}_strerror')(st).decode()})")
+
+
 # ------------------------------------------------------------------------------------------ batched (libb200_batched.so)
 def batched_variant(dtype, acc: str | int = "fp32") -> int | None:
     """The ``variant`` argument of include/b200_batched.h (the GemmType index): 0 fp16 with fp32 accumulation, 1 fp16
@@ -540,9 +523,7 @@ def check_batched_operands(a, b_kmajor, acc: str | int = "fp32", masked_m=None, 
         (bsz, m, k), (bsz2, n, k2) = a.shape, b_kmajor.shape
     except ValueError:
         raise B200HgemmError(f"3-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
-    t = _operand_type(a, b_kmajor, a.dtype if out_dtype is None else out_dtype, acc, scaled=bool(scales))
-    if len(scales) != (0 if t.scale is None else 2):
-        raise B200HgemmError(f"{a.dtype} operands take {'no' if t.scale is None else 'two'} scales, got {len(scales)}")
+    t = _operand_type(a, b_kmajor, a.dtype if out_dtype is None else out_dtype, acc, scales, scaled=bool(scales))
     if bsz2 != bsz:
         raise B200HgemmError(f"batch counts differ: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}")
     if scales:
@@ -560,31 +541,12 @@ def gemm_batched(a, b_kmajor, c, acc: str | int = "fp32", masked_m=None, stream:
     CUDA tensors ([B,M,K], [B,N,K], [B,M,N]). ``masked_m``: an optional int32 CUDA tensor [B], read by the kernel when
     it runs: only rows [0, clamp(masked_m[b], 0, M)) of c[b] are computed (include/b200_batched.h). ``config_id``
     pins one kernel configuration (tests), ``max_ctas`` caps the CTAs (0: all SMs); default is the dispatcher."""
-    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("masked_m", masked_m)):
-        if x is not None and (not x.is_cuda or not x.is_contiguous()):
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
-    bsz, m, n, k = check_batched_operands(a, b_kmajor, acc, masked_m)
-    if c.dtype != a.dtype or tuple(c.shape) != (bsz, m, n):
-        raise B200HgemmError(f"c must be {a.dtype} [{bsz}, {m}, {n}], got {c.dtype} {tuple(c.shape)}")
-    lib = batched_lib()
-    variant = batched_variant(a.dtype, acc)
-    mm = None if masked_m is None else masked_m.data_ptr()
-    if config_id is None:
-        st = lib.b200_batched_gemm(variant, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), mm, bsz, m, n, k, stream)
-    else:
-        st = lib.b200_batched_gemm_run_config(variant, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), mm,
-                                              bsz, m, n, k, group_m, max_ctas, stream)
-    if st != 0:
-        raise B200HgemmError(f"b200_batched_gemm failed: status {st} ({lib.b200_batched_strerror(st).decode()})")
+    _tile_list_gemm("batched", a, b_kmajor, c, masked_m, acc, (), config_id, group_m, max_ctas, stream)
 
 
 def batched_select(variant: int, b: int, m: int, n: int, k: int) -> tuple[int, int]:
     """(config id, rasterisation group) the batched dispatcher uses (b200_batched_select)."""
-    cid, gm = ctypes.c_int(), ctypes.c_int()
-    st = batched_lib().b200_batched_select(variant, b, m, n, k, ctypes.byref(cid), ctypes.byref(gm))
-    if st != 0:
-        raise B200HgemmError(f"b200_batched_select failed: status {st}")
-    return cid.value, gm.value
+    return _select(batched_lib().b200_batched_select, variant, b, m, n, k)
 
 
 def batched_schedule(config_id: int, b: int, m: int, n: int, k: int, masked_m=None, num_sms: int = 132) -> dict:
@@ -615,9 +577,7 @@ def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32", out_dtype
     except ValueError:
         raise B200HgemmError(f"a [T, K] and b_kmajor [G, N, K] expected, got {tuple(a.shape)} and "
                              f"{tuple(b_kmajor.shape)}") from None
-    typ = _operand_type(a, b_kmajor, a.dtype if out_dtype is None else out_dtype, acc, scaled=bool(scales))
-    if len(scales) != (0 if typ.scale is None else 2):
-        raise B200HgemmError(f"{a.dtype} operands take {'no' if typ.scale is None else 'two'} scales, got {len(scales)}")
+    typ = _operand_type(a, b_kmajor, a.dtype if out_dtype is None else out_dtype, acc, scales, scaled=bool(scales))
     if scales:
         scale_granularity(t, n, *scales, k=k, groups=g)
     _check_k(a, b_kmajor, typ, n, k, k2, "[G, N, K]")
@@ -633,31 +593,12 @@ def gemm_grouped(a, b_kmajor, c, offs, acc: str | int = "fp32", config_id: int |
     group ends, read by the kernel when it runs (clamped as include/b200_grouped.h describes); rows of c at or past the
     last group's end are not written. ``config_id`` pins one kernel configuration (tests), ``max_ctas`` caps the CTAs
     (0: all SMs); default is the dispatcher."""
-    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("offs", offs)):
-        if not x.is_cuda or not x.is_contiguous():
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
-    g, t, n, k = check_grouped_operands(a, b_kmajor, offs, acc)
-    if c.dtype != a.dtype or tuple(c.shape) != (t, n):
-        raise B200HgemmError(f"c must be {a.dtype} [{t}, {n}], got {c.dtype} {tuple(c.shape)}")
-    lib = grouped_lib()
-    variant = batched_variant(a.dtype, acc)
-    if config_id is None:
-        st = lib.b200_grouped_gemm(variant, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), offs.data_ptr(), g, t, n, k,
-                                   stream)
-    else:
-        st = lib.b200_grouped_gemm_run_config(variant, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(),
-                                              offs.data_ptr(), g, t, n, k, group_m, max_ctas, stream)
-    if st != 0:
-        raise B200HgemmError(f"b200_grouped_gemm failed: status {st} ({lib.b200_grouped_strerror(st).decode()})")
+    _tile_list_gemm("grouped", a, b_kmajor, c, offs, acc, (), config_id, group_m, max_ctas, stream)
 
 
 def grouped_select(variant: int, g: int, t: int, n: int, k: int) -> tuple[int, int]:
     """(config id, rasterisation group) the grouped dispatcher uses (b200_grouped_select)."""
-    cid, gm = ctypes.c_int(), ctypes.c_int()
-    st = grouped_lib().b200_grouped_select(variant, g, t, n, k, ctypes.byref(cid), ctypes.byref(gm))
-    if st != 0:
-        raise B200HgemmError(f"b200_grouped_select failed: status {st}")
-    return cid.value, gm.value
+    return _select(grouped_lib().b200_grouped_select, variant, g, t, n, k)
 
 
 def grouped_schedule(config_id: int, t: int, n: int, k: int, offs, num_sms: int = 132) -> dict:
@@ -683,38 +624,12 @@ def fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs, config_id: int | No
     [G, ceil(N/128), ceil(K/128)] contiguous. ``offs``: an int32 CUDA tensor [G] of cumulative group ends, clamped as
     for :func:`gemm_grouped`; rows of c at or past the last group's end are not written. ``config_id`` pins one kernel
     configuration (tests), ``max_ctas`` caps the CTAs (0: all SMs); default is the dispatcher."""
-    import torch
-
-    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("scale_a", scale_a), ("scale_b", scale_b),
-                    ("offs", offs)):
-        if not x.is_cuda or not (x.is_contiguous() or name == "scale_a"):
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
-    g, t, n, k = check_grouped_operands(a, b_kmajor, offs, "fp32", c.dtype, (scale_a, scale_b))
-    if tuple(c.shape) != (t, n):
-        raise B200HgemmError(f"c must be [{t}, {n}], got {tuple(c.shape)}")
-    ld_a = blockwise_ld_a(scale_a)
-    if ld_a is None:
-        raise B200HgemmError(f"blockwise scale_a must be M-major with a row stride ld_a >= T, ld_a % 4 == 0, 16-byte "
-                             f"aligned, ceil(K/128) * ld_a floats readable; got strides {tuple(scale_a.stride())}")
-    lib = grouped_fp8_lib()
-    out_bf16 = int(c.dtype == torch.bfloat16)
-    args = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr())
-    if config_id is None:
-        st = lib.b200_grouped_fp8_gemm(*args, out_bf16, offs.data_ptr(), g, t, n, k, stream)
-    else:
-        st = lib.b200_grouped_fp8_gemm_run_config(config_id, out_bf16, *args, offs.data_ptr(), g, t, n, k, group_m,
-                                                  max_ctas, stream)
-    if st != 0:
-        raise B200HgemmError(f"b200_grouped_fp8_gemm failed: status {st} ({lib.b200_grouped_fp8_strerror(st).decode()})")
+    _tile_list_gemm("grouped", a, b_kmajor, c, offs, "fp32", (scale_a, scale_b), config_id, group_m, max_ctas, stream)
 
 
 def fp8_grouped_select(g: int, t: int, n: int, k: int) -> tuple[int, int]:
     """(config id, rasterisation group) the block-scaled grouped dispatcher uses (b200_grouped_fp8_select)."""
-    cid, gm = ctypes.c_int(), ctypes.c_int()
-    st = grouped_fp8_lib().b200_grouped_fp8_select(g, t, n, k, ctypes.byref(cid), ctypes.byref(gm))
-    if st != 0:
-        raise B200HgemmError(f"b200_grouped_fp8_select failed: status {st}")
-    return cid.value, gm.value
+    return _select(grouped_fp8_lib().b200_grouped_fp8_select, g, t, n, k)
 
 
 def fp8_grouped_launch_count() -> int:
@@ -731,40 +646,13 @@ def fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=None, config_id:
     [B], read by the kernel: only rows [0, clamp(masked_m[b], 0, M)) of c[b] are computed, as for
     :func:`gemm_batched`. ``config_id`` pins one kernel configuration (tests), ``max_ctas`` caps the CTAs (0: all SMs);
     default is the dispatcher."""
-    import torch
-
-    for name, x in (("a", a), ("b_kmajor", b_kmajor), ("c", c), ("scale_a", scale_a), ("scale_b", scale_b),
-                    ("masked_m", masked_m)):
-        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name == "scale_a")):
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
-    bsz, m, n, k = check_batched_operands(a, b_kmajor, "fp32", masked_m, c.dtype, (scale_a, scale_b))
-    if tuple(c.shape) != (bsz, m, n):
-        raise B200HgemmError(f"c must be [{bsz}, {m}, {n}], got {tuple(c.shape)}")
-    ld_a = batched_blockwise_ld_a(scale_a)
-    if ld_a is None:
-        raise B200HgemmError(f"batched blockwise scale_a must hold one M-major block per matrix, strides "
-                             f"(ceil(K/128) * ld_a, 1, ld_a) with ld_a >= M, ld_a % 4 == 0, 16-byte aligned, "
-                             f"B * ceil(K/128) * ld_a floats readable; got strides {tuple(scale_a.stride())}")
-    lib = batched_fp8_lib()
-    out_bf16 = int(c.dtype == torch.bfloat16)
-    args = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr())
-    mm = None if masked_m is None else masked_m.data_ptr()
-    if config_id is None:
-        st = lib.b200_batched_fp8_gemm(*args, out_bf16, mm, bsz, m, n, k, stream)
-    else:
-        st = lib.b200_batched_fp8_gemm_run_config(config_id, out_bf16, *args, mm, bsz, m, n, k, group_m, max_ctas,
-                                                  stream)
-    if st != 0:
-        raise B200HgemmError(f"b200_batched_fp8_gemm failed: status {st} ({lib.b200_batched_fp8_strerror(st).decode()})")
+    _tile_list_gemm("batched", a, b_kmajor, c, masked_m, "fp32", (scale_a, scale_b), config_id, group_m, max_ctas,
+                    stream)
 
 
 def fp8_batched_select(b: int, m: int, n: int, k: int) -> tuple[int, int]:
     """(config id, rasterisation group) the block-scaled batched dispatcher uses (b200_batched_fp8_select)."""
-    cid, gm = ctypes.c_int(), ctypes.c_int()
-    st = batched_fp8_lib().b200_batched_fp8_select(b, m, n, k, ctypes.byref(cid), ctypes.byref(gm))
-    if st != 0:
-        raise B200HgemmError(f"b200_batched_fp8_select failed: status {st}")
-    return cid.value, gm.value
+    return _select(batched_fp8_lib().b200_batched_fp8_select, b, m, n, k)
 
 
 def fp8_batched_launch_count() -> int:
@@ -809,10 +697,7 @@ def select_config(acc: str | int, m: int, n: int, k: int) -> int:
 
 def select(acc: str | int, m: int, n: int, k: int) -> tuple[int, int, int]:
     """(config id, rasterisation group, split-K factor) the dispatcher uses for this problem."""
-    cid, gm, sp = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    _check(hgemm_lib().b200_hgemm_select(ACC_BITS[acc], m, n, k, ctypes.byref(cid), ctypes.byref(gm), ctypes.byref(sp)),
-           "b200_hgemm_select")
-    return cid.value, gm.value, sp.value
+    return _select(hgemm_lib().b200_hgemm_select, ACC_BITS[acc], m, n, k)
 
 
 STREAMK_TAIL, STREAMK_TAIL_PLUS_WAVE = 100, 101      # `splits` codes of b200_hgemm_run_config

@@ -1,7 +1,7 @@
 // libb200_batched.so: the batched 16-bit GEMM (include/b200_batched.h). The kernels are the family's pipeline with
 // Batched<> configurations (hgemm_sm90.cuh): 3-D tensor maps and one flat tile list over all matrices. A library of its
-// own, so that libb200_hgemm.so's device code stays as it is. The library's core is tile_list (hgemm_configs.cuh),
-// shared with libb200_grouped.so; build.py compiles this file once per data type (B200_VARIANT).
+// own, so that libb200_hgemm.so's device code stays as it is. The library's core is tile_list (hgemm_configs.cuh,
+// hgemm_dispatch.cuh), shared by the four tile-list libraries; build.py compiles this file once per data type (B200_VARIANT).
 #include "../../include/b200_batched.h"
 
 #include "hgemm_configs.cuh"
@@ -13,7 +13,7 @@
 
 namespace b200 {
 namespace tile_list {
-B200_LIST_OBJECT(Batched);
+B200_LIST_OBJECT(Batched, B200_LIST_TYPES);
 }  // namespace tile_list
 }  // namespace b200
 
@@ -27,29 +27,21 @@ int b200_batched_gemm(int variant, const void* A, const void* B_kmajor, void* C,
                       int N, int K, void* stream) {
   using namespace b200;
   if (!tile_list::known_variant(variant)) return host::kBadConfig;
-  // the argument rules before the lookup, which wants a valid shape (the tile count is checked with the configuration)
-  if (const int st = host::validate(GemmType(variant), A, B_kmajor, C, Scales{nullptr, nullptr}, M, N, K, 0, B, 1,
-                                    masked_m))
-    return st;
-  if (tile_list::fewest_tiles<Batched>(B, M, N) > 0x7fffffffLL) return host::kBadShape;
-  const dispatch::Choice ch = dispatch::select_batched(GemmType(variant), B, M, N, K);
-  return tile_list::run<Batched>(variant, ch.config_id, A, B_kmajor, C, masked_m, B, M, N, K, ch.group_m, 0, stream);
+  return tile_list::gemm(tile_list::Library{}, GemmType(variant), A, B_kmajor, C, Scales{nullptr, nullptr}, 0,
+                         masked_m, B, M, N, K, stream);
 }
 
 int b200_batched_gemm_run_config(int variant, int config_id, const void* A, const void* B_kmajor, void* C,
                                  const int* masked_m, int B, int M, int N, int K, int group_m, int max_ctas,
                                  void* stream) {
-  return b200::tile_list::run<b200::Batched>(variant, config_id, A, B_kmajor, C, masked_m, B, M, N, K, group_m,
-                                             max_ctas, stream);
+  using namespace b200;
+  return tile_list::run(tile_list::Library{}, GemmType(variant), config_id, A, B_kmajor, C, Scales{nullptr, nullptr}, 0,
+                        masked_m, B, M, N, K, group_m, max_ctas, stream);
 }
 
 int b200_batched_select(int variant, int B, int M, int N, int K, int* config_id, int* group_m) {
   if (!b200::tile_list::known_variant(variant)) return b200::host::kBadConfig;
-  if (B <= 0 || M <= 0 || N <= 0 || K <= 0) return b200::host::kBadShape;
-  const b200::dispatch::Choice ch = b200::dispatch::select_batched(GemmType(variant), B, M, N, K);
-  if (config_id) *config_id = ch.config_id;
-  if (group_m) *group_m = ch.group_m;
-  return 0;
+  return b200::tile_list::select_into<b200::Batched>(GemmType(variant), B, M, N, K, config_id, group_m);
 }
 
 int b200_batched_schedule_units(int config_id, int B, int M, int N, int K, const int* masked_m_host, int num_sms,

@@ -3,7 +3,7 @@
 // Batched<BlockScaled<>> configurations (hgemm_sm90.cuh): the 3-D maps, tile list and masked store of
 // libb200_batched.so, the per-k-block promotion of libb200_fp8block.so. A library of its own, so that the device code
 // and kernel counts of those two stay as they are. The core is tile_list (hgemm_configs.cuh, hgemm_dispatch.cuh),
-// shared with libb200_grouped_fp8.so; build.py compiles this file once per output type (B200_VARIANT = 5: fp16, 6:
+// shared by the four tile-list libraries; build.py compiles this file once per output type (B200_VARIANT = 5: fp16, 6:
 // bf16, the GemmType index).
 #include "../../include/b200_batched_fp8.h"
 
@@ -16,7 +16,7 @@
 
 namespace b200 {
 namespace tile_list {
-B200_BLOCK_LIST_OBJECT(Batched);
+B200_LIST_OBJECT(Batched, B200_BLOCK_LIST_TYPES);
 
 // The batched wrapper keeps BlockScaled<>'s scale stage, ring depth and shared memory in every configuration that has a
 // block-scaled kernel, so that each batched kernel runs the 2-D block-scaled kernel's pipeline.
@@ -54,30 +54,23 @@ int b200_batched_fp8_gemm(const void* A, const void* B_kmajor, void* C, const vo
                           const void* scale_b, int out_bf16, const int* masked_m, int B, int M, int N, int K,
                           void* stream) {
   using namespace b200;
-  if (out_bf16 != 0 && out_bf16 != 1) return host::kBadConfig;
-  // the argument rules before the lookup, which wants a valid shape (the tile count is checked with the configuration)
-  const Scales sc{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
-  if (const int st = host::validate(GemmType::kE4M3F16Block, A, B_kmajor, C, sc, M, N, K, ld_a, B, 1, masked_m))
-    return st;
-  if (tile_list::fewest_tiles<Batched>(B, M, N, true) > 0x7fffffffLL) return host::kBadShape;
-  const dispatch::Choice ch = tile_list::select_block<Batched>(B, M, N, K);
-  return tile_list::run_block<Batched>(ch.config_id, out_bf16, A, B_kmajor, C, scale_a, ld_a, scale_b, masked_m, B, M,
-                                       N, K, ch.group_m, 0, stream);
+  if (!tile_list::known_out(out_bf16)) return host::kBadConfig;
+  return tile_list::gemm(tile_list::Library{}, tile_list::block_type(out_bf16), A, B_kmajor, C,
+                         tile_list::block_scales(scale_a, scale_b), ld_a, masked_m, B, M, N, K, stream);
 }
 
 int b200_batched_fp8_gemm_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
                                      const void* scale_a, int ld_a, const void* scale_b, const int* masked_m, int B,
                                      int M, int N, int K, int group_m, int max_ctas, void* stream) {
-  return b200::tile_list::run_block<b200::Batched>(config_id, out_bf16, A, B_kmajor, C, scale_a, ld_a, scale_b,
-                                                   masked_m, B, M, N, K, group_m, max_ctas, stream);
+  using namespace b200;
+  if (!tile_list::known_out(out_bf16)) return host::kBadConfig;
+  return tile_list::run(tile_list::Library{}, tile_list::block_type(out_bf16), config_id, A, B_kmajor, C,
+                        tile_list::block_scales(scale_a, scale_b), ld_a, masked_m, B, M, N, K, group_m, max_ctas,
+                        stream);
 }
 
 int b200_batched_fp8_select(int B, int M, int N, int K, int* config_id, int* group_m) {
-  if (B <= 0 || M <= 0 || N <= 0 || K <= 0) return b200::host::kBadShape;
-  const b200::dispatch::Choice ch = b200::tile_list::select_block<b200::Batched>(B, M, N, K);
-  if (config_id) *config_id = ch.config_id;
-  if (group_m) *group_m = ch.group_m;
-  return 0;
+  return b200::tile_list::select_into<b200::Batched>(GemmType::kE4M3F16Block, B, M, N, K, config_id, group_m);
 }
 
 unsigned long long b200_batched_fp8_launch_count(void) {

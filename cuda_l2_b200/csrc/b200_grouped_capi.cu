@@ -1,8 +1,8 @@
 // libb200_grouped.so: the grouped 16-bit GEMM over contiguous row groups (include/b200_grouped.h). The kernels are the
 // family's pipeline with Grouped<> configurations (hgemm_sm90.cuh): a 2-D map over A [T, K] and C [T, N], the batched
 // 3-D map over Bt [G, N, K], and one flat tile list over the groups' own rows. A library of its own, so that the device
-// code of libb200_hgemm.so and libb200_batched.so stays as it is. The library's core is tile_list (hgemm_configs.cuh),
-// shared with libb200_batched.so; build.py compiles this file once per data type (B200_VARIANT).
+// code of libb200_hgemm.so and libb200_batched.so stays as it is. The library's core is tile_list (hgemm_configs.cuh,
+// hgemm_dispatch.cuh), shared by the four tile-list libraries; build.py compiles this file once per data type (B200_VARIANT).
 #include "../../include/b200_grouped.h"
 
 #include "hgemm_configs.cuh"
@@ -14,7 +14,7 @@
 
 namespace b200 {
 namespace tile_list {
-B200_LIST_OBJECT(Grouped);
+B200_LIST_OBJECT(Grouped, B200_LIST_TYPES);
 }  // namespace tile_list
 }  // namespace b200
 
@@ -28,27 +28,20 @@ int b200_grouped_gemm(int variant, const void* A, const void* B_kmajor, void* C,
                       int K, void* stream) {
   using namespace b200;
   if (!tile_list::known_variant(variant)) return host::kBadConfig;
-  // the argument rules before the lookup, which wants a valid shape (the tile count is checked with the configuration)
-  if (const int st = host::validate_grouped(GemmType(variant), A, B_kmajor, C, offs, G, T, N, K, 1)) return st;
-  if (T == 0) return host::kOk;
-  if (tile_list::fewest_tiles<Grouped>(G, T, N) > 0x7fffffffLL) return host::kBadShape;
-  const dispatch::Choice ch = dispatch::select_grouped(GemmType(variant), G, T, N, K);
-  return tile_list::run<Grouped>(variant, ch.config_id, A, B_kmajor, C, offs, G, T, N, K, ch.group_m, 0, stream);
+  return tile_list::gemm(tile_list::Library{}, GemmType(variant), A, B_kmajor, C, Scales{nullptr, nullptr}, 0, offs, G,
+                         T, N, K, stream);
 }
 
 int b200_grouped_gemm_run_config(int variant, int config_id, const void* A, const void* B_kmajor, void* C,
                                  const int* offs, int G, int T, int N, int K, int group_m, int max_ctas, void* stream) {
-  return b200::tile_list::run<b200::Grouped>(variant, config_id, A, B_kmajor, C, offs, G, T, N, K, group_m, max_ctas,
-                                             stream);
+  using namespace b200;
+  return tile_list::run(tile_list::Library{}, GemmType(variant), config_id, A, B_kmajor, C, Scales{nullptr, nullptr}, 0,
+                        offs, G, T, N, K, group_m, max_ctas, stream);
 }
 
 int b200_grouped_select(int variant, int G, int T, int N, int K, int* config_id, int* group_m) {
   if (!b200::tile_list::known_variant(variant)) return b200::host::kBadConfig;
-  if (G <= 0 || T <= 0 || N <= 0 || K <= 0) return b200::host::kBadShape;
-  const b200::dispatch::Choice ch = b200::dispatch::select_grouped(GemmType(variant), G, T, N, K);
-  if (config_id) *config_id = ch.config_id;
-  if (group_m) *group_m = ch.group_m;
-  return 0;
+  return b200::tile_list::select_into<b200::Grouped>(GemmType(variant), G, T, N, K, config_id, group_m);
 }
 
 int b200_grouped_schedule_units(int config_id, int G, int T, int N, int K, const int* offs_host, int num_sms,

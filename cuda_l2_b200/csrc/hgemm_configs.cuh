@@ -129,7 +129,14 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
 // Wrapper<BlockScaled<...>>, with their scales.
 namespace tile_list {
 
+// The C entry points' selectors: a 16-bit library's `variant` is the GemmType index; a block-scaled library's
+// `out_bf16` (0: fp16, 1: bf16 output) names GemmType 5 + out_bf16, and its scales arrive as untyped pointers.
 inline bool known_variant(int v) { return v >= 0 && v <= 2; }
+inline bool known_out(int out_bf16) { return out_bf16 == 0 || out_bf16 == 1; }
+inline host::GemmType block_type(int out_bf16) { return host::GemmType(int(host::GemmType::kE4M3F16Block) + out_bf16); }
+inline Scales block_scales(const void* a, const void* b) {
+  return Scales{static_cast<const float*>(a), static_cast<const float*>(b)};
+}
 
 // Kernel launches of the library that holds it (b200_batched_launch_count, b200_grouped_launch_count,
 // b200_batched_fp8_launch_count, b200_grouped_fp8_launch_count): one counter for the library's objects; hidden, like
@@ -139,7 +146,7 @@ __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_l
 // A configuration without a kernel of variant T (block scales: not block::eligible) returns kBadConfig.
 template <template <class> class Wrapper, host::GemmType T>
 int run_config(int id, const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
-               int group_m, int max_ctas, cudaStream_t s, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0) {
+               int group_m, int max_ctas, cudaStream_t s, Scales scales, int ld_a) {
   constexpr host::GemmTypeTraits t = host::traits(T);
   static_assert(!t.scaled || t.block, "16-bit or block-scaled variants");
   int st = host::kBadConfig;
@@ -162,55 +169,40 @@ int run_config(int id, const void* A, const void* Bt, void* C, const int* list, 
   return st;
 }
 
-// A library compiles its source once per variant (-DB200_VARIANT = 0, 1, 2, or 5, 6 for block scales), in parallel:
-// each object instantiates its own variant's kernels, and the calls of the other objects' variants link against
-// theirs. The first variant's object also holds the C entry points.
+// A tile-list library: its wrapper (Batched or Grouped) and its variants, the tag that run() and gemm() take.
+template <template <class> class Wrapper, host::GemmType... Types>
+struct ListLibrary {};
+
+// The variants of each kind of tile-list library, listed once as X(W, T): the 16-bit libraries hold variants 0, 1, 2
+// (the GemmType index), the block-scaled e4m3 ones 5, 6.
+#define B200_LIST_TYPES(X, W) X(W, host::GemmType::kF16Acc32) X(W, host::GemmType::kF16Acc16) X(W, host::GemmType::kBF16)
+#define B200_BLOCK_LIST_TYPES(X, W) X(W, host::GemmType::kE4M3F16Block) X(W, host::GemmType::kE4M3BF16Block)
+
+// A library compiles its source once per variant (-DB200_VARIANT), in parallel: each object instantiates its own
+// variant's kernels, and the calls of the other objects' variants link against theirs. B200_LIST_OBJECT(W, TYPES)
+// declares this and names the library `Library` (W and the variants of TYPES), so that run() can launch no other
+// variant's kernels. The first variant's object also holds the C entry points.
 #define B200_LIST_RUN(W, T)                                                                                    \
   int run_config<W, T>(int, const void*, const void*, void*, const int*, int, int, int, int, int, int, cudaStream_t, \
                        Scales, int)
-#define B200_LIST_OBJECT(W)                                                                                    \
-  extern template B200_LIST_RUN(W, host::GemmType::kF16Acc32);                                                 \
-  extern template B200_LIST_RUN(W, host::GemmType::kF16Acc16);                                                 \
-  extern template B200_LIST_RUN(W, host::GemmType::kBF16);                                                     \
-  template B200_LIST_RUN(W, host::GemmType(B200_VARIANT))
-#define B200_BLOCK_LIST_OBJECT(W)                                                                              \
-  extern template B200_LIST_RUN(W, host::GemmType::kE4M3F16Block);                                             \
-  extern template B200_LIST_RUN(W, host::GemmType::kE4M3BF16Block);                                            \
-  template B200_LIST_RUN(W, host::GemmType(B200_VARIANT))
+#define B200_LIST_EXTERN(W, T) extern template B200_LIST_RUN(W, T);
+#define B200_LIST_ARG(W, T) , T
+#define B200_LIST_OBJECT(W, TYPES)                                                                             \
+  TYPES(B200_LIST_EXTERN, W)                                                                                   \
+  template B200_LIST_RUN(W, host::GemmType(B200_VARIANT));                                                     \
+  using Library = ListLibrary<W TYPES(B200_LIST_ARG, W)>
 
-template <template <class> class Wrapper>
-int run(int variant, int config_id, const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N,
-        int K, int group_m, int max_ctas, void* stream) {
+// Configuration `config_id` of variant `type`, with the block scales and ld_a of a block-scaled variant (ignored by
+// the 16-bit ones). A variant that is not the library's own is kBadConfig.
+template <template <class> class Wrapper, host::GemmType... Types>
+int run(ListLibrary<Wrapper, Types...>, host::GemmType type, int config_id, const void* A, const void* Bt, void* C,
+        Scales scales, int ld_a, const int* list, int count, int rows, int N, int K, int group_m, int max_ctas,
+        void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  switch (variant) {
-    case 0:
-      return run_config<Wrapper, host::GemmType::kF16Acc32>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
-                                                            max_ctas, s);
-    case 1:
-      return run_config<Wrapper, host::GemmType::kF16Acc16>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
-                                                            max_ctas, s);
-    case 2:
-      return run_config<Wrapper, host::GemmType::kBF16>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
-                                                        max_ctas, s);
-    default: return host::kBadConfig;
-  }
-}
-
-// The block-scaled tile-list libraries (libb200_batched_fp8.so, libb200_grouped_fp8.so): configuration `config_id`
-// with fp16 (out_bf16 = 0) or bf16 (1) output, A's and Bt's block scales and ld_a; any other out_bf16 is kBadConfig.
-template <template <class> class Wrapper>
-int run_block(int config_id, int out_bf16, const void* A, const void* Bt, void* C, const void* scale_a, int ld_a,
-              const void* scale_b, const int* list, int count, int rows, int N, int K, int group_m, int max_ctas,
-              void* stream) {
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const Scales sc{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
-  if (out_bf16 == 0)
-    return run_config<Wrapper, host::GemmType::kE4M3F16Block>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
-                                                               max_ctas, s, sc, ld_a);
-  if (out_bf16 == 1)
-    return run_config<Wrapper, host::GemmType::kE4M3BF16Block>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
-                                                                max_ctas, s, sc, ld_a);
-  return host::kBadConfig;
+  int st = host::kBadConfig;
+  (void)((type == Types && (st = run_config<Wrapper, Types>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
+                                                            max_ctas, s, scales, ld_a), true)) || ...);
+  return st;
 }
 
 // Host view of worker `worker`'s tiles, with the launcher's plan on a device of num_sms SMs (every cluster resident)

@@ -54,6 +54,40 @@ from . import capi
 
 _LIB = "cuda_l2_b200"
 
+
+def _inference_op(name: str, schema: str, shape, launch, why: str = "") -> None:
+    """Defines the inference-only operator cuda_l2_b200::<name> with ``schema``. ``shape(*args)`` checks the arguments
+    by the kernel's rules (meta tensors pass) and returns the result's shape and dtype: the fake implementation is an
+    empty tensor of those, and the CUDA one allocates the result ``c`` on the operands' device and calls
+    ``launch(c, *args, stream=...)`` there, on torch's current stream, so that it orders with the surrounding torch ops.
+    The CPU implementation raises (there is no fallback), and so does a backward through it (``why`` says why)."""
+    qualname = f"{_LIB}::{name}"
+    torch.library.define(qualname, schema)
+
+    def cuda(*args):
+        out_shape, dtype = shape(*args)
+        c = torch.empty(out_shape, dtype=dtype, device=args[0].device)
+        with torch.cuda.device(c.device):
+            launch(c, *args, stream=torch.cuda.current_stream(c.device).cuda_stream)
+        return c
+
+    def cpu(*args):
+        raise capi.B200HgemmError(f"{qualname} has no CPU implementation (and no fallback): move the tensors to an H100")
+
+    def fake(*args):
+        out_shape, dtype = shape(*args)
+        return args[0].new_empty(out_shape, dtype=dtype)
+
+    def no_backward(ctx, grad_c):
+        raise capi.B200HgemmError(f"{qualname} is inference only: it has no gradient{why}")
+
+    torch.library.impl(qualname, "CUDA")(cuda)
+    torch.library.impl(qualname, "CPU")(cpu)
+    torch.library.register_fake(qualname)(fake)
+    # No gradient formula: without this, autograd would only warn and hand back no gradient for the inputs.
+    torch.library.register_autograd(qualname, no_backward)
+
+
 torch.library.define(f"{_LIB}::hgemm", "(Tensor a, Tensor b_kmajor, str acc='fp32') -> Tensor")
 
 
@@ -172,39 +206,20 @@ def hgemm_batched(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32",
 
 
 # ------------------------------------------------------------------------------------------ grouped (libb200_grouped.so)
-torch.library.define(f"{_LIB}::hgemm_grouped", "(Tensor a, Tensor b_kmajor, Tensor offs, str acc='fp32') -> Tensor")
-
-
-@torch.library.impl(f"{_LIB}::hgemm_grouped", "CUDA")
-def _hgemm_grouped_cuda(a, b_kmajor, offs, acc="fp32"):
-    g, t, n, _ = capi.check_grouped_operands(a, b_kmajor, offs, acc)
-    a, b_kmajor, offs = a.contiguous(), b_kmajor.contiguous(), offs.contiguous()
-    c = torch.empty((t, n), dtype=a.dtype, device=a.device)
-    if g == 0 or t == 0:
-        return c
-    with torch.cuda.device(a.device):
-        capi.gemm_grouped(a, b_kmajor, c, offs, acc, stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
-
-
-@torch.library.impl(f"{_LIB}::hgemm_grouped", "CPU")
-def _hgemm_grouped_cpu(a, b_kmajor, offs, acc="fp32"):
-    raise capi.B200HgemmError("cuda_l2_b200::hgemm_grouped has no CPU implementation (and no fallback): move the tensors "
-                              "to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::hgemm_grouped")
-def _hgemm_grouped_fake(a, b_kmajor, offs, acc="fp32"):
+def _hgemm_grouped_shape(a, b_kmajor, offs, acc="fp32"):
     _, t, n, _ = capi.check_grouped_operands(a, b_kmajor, offs, acc)
-    return a.new_empty((t, n))
+    return (t, n), a.dtype
 
 
-def _hgemm_grouped_no_backward(ctx, grad_c):
-    raise capi.B200HgemmError("cuda_l2_b200::hgemm_grouped is inference only: it has no gradient (the weight gradient is "
-                              "a grouped product over K, a different kernel)")
+def _hgemm_grouped_launch(c, a, b_kmajor, offs, acc="fp32", *, stream):
+    if b_kmajor.shape[0] == 0 or c.shape[0] == 0:   # no group or no row
+        return
+    a, b_kmajor, offs = a.contiguous(), b_kmajor.contiguous(), offs.contiguous()
+    capi.gemm_grouped(a, b_kmajor, c, offs, acc, stream=stream)
 
 
-torch.library.register_autograd(f"{_LIB}::hgemm_grouped", _hgemm_grouped_no_backward)
+_inference_op("hgemm_grouped", "(Tensor a, Tensor b_kmajor, Tensor offs, str acc='fp32') -> Tensor", _hgemm_grouped_shape,
+              _hgemm_grouped_launch, " (the weight gradient is a grouped product over K, a different kernel)")
 
 
 def hgemm_grouped(a: torch.Tensor, b_kmajor: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -280,10 +295,6 @@ def replace_linear_modules(model: nn.Module, acc: str = "fp32", skip: tuple[str,
 # ------------------------------------------------------------------------------------------ FP8 (e4m3), inference only
 E4M3_MAX = 448.0   # largest finite float8_e4m3fn value
 
-torch.library.define(f"{_LIB}::fp8_gemm",
-                     "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor")
-
-
 def _rowwise_scale_arg(s: torch.Tensor) -> torch.Tensor:
     """A rowwise scale vector as the kernel reads it: contiguous and 16-byte aligned (a fresh copy if it is not)."""
     s = s.contiguous()
@@ -291,23 +302,27 @@ def _rowwise_scale_arg(s: torch.Tensor) -> torch.Tensor:
 
 
 def _m_major(s: torch.Tensor) -> torch.Tensor:
-    """A blockwise ``scale_a`` [M, nkb] as the kernel reads it: M-major with a row stride ld_a = M rounded up to 4
-    (``buf[:, :M].t()`` of an [nkb, ld_a] buffer), a device copy unless it is already laid out so."""
+    """A blockwise ``scale_a`` [M, nkb], or [B, M, nkb], as the kernels read it: one M-major [nkb, ld_a] block per
+    matrix, ld_a = M rounded up to 4 (``buf[..., :M].transpose(-2, -1)`` of an [nkb, ld_a] or [B, nkb, ld_a] buffer), a
+    device copy unless it is already laid out so."""
     if capi.blockwise_ld_a(s) is not None:
         return s
-    m, nkb = s.shape
-    buf = torch.empty((nkb, -(-m // 4) * 4), dtype=s.dtype, device=s.device)
-    buf[:, :m].copy_(s.t())
-    return buf[:, :m].t()
+    *lead, m, nkb = s.shape
+    buf = torch.empty((*lead, nkb, -(-m // 4) * 4), dtype=s.dtype, device=s.device)
+    buf[..., :m].copy_(s.transpose(-2, -1))
+    return buf[..., :m].transpose(-2, -1)
 
 
-@torch.library.impl(f"{_LIB}::fp8_gemm", "CUDA")
-def _fp8_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype):
-    m, n, k = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
+def _fp8_gemm_shape(a, b_kmajor, scale_a, scale_b, out_dtype):
+    m, n, _ = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
+    return (m, n), out_dtype
+
+
+def _fp8_gemm_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, *, stream):
+    (m, n), k = c.shape, a.shape[1]
     a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
-    c = torch.empty((m, n), dtype=out_dtype, device=a.device)
     if m == 0:
-        return c
+        return
     granularity = capi.scale_granularity(m, n, scale_a, scale_b, k=k)
     if granularity == "blockwise":
         scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
@@ -315,29 +330,12 @@ def _fp8_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype):
         scale_a, scale_b = _rowwise_scale_arg(scale_a), _rowwise_scale_arg(scale_b)
     else:
         scale_a, scale_b = scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous()
-    with torch.cuda.device(a.device):
-        capi.fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
+    capi.fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream=stream)
 
 
-@torch.library.impl(f"{_LIB}::fp8_gemm", "CPU")
-def _fp8_gemm_cpu(a, b_kmajor, scale_a, scale_b, out_dtype):
-    raise capi.B200HgemmError("cuda_l2_b200::fp8_gemm has no CPU implementation (and no fallback): move the tensors to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::fp8_gemm")
-def _fp8_gemm_fake(a, b_kmajor, scale_a, scale_b, out_dtype):
-    m, n, _ = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
-    return a.new_empty((m, n), dtype=out_dtype)
-
-
-def _fp8_gemm_no_backward(ctx, grad_c):
-    raise capi.B200HgemmError("cuda_l2_b200::fp8_gemm is inference only: it has no gradient (train with the fp16 / bf16 "
-                              "operator and quantise afterwards)")
-
-
-# No gradient formula: without this, autograd would only warn and hand back no gradient for the inputs.
-torch.library.register_autograd(f"{_LIB}::fp8_gemm", _fp8_gemm_no_backward)
+_inference_op("fp8_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor",
+              _fp8_gemm_shape, _fp8_gemm_launch,
+              " (train with the fp16 / bf16 operator and quantise afterwards)")
 
 
 def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
@@ -481,45 +479,21 @@ class B200Fp8Linear(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------ grouped FP8 (libb200_grouped_fp8.so)
-torch.library.define(f"{_LIB}::fp8_grouped_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, "
-                     "Tensor offs, ScalarType out_dtype) -> Tensor")
+def _fp8_grouped_shape(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
+    _, t, n, _ = capi.check_grouped_operands(a, b_kmajor, offs, "fp32", out_dtype, (scale_a, scale_b))
+    return (t, n), out_dtype
 
 
-def _fp8_grouped_check(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
-    return capi.check_grouped_operands(a, b_kmajor, offs, "fp32", out_dtype, (scale_a, scale_b))
-
-
-@torch.library.impl(f"{_LIB}::fp8_grouped_gemm", "CUDA")
-def _fp8_grouped_gemm_cuda(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
-    g, t, n, _ = _fp8_grouped_check(a, b_kmajor, scale_a, scale_b, offs, out_dtype)
-    c = torch.empty((t, n), dtype=out_dtype, device=a.device)
-    if g == 0 or t == 0:
-        return c
+def _fp8_grouped_launch(c, a, b_kmajor, scale_a, scale_b, offs, out_dtype, *, stream):
+    if b_kmajor.shape[0] == 0 or c.shape[0] == 0:   # no group or no row
+        return
     a, b_kmajor, offs = a.contiguous(), b_kmajor.contiguous(), offs.contiguous()
     scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
-    with torch.cuda.device(a.device):
-        capi.fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs,
-                              stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
+    capi.fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs, stream=stream)
 
 
-@torch.library.impl(f"{_LIB}::fp8_grouped_gemm", "CPU")
-def _fp8_grouped_gemm_cpu(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
-    raise capi.B200HgemmError("cuda_l2_b200::fp8_grouped_gemm has no CPU implementation (and no fallback): move the "
-                              "tensors to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::fp8_grouped_gemm")
-def _fp8_grouped_gemm_fake(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
-    _, t, n, _ = _fp8_grouped_check(a, b_kmajor, scale_a, scale_b, offs, out_dtype)
-    return a.new_empty((t, n), dtype=out_dtype)
-
-
-def _fp8_grouped_gemm_no_backward(ctx, grad_c):
-    raise capi.B200HgemmError("cuda_l2_b200::fp8_grouped_gemm is inference only: it has no gradient")
-
-
-torch.library.register_autograd(f"{_LIB}::fp8_grouped_gemm", _fp8_grouped_gemm_no_backward)
+_inference_op("fp8_grouped_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, Tensor offs, "
+              "ScalarType out_dtype) -> Tensor", _fp8_grouped_shape, _fp8_grouped_launch)
 
 
 def fp8_grouped_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
@@ -533,59 +507,23 @@ def fp8_grouped_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Ten
 
 
 # ------------------------------------------------------------------------------------------ batched FP8 (libb200_batched_fp8.so)
-torch.library.define(f"{_LIB}::fp8_batched_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, "
-                     "ScalarType out_dtype, Tensor? masked_m=None) -> Tensor")
+def _fp8_batched_shape(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None):
+    bsz, m, n, _ = capi.check_batched_operands(a, b_kmajor, "fp32", masked_m, out_dtype, (scale_a, scale_b))
+    return (bsz, m, n), out_dtype
 
 
-def _fp8_batched_check(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m):
-    return capi.check_batched_operands(a, b_kmajor, "fp32", masked_m, out_dtype, (scale_a, scale_b))
-
-
-def _batched_m_major(s: torch.Tensor) -> torch.Tensor:
-    """A batched blockwise ``scale_a`` [B, M, nkb] as the kernel reads it: one M-major [nkb, ld_a] block per matrix,
-    ld_a = M rounded up to 4 (``buf[:, :, :M].transpose(1, 2)`` of a [B, nkb, ld_a] buffer), a device copy unless it is
-    already laid out so."""
-    if capi.batched_blockwise_ld_a(s) is not None:
-        return s
-    bsz, m, nkb = s.shape
-    buf = torch.empty((bsz, nkb, -(-m // 4) * 4), dtype=s.dtype, device=s.device)
-    buf[:, :, :m].copy_(s.transpose(1, 2))
-    return buf[:, :, :m].transpose(1, 2)
-
-
-@torch.library.impl(f"{_LIB}::fp8_batched_gemm", "CUDA")
-def _fp8_batched_gemm_cuda(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None):
-    bsz, m, n, _ = _fp8_batched_check(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m)
-    c = torch.empty((bsz, m, n), dtype=out_dtype, device=a.device)
-    if bsz == 0 or m == 0:
-        return c
+def _fp8_batched_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None, *, stream):
+    if c.shape[0] == 0 or c.shape[1] == 0:   # no matrix or no row
+        return
     a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
-    scale_a, scale_b = _batched_m_major(scale_a), _rowwise_scale_arg(scale_b)
+    scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
     if masked_m is not None:
         masked_m = masked_m.contiguous()
-    with torch.cuda.device(a.device):
-        capi.fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=masked_m,
-                              stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
+    capi.fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=masked_m, stream=stream)
 
 
-@torch.library.impl(f"{_LIB}::fp8_batched_gemm", "CPU")
-def _fp8_batched_gemm_cpu(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None):
-    raise capi.B200HgemmError("cuda_l2_b200::fp8_batched_gemm has no CPU implementation (and no fallback): move the "
-                              "tensors to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::fp8_batched_gemm")
-def _fp8_batched_gemm_fake(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=None):
-    bsz, m, n, _ = _fp8_batched_check(a, b_kmajor, scale_a, scale_b, out_dtype, masked_m)
-    return a.new_empty((bsz, m, n), dtype=out_dtype)
-
-
-def _fp8_batched_gemm_no_backward(ctx, grad_c):
-    raise capi.B200HgemmError("cuda_l2_b200::fp8_batched_gemm is inference only: it has no gradient")
-
-
-torch.library.register_autograd(f"{_LIB}::fp8_batched_gemm", _fp8_batched_gemm_no_backward)
+_inference_op("fp8_batched_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype, "
+              "Tensor? masked_m=None) -> Tensor", _fp8_batched_shape, _fp8_batched_launch)
 
 
 def fp8_batched_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
