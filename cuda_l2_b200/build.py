@@ -8,6 +8,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
 * ``libb200_grouped.so`` — the grouped fp16 / bf16 GEMM over contiguous row groups (include/b200_grouped.h)
 * ``libb200_grouped_fp8.so`` — the block-scaled FP8 grouped GEMM over contiguous row groups (include/b200_grouped_fp8.h)
 * ``libb200_batched_fp8.so`` — the block-scaled FP8 batched GEMM with per-batch row counts (include/b200_batched_fp8.h)
+* ``libb200_nn.so``     — the row-major B (NN) fp16 / bf16 kernels, loaded by libb200_hgemm.so on its first call with
+  ``B_rowmajor`` (csrc/b200_nn.h; no public symbol)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -62,7 +64,8 @@ def _run(cmd: list[str], verbose: bool) -> None:
 
 
 def _headers() -> list[Path]:
-    return sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.inc")) + sorted((REPO / "include").glob("*.h"))
+    return (sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.inc")) + sorted(CSRC.glob("*.h")) +
+            sorted((REPO / "include").glob("*.h")))
 
 
 def _compile_and_link(out: Path, objects: list[tuple[Path, list[str]]], link_flags: list[str], verbose: bool,
@@ -95,7 +98,8 @@ def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, lis
 # Every library: key -> (file name, its (source, defines) objects, extra link flags). The libraries other than
 # libb200_hgemm.so hold kernels of their own, so that the device code of the others stays as it is. libb200_hgemm.so
 # compiles its 16-bit kernels (b200_hgemm_capi.cu) and its e4m3 ones (b200_fp8_capi.cu) in parallel; the tile-list
-# libraries compile one source per variant (31 kernels each for the 16-bit variants, 17 for the block-scaled ones).
+# libraries compile one source per variant (31 kernels each for the 16-bit variants, 17 for the block-scaled ones), and
+# so does libb200_nn.so (43 kernels per 16-bit variant).
 LIBRARIES = {
     "capi": ("libb200_hgemm.so", [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], []),
     "fp8block": ("libb200_fp8block.so", [(CSRC / "b200_fp8_block_capi.cu", [])], []),
@@ -103,6 +107,7 @@ LIBRARIES = {
     "grouped": ("libb200_grouped.so", _per_variant("b200_grouped_capi.cu", VARIANTS), []),
     "grouped_fp8": ("libb200_grouped_fp8.so", _per_variant("b200_grouped_fp8_capi.cu", BLOCK_VARIANTS), []),
     "batched_fp8": ("libb200_batched_fp8.so", _per_variant("b200_batched_fp8_capi.cu", BLOCK_VARIANTS), []),
+    "nn": ("libb200_nn.so", _per_variant("b200_nn.cu", VARIANTS), []),
     "baselines": ("libb200_baselines.so", [(CSRC / "b200_baselines_capi.cu", [])], ["-lcublas", "-lcublasLt"]),
 }
 

@@ -374,6 +374,45 @@ def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = No
     _check(st, "b200 gemm")
 
 
+def check_rowmajor_operands(a, b, out_dtype=None, acc: str | int = "fp32") -> tuple[int, int, int]:
+    """(M, N, K) of a[M,K] @ b[K,N] with ``b`` row-major (``torch.matmul``'s layout), by the rules of the 16-bit variant
+    the dtypes and ``acc`` name (fp16 with fp32 or fp16 accumulation, bf16 with fp32; the output dtype is the operands'):
+    2-D operands of one dtype, a shared K, N % 8 == 0 and K % 8 == 0 (16-byte rows of A, B and C). Checks shapes and
+    dtypes only (meta tensors pass); B200HgemmError otherwise."""
+    try:
+        (m, k), (k2, n) = a.shape, b.shape
+    except ValueError:
+        raise B200HgemmError(f"2-D operands expected, got {tuple(a.shape)} and {tuple(b.shape)}") from None
+    t = _operand_type(a, b, a.dtype if out_dtype is None else out_dtype, acc, (), scaled=False)
+    if k2 != k:
+        raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b {tuple(b.shape)} (row-major: [K, N])")
+    if not t.fits(n, k):
+        raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % {t.k_align} == 0 (16-byte TMA strides), "
+                             f"got N={n}, K={k}")
+    return m, n, k
+
+
+def gemm_rowmajor(a, b, c, acc: str | int = "fp32", stream: int | None = None) -> None:
+    """c[M,N] = a[M,K] @ b[K,N] with ``b`` row-major (N contiguous, ``torch.matmul(a, b)``'s layout), read in place by
+    the row-major B (NN) kernels of libb200_nn.so: the drop-in entry points called with ``B_rowmajor`` and no
+    ``B_kmajor`` (include/b200_hgemm.h). fp16 (fp32 or fp16 accumulation) or bf16 (fp32) operands, all three contiguous
+    CUDA tensors. The dispatcher's TN choice for the shape runs, BN = 32 configurations mapped to a BN = 64 sibling."""
+    import torch
+
+    for name, x in (("a", a), ("b", b), ("c", c)):
+        if not x.is_cuda or not x.is_contiguous():
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    m, n, k = check_rowmajor_operands(a, b, c.dtype, acc)
+    if tuple(c.shape) != (m, n):
+        raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b {tuple(b.shape)}, c {tuple(c.shape)}")
+    lib = hgemm_lib()
+    if a.dtype == torch.bfloat16:
+        fn = lib.b200_bgemm_f32acc
+    else:
+        fn = lib.b200_hgemm_f32acc if ACC_BITS[acc] == 32 else lib.b200_hgemm_f16acc
+    _check(fn(a.data_ptr(), b.data_ptr(), None, c.data_ptr(), m, n, k, stream), "b200 gemm (row-major B)")
+
+
 def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config_id: int | None = None,
              group_m: int = 0, splits: int = 1, max_ctas: int = 0) -> None:
     """c[M,N] = (a[M,K] @ b_kmajor[N,K]^T) scaled, with ``float8_e4m3fn`` operands, fp32 accumulation and one rounding

@@ -1,13 +1,18 @@
 // libb200_hgemm.so — C-ABI entry points declared in include/b200_hgemm.h: the 16-bit variants (fp16 with fp32 or fp16
 // accumulation, bf16), the configuration table and schedule queries, the host-buffer entry and resource management.
-// The e4m3 variants are in b200_fp8_capi.cu. No torch, no CUTLASS, no cuBLAS.
+// The e4m3 variants are in b200_fp8_capi.cu. The row-major B (NN) kernels are in libb200_nn.so, which the drop-in
+// entry points load on their first NN call. No torch, no CUTLASS, no cuBLAS.
 #include "../../include/b200_hgemm.h"
+
+#include <dlfcn.h>
 
 #include <cstdlib>
 #include <map>
 #include <memory>
 #include <mutex>
+#include <string>
 
+#include "b200_nn.h"
 #include "hgemm_configs.cuh"
 #include "hgemm_dispatch.cuh"
 
@@ -60,6 +65,36 @@ HostCtx& host_ctx(int dev) {
   auto& slot = g_host_ctx[dev];
   if (!slot) slot.reset(new HostCtx());
   return *slot;
+}
+
+// The entry point of libb200_nn.so, loaded from the directory of this library on the first NN call (once per process;
+// null if the library is missing or does not load). Every other call of this library works without it.
+b200::nn::RunConfigFn nn_run_config() {
+  static const b200::nn::RunConfigFn fn = []() -> b200::nn::RunConfigFn {
+    Dl_info self{};
+    if (!dladdr(reinterpret_cast<const void*>(&nn_run_config), &self) || !self.dli_fname) return nullptr;
+    const std::string here(self.dli_fname);
+    const size_t slash = here.rfind('/');
+    const std::string path = (slash == std::string::npos ? std::string() : here.substr(0, slash + 1)) + b200::nn::kLibrary;
+    void* lib = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    return lib ? reinterpret_cast<b200::nn::RunConfigFn>(dlsym(lib, b200::nn::kRunConfigSymbol)) : nullptr;
+  }();
+  return fn;
+}
+
+// The dispatched NN call of variant T: C = A B with B [K,N] row-major. The argument rules of the TN call, checked before
+// anything else; the TN choice mapped to its NN sibling (dispatch::select_rowmajor); the launch in libb200_nn.so, with
+// this library's split-K scratch, counted with this library's launches.
+template <GemmType T>
+int gemm_rowmajor(const void* A, const void* B_rowmajor, void* C, int M, int N, int K, void* stream) {
+  if (const int st = b200::host::validate(T, A, B_rowmajor, C, {}, M, N, K)) return st;
+  const b200::nn::RunConfigFn run = nn_run_config();
+  if (!run) return b200::host::kNoNNLibrary;
+  const b200::dispatch::Choice ch = b200::dispatch::select_rowmajor(T, M, N, K);
+  const int st = run(int(T), ch.config_id, A, B_rowmajor, C, M, N, K, ch.group_m, 0, ch.splits,
+                     &b200::host::splitk_scratch, stream);
+  if (st == b200::host::kOk) b200::g_launches.fetch_add(1, std::memory_order_relaxed);
+  return st;
 }
 
 }  // namespace
@@ -135,18 +170,21 @@ int b200_hgemm_run_config(int acc_bits, int config_id, const void* A, const void
   return b200::host::kBadConfig;
 }
 
-int b200_hgemm_f32acc(const void* A, const void* /*B_rowmajor*/, const void* B_kmajor, void* C, int M, int N,
+int b200_hgemm_f32acc(const void* A, const void* B_rowmajor, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
+  if (!B_kmajor && B_rowmajor) return gemm_rowmajor<GemmType::kF16Acc32>(A, B_rowmajor, C, M, N, K, stream);
   return b200::dispatch::gemm<GemmType::kF16Acc32>(A, B_kmajor, C, {}, M, N, K, stream);
 }
 
-int b200_hgemm_f16acc(const void* A, const void* /*B_rowmajor*/, const void* B_kmajor, void* C, int M, int N,
+int b200_hgemm_f16acc(const void* A, const void* B_rowmajor, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
+  if (!B_kmajor && B_rowmajor) return gemm_rowmajor<GemmType::kF16Acc16>(A, B_rowmajor, C, M, N, K, stream);
   return b200::dispatch::gemm<GemmType::kF16Acc16>(A, B_kmajor, C, {}, M, N, K, stream);
 }
 
-int b200_bgemm_f32acc(const void* A, const void* /*B_rowmajor*/, const void* B_kmajor, void* C, int M, int N,
+int b200_bgemm_f32acc(const void* A, const void* B_rowmajor, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
+  if (!B_kmajor && B_rowmajor) return gemm_rowmajor<GemmType::kBF16>(A, B_rowmajor, C, M, N, K, stream);
   return b200::dispatch::gemm<GemmType::kBF16>(A, B_kmajor, C, {}, M, N, K, stream);
 }
 

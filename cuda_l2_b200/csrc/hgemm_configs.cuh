@@ -96,6 +96,38 @@ static_assert(every_config_has_an_eligible_sibling(), "the configuration table l
 
 }  // namespace block
 
+// The row-major B (NN) configurations (libb200_nn.so, RowMajorB<>). Host code: libb200_hgemm.so maps the dispatcher's
+// choice through this rule before it calls the NN library.
+namespace nn {
+
+// An MN-major B stage is whole 64-column atom columns: every configuration but the BN = 32 ones has an NN kernel.
+constexpr bool has_kernel(int id) { return kConfigs[id].bn % 64 == 0; }
+
+// The NN stand-in of configuration `id`: itself if it has an NN kernel; otherwise the BN = 64 configuration with the
+// same CTA group, cluster_m and M_REP and the widest cluster_n up to its own (the same cluster where there is one).
+constexpr int sibling(int id) {
+  const ConfigDesc& c = kConfigs[id];
+  if (has_kernel(id)) return id;
+  int best = -1;
+  for (int j = 0; j < kNumConfigs; ++j) {
+    const ConfigDesc& d = kConfigs[j];
+    if (d.bn == 64 && d.cta_group == c.cta_group && d.cluster_m == c.cluster_m && d.m_rep == c.m_rep &&
+        d.cluster_n <= c.cluster_n && (best < 0 || d.cluster_n > kConfigs[best].cluster_n))
+      best = j;
+  }
+  return best;
+}
+constexpr bool every_config_has_a_sibling() {
+  for (int id = 0; id < kNumConfigs; ++id) {
+    const int s = sibling(id);
+    if (s < 0 || !has_kernel(s) || (has_kernel(id) && s != id)) return false;
+  }
+  return true;
+}
+static_assert(every_config_has_a_sibling(), "the configuration table lost a row-major B sibling");
+
+}  // namespace nn
+
 // Kernel launches the library has issued (b200_hgemm_launch_count). One counter for every translation unit of the
 // library; hidden, so that no other shared object's copy is bound to it.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_launches{0};

@@ -29,6 +29,7 @@ enum Status : int {
   kNoScratch = -8,       // internal: no split-K scratch for this (device, stream) and none can be allocated now (stream capture)
   kBadFp8K = -9,         // e4m3 operands: K % 16 == 0 (16-byte TMA strides at one byte per element)
   kBadScaleLd = -10,     // block scales: the row stride of A's scales must be >= M and a multiple of 4
+  kNoNNLibrary = -11,    // row-major B: libb200_nn.so, next to libb200_hgemm.so, is missing or does not load
   // > 0: a cudaError_t from the launch
 };
 
@@ -45,6 +46,7 @@ inline const char* status_string(int s) {
     case kNoScratch: return "split-K scratch unavailable (allocate it outside stream capture with b200_hgemm_prewarm)";
     case kBadFp8K: return "e4m3 operands need K % 16 == 0 (16-byte row strides at one byte per element)";
     case kBadScaleLd: return "block scales need ld_a >= M and ld_a % 4 == 0 (16-byte aligned k-block rows of A's scales)";
+    case kNoNNLibrary: return "row-major B needs libb200_nn.so next to libb200_hgemm.so (missing, or it does not load)";
     default: return s > 0 ? cudaGetErrorString(static_cast<cudaError_t>(s)) : "unknown error";
   }
 }
@@ -179,6 +181,10 @@ inline const DeviceInfo& device_info() {
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev != cached_dev) {
+    // The tensor-map encoder is a driver call and needs the device's primary context current on this thread. A thread
+    // whose first CUDA work is a call of this library (an autograd worker running a backward) has none yet:
+    // cudaSetDevice makes it current (CUDA 12), and is legal during a stream capture.
+    cudaSetDevice(dev);
     cudaDeviceGetAttribute(&info.num_sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&info.cc_major, cudaDevAttrComputeCapabilityMajor, dev);
     info.dev = dev;
@@ -256,6 +262,11 @@ inline int splitk_scratch(int dev, cudaStream_t stream, SplitKScratch** out) {
   *out = slot;
   return kOk;
 }
+// Where a launch finds the scratch of (device, stream): this library's pool (splitk_scratch), or, for the row-major B
+// kernels of libb200_nn.so, the pool of libb200_hgemm.so, handed over with each call, so that b200_hgemm_prewarm and
+// b200_hgemm_release serve both libraries and a process holds one pool.
+using ScratchFn = int (*)(int dev, cudaStream_t stream, SplitKScratch** out);
+
 // Frees every scratch allocation of this process (all devices). The caller guarantees that no launch of this
 // library is in flight or issued concurrently.
 inline void release_scratch() {
@@ -515,10 +526,12 @@ constexpr int default_group_m() { return Cfg::CTA_GROUP == 2 ? 8 : 16; }
 // split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
 // mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
 // kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor or rowwise scales
-// of a scaled variant (device pointers), unused otherwise; `ld_a`: the row stride of block scales.
+// of a scaled variant (device pointers), unused otherwise; `ld_a`: the row stride of block scales. RowMajorB<>
+// configurations read `Bt` as B [K, N] row-major. `scratch`: where the workspace of split-K and stream-K comes from.
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
-           int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0) {
+           int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0,
+           ScratchFn scratch = splitk_scratch) {
   constexpr GemmType kType = gemm_type<Cfg>();
   int st = validate(kType, A, Bt, C, scales, M, N, K, ld_a);
   if (st != kOk) return st;
@@ -529,14 +542,18 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   MapCache& cache = map_cache();
   const Elem operand = traits(kType).operand, output = traits(kType).output;
   if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, operand)) != kOk) return st;
-  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, operand)) != kOk) return st;
+  if constexpr (row_major_b<Cfg>()) {   // B [K, N]: boxes of 64 columns (one atom column) by this CTA's K slice
+    if ((st = cache.get(Bt, K, N, Cfg::B_K_ROWS, &a.mb, 64, operand)) != kOk) return st;
+  } else {
+    if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, operand)) != kOk) return st;
+  }
   if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk) return st;
 
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = plan<Cfg, MODES>(M, N, K, splits, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
   if (a.plan.mode == kWorkspaceSplitK || a.plan.mode == kStreamK) {
     SplitKScratch* sk = nullptr;
-    if (splitk_scratch(di.dev, stream, &sk) == kOk) {
+    if (scratch(di.dev, stream, &sk) == kOk) {
       a.ws = sk->ws; a.ctr = sk->ctr;
     } else {
       cudaGetLastError();   // no scratch (allocation failed, or first use inside a stream capture): run undivided

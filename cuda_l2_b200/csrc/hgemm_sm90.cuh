@@ -99,8 +99,8 @@ struct Config {
   // which K-decompositions this configuration's kernel carries
   static constexpr bool STREAM_K = CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
   static constexpr bool SPLIT_K = STREAM_K && CTA_GROUP_ == 1;
-  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>) override these
-  static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false;
+  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>, RowMajorB<>) override these
+  static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false, ROW_MAJOR_B = false;
   using Cursor = NoBatches;   // the flat tile list the kernel walks (hgemm_schedule.cuh): none
   static constexpr int EPI_BYTES = 8 * EPI_ROWS * 64 * 2;    // 8 consumer warps x one staging buffer (sized for EPI_N = 64)
   static constexpr int BAR_BYTES = 256;
@@ -205,6 +205,30 @@ struct Grouped<BlockScaled<Base>> : BlockScaled<Base> {
 };
 template <class Cfg>
 __host__ __device__ constexpr bool grouped() { return Cfg::GROUPED; }
+
+// Row-major B (NN, libb200_nn.so): C = A B with B [K, N] row-major (N contiguous), the layout of torch.matmul(a, b),
+// read in place instead of through a transposed copy. wgmma reads a 16-bit B operand MN-major (imm-trans-b = 1), so
+// only the B load and the B descriptor change. A B stage holds BN / 64 MN-major SW128 atom columns, each 64 N x 64 K
+// rows of 128 B (8 KB, the descriptor's LBO), 8-row K groups 1024 B apart (SBO); a k16 step advances 16 K rows. TMA
+// loads a {64 N, rows} box of B's {N, K} map into an atom column, zero-filling past K and N as for Bt. Multicast is
+// sliced along K: each of the MCAST_M CTAs loads K rows [mi * B_K_ROWS, (mi + 1) * B_K_ROWS) of every atom column, so
+// every slice is whole 8-row swizzle groups (1 KB aligned) and any per-CTA N extent works. e4m3 wgmma takes K-major
+// operands only, and a BN = 32 tile has no 128-byte N row: those configurations have no NN kernel (nn::sibling). A
+// wrapper, like BlockScaled<>, so that the other kernels and their names stay as they are.
+template <class Base>
+struct RowMajorB : Base {
+  static constexpr bool ROW_MAJOR_B = true;
+  static_assert(!Base::E4M3 && !Base::BLOCK_SCALED && !Base::BATCHED && !Base::GROUPED,
+                "row-major B: the 2-D 16-bit kernels only");
+  static_assert(Base::BN % 64 == 0, "row-major B: whole 64-column atom columns");
+  static constexpr int B_ATOMS = Base::BN / 64;                       // atom columns per stage
+  static constexpr int B_ATOM_BYTES = 64 * kBlockK * 2;               // one atom column: 64 K rows of 128 B
+  static constexpr int B_K_ROWS = kBlockK / Base::MCAST_M;            // K rows of each atom column this CTA loads
+  static_assert(B_K_ROWS % 8 == 0, "K slices of whole 8-row swizzle groups");
+  static_assert(B_ATOMS * B_ATOM_BYTES == Base::B_STAGE_BYTES, "the stage holds the same bytes as the K-major one");
+};
+template <class Cfg>
+__host__ __device__ constexpr bool row_major_b() { return Cfg::ROW_MAJOR_B; }
 
 // Scales of an e4m3 launch, in device memory (null for the 16-bit operand types). Per tensor: one fp32 value each.
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
@@ -571,7 +595,8 @@ __device__ __forceinline__ void streamk_own(Reg (&d)[NR], int t, int ew, int lan
 template <class Cfg, int KMODE = kPlain>
 __global__ void __launch_bounds__(kNumThreads, 1)
 hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {BLOCK_K, A_BOX_ROWS}
-                const __grid_constant__ CUtensorMap tmap_b,   // Bt [N,K]  box {BLOCK_K, B_BOX_ROWS}
+                const __grid_constant__ CUtensorMap tmap_b,   // Bt [N,K]  box {BLOCK_K, B_BOX_ROWS}; row-major
+                                                              // B (RowMajorB<>): B [K,N] box {64, B_K_ROWS}
                 const __grid_constant__ CUtensorMap tmap_c,   // C  [M,N]  box {EPI_N, EPI_ROWS}
                 int M, int N, int K, int group_m,
                 int splits_arg,                   // split-K factor (modes kWorkspaceSplitK / kClusterSplitK: one unit per CTA);
@@ -616,6 +641,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   constexpr bool kBatched = batched<Cfg>();
   constexpr bool kGrouped = grouped<Cfg>();
   constexpr bool kTileList = kBatched || kGrouped;   // the schedule walks a cursor's flat tile list
+  constexpr bool kRowMajorB = row_major_b<Cfg>();    // B [K, N] in MN-major atom columns (RowMajorB<>)
   static_assert(!kTileList || KMODE == kPlain, "batched / grouped: plain schedule only");
   // grouped kernels: the group count and the offsets, in the same places (M is then T, the rows of A and C)
   [[maybe_unused]] const int num_batches = kTileList ? splits_arg : 1;
@@ -750,8 +776,21 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
             } else {
             if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, mask_a, hint_a);
             else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, hint_a);
+            if constexpr (kRowMajorB) {
+              // B [K, N]: this CTA's K slice of every atom column of the tile, multicast to its cluster column
+              const uint32_t dst = smem_b + stage * Cfg::B_STAGE_BYTES + uint32_t(mi) * (Cfg::B_K_ROWS * kBlockKBytes);
+              const int nb = (tc.n_blk * CN + cn) * BN, kr = kb * Cfg::BLOCK_K + mi * Cfg::B_K_ROWS;
+#pragma unroll
+              for (int j = 0; j < Cfg::B_ATOMS; ++j) {
+                if constexpr (EM > 1)
+                  tma_load_2d_mcast_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, mask_b, hint_b);
+                else
+                  tma_load_2d_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, hint_b);
+              }
+            } else {
             if constexpr (EM > 1) tma_load_2d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, mask_b, hint_b);
             else tma_load_2d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, hint_b);
+            }
             }
           }
           __syncwarp();
@@ -770,7 +809,10 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   } else {
     setmaxnreg_inc<kConsumerRegs>();
     // ===== consumers: warpgroup wg owns rows [wg * 64 * MR, (wg + 1) * 64 * MR) of the CTA's tile =====
-    using W = Wgmma<BN, Cfg::ACC_F32, Cfg::BF16 && !Cfg::E4M3, Cfg::E4M3>;
+    using W = Wgmma<BN, Cfg::ACC_F32, Cfg::BF16 && !Cfg::E4M3, Cfg::E4M3, kRowMajorB>;
+    // B's descriptor and its advance per k16 step (in 16-byte units): K-major, +32 B; MN-major (RowMajorB<>), +16 K
+    // rows of 128 B, atom columns 8 KB apart
+    constexpr int kDescBStep = kRowMajorB ? 16 * kBlockKBytes / 16 : 2;
     using Reg = typename W::Reg;
     constexpr int NR = W::kRegs;
     const int wg = warp / 4 - 1;
@@ -852,7 +894,9 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       for (int kb = u.kb0; kb < u.kb1; ++kb) {
         mbar_wait(bar_full + 8 * stage, phase);
         const uint64_t da = make_smem_desc(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg * MR) * (64 * kBlockK * 2));
-        const uint64_t db = make_smem_desc(smem_b + stage * Cfg::B_STAGE_BYTES);
+        uint64_t db;
+        if constexpr (kRowMajorB) db = make_smem_desc_mn(smem_b + stage * Cfg::B_STAGE_BYTES, 64 * kBlockKBytes);
+        else db = make_smem_desc(smem_b + stage * Cfg::B_STAGE_BYTES);
 #pragma unroll
         for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
         wgmma_fence();
@@ -860,7 +904,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         for (int k = 0; k < kBlockK / kWgmmaK; ++k) {   // four wgmmas of 32 bytes of K each, for every operand type
 #pragma unroll
           for (int r = 0; r < MR; ++r)
-            W::mma(da + uint64_t(r * ((64 * kBlockK * 2) >> 4) + 2 * k), db + uint64_t(2 * k), acc[r],
+            W::mma(da + uint64_t(r * ((64 * kBlockK * 2) >> 4) + 2 * k), db + uint64_t(kDescBStep * k), acc[r],
                    (kb > u.kb0 || k > 0) ? 1u : 0u);
         }
         wgmma_commit();

@@ -184,6 +184,17 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   d |= uint64_t(1) << 62;   // SWIZZLE_128B
   return d;
 }
+// The same for an MN-major 16-bit tile (B read with imm-trans-b = 1), 128B swizzle: rows of 64 N elements (128 B) for
+// one k each, 8-row K groups 1024 B apart (SBO), 64-column atom columns `lbo` bytes apart (LBO). +16 K rows (one k16
+// step) is +2048 B, +128 in the address field.
+__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr, uint32_t lbo) {
+  uint64_t d = 0;
+  d |= uint64_t((smem_addr & 0x3FFFF) >> 4);
+  d |= uint64_t((lbo & 0x3FFFF) >> 4) << 16;
+  d |= uint64_t(1024 >> 4) << 32;
+  d |= uint64_t(1) << 62;   // SWIZZLE_128B
+  return d;
+}
 // make the accumulator registers (and the operands in shared memory) visible to the next wgmma.mma_async
 __device__ __forceinline__ void wgmma_fence() {
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");

@@ -8,6 +8,9 @@ the nearest grid shape — so deployment is a plain operator:
 * ``torch.ops.cuda_l2_b200.hgemm(a, b_kmajor, acc)``: ``a`` [M,K] times B given K-major as ``b_kmajor`` [N,K]
   (exactly the layout of an ``nn.Linear`` weight: ``[out_features, in_features]``), returns [M,N]. fp16 or bf16
   operands (bf16 always accumulates in fp32); ``acc`` = "fp32" | "fp16".
+* ``torch.ops.cuda_l2_b200.hgemm_nn(a, b, acc)``: ``a`` [M,K] times ``b`` [K,N] row-major (``torch.matmul(a, b)``'s
+  layout, such as attention's P·V), returns [M,N]. ``b`` is read in place by the row-major B kernels: no transposed
+  copy. Its gradient needs no transposed copy of ``b`` either.
 * ``torch.ops.cuda_l2_b200.hgemm_batched(a, b_kmajor, acc, masked_m=None)``: ``a`` [B,M,K] times ``b_kmajor``
   [B,N,K] per batch, returns [B,M,N] — ``torch.bmm(a, b_kmajor.transpose(1, 2))`` in one launch (per-head attention
   products, per-expert projections). ``masked_m``, an int32 CUDA tensor [B] read by the kernel (no host
@@ -41,9 +44,10 @@ the nearest grid shape — so deployment is a plain operator:
   ``forward`` takes the prefill layout, ``forward_masked`` the decode layout.
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
-raises. Backward (training is not what the reference targets) is provided through the same kernel on explicitly
-transposed copies, so a fine-tuning loop works, at the price of two transposes per layer. The FP8 operator has no
-gradient: a backward through it raises.
+raises. Backward (training is not what the reference targets) is provided through the same kernels, so a fine-tuning
+loop works: ``hgemm``'s input gradient reads the weight in place through the row-major B kernels, and its weight
+gradient pays one transposed copy (of the output gradient). The FP8 operator has no gradient: a backward through it
+raises.
 """
 from __future__ import annotations
 
@@ -120,11 +124,13 @@ def _hgemm_backward(ctx, grad_c):
     a, b_kmajor = ctx.saved_tensors
     grad_a = grad_b = None
     g = grad_c.contiguous()
-    # C = A Bt^T  =>  dA = dC Bt  (reduction over N: B operand K-major in N = Bt^T),  dBt = dC^T A  (reduction over M)
+    # C = A Bt^T  =>  dA = dC Bt  (reduction over N: Bt [N,K] is B row-major),  dBt = dC^T A  (reduction over M: A [M,K]
+    # is B row-major). The row-major B kernels read both in place; only dC^T is copied. They compute what the K-major
+    # kernels compute on transposed copies, bit for bit.
     if ctx.needs_input_grad[0]:
-        grad_a = torch.ops.cuda_l2_b200.hgemm(g, b_kmajor.t().contiguous(), "fp32")
+        grad_a = torch.ops.cuda_l2_b200.hgemm_nn(g, b_kmajor, "fp32")
     if ctx.needs_input_grad[1]:
-        grad_b = torch.ops.cuda_l2_b200.hgemm(g.t().contiguous(), a.t().contiguous(), "fp32")
+        grad_b = torch.ops.cuda_l2_b200.hgemm_nn(g.t().contiguous(), a, "fp32")
     return grad_a, grad_b, None
 
 
@@ -139,6 +145,61 @@ torch.library.register_autograd(f"{_LIB}::hgemm", _hgemm_backward, setup_context
 def hgemm(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
     """``a`` [M,K] @ ``b_kmajor`` [N,K]^T -> [M,N] through the H100 kernel (see the module docstring)."""
     return torch.ops.cuda_l2_b200.hgemm(a, b_kmajor, acc)
+
+
+# ------------------------------------------------------------------------------------------ row-major B (libb200_nn.so)
+torch.library.define(f"{_LIB}::hgemm_nn", "(Tensor a, Tensor b, str acc='fp32') -> Tensor")
+
+
+@torch.library.impl(f"{_LIB}::hgemm_nn", "CUDA")
+def _hgemm_nn_cuda(a: torch.Tensor, b: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
+    m, n, _ = capi.check_rowmajor_operands(a, b, a.dtype, acc)
+    a, b = a.contiguous(), b.contiguous()
+    c = torch.empty((m, n), dtype=a.dtype, device=a.device)
+    if m == 0:
+        return c
+    with torch.cuda.device(a.device):
+        capi.gemm_rowmajor(a, b, c, acc, stream=torch.cuda.current_stream(a.device).cuda_stream)
+    return c
+
+
+@torch.library.impl(f"{_LIB}::hgemm_nn", "CPU")
+def _hgemm_nn_cpu(a, b, acc="fp32"):
+    raise capi.B200HgemmError("cuda_l2_b200::hgemm_nn has no CPU implementation (and no fallback): move the tensors to "
+                              "an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::hgemm_nn")
+def _hgemm_nn_fake(a, b, acc="fp32"):
+    m, n, _ = capi.check_rowmajor_operands(a, b, a.dtype, acc)
+    return a.new_empty((m, n))
+
+
+def _hgemm_nn_backward(ctx, grad_c):
+    a, b = ctx.saved_tensors
+    grad_a = grad_b = None
+    g = grad_c.contiguous()
+    # C = A B  =>  dA = dC B^T (B [K,N] is K-major in the reduced N: the K-major kernels read it in place),
+    # dB = A^T dC (dC [M,N] is row-major in the reduced M; A^T is copied)
+    if ctx.needs_input_grad[0]:
+        grad_a = torch.ops.cuda_l2_b200.hgemm(g, b, "fp32")
+    if ctx.needs_input_grad[1]:
+        grad_b = torch.ops.cuda_l2_b200.hgemm_nn(a.t().contiguous(), g, "fp32")
+    return grad_a, grad_b, None
+
+
+def _hgemm_nn_setup_context(ctx, inputs, output):
+    a, b, _ = inputs
+    ctx.save_for_backward(a, b)
+
+
+torch.library.register_autograd(f"{_LIB}::hgemm_nn", _hgemm_nn_backward, setup_context=_hgemm_nn_setup_context)
+
+
+def hgemm_nn(a: torch.Tensor, b: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
+    """``a`` [M,K] @ ``b`` [K,N] -> [M,N] (``torch.matmul(a, b)``) with ``b`` row-major, read in place by the H100
+    row-major B kernels (see the module docstring)."""
+    return torch.ops.cuda_l2_b200.hgemm_nn(a, b, acc)
 
 
 # ------------------------------------------------------------------------------------------ batched (libb200_batched.so)
@@ -597,6 +658,6 @@ class B200Fp8GroupedLinear(nn.Module):
                 f"out_dtype={self.out_dtype}")
 
 
-__all__ = ["hgemm", "hgemm_batched", "hgemm_grouped", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
+__all__ = ["hgemm", "hgemm_nn", "hgemm_batched", "hgemm_grouped", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear",
            "fp8_grouped_gemm", "fp8_batched_gemm", "B200Fp8GroupedLinear"]

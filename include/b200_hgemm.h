@@ -10,9 +10,13 @@
  *
  * Conventions (same as the reference's kernels, kernels/a100_F32F16F16F32/4096_4096_4096.cu:292-310):
  *   A          [M,K] row-major fp16 (K contiguous)
- *   B_rowmajor [K,N] row-major fp16 — accepted for signature parity, never read (may be NULL)
+ *   B_rowmajor [K,N] row-major fp16 (N contiguous), the layout of torch.matmul(a, b). Read only when B_kmajor is
+ *              NULL: the drop-in calls below then run the row-major B (NN) kernels of libb200_nn.so, which the
+ *              library loads from its own directory on the first such call (status -11 if it is missing). Same
+ *              rules and dispatcher choice as K-major B (a BN = 32 configuration maps to a BN = 64 one); the result
+ *              is bit-identical to the K-major call on a transposed copy. NULL otherwise (ignored when B_kmajor is set).
  *   B_kmajor   B transposed in memory: [N,K] row-major (K contiguous) — the harness's `b_col_major`
- *              (tools/utils.py:110-115)
+ *              (tools/utils.py:110-115). Takes precedence over B_rowmajor; both NULL is status -5.
  *   C          [M,N] row-major fp16, fully overwritten (alpha = 1, beta = 0), nothing else is written
  *   stream     a cudaStream_t (NULL = the legacy default stream the reference launches on)
  * All pointers are device pointers, 16-byte aligned; K % 8 == 0 and N % 8 == 0 (TMA stride rule).
