@@ -99,12 +99,28 @@ ABI = {
         "b200_bl_lt_autotune_info": ([_i, _i, _ip, ctypes.POINTER(ctypes.c_float)], _i),
     },
 }
+# Libraries without a public ABI: their entry points are declared in an internal header under cuda_l2_b200/csrc/ and
+# none under include/, so they are kept out of ABI (which mirrors the headers). Same form: {symbol: (argtypes, restype)}.
+GROUPED_BWD_LIB = "libb200_grouped_bwd.so"   # csrc/b200_grouped_bwd.h
+_BWD_RUN = ([_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i)
+_BWD_SELECT = ([_i, _i, _i, _i, _i, _ip, _ip], _i)
+INTERNAL_ABI = {
+    GROUPED_BWD_LIB: {
+        "cuda_l2_b200_grouped_bwd_nn": _BWD_RUN,
+        "cuda_l2_b200_grouped_bwd_wgrad": _BWD_RUN,
+        "cuda_l2_b200_grouped_bwd_nn_select": _BWD_SELECT,
+        "cuda_l2_b200_grouped_bwd_wgrad_select": _BWD_SELECT,
+        "cuda_l2_b200_grouped_bwd_wgrad_schedule": ([_i, _i, _i, _i, _i, _ip, _i, _i, _ip, _i, _ip], _i),
+        "cuda_l2_b200_grouped_bwd_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_grouped_bwd_strerror": ([_i], ctypes.c_char_p),
+    },
+}
 _libs: dict = {}
 
 
 def load(name: str) -> ctypes.CDLL:
-    """The library ``name`` (a key of :data:`ABI`), loaded once with its table's argtypes and restypes applied: a
-    symbol it does not export raises."""
+    """The library ``name`` (a key of :data:`ABI` or :data:`INTERNAL_ABI`), loaded once with its table's argtypes and
+    restypes applied: a symbol it does not export raises."""
     if name not in _libs:
         path = LIB_DIR / name
         if not path.exists():
@@ -112,7 +128,7 @@ def load(name: str) -> ctypes.CDLL:
                 f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(or `python cuda_l2_b200/build.py`). There is no fallback path.")
         lib = ctypes.CDLL(str(path))
-        for sym, (args, res) in ABI[name].items():
+        for sym, (args, res) in (ABI[name] if name in ABI else INTERNAL_ABI[name]).items():
             fn = getattr(lib, sym)
             fn.argtypes, fn.restype = args, res
         _libs[name] = lib
@@ -652,6 +668,160 @@ def grouped_schedule(config_id: int, t: int, n: int, k: int, offs, num_sms: int 
 
 def grouped_launch_count() -> int:
     return int(grouped_lib().b200_grouped_launch_count())
+
+
+# ------------------------------------------------------------------------------------------ grouped backward
+#                                                                                            (libb200_grouped_bwd.so)
+def grouped_bwd_lib() -> ctypes.CDLL:
+    """libb200_grouped_bwd.so: the backward of the grouped fp16 / bf16 GEMM (csrc/b200_grouped_bwd.h, no public ABI)."""
+    return load(GROUPED_BWD_LIB)
+
+
+def _bwd_variant(dtype, acc: str | int) -> int:
+    """The ``variant`` of the grouped backward: 0 fp16 or 2 bf16, both with fp32 accumulation; B200HgemmError
+    otherwise."""
+    v = batched_variant(dtype, acc)
+    if v not in (0, 2):
+        raise B200HgemmError(f"the grouped backward takes fp16 or bf16 operands with fp32 accumulation, got {dtype} "
+                             f"with acc={acc!r}")
+    return v
+
+
+def _check_offs(offs, g: int) -> None:
+    import torch
+
+    if offs.dtype != torch.int32 or tuple(offs.shape) != (g,):
+        raise B200HgemmError(f"offs must be an int32 tensor of shape [{g}], got {offs.dtype} {tuple(offs.shape)}")
+
+
+def check_grouped_nn_operands(a, b, offs, acc: str | int = "fp32") -> tuple[int, int, int, int]:
+    """(G, T, N, K) of the grouped row-major B product a[T,K] by b[G,K,N] (rows [start_g, end_g) of the result are
+    those rows of ``a`` times ``b[g]``; ``torch._grouped_mm(a, b, offs=offs)``) with the int32 group ends ``offs`` [G]:
+    one dtype, fp16 or bf16 with fp32 accumulation, N % 8 == 0 and K % 8 == 0. Checks shapes and dtypes only (meta
+    tensors pass); B200HgemmError otherwise."""
+    try:
+        (t, k), (g, k2, n) = a.shape, b.shape
+    except ValueError:
+        raise B200HgemmError(f"a [T, K] and b [G, K, N] expected, got {tuple(a.shape)} and {tuple(b.shape)}") from None
+    if b.dtype != a.dtype:
+        raise B200HgemmError(f"operands of one dtype expected, got {a.dtype} and {b.dtype}")
+    _bwd_variant(a.dtype, acc)
+    if k2 != k:
+        raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b {tuple(b.shape)} (row-major: [G, K, N])")
+    if n % 8 or k % 8:
+        raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % 8 == 0 (16-byte TMA strides), got N={n}, K={k}")
+    _check_offs(offs, g)
+    return g, t, n, k
+
+
+def check_grouped_wgrad_operands(a, b, offs, acc: str | int = "fp32") -> tuple[int, int, int, int]:
+    """(G, T, M, N) of the K-grouped product: for every group g, a[start_g:end_g]^T @ b[start_g:end_g] -> [M, N], with
+    a [T,M], b [T,N] and the int32 group ends ``offs`` [G] (``torch._grouped_mm(a.t(), b, offs=offs)``): one dtype, fp16
+    or bf16 with fp32 accumulation, M % 8 == 0 and N % 8 == 0. Checks shapes and dtypes only (meta tensors pass);
+    B200HgemmError otherwise."""
+    try:
+        (t, m), (t2, n) = a.shape, b.shape
+        (g,) = offs.shape
+    except ValueError:
+        raise B200HgemmError(f"a [T, M], b [T, N] and offs [G] expected, got {tuple(a.shape)}, {tuple(b.shape)} and "
+                             f"{tuple(offs.shape)}") from None
+    if b.dtype != a.dtype:
+        raise B200HgemmError(f"operands of one dtype expected, got {a.dtype} and {b.dtype}")
+    _bwd_variant(a.dtype, acc)
+    if t2 != t:
+        raise B200HgemmError(f"row counts differ: a {tuple(a.shape)}, b {tuple(b.shape)}")
+    if m % 8 or n % 8:
+        raise B200HgemmError(f"{a.dtype} operands need M % 8 == 0 and N % 8 == 0 (16-byte TMA strides), got M={m}, N={n}")
+    if g < 1:
+        raise B200HgemmError("offs must hold at least one group")
+    _check_offs(offs, g)
+    return g, t, m, n
+
+
+def _bwd_call(symbol: str, variant: int, ptrs: tuple, problem: tuple, config_id: int | None, group_m: int,
+              max_ctas: int, stream: int | None) -> None:
+    lib = grouped_bwd_lib()
+    st = getattr(lib, symbol)(variant, -1 if config_id is None else config_id, *ptrs, *problem, group_m, max_ctas,
+                              stream)
+    if st != 0:
+        raise B200HgemmError(f"{symbol} failed: status {st} ({lib.cuda_l2_b200_grouped_bwd_strerror(st).decode()})")
+
+
+def _contiguous_cuda(**tensors) -> None:
+    for name, x in tensors.items():
+        if not x.is_cuda or not x.is_contiguous():
+            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+
+
+def gemm_grouped_nn(a, b, c, offs, acc: str | int = "fp32", config_id: int | None = None, group_m: int = 0,
+                    max_ctas: int = 0, stream: int | None = None) -> None:
+    """c[start_g:end_g] = a[start_g:end_g] @ b[g] for every group g, with ``b`` [G,K,N] row-major (an expert weight
+    stack [G, N_model, K_model] read in place: the input gradient of the grouped product), fp16 or bf16 operands with
+    fp32 accumulation, all contiguous CUDA tensors ([T,K], [G,K,N], [T,N]). ``offs``: int32 CUDA tensor [G] of
+    cumulative group ends, read by the kernel and clamped as for :func:`gemm_grouped`; rows of c at or past the last
+    group's end are not written. ``config_id`` pins one kernel configuration (one with BN >= 64), ``max_ctas`` caps the
+    CTAs (0: all SMs); default is the dispatcher."""
+    _contiguous_cuda(a=a, b=b, c=c, offs=offs)
+    g, t, n, k = check_grouped_nn_operands(a, b, offs, acc)
+    if c.dtype != a.dtype or tuple(c.shape) != (t, n):
+        raise B200HgemmError(f"c must be {a.dtype} {[t, n]}, got {c.dtype} {tuple(c.shape)}")
+    _bwd_call("cuda_l2_b200_grouped_bwd_nn", _bwd_variant(a.dtype, acc), (a.data_ptr(), b.data_ptr(), c.data_ptr(),
+              offs.data_ptr()), (g, t, n, k), config_id, group_m, max_ctas, stream)
+
+
+def gemm_grouped_wgrad(a, b, c, offs, acc: str | int = "fp32", config_id: int | None = None, group_m: int = 0,
+                       max_ctas: int = 0, stream: int | None = None) -> None:
+    """c[g] = a[start_g:end_g]^T @ b[start_g:end_g] for every group g (the weight gradient of the grouped product), a
+    [T,M] and b [T,N] fp16 or bf16 with fp32 accumulation, c [G,M,N], all contiguous CUDA tensors. ``offs``: int32
+    CUDA tensor [G] of cumulative group ends, read by the kernel and clamped as for :func:`gemm_grouped`. Every matrix
+    of c is written: an empty group's with zeros, and T == 0 zero-fills c without a launch. ``config_id`` pins one
+    kernel configuration (one with BN >= 64), ``max_ctas`` caps the CTAs (0: all SMs); default is the dispatcher."""
+    _contiguous_cuda(a=a, b=b, c=c, offs=offs)
+    g, t, m, n = check_grouped_wgrad_operands(a, b, offs, acc)
+    if c.dtype != a.dtype or tuple(c.shape) != (g, m, n):
+        raise B200HgemmError(f"c must be {a.dtype} {[g, m, n]}, got {c.dtype} {tuple(c.shape)}")
+    _bwd_call("cuda_l2_b200_grouped_bwd_wgrad", _bwd_variant(a.dtype, acc), (a.data_ptr(), b.data_ptr(), c.data_ptr(),
+              offs.data_ptr()), (g, t, m, n), config_id, group_m, max_ctas, stream)
+
+
+def grouped_nn_select(variant: int, g: int, t: int, n: int, k: int) -> tuple[int, int]:
+    """(config id, rasterisation group) the dispatcher of :func:`gemm_grouped_nn` uses."""
+    return _select(grouped_bwd_lib().cuda_l2_b200_grouped_bwd_nn_select, variant, g, t, n, k)
+
+
+def grouped_wgrad_select(variant: int, g: int, t: int, m: int, n: int) -> tuple[int, int]:
+    """(config id, rasterisation group) the dispatcher of :func:`gemm_grouped_wgrad` uses."""
+    return _select(grouped_bwd_lib().cuda_l2_b200_grouped_bwd_wgrad_select, variant, g, t, m, n)
+
+
+def grouped_wgrad_schedule(config_id: int, t: int, m: int, n: int, offs, num_sms: int = 132) -> dict:
+    """Host-side view of a K-grouped launch's schedule (no GPU needed; the kernel walks the same code), with the
+    launcher's default rasterisation. ``offs``: the cumulative group ends (a sequence of ints, G of them).
+
+    Returns ``{"workers": W, "units": [[(group, m_block, n_block, k_blocks), ...] per worker]}``; blocks are cluster
+    blocks, k_blocks the tile's 64-row k-blocks of its group (0 for an empty group)."""
+    fn = grouped_bwd_lib().cuda_l2_b200_grouped_bwd_wgrad_schedule
+    ends = (ctypes.c_int * len(offs))(*offs)
+    args = (config_id, len(offs), t, m, n, ends, num_sms)
+    nw = ctypes.c_int()
+    cap = 256
+    buf = (ctypes.c_int * (4 * cap))()
+    st = fn(*args, 0, buf, cap, ctypes.byref(nw))
+    if st < 0:
+        raise B200HgemmError(f"cuda_l2_b200_grouped_bwd_wgrad_schedule failed: status {st}")
+    units = []
+    for w in range(nw.value):
+        cnt = fn(*args, w, buf, cap, None)
+        if cnt > cap:
+            cap = cnt
+            buf = (ctypes.c_int * (4 * cap))()
+            cnt = fn(*args, w, buf, cap, None)
+        units.append([tuple(buf[4 * j:4 * j + 4]) for j in range(cnt)])
+    return {"workers": nw.value, "units": units}
+
+
+def grouped_bwd_launch_count() -> int:
+    return int(grouped_bwd_lib().cuda_l2_b200_grouped_bwd_launch_count())
 
 
 def fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs, config_id: int | None = None, group_m: int = 0,

@@ -501,9 +501,9 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   cfg.attrs = attr;
   cfg.numAttrs = na;
   const int aux = block_scaled<Cfg>() ? a.ld_a : a.plan.sk_tiles;   // the kernel's aux_arg
-  // batched kernels (plain only) take the batch count as splits_arg and the row counts as splitk_ctr; grouped kernels
-  // the group count and the offsets
-  constexpr bool kTileList = batched<Cfg>() || grouped<Cfg>();
+  // batched kernels (plain only) take the batch count as splits_arg and the row counts as splitk_ctr; grouped and
+  // K-grouped kernels the group count and the offsets
+  constexpr bool kTileList = batched<Cfg>() || grouped<Cfg>() || k_grouped<Cfg>();
   const int splits_arg = kTileList ? a.batches : a.plan.splits;
   unsigned* ctr = kTileList ? reinterpret_cast<unsigned*>(const_cast<int*>(a.masked_m)) : a.ctr;
   cudaError_t e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
@@ -627,7 +627,19 @@ inline int validate_grouped(GemmType type, const void* A, const void* Bt, const 
   return validate(type, A, Bt, C, scales, T > 0 ? T : 1, N, K, ld_a, 1, worst_tiles, offs);
 }
 
-// One launch of a Batched<> or Grouped<> configuration, which walks the flat tile list of its Cfg::Cursor over
+// The argument rules of a K-grouped launch (GroupedK<>): A [T, M], B [T, N] and C [G, M, N] with 16-byte rows (M % 8 and
+// N % 8: validate's rule for K and N, with M in K's place), G >= 1 groups whose offsets are non-null and 4-byte aligned,
+// T >= 0 (an empty reduction), and a tile list (`tiles`, the dense G x M x N one) of at most INT_MAX tiles. With T == 0
+// neither operand is read, and A and B may be null (torch's pointer for a tensor without elements).
+inline int validate_k_grouped(GemmType type, const void* A, const void* B, const void* C, const int* offs, int groups,
+                              int T, int M, int N, long long tiles) {
+  if (!C || !offs || (T != 0 && (!A || !B))) return kNullPointer;
+  if (T < 0 || groups < 1) return kBadShape;
+  if (T == 0) A = B = C;   // not read
+  return validate(type, A, B, C, Scales{nullptr, nullptr}, M, N, M, 0, 1, tiles, offs);
+}
+
+// One launch of a Batched<>, Grouped<> or GroupedK<> configuration, which walks the flat tile list of its Cfg::Cursor over
 // `count` matrices or groups. No L2 eviction hints: which operand is re-read depends on the batch or group as much as
 // on the shapes. rows == 0 launches nothing.
 //   Batched<>: C[b] = A[b] Bt[b]^T for b < count, A [count, rows, K], Bt [count, N, K], C [count, rows, N], all
@@ -642,28 +654,53 @@ inline int validate_grouped(GemmType type, const void* A, const void* Bt, const 
 //   Batched<BlockScaled<>> (e4m3 operands): the batched product, with one [ceil(K/128), ld_a] block of A's scales per
 //   matrix, stacked (value (b, m, kb) at scales.a[(b * ceil(K/128) + kb) * ld_a + m]), and one [ceil(N/128),
 //   ceil(K/128)] matrix of Bt's scales per batch (`scales.b`).
+//   Grouped<RowMajorB<>>: Grouped<>'s product with `Bt` read as B [count, K, N] row-major: C[start_g : end_g] =
+//   A[start_g : end_g] B[g].
+//   GroupedK<> (`rows` is M, `K` is T): C[g] = A[start_g : end_g]^T B[start_g : end_g] for g < count, A [T, M] and
+//   `Bt` as B [T, N] row-major, C [count, M, N], the groups as for Grouped<>. Every matrix of C is written, an empty
+//   group's with +0.0; T == 0 zero-fills C on the stream and launches nothing (a map needs at least one row).
 template <class Cfg>
 int launch_list(const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
                 cudaStream_t stream, int group_m = 0, int max_ctas = 0, Scales scales = Scales{nullptr, nullptr},
                 int ld_a = 0) {
-  static_assert(batched<Cfg>() || grouped<Cfg>(), "a Batched<> or Grouped<> configuration");
+  static_assert(batched<Cfg>() || grouped<Cfg>() || k_grouped<Cfg>(), "a Batched<>, Grouped<> or GroupedK<> configuration");
   constexpr GemmType kType = gemm_type<Cfg>();
   const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
-  int st = grouped<Cfg>() ? validate_grouped(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a)
-                          : validate(kType, A, Bt, C, scales, rows, N, K, ld_a, count, tiles, list);
+  int st = k_grouped<Cfg>() ? validate_k_grouped(kType, A, Bt, C, list, count, K, rows, N, tiles)
+           : grouped<Cfg>() ? validate_grouped(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a)
+                            : validate(kType, A, Bt, C, scales, rows, N, K, ld_a, count, tiles, list);
   if (st != kOk || rows == 0) return st;
+  const Elem elem = traits(kType).operand, output = traits(kType).output;
+  if constexpr (k_grouped<Cfg>()) {
+    if (K == 0) {   // no row to reduce over: every matrix of C is zero
+      const cudaError_t e = cudaMemsetAsync(C, 0, size_t(count) * size_t(rows) * size_t(N) * elem_bytes(output),
+                                            stream);
+      return e == cudaSuccess ? kOk : int(e);
+    }
+  }
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
 
   LaunchArgs a{};
   MapCache& cache = map_cache();
-  const Elem elem = traits(kType).operand, output = traits(kType).output;
-  // Bt is one N x K matrix per batch or group; A and C are one matrix per batch (3-D maps, so that TMA clips each box
-  // at its own matrix's edge), or the rows of all groups (2-D maps)
+  if constexpr (k_grouped<Cfg>()) {
+    // A [T, M] and B [T, N] in boxes of 64 columns (one atom column) by this CTA's K slice; C one M x N matrix per group
+    if ((st = cache.get(A, K, rows, Cfg::A_K_ROWS, &a.ma, 64, elem)) != kOk) return st;
+    if ((st = cache.get(Bt, K, N, Cfg::B_K_ROWS, &a.mb, 64, elem)) != kOk) return st;
+    if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, count)) != kOk) return st;
+  } else {
+  // Bt is one N x K matrix per batch or group (row-major B: one K x N matrix per group, in atom-column boxes); A and C
+  // are one matrix per batch (3-D maps, so that TMA clips each box at its own matrix's edge), or the rows of all groups
+  // (2-D maps)
   const int depth = batched<Cfg>() ? count : 0;
   if ((st = cache.get(A, rows, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem, depth)) != kOk) return st;
-  if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, count)) != kOk) return st;
+  if constexpr (row_major_b<Cfg>()) {
+    if ((st = cache.get(Bt, K, N, Cfg::B_K_ROWS, &a.mb, 64, elem, count)) != kOk) return st;
+  } else {
+    if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, count)) != kOk) return st;
+  }
   if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, depth)) != kOk) return st;
+  }
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = list_plan<Cfg>(tiles, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
   a.M = rows; a.N = N; a.K = K;

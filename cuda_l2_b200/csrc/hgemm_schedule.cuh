@@ -220,6 +220,63 @@ struct GroupCursor {
   }
 };
 
+// K-grouped launches (the weight gradient of the grouped product: C[g] = A[start_g : end_g]^T B[start_g : end_g] for
+// g < num_groups, plain schedule): the reduction runs over the group's own rows of A [T, M] and B [T, N], with the
+// groups of GroupCursor (end_g = clamp(offs[g], start_g, T)). The output is one M x N matrix per group, so the list is
+// BatchCursor's dense one over num_groups matrices; what differs per tile is its k-range: ceil((end_g - start_g) / 64)
+// k-blocks of 64 rows from start_g on (none for an empty group). unit() gives a work unit that k-range: the producer,
+// the consumers and the host's schedule view all bound a unit through it. locate() returns the group as `batch` and M
+// as `rows`, and leaves the group's rows in [start, end).
+struct GroupKCursor {
+  static constexpr int kRowsPerKBlock = 64;   // kBlockK of the 16-bit kernels
+  const int* offs;   // cumulative ends of the groups (torch._grouped_mm's offs)
+  int num_groups, M, T, block_rows, n_blocks, group_m, m_blocks;
+  int group, start, end;   // the current group: rows [start, end) of A and B
+
+  __host__ __device__ GroupKCursor(const int* offs_, int num_groups_, int M_, int T_, int block_rows_, int n_blocks_,
+                                   int group_m_)
+      : offs(offs_), num_groups(num_groups_), M(M_), T(T_), block_rows(block_rows_), n_blocks(n_blocks_),
+        group_m(group_m_), m_blocks((M_ + block_rows_ - 1) / block_rows_), group(0), start(0) {
+    end = end_of(0, 0);
+  }
+
+  // The length of the list of a launch of Cfg over num_groups matrices of M x N: BatchCursor's dense list.
+  template <class Cfg>
+  static constexpr long long max_tiles(int num_groups, int M, int N) {
+    return BatchCursor::max_tiles<Cfg>(num_groups, M, N);
+  }
+
+  __host__ __device__ __forceinline__ int end_of(int g, int s) const {
+    if (g >= num_groups) return s;
+    const int e = offs[g];
+    return e < s ? s : e < T ? e : T;
+  }
+  __host__ __device__ __forceinline__ int total() const { return num_groups * m_blocks * n_blocks; }
+  // tile t < total() of the list; t must not be smaller than at the previous call
+  __host__ __device__ __forceinline__ BatchTile locate(int t) {
+    const int per = m_blocks * n_blocks;
+    const int g = t / per;
+    while (group < g) {
+      start = end;
+      end = end_of(++group, start);
+    }
+    BatchTile r;
+    r.batch = g;
+    r.rows = M;
+    r.tc = tile_coord(t - g * per, m_blocks, n_blocks, group_m);
+    return r;
+  }
+  // the k-blocks of the current group
+  __host__ __device__ __forceinline__ int k_blocks() const { return (end - start + kRowsPerKBlock - 1) / kRowsPerKBlock; }
+  // the tile of unit u (from WorkIter's plain schedule), with u's k-range set to the tile's group: [0, k_blocks())
+  __host__ __device__ __forceinline__ BatchTile unit(WorkUnit& u) {
+    const BatchTile r = locate(u.tile);
+    u.kb0 = 0;
+    u.kb1 = k_blocks();
+    return r;
+  }
+};
+
 // What the kernels of the other variants hold in place of a BatchCursor: nothing.
 struct NoBatches {
   __host__ __device__ NoBatches(const int*, int, int, int, int, int) {}

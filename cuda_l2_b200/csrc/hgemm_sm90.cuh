@@ -34,6 +34,7 @@
 #include <cuda.h>          // CUtensorMap (type only; the encoder is fetched at run time)
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <type_traits>
 
 #include "hgemm_schedule.cuh"
 #include "ptx_sm90.cuh"
@@ -99,8 +100,8 @@ struct Config {
   // which K-decompositions this configuration's kernel carries
   static constexpr bool STREAM_K = CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
   static constexpr bool SPLIT_K = STREAM_K && CTA_GROUP_ == 1;
-  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>, RowMajorB<>) override these
-  static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false, ROW_MAJOR_B = false;
+  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>, RowMajorB<>, GroupedK<>) override these
+  static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false, ROW_MAJOR_B = false, K_GROUPED = false;
   using Cursor = NoBatches;   // the flat tile list the kernel walks (hgemm_schedule.cuh): none
   static constexpr int EPI_BYTES = 8 * EPI_ROWS * 64 * 2;    // 8 consumer warps x one staging buffer (sized for EPI_N = 64)
   static constexpr int BAR_BYTES = 256;
@@ -229,6 +230,48 @@ struct RowMajorB : Base {
 };
 template <class Cfg>
 __host__ __device__ constexpr bool row_major_b() { return Cfg::ROW_MAJOR_B; }
+
+// Grouped<RowMajorB<...>> (libb200_grouped_bwd.so, the input gradient of the grouped product): C[start_g : end_g] =
+// A[start_g : end_g] B[g] with B [G, K, N] row-major, one expert's weight [N_model, K_model] read in place. A and the
+// epilogue are Grouped<>'s; B is RowMajorB<>'s atom columns, loaded from the 3-D map {N, K, G}, so each expert's
+// matrix clips its own boxes and K is zero-filled per expert as in 2-D. Nothing else changes: the partial
+// specialisation only names the combination (RowMajorB<> itself still refuses a grouped, batched or e4m3 base).
+template <class Base>
+struct Grouped<RowMajorB<Base>> : RowMajorB<Base> {
+  static constexpr bool GROUPED = true;
+  using Cursor = GroupCursor;
+};
+
+// K-grouped row-major operands (libb200_grouped_bwd.so, the weight gradient of the grouped product):
+// C[g] = A[start_g : end_g]^T B[start_g : end_g] for g < G, A [T, M] and B [T, N] row-major, C [G, M, N]. The reduction
+// runs over the group's own rows (GroupKCursor), so both operands are MN-major: A is read with imm-trans-a = 1 in
+// CTA_M / 64 SW128 atom columns of 64 M x 64 K rows (8 KB each, the same bytes as the K-major stage), loaded as
+// {64, A_K_ROWS} boxes of A's {M, T} map; the CTAs of a cluster row multicast A sliced along K, A_K_ROWS rows each,
+// as RowMajorB<> does for B along the cluster column. B is RowMajorB<>'s over B's {N, T} map, C the batched 3-D map
+// {N, M, G}. A group's last k-block may hold r < 64 of its rows; rows [r, 64) of that stage belong to the next group
+// (or lie past T, already zero), and the consumers zero them in both operands before the wgmma reads them (0 * Inf
+// is NaN). A group without rows gives a tile of +0.0. Plain schedule, fp32 accumulation.
+template <class Base>
+struct GroupedK : Base {
+  static constexpr bool K_GROUPED = true;
+  using Cursor = GroupKCursor;
+  static_assert(Base::ROW_MAJOR_B && !Base::GROUPED && Base::ACC_F32, "K-grouped: RowMajorB<> 16-bit configurations, fp32 accumulation");
+  static constexpr int A_ATOMS = Base::CTA_M / 64;                    // atom columns of an A stage
+  static constexpr int A_K_ROWS = kBlockK / Base::CLUSTER_N;          // K rows of each atom column this CTA loads
+  static_assert(A_K_ROWS % 8 == 0, "K slices of whole 8-row swizzle groups");
+  static_assert(A_ATOMS * Base::B_ATOM_BYTES == Base::A_STAGE_BYTES, "the stage holds the same bytes as the K-major one");
+};
+template <class Cfg>
+__host__ __device__ constexpr bool k_grouped() { return Cfg::K_GROUPED; }
+
+// The tile list a kernel of Cfg walks (Cfg::Cursor) over `count` matrices or groups; the K-grouped list also needs the
+// reduction's rows, K.
+template <class Cfg>
+__host__ __device__ __forceinline__ typename Cfg::Cursor make_cursor(const int* list, int count, int M, int K,
+                                                                     int block_rows, int n_blocks, int group_m) {
+  if constexpr (k_grouped<Cfg>()) return typename Cfg::Cursor(list, count, M, K, block_rows, n_blocks, group_m);
+  else return typename Cfg::Cursor(list, count, M, block_rows, n_blocks, group_m);
+}
 
 // Scales of an e4m3 launch, in device memory (null for the 16-bit operand types). Per tensor: one fp32 value each.
 // Rowwise: `a` holds M values (one per row of A and C), `b` N values (one per row of Bt, i.e. per column of C), both
@@ -360,10 +403,26 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
   }
   if (lane == 0) {
     if (row0 < M && col0 < N) {   // rows/cols past the edge are clipped by the tensor map
-      if constexpr (batched<Cfg>()) tma_store_3d(tmap_c, epi_buf, col0, row0, batch);
+      if constexpr (batched<Cfg>() || k_grouped<Cfg>()) tma_store_3d(tmap_c, epi_buf, col0, row0, batch);
       else tma_store_2d(tmap_c, epi_buf, col0, row0);
     }
     tma_store_commit();
+  }
+}
+
+// The tile of an empty group of a K-grouped kernel (GroupedK<>): +0.0 in this warp's MR x 16 rows from row0 (of
+// matrix `batch` of C [., M, N]) and BN columns from col0, clipped at M and N, with 16-byte generic stores.
+template <class Cfg>
+__device__ __forceinline__ void zero_tile_store(__half* __restrict__ c, int batch, int row0, int col0, int M, int N,
+                                                int lane) {
+  constexpr int CPR = Cfg::BN / 8;   // 16-byte chunks per row
+#pragma unroll 1
+  for (int r = 0; r < Cfg::M_REP; ++r) {
+#pragma unroll 1
+    for (int i = lane; i < Cfg::EPI_ROWS * CPR; i += 32) {
+      const int gm = row0 + r * 64 + i / CPR, gn = col0 + 8 * (i % CPR);
+      if (gm < M && gn < N) *reinterpret_cast<uint4*>(c + (size_t(batch) * M + gm) * N + gn) = make_uint4(0u, 0u, 0u, 0u);
+    }
   }
 }
 
@@ -640,7 +699,8 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   [[maybe_unused]] const uint32_t smem_scales = smem_bar + Cfg::BAR_BYTES;   // block scales: [STAGES] scale stages
   constexpr bool kBatched = batched<Cfg>();
   constexpr bool kGrouped = grouped<Cfg>();
-  constexpr bool kTileList = kBatched || kGrouped;   // the schedule walks a cursor's flat tile list
+  constexpr bool kKGrouped = k_grouped<Cfg>();       // A [T, M] MN-major too, k-range per group (GroupedK<>)
+  constexpr bool kTileList = kBatched || kGrouped || kKGrouped;   // the schedule walks a cursor's flat tile list
   constexpr bool kRowMajorB = row_major_b<Cfg>();    // B [K, N] in MN-major atom columns (RowMajorB<>)
   static_assert(!kTileList || KMODE == kPlain, "batched / grouped: plain schedule only");
   // grouped kernels: the group count and the offsets, in the same places (M is then T, the rows of A and C)
@@ -711,12 +771,13 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       const uint32_t b_slice = uint32_t(mi) * (Cfg::B_BOX_ROWS * kBlockK * 2);
       int stage = 0; uint32_t phase = 0;
       // batched: the list of (batch, cluster block) tiles, summed over the row counts (read after the dependency wait)
-      [[maybe_unused]] Cursor batches(masked_m, num_batches, M, Cfg::CTA_M * EM, num_n_blocks, group_m);
+      [[maybe_unused]] Cursor batches = make_cursor<Cfg>(masked_m, num_batches, M, K, Cfg::CTA_M * EM, num_n_blocks, group_m);
       WorkIter work(worker, num_workers, kTileList ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
       WorkUnit u;
       while (work.next(u)) {
         [[maybe_unused]] BatchTile bt{0, M, TileCoord{0, 0}};
-        if constexpr (kTileList) bt = batches.locate(u.tile);
+        if constexpr (kKGrouped) bt = batches.unit(u);   // the group's k-range; none for an empty group
+        else if constexpr (kTileList) bt = batches.locate(u.tile);
         const TileCoord tc = kTileList ? bt.tc : tile_coord(u.tile, num_m_blocks, num_n_blocks, group_m);
         const int m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M + cn * Cfg::A_BOX_ROWS;
         const int n0 = (tc.n_blk * CN + cn) * BN + mi * Cfg::B_BOX_ROWS;
@@ -771,8 +832,43 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
               const int ma = batches.start + m0, g = bt.batch;
               if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, ma, mask_a, hint_a);
               else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, ma, hint_a);
+              if constexpr (kRowMajorB) {
+                // B [G, K, N]: this CTA's K slice of every atom column of the group's matrix (Grouped<RowMajorB<>>)
+                const uint32_t dst = smem_b + stage * Cfg::B_STAGE_BYTES + uint32_t(mi) * (Cfg::B_K_ROWS * kBlockKBytes);
+                const int nb = (tc.n_blk * CN + cn) * BN, kr = kb * Cfg::BLOCK_K + mi * Cfg::B_K_ROWS;
+#pragma unroll
+                for (int j = 0; j < Cfg::B_ATOMS; ++j) {
+                  if constexpr (EM > 1)
+                    tma_load_3d_mcast_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, g, mask_b, hint_b);
+                  else
+                    tma_load_3d_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, g, hint_b);
+                }
+              } else {
               if constexpr (EM > 1) tma_load_3d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, g, mask_b, hint_b);
               else tma_load_3d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, g, hint_b);
+              }
+            } else if constexpr (kKGrouped) {
+              // A [T, M] and B [T, N], rows from the group's first row on: this CTA's K slice of every atom column of
+              // A (multicast to its cluster row) and of B (to its cluster column)
+              const int t0 = batches.start + kb * Cfg::BLOCK_K;
+              const uint32_t da = smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(cn) * (Cfg::A_K_ROWS * kBlockKBytes);
+              const int ma = (tc.m_blk * EM + mi) * Cfg::CTA_M, ka = t0 + cn * Cfg::A_K_ROWS;
+#pragma unroll
+              for (int j = 0; j < Cfg::A_ATOMS; ++j) {
+                if constexpr (CN > 1)
+                  tma_load_2d_mcast_hint(da + j * Cfg::B_ATOM_BYTES, &tmap_a, full, ma + 64 * j, ka, mask_a, hint_a);
+                else
+                  tma_load_2d_hint(da + j * Cfg::B_ATOM_BYTES, &tmap_a, full, ma + 64 * j, ka, hint_a);
+              }
+              const uint32_t db = smem_b + stage * Cfg::B_STAGE_BYTES + uint32_t(mi) * (Cfg::B_K_ROWS * kBlockKBytes);
+              const int nb = (tc.n_blk * CN + cn) * BN, kr = t0 + mi * Cfg::B_K_ROWS;
+#pragma unroll
+              for (int j = 0; j < Cfg::B_ATOMS; ++j) {
+                if constexpr (EM > 1)
+                  tma_load_2d_mcast_hint(db + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, mask_b, hint_b);
+                else
+                  tma_load_2d_hint(db + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, hint_b);
+              }
             } else {
             if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, mask_a, hint_a);
             else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, hint_a);
@@ -809,10 +905,12 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
   } else {
     setmaxnreg_inc<kConsumerRegs>();
     // ===== consumers: warpgroup wg owns rows [wg * 64 * MR, (wg + 1) * 64 * MR) of the CTA's tile =====
-    using W = Wgmma<BN, Cfg::ACC_F32, Cfg::BF16 && !Cfg::E4M3, Cfg::E4M3, kRowMajorB>;
+    using W = typename std::conditional<kKGrouped, Wgmma<BN, true, Cfg::BF16, false, true, true>,
+                                        Wgmma<BN, Cfg::ACC_F32, Cfg::BF16 && !Cfg::E4M3, Cfg::E4M3, kRowMajorB>>::type;
     // B's descriptor and its advance per k16 step (in 16-byte units): K-major, +32 B; MN-major (RowMajorB<>), +16 K
-    // rows of 128 B, atom columns 8 KB apart
+    // rows of 128 B, atom columns 8 KB apart. The same for A: MN-major in the K-grouped kernels (GroupedK<>).
     constexpr int kDescBStep = kRowMajorB ? 16 * kBlockKBytes / 16 : 2;
+    constexpr int kDescAStep = kKGrouped ? 16 * kBlockKBytes / 16 : 2;
     using Reg = typename W::Reg;
     constexpr int NR = W::kRegs;
     const int wg = warp / 4 - 1;
@@ -844,10 +942,21 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       }
     };
     int stage = 0; uint32_t phase = 0;
-    [[maybe_unused]] Cursor batches(masked_m, num_batches, M, Cfg::CTA_M * EM, num_n_blocks, group_m);
+    [[maybe_unused]] Cursor batches = make_cursor<Cfg>(masked_m, num_batches, M, K, Cfg::CTA_M * EM, num_n_blocks, group_m);
     WorkIter work(worker, num_workers, kTileList ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
     WorkUnit u;
     while (work.next(u)) {
+      if constexpr (kKGrouped) {
+        const BatchTile zt = batches.unit(u);   // the group's k-range, as the producer bounds it
+        if (u.kb1 == 0) {
+          // An empty group: the producer loaded nothing, and acc still holds the previous unit's sums (only a first
+          // wgmma's scale-d = 0 clears it). Its tile of +0.0 goes straight to C; acc is left alone, which keeps the
+          // accumulators out of a branch that ptxas would otherwise serve from local memory.
+          zero_tile_store<Cfg>(c_raw, zt.batch, (zt.tc.m_blk * EM + mi) * Cfg::CTA_M + wg * MR * 64 + wq * 16,
+                               (zt.tc.n_blk * CN + cn) * BN, M, N, lane);
+          continue;
+        }
+      }
       if constexpr (kBlock) {
         // ---- block-scaled main loop: each k-block's wgmma group sums into `part` (its first wgmma overwrites it),
         // is retired, and is promoted into acc with fp32(sa[m] * sb): acc = p * s on the unit's first k-block (keeps
@@ -893,7 +1002,29 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
       int prev = -1;
       for (int kb = u.kb0; kb < u.kb1; ++kb) {
         mbar_wait(bar_full + 8 * stage, phase);
-        const uint64_t da = make_smem_desc(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg * MR) * (64 * kBlockK * 2));
+        if constexpr (kKGrouped) {
+          // the group's last k-block: rows [r, 64) of every atom column of both operands belong to the next group (or
+          // lie past T). A K row of an SW128 atom column is one contiguous 128-byte row, so each is one byte range.
+          const int r = (batches.end - batches.start) - kb * Cfg::BLOCK_K;
+          if (r < Cfg::BLOCK_K) {
+            const uint32_t a0 = smem_a + stage * Cfg::A_STAGE_BYTES, b0 = smem_b + stage * Cfg::B_STAGE_BYTES;
+            // 16 bytes per thread and atom column, 4 KB per pass over the 256 consumer threads: at most two passes
+#pragma unroll 1
+            for (uint32_t o = uint32_t(r * kBlockKBytes + 16 * t); o < uint32_t(Cfg::B_ATOM_BYTES); o += 16u * kConsumerThreads) {
+#pragma unroll
+              for (int j = 0; j < Cfg::A_ATOMS; ++j) st_shared_zero_v4(a0 + uint32_t(j * Cfg::B_ATOM_BYTES) + o);
+#pragma unroll
+              for (int j = 0; j < Cfg::B_ATOMS; ++j) st_shared_zero_v4(b0 + uint32_t(j * Cfg::B_ATOM_BYTES) + o);
+            }
+            fence_proxy_async_smem();   // the generic-proxy zeros before the wgmma's (async-proxy) reads
+            asm volatile("bar.sync 2, %0;" ::"n"(kConsumerThreads) : "memory");
+          }
+        }
+        uint64_t da;
+        if constexpr (kKGrouped)
+          da = make_smem_desc_mn(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg * MR) * (64 * kBlockK * 2), 64 * kBlockKBytes);
+        else
+          da = make_smem_desc(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg * MR) * (64 * kBlockK * 2));
         uint64_t db;
         if constexpr (kRowMajorB) db = make_smem_desc_mn(smem_b + stage * Cfg::B_STAGE_BYTES, 64 * kBlockKBytes);
         else db = make_smem_desc(smem_b + stage * Cfg::B_STAGE_BYTES);
@@ -904,7 +1035,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
         for (int k = 0; k < kBlockK / kWgmmaK; ++k) {   // four wgmmas of 32 bytes of K each, for every operand type
 #pragma unroll
           for (int r = 0; r < MR; ++r)
-            W::mma(da + uint64_t(r * ((64 * kBlockK * 2) >> 4) + 2 * k), db + uint64_t(kDescBStep * k), acc[r],
+            W::mma(da + uint64_t(r * ((64 * kBlockK * 2) >> 4) + kDescAStep * k), db + uint64_t(kDescBStep * k), acc[r],
                    (kb > u.kb0 || k > 0) ? 1u : 0u);
         }
         wgmma_commit();

@@ -253,6 +253,10 @@ __device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
 __device__ __forceinline__ void st_shared_v2f(uint32_t addr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
+// 16 zero bytes (addr 16-byte aligned)
+__device__ __forceinline__ void st_shared_zero_v4(uint32_t addr) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(addr), "r"(0u) : "memory");
+}
 // load from the shared memory of any CTA in the cluster (address from mapa)
 __device__ __forceinline__ float4 ld_dsmem_v4f(uint32_t cluster_addr) {
   float4 v;

@@ -20,6 +20,16 @@ the nearest grid shape — so deployment is a plain operator:
   groups, ``b_kmajor`` [G,N,K] one weight per group, ``offs`` the int32 cumulative group ends on the GPU; returns
   [T,N] — ``torch._grouped_mm(a, b_kmajor.transpose(-2, -1), offs=offs)`` in one launch, the MoE prefill layout.
   Inference only.
+* ``torch.ops.cuda_l2_b200.hgemm_grouped_nn(a, b, offs, acc)``: ``a`` [T,K] in the same groups times ``b`` [G,K,N]
+  row-major per group -> [T,N] (``torch._grouped_mm(a, b, offs=offs)``): an expert weight stack [G, N_model,
+  K_model] is read in place as the B of the input gradient. Rows at or past ``offs[-1]`` are unspecified.
+* ``torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(a, b, offs, acc)``: ``a`` [T,M] and ``b`` [T,N] in the same groups ->
+  [G,M,N], ``a[start_g:end_g]^T @ b[start_g:end_g]`` per group (``torch._grouped_mm(a.t(), b, offs=offs)``), the
+  weight gradient; an empty group's matrix is zero.
+* :func:`grouped_linear` (``torch.ops.cuda_l2_b200.grouped_linear(x, w, offs, acc)``) and :class:`B200GroupedLinear`:
+  ``hgemm_grouped``'s product with a gradient. The forward is ``hgemm_grouped``'s kernel; ``dX`` runs
+  ``hgemm_grouped_nn`` on the weight stack in place and ``dW`` ``hgemm_grouped_wgrad``, so a training step of the
+  experts copies no operand. fp16 or bf16 with fp32 accumulation.
 * :class:`B200Linear`: ``y = x @ W^T (+ b)`` for any leading dimensions; :func:`replace_linear_modules` swaps the
   eligible ``nn.Linear`` layers of a model in place.
 * ``torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)``: ``float8_e4m3fn`` operands in the same
@@ -46,8 +56,8 @@ the nearest grid shape — so deployment is a plain operator:
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernels, so a fine-tuning
 loop works: ``hgemm``'s input gradient reads the weight in place through the row-major B kernels, and its weight
-gradient pays one transposed copy (of the output gradient). The FP8 operator has no gradient: a backward through it
-raises.
+gradient pays one transposed copy (of the output gradient). The grouped product trains through :func:`grouped_linear`
+(``hgemm_grouped`` itself stays inference only). The FP8 operators have no gradient: a backward through them raises.
 """
 from __future__ import annotations
 
@@ -280,7 +290,7 @@ def _hgemm_grouped_launch(c, a, b_kmajor, offs, acc="fp32", *, stream):
 
 
 _inference_op("hgemm_grouped", "(Tensor a, Tensor b_kmajor, Tensor offs, str acc='fp32') -> Tensor", _hgemm_grouped_shape,
-              _hgemm_grouped_launch, " (the weight gradient is a grouped product over K, a different kernel)")
+              _hgemm_grouped_launch, " (train through grouped_linear, the same product with a gradient)")
 
 
 def hgemm_grouped(a: torch.Tensor, b_kmajor: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -289,6 +299,158 @@ def hgemm_grouped(a: torch.Tensor, b_kmajor: torch.Tensor, offs: torch.Tensor, a
     offs=offs)``), in one launch. ``offs``: int32 CUDA tensor [G] of cumulative group ends, read by the kernel (no host
     synchronisation) and clamped to [previous end, T]. Rows at or past ``offs[-1]`` are unspecified. Inference only."""
     return torch.ops.cuda_l2_b200.hgemm_grouped(a, b_kmajor, offs, acc)
+
+
+# ------------------------------------------------------------------------------------------ grouped backward
+#                                                                                            (libb200_grouped_bwd.so)
+def _hgemm_grouped_nn_shape(a, b, offs, acc="fp32"):
+    _, t, n, _ = capi.check_grouped_nn_operands(a, b, offs, acc)
+    return (t, n), a.dtype
+
+
+def _hgemm_grouped_nn_launch(c, a, b, offs, acc="fp32", *, stream):
+    if b.shape[0] == 0 or c.shape[0] == 0:   # no group or no row
+        return
+    capi.gemm_grouped_nn(a.contiguous(), b.contiguous(), c, offs.contiguous(), acc, stream=stream)
+
+
+_inference_op("hgemm_grouped_nn", "(Tensor a, Tensor b, Tensor offs, str acc='fp32') -> Tensor", _hgemm_grouped_nn_shape,
+              _hgemm_grouped_nn_launch, " (it is a backward kernel: train through grouped_linear)")
+
+
+def hgemm_grouped_nn(a: torch.Tensor, b: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
+    """``a`` [T,K] by ``b`` [G,K,N] row-major over contiguous row groups -> [T,N]: rows [offs[g-1], offs[g]) of the
+    result are those rows of ``a`` times ``b[g]`` (``torch._grouped_mm(a, b, offs=offs)``), in one launch. ``offs`` as
+    for :func:`hgemm_grouped`. Rows at or past ``offs[-1]`` are unspecified. fp16 or bf16, fp32 accumulation."""
+    return torch.ops.cuda_l2_b200.hgemm_grouped_nn(a, b, offs, acc)
+
+
+def _hgemm_grouped_wgrad_shape(a, b, offs, acc="fp32"):
+    g, _, m, n = capi.check_grouped_wgrad_operands(a, b, offs, acc)
+    return (g, m, n), a.dtype
+
+
+def _hgemm_grouped_wgrad_launch(c, a, b, offs, acc="fp32", *, stream):
+    if c.numel() == 0:
+        return
+    capi.gemm_grouped_wgrad(a.contiguous(), b.contiguous(), c, offs.contiguous(), acc, stream=stream)
+
+
+_inference_op("hgemm_grouped_wgrad", "(Tensor a, Tensor b, Tensor offs, str acc='fp32') -> Tensor",
+              _hgemm_grouped_wgrad_shape, _hgemm_grouped_wgrad_launch,
+              " (it is a backward kernel: train through grouped_linear)")
+
+
+def hgemm_grouped_wgrad(a: torch.Tensor, b: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
+    """``a`` [T,M] and ``b`` [T,N] over contiguous row groups -> [G,M,N]: matrix g is ``a[start_g:end_g]^T @
+    b[start_g:end_g]`` (``torch._grouped_mm(a.t(), b, offs=offs)``), in one launch, with the groups of
+    :func:`hgemm_grouped`; an empty group's matrix is zero. fp16 or bf16, fp32 accumulation."""
+    return torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(a, b, offs, acc)
+
+
+torch.library.define(f"{_LIB}::grouped_linear", "(Tensor x, Tensor w, Tensor offs, str acc='fp32') -> Tensor")
+
+
+@torch.library.impl(f"{_LIB}::grouped_linear", "CUDA")
+def _grouped_linear_cuda(x, w, offs, acc="fp32"):
+    capi._bwd_variant(x.dtype, acc)   # a product the backward can run
+    return torch.ops.cuda_l2_b200.hgemm_grouped(x, w, offs, acc)
+
+
+@torch.library.impl(f"{_LIB}::grouped_linear", "CPU")
+def _grouped_linear_cpu(x, w, offs, acc="fp32"):
+    raise capi.B200HgemmError("cuda_l2_b200::grouped_linear has no CPU implementation (and no fallback): move the "
+                              "tensors to an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::grouped_linear")
+def _grouped_linear_fake(x, w, offs, acc="fp32"):
+    capi._bwd_variant(x.dtype, acc)
+    _, t, n, _ = capi.check_grouped_operands(x, w, offs, acc)
+    return x.new_empty((t, n))
+
+
+def _grouped_linear_backward(ctx, grad_y):
+    x, w, offs = ctx.saved_tensors
+    grad_x = grad_w = None
+    g = grad_y.contiguous()
+    # Y[s:e] = X[s:e] W[g]^T  =>  dX[s:e] = dY[s:e] W[g] (W [G, N, K] is a row-major B over the reduced N, read in
+    # place), dW[g] = dY[s:e]^T X[s:e] (the K-grouped product). Rows of dY at or past the last end are never read.
+    if ctx.needs_input_grad[0]:
+        # into zeros: rows of dX at or past the last end get no group and stay zero
+        grad_x = torch.zeros_like(x)
+        if x.shape[0] > 0:
+            with torch.cuda.device(x.device):
+                capi.gemm_grouped_nn(g, w.contiguous(), grad_x, offs.contiguous(), ctx.acc,
+                                     stream=torch.cuda.current_stream(x.device).cuda_stream)
+    if ctx.needs_input_grad[1]:
+        grad_w = torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(g, x, offs, ctx.acc)
+    return grad_x, grad_w, None, None
+
+
+def _grouped_linear_setup_context(ctx, inputs, output):
+    x, w, offs, acc = inputs
+    ctx.acc = acc
+    ctx.save_for_backward(x, w, offs)
+
+
+torch.library.register_autograd(f"{_LIB}::grouped_linear", _grouped_linear_backward,
+                                setup_context=_grouped_linear_setup_context)
+
+
+def grouped_linear(x: torch.Tensor, w: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
+    """The experts of a mixture-of-experts layer with a gradient: ``x`` [T,K] sorted into contiguous groups by the
+    int32 cumulative ends ``offs`` [G] (on the GPU), ``w`` [G,N,K] one weight per group -> [T,N], rows [offs[g-1],
+    offs[g]) being ``x[rows] @ w[g]^T``. The forward is :func:`hgemm_grouped`'s kernel, bit for bit; the backward
+    gives ``dX`` (rows at or past ``offs[-1]`` zero) from :func:`hgemm_grouped_nn` on ``w`` in place and ``dW`` from
+    :func:`hgemm_grouped_wgrad`, and never reads rows of the output gradient at or past ``offs[-1]``. Rows of the
+    result at or past ``offs[-1]`` are unspecified. fp16 or bf16 with fp32 accumulation."""
+    return torch.ops.cuda_l2_b200.grouped_linear(x, w, offs, acc)
+
+
+class B200GroupedLinear(nn.Module):
+    """Trainable experts of a mixture-of-experts layer: G ``nn.Linear`` weights [N, K] without bias, stacked as the
+    Parameter ``weight`` [G, N, K] (fp16 or bf16). ``forward(x, offs)`` takes the tokens sorted by expert, ``x`` [T, K],
+    and the int32 cumulative group ends ``offs`` [G] on the GPU, and runs :func:`grouped_linear`: no host
+    synchronisation in either direction. Rows at or past ``offs[-1]`` of the result are unspecified. Needs
+    K % 8 == 0 and N % 8 == 0."""
+
+    def __init__(self, num_groups: int, in_features: int, out_features: int, device=None,
+                 dtype: torch.dtype = torch.bfloat16, acc: str = "fp32"):
+        super().__init__()
+        self._check(num_groups, in_features, out_features, dtype, acc)
+        self.num_groups, self.in_features, self.out_features, self.acc = num_groups, in_features, out_features, acc
+        self.weight = nn.Parameter(torch.empty((num_groups, out_features, in_features), device=device, dtype=dtype))
+        bound = 1.0 / (in_features ** 0.5)
+        with torch.no_grad():
+            self.weight.uniform_(-bound, bound)
+
+    @staticmethod
+    def _check(g: int, k: int, n: int, dtype: torch.dtype, acc: str) -> None:
+        if g < 1 or not linear_supported(k, n, dtype):
+            raise capi.B200HgemmError(f"B200GroupedLinear needs G >= 1, fp16 / bf16 and feature counts divisible by 8, "
+                                      f"got G={g}, {k}->{n} {dtype}")
+        capi._bwd_variant(dtype, acc)
+
+    @classmethod
+    def from_weights(cls, w: torch.Tensor, acc: str = "fp32") -> "B200GroupedLinear":
+        """The experts of a weight stack ``w`` [G, N, K] (a Parameter or a tensor), sharing its storage: no copy."""
+        if w.dim() != 3:
+            raise capi.B200HgemmError(f"from_weights needs a weight stack [G, N, K], got {list(w.shape)}")
+        g, n, k = w.shape
+        cls._check(g, k, n, w.dtype, acc)
+        new = cls.__new__(cls)
+        nn.Module.__init__(new)
+        new.num_groups, new.in_features, new.out_features, new.acc = g, k, n, acc
+        new.weight = w if isinstance(w, nn.Parameter) else nn.Parameter(w)
+        return new
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+        return grouped_linear(x, self.weight, offs, self.acc)
+
+    def extra_repr(self) -> str:
+        return (f"num_groups={self.num_groups}, in_features={self.in_features}, out_features={self.out_features}, "
+                f"acc={self.acc}")
 
 
 def linear_supported(in_features: int, out_features: int, dtype: torch.dtype) -> bool:
@@ -658,6 +820,7 @@ class B200Fp8GroupedLinear(nn.Module):
                 f"out_dtype={self.out_dtype}")
 
 
-__all__ = ["hgemm", "hgemm_nn", "hgemm_batched", "hgemm_grouped", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
+__all__ = ["hgemm", "hgemm_nn", "hgemm_batched", "hgemm_grouped", "hgemm_grouped_nn", "hgemm_grouped_wgrad",
+           "grouped_linear", "B200GroupedLinear", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear",
            "fp8_grouped_gemm", "fp8_batched_gemm", "B200Fp8GroupedLinear"]
