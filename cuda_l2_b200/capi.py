@@ -351,13 +351,18 @@ def _check_k(a, b_kmajor, t: GemmType, n: int, k: int, k2: int, b_layout: str) -
                              f"got N={n}, K={k}")
 
 
-def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = (), strided_scale_a: bool = False
-                     ) -> tuple[int, int, int]:
-    """check_operands for c = a @ b_kmajor^T, all of them (scales included) contiguous CUDA tensors, c of shape [M,N].
-    ``strided_scale_a``: scale_a need not be contiguous (blockwise scales are read M-major)."""
-    for name, x in zip(("a", "b_kmajor", "c", "scale_a", "scale_b"), (a, b_kmajor, c, *scales)):
-        if not x.is_cuda or not (x.is_contiguous() or (strided_scale_a and name == "scale_a")):
+def _contiguous_cuda(**tensors) -> None:
+    """B200HgemmError unless every tensor given (None: not passed) is a contiguous CUDA tensor. ``scale_a`` need not be
+    contiguous: blockwise scales are read M-major, in place (:func:`blockwise_ld_a`)."""
+    for name, x in tensors.items():
+        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name == "scale_a")):
             raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+
+
+def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = ()) -> tuple[int, int, int]:
+    """check_operands for c = a @ b_kmajor^T, all of them (scales included, scale_a as :func:`_contiguous_cuda` allows)
+    CUDA tensors, c of shape [M,N]."""
+    _contiguous_cuda(a=a, b_kmajor=b_kmajor, c=c, **dict(zip(("scale_a", "scale_b"), scales)))
     m, n, k = check_operands(a, b_kmajor, c.dtype, acc, scales)
     if c.shape != (m, n):
         raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
@@ -415,9 +420,7 @@ def gemm_rowmajor(a, b, c, acc: str | int = "fp32", stream: int | None = None) -
     CUDA tensors. The dispatcher's TN choice for the shape runs, BN = 32 configurations mapped to a BN = 64 sibling."""
     import torch
 
-    for name, x in (("a", a), ("b", b), ("c", c)):
-        if not x.is_cuda or not x.is_contiguous():
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    _contiguous_cuda(a=a, b=b, c=c)
     m, n, k = check_rowmajor_operands(a, b, c.dtype, acc)
     if tuple(c.shape) != (m, n):
         raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b {tuple(b.shape)}, c {tuple(c.shape)}")
@@ -440,7 +443,7 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     b200_hgemm_run_config; ``max_ctas`` as in :func:`gemm_kmajor`); default is the dispatcher."""
     import torch
 
-    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b), strided_scale_a=True)
+    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b))
     out_bf16 = int(c.dtype == torch.bfloat16)
     granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
     if granularity == "blockwise":
@@ -493,12 +496,12 @@ def fp8block_launch_count() -> int:
     return int(fp8block_lib().b200_fp8block_launch_count())
 
 
-def _tile_list_schedule(schedule_units, *args) -> dict:
-    """Every worker's units from a tile-list library's ``schedule_units`` entry point, called with ``args`` (config id,
-    count, rows, N, K, host list, SMs) and then the worker and its buffer."""
+def _tile_list_schedule(schedule_units, ints: int, *args) -> dict:
+    """Every worker's units, ``ints`` values each, from a tile-list library's ``schedule_units`` entry point, called
+    with ``args`` (config id, the list's count, rows, N and K, host list, SMs) and then the worker and its buffer."""
     nw = ctypes.c_int()
     cap = 256
-    buf = (ctypes.c_int * (3 * cap))()
+    buf = (ctypes.c_int * (ints * cap))()
     st = schedule_units(*args, 0, buf, cap, ctypes.byref(nw))
     if st < 0:
         raise B200HgemmError(f"{schedule_units.__name__} failed: status {st}")
@@ -507,9 +510,9 @@ def _tile_list_schedule(schedule_units, *args) -> dict:
         cnt = schedule_units(*args, w, buf, cap, None)
         if cnt > cap:
             cap = cnt
-            buf = (ctypes.c_int * (3 * cap))()
+            buf = (ctypes.c_int * (ints * cap))()
             cnt = schedule_units(*args, w, buf, cap, None)
-        units.append([(buf[3 * j], buf[3 * j + 1], buf[3 * j + 2]) for j in range(cnt)])
+        units.append([tuple(buf[ints * j:ints * (j + 1)]) for j in range(cnt)])
     return {"workers": nw.value, "units": units}
 
 
@@ -522,10 +525,7 @@ def _tile_list_gemm(kind: str, a, b_kmajor, c, lst, acc: str | int, scales: tupl
     import torch
 
     list_name = "masked_m" if kind == "batched" else "offs"
-    for name, x in zip(("a", "b_kmajor", "c", *("scale_a", "scale_b")[:len(scales)], list_name),
-                       (a, b_kmajor, c, *scales, lst)):
-        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name == "scale_a")):
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
+    _contiguous_cuda(a=a, b_kmajor=b_kmajor, c=c, **dict(zip(("scale_a", "scale_b"), scales)), **{list_name: lst})
     out_dtype = c.dtype if scales else None
     if kind == "batched":
         count, rows, n, k = check_batched_operands(a, b_kmajor, acc, lst, out_dtype, scales)
@@ -610,7 +610,7 @@ def batched_schedule(config_id: int, b: int, m: int, n: int, k: int, masked_m=No
 
     Returns ``{"workers": W, "units": [[(batch, m_block, n_block), ...] per worker]}``; blocks are cluster blocks."""
     counts = None if masked_m is None else (ctypes.c_int * b)(*masked_m)
-    return _tile_list_schedule(batched_lib().b200_batched_schedule_units, config_id, b, m, n, k, counts, num_sms)
+    return _tile_list_schedule(batched_lib().b200_batched_schedule_units, 3, config_id, b, m, n, k, counts, num_sms)
 
 
 def batched_launch_count() -> int:
@@ -625,8 +625,6 @@ def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32", out_dtype
     name (the 2-D rules, :meth:`GemmType.fits`): a 16-bit one with the output dtype of the operands, or e4m3 operands
     with ``out_dtype`` fp16 / bf16 and two blockwise ``scales`` (:func:`scale_granularity` with ``groups``). Checks
     shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
-    import torch
-
     try:
         (t, k), (g, n, k2) = a.shape, b_kmajor.shape
     except ValueError:
@@ -636,9 +634,16 @@ def check_grouped_operands(a, b_kmajor, offs, acc: str | int = "fp32", out_dtype
     if scales:
         scale_granularity(t, n, *scales, k=k, groups=g)
     _check_k(a, b_kmajor, typ, n, k, k2, "[G, N, K]")
+    _check_offs(offs, g)
+    return g, t, n, k
+
+
+def _check_offs(offs, g: int) -> None:
+    """The group ends of a grouped product of ``g`` groups: an int32 tensor [g]. B200HgemmError otherwise."""
+    import torch
+
     if offs.dtype != torch.int32 or tuple(offs.shape) != (g,):
         raise B200HgemmError(f"offs must be an int32 tensor of shape [{g}], got {offs.dtype} {tuple(offs.shape)}")
-    return g, t, n, k
 
 
 def gemm_grouped(a, b_kmajor, c, offs, acc: str | int = "fp32", config_id: int | None = None, group_m: int = 0,
@@ -663,7 +668,8 @@ def grouped_schedule(config_id: int, t: int, n: int, k: int, offs, num_sms: int 
     Returns ``{"workers": W, "units": [[(group, m_block, n_block), ...] per worker]}``; blocks are cluster blocks, and
     m-blocks count from the group's first row."""
     ends = (ctypes.c_int * len(offs))(*offs)
-    return _tile_list_schedule(grouped_lib().b200_grouped_schedule_units, config_id, len(offs), t, n, k, ends, num_sms)
+    return _tile_list_schedule(grouped_lib().b200_grouped_schedule_units, 3, config_id, len(offs), t, n, k, ends,
+                               num_sms)
 
 
 def grouped_launch_count() -> int:
@@ -687,11 +693,12 @@ def _bwd_variant(dtype, acc: str | int) -> int:
     return v
 
 
-def _check_offs(offs, g: int) -> None:
-    import torch
-
-    if offs.dtype != torch.int32 or tuple(offs.shape) != (g,):
-        raise B200HgemmError(f"offs must be an int32 tensor of shape [{g}], got {offs.dtype} {tuple(offs.shape)}")
+def _bwd_operand_type(a, b, acc: str | int) -> GemmType:
+    """The 16-bit variant of the operands (:func:`_operand_type`), one that the grouped backward runs (fp32
+    accumulation). B200HgemmError otherwise."""
+    t = _operand_type(a, b, a.dtype, acc, (), scaled=False)
+    _bwd_variant(a.dtype, acc)
+    return t
 
 
 def check_grouped_nn_operands(a, b, offs, acc: str | int = "fp32") -> tuple[int, int, int, int]:
@@ -703,12 +710,10 @@ def check_grouped_nn_operands(a, b, offs, acc: str | int = "fp32") -> tuple[int,
         (t, k), (g, k2, n) = a.shape, b.shape
     except ValueError:
         raise B200HgemmError(f"a [T, K] and b [G, K, N] expected, got {tuple(a.shape)} and {tuple(b.shape)}") from None
-    if b.dtype != a.dtype:
-        raise B200HgemmError(f"operands of one dtype expected, got {a.dtype} and {b.dtype}")
-    _bwd_variant(a.dtype, acc)
+    typ = _bwd_operand_type(a, b, acc)
     if k2 != k:
         raise B200HgemmError(f"inner dimensions differ: a {tuple(a.shape)}, b {tuple(b.shape)} (row-major: [G, K, N])")
-    if n % 8 or k % 8:
+    if not typ.fits(n, k):
         raise B200HgemmError(f"{a.dtype} operands need N % 8 == 0 and K % 8 == 0 (16-byte TMA strides), got N={n}, K={k}")
     _check_offs(offs, g)
     return g, t, n, k
@@ -725,12 +730,10 @@ def check_grouped_wgrad_operands(a, b, offs, acc: str | int = "fp32") -> tuple[i
     except ValueError:
         raise B200HgemmError(f"a [T, M], b [T, N] and offs [G] expected, got {tuple(a.shape)}, {tuple(b.shape)} and "
                              f"{tuple(offs.shape)}") from None
-    if b.dtype != a.dtype:
-        raise B200HgemmError(f"operands of one dtype expected, got {a.dtype} and {b.dtype}")
-    _bwd_variant(a.dtype, acc)
+    typ = _bwd_operand_type(a, b, acc)
     if t2 != t:
         raise B200HgemmError(f"row counts differ: a {tuple(a.shape)}, b {tuple(b.shape)}")
-    if m % 8 or n % 8:
+    if not typ.fits(n, m):   # M is the K-major product's K: the rows of A hold it
         raise B200HgemmError(f"{a.dtype} operands need M % 8 == 0 and N % 8 == 0 (16-byte TMA strides), got M={m}, N={n}")
     if g < 1:
         raise B200HgemmError("offs must hold at least one group")
@@ -745,12 +748,6 @@ def _bwd_call(symbol: str, variant: int, ptrs: tuple, problem: tuple, config_id:
                               stream)
     if st != 0:
         raise B200HgemmError(f"{symbol} failed: status {st} ({lib.cuda_l2_b200_grouped_bwd_strerror(st).decode()})")
-
-
-def _contiguous_cuda(**tensors) -> None:
-    for name, x in tensors.items():
-        if not x.is_cuda or not x.is_contiguous():
-            raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
 
 
 def gemm_grouped_nn(a, b, c, offs, acc: str | int = "fp32", config_id: int | None = None, group_m: int = 0,
@@ -800,24 +797,9 @@ def grouped_wgrad_schedule(config_id: int, t: int, m: int, n: int, offs, num_sms
 
     Returns ``{"workers": W, "units": [[(group, m_block, n_block, k_blocks), ...] per worker]}``; blocks are cluster
     blocks, k_blocks the tile's 64-row k-blocks of its group (0 for an empty group)."""
-    fn = grouped_bwd_lib().cuda_l2_b200_grouped_bwd_wgrad_schedule
     ends = (ctypes.c_int * len(offs))(*offs)
-    args = (config_id, len(offs), t, m, n, ends, num_sms)
-    nw = ctypes.c_int()
-    cap = 256
-    buf = (ctypes.c_int * (4 * cap))()
-    st = fn(*args, 0, buf, cap, ctypes.byref(nw))
-    if st < 0:
-        raise B200HgemmError(f"cuda_l2_b200_grouped_bwd_wgrad_schedule failed: status {st}")
-    units = []
-    for w in range(nw.value):
-        cnt = fn(*args, w, buf, cap, None)
-        if cnt > cap:
-            cap = cnt
-            buf = (ctypes.c_int * (4 * cap))()
-            cnt = fn(*args, w, buf, cap, None)
-        units.append([tuple(buf[4 * j:4 * j + 4]) for j in range(cnt)])
-    return {"workers": nw.value, "units": units}
+    return _tile_list_schedule(grouped_bwd_lib().cuda_l2_b200_grouped_bwd_wgrad_schedule, 4, config_id, len(offs), t,
+                               m, n, ends, num_sms)
 
 
 def grouped_bwd_launch_count() -> int:

@@ -16,7 +16,7 @@
 
 namespace b200 {
 namespace tile_list {
-B200_LIST_OBJECT(Batched, B200_BLOCK_LIST_TYPES);
+B200_LIST_OBJECT(Library, Batched, B200_BLOCK_LIST_TYPES);
 
 // The batched wrapper keeps BlockScaled<>'s scale stage, ring depth and shared memory in every configuration that has a
 // block-scaled kernel, so that each batched kernel runs the 2-D block-scaled kernel's pipeline.

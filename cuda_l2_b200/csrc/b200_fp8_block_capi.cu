@@ -11,7 +11,7 @@ using b200::host::GemmType;
 namespace b200 {
 namespace block {
 
-// (eligible() and sibling() are in hgemm_configs.cuh.)
+// (eligible(), sibling() and kModes are in hgemm_configs.cuh.)
 // The dispatcher's `splits` code for the sibling: workspace split-K becomes cluster split-K of the largest of 8/4/2
 // not above it, stream-K the plain schedule; only configurations with split-K kernels keep a split.
 constexpr int sibling_splits(int id, int splits) {
@@ -20,34 +20,6 @@ constexpr int sibling_splits(int id, int splits) {
   if (r.mode == kWorkspaceSplitK) return r.factor >= 8 ? -8 : r.factor >= 4 ? -4 : -2;
   if (r.mode == kClusterSplitK) return splits;
   return 1;
-}
-
-// Workspace split-K and stream-K are not compiled for this variant: plan() runs such requests plain.
-constexpr unsigned kModes = (1u << kPlain) | (1u << kClusterSplitK);
-
-// Kernel launches of this library (b200_fp8block_launch_count).
-__attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_block_launches{0};
-
-template <GemmType T>
-int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, int ld_a, int M, int N, int K,
-               int group_m, int max_ctas, int splits, cudaStream_t s) {
-  constexpr host::GemmTypeTraits t = host::traits(T);
-  static_assert(t.block && t.e4m3() && t.acc_f32, "block-scaled e4m3 variants only");
-  int st = host::kBadConfig;
-  switch (id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
-  case ID:                                                                                                     \
-    if constexpr (eligible(ID))                                                                                \
-      st = host::launch<BlockScaled<Config<BN, STAGES, CG, true, CM, CN, MR, t.bf16(), true>>, kModes>(         \
-          A, Bt, C, M, N, K, s, group_m, max_ctas, splits, scales, ld_a);                                           \
-    break;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      break;
-  }
-  if (st == host::kOk) g_block_launches.fetch_add(1, std::memory_order_relaxed);
-  return st;
 }
 
 dispatch::Choice select(int M, int N, int K) {
@@ -63,11 +35,12 @@ Scales scales_of(const void* scale_a, const void* scale_b) {
 
 int run(int config_id, int out_bf16, const void* A, const void* Bt, void* C, Scales sc, int ld_a, int M, int N, int K,
         int group_m, int max_ctas, int splits, void* stream) {
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (out_bf16 == 0)
-    return run_config<GemmType::kE4M3F16Block>(config_id, A, Bt, C, sc, ld_a, M, N, K, group_m, max_ctas, splits, s);
+    return run_config<GemmType::kE4M3F16Block, BlockScaled>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas,
+                                                            splits, stream, ld_a);
   if (out_bf16 == 1)
-    return run_config<GemmType::kE4M3BF16Block>(config_id, A, Bt, C, sc, ld_a, M, N, K, group_m, max_ctas, splits, s);
+    return run_config<GemmType::kE4M3BF16Block, BlockScaled>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas,
+                                                             splits, stream, ld_a);
   return host::kBadConfig;
 }
 
@@ -103,7 +76,7 @@ int b200_fp8gemm_blockwise_select(int M, int N, int K, int* config_id, int* grou
 }
 
 unsigned long long b200_fp8block_launch_count(void) {
-  return b200::block::g_block_launches.load(std::memory_order_relaxed);
+  return b200::g_launches.load(std::memory_order_relaxed);
 }
 
 const char* b200_fp8block_strerror(int status) { return b200::host::status_string(status); }

@@ -14,7 +14,7 @@
 
 namespace b200 {
 namespace tile_list {
-B200_LIST_OBJECT(Grouped, B200_LIST_TYPES);
+B200_LIST_OBJECT(Library, Grouped, B200_LIST_TYPES);
 }  // namespace tile_list
 }  // namespace b200
 
@@ -27,7 +27,7 @@ extern "C" {
 int b200_grouped_gemm(int variant, const void* A, const void* B_kmajor, void* C, const int* offs, int G, int T, int N,
                       int K, void* stream) {
   using namespace b200;
-  if (!tile_list::known_variant(variant)) return host::kBadConfig;
+  if (!tile_list::holds(tile_list::Library{}, variant)) return host::kBadConfig;
   return tile_list::gemm(tile_list::Library{}, GemmType(variant), A, B_kmajor, C, Scales{nullptr, nullptr}, 0, offs, G,
                          T, N, K, stream);
 }
@@ -40,7 +40,7 @@ int b200_grouped_gemm_run_config(int variant, int config_id, const void* A, cons
 }
 
 int b200_grouped_select(int variant, int G, int T, int N, int K, int* config_id, int* group_m) {
-  if (!b200::tile_list::known_variant(variant)) return b200::host::kBadConfig;
+  if (!b200::tile_list::holds(b200::tile_list::Library{}, variant)) return b200::host::kBadConfig;
   return b200::tile_list::select_into<b200::Grouped>(GemmType(variant), G, T, N, K, config_id, group_m);
 }
 

@@ -15,7 +15,7 @@
 
 namespace b200 {
 namespace tile_list {
-B200_LIST_OBJECT(Grouped, B200_BLOCK_LIST_TYPES);
+B200_LIST_OBJECT(Library, Grouped, B200_BLOCK_LIST_TYPES);
 }  // namespace tile_list
 }  // namespace b200
 

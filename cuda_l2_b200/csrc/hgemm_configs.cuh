@@ -10,6 +10,7 @@
 // CLUSTER_M x CLUSTER_N > 1: TMA-multicast clusters of groups (single CTAs or CTA pairs): A shared along N, B along M.
 #pragma once
 #include <atomic>
+#include <type_traits>
 
 #include "hgemm_host.cuh"
 
@@ -94,6 +95,9 @@ constexpr bool every_config_has_an_eligible_sibling() {
 }
 static_assert(every_config_has_an_eligible_sibling(), "the configuration table lost a block-scaled sibling");
 
+// Workspace split-K and stream-K are not compiled for the block-scaled kernels: plan() runs such requests plain.
+constexpr unsigned kModes = (1u << kPlain) | (1u << kClusterSplitK);
+
 }  // namespace block
 
 // The row-major B (NN) configurations (libb200_nn.so, RowMajorB<>). Host code: libb200_hgemm.so maps the dispatcher's
@@ -128,28 +132,47 @@ static_assert(every_config_has_a_sibling(), "the configuration table lost a row-
 
 }  // namespace nn
 
-// Kernel launches the library has issued (b200_hgemm_launch_count). One counter for every translation unit of the
-// library; hidden, so that no other shared object's copy is bound to it.
+// What the kernels of a configuration wrapper cover, read from Probe, the wrapper's type of configuration 1 (BN = 128,
+// one CTA, no cluster), which every wrapper compiles: block-scaled kernels exist for the block::eligible
+// configurations and carry block::kModes, row-major B ones exist for the nn::has_kernel configurations; every other
+// wrapper has every configuration in every K-mode.
+template <class Probe>
+constexpr bool has_kernel(int id) {
+  return block_scaled<Probe>() ? block::eligible(id) : row_major_b<Probe>() ? nn::has_kernel(id) : true;
+}
+template <class Probe>
+constexpr unsigned k_modes() { return block_scaled<Probe>() ? block::kModes : 0xFu; }
+
+// The wrapper of the TN, per-tensor and rowwise configurations: none.
+template <class Cfg>
+using Unwrapped = Cfg;
+
+// Kernel launches the library has issued (b200_hgemm_launch_count, b200_fp8block_launch_count). One counter for every
+// translation unit of the library; hidden, so that no other shared object's copy is bound to it.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_launches{0};
 
-// Launch configuration `id` of variant T. An instantiation compiles the kernels of all configurations for T, so each
-// translation unit of the library instantiates only the variants it exports.
-template <host::GemmType T>
+// Launch configuration `id` of variant T in Wrapper (Unwrapped, BlockScaled or RowMajorB), with the block scales' ld_a
+// and the split-K scratch source of host::launch. A configuration without a kernel is kBadConfig. An instantiation
+// compiles the kernels of all configurations for T, so each translation unit of a library instantiates only the
+// variants it exports.
+template <host::GemmType T, template <class> class Wrapper = Unwrapped>
 int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, int M, int N, int K, int group_m,
-               int max_ctas, int splits, void* stream) {
+               int max_ctas, int splits, void* stream, int ld_a = 0, host::ScratchFn scratch = host::splitk_scratch) {
   constexpr host::GemmTypeTraits t = host::traits(T);
+  using Probe = Wrapper<Config<128, 6, 1, t.acc_f32, 1, 1, 1, t.bf16(), t.e4m3()>>;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int st;
+  int st = host::kBadConfig;
   switch (id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                    \
-  case ID:                                                                                                       \
-    st = host::launch<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16(), t.e4m3()>>(A, Bt, C, M, N, K, s, group_m, \
-                                                                                         max_ctas, splits, scales); \
+#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
+  case ID:                                                                                                     \
+    if constexpr (has_kernel<Probe>(ID))                                                                       \
+      st = host::launch<Wrapper<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16(), t.e4m3()>>,            \
+                        k_modes<Probe>()>(A, Bt, C, M, N, K, s, group_m, max_ctas, splits, scales, ld_a, scratch); \
     break;
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE
     default:
-      return host::kBadConfig;
+      break;
   }
   if (st == host::kOk) g_launches.fetch_add(1, std::memory_order_relaxed);
   return st;
@@ -158,12 +181,12 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
 // The tile-list libraries (libb200_batched.so, libb200_grouped.so): the 16-bit variants 0, 1, 2 (the GemmType index) of
 // every configuration, wrapped in Wrapper (Batched or Grouped), launched by host::launch_list. libb200_batched_fp8.so,
 // libb200_grouped_fp8.so: the block-scaled e4m3 variants 5, 6 of the block-scaled configurations,
-// Wrapper<BlockScaled<...>>, with their scales.
+// Wrapper<BlockScaled<...>>, with their scales. libb200_grouped_bwd.so: variants 0 and 2 of the configurations with a
+// row-major B kernel, wrapped in Grouped<RowMajorB<>> or GroupedK<RowMajorB<>>.
 namespace tile_list {
 
-// The C entry points' selectors: a 16-bit library's `variant` is the GemmType index; a block-scaled library's
-// `out_bf16` (0: fp16, 1: bf16 output) names GemmType 5 + out_bf16, and its scales arrive as untyped pointers.
-inline bool known_variant(int v) { return v >= 0 && v <= 2; }
+// The C entry points' selectors: a block-scaled library's `out_bf16` (0: fp16, 1: bf16 output) names GemmType
+// 5 + out_bf16, and its scales arrive as untyped pointers; the other libraries' `variant` is the GemmType index.
 inline bool known_out(int out_bf16) { return out_bf16 == 0 || out_bf16 == 1; }
 inline host::GemmType block_type(int out_bf16) { return host::GemmType(int(host::GemmType::kE4M3F16Block) + out_bf16); }
 inline Scales block_scales(const void* a, const void* b) {
@@ -171,25 +194,27 @@ inline Scales block_scales(const void* a, const void* b) {
 }
 
 // Kernel launches of the library that holds it (b200_batched_launch_count, b200_grouped_launch_count,
-// b200_batched_fp8_launch_count, b200_grouped_fp8_launch_count): one counter for the library's objects; hidden, like
-// g_launches.
+// b200_batched_fp8_launch_count, b200_grouped_fp8_launch_count, cuda_l2_b200_grouped_bwd_launch_count): one counter
+// for the library's objects; hidden, like g_launches.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_list_launches{0};
 
-// A configuration without a kernel of variant T (block scales: not block::eligible) returns kBadConfig.
+// The configuration Cfg of variant T in a tile-list library: a block-scaled variant's configurations are BlockScaled<>.
+template <host::GemmType T, class Cfg>
+using Variant = std::conditional_t<host::traits(T).block, BlockScaled<Cfg>, Cfg>;
+
+// A configuration without a kernel of Wrapper and T (has_kernel) returns kBadConfig.
 template <template <class> class Wrapper, host::GemmType T>
 int run_config(int id, const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
                int group_m, int max_ctas, cudaStream_t s, Scales scales, int ld_a) {
   constexpr host::GemmTypeTraits t = host::traits(T);
   static_assert(!t.scaled || t.block, "16-bit or block-scaled variants");
+  using Probe = Wrapper<Variant<T, Config<128, 6, 1, t.acc_f32, 1, 1, 1, t.bf16(), t.e4m3()>>>;
   int st = host::kBadConfig;
   switch (id) {
 #define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
   case ID:                                                                                                     \
-    if constexpr (!t.block)                                                                                    \
-      st = host::launch_list<Wrapper<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16()>>>(                \
-          A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas);                                             \
-    else if constexpr (block::eligible(ID))                                                                    \
-      st = host::launch_list<Wrapper<BlockScaled<Config<BN, STAGES, CG, true, CM, CN, MR, t.bf16(), true>>>>(  \
+    if constexpr (has_kernel<Probe>(ID))                                                                       \
+      st = host::launch_list<Wrapper<Variant<T, Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16(), t.e4m3()>>>>( \
           A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas, scales, ld_a);                               \
     break;
     B200_HGEMM_CONFIGS(B200_CASE)
@@ -197,13 +222,26 @@ int run_config(int id, const void* A, const void* Bt, void* C, const int* list, 
     default:
       break;
   }
-  if (st == host::kOk && rows > 0) g_list_launches.fetch_add(1, std::memory_order_relaxed);   // rows == 0: no launch
+  // no launch for an empty problem: no rows, or no reduction (the K-grouped T == 0, which only zero-fills C)
+  if (st == host::kOk && rows > 0 && K > 0) g_list_launches.fetch_add(1, std::memory_order_relaxed);
   return st;
 }
 
-// A tile-list library: its wrapper (Batched or Grouped) and its variants, the tag that run() and gemm() take.
+// A tile-list library: its wrapper (Batched, Grouped, or a row-major B alias) and its variants, the tag that run() and
+// gemm() take.
 template <template <class> class Wrapper, host::GemmType... Types>
 struct ListLibrary {};
+
+// Whether `variant` (a GemmType index) is one of the library's.
+template <template <class> class Wrapper, host::GemmType... Types>
+constexpr bool holds(ListLibrary<Wrapper, Types...>, int variant) {
+  return ((variant == int(Types)) || ...);
+}
+
+// The wrapper's fp16 configuration 1 (BN = 128, one CTA, no cluster), which every tile-list wrapper compiles: what
+// does not depend on the variant (the kind of list, has_kernel of the 16-bit variants) is read from it.
+template <template <class> class Wrapper>
+using ListProbe = Wrapper<Config<128, 6, 1, true>>;
 
 // The variants of each kind of tile-list library, listed once as X(W, T): the 16-bit libraries hold variants 0, 1, 2
 // (the GemmType index), the block-scaled e4m3 ones 5, 6.
@@ -211,18 +249,18 @@ struct ListLibrary {};
 #define B200_BLOCK_LIST_TYPES(X, W) X(W, host::GemmType::kE4M3F16Block) X(W, host::GemmType::kE4M3BF16Block)
 
 // A library compiles its source once per variant (-DB200_VARIANT), in parallel: each object instantiates its own
-// variant's kernels, and the calls of the other objects' variants link against theirs. B200_LIST_OBJECT(W, TYPES)
-// declares this and names the library `Library` (W and the variants of TYPES), so that run() can launch no other
-// variant's kernels. The first variant's object also holds the C entry points.
+// variant's kernels, and the calls of the other objects' variants link against theirs. B200_LIST_OBJECT(NAME, W, TYPES)
+// declares this and names the library NAME (W and the variants of TYPES), so that run() can launch no other variant's
+// kernels. The first variant's object also holds the C entry points.
 #define B200_LIST_RUN(W, T)                                                                                    \
   int run_config<W, T>(int, const void*, const void*, void*, const int*, int, int, int, int, int, int, cudaStream_t, \
                        Scales, int)
 #define B200_LIST_EXTERN(W, T) extern template B200_LIST_RUN(W, T);
 #define B200_LIST_ARG(W, T) , T
-#define B200_LIST_OBJECT(W, TYPES)                                                                             \
+#define B200_LIST_OBJECT(NAME, W, TYPES)                                                                       \
   TYPES(B200_LIST_EXTERN, W)                                                                                   \
   template B200_LIST_RUN(W, host::GemmType(B200_VARIANT));                                                     \
-  using Library = ListLibrary<W TYPES(B200_LIST_ARG, W)>
+  using NAME = ListLibrary<W TYPES(B200_LIST_ARG, W)>
 
 // Configuration `config_id` of variant `type`, with the block scales and ld_a of a block-scaled variant (ignored by
 // the 16-bit ones). A variant that is not the library's own is kBadConfig.
@@ -238,7 +276,8 @@ int run(ListLibrary<Wrapper, Types...>, host::GemmType type, int config_id, cons
 }
 
 // Host view of worker `worker`'s tiles, with the launcher's plan on a device of num_sms SMs (every cluster resident)
-// and its default group_m: (index, m_block, n_block) per tile into `units` (at most max_units); returns the count.
+// and its default group_m: (index, m_block, n_block) per tile into `units` (at most max_units), and for a K-grouped
+// configuration a fourth value, the tile's k-blocks; returns the count.
 template <class Cfg>
 int schedule_units(int count, int rows, int N, int K, const int* list, int num_sms, int worker, int* units,
                    int max_units, int* num_workers) {
@@ -249,50 +288,62 @@ int schedule_units(int count, int rows, int N, int K, const int* list, int num_s
   if (num_workers) *num_workers = p.workers;
   if (worker < 0 || worker >= p.workers) return host::kBadShape;
   const int n_blocks = (N + Cfg::BN * Cfg::CLUSTER_N - 1) / (Cfg::BN * Cfg::CLUSTER_N);
-  typename Cfg::Cursor cursor(list, count, rows, Cfg::TILE_M * Cfg::CLUSTER_M, n_blocks, host::default_group_m<Cfg>());
+  typename Cfg::Cursor cursor = make_cursor<Cfg>(list, count, rows, K, Cfg::TILE_M * Cfg::CLUSTER_M, n_blocks,
+                                                 host::default_group_m<Cfg>());
+  constexpr int kInts = k_grouped<Cfg>() ? 4 : 3;
   WorkIter it(worker, p.workers, cursor.total(), p.nkb, 1, 0);
   WorkUnit u;
   int n = 0;
   while (it.next(u)) {
-    const BatchTile bt = cursor.locate(u.tile);
+    BatchTile bt;
+    if constexpr (k_grouped<Cfg>()) bt = cursor.unit(u);   // bounds u's k-range to the tile's group
+    else bt = cursor.locate(u.tile);
     if (n < max_units && units) {
-      units[3 * n] = bt.batch; units[3 * n + 1] = bt.tc.m_blk; units[3 * n + 2] = bt.tc.n_blk;
+      int* v = units + kInts * n;
+      v[0] = bt.batch; v[1] = bt.tc.m_blk; v[2] = bt.tc.n_blk;
+      if constexpr (k_grouped<Cfg>()) v[3] = u.kb1 - u.kb0;
     }
     ++n;
   }
   return n;
 }
 
-// The shortest worst-case tile list (Cursor::max_tiles) of any configuration (block_only: of any block::eligible one).
-// When it passes INT_MAX, every configuration refuses the shape, so the dispatched call refuses it before the lookup.
+// The shortest worst-case tile list (Cursor::max_tiles) of any configuration with a kernel (block_only: of any
+// block::eligible one). When it passes INT_MAX, every configuration refuses the shape, so the dispatched call refuses
+// it before the lookup.
 template <template <class> class Wrapper>
 long long fewest_tiles(int count, int rows, int N, bool block_only = false) {
   long long fewest = 0x7fffffffffffffffLL;
 #define B200_TILES(ID, BN, STAGES, CG, CM, CN, MR)                                                               \
-  if (!block_only || block::eligible(ID)) {                                                                     \
+  if constexpr (has_kernel<ListProbe<Wrapper>>(ID)) {                                                           \
     using W = Wrapper<Config<BN, STAGES, CG, true, CM, CN, MR>>;                                                \
-    fewest = std::min(fewest, W::Cursor::template max_tiles<W>(count, rows, N));                                \
+    if (!block_only || block::eligible(ID))                                                                     \
+      fewest = std::min(fewest, W::Cursor::template max_tiles<W>(count, rows, N));                              \
   }
   B200_HGEMM_CONFIGS(B200_TILES)
 #undef B200_TILES
   return fewest;
 }
 
-// The same for configuration `config_id` (fp32-accumulating fp16: the schedule does not depend on the variant).
+// The same for configuration `config_id` (fp32-accumulating fp16: the schedule does not depend on the variant). A
+// configuration without a kernel is kBadConfig.
 template <template <class> class Wrapper>
 int schedule_config(int config_id, int count, int rows, int N, int K, const int* list, int num_sms, int worker,
                     int* units, int max_units, int* num_workers) {
   switch (config_id) {
 #define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                 \
   case ID:                                                                                                      \
-    return schedule_units<Wrapper<Config<BN, STAGES, CG, true, CM, CN, MR>>>(count, rows, N, K, list, num_sms,  \
-                                                                             worker, units, max_units,          \
-                                                                             num_workers);
+    if constexpr (has_kernel<ListProbe<Wrapper>>(ID))                                                           \
+      return schedule_units<Wrapper<Config<BN, STAGES, CG, true, CM, CN, MR>>>(count, rows, N, K, list, num_sms, \
+                                                                               worker, units, max_units,        \
+                                                                               num_workers);                    \
+    break;
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE
     default:
-      return host::kBadConfig;
+      break;
   }
+  return host::kBadConfig;
 }
 
 }  // namespace tile_list

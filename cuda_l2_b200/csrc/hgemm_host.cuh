@@ -639,6 +639,15 @@ inline int validate_k_grouped(GemmType type, const void* A, const void* B, const
   return validate(type, A, B, C, Scales{nullptr, nullptr}, M, N, M, 0, 1, tiles, offs);
 }
 
+// The argument rules of a tile-list launch of Cfg's kind, with launch_list's arguments.
+template <class Cfg>
+int validate_list(GemmType type, const void* A, const void* Bt, const void* C, const int* list, int count, int rows,
+                  int N, int K, long long tiles, Scales scales, int ld_a) {
+  return k_grouped<Cfg>() ? validate_k_grouped(type, A, Bt, C, list, count, K, rows, N, tiles)
+         : grouped<Cfg>() ? validate_grouped(type, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a)
+                          : validate(type, A, Bt, C, scales, rows, N, K, ld_a, count, tiles, list);
+}
+
 // One launch of a Batched<>, Grouped<> or GroupedK<> configuration, which walks the flat tile list of its Cfg::Cursor over
 // `count` matrices or groups. No L2 eviction hints: which operand is re-read depends on the batch or group as much as
 // on the shapes. rows == 0 launches nothing.
@@ -666,9 +675,7 @@ int launch_list(const void* A, const void* Bt, void* C, const int* list, int cou
   static_assert(batched<Cfg>() || grouped<Cfg>() || k_grouped<Cfg>(), "a Batched<>, Grouped<> or GroupedK<> configuration");
   constexpr GemmType kType = gemm_type<Cfg>();
   const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
-  int st = k_grouped<Cfg>() ? validate_k_grouped(kType, A, Bt, C, list, count, K, rows, N, tiles)
-           : grouped<Cfg>() ? validate_grouped(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a)
-                            : validate(kType, A, Bt, C, scales, rows, N, K, ld_a, count, tiles, list);
+  int st = validate_list<Cfg>(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a);
   if (st != kOk || rows == 0) return st;
   const Elem elem = traits(kType).operand, output = traits(kType).output;
   if constexpr (k_grouped<Cfg>()) {
