@@ -102,6 +102,17 @@ def _inference_op(name: str, schema: str, shape, launch, why: str = "") -> None:
     torch.library.register_autograd(qualname, no_backward)
 
 
+def _empty_product(c: torch.Tensor, k: int) -> bool:
+    """Whether the product into ``c`` needs no kernel, as torch.matmul's: ``c`` has no element (M, N or B == 0), or
+    the reduction is empty (K == 0), which makes ``c`` zero here. The C ABI rejects both with kBadShape."""
+    if c.numel() == 0:
+        return True
+    if k == 0:
+        c.zero_()
+        return True
+    return False
+
+
 torch.library.define(f"{_LIB}::hgemm", "(Tensor a, Tensor b_kmajor, str acc='fp32') -> Tensor")
 
 
@@ -111,7 +122,7 @@ def _hgemm_cuda(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> t
     a = a.contiguous()
     b_kmajor = b_kmajor.contiguous()
     c = torch.empty((m, n), dtype=a.dtype, device=a.device)
-    if m == 0:
+    if _empty_product(c, k):
         return c
     with torch.cuda.device(a.device):
         # the kernel is launched on torch's current stream, so it orders with the surrounding torch ops
@@ -163,10 +174,10 @@ torch.library.define(f"{_LIB}::hgemm_nn", "(Tensor a, Tensor b, str acc='fp32') 
 
 @torch.library.impl(f"{_LIB}::hgemm_nn", "CUDA")
 def _hgemm_nn_cuda(a: torch.Tensor, b: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
-    m, n, _ = capi.check_rowmajor_operands(a, b, a.dtype, acc)
+    m, n, k = capi.check_rowmajor_operands(a, b, a.dtype, acc)
     a, b = a.contiguous(), b.contiguous()
     c = torch.empty((m, n), dtype=a.dtype, device=a.device)
-    if m == 0:
+    if _empty_product(c, k):
         return c
     with torch.cuda.device(a.device):
         capi.gemm_rowmajor(a, b, c, acc, stream=torch.cuda.current_stream(a.device).cuda_stream)
@@ -219,10 +230,10 @@ torch.library.define(f"{_LIB}::hgemm_batched",
 
 @torch.library.impl(f"{_LIB}::hgemm_batched", "CUDA")
 def _hgemm_batched_cuda(a, b_kmajor, acc="fp32", masked_m=None):
-    bsz, m, n, _ = capi.check_batched_operands(a, b_kmajor, acc, masked_m)
+    bsz, m, n, k = capi.check_batched_operands(a, b_kmajor, acc, masked_m)
     a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
     c = torch.empty((bsz, m, n), dtype=a.dtype, device=a.device)
-    if bsz == 0 or m == 0:
+    if _empty_product(c, k):
         return c
     if masked_m is not None:
         masked_m = masked_m.contiguous()
@@ -283,7 +294,7 @@ def _hgemm_grouped_shape(a, b_kmajor, offs, acc="fp32"):
 
 
 def _hgemm_grouped_launch(c, a, b_kmajor, offs, acc="fp32", *, stream):
-    if b_kmajor.shape[0] == 0 or c.shape[0] == 0:   # no group or no row
+    if b_kmajor.shape[0] == 0 or _empty_product(c, a.shape[1]):   # no group, no element or no reduction
         return
     a, b_kmajor, offs = a.contiguous(), b_kmajor.contiguous(), offs.contiguous()
     capi.gemm_grouped(a, b_kmajor, c, offs, acc, stream=stream)
@@ -309,7 +320,7 @@ def _hgemm_grouped_nn_shape(a, b, offs, acc="fp32"):
 
 
 def _hgemm_grouped_nn_launch(c, a, b, offs, acc="fp32", *, stream):
-    if b.shape[0] == 0 or c.shape[0] == 0:   # no group or no row
+    if b.shape[0] == 0 or _empty_product(c, a.shape[1]):   # no group, no element or no reduction
         return
     capi.gemm_grouped_nn(a.contiguous(), b.contiguous(), c, offs.contiguous(), acc, stream=stream)
 
@@ -379,7 +390,7 @@ def _grouped_linear_backward(ctx, grad_y):
     if ctx.needs_input_grad[0]:
         # into zeros: rows of dX at or past the last end get no group and stay zero
         grad_x = torch.zeros_like(x)
-        if x.shape[0] > 0:
+        if x.numel() > 0 and g.shape[1] > 0:   # an empty reduction (N == 0) leaves dX zero
             with torch.cuda.device(x.device):
                 capi.gemm_grouped_nn(g, w.contiguous(), grad_x, offs.contiguous(), ctx.acc,
                                      stream=torch.cuda.current_stream(x.device).cuda_stream)
