@@ -12,6 +12,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
   ``B_rowmajor`` (csrc/b200_nn.h; no public symbol)
 * ``libb200_grouped_bwd.so`` — the backward of the grouped fp16 / bf16 GEMM: the grouped row-major B (NN) kernels of
   the input gradient and the K-grouped kernels of the weight gradient (csrc/b200_grouped_bwd.h; no public symbol)
+* ``libb200_epilogue.so`` — the 2-D fp16 / bf16 / e4m3 GEMM with a fused bias + ReLU / tanh-GELU epilogue
+  (csrc/b200_epilogue.h; no public symbol)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -91,6 +93,7 @@ def _compile_and_link(out: Path, objects: list[tuple[Path, list[str]]], link_fla
 VARIANTS = (0, 1, 2)   # fp16 with fp32 accumulation, fp16 with fp16 accumulation, bf16 (the GemmType index)
 BLOCK_VARIANTS = (5, 6)   # block-scaled e4m3 with fp16 / bf16 output (the GemmType index)
 BWD_VARIANTS = (0, 2)     # the grouped backward: fp16 and bf16, both with fp32 accumulation (the GemmType index)
+EPILOGUE_VARIANTS = (0, 2, 3, 4)   # bias + activation: fp16, bf16, e4m3 to fp16, e4m3 to bf16 (the GemmType index)
 
 
 def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, list[str]]]:
@@ -102,8 +105,8 @@ def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, lis
 # libb200_hgemm.so hold kernels of their own, so that the device code of the others stays as it is. libb200_hgemm.so
 # compiles its 16-bit kernels (b200_hgemm_capi.cu) and its e4m3 ones (b200_fp8_capi.cu) in parallel; the tile-list
 # libraries compile one source per variant (31 kernels each for the 16-bit variants, 17 for the block-scaled ones), and
-# so does libb200_nn.so (43 kernels per 16-bit variant) and libb200_grouped_bwd.so (56 per variant: 28 configurations
-# times two kinds).
+# so does libb200_nn.so (43 kernels per 16-bit variant), libb200_grouped_bwd.so (56 per variant: 28 configurations
+# times two kinds) and libb200_epilogue.so (46 per variant: libb200_hgemm.so's (configuration, K-mode) pairs).
 LIBRARIES = {
     "capi": ("libb200_hgemm.so", [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], []),
     "fp8block": ("libb200_fp8block.so", [(CSRC / "b200_fp8_block_capi.cu", [])], []),
@@ -113,6 +116,7 @@ LIBRARIES = {
     "batched_fp8": ("libb200_batched_fp8.so", _per_variant("b200_batched_fp8_capi.cu", BLOCK_VARIANTS), []),
     "nn": ("libb200_nn.so", _per_variant("b200_nn.cu", VARIANTS), []),
     "grouped_bwd": ("libb200_grouped_bwd.so", _per_variant("b200_grouped_bwd.cu", BWD_VARIANTS), []),
+    "epilogue": ("libb200_epilogue.so", _per_variant("b200_epilogue.cu", EPILOGUE_VARIANTS), []),
     "baselines": ("libb200_baselines.so", [(CSRC / "b200_baselines_capi.cu", [])], ["-lcublas", "-lcublasLt"]),
 }
 

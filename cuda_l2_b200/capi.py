@@ -104,6 +104,7 @@ ABI = {
 GROUPED_BWD_LIB = "libb200_grouped_bwd.so"   # csrc/b200_grouped_bwd.h
 _BWD_RUN = ([_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i)
 _BWD_SELECT = ([_i, _i, _i, _i, _i, _ip, _ip], _i)
+EPILOGUE_LIB = "libb200_epilogue.so"         # csrc/b200_epilogue.h
 INTERNAL_ABI = {
     GROUPED_BWD_LIB: {
         "cuda_l2_b200_grouped_bwd_nn": _BWD_RUN,
@@ -113,6 +114,16 @@ INTERNAL_ABI = {
         "cuda_l2_b200_grouped_bwd_wgrad_schedule": ([_i, _i, _i, _i, _i, _ip, _i, _i, _ip, _i, _ip], _i),
         "cuda_l2_b200_grouped_bwd_launch_count": ([], ctypes.c_ulonglong),
         "cuda_l2_b200_grouped_bwd_strerror": ([_i], ctypes.c_char_p),
+    },
+    EPILOGUE_LIB: {
+        "cuda_l2_b200_epilogue_run": ([_i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_epilogue_run_config": ([_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i,
+                                              _vp], _i),
+        "cuda_l2_b200_epilogue_select": ([_i, _i, _i, _i, _ip, _ip, _ip], _i),
+        "cuda_l2_b200_epilogue_prewarm": ([_vp], _i),
+        "cuda_l2_b200_epilogue_release": ([], _i),
+        "cuda_l2_b200_epilogue_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_epilogue_strerror": ([_i], ctypes.c_char_p),
     },
 }
 _libs: dict = {}
@@ -1023,3 +1034,106 @@ class Baselines:
 
     def lt_autotune(self, layout, a, b, c):
         self._call(self.lib.b200_bl_lt_autotune, layout, a, b, c)
+
+
+# ------------------------------------------------------------------------------- bias + activation (libb200_epilogue.so)
+ACTIVATIONS = {"none": 0, "relu": 1, "gelu_tanh": 2}   # the activation codes of csrc/b200_epilogue.h
+
+
+def epilogue_lib() -> ctypes.CDLL:
+    """libb200_epilogue.so: the 2-D GEMM with a fused bias + activation epilogue (csrc/b200_epilogue.h, no public ABI)."""
+    return load(EPILOGUE_LIB)
+
+
+def epilogue_variant(operand, out_dtype) -> int:
+    """The GemmType index of the bias + activation kernels for these dtypes: 0 fp16, 2 bf16, 3 / 4 e4m3 with fp16 / bf16
+    output (fp32 accumulation). B200HgemmError for any other pair."""
+    import torch
+
+    variants = {(torch.float16, torch.float16): 0, (torch.bfloat16, torch.bfloat16): 2,
+                (torch.float8_e4m3fn, torch.float16): 3, (torch.float8_e4m3fn, torch.bfloat16): 4}
+    if (operand, out_dtype) not in variants:
+        raise B200HgemmError(f"no bias + activation kernel for {operand} -> {out_dtype} (fp16, bf16 with fp32 accumulation; "
+                             f"e4m3 -> fp16 / bf16 with per-tensor or rowwise scales)")
+    return variants[(operand, out_dtype)]
+
+
+def activation_code(activation: str) -> int:
+    if activation not in ACTIVATIONS:
+        raise B200HgemmError(f"unknown activation {activation!r}: one of {', '.join(ACTIVATIONS)}")
+    return ACTIVATIONS[activation]
+
+
+def check_bias(bias, n: int, out_dtype) -> None:
+    """B200HgemmError unless ``bias`` is None or a 1-D tensor of ``n`` elements of ``out_dtype`` (shape and dtype only:
+    meta tensors pass)."""
+    if bias is not None and (bias.dim() != 1 or bias.shape[0] != n or bias.dtype != out_dtype):
+        raise B200HgemmError(f"bias must be 1-D with N = {n} elements of {out_dtype}, got {bias.dtype} "
+                             f"{tuple(bias.shape)}")
+
+
+def _bias_arg(bias):
+    """The bias as the kernels read it: contiguous and 16-byte aligned (a fresh copy if it is not)."""
+    if bias is None:
+        return None
+    bias = bias.contiguous()
+    return bias if bias.data_ptr() % 16 == 0 else bias.clone()
+
+
+def gemm_bias_act(a, b_kmajor, c, bias=None, activation: str = "none", scale_a=None, scale_b=None,
+                  stream: int | None = None, config_id: int | None = None, group_m: int = 0, splits: int = 1,
+                  max_ctas: int = 0) -> None:
+    """c[M,N] = act(a[M,K] @ b_kmajor[N,K]^T (scaled) + bias), fp32 throughout and one rounding to ``c``'s dtype
+    (csrc/b200_epilogue.h). fp16 or bf16 operands with fp32 accumulation (no scales), or ``float8_e4m3fn`` operands with
+    per-tensor or rowwise scales as for :func:`fp8_gemm` (blockwise scales have no bias kernel). ``bias``: None or a 1-D
+    CUDA tensor of N elements of ``c``'s dtype; a misaligned one is copied. ``activation``: "none", "relu" or
+    "gelu_tanh". ``config_id`` pins one kernel configuration (tests; ``group_m``, ``splits`` and ``max_ctas`` as for
+    :func:`gemm_kmajor`); default is the dispatcher's choice for the same variant."""
+    scales = () if scale_a is None and scale_b is None else (scale_a, scale_b)
+    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", scales)
+    variant = epilogue_variant(a.dtype, c.dtype)
+    act = activation_code(activation)
+    _contiguous_cuda(bias=bias)
+    check_bias(bias, n, c.dtype)
+    rowwise = 0
+    if scales:
+        granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
+        if granularity == "blockwise":
+            raise B200HgemmError("blockwise e4m3 scales have no bias + activation kernel (per-tensor or rowwise only)")
+        rowwise = int(granularity == "rowwise")
+        if not scale_a.is_contiguous():
+            raise B200HgemmError("scale_a must be a contiguous CUDA tensor")
+    bias = _bias_arg(bias)
+    args = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr() if scales else None,
+            scale_b.data_ptr() if scales else None, rowwise, None if bias is None else bias.data_ptr(), act, m, n, k)
+    lib = epilogue_lib()
+    if config_id is None:
+        st = lib.cuda_l2_b200_epilogue_run(variant, *args, stream)
+    else:
+        st = lib.cuda_l2_b200_epilogue_run_config(variant, config_id, *args, group_m, max_ctas, splits, stream)
+    _epilogue_check(st, "cuda_l2_b200_epilogue")
+
+
+def epilogue_select(variant: int, m: int, n: int, k: int) -> tuple[int, int, int]:
+    """(config_id, group_m, splits): the dispatched bias + activation call's choice for variant ``variant``."""
+    return _select(epilogue_lib().cuda_l2_b200_epilogue_select, variant, m, n, k)
+
+
+def _epilogue_check(st: int, what: str) -> None:
+    if st != 0:
+        raise B200HgemmError(f"{what} failed: status {st} ({epilogue_lib().cuda_l2_b200_epilogue_strerror(st).decode()})")
+
+
+def epilogue_prewarm(stream: int | None = None) -> None:
+    """Allocate libb200_epilogue.so's split-K scratch for ``stream`` ahead of a CUDA-graph capture (a first split-K or
+    stream-K call inside a capture runs undivided without it)."""
+    _epilogue_check(epilogue_lib().cuda_l2_b200_epilogue_prewarm(stream), "cuda_l2_b200_epilogue_prewarm")
+
+
+def epilogue_release() -> None:
+    """Free libb200_epilogue.so's split-K scratch (no launch of it may be in flight)."""
+    _epilogue_check(epilogue_lib().cuda_l2_b200_epilogue_release(), "cuda_l2_b200_epilogue_release")
+
+
+def epilogue_launch_count() -> int:
+    return int(epilogue_lib().cuda_l2_b200_epilogue_launch_count())

@@ -30,6 +30,7 @@ enum Status : int {
   kBadFp8K = -9,         // e4m3 operands: K % 16 == 0 (16-byte TMA strides at one byte per element)
   kBadScaleLd = -10,     // block scales: the row stride of A's scales must be >= M and a multiple of 4
   kNoNNLibrary = -11,    // row-major B: libb200_nn.so, next to libb200_hgemm.so, is missing or does not load
+  kBadActivation = -12,  // bias + activation epilogue: the activation code is not one of Activation's
   // > 0: a cudaError_t from the launch
 };
 
@@ -47,6 +48,7 @@ inline const char* status_string(int s) {
     case kBadFp8K: return "e4m3 operands need K % 16 == 0 (16-byte row strides at one byte per element)";
     case kBadScaleLd: return "block scales need ld_a >= M and ld_a % 4 == 0 (16-byte aligned k-block rows of A's scales)";
     case kNoNNLibrary: return "row-major B needs libb200_nn.so next to libb200_hgemm.so (missing, or it does not load)";
+    case kBadActivation: return "unknown activation code (0 none, 1 relu, 2 gelu_tanh)";
     default: return s > 0 ? cudaGetErrorString(static_cast<cudaError_t>(s)) : "unknown error";
   }
 }
@@ -217,6 +219,14 @@ inline int validate(GemmType type, const void* A, const void* Bt, const void* C,
   }
   if (t.scaled && ((reinterpret_cast<uintptr_t>(scales.a) | reinterpret_cast<uintptr_t>(scales.b)) & (scales.rowwise ? 15 : 3)))
     return kBadAlignment;
+  return kOk;
+}
+
+// The argument rules of the bias + activation epilogue (BiasAct<>), after validate()'s: a known activation code, and a
+// bias that is null or 16-byte aligned (the split-K reductions read it 8 bytes at a time, at every fourth column).
+inline int validate_bias_act(const void* bias, int act) {
+  if (act < 0 || act >= kNumActivations) return kBadActivation;
+  if (reinterpret_cast<uintptr_t>(bias) & 15) return kBadAlignment;
   return kOk;
 }
 
@@ -409,7 +419,7 @@ int max_resident_clusters(const DeviceInfo& di) {
     pa[0].val.clusterDim.x = Cfg::CLUSTER_CTAS; pa[0].val.clusterDim.y = 1; pa[0].val.clusterDim.z = 1;
     probe.attrs = pa; probe.numAttrs = 1;
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, hgemm_tn_kernel<Cfg>, &probe) != cudaSuccess || n < 1) {
+    if (cudaOccupancyMaxActiveClusters(&n, kernel_of<Cfg, kPlain>(), &probe) != cudaSuccess || n < 1) {
       cudaGetLastError();
       n = std::max(1, di.num_sms / Cfg::CLUSTER_CTAS * 7 / 8);
     }
@@ -445,16 +455,25 @@ struct LaunchArgs {
   int batches;          // batched kernels: the batch count ...
   const int* masked_m;  // ... and the row counts per batch (null: dense); grouped kernels: G and the offsets
   cudaStream_t stream;
+  const void* bias;     // BiasAct<> kernels: the bias (or null) ...
+  int act;              // ... and the activation code
 };
+
+// The kernel's last argument: the scales, or BiasAct<>'s BiasActArgs.
+template <class Cfg>
+typename Cfg::EpiArgs epi_args(const LaunchArgs& a) {
+  if constexpr (bias_act<Cfg>()) return BiasActArgs{a.scales, a.bias, a.act};
+  else return a.scales;
+}
 
 template <class Cfg, int KMODE>
 int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   static thread_local int attr_dev = -1;
   static thread_local const void* attr_fn = nullptr;
-  const void* this_fn = reinterpret_cast<const void*>(&hgemm_tn_kernel<Cfg, KMODE>);
+  constexpr auto kernel = kernel_of<Cfg, KMODE>();
+  const void* this_fn = reinterpret_cast<const void*>(kernel);
   if (attr_dev != di.dev || attr_fn != this_fn) {
-    cudaError_t e = cudaFuncSetAttribute(hgemm_tn_kernel<Cfg, KMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return int(e);
     attr_dev = di.dev;
     attr_fn = this_fn;
@@ -506,14 +525,14 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   constexpr bool kTileList = batched<Cfg>() || grouped<Cfg>() || k_grouped<Cfg>();
   const int splits_arg = kTileList ? a.batches : a.plan.splits;
   unsigned* ctr = kTileList ? reinterpret_cast<unsigned*>(const_cast<int*>(a.masked_m)) : a.ctr;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                                     splits_arg, aux, a.ws, ctr, a.c, a.hint_a, a.hint_b, a.scales);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m, splits_arg, aux, a.ws,
+                                     ctr, a.c, a.hint_a, a.hint_b, epi_args<Cfg>(a));
   if (e != cudaSuccess && coop && pdl && e != cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
     coop_pdl_ok = false;               // the pair of attributes is not accepted here: cooperative only, from now on
     cfg.numAttrs = na - 1;
-    e = cudaLaunchKernelEx(&cfg, hgemm_tn_kernel<Cfg, KMODE>, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m,
-                           splits_arg, aux, a.ws, ctr, a.c, a.hint_a, a.hint_b, a.scales);
+    e = cudaLaunchKernelEx(&cfg, kernel, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m, splits_arg, aux, a.ws, ctr, a.c,
+                           a.hint_a, a.hint_b, epi_args<Cfg>(a));
   }
   return e == cudaSuccess ? kOk : int(e);
 }
@@ -528,13 +547,17 @@ constexpr int default_group_m() { return Cfg::CTA_GROUP == 2 ? 8 : 16; }
 // kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor or rowwise scales
 // of a scaled variant (device pointers), unused otherwise; `ld_a`: the row stride of block scales. RowMajorB<>
 // configurations read `Bt` as B [K, N] row-major. `scratch`: where the workspace of split-K and stream-K comes from.
+// BiasAct<> configurations: the bias (null, or N values of the output type) and the activation code.
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
            int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0,
-           ScratchFn scratch = splitk_scratch) {
+           ScratchFn scratch = splitk_scratch, const void* bias = nullptr, int act = kActNone) {
   constexpr GemmType kType = gemm_type<Cfg>();
   int st = validate(kType, A, Bt, C, scales, M, N, K, ld_a);
   if (st != kOk) return st;
+  if constexpr (bias_act<Cfg>()) {
+    if ((st = validate_bias_act(bias, act)) != kOk) return st;
+  }
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
 
@@ -566,6 +589,8 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   a.scales = scales;
   a.ld_a = ld_a;
   a.stream = stream;
+  a.bias = bias;
+  a.act = act;
   // L2 eviction priorities: when one operand is streamed (about) once while the other is re-read by every tile row
   // or column and is small enough to live in L2, keep the small one and let the streamed one go first.
   a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;

@@ -56,6 +56,7 @@ constexpr int kSmemLimit = 232448;   // 227 KB of dynamic shared memory per bloc
 // How a launch divides K. The kernel is compiled once per (configuration, mode), so that the plain schedule — nearly
 // every launch — carries none of the three other epilogues.
 enum KMode : int { kPlain = 0, kWorkspaceSplitK = 1, kClusterSplitK = 2, kStreamK = 3 };
+struct Scales;   // the epilogue arguments of every configuration but BiasAct<>'s (below)
 
 template <int BN_, int STAGES_, int CTA_GROUP_, bool ACC_F32_, int CLUSTER_M_ = 1, int CLUSTER_N_ = 1, int M_REP_ = 1, bool BF16_ = false,
           bool E4M3_ = false>
@@ -100,9 +101,11 @@ struct Config {
   // which K-decompositions this configuration's kernel carries
   static constexpr bool STREAM_K = CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
   static constexpr bool SPLIT_K = STREAM_K && CTA_GROUP_ == 1;
-  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>, RowMajorB<>, GroupedK<>) override these
-  static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false, ROW_MAJOR_B = false, K_GROUPED = false;
+  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>, RowMajorB<>, GroupedK<>, BiasAct<>) override these
+  static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false, ROW_MAJOR_B = false, K_GROUPED = false,
+                        BIAS_ACT = false;
   using Cursor = NoBatches;   // the flat tile list the kernel walks (hgemm_schedule.cuh): none
+  using EpiArgs = Scales;     // the kernel's last parameter
   static constexpr int EPI_BYTES = 8 * EPI_ROWS * 64 * 2;    // 8 consumer warps x one staging buffer (sized for EPI_N = 64)
   static constexpr int BAR_BYTES = 256;
   // STAGES_ is the requested ring depth; on sm_90 every CTA of a pair holds the whole B tile, so the depth is capped
@@ -283,6 +286,56 @@ __host__ __device__ __forceinline__ typename Cfg::Cursor make_cursor(const int* 
 // other e4m3 kernels.
 struct Scales { const float* a; const float* b; bool rowwise = false; };
 
+// Fused bias + activation epilogue (libb200_epilogue.so): C[m,n] = RN_out(act(s(m,n) + fp32(bias[n]))), fp32 throughout
+// and one rounding, where s is what the wrapped kernel rounds (the fp32 sum; e4m3: the sum after its per-tensor or
+// rowwise scales). `bias` has the output's type, N values, 16-byte aligned; null adds nothing (the kernel then adds
+// -0.0, which leaves every value, -0.0 included, as it is). The activation code is a run-time value, the same for the
+// whole launch, so one kernel serves all three. Only the finished sum sees either: partial tiles, DSMEM tiles and
+// stream-K register images are those of the wrapped kernel. The 2-D kernels with fp32 accumulation (fp16, bf16, e4m3
+// per-tensor and rowwise) in every K-mode; fp16 accumulation and block scales have no bias kernel. A wrapper, like
+// BlockScaled<>, so that the other kernels and their names stay as they are; the kernel takes BiasActArgs as its last
+// parameter (hgemm_bias_act_kernel) where the others take Scales.
+enum Activation : int { kActNone = 0, kActRelu = 1, kActGeluTanh = 2 };
+constexpr int kNumActivations = 3;
+struct BiasActArgs { Scales scales; const void* bias; int act; };
+template <class Base>
+struct BiasAct : Base {
+  static constexpr bool BIAS_ACT = true;
+  using EpiArgs = BiasActArgs;
+  static_assert(Base::ACC_F32 && !Base::BLOCK_SCALED && !Base::BATCHED && !Base::GROUPED && !Base::ROW_MAJOR_B &&
+                    !Base::K_GROUPED,
+                "bias + activation: the 2-D TN kernels with fp32 accumulation only");
+};
+template <class Cfg>
+__host__ __device__ constexpr bool bias_act() { return Cfg::BIAS_ACT; }
+__host__ __device__ __forceinline__ const Scales& scales_of(const Scales& s) { return s; }
+__host__ __device__ __forceinline__ const Scales& scales_of(const BiasActArgs& e) { return e.scales; }
+
+// act(z) in fp32; `act` is warp-uniform. relu: max(z, +0.0) (+0.0 for -0.0 and NaN). gelu_tanh: 0.5 z (1 + tanhf(u)),
+// u = sqrt(2/pi) (z + 0.044715 z^3), torch's tanh approximation (F.gelu(approximate="tanh"), _addmm_activation), each
+// step one IEEE fp32 operation and tanhf CUDA's full-precision one (no tanh.approx.f32). Where tanh(u) nears -1 (z below
+// about -3) 1 + tanhf(u) keeps few bits: there the result carries an absolute error of a few 2^-24 |z|, as fp32 torch's
+// does, and is -0.0 once tanhf(u) rounds to -1 (z below about -5.2).
+__device__ __forceinline__ float activate(float z, int act) {
+  if (act == kActRelu) return z > 0.f ? z : 0.f;
+  if (act == kActGeluTanh) {
+    const float inner = __fadd_rn(z, __fmul_rn(0.044715f, __fmul_rn(__fmul_rn(z, z), z)));
+    const float u = __fmul_rn(0.7978845608028654f, inner);
+    return __fmul_rn(__fmul_rn(0.5f, z), __fadd_rn(1.f, tanhf(u)));
+  }
+  return z;
+}
+// Two 16-bit bias values of the output type (low half: the lower column) as fp32.
+template <class Cfg>
+__device__ __forceinline__ float2 unpack_out_x2(uint32_t v) {
+  if constexpr (Cfg::BF16) return make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u));
+  else {
+    const __half2 h = *reinterpret_cast<const __half2*>(&v);
+    return make_float2(__low2float(h), __high2float(h));
+  }
+}
+constexpr uint32_t kNegZeroPair = 0x80008000u;   // -0.0 in both halves, fp16 and bf16: the bias of a null pointer
+
 // The uniform factor applied to the finished fp32 sum before it is rounded to the output type: fp32(scale_a * scale_b)
 // for per-tensor e4m3 scales, read where it is used (after the grid dependency wait, so a preceding kernel may have just
 // written it). Rowwise launches scale per element instead (scale_quad, the plain epilogue) and do not read it; block-
@@ -307,6 +360,19 @@ __device__ __forceinline__ void scale_quad(float4& acc, float scale, const Scale
       acc.x = __fmul_rn(acc.x, scale); acc.y = __fmul_rn(acc.y, scale);
       acc.z = __fmul_rn(acc.z, scale); acc.w = __fmul_rn(acc.w, scale);
     }
+  }
+}
+
+// The bias and the activation of one finished, scaled float4 of the split-K reductions (BiasAct<> kernels only): one
+// 8-byte load of the bias at columns gn .. gn+3.
+template <class Cfg>
+__device__ __forceinline__ void bias_act_quad(float4& acc, const typename Cfg::EpiArgs& epi, int gn) {
+  if constexpr (bias_act<Cfg>()) {
+    uint2 bv = make_uint2(kNegZeroPair, kNegZeroPair);
+    if (epi.bias) bv = *reinterpret_cast<const uint2*>(static_cast<const uint16_t*>(epi.bias) + gn);
+    const float2 lo = unpack_out_x2<Cfg>(bv.x), hi = unpack_out_x2<Cfg>(bv.y);
+    acc.x = activate(__fadd_rn(acc.x, lo.x), epi.act); acc.y = activate(__fadd_rn(acc.y, lo.y), epi.act);
+    acc.z = activate(__fadd_rn(acc.z, hi.x), epi.act); acc.w = activate(__fadd_rn(acc.w, hi.y), epi.act);
   }
 }
 
@@ -336,18 +402,115 @@ __device__ __forceinline__ uint32_t acc_packed(const Reg (&d)[NR], int p) {
   else return d[p];   // fp16 accumulators are already the output format
 }
 
+// BiasAct<> kernels: the unit's bias, column scales and (rowwise) row scales, prefetched into L1 by one warp as the
+// unit starts, so that bias_in_place, which reads them one at a time where they are used, finds them there rather than
+// waiting on L2 for each. A prefetch holds no register. n0: the tile's first column; m0: the warpgroup's first row.
+template <class Cfg>
+__device__ __forceinline__ void bias_act_prefetch(const BiasActArgs& epi, int m0, int n0, int M, int N, int lane) {
+  constexpr int kLine = 128;
+  const int cols = min(Cfg::BN, N - n0), rows = min(64 * Cfg::M_REP, M - m0);
+  if (cols <= 0) return;
+  auto fetch = [&](const void* base, int bytes, int first_line) {
+    const int i = lane - first_line;   // the lanes [first_line, first_line + lines) each take one line
+    if (i >= 0 && i * kLine < bytes) asm volatile("prefetch.global.L1 [%0];" ::"l"(static_cast<const char*>(base) + i * kLine));
+  };
+  // up to 4 lines of bias (lanes 0-3), 8 of column scales (4-11) and 2 of row scales per 64 rows (12-15)
+  if (epi.bias) fetch(static_cast<const uint16_t*>(epi.bias) + n0, cols * 2, 0);
+  if constexpr (Cfg::E4M3) {
+    if (epi.scales.rowwise) {
+      fetch(epi.scales.b + n0, cols * 4, 4);
+      if (rows > 0) fetch(epi.scales.a + m0, rows * 4, 12);
+    }
+  }
+}
+
+// BiasAct<> kernels, plain epilogue: the finished sums of the warpgroup's MR 64-row blocks (this warp's rows m_row0 +
+// 64 r .. + 15, columns n0 ..), in place, scaled as the wrapped kernel scales them (e4m3 per tensor:
+// fp32(acc * fp32(sa * sb)); rowwise: fp32(fp32(acc * sb[n]) * sa[m])) and then biased (one fp32 addition; -0.0 for a
+// null bias). The loop runs over the thread's column pairs. The bias and the column scales are read where they are used
+// (from L1: bias_act_prefetch), once per column pair for all its rows, so that nothing is held across the accumulators;
+// the store (epilogue_store_chunk) then only adds the activation's temporaries to them.
+template <class Cfg, class Reg, int MR, int NR>
+__device__ __forceinline__ void bias_in_place(Reg (&d)[MR][NR], int lane, int m_row0, int n0, int M, int N,
+                                              const BiasActArgs& epi) {
+  const uint32_t* bias = static_cast<const uint32_t*>(epi.bias);
+  [[maybe_unused]] const float scale = output_scale<Cfg>(epi.scales);
+  // rowwise, one 64-row block: its two row scales stay in registers; with two blocks (M_REP = 2) there is no room for
+  // their four next to the accumulators, and each is read where it is used
+  [[maybe_unused]] float sa_held[2] = {0.f, 0.f};
+  if constexpr (Cfg::E4M3 && MR == 1) {
+    if (epi.scales.rowwise) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m_row0 + frag_row(lane, h);
+        sa_held[h] = m < M ? epi.scales.a[m] : 0.f;
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < NR / 4; ++c) {   // pairs 2c (rows l/4) and 2c + 1 (rows l/4 + 8) of every block share two columns
+    const int n = n0 + frag_col(lane, 2 * c);   // even, and N % 8 == 0: n < N covers n + 1; past N nothing is stored
+    const float2 b = unpack_out_x2<Cfg>(bias && n < N ? __ldg(bias + n / 2) : kNegZeroPair);
+    [[maybe_unused]] float2 sb = make_float2(0.f, 0.f);
+    if constexpr (Cfg::E4M3) {
+      if (epi.scales.rowwise && n < N) sb = __ldg(reinterpret_cast<const float2*>(epi.scales.b + n));
+    }
+#pragma unroll
+    for (int r = 0; r < MR; ++r) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int p = 2 * c + h;
+        float x = d[r][2 * p], y = d[r][2 * p + 1];
+        if constexpr (Cfg::E4M3) {
+          if (epi.scales.rowwise) {   // warp-uniform
+            float sa = sa_held[h];
+            if constexpr (MR > 1) {
+              const int m = m_row0 + 64 * r + frag_row(lane, p);
+              sa = m < M ? __ldg(epi.scales.a + m) : 0.f;
+            }
+            x = __fmul_rn(__fmul_rn(x, sb.x), sa);
+            y = __fmul_rn(__fmul_rn(y, sb.y), sa);
+          } else {
+            x = __fmul_rn(x, scale);
+            y = __fmul_rn(y, scale);
+          }
+        }
+        d[r][2 * p] = __fadd_rn(x, b.x);
+        d[r][2 * p + 1] = __fadd_rn(y, b.y);
+      }
+    }
+  }
+}
+
+// The packed, activated values of one store chunk into the staging buffer (epilogue_store_chunk, BiasAct<> kernels), one
+// loop per activation, so that each is straight-line code.
+template <class Cfg, int ACT, class Reg, int NR>
+__device__ __forceinline__ void store_activated(const Reg (&d)[NR], int chunk, uint32_t epi_buf, int lane) {
+  constexpr int EN = Cfg::EPI_N;
+  constexpr int PER_CHUNK = EN / 4;
+#pragma unroll
+  for (int q = 0; q < PER_CHUNK; ++q) {
+    uint32_t off = uint32_t(frag_row(lane, q) * (EN * 2) + frag_col(lane, q) * 2);
+    off ^= (EN == 64 ? ((off >> 7) & 7u) : ((off >> 7) & 3u)) << 4;
+    const float2 v = acc_pair<Cfg>(d, chunk * PER_CHUNK + q);
+    ptx::st_shared_b32(epi_buf + off, ptx::pack_out_x2_rn<Cfg::BF16>(activate(v.x, ACT), activate(v.y, ACT)));
+  }
+}
+
 // registers -> swizzled staging buffer -> TMA store of one EPI_ROWS x EPI_N chunk of this warp. Grouped kernels: M is
 // the end row of the tile's group, and a box that straddles it is copied out row by row instead (c_raw: C [., N]).
 // With rowwise e4m3 scales
 // (`rw` non-null) each fp32 pair is scaled by its column scales, then its row scale, right before the rounding. The
 // column scales of a chunk are loaded here, after the previous chunk's store wait, one float2 (one column pair) per
 // lane, and reach the lanes that need them by shuffle: two registers per thread instead of the chunk's 16, which the
-// 128 accumulators of a BN = 256 (or M_REP = 2) tile leave no room for.
+// 128 accumulators of a BN = 256 (or M_REP = 2) tile leave no room for. BiasAct<> kernels (`epi`: their BiasActArgs)
+// find their scales and bias applied (bias_in_place) and apply the activation as they pack.
 template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chunk, uint32_t epi_buf, int lane,
                                                      const CUtensorMap* tmap_c, int col0, int row0, int M, int N,
                                                      const RowwiseEpi* rw = nullptr, int batch = 0,
-                                                     __half* __restrict__ c_raw = nullptr) {
+                                                     __half* __restrict__ c_raw = nullptr,
+                                                     const typename Cfg::EpiArgs* epi = nullptr) {
   using namespace ptx;
   constexpr int EN = Cfg::EPI_N;
   constexpr int PER_CHUNK = EN / 4;   // packed pairs of one chunk per thread
@@ -360,6 +523,12 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
     const int n = col0 + 2 * lane;   // even, and N % 8 == 0: n < N covers n + 1
     if (rw && 2 * lane < EN && n < N) sb_lane = *reinterpret_cast<const float2*>(rw->sb + n);
   }
+  if constexpr (bias_act<Cfg>()) {
+    // the values are scaled and biased already (bias_in_place): the activation, then the one rounding
+    if (epi->act == kActGeluTanh) store_activated<Cfg, kActGeluTanh>(d, chunk, epi_buf, lane);
+    else if (epi->act == kActRelu) store_activated<Cfg, kActRelu>(d, chunk, epi_buf, lane);
+    else store_activated<Cfg, kActNone>(d, chunk, epi_buf, lane);
+  } else {
 #pragma unroll
   for (int q = 0; q < PER_CHUNK; ++q) {
     uint32_t off = uint32_t(frag_row(lane, q) * (EN * 2) + frag_col(lane, q) * 2);
@@ -380,6 +549,7 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
       }
     }
     st_shared_b32(epi_buf + off, acc_packed<Cfg>(d, chunk * PER_CHUNK + q));
+  }
   }
   fence_proxy_async_smem();
   __syncwarp();
@@ -410,6 +580,30 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
   }
 }
 
+// The plain epilogue of a BiasAct<> unit: the scales and the bias in place (bias_in_place), then for every 64-row block R
+// of the warpgroup (rows m_row0 + 64 R ..) its store chunks J. The blocks and chunks are unrolled by recursion rather
+// than by loop pragmas, which the compiler declines for bodies of this size: a chunk index that is not a constant would
+// move the accumulators to local memory.
+template <class Cfg, int R = 0, int J = 0, class Reg, int MR, int NR>
+__device__ __forceinline__ void bias_act_epilogue(Reg (&acc)[MR][NR], uint32_t epi_buf, int lane, const CUtensorMap* tmap_c,
+                                                  int m_row0, int n0, int M, int N, const BiasActArgs& epi) {
+  if constexpr (R < MR) {
+    const int row0 = m_row0 + R * 64;
+    if constexpr (R == 0 && J == 0) {
+      bias_in_place<Cfg>(acc, lane, m_row0, n0, M, N, epi);
+#pragma unroll
+      for (int r = 0; r < MR; ++r) ptx::reg_fence(acc[r]);
+    }
+    if constexpr (J < Cfg::EPI_CHUNKS) {
+      epilogue_store_chunk<Cfg>(acc[R], J, epi_buf, lane, tmap_c, n0 + J * Cfg::EPI_N, row0, M, N, nullptr, 0, nullptr,
+                                &epi);
+      bias_act_epilogue<Cfg, R, J + 1>(acc, epi_buf, lane, tmap_c, m_row0, n0, M, N, epi);
+    } else {
+      bias_act_epilogue<Cfg, R + 1, 0>(acc, epi_buf, lane, tmap_c, m_row0, n0, M, N, epi);
+    }
+  }
+}
+
 // The tile of an empty group of a K-grouped kernel (GroupedK<>): +0.0 in this warp's MR x 16 rows from row0 (of
 // matrix `batch` of C [., M, N]) and BN columns from col0, clipped at M and N, with 16-byte generic stores.
 template <class Cfg>
@@ -436,9 +630,11 @@ template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void splitk_epilogue(const Reg (&d)[NR], int e, int row_base, int lane, int tile, int split,
                                                 int splits, int m_base, int n0, int M, int N, float* __restrict__ ws,
                                                 unsigned* __restrict__ ctr, __half* __restrict__ C,
-                                                uint32_t red_smem, uint32_t red_bar, const Scales& scales) {
+                                                uint32_t red_smem, uint32_t red_bar,
+                                                const typename Cfg::EpiArgs& epi) {
   using namespace ptx;
   constexpr int BN = Cfg::BN;
+  const Scales& scales = scales_of(epi);
   float* slot = ws + (size_t(tile) * splits + split) * (kBlockM * BN);
 #pragma unroll
   for (int p = 0; p < NR * (Cfg::ACC_F32 ? 1 : 2) / 2; ++p) {
@@ -487,6 +683,7 @@ __device__ __forceinline__ void splitk_epilogue(const Reg (&d)[NR], int e, int r
         acc.x += p.x; acc.y += p.y; acc.z += p.z; acc.w += p.w;
       }
       scale_quad<Cfg>(acc, scale, scales, gm, gn);
+      bias_act_quad<Cfg>(acc, epi, gn);
       uint2 out;
       out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
       out.y = pack_out_x2_rn<Cfg::BF16>(acc.z, acc.w);
@@ -525,8 +722,9 @@ __device__ __forceinline__ void cluster_splitk_park(const Reg (&d)[NR], int row_
 template <class Cfg>
 __device__ __forceinline__ void cluster_splitk_reduce(int e, int split, int splits, int m_base, int n0, int M, int N,
                                                       uint32_t part_smem, __half* __restrict__ C,
-                                                      const Scales& scales) {
+                                                      const typename Cfg::EpiArgs& epi) {
   using namespace ptx;
+  const Scales& scales = scales_of(epi);
   constexpr int BN = Cfg::BN;
   constexpr int V = BN / 4;
   const float scale = output_scale<Cfg>(scales);
@@ -549,6 +747,7 @@ __device__ __forceinline__ void cluster_splitk_reduce(int e, int split, int spli
       }
     }
     scale_quad<Cfg>(acc, scale, scales, gm, gn);
+    bias_act_quad<Cfg>(acc, epi, gn);
     uint2 out;
     out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
     out.y = pack_out_x2_rn<Cfg::BF16>(acc.z, acc.w);
@@ -651,6 +850,9 @@ __device__ __forceinline__ void streamk_own(Reg (&d)[NR], int t, int ew, int lan
     for (int p = 0; p < n; ++p) flags[(slot0 + p * slot_stride) * kStreamKFlagsPerSlot + ew] = 0u;
 }
 
+// The kernel: hgemm_tn_kernel for every configuration but BiasAct<>'s, hgemm_bias_act_kernel for those. They differ in
+// their last parameter only (Cfg::EpiArgs) and share their body, hgemm_tn_kernel_body.inc, which reads the scales as
+// `scales` and hands the epilogues `epi`, the kernel's EpiArgs.
 template <class Cfg, int KMODE = kPlain>
 __global__ void __launch_bounds__(kNumThreads, 1)
 hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {BLOCK_K, A_BOX_ROWS}
@@ -670,472 +872,28 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
                 __half* __restrict__ c_raw,       // C base pointer, used by the split-K reductions' direct stores
                 uint64_t hint_a, uint64_t hint_b, // L2 eviction priority of the A / B loads (ptx::kL2Evict*)
                 Scales scales                     /* e4m3: the per-tensor scales (not read by the 16-bit kernels) */) {
-  constexpr int BN = Cfg::BN;
-  constexpr int STAGES = Cfg::STAGES;
-  constexpr int EM = Cfg::MCAST_M;
-  constexpr int CN = Cfg::CLUSTER_N;
-  constexpr int MR = Cfg::M_REP;
-  constexpr bool kSplit = (KMODE == kWorkspaceSplitK || KMODE == kClusterSplitK);
-  static_assert(!kSplit || Cfg::SPLIT_K, "this configuration has no split-K epilogues");
-  static_assert(KMODE != kStreamK || Cfg::STREAM_K, "this configuration has no stream-K epilogues");
-  static_assert(!kSplit || (kBlockM + 32) * BN * 4 <= STAGES * Cfg::STAGE_BYTES, "split-K partials must fit the pipeline smem");
-  // the schedule parameters a mode does not use are constants for it
-  const int splits = kSplit ? splits_arg : 1;
-  const int sk_tiles = (KMODE == kStreamK) ? aux_arg : 0;
-  using namespace ptx;
+  static_assert(!bias_act<Cfg>(), "BiasAct<> configurations: hgemm_bias_act_kernel");
+  const Scales& epi = scales;
+#include "hgemm_tn_kernel_body.inc"
+}
 
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t smem_a = smem_base;
-  const uint32_t smem_b = smem_a + STAGES * Cfg::A_STAGE_BYTES;
-  const uint32_t smem_epi = smem_b + STAGES * Cfg::B_STAGE_BYTES;
-  const uint32_t smem_bar = smem_epi + Cfg::EPI_BYTES;
-  const uint32_t bar_full = smem_bar;                        // [STAGES]
-  const uint32_t bar_empty = bar_full + 8 * STAGES;          // [STAGES]
-  const uint32_t bar_splitk = bar_empty + 8 * STAGES;        // split-K: bulk loads of the partial slices
-  constexpr bool kBlock = block_scaled<Cfg>();
-  static_assert(!kBlock || KMODE == kPlain || KMODE == kClusterSplitK, "block scales: plain and cluster split-K only");
-  [[maybe_unused]] const int ld_a = kBlock ? aux_arg : 0;
-  [[maybe_unused]] const uint32_t smem_scales = smem_bar + Cfg::BAR_BYTES;   // block scales: [STAGES] scale stages
-  constexpr bool kBatched = batched<Cfg>();
-  constexpr bool kGrouped = grouped<Cfg>();
-  constexpr bool kKGrouped = k_grouped<Cfg>();       // A [T, M] MN-major too, k-range per group (GroupedK<>)
-  constexpr bool kTileList = kBatched || kGrouped || kKGrouped;   // the schedule walks a cursor's flat tile list
-  constexpr bool kRowMajorB = row_major_b<Cfg>();    // B [K, N] in MN-major atom columns (RowMajorB<>)
-  static_assert(!kTileList || KMODE == kPlain, "batched / grouped: plain schedule only");
-  // grouped kernels: the group count and the offsets, in the same places (M is then T, the rows of A and C)
-  [[maybe_unused]] const int num_batches = kTileList ? splits_arg : 1;
-  [[maybe_unused]] const int* masked_m = kTileList ? reinterpret_cast<const int*>(splitk_ctr) : nullptr;
-  // the tile list of a batched or grouped launch; an empty stand-in for the other kernels, so that their code is as
-  // it was
-  using Cursor = typename Cfg::Cursor;
+// The same with a bias and an activation (BiasAct<>): the parameters of hgemm_tn_kernel, BiasActArgs last.
+template <class Cfg, int KMODE = kPlain>
+__global__ void __launch_bounds__(kNumThreads, 1)
+hgemm_bias_act_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                      const __grid_constant__ CUtensorMap tmap_c, int M, int N, int K, int group_m, int splits_arg,
+                      int aux_arg, float* __restrict__ splitk_ws, unsigned* __restrict__ splitk_ctr,
+                      __half* __restrict__ c_raw, uint64_t hint_a, uint64_t hint_b, BiasActArgs epi) {
+  static_assert(bias_act<Cfg>(), "a BiasAct<> configuration");
+  const Scales& scales = epi.scales;
+#include "hgemm_tn_kernel_body.inc"
+}
 
-  const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x) >> 5, 0);
-  const int lane = threadIdx.x & 31;
-  // Position inside the cluster: rank = mi + MCAST_M * cn (a cluster split-K launch of a plain config also has
-  // ranks, but does not use them here).
-  const uint32_t cluster_rank = (Cfg::CLUSTER_CTAS > 1) ? cluster_ctarank() : 0u;
-  const int mi = int(cluster_rank) % EM;
-  const int cn = int(cluster_rank) / EM;
-
-  // The schedule is over cluster blocks of (MCAST_M x CTA_M) x (CN x BN); a plain config has 1 x 1 blocks.
-  const int num_m_blocks = (M + Cfg::CTA_M * EM - 1) / (Cfg::CTA_M * EM);
-  const int num_n_blocks = (N + BN * CN - 1) / (BN * CN);
-  const int num_tiles = num_m_blocks * num_n_blocks;
-  const int num_k_blocks = (K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
-  const int num_workers = gridDim.x / Cfg::CLUSTER_CTAS;   // clusters (or single CTAs)
-  const int worker = blockIdx.x / Cfg::CLUSTER_CTAS;
-  // A work unit is (tile, k-block range), see hgemm_schedule.cuh. splits == 1: whole tiles walked persistently
-  // (after the worker's stream-K slice, if any). splits > 1: the host launches exactly one CTA per (tile, split)
-  // unit, so the sibling splits of a tile run concurrently.
-
-  // ------------------------------------------------------------------ one-time setup
-  // A stage of CTA X is refilled only after every CTA that X's loads land in (its cluster row and column) has
-  // released it: one arrive per consumer warp of each of those CTAs.
-  constexpr int kReleaseTargets = EM + CN - 1;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(bar_full + 8 * s, 1);                                  // the producer's arrive.expect_tx
-      mbar_init(bar_empty + 8 * s, 8 * kReleaseTargets);
-    }
-    mbar_init(bar_splitk, 1);
-    fence_mbar_init();
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_c);
-  }
-  if constexpr (Cfg::CLUSTER_CTAS > 1) cluster_sync_all(); else __syncthreads();
-
-  // Programmatic dependent launch (the host sets cudaLaunchAttributeProgrammaticStreamSerialization): this grid may have
-  // been started while the previous kernel of the stream was still running, so that everything above — barrier
-  // initialisation, descriptor prefetch, the set-up barrier — overlaps that kernel's tail instead of following it.
-  // Nothing above touches global memory; everything below may, so every thread first waits until the prerequisite
-  // grids have completed and their writes are visible (a no-op for an ordinary launch). The next kernel of the
-  // stream may in turn begin ITS prologue as soon as SMs free up.
-  grid_dependency_launch_dependents();
-  grid_dependency_wait();
-
-  // ------------------------------------------------------------------ roles
-  if (warp < kEpiWarp0) {
-    setmaxnreg_dec<kProducerRegs>();
-    if (warp == 0) {
-      // ===== TMA producer: the warp walks the schedule, one elected lane issues =====
-      // multicast masks: my A slice goes to the CTAs of my cluster row (same mi), my B slice to those of my
-      // cluster column (same cn)
-      uint16_t mask_a = 0, mask_b = 0;
-#pragma unroll
-      for (int j = 0; j < CN; ++j) mask_a |= uint16_t(1u << (mi + EM * j));
-#pragma unroll
-      for (int i = 0; i < EM; ++i) mask_b |= uint16_t(1u << (i + EM * cn));
-      const uint32_t a_slice = uint32_t(cn) * (Cfg::A_BOX_ROWS * kBlockK * 2);
-      const uint32_t b_slice = uint32_t(mi) * (Cfg::B_BOX_ROWS * kBlockK * 2);
-      int stage = 0; uint32_t phase = 0;
-      // batched: the list of (batch, cluster block) tiles, summed over the row counts (read after the dependency wait)
-      [[maybe_unused]] Cursor batches = make_cursor<Cfg>(masked_m, num_batches, M, K, Cfg::CTA_M * EM, num_n_blocks, group_m);
-      WorkIter work(worker, num_workers, kTileList ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
-      WorkUnit u;
-      while (work.next(u)) {
-        [[maybe_unused]] BatchTile bt{0, M, TileCoord{0, 0}};
-        if constexpr (kKGrouped) bt = batches.unit(u);   // the group's k-range; none for an empty group
-        else if constexpr (kTileList) bt = batches.locate(u.tile);
-        const TileCoord tc = kTileList ? bt.tc : tile_coord(u.tile, num_m_blocks, num_n_blocks, group_m);
-        const int m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M + cn * Cfg::A_BOX_ROWS;
-        const int n0 = (tc.n_blk * CN + cn) * BN + mi * Cfg::B_BOX_ROWS;
-        // block scales: this CTA's own rows of A's scales (never multicast; none past ld_a, so a padding CTA loads
-        // none) and the row of Bt's scales that holds the tile (none for a tile past N)
-        [[maybe_unused]] int sa_m0 = (tc.m_blk * EM + mi) * Cfg::CTA_M;
-        [[maybe_unused]] int sa_rows = kBlock ? max(0, min(Cfg::CTA_M, ld_a - sa_m0)) : 0;
-        [[maybe_unused]] const int sb_n0 = (tc.n_blk * CN + cn) * BN;
-        [[maybe_unused]] const float* sb_row = (kBlock && sb_n0 < N) ? scales.b + size_t(sb_n0 / 128) * num_k_blocks : nullptr;
-        if constexpr (kBlock && kGrouped) {
-          // the aligned window around the CTA's rows from the group's first row on (Grouped<BlockScaled<>>)
-          const int r0 = batches.start + sa_m0;
-          sa_m0 = r0 & ~3;
-          sa_rows = max(0, min(ld_a - sa_m0, ((r0 & 3) + Cfg::CTA_M + 3) & ~3));
-        }
-        if constexpr (kBlock && kTileList) {   // the scales of the batch's or group's own Bt
-          if (sb_row) sb_row += size_t(bt.batch) * ((N + 127) / 128) * num_k_blocks;
-        }
-        [[maybe_unused]] float sb_chunk = 0.f;   // lane j: Bt's scale of k-block kb0 + 32 i + j
-        for (int kb = u.kb0; kb < u.kb1; ++kb) {
-          mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-          [[maybe_unused]] float sb_kb = 0.f;
-          if constexpr (kBlock) {   // one global load per lane and 32 k-blocks, handed to the issuing lane by shuffle
-            if (((kb - u.kb0) & 31) == 0) sb_chunk = (sb_row && kb + lane < u.kb1) ? sb_row[kb + lane] : 0.f;
-            sb_kb = __shfl_sync(0xffffffffu, sb_chunk, (kb - u.kb0) & 31);
-          }
-          if (elect_one()) {
-            const uint32_t full = bar_full + 8 * stage;
-            if constexpr (kBlock) {
-              const uint32_t sc = smem_scales + stage * Cfg::SCALE_STAGE_BYTES;
-              st_shared_f32(sc + Cfg::SA_WINDOW_BYTES, sb_kb);   // published to the consumers by the arrive below
-              mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES + uint32_t(sa_rows) * 4u);
-              if (sa_rows > 0) {
-                if constexpr (kBatched)   // matrix b's [nkb, ld_a] block of A's scales (Batched<BlockScaled<>>)
-                  bulk_load_1d(sc, scales.a + (size_t(bt.batch) * num_k_blocks + kb) * ld_a + sa_m0,
-                               uint32_t(sa_rows) * 4u, full);
-                else
-                  bulk_load_1d(sc, scales.a + size_t(kb) * ld_a + sa_m0, uint32_t(sa_rows) * 4u, full);
-              }
-            } else {
-              mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);   // the whole stage lands here, from this CTA and its peers
-            }
-            const uint32_t dst_a = smem_a + stage * Cfg::A_STAGE_BYTES + a_slice;
-            const uint32_t dst_b = smem_b + stage * Cfg::B_STAGE_BYTES + b_slice;
-            if constexpr (kBatched) {
-              const int b = bt.batch;
-              if constexpr (CN > 1) tma_load_3d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, b, mask_a, hint_a);
-              else tma_load_3d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, b, hint_a);
-              if constexpr (EM > 1) tma_load_3d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, b, mask_b, hint_b);
-              else tma_load_3d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, b, hint_b);
-            } else if constexpr (kGrouped) {   // A rows from the group's first row on (rows past T read as zero)
-              const int ma = batches.start + m0, g = bt.batch;
-              if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, ma, mask_a, hint_a);
-              else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, ma, hint_a);
-              if constexpr (kRowMajorB) {
-                // B [G, K, N]: this CTA's K slice of every atom column of the group's matrix (Grouped<RowMajorB<>>)
-                const uint32_t dst = smem_b + stage * Cfg::B_STAGE_BYTES + uint32_t(mi) * (Cfg::B_K_ROWS * kBlockKBytes);
-                const int nb = (tc.n_blk * CN + cn) * BN, kr = kb * Cfg::BLOCK_K + mi * Cfg::B_K_ROWS;
-#pragma unroll
-                for (int j = 0; j < Cfg::B_ATOMS; ++j) {
-                  if constexpr (EM > 1)
-                    tma_load_3d_mcast_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, g, mask_b, hint_b);
-                  else
-                    tma_load_3d_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, g, hint_b);
-                }
-              } else {
-              if constexpr (EM > 1) tma_load_3d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, g, mask_b, hint_b);
-              else tma_load_3d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, g, hint_b);
-              }
-            } else if constexpr (kKGrouped) {
-              // A [T, M] and B [T, N], rows from the group's first row on: this CTA's K slice of every atom column of
-              // A (multicast to its cluster row) and of B (to its cluster column)
-              const int t0 = batches.start + kb * Cfg::BLOCK_K;
-              const uint32_t da = smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(cn) * (Cfg::A_K_ROWS * kBlockKBytes);
-              const int ma = (tc.m_blk * EM + mi) * Cfg::CTA_M, ka = t0 + cn * Cfg::A_K_ROWS;
-#pragma unroll
-              for (int j = 0; j < Cfg::A_ATOMS; ++j) {
-                if constexpr (CN > 1)
-                  tma_load_2d_mcast_hint(da + j * Cfg::B_ATOM_BYTES, &tmap_a, full, ma + 64 * j, ka, mask_a, hint_a);
-                else
-                  tma_load_2d_hint(da + j * Cfg::B_ATOM_BYTES, &tmap_a, full, ma + 64 * j, ka, hint_a);
-              }
-              const uint32_t db = smem_b + stage * Cfg::B_STAGE_BYTES + uint32_t(mi) * (Cfg::B_K_ROWS * kBlockKBytes);
-              const int nb = (tc.n_blk * CN + cn) * BN, kr = t0 + mi * Cfg::B_K_ROWS;
-#pragma unroll
-              for (int j = 0; j < Cfg::B_ATOMS; ++j) {
-                if constexpr (EM > 1)
-                  tma_load_2d_mcast_hint(db + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, mask_b, hint_b);
-                else
-                  tma_load_2d_hint(db + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, hint_b);
-              }
-            } else {
-            if constexpr (CN > 1) tma_load_2d_mcast_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, mask_a, hint_a);
-            else tma_load_2d_hint(dst_a, &tmap_a, full, kb * Cfg::BLOCK_K, m0, hint_a);
-            if constexpr (kRowMajorB) {
-              // B [K, N]: this CTA's K slice of every atom column of the tile, multicast to its cluster column
-              const uint32_t dst = smem_b + stage * Cfg::B_STAGE_BYTES + uint32_t(mi) * (Cfg::B_K_ROWS * kBlockKBytes);
-              const int nb = (tc.n_blk * CN + cn) * BN, kr = kb * Cfg::BLOCK_K + mi * Cfg::B_K_ROWS;
-#pragma unroll
-              for (int j = 0; j < Cfg::B_ATOMS; ++j) {
-                if constexpr (EM > 1)
-                  tma_load_2d_mcast_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, mask_b, hint_b);
-                else
-                  tma_load_2d_hint(dst + j * Cfg::B_ATOM_BYTES, &tmap_b, full, nb + 64 * j, kr, hint_b);
-              }
-            } else {
-            if constexpr (EM > 1) tma_load_2d_mcast_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, mask_b, hint_b);
-            else tma_load_2d_hint(dst_b, &tmap_b, full, kb * Cfg::BLOCK_K, n0, hint_b);
-            }
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    // every warpgroup ends inside its own branch: these warps run with the reduced register budget from here on
-    __syncwarp();
-    if constexpr (KMODE == kClusterSplitK) {
-      cluster_sync_all();   // the consumers' two cluster barriers around the split-K reduction
-      cluster_sync_all();
-    } else if constexpr (Cfg::CLUSTER_CTAS > 1) {
-      cluster_sync_all();   // no CTA of a cluster leaves while a peer may still multicast into it or arrive on its barriers
-    }
-  } else {
-    setmaxnreg_inc<kConsumerRegs>();
-    // ===== consumers: warpgroup wg owns rows [wg * 64 * MR, (wg + 1) * 64 * MR) of the CTA's tile =====
-    using W = typename std::conditional<kKGrouped, Wgmma<BN, true, Cfg::BF16, false, true, true>,
-                                        Wgmma<BN, Cfg::ACC_F32, Cfg::BF16 && !Cfg::E4M3, Cfg::E4M3, kRowMajorB>>::type;
-    // B's descriptor and its advance per k16 step (in 16-byte units): K-major, +32 B; MN-major (RowMajorB<>), +16 K
-    // rows of 128 B, atom columns 8 KB apart. The same for A: MN-major in the K-grouped kernels (GroupedK<>).
-    constexpr int kDescBStep = kRowMajorB ? 16 * kBlockKBytes / 16 : 2;
-    constexpr int kDescAStep = kKGrouped ? 16 * kBlockKBytes / 16 : 2;
-    using Reg = typename W::Reg;
-    constexpr int NR = W::kRegs;
-    const int wg = warp / 4 - 1;
-    const int wq = warp % 4;                       // warp inside the warpgroup: rows [16 wq, 16 wq + 16) of a 64-row block
-    const int ew = warp - kEpiWarp0;               // 0..7
-    const int t = int(threadIdx.x) - 128;          // 0..255
-    const uint32_t epi_buf = smem_epi + uint32_t(ew) * (Cfg::EPI_ROWS * 64 * 2);
-    [[maybe_unused]] int ck_m_base = 0, ck_n0 = 0, ck_split = 0;   // cluster split-K: where this CTA's unit lives
-    Reg acc[MR][NR];
-#pragma unroll
-    for (int r = 0; r < MR; ++r)
-#pragma unroll
-      for (int i = 0; i < NR; ++i) acc[r][i] = Reg(0);
-    // lanes 0 .. kReleaseTargets-1 each release a stage at one CTA: first my cluster column (including myself),
-    // then the rest of my cluster row
-    uint32_t empty_target = bar_empty;
-    if constexpr (kReleaseTargets > 1) {
-      uint32_t rank = cluster_rank;
-      if (lane < EM) rank = uint32_t(lane + EM * cn);
-      else if (lane < kReleaseTargets) { const int j = lane - EM; rank = uint32_t(mi + EM * (j < cn ? j : j + 1)); }
-      empty_target = mapa(bar_empty, rank);
-    }
-    auto release = [&](int s) {
-      __syncwarp();
-      if constexpr (kReleaseTargets > 1) {
-        if (lane < kReleaseTargets) mbar_arrive_cluster(empty_target + 8 * s);
-      } else {
-        if (lane == 0) mbar_arrive(bar_empty + 8 * s);
-      }
-    };
-    int stage = 0; uint32_t phase = 0;
-    [[maybe_unused]] Cursor batches = make_cursor<Cfg>(masked_m, num_batches, M, K, Cfg::CTA_M * EM, num_n_blocks, group_m);
-    WorkIter work(worker, num_workers, kTileList ? batches.total() : num_tiles, num_k_blocks, splits, sk_tiles);
-    WorkUnit u;
-    while (work.next(u)) {
-      if constexpr (kKGrouped) {
-        const BatchTile zt = batches.unit(u);   // the group's k-range, as the producer bounds it
-        if (u.kb1 == 0) {
-          // An empty group: the producer loaded nothing, and acc still holds the previous unit's sums (only a first
-          // wgmma's scale-d = 0 clears it). Its tile of +0.0 goes straight to C; acc is left alone, which keeps the
-          // accumulators out of a branch that ptxas would otherwise serve from local memory.
-          zero_tile_store<Cfg>(c_raw, zt.batch, (zt.tc.m_blk * EM + mi) * Cfg::CTA_M + wg * MR * 64 + wq * 16,
-                               (zt.tc.n_blk * CN + cn) * BN, M, N, lane);
-          continue;
-        }
-      }
-      if constexpr (kBlock) {
-        // ---- block-scaled main loop: each k-block's wgmma group sums into `part` (its first wgmma overwrites it),
-        // is retired, and is promoted into acc with fp32(sa[m] * sb): acc = p * s on the unit's first k-block (keeps
-        // the sign of zero), fmaf(p, s, acc) after it. The warpgroup's tensor-core work pauses during the promotion;
-        // the other consumer warpgroup, out of phase with it, keeps the tensor core busy.
-        static_assert(MR == 1 && Cfg::ACC_F32, "one 64-row block of fp32 accumulators per warpgroup");
-        Reg part[NR];
-        // row l/4 of the warp's 16; +8: +32 B. Grouped: the window starts start_g & 3 rows before the CTA's first row
-        [[maybe_unused]] uint32_t sa_shift = 0;
-        if constexpr (kGrouped) {
-          batches.locate(u.tile);
-          sa_shift = uint32_t(batches.start & 3) * 4u;
-        }
-        const uint32_t sa_off = uint32_t(wg * 64 + wq * 16 + (lane >> 2)) * 4u + sa_shift;
-        for (int kb = u.kb0; kb < u.kb1; ++kb) {
-          mbar_wait(bar_full + 8 * stage, phase);
-          const uint64_t da = make_smem_desc(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg) * (64 * kBlockK * 2));
-          const uint64_t db = make_smem_desc(smem_b + stage * Cfg::B_STAGE_BYTES);
-          reg_fence(part);
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < kBlockK / kWgmmaK; ++k) W::mma(da + uint64_t(2 * k), db + uint64_t(2 * k), part, k > 0 ? 1u : 0u);
-          wgmma_commit();
-          wgmma_wait<0>();
-          reg_fence(part);
-          const uint32_t sc = smem_scales + stage * Cfg::SCALE_STAGE_BYTES;
-          const float sb = ld_shared_f32(sc + Cfg::SA_WINDOW_BYTES);
-          const float s_lo = __fmul_rn(ld_shared_f32(sc + sa_off), sb);
-          const float s_hi = __fmul_rn(ld_shared_f32(sc + sa_off + 32u), sb);
-          release(stage);   // operands read by the retired group, scales in registers
-          if (kb == u.kb0) {
-#pragma unroll
-            for (int i = 0; i < NR; ++i) acc[0][i] = __fmul_rn(part[i], (i & 2) ? s_hi : s_lo);
-          } else {
-#pragma unroll
-            for (int i = 0; i < NR; ++i) acc[0][i] = __fmaf_rn(part[i], (i & 2) ? s_hi : s_lo, acc[0][i]);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        reg_fence(acc[0]);
-      } else {
-      // ---- main loop: one wgmma group per k-block, the previous one retired before its stage is released
-      int prev = -1;
-      for (int kb = u.kb0; kb < u.kb1; ++kb) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        if constexpr (kKGrouped) {
-          // the group's last k-block: rows [r, 64) of every atom column of both operands belong to the next group (or
-          // lie past T). A K row of an SW128 atom column is one contiguous 128-byte row, so each is one byte range.
-          const int r = (batches.end - batches.start) - kb * Cfg::BLOCK_K;
-          if (r < Cfg::BLOCK_K) {
-            const uint32_t a0 = smem_a + stage * Cfg::A_STAGE_BYTES, b0 = smem_b + stage * Cfg::B_STAGE_BYTES;
-            // 16 bytes per thread and atom column, 4 KB per pass over the 256 consumer threads: at most two passes
-#pragma unroll 1
-            for (uint32_t o = uint32_t(r * kBlockKBytes + 16 * t); o < uint32_t(Cfg::B_ATOM_BYTES); o += 16u * kConsumerThreads) {
-#pragma unroll
-              for (int j = 0; j < Cfg::A_ATOMS; ++j) st_shared_zero_v4(a0 + uint32_t(j * Cfg::B_ATOM_BYTES) + o);
-#pragma unroll
-              for (int j = 0; j < Cfg::B_ATOMS; ++j) st_shared_zero_v4(b0 + uint32_t(j * Cfg::B_ATOM_BYTES) + o);
-            }
-            fence_proxy_async_smem();   // the generic-proxy zeros before the wgmma's (async-proxy) reads
-            asm volatile("bar.sync 2, %0;" ::"n"(kConsumerThreads) : "memory");
-          }
-        }
-        uint64_t da;
-        if constexpr (kKGrouped)
-          da = make_smem_desc_mn(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg * MR) * (64 * kBlockK * 2), 64 * kBlockKBytes);
-        else
-          da = make_smem_desc(smem_a + stage * Cfg::A_STAGE_BYTES + uint32_t(wg * MR) * (64 * kBlockK * 2));
-        uint64_t db;
-        if constexpr (kRowMajorB) db = make_smem_desc_mn(smem_b + stage * Cfg::B_STAGE_BYTES, 64 * kBlockKBytes);
-        else db = make_smem_desc(smem_b + stage * Cfg::B_STAGE_BYTES);
-#pragma unroll
-        for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {   // four wgmmas of 32 bytes of K each, for every operand type
-#pragma unroll
-          for (int r = 0; r < MR; ++r)
-            W::mma(da + uint64_t(r * ((64 * kBlockK * 2) >> 4) + kDescAStep * k), db + uint64_t(kDescBStep * k), acc[r],
-                   (kb > u.kb0 || k > 0) ? 1u : 0u);
-        }
-        wgmma_commit();
-        // One group stays in flight while the next stage is awaited. The stream-K kernels carry the owner and contributor
-        // epilogues as well and spill under the 168-register launch bound; a spilled accumulator of an in-flight group
-        // would be read before the wgmma wrote it, so there every group is retired before anything else runs.
-        if constexpr (KMODE == kStreamK) wgmma_wait<0>();
-        else wgmma_wait<1>();
-#pragma unroll
-        for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
-        if (prev >= 0) release(prev);
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-#pragma unroll
-      for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
-      release(prev);
-      }
-
-      // ---- epilogue of the unit
-      const int tile = u.tile;
-      [[maybe_unused]] BatchTile bt{0, M, TileCoord{0, 0}};
-      if constexpr (kTileList) bt = batches.locate(tile);   // its boxes are stored only where they start below bt.rows
-      const TileCoord tc = kTileList ? bt.tc : tile_coord(tile, num_m_blocks, num_n_blocks, group_m);
-      const int m_cta = (tc.m_blk * EM + mi) * Cfg::CTA_M;
-      const int n0 = (tc.n_blk * CN + cn) * BN;
-      [[maybe_unused]] uint4* ws4 = reinterpret_cast<uint4*>(splitk_ws);
-      [[maybe_unused]] unsigned* sk_flags = splitk_ctr + 2 * kMaxSplitTiles;
-      if constexpr (KMODE == kStreamK) {
-        const int slot = worker * Cfg::CLUSTER_CTAS + int(cluster_rank);
-        if (u.kb0 > 0) {   // a later part of a tile's k-range, handed to the tile's owner
-          streamk_contribute<Cfg>(acc[0], t, ew, lane, ws4, sk_flags, slot);
-          continue;
-        }
-        if (u.kb1 < num_k_blocks) {   // the head of a tile, which owns it: add the rest of its k-range
-          const int n = streamk_contributors(worker, num_workers, sk_tiles * num_k_blocks, tile, num_k_blocks);
-          streamk_own<Cfg>(acc[0], t, ew, lane, ws4, sk_flags, slot + Cfg::CLUSTER_CTAS, Cfg::CLUSTER_CTAS, n);
-        }
-      }
-      if constexpr (KMODE == kClusterSplitK) {
-        // the partial tile goes where the operands were: both warpgroups must be done reading them
-        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
-        cluster_splitk_park<Cfg>(acc[0], wg * 64 + wq * 16, lane, smem_a);
-        ck_m_base = m_cta; ck_n0 = n0; ck_split = worker - tile * splits;   // the reduction runs after the cluster barrier below
-      } else if constexpr (KMODE == kWorkspaceSplitK) {
-        splitk_epilogue<Cfg>(acc[0], t, wg * 64 + wq * 16, lane, tile, worker - tile * splits, splits, m_cta, n0, M, N,
-                             splitk_ws, splitk_ctr, c_raw, smem_a, bar_splitk, scales);
-      } else {
-        if constexpr (Cfg::E4M3 && !kBlock) {   // block-scaled sums are already scaled: the epilogue only rounds
-          if (scales.rowwise) {
-            // each element gets its own factor, applied as it is packed for the store (epilogue_store_chunk)
-#pragma unroll
-            for (int r = 0; r < MR; ++r) {
-              const int row0 = m_cta + (wg * MR + r) * 64 + wq * 16;
-              const int ra = row0 + (lane >> 2), rb = ra + 8;   // frag_row of the even / odd pairs
-              const RowwiseEpi rw{ra < M ? scales.a[ra] : 0.f, rb < M ? scales.a[rb] : 0.f, scales.b};
-#pragma unroll
-              for (int j = 0; j < Cfg::EPI_CHUNKS; ++j)
-                epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, row0, M, N, &rw);
-            }
-            continue;   // the unit is done
-          }
-          // the finished sums are scaled in place, right before the epilogue rounds them: the scale is read per unit,
-          // after the main loop, and is dead before the epilogue's own temporaries are live
-          const float scale = output_scale<Cfg>(scales);
-#pragma unroll
-          for (int r = 0; r < MR; ++r)
-#pragma unroll
-            for (int i = 0; i < NR; ++i) acc[r][i] = __fmul_rn(acc[r][i], scale);
-#pragma unroll
-          for (int r = 0; r < MR; ++r) reg_fence(acc[r]);
-        }
-#pragma unroll
-        for (int r = 0; r < MR; ++r) {
-          const int row0 = m_cta + (wg * MR + r) * 64 + wq * 16;
-#pragma unroll
-          for (int j = 0; j < Cfg::EPI_CHUNKS; ++j) {
-            if constexpr (kGrouped)   // rows of C from the group's first row on, stored only below the group's end
-              epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, batches.start + row0,
-                                        batches.end, N, nullptr, 0, c_raw);
-            else
-              epilogue_store_chunk<Cfg>(acc[r], j, epi_buf, lane, &tmap_c, n0 + j * Cfg::EPI_N, row0,
-                                        kBatched ? bt.rows : M, N, nullptr, bt.batch);
-          }
-        }
-      }
-    }
-    // smem may be released once the bulk stores have READ it; their global writes complete with the grid
-    if (lane == 0) tma_store_wait_read<0>();
-    __syncwarp();
-    if constexpr (KMODE == kClusterSplitK) {
-      cluster_sync_all();   // every split's partial tile is parked in its CTA's shared memory
-      cluster_splitk_reduce<Cfg>(t, ck_split, splits, ck_m_base, ck_n0, M, N, smem_a, c_raw, scales);
-      __syncwarp();
-      cluster_sync_all();   // no CTA leaves (and frees its smem) while a peer may still be reading it
-    } else if constexpr (Cfg::CLUSTER_CTAS > 1) {
-      cluster_sync_all();   // no CTA of a cluster leaves while a peer may still multicast into it or arrive on its barriers
-    }
-  }
+// The kernel of (Cfg, KMODE).
+template <class Cfg, int KMODE>
+constexpr auto kernel_of() {
+  if constexpr (bias_act<Cfg>()) return &hgemm_bias_act_kernel<Cfg, KMODE>;
+  else return &hgemm_tn_kernel<Cfg, KMODE>;
 }
 
 }  // namespace b200

@@ -30,6 +30,13 @@ the nearest grid shape — so deployment is a plain operator:
   ``hgemm_grouped``'s product with a gradient. The forward is ``hgemm_grouped``'s kernel; ``dX`` runs
   ``hgemm_grouped_nn`` on the weight stack in place and ``dW`` ``hgemm_grouped_wgrad``, so a training step of the
   experts copies no operand. fp16 or bf16 with fp32 accumulation.
+* ``torch.ops.cuda_l2_b200.hgemm_bias_act(a, b_kmajor, bias=None, activation='none')``: ``act(a @ b_kmajor^T + bias)``
+  in one launch, fp16 or bf16 with fp32 accumulation; ``activation`` is "none", "relu" or "gelu_tanh" (torch's
+  ``_addmm_activation`` set). The bias is added to the fp32 sum and the activation applied before the one rounding to
+  the output type (libb200_epilogue.so, csrc/b200_epilogue.h). Its gradient reads relu's mask from the output and
+  recomputes gelu_tanh's pre-activation with one more launch. :func:`linear` is ``F.linear`` plus the activation on it,
+  for any leading dimensions. ``fp8_gemm_bias_act(a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype)`` is the
+  same epilogue after ``fp8_gemm``'s per-tensor or rowwise scales (inference only).
 * :class:`B200Linear`: ``y = x @ W^T (+ b)`` for any leading dimensions; :func:`replace_linear_modules` swaps the
   eligible ``nn.Linear`` layers of a model in place.
 * ``torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)``: ``float8_e4m3fn`` operands in the same
@@ -141,18 +148,23 @@ def _hgemm_fake(a, b_kmajor, acc="fp32"):
     return a.new_empty((m, n))
 
 
-def _hgemm_backward(ctx, grad_c):
-    a, b_kmajor = ctx.saved_tensors
+def _product_grads(a, b_kmajor, grad_c, need_a: bool, need_b: bool):
+    """(dA, dBt) of C = A Bt^T for the output gradient ``grad_c`` (None where not needed)."""
     grad_a = grad_b = None
     g = grad_c.contiguous()
     # C = A Bt^T  =>  dA = dC Bt  (reduction over N: Bt [N,K] is B row-major),  dBt = dC^T A  (reduction over M: A [M,K]
     # is B row-major). The row-major B kernels read both in place; only dC^T is copied. They compute what the K-major
     # kernels compute on transposed copies, bit for bit.
-    if ctx.needs_input_grad[0]:
+    if need_a:
         grad_a = torch.ops.cuda_l2_b200.hgemm_nn(g, b_kmajor, "fp32")
-    if ctx.needs_input_grad[1]:
+    if need_b:
         grad_b = torch.ops.cuda_l2_b200.hgemm_nn(g.t().contiguous(), a, "fp32")
-    return grad_a, grad_b, None
+    return grad_a, grad_b
+
+
+def _hgemm_backward(ctx, grad_c):
+    a, b_kmajor = ctx.saved_tensors
+    return (*_product_grads(a, b_kmajor, grad_c, ctx.needs_input_grad[0], ctx.needs_input_grad[1]), None)
 
 
 def _hgemm_setup_context(ctx, inputs, output):
@@ -526,6 +538,113 @@ def replace_linear_modules(model: nn.Module, acc: str = "fp32", skip: tuple[str,
     return done
 
 
+# ------------------------------------------------------------------------ bias + activation epilogue (libb200_epilogue.so)
+def _activate(z: torch.Tensor, activation: str) -> torch.Tensor:
+    if activation == "relu":
+        return torch.relu(z)
+    if activation == "gelu_tanh":
+        return torch.nn.functional.gelu(z, approximate="tanh")
+    return z
+
+
+def _bias_act_empty(c: torch.Tensor, k: int, bias, activation: str) -> bool:
+    """Whether the fused product into ``c`` needs no kernel: ``c`` has no element (M or N == 0), or the reduction is
+    empty (K == 0), which makes ``c`` act(bias) broadcast over the rows (act(0) without a bias), rounded once, as
+    ``addmm`` with an empty reduction gives. The C ABI rejects both with kBadShape."""
+    if c.numel() == 0:
+        return True
+    if k == 0:
+        z = torch.zeros(c.shape[1], dtype=torch.float32, device=c.device)
+        if bias is not None:
+            z = z + bias.float()
+        c.copy_(_activate(z, activation).expand_as(c))
+        return True
+    return False
+
+
+def _hgemm_bias_act_shape(a, b_kmajor, bias, activation):
+    m, n, k = capi.check_operands(a, b_kmajor, a.dtype, "fp32")
+    capi.epilogue_variant(a.dtype, a.dtype)
+    capi.check_bias(bias, n, a.dtype)
+    capi.activation_code(activation)
+    return m, n, k
+
+
+torch.library.define(f"{_LIB}::hgemm_bias_act",
+                     "(Tensor a, Tensor b_kmajor, Tensor? bias, str activation='none') -> Tensor")
+
+
+@torch.library.impl(f"{_LIB}::hgemm_bias_act", "CUDA")
+def _hgemm_bias_act_cuda(a, b_kmajor, bias=None, activation="none"):
+    m, n, k = _hgemm_bias_act_shape(a, b_kmajor, bias, activation)
+    c = torch.empty((m, n), dtype=a.dtype, device=a.device)
+    if _bias_act_empty(c, k, bias, activation):
+        return c
+    with torch.cuda.device(a.device):
+        capi.gemm_bias_act(a.contiguous(), b_kmajor.contiguous(), c, bias, activation,
+                           stream=torch.cuda.current_stream(a.device).cuda_stream)
+    return c
+
+
+@torch.library.impl(f"{_LIB}::hgemm_bias_act", "CPU")
+def _hgemm_bias_act_cpu(a, b_kmajor, bias=None, activation="none"):
+    raise capi.B200HgemmError("cuda_l2_b200::hgemm_bias_act has no CPU implementation (and no fallback): move the "
+                              "tensors to an H100")
+
+
+@torch.library.register_fake(f"{_LIB}::hgemm_bias_act")
+def _hgemm_bias_act_fake(a, b_kmajor, bias=None, activation="none"):
+    m, n, _ = _hgemm_bias_act_shape(a, b_kmajor, bias, activation)
+    return a.new_empty((m, n))
+
+
+def _hgemm_bias_act_backward(ctx, grad_y):
+    a, b_kmajor, bias, y = ctx.saved_tensors
+    # dZ, the gradient at the pre-activation z = A Bt^T + bias: relu's mask from the saved output (y > 0 exactly where
+    # z > 0 survived the rounding); gelu_tanh's derivative at z recomputed by the same kernel without the activation,
+    # so that the forward saves no pre-activation tensor.
+    if ctx.activation == "relu":
+        grad_z = grad_y * (y > 0)
+    elif ctx.activation == "gelu_tanh":
+        z = torch.ops.cuda_l2_b200.hgemm_bias_act(a, b_kmajor, bias, "none")
+        grad_z = torch.ops.aten.gelu_backward(grad_y, z, approximate="tanh")
+    else:
+        grad_z = grad_y
+    grad_a, grad_b = _product_grads(a, b_kmajor, grad_z, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+    grad_bias = None
+    if bias is not None and ctx.needs_input_grad[2]:
+        grad_bias = grad_z.sum(0, dtype=torch.float32).to(bias.dtype)
+    return grad_a, grad_b, grad_bias, None
+
+
+def _hgemm_bias_act_setup_context(ctx, inputs, output):
+    a, b_kmajor, bias, activation = inputs
+    ctx.activation = activation
+    ctx.save_for_backward(a, b_kmajor, bias, output if activation == "relu" else None)
+
+
+torch.library.register_autograd(f"{_LIB}::hgemm_bias_act", _hgemm_bias_act_backward,
+                                setup_context=_hgemm_bias_act_setup_context)
+
+
+def hgemm_bias_act(a: torch.Tensor, b_kmajor: torch.Tensor, bias: torch.Tensor | None = None,
+                   activation: str = "none") -> torch.Tensor:
+    """act(``a`` [M,K] @ ``b_kmajor`` [N,K]^T + ``bias``) -> [M,N] in one launch, fp32 until one rounding (see the
+    module docstring)."""
+    return torch.ops.cuda_l2_b200.hgemm_bias_act(a, b_kmajor, bias, activation)
+
+
+def linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = None,
+           activation: str = "none") -> torch.Tensor:
+    """``act(F.linear(x, weight, bias))`` for ``x`` [..., in_features] and ``weight`` [out_features, in_features]
+    (``F.linear``'s shapes), one fused launch of :func:`hgemm_bias_act`, with a gradient."""
+    if x.dim() == 0 or weight.dim() != 2:
+        raise capi.B200HgemmError(f"linear: x [..., in_features] and weight [out_features, in_features] expected, got "
+                                  f"{tuple(x.shape)} and {tuple(weight.shape)}")
+    y = torch.ops.cuda_l2_b200.hgemm_bias_act(x.reshape(-1, x.shape[-1]), weight, bias, activation)
+    return y.view(*x.shape[:-1], weight.shape[0])
+
+
 # ------------------------------------------------------------------------------------------ FP8 (e4m3), inference only
 E4M3_MAX = 448.0   # largest finite float8_e4m3fn value
 
@@ -578,6 +697,42 @@ def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, sca
     Per-tensor scales: one element each. Rowwise scales: ``scale_a`` [M,1], ``scale_b`` [1,N]. Blockwise scales:
     ``scale_a`` [M, ceil(K/128)] in any layout, ``scale_b`` [ceil(N/128), ceil(K/128)]."""
     return torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)
+
+
+def _fp8_bias_act_shape(a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype):
+    m, n, k = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
+    if capi.scale_granularity(m, n, scale_a, scale_b, k=k) == "blockwise":
+        raise capi.B200HgemmError("fp8_gemm_bias_act: blockwise scales have no bias + activation kernel (per-tensor or "
+                                  "rowwise scales only; run fp8_gemm and add the bias)")
+    capi.check_bias(bias, n, out_dtype)
+    capi.activation_code(activation)
+    return (m, n), out_dtype
+
+
+def _fp8_bias_act_launch(c, a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype, *, stream):
+    (m, n), k = c.shape, a.shape[1]
+    if _bias_act_empty(c, k, bias, activation):
+        return
+    if capi.scale_granularity(m, n, scale_a, scale_b, k=k) == "rowwise":
+        scale_a, scale_b = _rowwise_scale_arg(scale_a), _rowwise_scale_arg(scale_b)
+    else:
+        scale_a, scale_b = scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous()
+    capi.gemm_bias_act(a.contiguous(), b_kmajor.contiguous(), c, bias, activation, scale_a, scale_b, stream=stream)
+
+
+_inference_op("fp8_gemm_bias_act",
+              "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, Tensor? bias, str activation, "
+              "ScalarType out_dtype) -> Tensor",
+              _fp8_bias_act_shape, _fp8_bias_act_launch,
+              " (train with the fp16 / bf16 operator hgemm_bias_act and quantise afterwards)")
+
+
+def fp8_gemm_bias_act(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
+                      bias: torch.Tensor | None = None, activation: str = "none",
+                      out_dtype: torch.dtype = torch.float16) -> torch.Tensor:
+    """act((``a`` @ ``b_kmajor``^T) scaled + ``bias``) -> [M,N] ``out_dtype``, e4m3 operands with per-tensor or rowwise
+    scales (as :func:`fp8_gemm`), in one launch."""
+    return torch.ops.cuda_l2_b200.fp8_gemm_bias_act(a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype)
 
 
 def quantize_e4m3(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
