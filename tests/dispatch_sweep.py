@@ -16,6 +16,11 @@ test_gpu_dispatch_sweep.py (the results):
   the points where the nearest grid value changes, and shapes whose borrowed entry ``usable()`` rejects), at most
   ``OFFGRID_MAX_FLOP`` each;
 * :func:`tile_list_cases`: batched and grouped problems shaped like bmm and MoE layers.
+
+The row-major B (NN) and bias + activation legs (NN_LEGS, EPI_LEGS) and :func:`grouped_bwd_cases` (the MoE expert
+backward) are shared the same way by test_dispatch_sweep_late_cpu.py and test_gpu_dispatch_sweep_late.py. The bias legs'
+reference keeps the exact domain: :func:`epi_bias` draws biases exact in the output type, :func:`epilogue_blocks` adds
+them to the exact product in one fp32 addition, and gelu_tanh is held to epilogue_ref's allowance (:func:`gelu_ok`).
 """
 from __future__ import annotations
 
@@ -50,6 +55,31 @@ LEG_LISTS = {leg: ("grid", "offgrid") for leg in LEGS}
 LEG_LISTS["e4m3_block_fp16"] = ("grid",)
 LEG_LISTS["e4m3_block_bf16"] = ("offgrid",)
 TILE_LIST_VARIANTS = {"fp16": 0, "fp16acc16": 1, "bf16": 2}      # include/b200_batched.h's `variant`
+
+# The legs of the row-major B (NN) and bias + activation libraries (test_gpu_dispatch_sweep_late.py), kept apart from
+# LEGS so that the legs above, their lists and their seeds stay as they are. Same fields as LEGS.
+NN_LEGS = {
+    "nn_fp16": dict(operand="fp16", out="fp16", acc="fp32", scales=None, k_div=1, k_align=8),
+    "nn_fp16acc16": dict(operand="fp16", out="fp16", acc="fp16", scales=None, k_div=1, k_align=8),
+    "nn_bf16": dict(operand="bf16", out="bf16", acc="fp32", scales=None, k_div=1, k_align=8),
+}
+EPI_LEGS = {
+    "epi_fp16": dict(operand="fp16", out="fp16", acc="fp32", scales=None, k_div=1, k_align=8),
+    "epi_bf16": dict(operand="bf16", out="bf16", acc="fp32", scales=None, k_div=1, k_align=8),
+    "epi_e4m3_tensor_fp16": dict(operand="e4m3", out="fp16", acc="fp32", scales="tensor", k_div=2, k_align=16),
+    "epi_e4m3_rowwise_bf16": dict(operand="e4m3", out="bf16", acc="fp32", scales="rowwise", k_div=2, k_align=16),
+}
+LATE_LEGS = {**NN_LEGS, **EPI_LEGS}
+LATE_LEG_LISTS = {"nn_fp16": ("grid", "offgrid"), "nn_bf16": ("grid",), "nn_fp16acc16": ("offgrid",),
+                  "epi_fp16": ("grid",), "epi_e4m3_tensor_fp16": ("grid",), "epi_bf16": ("offgrid",),
+                  "epi_e4m3_rowwise_bf16": ("offgrid",)}
+EPI_VARIANTS = {"epi_fp16": 0, "epi_bf16": 2, "epi_e4m3_tensor_fp16": 3, "epi_e4m3_rowwise_bf16": 4}   # b200_epilogue.h
+ACTIVATIONS = ("none", "relu", "gelu_tanh")
+
+
+def leg_spec(leg: str) -> dict:
+    """The fields of ``leg``, a key of LEGS or of LATE_LEGS."""
+    return LEGS[leg] if leg in LEGS else LATE_LEGS[leg]
 
 
 def shape_seed(*dims) -> int:
@@ -120,7 +150,7 @@ def plan(leg: str, cfg: int, m: int, n: int, k: int, splits: int) -> tuple[str, 
     lib = capi.hgemm_lib()
     nw, sk, mode = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
     buf, contrib = (ctypes.c_int * 3)(), (ctypes.c_int * 1)()
-    kk = max(k // LEGS[leg]["k_div"], 1)
+    kk = max(k // leg_spec(leg)["k_div"], 1)
     st = lib.b200_hgemm_schedule_units(cfg, m, n, kk, splits, NUM_SMS, 0, buf, 0, ctypes.byref(nw), ctypes.byref(sk),
                                        ctypes.byref(mode), contrib)
     assert st >= 0, (leg, cfg, m, n, k, splits, st)
@@ -134,6 +164,37 @@ def l2_hint(cfg: dict, m: int, n: int, k: int, op_bytes: int) -> bool:
     n_tiles, m_tiles = -(-n // cfg["bn"]), -(-m // (128 * cfg["m_rep"] * cfg["cta_group"]))
     keep, stream = 20 << 20, 40 << 20
     return (a_bytes >= stream and b_bytes <= keep and n_tiles <= 4) or (b_bytes >= stream and a_bytes <= keep and m_tiles <= 4)
+
+
+def nn_sibling(configs: list, cid: int) -> int:
+    """hgemm_configs.cuh's nn::sibling: the configuration itself if it has a row-major B kernel (BN % 64 == 0), else the
+    BN = 64 one with the same CTA group, cluster_m and M_REP and the widest cluster_n up to its own."""
+    c = configs[cid]
+    if c["bn"] % 64 == 0:
+        return cid
+    cands = [d for d in configs if d["bn"] == 64 and d["cta_group"] == c["cta_group"] and d["cluster_m"] == c["cluster_m"]
+             and d["m_rep"] == c["m_rep"] and d["cluster_n"] <= c["cluster_n"]]
+    return max(cands, key=lambda d: d["cluster_n"])["id"]
+
+
+def nn_choice(leg: str, m: int, n: int, k: int) -> tuple[int, int, int, int]:
+    """hgemm_dispatch.cuh's select_rowmajor in Python: (cfg, group_m, splits) the dispatched NN call of ``leg`` runs,
+    and the TN configuration it was mapped from. A mapped BN = 32 choice loses its split code."""
+    from cuda_l2_b200 import capi
+    tn, gm, sp = capi.select(NN_LEGS[leg]["acc"], m, n, k)
+    cfg = nn_sibling(capi.configs(), tn)
+    return cfg, gm, sp if cfg == tn else 1, tn
+
+
+def epi_choice(leg: str, m: int, n: int, k: int) -> tuple[int, int, int]:
+    """(cfg, group_m, splits) the dispatched bias + activation call of ``leg`` uses."""
+    from cuda_l2_b200 import capi
+    return capi.epilogue_select(EPI_VARIANTS[leg], m, n, k)
+
+
+def epi_activation(leg: str, m: int, n: int, k: int) -> str:
+    """The activation an epilogue leg runs at (M, N, K): a seeded draw per shape and leg."""
+    return ACTIVATIONS[random.Random(shape_seed(m, n, k, len(leg), *map(ord, leg))).randrange(3)]
 
 
 # ------------------------------------------------------------------------------------------------- shape lists
@@ -156,8 +217,8 @@ def offgrid_shapes(leg: str) -> list[tuple[int, int, int]]:
     """A seeded off-grid sample for ``leg`` (a few hundred shapes): M = 1..16, odd M, ragged N (multiples of 8) and K
     (multiples of the leg's 16-byte K rule), neighbours g +- 8 / g +- 64 of grid values and of the points where the
     nearest grid value flips, and shapes that the heuristic decides because usable() rejects the borrowed entry. Every
-    shape does at most OFFGRID_MAX_FLOP."""
-    spec = LEGS[leg]
+    shape does at most OFFGRID_MAX_FLOP. ``leg``: a key of LEGS or of LATE_LEGS (seeded by its name either way)."""
+    spec = leg_spec(leg)
     ka = spec["k_align"]
     rng = random.Random(shape_seed(len(leg), *map(ord, leg)))
     grid = set(grid_shapes())
@@ -217,7 +278,7 @@ def offgrid_shapes(leg: str) -> list[tuple[int, int, int]]:
 
 def leg_shapes(leg: str) -> list[tuple[int, int, int]]:
     shapes = []
-    for name in LEG_LISTS[leg]:
+    for name in (LEG_LISTS[leg] if leg in LEG_LISTS else LATE_LEG_LISTS[leg]):
         shapes += grid_shapes() if name == "grid" else offgrid_shapes(leg)
     return shapes
 
@@ -260,6 +321,54 @@ def tile_list_cases() -> list[dict]:
         sizes[max(range(g), key=lambda j: w[j])] += used - sum(sizes)
         offs = list(np.cumsum(sizes).astype(int))
         cases.append(dict(kind="grouped", g=g, t=t, n=n, k=k, offs=[int(x) for x in offs]))
+    return cases
+
+
+GROUPED_BWD_VARIANTS = {"fp16": 0, "bf16": 2}       # csrc/b200_grouped_bwd.h's `variant`
+GROUPED_BWD_OUT_MAX = 2 ** 28                        # elements of the weight gradient, G * M * N
+
+
+@functools.lru_cache(maxsize=None)
+def grouped_bwd_cases() -> list[dict]:
+    """MoE-shaped backward problems of an expert layer x [T, d_in] -> y [T, d_out] with G experts: the input gradient
+    dX [T, d_in] = dY [T, d_out] @ W[g] (the grouped NN call, N = d_in, K = d_out) and the weight gradient
+    dW[g] = dY[s:e]^T X[s:e] [d_out, d_in] (the K-grouped call, M = d_out, N = d_in). Hidden sizes 1024..7168 and
+    expert widths 1408 / 2816 in either role, G in {1, 8, 64, 256}, T up to 64k, at most 2^37 FLOP (tile_list_cases'
+    cap) and GROUPED_BWD_OUT_MAX weight-gradient elements. Skewed group sizes with empty groups, one-row groups, starts
+    off every multiple of 8, the last end before T in one case of three; then T == 0 and an all-empty histogram.
+    Dicts: g, t, d_in, d_out, offs."""
+    rng = random.Random(20261017)
+    hidden, expert = (1024, 2048, 2560, 4096, 5120, 7168), (1408, 2816)
+    cases = []
+    for i in range(28):
+        g = (1, 8, 64, 256)[i % 4]
+        t = rng.choice((256, 1000, 2048, 4000, 8192, 16000, 30000, 65536))
+        h, e = rng.choice(hidden), rng.choice(expert)
+        d_in, d_out = (h, e) if i % 2 else (e, h)
+        if i == 0:
+            t, d_in, d_out = 65536, 1024, 1024                       # the longest T, at the FLOP cap
+        while 2 * t * d_in * d_out > 2 ** 37 or g * d_in * d_out > GROUPED_BWD_OUT_MAX:
+            if t > 2048 and 2 * t * d_in * d_out > 2 ** 37:
+                t //= 2
+            elif d_in >= d_out:
+                d_in = _round_up(d_in // 2, 8)
+            else:
+                d_out = _round_up(d_out // 2, 8)
+        w = [0.0 if rng.random() < 0.2 else 1.0 / (1 + rng.randrange(g)) ** 1.2 for _ in range(g)]
+        if not any(w):
+            w[0] = 1.0
+        used = t if i % 3 else t - rng.randrange(1, t // 4 + 2)       # one in three ends before T
+        sizes = [int(used * x / sum(w)) for x in w]
+        big = max(range(g), key=lambda j: w[j])
+        sizes[big] += used - sum(sizes)
+        j = (big + 1) % g
+        if g > 1 and sizes[big] + sizes[j] >= 2:                      # a one-row group, the total kept
+            sizes[big] += sizes[j] - 1
+            sizes[j] = 1
+        offs = [int(x) for x in np.cumsum(sizes)]
+        cases.append(dict(g=g, t=t, d_in=d_in, d_out=d_out, offs=offs))
+    cases.append(dict(g=8, t=0, d_in=1408, d_out=1024, offs=[0] * 8))           # T == 0 (weight gradient only)
+    cases.append(dict(g=64, t=1000, d_in=1024, d_out=1408, offs=[0] * 64))      # every group empty
     return cases
 
 
@@ -394,6 +503,13 @@ def _block_factors(s, k: int):
 def reference_blocks(torch, ops, out: str, scales=None, granularity=None, rows_per_block=None):
     """Yield (lo, hi, bits) for row blocks of the true output: int16 bits [hi - lo, N]. ``scales``: the float64 numpy
     values of e4m3_scales for ``granularity``. The product is a float64 GEMM on the operands' device."""
+    for lo, hi, y in exact_blocks(torch, ops, scales, granularity, rows_per_block):
+        yield lo, hi, round_to(torch, y, out)
+
+
+def exact_blocks(torch, ops, scales=None, granularity=None, rows_per_block=None):
+    """Yield (lo, hi, y) for row blocks of the exact scaled product, float64 [hi - lo, N] (reference_blocks before its
+    one rounding)."""
     a, bt = ops.a, ops.bt
     (m, k), n = a.shape, bt.shape[0]
     dev = a.device
@@ -418,7 +534,7 @@ def reference_blocks(torch, ops, out: str, scales=None, granularity=None, rows_p
         elif granularity == "rowwise":
             y *= sb[None, :]
             y *= sa[lo:hi, None]
-        yield lo, hi, round_to(torch, y, out)
+        yield lo, hi, y
 
 
 def numpy_rows(torch, ops, rows, cols, out: str, scales=None, granularity=None) -> np.ndarray:
@@ -459,3 +575,146 @@ def sample_cols(n: int, seed: int, limit: int = 1024) -> list[int]:
         return list(range(n))
     rng = random.Random(seed)
     return sorted(set(rng.sample(range(n), limit - 2)) | {0, n - 1})
+
+
+# ------------------------------------------------------------------------------------------------- bias + activation
+BIAS_NEG_ZERO, BIAS_POS_ZERO = 0.25, 0.05     # fractions of the columns whose bias is -0.0 / +0.0
+GELU_ABS = 2.0 ** -22                          # epilogue_ref.GELU_ABS
+_OUT_DTYPE = {"fp16": "float16", "bf16": "bfloat16"}
+
+
+def _median(values) -> int:
+    return sorted(values)[len(values) // 2]
+
+
+def _sum_log2(spec: dict, k: int) -> float:
+    """log2 of the spread of a random row's sum_k i j (operands16 / operands_e4m3): sqrt(K) lim_a lim_b / 3 for the
+    uniform 16-bit integers, sqrt(4/9 nonzeros) for the e4m3 +-1 / 0 ones."""
+    if spec["operand"] == "e4m3":
+        return 0.5 * math.log2(4 / 9 * min(k, E4M3_NNZ))
+    lim_b = 63 if spec["operand"] == "fp16" else 31
+    lim_a = min(2047 if spec["operand"] == "fp16" else 255, (ed.EXACT_SUM_BOUND - 1) // (k * lim_b))
+    return math.log2(math.sqrt(k) * lim_a * lim_b / 3)
+
+
+def epi_bias(torch, leg: str, ops, scales, n: int, k: int, seed: int, device="cuda"):
+    """The bias [N] of an epilogue leg, in the output type, every value exact there: a quarter of the columns -0.0 (z is
+    the product itself, so the probe rows' planted rounding targets still round), a few +0.0, the rest +-q 2^e with a
+    significand q of the output's width and an exponent within a few binades of what the column's product reaches at a
+    typical row (the column exponent of operands16, or the e4m3 scales, at the median row exponent), so that
+    z = s + bias takes the bias's sign on the rows of smaller exponent and the product's on the others."""
+    spec = EPI_LEGS[leg]
+    out = spec["out"]
+    p, emin, emax = (11, -24, 15) if out == "fp16" else (8, -133, 127)
+    if spec["operand"] != "e4m3":
+        col = ops.col_exp.to(torch.float64) + _median(ed.ROW_EXP[spec["operand"]])
+    elif spec["scales"] == "tensor":
+        col = torch.full((n,), math.log2(float(np.float32(scales[0]) * np.float32(scales[1]))), dtype=torch.float64,
+                         device=device)
+    else:
+        q = _median(ed.E4M3_Q[out])
+        col = torch.log2(torch.from_numpy(scales[1]).to(device)) + math.log2(q) + _median(ed.E4M3_ROW_EXP)
+    gen = torch.Generator(device=device).manual_seed(seed)
+    u = torch.rand((n,), generator=gen, device=device, dtype=torch.float64)
+    q = torch.randint(1 << (p - 1), 1 << p, (n,), generator=gen, device=device).to(torch.float64)
+    sign = torch.randint(0, 2, (n,), generator=gen, device=device).to(torch.float64) * 2 - 1
+    jitter = torch.randint(-3, 3, (n,), generator=gen, device=device).to(torch.float64)
+    e = (torch.round(col + _sum_log2(spec, k)) + jitter - (p - 1)).clamp(emin, emax - (p - 1))
+    val = sign * q * torch.exp2(e)
+    val[u < BIAS_NEG_ZERO + BIAS_POS_ZERO] = 0.0
+    val[u < BIAS_NEG_ZERO] = -0.0
+    bias = val.to(getattr(torch, _OUT_DTYPE[out]))
+    assert torch.equal(bias.to(torch.float64), val), "bias not exact in the output type"
+    return bias
+
+
+def epilogue_blocks(torch, ops, bias, scales=None, granularity=None, rows_per_block=None):
+    """Yield (lo, hi, z) for row blocks of the fused call's pre-activation, fp32 [hi - lo, N]: the exact scaled product s
+    (exact_blocks; asserted exact in fp32, per-tensor e4m3 scales may take it past the largest fp32, to inf as in the
+    kernel) plus the bias, one IEEE fp32 addition on the operands' device."""
+    b32 = bias.to(torch.float32)
+    for lo, hi, y in exact_blocks(torch, ops, scales, granularity, rows_per_block):
+        s = y.to(torch.float32)
+        fin = torch.isfinite(s)
+        assert torch.equal(s[fin].to(torch.float64), y[fin]), "not exact in fp32"
+        del y, fin
+        yield lo, hi, s.add_(b32[None, :])
+
+
+def activated_bits(torch, z, activation: str, out: str):
+    """int16 bits of none / relu of fp32 z, rounded once to ``out``: relu is z > 0 ? z : +0.0."""
+    if activation == "relu":
+        z = torch.where(z > 0, z, torch.zeros_like(z))
+    else:
+        assert activation == "none", activation
+    return z.to(getattr(torch, _OUT_DTYPE[out])).view(torch.int16)
+
+
+def _ulp_at(torch, x, out: str):
+    """epilogue_ref.ulp_at on the device."""
+    p, emin = (11, -14) if out == "fp16" else (8, -126)
+    ax = x.abs()
+    e = torch.where(ax > 0, torch.clamp(torch.frexp(ax).exponent.to(torch.float64) - 1, min=emin),
+                    torch.full_like(ax, emin))
+    return torch.exp2(e - (p - 1))
+
+
+def gelu_ok(torch, got_bits, z, out: str):
+    """Where a gelu_tanh output is what epilogue_ref.gelu_excess allows (within one unit in the last place of the
+    float64 tanh form, plus |z| GELU_ABS), on the device; an output equal to the float64 form rounded (infinities) or
+    NaN where it is NaN passes too. Bool [like z]."""
+    z64 = z.to(torch.float64)
+    want = 0.5 * z64 * (1.0 + torch.tanh(math.sqrt(2.0 / math.pi) * (z64 + 0.044715 * z64 ** 3)))
+    dt = getattr(torch, _OUT_DTYPE[out])
+    got = got_bits.view(dt).to(torch.float64)
+    excess = (got - want).abs() - (_ulp_at(torch, want, out) + z64.abs() * GELU_ABS)
+    return (excess <= 0) | (got == want.to(torch.float32).to(dt).to(torch.float64)) | (got.isnan() & want.isnan())
+
+
+def epilogue_numpy_rows(torch, ops, rows, cols, bias, activation: str, out: str, scales=None, granularity=None):
+    """epilogue_ref on ``rows`` x ``cols``, in numpy from the operands: (fp32 z, output bits or None for gelu_tanh)."""
+    import epilogue_ref
+    ri, ci = torch.as_tensor(rows, device=ops.a.device), torch.as_tensor(cols, device=ops.a.device)
+    a = ops.a[ri].to(torch.float32).cpu().numpy().astype(np.float64)
+    b = ops.bt[ci].to(torch.float32).cpu().numpy().astype(np.float64)
+    b32 = bias[ci].to(torch.float32).cpu().numpy()
+    sa = sb = None
+    if granularity == "tensor":
+        sa, sb = np.float32(scales[0]), np.float32(scales[1])
+    elif granularity == "rowwise":
+        sa, sb = scales[0][np.asarray(rows)], scales[1][np.asarray(cols)]
+    rowwise = granularity == "rowwise"
+    with np.errstate(over="ignore", invalid="ignore"):
+        z = epilogue_ref.pre_activation(a, b, b32, sa, sb, rowwise)
+        bits = None if activation == "gelu_tanh" else epilogue_ref.reference(a, b, b32, activation, out, sa, sb, rowwise)
+    return z, bits
+
+
+# ------------------------------------------------------------------------------------------------- grouped backward
+def grouped_nn_operands(torch, t: int, g: int, n: int, k: int, kind: str, seed: int, device="cuda"):
+    """a [T, K] and b [G, K, N] row-major of the grouped NN call: operands16(T, G N, K), b[g] = bt[g]^T."""
+    ops = operands16(torch, t, g * n, k, kind, seed, device=device)
+    return ops.a, ops.bt.view(g, n, k).transpose(1, 2).contiguous()
+
+
+def wgrad_operands(torch, t: int, m: int, n: int, kind: str, seed: int, device="cuda"):
+    """a [T, M] and b [T, N] of the K-grouped call: operands16(M, N, T) transposed, so that each row and column exponent
+    is constant along the reduction axis T. A group's sum over rows [s, e) of T is then a subset of an exactly summable
+    row sum, and exact too. T == 0: empty operands."""
+    dtype = torch.float16 if kind == "fp16" else torch.bfloat16
+    if t == 0:
+        return torch.empty((0, m), dtype=dtype, device=device), torch.empty((0, n), dtype=dtype, device=device)
+    ops = operands16(torch, m, n, t, kind, seed, device=device)
+    return ops.a.t().contiguous(), ops.bt.t().contiguous()
+
+
+def grouped_nn_reference(torch, a, b, s: int, e: int, g: int, out: str):
+    """int16 bits of group g's rows [s, e) of the grouped NN product, rounded once."""
+    return round_to(torch, a[s:e].to(torch.float64) @ b[g].to(torch.float64), out)
+
+
+def wgrad_reference(torch, a, b, s: int, e: int, out: str):
+    """int16 bits of one group's weight gradient a[s:e]^T b[s:e] [M, N], rounded once (+0.0 for an empty group). A sum
+    of zero products is +0.0, as in an accumulator that starts at +0.0: a one-row group's float64 product of 0 and a
+    negative value is -0.0, so the zeros are normalised (y + 0.0)."""
+    return round_to(torch, (a[s:e].to(torch.float64).T @ b[s:e].to(torch.float64)).add_(0.0), out)
