@@ -14,6 +14,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
   the input gradient and the K-grouped kernels of the weight gradient (csrc/b200_grouped_bwd.h; no public symbol)
 * ``libb200_epilogue.so`` — the 2-D fp16 / bf16 / e4m3 GEMM with a fused bias + ReLU / tanh-GELU epilogue
   (csrc/b200_epilogue.h; no public symbol)
+* ``libb200_quant.so``  — the one-pass e4m3 quantisers of FP8 activations: per tensor, rowwise, 1 x 128 blocks and
+  SwiGLU + 1 x 128 blocks (csrc/b200_quant.h; no public symbol)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -117,6 +119,7 @@ LIBRARIES = {
     "nn": ("libb200_nn.so", _per_variant("b200_nn.cu", VARIANTS), []),
     "grouped_bwd": ("libb200_grouped_bwd.so", _per_variant("b200_grouped_bwd.cu", BWD_VARIANTS), []),
     "epilogue": ("libb200_epilogue.so", _per_variant("b200_epilogue.cu", EPILOGUE_VARIANTS), []),
+    "quant": ("libb200_quant.so", [(CSRC / "b200_quant.cu", [])], []),
     "baselines": ("libb200_baselines.so", [(CSRC / "b200_baselines_capi.cu", [])], ["-lcublas", "-lcublasLt"]),
 }
 

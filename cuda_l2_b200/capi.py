@@ -105,6 +105,8 @@ GROUPED_BWD_LIB = "libb200_grouped_bwd.so"   # csrc/b200_grouped_bwd.h
 _BWD_RUN = ([_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i)
 _BWD_SELECT = ([_i, _i, _i, _i, _i, _ip, _ip], _i)
 EPILOGUE_LIB = "libb200_epilogue.so"         # csrc/b200_epilogue.h
+QUANT_LIB = "libb200_quant.so"               # csrc/b200_quant.h
+_QUANT_BLOCKWISE = ([_i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp], _i)
 INTERNAL_ABI = {
     GROUPED_BWD_LIB: {
         "cuda_l2_b200_grouped_bwd_nn": _BWD_RUN,
@@ -124,6 +126,14 @@ INTERNAL_ABI = {
         "cuda_l2_b200_epilogue_release": ([], _i),
         "cuda_l2_b200_epilogue_launch_count": ([], ctypes.c_ulonglong),
         "cuda_l2_b200_epilogue_strerror": ([_i], ctypes.c_char_p),
+    },
+    QUANT_LIB: {
+        "cuda_l2_b200_quant_e4m3_tensor": ([_i, _vp, ctypes.c_longlong, _vp, _vp, _vp, _vp], _i),
+        "cuda_l2_b200_quant_e4m3_rowwise": ([_i, _vp, _i, _i, _vp, _vp, _vp], _i),
+        "cuda_l2_b200_quant_e4m3_blockwise": _QUANT_BLOCKWISE,
+        "cuda_l2_b200_quant_silu_mul_e4m3_blockwise": _QUANT_BLOCKWISE,
+        "cuda_l2_b200_quant_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_quant_strerror": ([_i], ctypes.c_char_p),
     },
 }
 _libs: dict = {}
@@ -1137,3 +1147,127 @@ def epilogue_release() -> None:
 
 def epilogue_launch_count() -> int:
     return int(epilogue_lib().cuda_l2_b200_epilogue_launch_count())
+
+
+# ------------------------------------------------------------------------------------------ e4m3 quantisers
+#                                                                                            (libb200_quant.so)
+QUANT_TENSOR_WORKSPACE = 1024   # floats of the per-tensor quantiser's workspace (csrc/b200_quant.h)
+
+
+def quant_lib() -> ctypes.CDLL:
+    """libb200_quant.so: the one-pass e4m3 quantisers of FP8 activations (csrc/b200_quant.h, no public ABI)."""
+    return load(QUANT_LIB)
+
+
+def quant_dtype(dtype, silu_mul: bool = False) -> int | None:
+    """The ``dtype`` code of csrc/b200_quant.h for an input of this torch dtype: 0 fp16, 1 bf16, 2 fp32 (the SwiGLU
+    kernel takes fp16 and bf16 only); None if no kernel takes it."""
+    import torch
+
+    codes = {torch.float16: 0, torch.bfloat16: 1} if silu_mul else {torch.float16: 0, torch.bfloat16: 1,
+                                                                     torch.float32: 2}
+    return codes.get(dtype)
+
+
+def _quant_check(st: int, what: str) -> None:
+    if st != 0:
+        raise B200HgemmError(f"{what} failed: status {st} ({quant_lib().cuda_l2_b200_quant_strerror(st).decode()})")
+
+
+def _quant_input(x, silu_mul: bool = False) -> int:
+    """The dtype code of ``x``, a contiguous CUDA tensor of a dtype a quantiser takes; B200HgemmError otherwise."""
+    code = quant_dtype(x.dtype, silu_mul)
+    if code is None:
+        raise B200HgemmError(f"no e4m3 quantiser for {x.dtype} input (fp16, bf16{'' if silu_mul else ', fp32'})")
+    _contiguous_cuda(x=x)
+    return code
+
+
+def _quant_output(q, shape, x) -> None:
+    import torch
+
+    if q.dtype != torch.float8_e4m3fn or tuple(q.shape) != tuple(shape) or not q.is_contiguous() or \
+            q.device != x.device:
+        raise B200HgemmError(f"q must be a contiguous float8_e4m3fn tensor {list(shape)} on {x.device}, got {q.dtype} "
+                             f"{tuple(q.shape)} on {q.device}")
+
+
+def _fp32_on(t, x, name: str, shape) -> None:
+    import torch
+
+    if t.dtype != torch.float32 or tuple(t.shape) != tuple(shape) or t.device != x.device:
+        raise B200HgemmError(f"{name} must be an fp32 tensor {list(shape)} on {x.device}, got {t.dtype} "
+                             f"{tuple(t.shape)} on {t.device}")
+
+
+def quantize_e4m3(x, q, scale, workspace, stream: int | None = None) -> None:
+    """Per-tensor quantisation of ``x`` (fp16, bf16 or fp32, contiguous, at least one element) into ``q`` (e4m3,
+    x's shape) and ``scale`` (one fp32 element), in two launches; ``workspace``: QUANT_TENSOR_WORKSPACE fp32 elements
+    of device memory that no other call uses until this one has run (csrc/b200_quant.h)."""
+    code = _quant_input(x)
+    _quant_output(q, x.shape, x)
+    _fp32_on(scale, x, "scale", (1,))
+    _fp32_on(workspace, x, "workspace", (QUANT_TENSOR_WORKSPACE,))
+    _contiguous_cuda(workspace=workspace)
+    _quant_check(quant_lib().cuda_l2_b200_quant_e4m3_tensor(code, x.data_ptr(), x.numel(), q.data_ptr(),
+                                                            scale.data_ptr(), workspace.data_ptr(), stream),
+                 "cuda_l2_b200_quant_e4m3_tensor")
+
+
+def quantize_e4m3_rowwise(x, q, scale, stream: int | None = None) -> None:
+    """Rowwise quantisation of a 2-D ``x`` [rows, cols] (fp16, bf16 or fp32, contiguous) into ``q`` (e4m3 [rows, cols])
+    and ``scale`` (fp32 [rows, 1], contiguous), in one launch."""
+    code = _quant_input(x)
+    if x.dim() != 2:
+        raise B200HgemmError(f"the rowwise quantiser takes a 2-D [rows, cols] tensor, got {list(x.shape)}")
+    rows, cols = x.shape
+    _quant_output(q, x.shape, x)
+    _fp32_on(scale, x, "scale", (rows, 1))
+    _contiguous_cuda(scale=scale)
+    _quant_check(quant_lib().cuda_l2_b200_quant_e4m3_rowwise(code, x.data_ptr(), rows, cols, q.data_ptr(),
+                                                             scale.data_ptr(), stream),
+                 "cuda_l2_b200_quant_e4m3_rowwise")
+
+
+def _blockwise_call(symbol: str, x, q, scale, masked_m, k: int, silu_mul: bool, stream) -> None:
+    """The 1 x 128 quantisers: ``x`` [(B,) M, K] (or SwiGLU's h [(B,) M, 2K]) into ``q`` [(B,) M, K] and ``scale``
+    [(B,) M, ceil(K/128)] in the M-major layout of :func:`blockwise_ld_a`, with optional int32 ``masked_m`` [B]."""
+    import torch
+
+    code = _quant_input(x, silu_mul)
+    if x.dim() not in (2, 3):
+        raise B200HgemmError(f"the 1 x 128 quantisers take [M, K] or [B, M, K] inputs, got {list(x.shape)}")
+    *lead, m, _ = x.shape
+    bsz = lead[0] if lead else 1
+    _quant_output(q, (*lead, m, k), x)
+    _fp32_on(scale, x, "scale", (*lead, m, num_k_blocks(k)))
+    ld_a = _scale_ld_a(scale)
+    if masked_m is not None:
+        _contiguous_cuda(masked_m=masked_m)
+        if masked_m.dtype != torch.int32 or tuple(masked_m.shape) != (bsz,) or masked_m.device != x.device:
+            raise B200HgemmError(f"masked_m must be an int32 tensor of shape [{bsz}] on {x.device}, got "
+                                 f"{masked_m.dtype} {tuple(masked_m.shape)} on {masked_m.device}")
+    _quant_check(getattr(quant_lib(), symbol)(code, x.data_ptr(), bsz, m, k, q.data_ptr(), scale.data_ptr(), ld_a,
+                                              None if masked_m is None else masked_m.data_ptr(), stream), symbol)
+
+
+def quantize_e4m3_blockwise(x, q, scale, masked_m=None, stream: int | None = None) -> None:
+    """1 x 128 quantisation of ``x`` [(B,) M, K] (fp16, bf16 or fp32, contiguous) into ``q`` (e4m3, x's shape) and
+    ``scale`` [(B,) M, ceil(K/128)], written in place in its M-major layout (:func:`blockwise_ld_a`: a view of a
+    [(B,) ceil(K/128), ld_a] buffer), in one launch. ``masked_m``: an optional int32 CUDA tensor [B]; only rows
+    [0, clamp(masked_m[b], 0, M)) of matrix b are read and written, in q and in scale."""
+    _blockwise_call("cuda_l2_b200_quant_e4m3_blockwise", x, q, scale, masked_m, x.shape[-1], False, stream)
+
+
+def silu_mul_quantize_e4m3_blockwise(h, q, scale, masked_m=None, stream: int | None = None) -> None:
+    """1 x 128 quantisation of silu(g) * u, with g = h[..., :I] and u = h[..., I:] of ``h`` [(B,) M, 2I] (fp16 or
+    bf16, contiguous), into ``q`` [(B,) M, I] and ``scale`` [(B,) M, ceil(I/128)] as for
+    :func:`quantize_e4m3_blockwise`, ``masked_m`` likewise, in one launch."""
+    if h.shape[-1] % 2:
+        raise B200HgemmError(f"h must be [(B,) M, 2I], got {list(h.shape)}")
+    _blockwise_call("cuda_l2_b200_quant_silu_mul_e4m3_blockwise", h, q, scale, masked_m, h.shape[-1] // 2, True,
+                    stream)
+
+
+def quant_launch_count() -> int:
+    return int(quant_lib().cuda_l2_b200_quant_launch_count())

@@ -59,6 +59,14 @@ the nearest grid shape — so deployment is a plain operator:
 * :class:`B200Fp8GroupedLinear`: those experts as a module, from a checkpoint's stacked e4m3 weights and block scales
   (:meth:`B200Fp8GroupedLinear.from_fp8`) or from a 16-bit stack (:meth:`B200Fp8GroupedLinear.from_weights`);
   ``forward`` takes the prefill layout, ``forward_masked`` the decode layout.
+* ``torch.ops.cuda_l2_b200.quantize_e4m3(x)``, ``quantize_e4m3_rowwise(x)``, ``quantize_e4m3_blockwise(x,
+  masked_m=None)`` and ``silu_mul_quantize_e4m3_blockwise(h, masked_m=None)``: the FP8 GEMMs' A operand and scales in
+  one pass over a 16-bit or fp32 activation (libb200_quant.so, csrc/b200_quant.h), each returning ``(q, scale)`` with
+  the bits of the torch composition :func:`quantize_e4m3` and its siblings keep as ``*_reference``. The last one
+  quantises ``F.silu(g) * u`` of a gate/up product ``h = [g | u]``. :func:`quantize_e4m3` and its siblings route CUDA
+  tensors to them. Inference only.
+* :class:`B200Fp8GroupedMLP`: the routed experts of an FP8 MoE checkpoint as a gated MLP, four launches per forward
+  (quantise, gate/up GEMM, SwiGLU + quantise, down GEMM), in the prefill or the decode layout.
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernels, so a fine-tuning
@@ -76,30 +84,41 @@ from . import capi
 _LIB = "cuda_l2_b200"
 
 
-def _inference_op(name: str, schema: str, shape, launch, why: str = "") -> None:
+def _inference_op(name: str, schema: str, shape, launch, why: str = "", outputs=None) -> None:
     """Defines the inference-only operator cuda_l2_b200::<name> with ``schema``. ``shape(*args)`` checks the arguments
     by the kernel's rules (meta tensors pass) and returns the result's shape and dtype: the fake implementation is an
     empty tensor of those, and the CUDA one allocates the result ``c`` on the operands' device and calls
     ``launch(c, *args, stream=...)`` there, on torch's current stream, so that it orders with the surrounding torch ops.
-    The CPU implementation raises (there is no fallback), and so does a backward through it (``why`` says why)."""
+    An operator with several results passes ``outputs`` instead of ``shape``: ``outputs(*args)`` checks the arguments
+    the same way and returns the tuple of empty results, allocated on the device of ``args[0]`` in their final layout;
+    the CUDA and the fake implementation both call it, so the fake results have the real ones' shapes and strides, and
+    ``launch`` receives the tuple. The CPU implementation raises (there is no fallback), and so does a backward through
+    it (``why`` says why)."""
     qualname = f"{_LIB}::{name}"
     torch.library.define(qualname, schema)
 
     def cuda(*args):
-        out_shape, dtype = shape(*args)
-        c = torch.empty(out_shape, dtype=dtype, device=args[0].device)
-        with torch.cuda.device(c.device):
-            launch(c, *args, stream=torch.cuda.current_stream(c.device).cuda_stream)
+        if outputs is not None:
+            c = outputs(*args)
+            device = args[0].device
+        else:
+            out_shape, dtype = shape(*args)
+            c = torch.empty(out_shape, dtype=dtype, device=args[0].device)
+            device = c.device
+        with torch.cuda.device(device):
+            launch(c, *args, stream=torch.cuda.current_stream(device).cuda_stream)
         return c
 
     def cpu(*args):
         raise capi.B200HgemmError(f"{qualname} has no CPU implementation (and no fallback): move the tensors to an H100")
 
     def fake(*args):
+        if outputs is not None:
+            return outputs(*args)
         out_shape, dtype = shape(*args)
         return args[0].new_empty(out_shape, dtype=dtype)
 
-    def no_backward(ctx, grad_c):
+    def no_backward(ctx, *grads):
         raise capi.B200HgemmError(f"{qualname} is inference only: it has no gradient{why}")
 
     torch.library.impl(qualname, "CUDA")(cuda)
@@ -735,29 +754,37 @@ def fp8_gemm_bias_act(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Te
     return torch.ops.cuda_l2_b200.fp8_gemm_bias_act(a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype)
 
 
-def quantize_e4m3(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
-    """Per-tensor quantisation on x's device: scale = amax(|x|) / 448 (a one-element fp32 tensor), q = e4m3(x / scale).
-    Torch ops only, no host synchronisation."""
+# ------------------------------------------------------------------------------------------ e4m3 quantisers of
+#                                                                                            activations (libb200_quant.so)
+# Each quantiser has a torch composition, the ``*_reference`` function, and an operator that runs the one-pass kernel
+# of libb200_quant.so with the reference's bits on CUDA (csrc/b200_quant.h). The public function routes a non-empty
+# CUDA tensor of a dtype a kernel takes to the operator and anything else (CPU tensors in particular) to the reference.
+def quantize_e4m3_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """:func:`quantize_e4m3` as a composition of torch ops."""
     scale = (x.abs().amax().float() / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny).reshape(1)
     q = (x.float() / scale).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
     return q, scale
 
 
-def quantize_e4m3_rowwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
-    """Per-row quantisation of a 2-D ``x`` [rows, cols] on its device: scale[r] = amax(|x[r]|) / 448 (an fp32
-    [rows, 1] tensor), q = e4m3(x / scale). One outlier row no longer squeezes every other row into e4m3's few low
-    codes. Torch ops only, no host synchronisation."""
+def quantize_e4m3_rowwise_reference(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """:func:`quantize_e4m3_rowwise` as a composition of torch ops."""
     scale = (x.abs().amax(dim=1, keepdim=True).float() / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
     q = (x.float() / scale).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
     return q, scale
 
 
-def quantize_e4m3_blockwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
-    """Per 1 x 128 block quantisation of activations ``x`` [M, K] on its device: scale[m, kb] = amax(|x[m, 128 kb :
-    128 kb + 128]|) / 448, q = e4m3(x / scale). The scale comes back as the M-major [M, ceil(K/128)] view the kernel
-    reads in place (strides (1, ld_a), ld_a = M rounded up to 4). A batch ``x`` [B, M, K] is quantised per matrix, the
-    same way: its scale is [B, M, ceil(K/128)], a view of a [B, ceil(K/128), ld_a] buffer that the batched kernel reads
-    in place (strides (ceil(K/128) * ld_a, 1, ld_a)). Torch ops only, no host synchronisation."""
+def _blockwise_scale(lead, m: int, nkb: int, device) -> torch.Tensor:
+    """An empty blockwise scale [(B,) M, nkb] in the layout of the reference's: the view
+    ``buf[..., :M].transpose(-2, -1)`` of a [(B,) nkb, ld_a] buffer, ld_a = M rounded up to 4, which the block-scaled
+    GEMMs read in place."""
+    buf = torch.empty((*lead, nkb, -(-m // 4) * 4), dtype=torch.float32, device=device)
+    return buf[..., :m].transpose(-2, -1)
+
+
+def quantize_e4m3_blockwise_reference(x: torch.Tensor, masked_m: torch.Tensor | None = None
+                                      ) -> tuple[torch.Tensor, torch.Tensor]:
+    """:func:`quantize_e4m3_blockwise` as a composition of torch ops. ``masked_m`` changes nothing here: every row is
+    computed."""
     if x.dim() not in (2, 3):
         raise capi.B200HgemmError(f"quantize_e4m3_blockwise takes [M, K] or [B, M, K], got {list(x.shape)}")
     *lead, m, k = x.shape
@@ -768,6 +795,147 @@ def quantize_e4m3_blockwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor
     buf = torch.empty((*lead, nkb, -(-m // 4) * 4), dtype=torch.float32, device=x.device)
     buf[..., :m].copy_(scale.transpose(-2, -1))
     return q[..., :k].contiguous(), buf[..., :m].transpose(-2, -1)
+
+
+def silu_mul_quantize_e4m3_blockwise_reference(h: torch.Tensor, masked_m: torch.Tensor | None = None
+                                               ) -> tuple[torch.Tensor, torch.Tensor]:
+    """:func:`silu_mul_quantize_e4m3_blockwise` as a composition of torch ops: ``F.silu(g) * u``, then
+    :func:`quantize_e4m3_blockwise_reference`. ``masked_m`` changes nothing here."""
+    i = _swiglu_width(h)
+    return quantize_e4m3_blockwise_reference(nn.functional.silu(h[..., :i]) * h[..., i:])
+
+
+def _swiglu_width(h: torch.Tensor) -> int:
+    """I of a SwiGLU input h [(B,) M, 2I]; B200HgemmError for any other shape."""
+    if h.dim() not in (2, 3) or h.shape[-1] % 2:
+        raise capi.B200HgemmError(f"h must be [M, 2I] or [B, M, 2I], got {list(h.shape)}")
+    return h.shape[-1] // 2
+
+
+def _quant_routed(x: torch.Tensor, silu_mul: bool = False) -> bool:
+    """Whether a quantiser of libb200_quant.so runs on ``x``: a non-empty CUDA tensor of a dtype it takes."""
+    return x.is_cuda and x.numel() > 0 and capi.quant_dtype(x.dtype, silu_mul) is not None
+
+
+def _quant_input(x: torch.Tensor, silu_mul: bool = False) -> None:
+    if capi.quant_dtype(x.dtype, silu_mul) is None:
+        raise capi.B200HgemmError(f"no e4m3 quantiser for {x.dtype} input (fp16, bf16{'' if silu_mul else ', fp32'})")
+    if x.numel() == 0:
+        raise capi.B200HgemmError(f"the e4m3 quantisers take non-empty inputs, got {list(x.shape)}")
+
+
+def _check_masked_m(masked_m, bsz: int) -> None:
+    if masked_m is not None and (masked_m.dtype != torch.int32 or tuple(masked_m.shape) != (bsz,)):
+        raise capi.B200HgemmError(f"masked_m must be an int32 tensor of shape [{bsz}], got {masked_m.dtype} "
+                                  f"{tuple(masked_m.shape)}")
+
+
+def _quantize_e4m3_outputs(x):
+    _quant_input(x)
+    return x.new_empty(x.shape, dtype=torch.float8_e4m3fn), x.new_empty((1,), dtype=torch.float32)
+
+
+def _quantize_e4m3_launch(out, x, *, stream):
+    workspace = torch.empty(capi.QUANT_TENSOR_WORKSPACE, dtype=torch.float32, device=x.device)
+    capi.quantize_e4m3(x.contiguous(), *out, workspace, stream=stream)
+
+
+def _quantize_e4m3_rowwise_outputs(x):
+    _quant_input(x)
+    if x.dim() != 2:
+        raise capi.B200HgemmError(f"quantize_e4m3_rowwise takes [rows, cols], got {list(x.shape)}")
+    return x.new_empty(x.shape, dtype=torch.float8_e4m3fn), x.new_empty((x.shape[0], 1), dtype=torch.float32)
+
+
+def _quantize_e4m3_rowwise_launch(out, x, *, stream):
+    capi.quantize_e4m3_rowwise(x.contiguous(), *out, stream=stream)
+
+
+def _blockwise_outputs(x, k: int, masked_m):
+    *lead, m, _ = x.shape
+    _check_masked_m(masked_m, lead[0] if lead else 1)
+    return (x.new_empty((*lead, m, k), dtype=torch.float8_e4m3fn),
+            _blockwise_scale(lead, m, capi.num_k_blocks(k), x.device))
+
+
+def _quantize_e4m3_blockwise_outputs(x, masked_m=None):
+    _quant_input(x)
+    if x.dim() not in (2, 3):
+        raise capi.B200HgemmError(f"quantize_e4m3_blockwise takes [M, K] or [B, M, K], got {list(x.shape)}")
+    return _blockwise_outputs(x, x.shape[-1], masked_m)
+
+
+def _quantize_e4m3_blockwise_launch(out, x, masked_m=None, *, stream):
+    capi.quantize_e4m3_blockwise(x.contiguous(), *out, None if masked_m is None else masked_m.contiguous(),
+                                 stream=stream)
+
+
+def _silu_mul_outputs(h, masked_m=None):
+    _quant_input(h, silu_mul=True)
+    return _blockwise_outputs(h, _swiglu_width(h), masked_m)
+
+
+def _silu_mul_launch(out, h, masked_m=None, *, stream):
+    capi.silu_mul_quantize_e4m3_blockwise(h.contiguous(), *out, None if masked_m is None else masked_m.contiguous(),
+                                          stream=stream)
+
+
+_QUANT_WHY = " (quantisation is not differentiable: train the 16-bit model and quantise afterwards)"
+_inference_op("quantize_e4m3", "(Tensor x) -> (Tensor, Tensor)", None, _quantize_e4m3_launch, _QUANT_WHY,
+              outputs=_quantize_e4m3_outputs)
+_inference_op("quantize_e4m3_rowwise", "(Tensor x) -> (Tensor, Tensor)", None, _quantize_e4m3_rowwise_launch,
+              _QUANT_WHY, outputs=_quantize_e4m3_rowwise_outputs)
+_inference_op("quantize_e4m3_blockwise", "(Tensor x, Tensor? masked_m=None) -> (Tensor, Tensor)", None,
+              _quantize_e4m3_blockwise_launch, _QUANT_WHY, outputs=_quantize_e4m3_blockwise_outputs)
+_inference_op("silu_mul_quantize_e4m3_blockwise", "(Tensor h, Tensor? masked_m=None) -> (Tensor, Tensor)", None,
+              _silu_mul_launch, _QUANT_WHY, outputs=_silu_mul_outputs)
+
+
+def quantize_e4m3(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per-tensor quantisation on x's device: scale = amax(|x|) / 448 (a one-element fp32 tensor), q = e4m3(x / scale).
+    No host synchronisation. A CUDA fp16 / bf16 / fp32 tensor runs ``cuda_l2_b200::quantize_e4m3`` (two launches),
+    anything else :func:`quantize_e4m3_reference`, with the same bits."""
+    if _quant_routed(x):
+        return torch.ops.cuda_l2_b200.quantize_e4m3(x)
+    return quantize_e4m3_reference(x)
+
+
+def quantize_e4m3_rowwise(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per-row quantisation of a 2-D ``x`` [rows, cols] on its device: scale[r] = amax(|x[r]|) / 448 (an fp32
+    [rows, 1] tensor), q = e4m3(x / scale). One outlier row no longer squeezes every other row into e4m3's few low
+    codes. No host synchronisation. A 2-D CUDA fp16 / bf16 / fp32 tensor runs ``cuda_l2_b200::quantize_e4m3_rowwise``
+    (one launch), anything else :func:`quantize_e4m3_rowwise_reference`, with the same bits."""
+    if x.dim() == 2 and _quant_routed(x):
+        return torch.ops.cuda_l2_b200.quantize_e4m3_rowwise(x)
+    return quantize_e4m3_rowwise_reference(x)
+
+
+def quantize_e4m3_blockwise(x: torch.Tensor, masked_m: torch.Tensor | None = None
+                            ) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per 1 x 128 block quantisation of activations ``x`` [M, K] on its device: scale[m, kb] = amax(|x[m, 128 kb :
+    128 kb + 128]|) / 448, q = e4m3(x / scale). The scale comes back as the M-major [M, ceil(K/128)] view the kernel
+    reads in place (strides (1, ld_a), ld_a = M rounded up to 4). A batch ``x`` [B, M, K] is quantised per matrix, the
+    same way: its scale is [B, M, ceil(K/128)], a view of a [B, ceil(K/128), ld_a] buffer that the batched kernel reads
+    in place (strides (ceil(K/128) * ld_a, 1, ld_a)). No host synchronisation. A CUDA fp16 / bf16 / fp32 tensor runs
+    ``cuda_l2_b200::quantize_e4m3_blockwise`` (one launch), anything else :func:`quantize_e4m3_blockwise_reference`,
+    with the same bits. ``masked_m``: optional int32 tensor [B] on x's device, the per-matrix row counts of the
+    masked batched GEMM; the kernel then reads and writes only rows [0, clamp(masked_m[b], 0, M)) of matrix b (the
+    rest of q and scale is unspecified), the reference computes every row."""
+    if x.dim() in (2, 3) and _quant_routed(x):
+        return torch.ops.cuda_l2_b200.quantize_e4m3_blockwise(x, masked_m)
+    return quantize_e4m3_blockwise_reference(x, masked_m)
+
+
+def silu_mul_quantize_e4m3_blockwise(h: torch.Tensor, masked_m: torch.Tensor | None = None
+                                     ) -> tuple[torch.Tensor, torch.Tensor]:
+    """The SwiGLU of a gated MLP, quantised for the next FP8 GEMM: ``h`` [(B,) M, 2I] holds the gate g = h[..., :I]
+    and the up projection u = h[..., I:] (the fused w13 layout of vLLM / SGLang checkpoints); returns
+    :func:`quantize_e4m3_blockwise` of ``F.silu(g) * u`` [(B,) M, I], bit for bit. A CUDA fp16 / bf16 tensor runs
+    ``cuda_l2_b200::silu_mul_quantize_e4m3_blockwise`` (one launch, no intermediate in memory), anything else
+    :func:`silu_mul_quantize_e4m3_blockwise_reference`. ``masked_m`` as for :func:`quantize_e4m3_blockwise`."""
+    if _quant_routed(h, silu_mul=True) and h.dim() in (2, 3) and h.shape[-1] % 2 == 0:
+        return torch.ops.cuda_l2_b200.silu_mul_quantize_e4m3_blockwise(h, masked_m)
+    return silu_mul_quantize_e4m3_blockwise_reference(h, masked_m)
 
 
 def quantize_e4m3_block128x128(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
@@ -976,8 +1144,9 @@ class B200Fp8GroupedLinear(nn.Module):
         int32 token counts ``masked_m`` [G] on the GPU -> [G, M, N]. Rows [0, clamp(masked_m[g], 0, M)) of expert g are
         computed; the rest of its slot in the result is unspecified. Quantises ``x`` per token and 128 input channels
         on the device and runs ``cuda_l2_b200::fp8_batched_gemm``: no host synchronisation, so it can be captured in a
-        CUDA graph."""
-        x_q, x_scale = quantize_e4m3_blockwise(x)
+        CUDA graph. The quantiser, too, reads and writes only the counted rows: the others are rows the GEMM treats
+        as unspecified."""
+        x_q, x_scale = quantize_e4m3_blockwise(x, masked_m)
         return torch.ops.cuda_l2_b200.fp8_batched_gemm(x_q, self.weight_fp8, x_scale, self.weight_scale,
                                                        self.out_dtype, masked_m)
 
@@ -986,7 +1155,86 @@ class B200Fp8GroupedLinear(nn.Module):
                 f"out_dtype={self.out_dtype}")
 
 
+class B200Fp8GroupedMLP(nn.Module):
+    """Inference-only routed experts of an FP8 mixture-of-experts checkpoint as a gated MLP: for the tokens of expert
+    g, ``y = (silu(x W1[g]^T) * (x W3[g]^T)) W2[g]^T``, with the gate and up projections fused in one stack
+    ``w13_fp8`` [G, 2I, H] (W1 in rows [0, I), W3 in rows [I, 2I): the w13 layout of vLLM / SGLang checkpoints) and
+    ``w2_fp8`` [G, H, I], both e4m3 with 128 x 128 block scales. A forward is four launches and no host
+    synchronisation: :func:`quantize_e4m3_blockwise` of x, the gate/up FP8 GEMM (out_dtype h [.., 2I]),
+    :func:`silu_mul_quantize_e4m3_blockwise` of h, and the down FP8 GEMM. Needs H % 16 == 0 and I % 16 == 0."""
+
+    @classmethod
+    def from_fp8(cls, w13_fp8: torch.Tensor, w13_scale: torch.Tensor, w2_fp8: torch.Tensor, w2_scale: torch.Tensor,
+                 out_dtype: torch.dtype = torch.bfloat16) -> "B200Fp8GroupedMLP":
+        """The experts of a checkpoint, taken as they are: the e4m3 stacks ``w13_fp8`` [G, 2I, H] and ``w2_fp8``
+        [G, H, I] with their fp32 128 x 128 block scales [G, ceil(2I/128), ceil(H/128)] and [G, ceil(H/128),
+        ceil(I/128)]. ``out_dtype`` (fp16 or bf16) is that of the gate/up product and of the result."""
+        try:
+            g, two_i, hid = w13_fp8.shape
+            g2, hid2, i = w2_fp8.shape
+        except ValueError:
+            raise capi.B200HgemmError(f"from_fp8 needs stacks w13 [G, 2I, H] and w2 [G, H, I], got "
+                                      f"{list(w13_fp8.shape)} and {list(w2_fp8.shape)}") from None
+        if g < 1 or g2 != g or hid2 != hid or two_i != 2 * i or hid % 16 or i % 16:
+            raise capi.B200HgemmError(f"B200Fp8GroupedMLP needs w13 [G, 2I, H] and w2 [G, H, I] with G >= 1, "
+                                      f"H % 16 == 0 and I % 16 == 0, got {list(w13_fp8.shape)} and "
+                                      f"{list(w2_fp8.shape)}")
+        if out_dtype not in (torch.float16, torch.bfloat16):
+            raise capi.B200HgemmError(f"out_dtype must be fp16 or bf16, got {out_dtype}")
+        for name, w, s in (("w13", w13_fp8, w13_scale), ("w2", w2_fp8, w2_scale)):
+            want = (g, -(-w.shape[1] // capi.BLOCK), capi.num_k_blocks(w.shape[2]))
+            if w.dtype != torch.float8_e4m3fn or s.dtype != torch.float32 or tuple(s.shape) != want:
+                raise capi.B200HgemmError(f"{name} must be a float8_e4m3fn stack with fp32 block scales of shape "
+                                          f"{list(want)}, got {w.dtype} and {s.dtype} {list(s.shape)}")
+        new = cls()
+        new.num_experts, new.hidden_size, new.intermediate_size, new.out_dtype = g, hid, i, out_dtype
+        new.register_buffer("w13_fp8", w13_fp8.contiguous())
+        new.register_buffer("w13_scale", w13_scale.contiguous())
+        new.register_buffer("w2_fp8", w2_fp8.contiguous())
+        new.register_buffer("w2_scale", w2_scale.contiguous())
+        return new
+
+    @classmethod
+    def from_weights(cls, w13: torch.Tensor, w2: torch.Tensor) -> "B200Fp8GroupedMLP":
+        """The experts from 16-bit stacks ``w13`` [G, 2I, H] and ``w2`` [G, H, I] of one dtype, quantised per
+        128 x 128 block; the output dtype is theirs."""
+        if w13.dtype not in (torch.float16, torch.bfloat16) or w2.dtype != w13.dtype or w13.dim() != 3 or \
+                w2.dim() != 3:
+            raise capi.B200HgemmError(f"from_weights needs fp16 / bf16 stacks w13 [G, 2I, H] and w2 [G, H, I] of one "
+                                      f"dtype, got {w13.dtype} {list(w13.shape)} and {w2.dtype} {list(w2.shape)}")
+        with torch.no_grad():
+            w13_q, w13_s = quantize_e4m3_block128x128(w13)
+            w2_q, w2_s = quantize_e4m3_block128x128(w2)
+        return cls.from_fp8(w13_q, w13_s, w2_q, w2_s, w13.dtype)
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+        """``x`` [T, H], the tokens sorted by expert, and the int32 cumulative group ends ``offs`` [G] on the GPU ->
+        [T, H]. Rows at or past ``offs[-1]`` of the result are unspecified."""
+        x_q, x_scale = quantize_e4m3_blockwise(x)
+        h = torch.ops.cuda_l2_b200.fp8_grouped_gemm(x_q, self.w13_fp8, x_scale, self.w13_scale, offs, self.out_dtype)
+        p_q, p_scale = silu_mul_quantize_e4m3_blockwise(h)
+        return torch.ops.cuda_l2_b200.fp8_grouped_gemm(p_q, self.w2_fp8, p_scale, self.w2_scale, offs,
+                                                       self.out_dtype)
+
+    def forward_masked(self, x: torch.Tensor, masked_m: torch.Tensor) -> torch.Tensor:
+        """The same experts in the padded decode layout: ``x`` [G, M, H], one slot of M tokens per expert, and the
+        int32 token counts ``masked_m`` [G] on the GPU -> [G, M, H]. Rows [0, clamp(masked_m[g], 0, M)) of expert g
+        are computed; the rest of its slot in the result is unspecified. Both quantisers take ``masked_m`` too, so
+        no launch reads or writes a row past the counts."""
+        x_q, x_scale = quantize_e4m3_blockwise(x, masked_m)
+        h = torch.ops.cuda_l2_b200.fp8_batched_gemm(x_q, self.w13_fp8, x_scale, self.w13_scale, self.out_dtype,
+                                                    masked_m)
+        p_q, p_scale = silu_mul_quantize_e4m3_blockwise(h, masked_m)
+        return torch.ops.cuda_l2_b200.fp8_batched_gemm(p_q, self.w2_fp8, p_scale, self.w2_scale, self.out_dtype,
+                                                       masked_m)
+
+    def extra_repr(self) -> str:
+        return (f"num_experts={self.num_experts}, hidden_size={self.hidden_size}, "
+                f"intermediate_size={self.intermediate_size}, out_dtype={self.out_dtype}")
+
+
 __all__ = ["hgemm", "hgemm_nn", "hgemm_batched", "hgemm_grouped", "hgemm_grouped_nn", "hgemm_grouped_wgrad",
            "grouped_linear", "B200GroupedLinear", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear",
-           "fp8_grouped_gemm", "fp8_batched_gemm", "B200Fp8GroupedLinear"]
+           "fp8_grouped_gemm", "fp8_batched_gemm", "B200Fp8GroupedLinear", "silu_mul_quantize_e4m3_blockwise",
+           "B200Fp8GroupedMLP"]
