@@ -16,6 +16,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
   (csrc/b200_epilogue.h; no public symbol)
 * ``libb200_quant.so``  — the one-pass e4m3 quantisers of FP8 activations: per tensor, rowwise, 1 x 128 blocks and
   SwiGLU + 1 x 128 blocks (csrc/b200_quant.h; no public symbol)
+* ``libb200_quant_dual.so`` — the dual-orientation rowwise e4m3 quantiser of FP8 training: x and x^T quantised from
+  one tensor (csrc/b200_quant_dual.h; no public symbol)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -120,6 +122,7 @@ LIBRARIES = {
     "grouped_bwd": ("libb200_grouped_bwd.so", _per_variant("b200_grouped_bwd.cu", BWD_VARIANTS), []),
     "epilogue": ("libb200_epilogue.so", _per_variant("b200_epilogue.cu", EPILOGUE_VARIANTS), []),
     "quant": ("libb200_quant.so", [(CSRC / "b200_quant.cu", [])], []),
+    "quant_dual": ("libb200_quant_dual.so", [(CSRC / "b200_quant_dual.cu", [])], []),
     "baselines": ("libb200_baselines.so", [(CSRC / "b200_baselines_capi.cu", [])], ["-lcublas", "-lcublasLt"]),
 }
 

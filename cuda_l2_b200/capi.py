@@ -106,6 +106,7 @@ _BWD_RUN = ([_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i)
 _BWD_SELECT = ([_i, _i, _i, _i, _i, _ip, _ip], _i)
 EPILOGUE_LIB = "libb200_epilogue.so"         # csrc/b200_epilogue.h
 QUANT_LIB = "libb200_quant.so"               # csrc/b200_quant.h
+QUANT_DUAL_LIB = "libb200_quant_dual.so"     # csrc/b200_quant_dual.h
 _QUANT_BLOCKWISE = ([_i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp], _i)
 INTERNAL_ABI = {
     GROUPED_BWD_LIB: {
@@ -134,6 +135,11 @@ INTERNAL_ABI = {
         "cuda_l2_b200_quant_silu_mul_e4m3_blockwise": _QUANT_BLOCKWISE,
         "cuda_l2_b200_quant_launch_count": ([], ctypes.c_ulonglong),
         "cuda_l2_b200_quant_strerror": ([_i], ctypes.c_char_p),
+    },
+    QUANT_DUAL_LIB: {
+        "cuda_l2_b200_quant_dual_e4m3_rowwise": ([_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
+        "cuda_l2_b200_quant_dual_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_quant_dual_strerror": ([_i], ctypes.c_char_p),
     },
 }
 _libs: dict = {}
@@ -1271,3 +1277,49 @@ def silu_mul_quantize_e4m3_blockwise(h, q, scale, masked_m=None, stream: int | N
 
 def quant_launch_count() -> int:
     return int(quant_lib().cuda_l2_b200_quant_launch_count())
+
+
+# ------------------------------------------------------------------------------------------ dual-orientation rowwise
+#                                                                                            e4m3 (libb200_quant_dual.so)
+def quant_dual_lib() -> ctypes.CDLL:
+    """libb200_quant_dual.so: x and x^T quantised rowwise to e4m3 from one tensor (csrc/b200_quant_dual.h, no public
+    ABI)."""
+    return load(QUANT_DUAL_LIB)
+
+
+def dual_ld_t(rows: int) -> int:
+    """The row length of the transposed e4m3 copy of an x with ``rows`` rows: rows rounded up to 16, so that it is a
+    K-major FP8 GEMM operand (K % 16 == 0)."""
+    return -(-rows // 16) * 16
+
+
+def quant_dual_workspace(rows: int, cols: int) -> int:
+    """Floats of the workspace of :func:`quantize_e4m3_rowwise_dual` (CUDA_L2_B200_QUANT_DUAL_WORKSPACE)."""
+    return rows + cols
+
+
+def quantize_e4m3_rowwise_dual(x, q, scale, q_t, scale_t, workspace, stream: int | None = None) -> None:
+    """Both rowwise quantisations of a 2-D ``x`` [rows, cols] (fp16, bf16 or fp32, contiguous): ``q`` (e4m3
+    [rows, cols]) with ``scale`` (fp32 [rows]), and ``q_t`` (e4m3 [cols, dual_ld_t(rows)], x^T zero-padded) with
+    ``scale_t`` (fp32 [cols]), in one memset and two launches; ``workspace``: quant_dual_workspace(rows, cols) fp32
+    elements of device memory that no other call uses until this one has run (csrc/b200_quant_dual.h)."""
+    code = _quant_input(x)
+    if x.dim() != 2:
+        raise B200HgemmError(f"the dual rowwise quantiser takes a 2-D [rows, cols] tensor, got {list(x.shape)}")
+    rows, cols = x.shape
+    _quant_output(q, x.shape, x)
+    _quant_output(q_t, (cols, dual_ld_t(rows)), x)
+    _fp32_on(scale, x, "scale", (rows,))
+    _fp32_on(scale_t, x, "scale_t", (cols,))
+    _fp32_on(workspace, x, "workspace", (quant_dual_workspace(rows, cols),))
+    _contiguous_cuda(scale=scale, scale_t=scale_t, workspace=workspace)
+    st = quant_dual_lib().cuda_l2_b200_quant_dual_e4m3_rowwise(code, x.data_ptr(), rows, cols, q.data_ptr(),
+                                                               scale.data_ptr(), q_t.data_ptr(), scale_t.data_ptr(),
+                                                               workspace.data_ptr(), stream)
+    if st != 0:
+        raise B200HgemmError(f"cuda_l2_b200_quant_dual_e4m3_rowwise failed: status {st} "
+                             f"({quant_dual_lib().cuda_l2_b200_quant_dual_strerror(st).decode()})")
+
+
+def quant_dual_launch_count() -> int:
+    return int(quant_dual_lib().cuda_l2_b200_quant_dual_launch_count())

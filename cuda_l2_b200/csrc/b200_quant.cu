@@ -1,7 +1,9 @@
 // libb200_quant.so — the one-pass e4m3 quantisers of FP8 activations (b200_quant.h). Memory-bound kernels:
 // every element is loaded once into registers, its group's amax is reduced on chip, and the quantised bytes are stored
-// from the same registers. A library of its own, so that the device code of the GEMM libraries stays as it is.
+// from the same registers. A library of its own, so that the device code of the GEMM libraries stays as it is. The
+// element arithmetic is in b200_quant_arith.cuh, shared with libb200_quant_dual.so.
 #include "b200_quant.h"
+#include "b200_quant_arith.cuh"
 
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -24,78 +26,9 @@ enum Status : int {
   kBadScaleLd = -10,
 };
 
-constexpr float kE4M3Max = 448.0f;
-// torch's CUDA `tensor / 448.0` multiplies by the fp32 reciprocal of the scalar (see b200_quant.h)
-constexpr float kInvE4M3Max = 1.0f / 448.0f;
 constexpr int kBlock = 128;   // the 1 x 128 scale block
 
-// ------------------------------------------------------------------------------------------------ element arithmetic
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
-__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
-__device__ __forceinline__ float to_f32(float v) { return v; }
-
-// max that keeps a NaN once it has seen one (torch.amax), unlike fmaxf
-__device__ __forceinline__ float nan_max(float m, float a) { return (a > m || a != a) ? a : m; }
-
-__device__ __forceinline__ float scale_of(float amax) {
-  const float s = amax * kInvE4M3Max;
-  return s < FLT_MIN ? FLT_MIN : s;   // clamp_min(FLT_MIN); NaN stays NaN
-}
-
-// clamp(x / s, -448, 448) with an IEEE division; a NaN quotient passes the clamp unchanged
-__device__ __forceinline__ float quotient(float x, float s) {
-  const float v = __fdiv_rn(x, s);
-  return v != v ? v : fminf(fmaxf(v, -kE4M3Max), kE4M3Max);
-}
-
-// e4m3fn bytes of two clamped quotients, lo in bits 0-7: round to nearest even; NaN is 0x7f with the input's sign
-__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
-  unsigned short r;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-  uint32_t out = r;
-  if (lo != lo) out = (out & 0xff00u) | 0x7fu | ((__float_as_uint(lo) >> 24) & 0x80u);
-  if (hi != hi) out = (out & 0x00ffu) | ((0x7fu | ((__float_as_uint(hi) >> 24) & 0x80u)) << 8);
-  return out;
-}
-
-__device__ __forceinline__ uint8_t e4m3(float v) { return uint8_t(e4m3x2(v, 0.0f)); }
-
-// EPL consecutive elements from p, as fp32: one 16-byte load when kVec, EPL element loads otherwise (only the first
-// `valid` of them are read; the rest are 0)
-template <typename T, int EPL, bool kVec>
-__device__ __forceinline__ void load_f32(const T* p, int valid, float (&v)[EPL]) {
-  if constexpr (kVec) {
-    static_assert(EPL * sizeof(T) == 16, "one 16-byte vector");
-    const uint4 raw = __ldg(reinterpret_cast<const uint4*>(p));
-    const T* e = reinterpret_cast<const T*>(&raw);
-#pragma unroll
-    for (int j = 0; j < EPL; ++j) v[j] = to_f32(e[j]);
-  } else {
-#pragma unroll
-    for (int j = 0; j < EPL; ++j) v[j] = j < valid ? to_f32(p[j]) : 0.0f;
-  }
-}
-
-// EPL quantised bytes to q: one 4- or 8-byte store when kVec, byte stores of the first `valid` otherwise
-template <int EPL, bool kVec>
-__device__ __forceinline__ void store_e4m3(uint8_t* q, int valid, const float (&v)[EPL], float s) {
-  if constexpr (kVec) {
-    uint32_t w[EPL / 4];
-#pragma unroll
-    for (int j = 0; j < EPL / 4; ++j)
-      w[j] = e4m3x2(quotient(v[4 * j], s), quotient(v[4 * j + 1], s)) |
-             (e4m3x2(quotient(v[4 * j + 2], s), quotient(v[4 * j + 3], s)) << 16);
-    if constexpr (EPL == 8)
-      *reinterpret_cast<uint2*>(q) = make_uint2(w[0], w[1]);
-    else
-      *reinterpret_cast<uint32_t*>(q) = w[0];
-  } else {
-#pragma unroll
-    for (int j = 0; j < EPL; ++j)
-      if (j < valid) q[j] = e4m3(quotient(v[j], s));
-  }
-}
-
+// ------------------------------------------------------------------------------------------------ SwiGLU
 // the SwiGLU product p = RN(fp32(RN(silu(g))) * fp32(u)) of torch's `F.silu(g) * u` on 16-bit tensors
 __device__ __forceinline__ float round_to(float v, __half) { return __half2float(__float2half_rn(v)); }
 __device__ __forceinline__ float round_to(float v, __nv_bfloat16) { return __bfloat162float(__float2bfloat16_rn(v)); }
@@ -104,24 +37,6 @@ template <typename T>
 __device__ __forceinline__ float silu_mul(float g, float u) {
   const float s = round_to(__fdiv_rn(g, 1.0f + expf(-g)), T());
   return round_to(s * u, T());
-}
-
-template <int LANES>
-__device__ __forceinline__ float group_amax(float m) {   // over aligned groups of LANES lanes
-#pragma unroll
-  for (int off = LANES / 2; off > 0; off /= 2) m = nan_max(m, __shfl_xor_sync(0xffffffffu, m, off));
-  return m;
-}
-
-// every thread gets the CTA's amax; red holds a float per warp of the CTA (blockDim.x a multiple of 32)
-__device__ __forceinline__ float cta_amax(float m, float* red) {
-  m = group_amax<32>(m);
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  __syncthreads();   // red may still be read from an earlier call
-  if (lane == 0) red[warp] = m;
-  __syncthreads();
-  m = lane < int(blockDim.x / 32) ? red[lane] : 0.0f;
-  return group_amax<32>(m);
 }
 
 // ------------------------------------------------------------------------------------------------ 1 x 128 blocks

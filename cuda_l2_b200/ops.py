@@ -67,12 +67,18 @@ the nearest grid shape — so deployment is a plain operator:
   tensors to them. Inference only.
 * :class:`B200Fp8GroupedMLP`: the routed experts of an FP8 MoE checkpoint as a gated MLP, four launches per forward
   (quantise, gate/up GEMM, SwiGLU + quantise, down GEMM), in the prefill or the decode layout.
+* ``torch.ops.cuda_l2_b200.quantize_e4m3_rowwise_dual(x)``: ``(q, scale, q_t, scale_t)``, the rowwise quantisation of
+  ``x`` [rows, cols] and of ``x^T`` zero-padded to a multiple of 16 columns, from one tensor (libb200_quant_dual.so,
+  csrc/b200_quant_dual.h): the two K-major e4m3 operands FP8 training needs of each tensor. Inference only itself.
+* :func:`fp8_linear` and :class:`B200Fp8TrainLinear`: ``x @ W^T`` trained in FP8, a rowwise-scaled e4m3 forward and
+  backward (three ``fp8_gemm`` calls per step) over a trainable 16-bit weight.
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernels, so a fine-tuning
 loop works: ``hgemm``'s input gradient reads the weight in place through the row-major B kernels, and its weight
 gradient pays one transposed copy (of the output gradient). The grouped product trains through :func:`grouped_linear`
 (``hgemm_grouped`` itself stays inference only). The FP8 operators have no gradient: a backward through them raises.
+FP8 training goes through :func:`fp8_linear`, whose own backward runs those operators.
 """
 from __future__ import annotations
 
@@ -1035,6 +1041,179 @@ class B200Fp8Linear(nn.Module):
                 f"out_dtype={self.out_dtype}, granularity={self.granularity}")
 
 
+# ------------------------------------------------------------------------------------------ FP8 training of linear layers
+#                                                                                            (libb200_quant_dual.so)
+# e4m3 wgmma reads K-major operands only, so the input gradient dX = dY W and the weight gradient dW = dY^T X need W,
+# dY and X transposed, each quantised along its other axis. The dual quantiser writes both orientations of a tensor
+# from one read of it; every GEMM of the step is then fp8_gemm with rowwise scales.
+def quantize_e4m3_rowwise_dual_reference(x: torch.Tensor
+                                         ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """:func:`quantize_e4m3_rowwise_dual` as a composition of torch ops: the rowwise quantisation of ``x`` and of
+    ``x^T`` zero-padded to a multiple of 16 columns, with the scales as vectors."""
+    if x.dim() != 2:
+        raise capi.B200HgemmError(f"quantize_e4m3_rowwise_dual takes [rows, cols], got {list(x.shape)}")
+    rows, cols = x.shape
+    q, scale = quantize_e4m3_rowwise_reference(x)
+    q_t, scale_t = quantize_e4m3_rowwise_reference(
+        nn.functional.pad(x.t(), (0, capi.dual_ld_t(rows) - rows)).contiguous())
+    return q, scale.reshape(rows), q_t, scale_t.reshape(cols)
+
+
+def _quantize_e4m3_rowwise_dual_outputs(x):
+    _quant_input(x)
+    if x.dim() != 2:
+        raise capi.B200HgemmError(f"quantize_e4m3_rowwise_dual takes [rows, cols], got {list(x.shape)}")
+    rows, cols = x.shape
+    return (x.new_empty((rows, cols), dtype=torch.float8_e4m3fn), x.new_empty((rows,), dtype=torch.float32),
+            x.new_empty((cols, capi.dual_ld_t(rows)), dtype=torch.float8_e4m3fn),
+            x.new_empty((cols,), dtype=torch.float32))
+
+
+def _quantize_e4m3_rowwise_dual_launch(out, x, *, stream):
+    workspace = torch.empty(capi.quant_dual_workspace(*x.shape), dtype=torch.float32, device=x.device)
+    capi.quantize_e4m3_rowwise_dual(x.contiguous(), *out, workspace, stream=stream)
+
+
+_inference_op("quantize_e4m3_rowwise_dual", "(Tensor x) -> (Tensor, Tensor, Tensor, Tensor)", None,
+              _quantize_e4m3_rowwise_dual_launch, _QUANT_WHY, outputs=_quantize_e4m3_rowwise_dual_outputs)
+
+
+def quantize_e4m3_rowwise_dual(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Both rowwise quantisations of a 2-D ``x`` [rows, cols] on its device: ``(q, scale, q_t, scale_t)``, where
+    ``q`` [rows, cols] and ``scale`` [rows] are :func:`quantize_e4m3_rowwise`'s (the scale as a vector), and ``q_t``
+    [cols, ld_t] and ``scale_t`` [cols] are the same for ``x^T`` zero-padded to ``ld_t`` = rows rounded up to 16
+    columns: a K-major FP8 GEMM operand whose reduction runs along x's rows. A padding byte is e4m3(0 / scale_t), 0x00
+    unless the column's scale is NaN. No host synchronisation. A non-empty 2-D CUDA fp16 / bf16 / fp32 tensor runs
+    ``cuda_l2_b200::quantize_e4m3_rowwise_dual`` (a memset and two launches, x read twice), anything else
+    :func:`quantize_e4m3_rowwise_dual_reference`, with the same bits."""
+    if x.dim() == 2 and _quant_routed(x):
+        return torch.ops.cuda_l2_b200.quantize_e4m3_rowwise_dual(x)
+    return quantize_e4m3_rowwise_dual_reference(x)
+
+
+def _check_fp8_linear(in_features: int, out_features: int, dtype: torch.dtype, what) -> None:
+    """The rules of :func:`fp8_linear`'s three GEMMs: fp16 / bf16, and in_features and out_features multiples of 16
+    (each is the reduction of one of them, and e4m3 rows must be 16 bytes)."""
+    if dtype not in (torch.float16, torch.bfloat16) or in_features % 16 or out_features % 16:
+        raise capi.B200HgemmError(f"FP8 training of {what} needs fp16 / bf16 and in_features % 16 == 0, "
+                                  f"out_features % 16 == 0, got {in_features}->{out_features} {dtype}")
+
+
+def _rowwise_gemm(a, a_scale, b_kmajor, b_scale, out_dtype):
+    """fp8_gemm with rowwise scales given as vectors: a_scale [M], b_scale [N]."""
+    return torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, a_scale.reshape(-1, 1), b_scale.reshape(1, -1), out_dtype)
+
+
+class _Fp8LinearFunction(torch.autograd.Function):
+    """y = x W^T with a gradient, every product an e4m3 rowwise-scaled fp8_gemm. The forward saves the transposed e4m3
+    copies its backward reads, not x and W, and only those of the gradients that will be asked for."""
+
+    @staticmethod
+    def forward(ctx, x2, weight):
+        need_x, need_w = ctx.needs_input_grad[:2]
+        ctx.shapes = (x2.shape, weight.shape)
+        ctx.dtypes = (x2.dtype, weight.dtype)
+        if x2.shape[0] == 0:
+            ctx.save_for_backward()
+            return x2.new_empty((0, weight.shape[0]))
+        # dW = q(dY^T) q(X^T)^T needs X transposed; dX = q(dY) q(W^T)^T needs W transposed
+        if need_w:
+            x_q, x_s, x_qt, x_st = quantize_e4m3_rowwise_dual(x2)
+        else:
+            x_q, x_s = quantize_e4m3_rowwise(x2)
+            x_qt = x_st = None
+        if need_x:
+            w_q, w_s, w_qt, w_st = quantize_e4m3_rowwise_dual(weight)
+        else:
+            w_q, w_s = quantize_e4m3_rowwise(weight)
+            w_qt = w_st = None
+        ctx.save_for_backward(x_qt, x_st, w_qt, w_st)
+        return _rowwise_gemm(x_q, x_s, w_q, w_s, x2.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        (x_shape, w_shape), (x_dtype, w_dtype) = ctx.shapes, ctx.dtypes
+        need_x, need_w = ctx.needs_input_grad[:2]
+        grad_x = grad_w = None
+        if x_shape[0] == 0:
+            if need_x:
+                grad_x = grad_y.new_empty(x_shape, dtype=x_dtype)
+            if need_w:
+                grad_w = grad_y.new_zeros(w_shape, dtype=w_dtype)
+            return grad_x, grad_w
+        x_qt, x_st, w_qt, w_st = ctx.saved_tensors
+        g = grad_y.contiguous()
+        if need_w:
+            g_q, g_s, g_qt, g_st = quantize_e4m3_rowwise_dual(g)
+            grad_w = _rowwise_gemm(g_qt, g_st, x_qt, x_st, w_dtype)       # [N, ld_t(M)] x [K, ld_t(M)] -> [N, K]
+        else:
+            g_q, g_s = quantize_e4m3_rowwise(g)
+        if need_x:
+            grad_x = _rowwise_gemm(g_q, g_s, w_qt, w_st, x_dtype)         # [M, N] x [K, N] -> [M, K]
+        return grad_x, grad_w
+
+
+def fp8_linear(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """``x @ weight^T`` for ``x`` [..., K] and ``weight`` [N, K] of one dtype (fp16 or bf16), K % 16 == 0 and
+    N % 16 == 0, in FP8 with a gradient: x and W are quantised to e4m3 with one fp32 scale per row (per token, per
+    output channel) and multiplied by ``fp8_gemm`` into x's dtype. The backward quantises dY the same way and runs two
+    more ``fp8_gemm`` calls, dX = dY W (scales per token and per input channel) and dW = dY^T X (both operands scaled
+    along the tokens), from the transposed e4m3 copies of W and x that the forward kept. Every product accumulates in
+    the FP8 tensor cores' fast mode. Without a gradient to compute, the forward is ``B200Fp8Linear``'s rowwise one, bit
+    for bit. No host synchronisation: a forward and backward can be captured in one CUDA graph."""
+    if x.dim() == 0 or weight.dim() != 2 or x.shape[-1] != weight.shape[1] or x.dtype != weight.dtype:
+        raise capi.B200HgemmError(f"fp8_linear: x [..., K] and weight [N, K] of one dtype expected, got "
+                                  f"{x.dtype} {tuple(x.shape)} and {weight.dtype} {tuple(weight.shape)}")
+    n, k = weight.shape
+    _check_fp8_linear(k, n, weight.dtype, f"a [{n}, {k}] weight")
+    x2 = x.reshape(-1, k)
+    if torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad):
+        y = _Fp8LinearFunction.apply(x2, weight)
+    elif x2.shape[0] == 0:
+        y = x2.new_empty((0, n))
+    else:
+        (x_q, x_s), (w_q, w_s) = quantize_e4m3_rowwise(x2), quantize_e4m3_rowwise(weight)
+        y = torch.ops.cuda_l2_b200.fp8_gemm(x_q, w_q, x_s, w_s.reshape(1, n), x.dtype)
+    return y.view(*x.shape[:-1], n)
+
+
+class B200Fp8TrainLinear(nn.Module):
+    """``nn.Linear`` trained in FP8: a trainable 16-bit ``weight`` [out_features, in_features] (and optional ``bias``),
+    the product run by :func:`fp8_linear` (rowwise-scaled e4m3 forward and backward), the bias added by torch after it
+    as :class:`B200Linear` does. In eval or no-grad mode the output is :class:`B200Fp8Linear`'s rowwise one, bit for
+    bit. Needs fp16 / bf16 and in_features % 16 == 0, out_features % 16 == 0."""
+
+    def __init__(self, in_features: int, out_features: int, bias: bool = True, device=None,
+                 dtype: torch.dtype = torch.bfloat16):
+        super().__init__()
+        _check_fp8_linear(in_features, out_features, dtype, "B200Fp8TrainLinear")
+        self.in_features, self.out_features = in_features, out_features
+        self.weight = nn.Parameter(torch.empty((out_features, in_features), device=device, dtype=dtype))
+        self.bias = nn.Parameter(torch.empty(out_features, device=device, dtype=dtype)) if bias else None
+        self.reset_parameters()
+
+    reset_parameters = B200Linear.reset_parameters
+
+    @classmethod
+    def from_linear(cls, lin: nn.Linear) -> "B200Fp8TrainLinear":
+        """A layer sharing ``lin``'s Parameters (no copy), as :meth:`B200Linear.from_linear`."""
+        _check_fp8_linear(lin.in_features, lin.out_features, lin.weight.dtype, lin)
+        new = cls.__new__(cls)
+        nn.Module.__init__(new)
+        new.in_features, new.out_features = lin.in_features, lin.out_features
+        new.weight, new.bias = lin.weight, lin.bias          # shared storage, no copy
+        return new
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        y = fp8_linear(x, self.weight)
+        if self.bias is not None:
+            y = y + self.bias
+        return y
+
+    def extra_repr(self) -> str:
+        return f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}"
+
+
 # ------------------------------------------------------------------------------------------ grouped FP8 (libb200_grouped_fp8.so)
 def _fp8_grouped_shape(a, b_kmajor, scale_a, scale_b, offs, out_dtype):
     _, t, n, _ = capi.check_grouped_operands(a, b_kmajor, offs, "fp32", out_dtype, (scale_a, scale_b))
@@ -1237,4 +1416,4 @@ __all__ = ["hgemm", "hgemm_nn", "hgemm_batched", "hgemm_grouped", "hgemm_grouped
            "grouped_linear", "B200GroupedLinear", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear",
            "fp8_grouped_gemm", "fp8_batched_gemm", "B200Fp8GroupedLinear", "silu_mul_quantize_e4m3_blockwise",
-           "B200Fp8GroupedMLP"]
+           "B200Fp8GroupedMLP", "quantize_e4m3_rowwise_dual", "fp8_linear", "B200Fp8TrainLinear"]
