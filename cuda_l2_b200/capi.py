@@ -142,6 +142,8 @@ INTERNAL_ABI = {
         "cuda_l2_b200_quant_dual_strerror": ([_i], ctypes.c_char_p),
     },
 }
+_TABLES = {**ABI, **INTERNAL_ABI}
+_LIBRARY_OF = {symbol: name for name, table in _TABLES.items() for symbol in table}   # entry point -> its library
 _libs: dict = {}
 
 
@@ -155,7 +157,7 @@ def load(name: str) -> ctypes.CDLL:
                 f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(or `python cuda_l2_b200/build.py`). There is no fallback path.")
         lib = ctypes.CDLL(str(path))
-        for sym, (args, res) in (ABI[name] if name in ABI else INTERNAL_ABI[name]).items():
+        for sym, (args, res) in _TABLES[name].items():
             fn = getattr(lib, sym)
             fn.argtypes, fn.restype = args, res
         _libs[name] = lib
@@ -208,9 +210,14 @@ def strerror(status: int) -> str:
     return hgemm_lib().b200_hgemm_strerror(status).decode()
 
 
-def _check(status: int, what: str) -> None:
+def _check(status: int, fn) -> None:
+    """B200HgemmError unless ``status``, what the entry point ``fn`` (a loaded function or its symbol) returned, is 0.
+    The message decodes the status with the strerror of the library that exports ``fn``, which knows its own codes."""
     if status != 0:
-        raise B200HgemmError(f"{what} failed: status {status} ({strerror(status)})")
+        symbol = fn if isinstance(fn, str) else fn.__name__
+        name = _LIBRARY_OF[symbol]
+        text = getattr(load(name), next(s for s in _TABLES[name] if s.endswith("_strerror")))(status).decode()
+        raise B200HgemmError(f"{symbol} failed: status {status} ({text})")
 
 
 def _shape_check(a, b_col_major, c):
@@ -237,7 +244,7 @@ def hgemm(a, b_col_major, c, acc: str | int = "fp32", stream: int | None = None)
     m, n, k = _shape_check(a, b_col_major, c)
     bits = ACC_BITS[acc]
     fn = hgemm_lib().b200_hgemm_f32acc if bits == 32 else hgemm_lib().b200_hgemm_f16acc
-    _check(fn(a.data_ptr(), None, b_col_major.data_ptr(), c.data_ptr(), m, n, k, stream), "b200_hgemm")
+    _check(fn(a.data_ptr(), None, b_col_major.data_ptr(), c.data_ptr(), m, n, k, stream), fn)
 
 
 class GemmType(NamedTuple):
@@ -407,19 +414,18 @@ def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = No
     m, n, k = _kmajor_operands(a, b_kmajor, c, acc)
     lib = hgemm_lib()
     bits = ACC_BITS[acc]
-    if a.dtype == torch.bfloat16:
-        if config_id is None:
-            st = lib.b200_bgemm_f32acc(a.data_ptr(), None, b_kmajor.data_ptr(), c.data_ptr(), m, n, k, stream)
-        else:
-            st = lib.b200_bgemm_run_config(config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m,
-                                           max_ctas, splits, stream)
-    elif config_id is None:
-        fn = lib.b200_hgemm_f32acc if bits == 32 else lib.b200_hgemm_f16acc
+    if config_id is None:
+        fn = (lib.b200_bgemm_f32acc if a.dtype == torch.bfloat16 else
+              lib.b200_hgemm_f32acc if bits == 32 else lib.b200_hgemm_f16acc)
         st = fn(a.data_ptr(), None, b_kmajor.data_ptr(), c.data_ptr(), m, n, k, stream)
+    elif a.dtype == torch.bfloat16:
+        fn = lib.b200_bgemm_run_config
+        st = fn(config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m, max_ctas, splits, stream)
     else:
-        st = lib.b200_hgemm_run_config(bits, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m,
-                                       max_ctas, splits, stream)
-    _check(st, "b200 gemm")
+        fn = lib.b200_hgemm_run_config
+        st = fn(bits, config_id, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), m, n, k, group_m, max_ctas, splits,
+                stream)
+    _check(st, fn)
 
 
 def check_rowmajor_operands(a, b, out_dtype=None, acc: str | int = "fp32") -> tuple[int, int, int]:
@@ -456,7 +462,7 @@ def gemm_rowmajor(a, b, c, acc: str | int = "fp32", stream: int | None = None) -
         fn = lib.b200_bgemm_f32acc
     else:
         fn = lib.b200_hgemm_f32acc if ACC_BITS[acc] == 32 else lib.b200_hgemm_f16acc
-    _check(fn(a.data_ptr(), b.data_ptr(), None, c.data_ptr(), m, n, k, stream), "b200 gemm (row-major B)")
+    _check(fn(a.data_ptr(), b.data_ptr(), None, c.data_ptr(), m, n, k, stream), fn)
 
 
 def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config_id: int | None = None,
@@ -477,14 +483,14 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
         ld_a = _scale_ld_a(scale_a)
         blk = fp8block_lib()
         if config_id is None:
-            st = blk.b200_fp8gemm_blockwise(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a,
-                                            scale_b.data_ptr(), out_bf16, m, n, k, stream)
+            fn = blk.b200_fp8gemm_blockwise
+            st = fn(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr(),
+                    out_bf16, m, n, k, stream)
         else:
-            st = blk.b200_fp8gemm_blockwise_run_config(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(),
-                                                       c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr(), m, n,
-                                                       k, group_m, max_ctas, splits, stream)
-        if st != 0:
-            raise B200HgemmError(f"b200_fp8gemm_blockwise failed: status {st} ({blk.b200_fp8block_strerror(st).decode()})")
+            fn = blk.b200_fp8gemm_blockwise_run_config
+            st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a,
+                    scale_b.data_ptr(), m, n, k, group_m, max_ctas, splits, stream)
+        _check(st, fn)
         return
     if not scale_a.is_contiguous():
         raise B200HgemmError("scale_a must be a contiguous CUDA tensor")
@@ -498,14 +504,14 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
         fn = lib.b200_fp8gemm_rowwise_run_config if rowwise else lib.b200_fp8gemm_run_config
         st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(),
                 scale_b.data_ptr(), m, n, k, group_m, max_ctas, splits, stream)
-    _check(st, "b200_fp8gemm_rowwise" if rowwise else "b200_fp8gemm")
+    _check(st, fn)
 
 
 def _select(fn, *args) -> tuple[int, ...]:
     """A *_select entry point's answer: ``fn`` called with ``args``, then one int out-parameter for each of its
     remaining arguments, whose values it returns. B200HgemmError on a non-zero status."""
     outs = [ctypes.c_int() for _ in fn.argtypes[len(args):]]
-    _check(fn(*args, *map(ctypes.byref, outs)), fn.__name__)
+    _check(fn(*args, *map(ctypes.byref, outs)), fn)
     return tuple(v.value for v in outs)
 
 
@@ -529,9 +535,7 @@ def _tile_list_schedule(schedule_units, ints: int, *args) -> dict:
     nw = ctypes.c_int()
     cap = 256
     buf = (ctypes.c_int * (ints * cap))()
-    st = schedule_units(*args, 0, buf, cap, ctypes.byref(nw))
-    if st < 0:
-        raise B200HgemmError(f"{schedule_units.__name__} failed: status {st}")
+    _check(min(schedule_units(*args, 0, buf, cap, ctypes.byref(nw)), 0), schedule_units)
     units = []
     for w in range(nw.value):
         cnt = schedule_units(*args, w, buf, cap, None)
@@ -574,13 +578,13 @@ def _tile_list_gemm(kind: str, a, b_kmajor, c, lst, acc: str | int, scales: tupl
     problem = (None if lst is None else lst.data_ptr(), count, rows, n, k)
     if config_id is None:
         args = (*ptrs, selector) if scales else (selector, *ptrs)
-        st = getattr(lib, f"b200_{prefix}_gemm")(*args, *problem, stream)
+        fn = getattr(lib, f"b200_{prefix}_gemm")
+        st = fn(*args, *problem, stream)
     else:
         head = (config_id, selector) if scales else (selector, config_id)
-        st = getattr(lib, f"b200_{prefix}_gemm_run_config")(*head, *ptrs, *problem, group_m, max_ctas, stream)
-    if st != 0:
-        raise B200HgemmError(f"b200_{prefix}_gemm failed: status {st} "
-                             f"({getattr(lib, f'b200_{prefix}_strerror')(st).decode()})")
+        fn = getattr(lib, f"b200_{prefix}_gemm_run_config")
+        st = fn(*head, *ptrs, *problem, group_m, max_ctas, stream)
+    _check(st, fn)
 
 
 # ------------------------------------------------------------------------------------------ batched (libb200_batched.so)
@@ -770,11 +774,8 @@ def check_grouped_wgrad_operands(a, b, offs, acc: str | int = "fp32") -> tuple[i
 
 def _bwd_call(symbol: str, variant: int, ptrs: tuple, problem: tuple, config_id: int | None, group_m: int,
               max_ctas: int, stream: int | None) -> None:
-    lib = grouped_bwd_lib()
-    st = getattr(lib, symbol)(variant, -1 if config_id is None else config_id, *ptrs, *problem, group_m, max_ctas,
-                              stream)
-    if st != 0:
-        raise B200HgemmError(f"{symbol} failed: status {st} ({lib.cuda_l2_b200_grouped_bwd_strerror(st).decode()})")
+    _check(getattr(grouped_bwd_lib(), symbol)(variant, -1 if config_id is None else config_id, *ptrs, *problem, group_m,
+                                              max_ctas, stream), symbol)
 
 
 def gemm_grouped_nn(a, b, c, offs, acc: str | int = "fp32", config_id: int | None = None, group_m: int = 0,
@@ -1124,10 +1125,12 @@ def gemm_bias_act(a, b_kmajor, c, bias=None, activation: str = "none", scale_a=N
             scale_b.data_ptr() if scales else None, rowwise, None if bias is None else bias.data_ptr(), act, m, n, k)
     lib = epilogue_lib()
     if config_id is None:
-        st = lib.cuda_l2_b200_epilogue_run(variant, *args, stream)
+        fn = lib.cuda_l2_b200_epilogue_run
+        st = fn(variant, *args, stream)
     else:
-        st = lib.cuda_l2_b200_epilogue_run_config(variant, config_id, *args, group_m, max_ctas, splits, stream)
-    _epilogue_check(st, "cuda_l2_b200_epilogue")
+        fn = lib.cuda_l2_b200_epilogue_run_config
+        st = fn(variant, config_id, *args, group_m, max_ctas, splits, stream)
+    _check(st, fn)
 
 
 def epilogue_select(variant: int, m: int, n: int, k: int) -> tuple[int, int, int]:
@@ -1135,20 +1138,15 @@ def epilogue_select(variant: int, m: int, n: int, k: int) -> tuple[int, int, int
     return _select(epilogue_lib().cuda_l2_b200_epilogue_select, variant, m, n, k)
 
 
-def _epilogue_check(st: int, what: str) -> None:
-    if st != 0:
-        raise B200HgemmError(f"{what} failed: status {st} ({epilogue_lib().cuda_l2_b200_epilogue_strerror(st).decode()})")
-
-
 def epilogue_prewarm(stream: int | None = None) -> None:
     """Allocate libb200_epilogue.so's split-K scratch for ``stream`` ahead of a CUDA-graph capture (a first split-K or
     stream-K call inside a capture runs undivided without it)."""
-    _epilogue_check(epilogue_lib().cuda_l2_b200_epilogue_prewarm(stream), "cuda_l2_b200_epilogue_prewarm")
+    _check(epilogue_lib().cuda_l2_b200_epilogue_prewarm(stream), "cuda_l2_b200_epilogue_prewarm")
 
 
 def epilogue_release() -> None:
     """Free libb200_epilogue.so's split-K scratch (no launch of it may be in flight)."""
-    _epilogue_check(epilogue_lib().cuda_l2_b200_epilogue_release(), "cuda_l2_b200_epilogue_release")
+    _check(epilogue_lib().cuda_l2_b200_epilogue_release(), "cuda_l2_b200_epilogue_release")
 
 
 def epilogue_launch_count() -> int:
@@ -1173,11 +1171,6 @@ def quant_dtype(dtype, silu_mul: bool = False) -> int | None:
     codes = {torch.float16: 0, torch.bfloat16: 1} if silu_mul else {torch.float16: 0, torch.bfloat16: 1,
                                                                      torch.float32: 2}
     return codes.get(dtype)
-
-
-def _quant_check(st: int, what: str) -> None:
-    if st != 0:
-        raise B200HgemmError(f"{what} failed: status {st} ({quant_lib().cuda_l2_b200_quant_strerror(st).decode()})")
 
 
 def _quant_input(x, silu_mul: bool = False) -> int:
@@ -1215,9 +1208,8 @@ def quantize_e4m3(x, q, scale, workspace, stream: int | None = None) -> None:
     _fp32_on(scale, x, "scale", (1,))
     _fp32_on(workspace, x, "workspace", (QUANT_TENSOR_WORKSPACE,))
     _contiguous_cuda(workspace=workspace)
-    _quant_check(quant_lib().cuda_l2_b200_quant_e4m3_tensor(code, x.data_ptr(), x.numel(), q.data_ptr(),
-                                                            scale.data_ptr(), workspace.data_ptr(), stream),
-                 "cuda_l2_b200_quant_e4m3_tensor")
+    _check(quant_lib().cuda_l2_b200_quant_e4m3_tensor(code, x.data_ptr(), x.numel(), q.data_ptr(), scale.data_ptr(),
+                                                      workspace.data_ptr(), stream), "cuda_l2_b200_quant_e4m3_tensor")
 
 
 def quantize_e4m3_rowwise(x, q, scale, stream: int | None = None) -> None:
@@ -1230,9 +1222,8 @@ def quantize_e4m3_rowwise(x, q, scale, stream: int | None = None) -> None:
     _quant_output(q, x.shape, x)
     _fp32_on(scale, x, "scale", (rows, 1))
     _contiguous_cuda(scale=scale)
-    _quant_check(quant_lib().cuda_l2_b200_quant_e4m3_rowwise(code, x.data_ptr(), rows, cols, q.data_ptr(),
-                                                             scale.data_ptr(), stream),
-                 "cuda_l2_b200_quant_e4m3_rowwise")
+    _check(quant_lib().cuda_l2_b200_quant_e4m3_rowwise(code, x.data_ptr(), rows, cols, q.data_ptr(), scale.data_ptr(),
+                                                       stream), "cuda_l2_b200_quant_e4m3_rowwise")
 
 
 def _blockwise_call(symbol: str, x, q, scale, masked_m, k: int, silu_mul: bool, stream) -> None:
@@ -1253,8 +1244,8 @@ def _blockwise_call(symbol: str, x, q, scale, masked_m, k: int, silu_mul: bool, 
         if masked_m.dtype != torch.int32 or tuple(masked_m.shape) != (bsz,) or masked_m.device != x.device:
             raise B200HgemmError(f"masked_m must be an int32 tensor of shape [{bsz}] on {x.device}, got "
                                  f"{masked_m.dtype} {tuple(masked_m.shape)} on {masked_m.device}")
-    _quant_check(getattr(quant_lib(), symbol)(code, x.data_ptr(), bsz, m, k, q.data_ptr(), scale.data_ptr(), ld_a,
-                                              None if masked_m is None else masked_m.data_ptr(), stream), symbol)
+    _check(getattr(quant_lib(), symbol)(code, x.data_ptr(), bsz, m, k, q.data_ptr(), scale.data_ptr(), ld_a,
+                                        None if masked_m is None else masked_m.data_ptr(), stream), symbol)
 
 
 def quantize_e4m3_blockwise(x, q, scale, masked_m=None, stream: int | None = None) -> None:
@@ -1313,12 +1304,9 @@ def quantize_e4m3_rowwise_dual(x, q, scale, q_t, scale_t, workspace, stream: int
     _fp32_on(scale_t, x, "scale_t", (cols,))
     _fp32_on(workspace, x, "workspace", (quant_dual_workspace(rows, cols),))
     _contiguous_cuda(scale=scale, scale_t=scale_t, workspace=workspace)
-    st = quant_dual_lib().cuda_l2_b200_quant_dual_e4m3_rowwise(code, x.data_ptr(), rows, cols, q.data_ptr(),
-                                                               scale.data_ptr(), q_t.data_ptr(), scale_t.data_ptr(),
-                                                               workspace.data_ptr(), stream)
-    if st != 0:
-        raise B200HgemmError(f"cuda_l2_b200_quant_dual_e4m3_rowwise failed: status {st} "
-                             f"({quant_dual_lib().cuda_l2_b200_quant_dual_strerror(st).decode()})")
+    fn = quant_dual_lib().cuda_l2_b200_quant_dual_e4m3_rowwise
+    _check(fn(code, x.data_ptr(), rows, cols, q.data_ptr(), scale.data_ptr(), q_t.data_ptr(), scale_t.data_ptr(),
+              workspace.data_ptr(), stream), fn)
 
 
 def quant_dual_launch_count() -> int:

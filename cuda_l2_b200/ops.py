@@ -90,16 +90,18 @@ from . import capi
 _LIB = "cuda_l2_b200"
 
 
-def _inference_op(name: str, schema: str, shape, launch, why: str = "", outputs=None) -> None:
-    """Defines the inference-only operator cuda_l2_b200::<name> with ``schema``. ``shape(*args)`` checks the arguments
-    by the kernel's rules (meta tensors pass) and returns the result's shape and dtype: the fake implementation is an
-    empty tensor of those, and the CUDA one allocates the result ``c`` on the operands' device and calls
-    ``launch(c, *args, stream=...)`` there, on torch's current stream, so that it orders with the surrounding torch ops.
+def _define_op(name: str, schema: str, shape, launch, why: str = "", outputs=None, backward=None,
+               setup_context=None) -> None:
+    """Defines the operator cuda_l2_b200::<name> with ``schema``. ``shape(*args)`` checks the arguments by the kernel's
+    rules (meta tensors pass) and returns the result's shape and dtype: the fake implementation is an empty tensor of
+    those, and the CUDA one allocates the result ``c`` on the operands' device and calls ``launch(c, *args,
+    stream=...)`` there, on torch's current stream, so that it orders with the surrounding torch ops.
     An operator with several results passes ``outputs`` instead of ``shape``: ``outputs(*args)`` checks the arguments
     the same way and returns the tuple of empty results, allocated on the device of ``args[0]`` in their final layout;
     the CUDA and the fake implementation both call it, so the fake results have the real ones' shapes and strides, and
-    ``launch`` receives the tuple. The CPU implementation raises (there is no fallback), and so does a backward through
-    it (``why`` says why)."""
+    ``launch`` receives the tuple. The CPU implementation raises (there is no fallback). ``backward`` and
+    ``setup_context`` are the operator's gradient, as torch.library.register_autograd takes them; without them it is
+    inference only, and a backward through it raises (``why`` says why)."""
     qualname = f"{_LIB}::{name}"
     torch.library.define(qualname, schema)
 
@@ -130,8 +132,8 @@ def _inference_op(name: str, schema: str, shape, launch, why: str = "", outputs=
     torch.library.impl(qualname, "CUDA")(cuda)
     torch.library.impl(qualname, "CPU")(cpu)
     torch.library.register_fake(qualname)(fake)
-    # No gradient formula: without this, autograd would only warn and hand back no gradient for the inputs.
-    torch.library.register_autograd(qualname, no_backward)
+    # Without a gradient formula autograd would only warn and hand back no gradient for the inputs: no_backward raises.
+    torch.library.register_autograd(qualname, backward or no_backward, setup_context=setup_context)
 
 
 def _empty_product(c: torch.Tensor, k: int) -> bool:
@@ -145,32 +147,14 @@ def _empty_product(c: torch.Tensor, k: int) -> bool:
     return False
 
 
-torch.library.define(f"{_LIB}::hgemm", "(Tensor a, Tensor b_kmajor, str acc='fp32') -> Tensor")
-
-
-@torch.library.impl(f"{_LIB}::hgemm", "CUDA")
-def _hgemm_cuda(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
-    m, n, k = capi.check_operands(a, b_kmajor, a.dtype, acc)
-    a = a.contiguous()
-    b_kmajor = b_kmajor.contiguous()
-    c = torch.empty((m, n), dtype=a.dtype, device=a.device)
-    if _empty_product(c, k):
-        return c
-    with torch.cuda.device(a.device):
-        # the kernel is launched on torch's current stream, so it orders with the surrounding torch ops
-        capi.gemm_kmajor(a, b_kmajor, c, acc, stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
-
-
-@torch.library.impl(f"{_LIB}::hgemm", "CPU")
-def _hgemm_cpu(a, b_kmajor, acc="fp32"):
-    raise capi.B200HgemmError("cuda_l2_b200::hgemm has no CPU implementation (and no fallback): move the tensors to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::hgemm")
-def _hgemm_fake(a, b_kmajor, acc="fp32"):
+def _hgemm_shape(a, b_kmajor, acc="fp32"):
     m, n, _ = capi.check_operands(a, b_kmajor, a.dtype, acc)
-    return a.new_empty((m, n))
+    return (m, n), a.dtype
+
+
+def _hgemm_launch(c, a, b_kmajor, acc="fp32", *, stream):
+    if not _empty_product(c, a.shape[1]):
+        capi.gemm_kmajor(a.contiguous(), b_kmajor.contiguous(), c, acc, stream=stream)
 
 
 def _product_grads(a, b_kmajor, grad_c, need_a: bool, need_b: bool):
@@ -197,7 +181,8 @@ def _hgemm_setup_context(ctx, inputs, output):
     ctx.save_for_backward(a, b_kmajor)
 
 
-torch.library.register_autograd(f"{_LIB}::hgemm", _hgemm_backward, setup_context=_hgemm_setup_context)
+_define_op("hgemm", "(Tensor a, Tensor b_kmajor, str acc='fp32') -> Tensor", _hgemm_shape, _hgemm_launch,
+           backward=_hgemm_backward, setup_context=_hgemm_setup_context)
 
 
 def hgemm(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -206,31 +191,14 @@ def hgemm(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32") -> torch.T
 
 
 # ------------------------------------------------------------------------------------------ row-major B (libb200_nn.so)
-torch.library.define(f"{_LIB}::hgemm_nn", "(Tensor a, Tensor b, str acc='fp32') -> Tensor")
-
-
-@torch.library.impl(f"{_LIB}::hgemm_nn", "CUDA")
-def _hgemm_nn_cuda(a: torch.Tensor, b: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
-    m, n, k = capi.check_rowmajor_operands(a, b, a.dtype, acc)
-    a, b = a.contiguous(), b.contiguous()
-    c = torch.empty((m, n), dtype=a.dtype, device=a.device)
-    if _empty_product(c, k):
-        return c
-    with torch.cuda.device(a.device):
-        capi.gemm_rowmajor(a, b, c, acc, stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
-
-
-@torch.library.impl(f"{_LIB}::hgemm_nn", "CPU")
-def _hgemm_nn_cpu(a, b, acc="fp32"):
-    raise capi.B200HgemmError("cuda_l2_b200::hgemm_nn has no CPU implementation (and no fallback): move the tensors to "
-                              "an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::hgemm_nn")
-def _hgemm_nn_fake(a, b, acc="fp32"):
+def _hgemm_nn_shape(a, b, acc="fp32"):
     m, n, _ = capi.check_rowmajor_operands(a, b, a.dtype, acc)
-    return a.new_empty((m, n))
+    return (m, n), a.dtype
+
+
+def _hgemm_nn_launch(c, a, b, acc="fp32", *, stream):
+    if not _empty_product(c, a.shape[1]):
+        capi.gemm_rowmajor(a.contiguous(), b.contiguous(), c, acc, stream=stream)
 
 
 def _hgemm_nn_backward(ctx, grad_c):
@@ -251,7 +219,8 @@ def _hgemm_nn_setup_context(ctx, inputs, output):
     ctx.save_for_backward(a, b)
 
 
-torch.library.register_autograd(f"{_LIB}::hgemm_nn", _hgemm_nn_backward, setup_context=_hgemm_nn_setup_context)
+_define_op("hgemm_nn", "(Tensor a, Tensor b, str acc='fp32') -> Tensor", _hgemm_nn_shape, _hgemm_nn_launch,
+           backward=_hgemm_nn_backward, setup_context=_hgemm_nn_setup_context)
 
 
 def hgemm_nn(a: torch.Tensor, b: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -261,34 +230,17 @@ def hgemm_nn(a: torch.Tensor, b: torch.Tensor, acc: str = "fp32") -> torch.Tenso
 
 
 # ------------------------------------------------------------------------------------------ batched (libb200_batched.so)
-torch.library.define(f"{_LIB}::hgemm_batched",
-                     "(Tensor a, Tensor b_kmajor, str acc='fp32', Tensor? masked_m=None) -> Tensor")
+def _hgemm_batched_shape(a, b_kmajor, acc="fp32", masked_m=None):
+    bsz, m, n, _ = capi.check_batched_operands(a, b_kmajor, acc, masked_m)
+    return (bsz, m, n), a.dtype
 
 
-@torch.library.impl(f"{_LIB}::hgemm_batched", "CUDA")
-def _hgemm_batched_cuda(a, b_kmajor, acc="fp32", masked_m=None):
-    bsz, m, n, k = capi.check_batched_operands(a, b_kmajor, acc, masked_m)
-    a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
-    c = torch.empty((bsz, m, n), dtype=a.dtype, device=a.device)
-    if _empty_product(c, k):
-        return c
+def _hgemm_batched_launch(c, a, b_kmajor, acc="fp32", masked_m=None, *, stream):
+    if _empty_product(c, a.shape[2]):
+        return
     if masked_m is not None:
         masked_m = masked_m.contiguous()
-    with torch.cuda.device(a.device):
-        capi.gemm_batched(a, b_kmajor, c, acc, masked_m=masked_m, stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
-
-
-@torch.library.impl(f"{_LIB}::hgemm_batched", "CPU")
-def _hgemm_batched_cpu(a, b_kmajor, acc="fp32", masked_m=None):
-    raise capi.B200HgemmError("cuda_l2_b200::hgemm_batched has no CPU implementation (and no fallback): move the tensors "
-                              "to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::hgemm_batched")
-def _hgemm_batched_fake(a, b_kmajor, acc="fp32", masked_m=None):
-    bsz, m, n, _ = capi.check_batched_operands(a, b_kmajor, acc, masked_m)
-    return a.new_empty((bsz, m, n))
+    capi.gemm_batched(a.contiguous(), b_kmajor.contiguous(), c, acc, masked_m=masked_m, stream=stream)
 
 
 def _hgemm_batched_backward(ctx, grad_c):
@@ -312,8 +264,9 @@ def _hgemm_batched_setup_context(ctx, inputs, output):
     ctx.save_for_backward(a, b_kmajor)
 
 
-torch.library.register_autograd(f"{_LIB}::hgemm_batched", _hgemm_batched_backward,
-                                setup_context=_hgemm_batched_setup_context)
+_define_op("hgemm_batched", "(Tensor a, Tensor b_kmajor, str acc='fp32', Tensor? masked_m=None) -> Tensor",
+           _hgemm_batched_shape, _hgemm_batched_launch, backward=_hgemm_batched_backward,
+           setup_context=_hgemm_batched_setup_context)
 
 
 def hgemm_batched(a: torch.Tensor, b_kmajor: torch.Tensor, acc: str = "fp32",
@@ -337,8 +290,8 @@ def _hgemm_grouped_launch(c, a, b_kmajor, offs, acc="fp32", *, stream):
     capi.gemm_grouped(a, b_kmajor, c, offs, acc, stream=stream)
 
 
-_inference_op("hgemm_grouped", "(Tensor a, Tensor b_kmajor, Tensor offs, str acc='fp32') -> Tensor", _hgemm_grouped_shape,
-              _hgemm_grouped_launch, " (train through grouped_linear, the same product with a gradient)")
+_define_op("hgemm_grouped", "(Tensor a, Tensor b_kmajor, Tensor offs, str acc='fp32') -> Tensor", _hgemm_grouped_shape,
+           _hgemm_grouped_launch, " (train through grouped_linear, the same product with a gradient)")
 
 
 def hgemm_grouped(a: torch.Tensor, b_kmajor: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -362,8 +315,8 @@ def _hgemm_grouped_nn_launch(c, a, b, offs, acc="fp32", *, stream):
     capi.gemm_grouped_nn(a.contiguous(), b.contiguous(), c, offs.contiguous(), acc, stream=stream)
 
 
-_inference_op("hgemm_grouped_nn", "(Tensor a, Tensor b, Tensor offs, str acc='fp32') -> Tensor", _hgemm_grouped_nn_shape,
-              _hgemm_grouped_nn_launch, " (it is a backward kernel: train through grouped_linear)")
+_define_op("hgemm_grouped_nn", "(Tensor a, Tensor b, Tensor offs, str acc='fp32') -> Tensor", _hgemm_grouped_nn_shape,
+           _hgemm_grouped_nn_launch, " (it is a backward kernel: train through grouped_linear)")
 
 
 def hgemm_grouped_nn(a: torch.Tensor, b: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -384,9 +337,9 @@ def _hgemm_grouped_wgrad_launch(c, a, b, offs, acc="fp32", *, stream):
     capi.gemm_grouped_wgrad(a.contiguous(), b.contiguous(), c, offs.contiguous(), acc, stream=stream)
 
 
-_inference_op("hgemm_grouped_wgrad", "(Tensor a, Tensor b, Tensor offs, str acc='fp32') -> Tensor",
-              _hgemm_grouped_wgrad_shape, _hgemm_grouped_wgrad_launch,
-              " (it is a backward kernel: train through grouped_linear)")
+_define_op("hgemm_grouped_wgrad", "(Tensor a, Tensor b, Tensor offs, str acc='fp32') -> Tensor",
+           _hgemm_grouped_wgrad_shape, _hgemm_grouped_wgrad_launch,
+           " (it is a backward kernel: train through grouped_linear)")
 
 
 def hgemm_grouped_wgrad(a: torch.Tensor, b: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -396,26 +349,9 @@ def hgemm_grouped_wgrad(a: torch.Tensor, b: torch.Tensor, offs: torch.Tensor, ac
     return torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(a, b, offs, acc)
 
 
-torch.library.define(f"{_LIB}::grouped_linear", "(Tensor x, Tensor w, Tensor offs, str acc='fp32') -> Tensor")
-
-
-@torch.library.impl(f"{_LIB}::grouped_linear", "CUDA")
-def _grouped_linear_cuda(x, w, offs, acc="fp32"):
+def _grouped_linear_shape(x, w, offs, acc="fp32"):
     capi._bwd_variant(x.dtype, acc)   # a product the backward can run
-    return torch.ops.cuda_l2_b200.hgemm_grouped(x, w, offs, acc)
-
-
-@torch.library.impl(f"{_LIB}::grouped_linear", "CPU")
-def _grouped_linear_cpu(x, w, offs, acc="fp32"):
-    raise capi.B200HgemmError("cuda_l2_b200::grouped_linear has no CPU implementation (and no fallback): move the "
-                              "tensors to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::grouped_linear")
-def _grouped_linear_fake(x, w, offs, acc="fp32"):
-    capi._bwd_variant(x.dtype, acc)
-    _, t, n, _ = capi.check_grouped_operands(x, w, offs, acc)
-    return x.new_empty((t, n))
+    return _hgemm_grouped_shape(x, w, offs, acc)
 
 
 def _grouped_linear_backward(ctx, grad_y):
@@ -442,8 +378,8 @@ def _grouped_linear_setup_context(ctx, inputs, output):
     ctx.save_for_backward(x, w, offs)
 
 
-torch.library.register_autograd(f"{_LIB}::grouped_linear", _grouped_linear_backward,
-                                setup_context=_grouped_linear_setup_context)
+_define_op("grouped_linear", "(Tensor x, Tensor w, Tensor offs, str acc='fp32') -> Tensor", _grouped_linear_shape,
+           _hgemm_grouped_launch, backward=_grouped_linear_backward, setup_context=_grouped_linear_setup_context)
 
 
 def grouped_linear(x: torch.Tensor, w: torch.Tensor, offs: torch.Tensor, acc: str = "fp32") -> torch.Tensor:
@@ -587,40 +523,17 @@ def _bias_act_empty(c: torch.Tensor, k: int, bias, activation: str) -> bool:
     return False
 
 
-def _hgemm_bias_act_shape(a, b_kmajor, bias, activation):
+def _hgemm_bias_act_shape(a, b_kmajor, bias, activation="none"):
     m, n, k = capi.check_operands(a, b_kmajor, a.dtype, "fp32")
     capi.epilogue_variant(a.dtype, a.dtype)
     capi.check_bias(bias, n, a.dtype)
     capi.activation_code(activation)
-    return m, n, k
+    return (m, n), a.dtype
 
 
-torch.library.define(f"{_LIB}::hgemm_bias_act",
-                     "(Tensor a, Tensor b_kmajor, Tensor? bias, str activation='none') -> Tensor")
-
-
-@torch.library.impl(f"{_LIB}::hgemm_bias_act", "CUDA")
-def _hgemm_bias_act_cuda(a, b_kmajor, bias=None, activation="none"):
-    m, n, k = _hgemm_bias_act_shape(a, b_kmajor, bias, activation)
-    c = torch.empty((m, n), dtype=a.dtype, device=a.device)
-    if _bias_act_empty(c, k, bias, activation):
-        return c
-    with torch.cuda.device(a.device):
-        capi.gemm_bias_act(a.contiguous(), b_kmajor.contiguous(), c, bias, activation,
-                           stream=torch.cuda.current_stream(a.device).cuda_stream)
-    return c
-
-
-@torch.library.impl(f"{_LIB}::hgemm_bias_act", "CPU")
-def _hgemm_bias_act_cpu(a, b_kmajor, bias=None, activation="none"):
-    raise capi.B200HgemmError("cuda_l2_b200::hgemm_bias_act has no CPU implementation (and no fallback): move the "
-                              "tensors to an H100")
-
-
-@torch.library.register_fake(f"{_LIB}::hgemm_bias_act")
-def _hgemm_bias_act_fake(a, b_kmajor, bias=None, activation="none"):
-    m, n, _ = _hgemm_bias_act_shape(a, b_kmajor, bias, activation)
-    return a.new_empty((m, n))
+def _hgemm_bias_act_launch(c, a, b_kmajor, bias=None, activation="none", *, stream):
+    if not _bias_act_empty(c, a.shape[1], bias, activation):
+        capi.gemm_bias_act(a.contiguous(), b_kmajor.contiguous(), c, bias, activation, stream=stream)
 
 
 def _hgemm_bias_act_backward(ctx, grad_y):
@@ -648,8 +561,9 @@ def _hgemm_bias_act_setup_context(ctx, inputs, output):
     ctx.save_for_backward(a, b_kmajor, bias, output if activation == "relu" else None)
 
 
-torch.library.register_autograd(f"{_LIB}::hgemm_bias_act", _hgemm_bias_act_backward,
-                                setup_context=_hgemm_bias_act_setup_context)
+_define_op("hgemm_bias_act", "(Tensor a, Tensor b_kmajor, Tensor? bias, str activation='none') -> Tensor",
+           _hgemm_bias_act_shape, _hgemm_bias_act_launch, backward=_hgemm_bias_act_backward,
+           setup_context=_hgemm_bias_act_setup_context)
 
 
 def hgemm_bias_act(a: torch.Tensor, b_kmajor: torch.Tensor, bias: torch.Tensor | None = None,
@@ -711,9 +625,9 @@ def _fp8_gemm_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, *, stream):
     capi.fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream=stream)
 
 
-_inference_op("fp8_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor",
-              _fp8_gemm_shape, _fp8_gemm_launch,
-              " (train with the fp16 / bf16 operator and quantise afterwards)")
+_define_op("fp8_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor",
+           _fp8_gemm_shape, _fp8_gemm_launch,
+           " (train with the fp16 / bf16 operator and quantise afterwards)")
 
 
 def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
@@ -745,11 +659,11 @@ def _fp8_bias_act_launch(c, a, b_kmajor, scale_a, scale_b, bias, activation, out
     capi.gemm_bias_act(a.contiguous(), b_kmajor.contiguous(), c, bias, activation, scale_a, scale_b, stream=stream)
 
 
-_inference_op("fp8_gemm_bias_act",
-              "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, Tensor? bias, str activation, "
-              "ScalarType out_dtype) -> Tensor",
-              _fp8_bias_act_shape, _fp8_bias_act_launch,
-              " (train with the fp16 / bf16 operator hgemm_bias_act and quantise afterwards)")
+_define_op("fp8_gemm_bias_act",
+           "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, Tensor? bias, str activation, "
+           "ScalarType out_dtype) -> Tensor",
+           _fp8_bias_act_shape, _fp8_bias_act_launch,
+           " (train with the fp16 / bf16 operator hgemm_bias_act and quantise afterwards)")
 
 
 def fp8_gemm_bias_act(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
@@ -887,14 +801,14 @@ def _silu_mul_launch(out, h, masked_m=None, *, stream):
 
 
 _QUANT_WHY = " (quantisation is not differentiable: train the 16-bit model and quantise afterwards)"
-_inference_op("quantize_e4m3", "(Tensor x) -> (Tensor, Tensor)", None, _quantize_e4m3_launch, _QUANT_WHY,
-              outputs=_quantize_e4m3_outputs)
-_inference_op("quantize_e4m3_rowwise", "(Tensor x) -> (Tensor, Tensor)", None, _quantize_e4m3_rowwise_launch,
-              _QUANT_WHY, outputs=_quantize_e4m3_rowwise_outputs)
-_inference_op("quantize_e4m3_blockwise", "(Tensor x, Tensor? masked_m=None) -> (Tensor, Tensor)", None,
-              _quantize_e4m3_blockwise_launch, _QUANT_WHY, outputs=_quantize_e4m3_blockwise_outputs)
-_inference_op("silu_mul_quantize_e4m3_blockwise", "(Tensor h, Tensor? masked_m=None) -> (Tensor, Tensor)", None,
-              _silu_mul_launch, _QUANT_WHY, outputs=_silu_mul_outputs)
+_define_op("quantize_e4m3", "(Tensor x) -> (Tensor, Tensor)", None, _quantize_e4m3_launch, _QUANT_WHY,
+           outputs=_quantize_e4m3_outputs)
+_define_op("quantize_e4m3_rowwise", "(Tensor x) -> (Tensor, Tensor)", None, _quantize_e4m3_rowwise_launch,
+           _QUANT_WHY, outputs=_quantize_e4m3_rowwise_outputs)
+_define_op("quantize_e4m3_blockwise", "(Tensor x, Tensor? masked_m=None) -> (Tensor, Tensor)", None,
+           _quantize_e4m3_blockwise_launch, _QUANT_WHY, outputs=_quantize_e4m3_blockwise_outputs)
+_define_op("silu_mul_quantize_e4m3_blockwise", "(Tensor h, Tensor? masked_m=None) -> (Tensor, Tensor)", None,
+           _silu_mul_launch, _QUANT_WHY, outputs=_silu_mul_outputs)
 
 
 def quantize_e4m3(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
@@ -1074,8 +988,8 @@ def _quantize_e4m3_rowwise_dual_launch(out, x, *, stream):
     capi.quantize_e4m3_rowwise_dual(x.contiguous(), *out, workspace, stream=stream)
 
 
-_inference_op("quantize_e4m3_rowwise_dual", "(Tensor x) -> (Tensor, Tensor, Tensor, Tensor)", None,
-              _quantize_e4m3_rowwise_dual_launch, _QUANT_WHY, outputs=_quantize_e4m3_rowwise_dual_outputs)
+_define_op("quantize_e4m3_rowwise_dual", "(Tensor x) -> (Tensor, Tensor, Tensor, Tensor)", None,
+           _quantize_e4m3_rowwise_dual_launch, _QUANT_WHY, outputs=_quantize_e4m3_rowwise_dual_outputs)
 
 
 def quantize_e4m3_rowwise_dual(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -1228,8 +1142,8 @@ def _fp8_grouped_launch(c, a, b_kmajor, scale_a, scale_b, offs, out_dtype, *, st
     capi.fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs, stream=stream)
 
 
-_inference_op("fp8_grouped_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, Tensor offs, "
-              "ScalarType out_dtype) -> Tensor", _fp8_grouped_shape, _fp8_grouped_launch)
+_define_op("fp8_grouped_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, Tensor offs, "
+           "ScalarType out_dtype) -> Tensor", _fp8_grouped_shape, _fp8_grouped_launch)
 
 
 def fp8_grouped_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,
@@ -1258,8 +1172,8 @@ def _fp8_batched_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=No
     capi.fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=masked_m, stream=stream)
 
 
-_inference_op("fp8_batched_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype, "
-              "Tensor? masked_m=None) -> Tensor", _fp8_batched_shape, _fp8_batched_launch)
+_define_op("fp8_batched_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype, "
+           "Tensor? masked_m=None) -> Tensor", _fp8_batched_shape, _fp8_batched_launch)
 
 
 def fp8_batched_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, scale_b: torch.Tensor,

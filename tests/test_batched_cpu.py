@@ -167,6 +167,9 @@ def test_schedule_rejects_bad_arguments(built_libs):
     assert lib.b200_batched_schedule_units(0, 2, 64, 64, 64, None, 0, 0, None, 0, None) == -1
     assert lib.b200_batched_schedule_units(0, 2, 64, 64, 64, None, 132, 5, None, 0, ctypes.byref(nw)) == -1
     assert nw.value == 2                                                     # one tile per matrix: two workers
+    with pytest.raises(capi.B200HgemmError) as err:                          # the status, with its text
+        capi.batched_schedule(NUM_CONFIGS, 2, 64, 64, 64)
+    assert str(err.value) == f"b200_batched_schedule_units failed: status -6 ({lib.b200_batched_strerror(-6).decode()})"
 
 
 def test_batched_sass(built_libs):
