@@ -4,6 +4,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
 
 * ``libb200_hgemm.so``  — the C-ABI product library (include/b200_hgemm.h)
 * ``libb200_fp8block.so`` — the block-scaled FP8 GEMM (include/b200_fp8_block.h)
+* ``libb200_fp8block_1d1d.so`` — the block-scaled FP8 GEMM with 1 x 128 scales on both operands, the weight gradient of
+  blockwise FP8 training (csrc/b200_fp8_block_1d1d.h; no public symbol)
 * ``libb200_batched.so`` — the batched fp16 / bf16 GEMM (include/b200_batched.h)
 * ``libb200_grouped.so`` — the grouped fp16 / bf16 GEMM over contiguous row groups (include/b200_grouped.h)
 * ``libb200_grouped_fp8.so`` — the block-scaled FP8 grouped GEMM over contiguous row groups (include/b200_grouped_fp8.h)
@@ -18,6 +20,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
   SwiGLU + 1 x 128 blocks (csrc/b200_quant.h; no public symbol)
 * ``libb200_quant_dual.so`` — the dual-orientation rowwise e4m3 quantiser of FP8 training: x and x^T quantised from
   one tensor (csrc/b200_quant_dual.h; no public symbol)
+* ``libb200_quant_block_dual.so`` — the dual-orientation 1 x 128 and 128 x 128 e4m3 quantisers of blockwise FP8
+  training: both orientations of a tensor from one read of it (csrc/b200_quant_block_dual.h; no public symbol)
 * ``libb200_baselines.so`` — cuBLAS / cuBLASLt comparators behind a C ABI (include/b200_baselines.h)
 * ``dev_check``         — standalone bring-up / tuning binary (developer tool)
 
@@ -98,6 +102,7 @@ VARIANTS = (0, 1, 2)   # fp16 with fp32 accumulation, fp16 with fp16 accumulatio
 BLOCK_VARIANTS = (5, 6)   # block-scaled e4m3 with fp16 / bf16 output (the GemmType index)
 BWD_VARIANTS = (0, 2)     # the grouped backward: fp16 and bf16, both with fp32 accumulation (the GemmType index)
 EPILOGUE_VARIANTS = (0, 2, 3, 4)   # bias + activation: fp16, bf16, e4m3 to fp16, e4m3 to bf16 (the GemmType index)
+BLOCK_1D1D_VARIANTS = (7, 8)      # 1 x 128 scales on both operands: e4m3 to fp16 / bf16 (the GemmType index)
 
 
 def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, list[str]]]:
@@ -110,10 +115,12 @@ def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, lis
 # compiles its 16-bit kernels (b200_hgemm_capi.cu) and its e4m3 ones (b200_fp8_capi.cu) in parallel; the tile-list
 # libraries compile one source per variant (31 kernels each for the 16-bit variants, 17 for the block-scaled ones), and
 # so does libb200_nn.so (43 kernels per 16-bit variant), libb200_grouped_bwd.so (56 per variant: 28 configurations
-# times two kinds) and libb200_epilogue.so (46 per variant: libb200_hgemm.so's (configuration, K-mode) pairs).
+# times two kinds), libb200_epilogue.so (46 per variant: libb200_hgemm.so's (configuration, K-mode) pairs) and
+# libb200_fp8block_1d1d.so (19 per output type, libb200_fp8block.so's configurations and K-modes).
 LIBRARIES = {
     "capi": ("libb200_hgemm.so", [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], []),
     "fp8block": ("libb200_fp8block.so", [(CSRC / "b200_fp8_block_capi.cu", [])], []),
+    "fp8block_1d1d": ("libb200_fp8block_1d1d.so", _per_variant("b200_fp8_block_1d1d.cu", BLOCK_1D1D_VARIANTS), []),
     "batched": ("libb200_batched.so", _per_variant("b200_batched_capi.cu", VARIANTS), []),
     "grouped": ("libb200_grouped.so", _per_variant("b200_grouped_capi.cu", VARIANTS), []),
     "grouped_fp8": ("libb200_grouped_fp8.so", _per_variant("b200_grouped_fp8_capi.cu", BLOCK_VARIANTS), []),
@@ -123,6 +130,7 @@ LIBRARIES = {
     "epilogue": ("libb200_epilogue.so", _per_variant("b200_epilogue.cu", EPILOGUE_VARIANTS), []),
     "quant": ("libb200_quant.so", [(CSRC / "b200_quant.cu", [])], []),
     "quant_dual": ("libb200_quant_dual.so", [(CSRC / "b200_quant_dual.cu", [])], []),
+    "quant_block_dual": ("libb200_quant_block_dual.so", [(CSRC / "b200_quant_block_dual.cu", [])], []),
     "baselines": ("libb200_baselines.so", [(CSRC / "b200_baselines_capi.cu", [])], ["-lcublas", "-lcublasLt"]),
 }
 

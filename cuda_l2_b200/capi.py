@@ -107,6 +107,9 @@ _BWD_SELECT = ([_i, _i, _i, _i, _i, _ip, _ip], _i)
 EPILOGUE_LIB = "libb200_epilogue.so"         # csrc/b200_epilogue.h
 QUANT_LIB = "libb200_quant.so"               # csrc/b200_quant.h
 QUANT_DUAL_LIB = "libb200_quant_dual.so"     # csrc/b200_quant_dual.h
+FP8BLOCK_1D1D_LIB = "libb200_fp8block_1d1d.so"       # csrc/b200_fp8_block_1d1d.h
+QUANT_BLOCK_DUAL_LIB = "libb200_quant_block_dual.so"  # csrc/b200_quant_block_dual.h
+_QUANT_BLOCK_DUAL = ([_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp], _i)
 _QUANT_BLOCKWISE = ([_i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp], _i)
 INTERNAL_ABI = {
     GROUPED_BWD_LIB: {
@@ -140,6 +143,20 @@ INTERNAL_ABI = {
         "cuda_l2_b200_quant_dual_e4m3_rowwise": ([_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp], _i),
         "cuda_l2_b200_quant_dual_launch_count": ([], ctypes.c_ulonglong),
         "cuda_l2_b200_quant_dual_strerror": ([_i], ctypes.c_char_p),
+    },
+    FP8BLOCK_1D1D_LIB: {
+        "cuda_l2_b200_fp8block_1d1d_run": ([_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_fp8block_1d1d_run_config": ([_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i,
+                                                   _vp], _i),
+        "cuda_l2_b200_fp8block_1d1d_select": ([_i, _i, _i, _ip, _ip, _ip], _i),
+        "cuda_l2_b200_fp8block_1d1d_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_fp8block_1d1d_strerror": ([_i], ctypes.c_char_p),
+    },
+    QUANT_BLOCK_DUAL_LIB: {
+        "cuda_l2_b200_quant_block_dual_e4m3_1x128": _QUANT_BLOCK_DUAL,
+        "cuda_l2_b200_quant_block_dual_e4m3_128x128": _QUANT_BLOCK_DUAL,
+        "cuda_l2_b200_quant_block_dual_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_quant_block_dual_strerror": ([_i], ctypes.c_char_p),
     },
 }
 _TABLES = {**ABI, **INTERNAL_ABI}
@@ -283,8 +300,10 @@ def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None, gr
     """torch._scaled_mm's rule for the scales of an [M,K] x [N,K] e4m3 product: two one-element fp32 tensors are
     ``"tensor"`` scales; ``scale_a`` [M,1] with ``scale_b`` [1,N], both fp32, are ``"rowwise"`` scales (one per row of A,
     one per output column); ``scale_a`` [M, nkb] with ``scale_b`` [ceil(N/128), nkb], nkb = ceil(K/128), both fp32, are
-    ``"blockwise"`` scales (one per row of A and 128 k, one per 128 x 128 block of Bt). Without ``k``, any nkb the two
-    agree on is accepted. ``groups``: the grouped product of M = T rows by ``groups`` matrices Bt [N,K], whose only
+    ``"blockwise"`` scales (one per row of A and 128 k, one per 128 x 128 block of Bt); ``scale_a`` [M, nkb] with
+    ``scale_b`` [N, nkb] are ``"blockwise_1d1d"`` scales (one per row and 128 k on both operands: the weight gradient of
+    blockwise FP8 training; N % 8 == 0, so N > ceil(N/128) and the two blockwise forms never meet). Without ``k``, any
+    nkb the two agree on is accepted. ``groups``: the grouped product of M = T rows by ``groups`` matrices Bt [N,K], whose only
     scales are blockwise, with ``scale_b`` [groups, ceil(N/128), nkb]. ``batches``: the batched product of ``batches``
     matrices [M,K] by as many Bt [N,K], whose only scales are blockwise, with ``scale_a`` [batches, M, nkb] and
     ``scale_b`` [batches, ceil(N/128), nkb]. Anything else, a mix of them included, raises B200HgemmError."""
@@ -302,6 +321,8 @@ def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None, gr
         nkb = num_k_blocks(k) if k is not None else (sa[-1] if len(sa) == 2 + len(lead_a) else -1)
         if sa == (*lead_a, m, nkb) and sb == (*lead, -(-n // BLOCK), nkb):
             return "blockwise"
+        if plain and sa == (m, nkb) and sb == (n, nkb) and n > -(-n // BLOCK):
+            return "blockwise_1d1d"
     if groups is not None:
         raise B200HgemmError(f"grouped scales must be fp32 blockwise scales, scale_a [{m}, ceil(K/128)] with scale_b "
                              f"[{groups}, ceil({n}/128), ceil(K/128)], got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
@@ -311,7 +332,8 @@ def scale_granularity(m: int, n: int, scale_a, scale_b, k: int | None = None, gr
                              f"{scale_b.dtype} {sb}")
     raise B200HgemmError(f"scales must be fp32 and either both one-element (per tensor), scale_a [{m}, 1] with "
                          f"scale_b [1, {n}] (rowwise), or scale_a [{m}, ceil(K/128)] with scale_b [ceil({n}/128), "
-                         f"ceil(K/128)] (blockwise), got {scale_a.dtype} {sa} and {scale_b.dtype} {sb}")
+                         f"ceil(K/128)] (blockwise) or [{n}, ceil(K/128)] (blockwise_1d1d), got {scale_a.dtype} {sa} and "
+                         f"{scale_b.dtype} {sb}")
 
 
 def blockwise_ld_a(scale_a) -> int | None:
@@ -335,11 +357,20 @@ def blockwise_ld_a(scale_a) -> int | None:
 batched_blockwise_ld_a = blockwise_ld_a   # the batched [B, M, nkb] form, by the name of the batched call
 
 
-def _scale_ld_a(scale_a) -> int:
-    """blockwise_ld_a of a ``scale_a`` the kernel reads in place; B200HgemmError if it cannot."""
+def scale_granularity_or_none(m: int, n: int, scale_a, scale_b, k: int | None = None) -> str | None:
+    """:func:`scale_granularity` of a plain product, or None where it raises."""
+    try:
+        return scale_granularity(m, n, scale_a, scale_b, k=k)
+    except B200HgemmError:
+        return None
+
+
+def _scale_ld_a(scale_a, name: str = "scale_a") -> int:
+    """blockwise_ld_a of a ``scale_a`` (or a 1 x 128 ``scale_b``, the same layout) the kernel reads in place;
+    B200HgemmError if it cannot."""
     ld_a = blockwise_ld_a(scale_a)
     if ld_a is None:
-        raise B200HgemmError(f"blockwise scale_a must hold one M-major [ceil(K/128), ld_a] block per matrix (strides "
+        raise B200HgemmError(f"blockwise {name} must hold one M-major [ceil(K/128), ld_a] block per matrix (strides "
                              f"(1, ld_a), batched (ceil(K/128) * ld_a, 1, ld_a)) with ld_a >= M, ld_a % 4 == 0, 16-byte "
                              f"aligned, every block readable; got strides {tuple(scale_a.stride())}")
     return ld_a
@@ -385,18 +416,19 @@ def _check_k(a, b_kmajor, t: GemmType, n: int, k: int, k2: int, b_layout: str) -
                              f"got N={n}, K={k}")
 
 
-def _contiguous_cuda(**tensors) -> None:
-    """B200HgemmError unless every tensor given (None: not passed) is a contiguous CUDA tensor. ``scale_a`` need not be
-    contiguous: blockwise scales are read M-major, in place (:func:`blockwise_ld_a`)."""
+def _contiguous_cuda(in_place=("scale_a",), **tensors) -> None:
+    """B200HgemmError unless every tensor given (None: not passed) is a contiguous CUDA tensor. The tensors named in
+    ``in_place`` (``scale_a``) need not be contiguous: blockwise scales are read M-major, in place
+    (:func:`blockwise_ld_a`)."""
     for name, x in tensors.items():
-        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name == "scale_a")):
+        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name in in_place)):
             raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
 
 
-def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = ()) -> tuple[int, int, int]:
-    """check_operands for c = a @ b_kmajor^T, all of them (scales included, scale_a as :func:`_contiguous_cuda` allows)
-    CUDA tensors, c of shape [M,N]."""
-    _contiguous_cuda(a=a, b_kmajor=b_kmajor, c=c, **dict(zip(("scale_a", "scale_b"), scales)))
+def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = (), in_place=("scale_a",)) -> tuple[int, int, int]:
+    """check_operands for c = a @ b_kmajor^T, all of them (scales included, those in ``in_place`` as
+    :func:`_contiguous_cuda` allows) CUDA tensors, c of shape [M,N]."""
+    _contiguous_cuda(in_place, a=a, b_kmajor=b_kmajor, c=c, **dict(zip(("scale_a", "scale_b"), scales)))
     m, n, k = check_operands(a, b_kmajor, c.dtype, acc, scales)
     if c.shape != (m, n):
         raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
@@ -472,13 +504,31 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     element each (per tensor: ``* scale_a * scale_b``), or ``scale_a`` [M,1] and ``scale_b`` [1,N], 16-byte aligned
     (rowwise: ``* scale_b[n]``, then ``* scale_a[m]``), or blockwise scales (include/b200_fp8_block.h): ``scale_a``
     [M, ceil(K/128)] M-major (strides (1, ld_a), see :func:`blockwise_ld_a`), ``scale_b`` [ceil(N/128), ceil(K/128)]
-    contiguous, run by libb200_fp8block.so. ``config_id`` pins one kernel configuration (tests; ``splits`` as in
+    contiguous, run by libb200_fp8block.so, or 1 x 128 scales on both operands (csrc/b200_fp8_block_1d1d.h):
+    ``scale_a`` as for blockwise, ``scale_b`` [N, ceil(K/128)] N-major in the same layout (strides (1, ld_b)), read in
+    place, run by libb200_fp8block_1d1d.so. ``config_id`` pins one kernel configuration (tests; ``splits`` as in
     b200_hgemm_run_config; ``max_ctas`` as in :func:`gemm_kmajor`); default is the dispatcher."""
     import torch
 
-    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b))
+    one_d = (a.dim() == 2 and b_kmajor.dim() == 2 and scale_granularity_or_none(
+        a.shape[0], b_kmajor.shape[0], scale_a, scale_b, k=a.shape[1]) == "blockwise_1d1d")
+    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b),
+                               ("scale_a", "scale_b") if one_d else ("scale_a",))
     out_bf16 = int(c.dtype == torch.bfloat16)
     granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
+    if granularity == "blockwise_1d1d":
+        ld_a, ld_b = _scale_ld_a(scale_a), _scale_ld_a(scale_b, "scale_b")
+        lib = fp8block_1d1d_lib()
+        if config_id is None:
+            fn = lib.cuda_l2_b200_fp8block_1d1d_run
+            st = fn(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr(), ld_b,
+                    out_bf16, m, n, k, stream)
+        else:
+            fn = lib.cuda_l2_b200_fp8block_1d1d_run_config
+            st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a,
+                    scale_b.data_ptr(), ld_b, m, n, k, group_m, max_ctas, splits, stream)
+        _check(st, fn)
+        return
     if granularity == "blockwise":
         ld_a = _scale_ld_a(scale_a)
         blk = fp8block_lib()
@@ -527,6 +577,22 @@ def fp8_blockwise_select(m: int, n: int, k: int) -> tuple[int, int, int]:
 
 def fp8block_launch_count() -> int:
     return int(fp8block_lib().b200_fp8block_launch_count())
+
+
+def fp8block_1d1d_lib() -> ctypes.CDLL:
+    """libb200_fp8block_1d1d.so: the block-scaled e4m3 GEMM with 1 x 128 scales on both operands
+    (csrc/b200_fp8_block_1d1d.h, no public ABI)."""
+    return load(FP8BLOCK_1D1D_LIB)
+
+
+def fp8_blockwise_1d1d_select(m: int, n: int, k: int) -> tuple[int, int, int]:
+    """(config id, rasterisation group, splits code) of the dispatched 1 x 128 x 1 x 128 call
+    (cuda_l2_b200_fp8block_1d1d_select: b200_fp8gemm_blockwise_select's choice)."""
+    return _select(fp8block_1d1d_lib().cuda_l2_b200_fp8block_1d1d_select, m, n, k)
+
+
+def fp8block_1d1d_launch_count() -> int:
+    return int(fp8block_1d1d_lib().cuda_l2_b200_fp8block_1d1d_launch_count())
 
 
 def _tile_list_schedule(schedule_units, ints: int, *args) -> dict:
@@ -1115,7 +1181,7 @@ def gemm_bias_act(a, b_kmajor, c, bias=None, activation: str = "none", scale_a=N
     rowwise = 0
     if scales:
         granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
-        if granularity == "blockwise":
+        if granularity in ("blockwise", "blockwise_1d1d"):
             raise B200HgemmError("blockwise e4m3 scales have no bias + activation kernel (per-tensor or rowwise only)")
         rowwise = int(granularity == "rowwise")
         if not scale_a.is_contiguous():
@@ -1311,3 +1377,58 @@ def quantize_e4m3_rowwise_dual(x, q, scale, q_t, scale_t, workspace, stream: int
 
 def quant_dual_launch_count() -> int:
     return int(quant_dual_lib().cuda_l2_b200_quant_dual_launch_count())
+
+
+# ------------------------------------------------------------------------------------------ dual-orientation block
+#                                                                                            e4m3 (libb200_quant_block_dual.so)
+def quant_block_dual_lib() -> ctypes.CDLL:
+    """libb200_quant_block_dual.so: x and x^T quantised per 1 x 128 group, or w and w^T per 128 x 128 block, from one
+    read of the tensor (csrc/b200_quant_block_dual.h, no public ABI)."""
+    return load(QUANT_BLOCK_DUAL_LIB)
+
+
+def _block_dual_input(x) -> tuple[int, int, int]:
+    """(dtype code, rows, cols) of a 2-D contiguous fp16 / bf16 CUDA ``x``; B200HgemmError otherwise."""
+    code = quant_dtype(x.dtype, silu_mul=True)   # fp16 and bf16 only, as for the SwiGLU kernel
+    if code is None or x.dim() != 2:
+        raise B200HgemmError(f"the dual block quantisers take a 2-D fp16 / bf16 [rows, cols] tensor, got {x.dtype} "
+                             f"{list(x.shape)}")
+    _contiguous_cuda(x=x)
+    return code, *x.shape
+
+
+def quantize_e4m3_blockwise_dual(x, q, scale, q_t, scale_t, stream: int | None = None) -> None:
+    """Both 1 x 128 quantisations of a 2-D ``x`` [rows, cols] (fp16 or bf16, contiguous) in one launch: ``q`` (e4m3
+    [rows, cols]) with ``scale`` [rows, ceil(cols/128)], and ``q_t`` (e4m3 [cols, dual_ld_t(rows)], x^T zero-padded)
+    with ``scale_t`` [cols, ceil(rows/128)], both scales written in place in the M-major layout of
+    :func:`blockwise_ld_a` with ld = rows (cols) rounded up to 4 (csrc/b200_quant_block_dual.h)."""
+    code, rows, cols = _block_dual_input(x)
+    _quant_output(q, x.shape, x)
+    _quant_output(q_t, (cols, dual_ld_t(rows)), x)
+    for name, s, (m, nkb) in (("scale", scale, (rows, num_k_blocks(cols))),
+                              ("scale_t", scale_t, (cols, num_k_blocks(rows)))):
+        _fp32_on(s, x, name, (m, nkb))
+        if blockwise_ld_a(s) != -(-m // 4) * 4:
+            raise B200HgemmError(f"{name} must be the M-major view of a [{nkb}, {-(-m // 4) * 4}] buffer")
+    fn = quant_block_dual_lib().cuda_l2_b200_quant_block_dual_e4m3_1x128
+    _check(fn(code, x.data_ptr(), rows, cols, q.data_ptr(), scale.data_ptr(), q_t.data_ptr(), scale_t.data_ptr(),
+              stream), fn)
+
+
+def quantize_e4m3_block128x128_dual(w, q, scale, q_t, scale_t, stream: int | None = None) -> None:
+    """Both 128 x 128 block quantisations of a 2-D ``w`` [rows, cols] (fp16 or bf16, contiguous) in one launch: ``q``
+    (e4m3 [rows, cols]) with ``scale`` (fp32 [ceil(rows/128), ceil(cols/128)], contiguous), and ``q_t`` = q^T (e4m3
+    [cols, rows]) with ``scale_t`` = scale^T (csrc/b200_quant_block_dual.h)."""
+    code, rows, cols = _block_dual_input(w)
+    _quant_output(q, w.shape, w)
+    _quant_output(q_t, (cols, rows), w)
+    _fp32_on(scale, w, "scale", (-(-rows // BLOCK), num_k_blocks(cols)))
+    _fp32_on(scale_t, w, "scale_t", (num_k_blocks(cols), -(-rows // BLOCK)))
+    _contiguous_cuda(scale=scale, scale_t=scale_t)
+    fn = quant_block_dual_lib().cuda_l2_b200_quant_block_dual_e4m3_128x128
+    _check(fn(code, w.data_ptr(), rows, cols, q.data_ptr(), scale.data_ptr(), q_t.data_ptr(), scale_t.data_ptr(),
+              stream), fn)
+
+
+def quant_block_dual_launch_count() -> int:
+    return int(quant_block_dual_lib().cuda_l2_b200_quant_block_dual_launch_count())

@@ -15,7 +15,7 @@ namespace b200 {
 
 #define B200_EPI_RUN(T)                                                                                       \
   int run_config<T, BiasAct>(int, const void*, const void*, void*, Scales, int, int, int, int, int, int, void*, \
-                             int, host::ScratchFn, const void*, int)
+                             int, host::ScratchFn, const void*, int, int)
 extern template B200_EPI_RUN(host::GemmType::kF16Acc32);
 extern template B200_EPI_RUN(host::GemmType::kBF16);
 extern template B200_EPI_RUN(host::GemmType::kE4M3F16);

@@ -11,23 +11,7 @@ using b200::host::GemmType;
 namespace b200 {
 namespace block {
 
-// (eligible(), sibling() and kModes are in hgemm_configs.cuh.)
-// The dispatcher's `splits` code for the sibling: workspace split-K becomes cluster split-K of the largest of 8/4/2
-// not above it, stream-K the plain schedule; only configurations with split-K kernels keep a split.
-constexpr int sibling_splits(int id, int splits) {
-  if (!kConfigs[id].split_k) return 1;
-  const host::KRequest r = host::decode_splits(splits);
-  if (r.mode == kWorkspaceSplitK) return r.factor >= 8 ? -8 : r.factor >= 4 ? -4 : -2;
-  if (r.mode == kClusterSplitK) return splits;
-  return 1;
-}
-
-dispatch::Choice select(int M, int N, int K) {
-  dispatch::Choice ch = dispatch::select(GemmType::kE4M3F16Block, M, N, K);
-  ch.config_id = sibling(ch.config_id);
-  ch.splits = sibling_splits(ch.config_id, ch.splits);
-  return ch;
-}
+// (eligible(), sibling() and kModes are in hgemm_configs.cuh, select() in hgemm_dispatch.cuh.)
 
 Scales scales_of(const void* scale_a, const void* scale_b) {
   return Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};

@@ -13,7 +13,7 @@ namespace b200 {
 
 #define B200_NN_RUN(T)                                                                                          \
   int run_config<T, RowMajorB>(int, const void*, const void*, void*, Scales, int, int, int, int, int, int, void*, \
-                               int, host::ScratchFn, const void*, int)
+                               int, host::ScratchFn, const void*, int, int)
 extern template B200_NN_RUN(host::GemmType::kF16Acc32);
 extern template B200_NN_RUN(host::GemmType::kF16Acc16);
 extern template B200_NN_RUN(host::GemmType::kBF16);

@@ -151,15 +151,16 @@ using Unwrapped = Cfg;
 // translation unit of the library; hidden, so that no other shared object's copy is bound to it.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_launches{0};
 
-// Launch configuration `id` of variant T in Wrapper (Unwrapped, BlockScaled, RowMajorB or BiasAct), with the block
-// scales' ld_a, the split-K scratch source, and BiasAct's bias and activation code, of host::launch. A configuration
+// Launch configuration `id` of variant T in Wrapper (Unwrapped, BlockScaled, BlockScaled1D1D, RowMajorB or BiasAct),
+// with the block scales' ld_a, the split-K scratch source, BiasAct's bias and activation code, and BlockScaled1D1D's
+// ld_b, of host::launch. A configuration
 // without a kernel is kBadConfig. An instantiation
 // compiles the kernels of all configurations for T, so each translation unit of a library instantiates only the
 // variants it exports.
 template <host::GemmType T, template <class> class Wrapper = Unwrapped>
 int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, int M, int N, int K, int group_m,
                int max_ctas, int splits, void* stream, int ld_a = 0, host::ScratchFn scratch = host::splitk_scratch,
-               const void* bias = nullptr, int act = kActNone) {
+               const void* bias = nullptr, int act = kActNone, int ld_b = 0) {
   constexpr host::GemmTypeTraits t = host::traits(T);
   using Probe = Wrapper<Config<128, 6, 1, t.acc_f32, 1, 1, 1, t.bf16(), t.e4m3()>>;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -170,7 +171,7 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
     if constexpr (has_kernel<Probe>(ID))                                                                       \
       st = host::launch<Wrapper<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16(), t.e4m3()>>,            \
                         k_modes<Probe>()>(A, Bt, C, M, N, K, s, group_m, max_ctas, splits, scales, ld_a, scratch, \
-                                          bias, act);                                                          \
+                                          bias, act, ld_b);                                                    \
     break;
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE

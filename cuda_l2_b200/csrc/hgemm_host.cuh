@@ -31,6 +31,7 @@ enum Status : int {
   kBadScaleLd = -10,     // block scales: the row stride of A's scales must be >= M and a multiple of 4
   kNoNNLibrary = -11,    // row-major B: libb200_nn.so, next to libb200_hgemm.so, is missing or does not load
   kBadActivation = -12,  // bias + activation epilogue: the activation code is not one of Activation's
+  kBadScaleLdB = -13,    // 1 x 128 scales of Bt (BlockScaled1D1D<>): their row stride must be >= N and a multiple of 4
   // > 0: a cudaError_t from the launch
 };
 
@@ -49,6 +50,7 @@ inline const char* status_string(int s) {
     case kBadScaleLd: return "block scales need ld_a >= M and ld_a % 4 == 0 (16-byte aligned k-block rows of A's scales)";
     case kNoNNLibrary: return "row-major B needs libb200_nn.so next to libb200_hgemm.so (missing, or it does not load)";
     case kBadActivation: return "unknown activation code (0 none, 1 relu, 2 gelu_tanh)";
+    case kBadScaleLdB: return "1 x 128 scales of Bt need ld_b >= N and ld_b % 4 == 0 (16-byte aligned k-block rows)";
     default: return s > 0 ? cudaGetErrorString(static_cast<cudaError_t>(s)) : "unknown error";
   }
 }
@@ -76,13 +78,15 @@ constexpr int elem_bytes(Elem e) { return e == Elem::kE4M3 ? 1 : 2; }
 
 // The data-type variants of the kernel family. Everything the host does differently per variant (which kernels it
 // instantiates, the argument rules, the tuned-table entry) reads the variant's row of kGemmTypes.
-enum class GemmType : int { kF16Acc32, kF16Acc16, kBF16, kE4M3F16, kE4M3BF16, kE4M3F16Block, kE4M3BF16Block };
+enum class GemmType : int { kF16Acc32, kF16Acc16, kBF16, kE4M3F16, kE4M3BF16, kE4M3F16Block, kE4M3BF16Block,
+                            kE4M3F16Block1D1D, kE4M3BF16Block1D1D };
 struct GemmTypeTraits {
   Elem operand, output;
   bool acc_f32;       // fp32 accumulation (fp16 otherwise); the dispatcher reads that accumulator's tuned entry ...
   int table_k_div;    // ... at K / table_k_div: the 16-bit problem that moves as many bytes per k-block
   bool scaled;        // takes fp32 scales in device memory (per tensor or rowwise, see Scales) ...
-  bool block = false; // ... or block scales (BlockScaled<> kernels, a library of their own)
+  bool block = false; // ... or block scales (BlockScaled<> kernels, a library of their own) ...
+  bool block_1d1d = false;   // ... with 1 x 128 scales on Bt too (BlockScaled1D1D<> kernels, another library)
   // the Config<> flags: BF16 names the output type, E4M3 the operand type
   constexpr bool bf16() const { return output == Elem::kBF16; }
   constexpr bool e4m3() const { return operand == Elem::kE4M3; }
@@ -95,6 +99,8 @@ constexpr GemmTypeTraits kGemmTypes[] = {
     {Elem::kE4M3, Elem::kBF16, true, 2, true},     // kE4M3BF16
     {Elem::kE4M3, Elem::kF16, true, 2, true, true},    // kE4M3F16Block
     {Elem::kE4M3, Elem::kBF16, true, 2, true, true},   // kE4M3BF16Block
+    {Elem::kE4M3, Elem::kF16, true, 2, true, true, true},    // kE4M3F16Block1D1D
+    {Elem::kE4M3, Elem::kBF16, true, 2, true, true, true},   // kE4M3BF16Block1D1D
 };
 constexpr const GemmTypeTraits& traits(GemmType t) { return kGemmTypes[int(t)]; }
 
@@ -102,7 +108,8 @@ constexpr const GemmTypeTraits& traits(GemmType t) { return kGemmTypes[int(t)]; 
 template <class Cfg>
 constexpr GemmType gemm_type(int t = 0) {
   const GemmTypeTraits& x = kGemmTypes[t];
-  return x.acc_f32 == Cfg::ACC_F32 && x.bf16() == Cfg::BF16 && x.e4m3() == Cfg::E4M3 && x.block == block_scaled<Cfg>()
+  return x.acc_f32 == Cfg::ACC_F32 && x.bf16() == Cfg::BF16 && x.e4m3() == Cfg::E4M3 && x.block == block_scaled<Cfg>() &&
+                 x.block_1d1d == block_1d1d<Cfg>()
              ? GemmType(t) : gemm_type<Cfg>(t + 1);
 }
 
@@ -199,7 +206,8 @@ inline const DeviceInfo& device_info() {
 // rows hold K operand elements (K % 8 == 0 at two bytes, K % 16 == 0 at one byte), C rows N 16-bit elements. The scales
 // of a scaled variant are fp32 values in device memory: 4-byte aligned per tensor, 16-byte aligned vectors (M and N
 // values) rowwise, where the split-K reductions read the column scales as float4. Block scales: `a` 16-byte aligned (one
-// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned. Tile-list launches (launch_list):
+// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned (1 x 128 scales of Bt: 16-byte aligned,
+// one bulk copy per k-block too; launch() checks their ld_b). Tile-list launches (launch_list):
 // batches >= 1 matrices, a tile list of at most INT_MAX `tiles`, and its device array `list` (a batched launch's
 // optional row counts) 4-byte aligned. Grouped launches (validate_grouped) pass their offsets as `list`.
 inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K,
@@ -213,7 +221,8 @@ inline int validate(GemmType type, const void* A, const void* Bt, const void* C,
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bt) | reinterpret_cast<uintptr_t>(C)) & 15)
     return kBadAlignment;
   if (t.block) {
-    if ((reinterpret_cast<uintptr_t>(scales.a) & 15) || (reinterpret_cast<uintptr_t>(scales.b) & 3)) return kBadAlignment;
+    if ((reinterpret_cast<uintptr_t>(scales.a) & 15) || (reinterpret_cast<uintptr_t>(scales.b) & (t.block_1d1d ? 15 : 3)))
+      return kBadAlignment;
     if (ld_a < M || ld_a % 4) return kBadScaleLd;
     return kOk;
   }
@@ -452,6 +461,7 @@ struct LaunchArgs {
   uint64_t hint_a, hint_b;
   Scales scales;
   int ld_a;             // block scales: the row stride of scales.a
+  int ld_b;             // 1 x 128 scales of Bt (BlockScaled1D1D<>): the row stride of scales.b
   int batches;          // batched kernels: the batch count ...
   const int* masked_m;  // ... and the row counts per batch (null: dense); grouped kernels: G and the offsets
   cudaStream_t stream;
@@ -459,10 +469,11 @@ struct LaunchArgs {
   int act;              // ... and the activation code
 };
 
-// The kernel's last argument: the scales, or BiasAct<>'s BiasActArgs.
+// The kernel's last argument: the scales, BiasAct<>'s BiasActArgs or BlockScaled1D1D<>'s Block1D1DArgs.
 template <class Cfg>
 typename Cfg::EpiArgs epi_args(const LaunchArgs& a) {
   if constexpr (bias_act<Cfg>()) return BiasActArgs{a.scales, a.bias, a.act};
+  else if constexpr (block_1d1d<Cfg>()) return Block1D1DArgs{a.scales, a.ld_b};
   else return a.scales;
 }
 
@@ -547,16 +558,20 @@ constexpr int default_group_m() { return Cfg::CTA_GROUP == 2 ? 8 : 16; }
 // kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor or rowwise scales
 // of a scaled variant (device pointers), unused otherwise; `ld_a`: the row stride of block scales. RowMajorB<>
 // configurations read `Bt` as B [K, N] row-major. `scratch`: where the workspace of split-K and stream-K comes from.
-// BiasAct<> configurations: the bias (null, or N values of the output type) and the activation code.
+// BiasAct<> configurations: the bias (null, or N values of the output type) and the activation code. BlockScaled1D1D<>
+// configurations: `ld_b`, the row stride of Bt's 1 x 128 scales.
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
            int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0,
-           ScratchFn scratch = splitk_scratch, const void* bias = nullptr, int act = kActNone) {
+           ScratchFn scratch = splitk_scratch, const void* bias = nullptr, int act = kActNone, int ld_b = 0) {
   constexpr GemmType kType = gemm_type<Cfg>();
   int st = validate(kType, A, Bt, C, scales, M, N, K, ld_a);
   if (st != kOk) return st;
   if constexpr (bias_act<Cfg>()) {
     if ((st = validate_bias_act(bias, act)) != kOk) return st;
+  }
+  if constexpr (block_1d1d<Cfg>()) {
+    if (ld_b < N || ld_b % 4) return kBadScaleLdB;
   }
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
@@ -588,6 +603,7 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   a.c = static_cast<__half*>(C);
   a.scales = scales;
   a.ld_a = ld_a;
+  a.ld_b = ld_b;
   a.stream = stream;
   a.bias = bias;
   a.act = act;

@@ -56,7 +56,8 @@ constexpr int kSmemLimit = 232448;   // 227 KB of dynamic shared memory per bloc
 // How a launch divides K. The kernel is compiled once per (configuration, mode), so that the plain schedule — nearly
 // every launch — carries none of the three other epilogues.
 enum KMode : int { kPlain = 0, kWorkspaceSplitK = 1, kClusterSplitK = 2, kStreamK = 3 };
-struct Scales;   // the epilogue arguments of every configuration but BiasAct<>'s (below)
+struct Scales;   // the epilogue arguments of every configuration but BiasAct<>'s and BlockScaled1D1D<>'s (below)
+struct Block1D1DArgs;
 
 template <int BN_, int STAGES_, int CTA_GROUP_, bool ACC_F32_, int CLUSTER_M_ = 1, int CLUSTER_N_ = 1, int M_REP_ = 1, bool BF16_ = false,
           bool E4M3_ = false>
@@ -101,9 +102,10 @@ struct Config {
   // which K-decompositions this configuration's kernel carries
   static constexpr bool STREAM_K = CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
   static constexpr bool SPLIT_K = STREAM_K && CTA_GROUP_ == 1;
-  // the variant wrappers below (BlockScaled<>, Batched<>, Grouped<>, RowMajorB<>, GroupedK<>, BiasAct<>) override these
+  // the variant wrappers below (BlockScaled<>, BlockScaled1D1D<>, Batched<>, Grouped<>, RowMajorB<>, GroupedK<>,
+  // BiasAct<>) override these
   static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false, ROW_MAJOR_B = false, K_GROUPED = false,
-                        BIAS_ACT = false;
+                        BIAS_ACT = false, BLOCK_1D1D = false;
   using Cursor = NoBatches;   // the flat tile list the kernel walks (hgemm_schedule.cuh): none
   using EpiArgs = Scales;     // the kernel's last parameter
   static constexpr int EPI_BYTES = 8 * EPI_ROWS * 64 * 2;    // 8 consumer warps x one staging buffer (sized for EPI_N = 64)
@@ -150,6 +152,30 @@ struct BlockScaled : Base {
 };
 template <class Cfg>
 __host__ __device__ constexpr bool block_scaled() { return Cfg::BLOCK_SCALED; }
+
+// Block-scaled e4m3 with 1 x 128 scales on both operands (libb200_fp8block_1d1d.so, the weight gradient of blockwise
+// FP8 training, dW = q(dY^T) q(X^T)^T, whose two operands are transposed activations): Bt's scales are one per (row of
+// Bt, 128-element k-block), N-major like A's, value (n, kb) at b[kb * ld_b + n]. BlockScaled<>'s main loop and
+// schedules; the promotion forms s = fp32(sa(m, kb) * sb(n, kb)) per element. Each ring stage's scale slice holds
+// CTA_M values of A's scales and then BN of Bt's, each one 1-D bulk copy counted in the stage's transaction bytes (rows
+// clamped at ld_a / ld_b, so a CTA past them loads none); the ring depth is recomputed for the larger stage. ld_b
+// travels in the kernel's Block1D1DArgs (hgemm_block_1d1d_kernel), not in Scales. A wrapper of its own, so that
+// BlockScaled<>'s kernels, and the other variants', stay as they are.
+template <class Base>
+struct BlockScaled1D1D : BlockScaled<Base> {
+  static constexpr bool BLOCK_1D1D = true;
+  using EpiArgs = Block1D1DArgs;
+  static constexpr int SA_WINDOW_BYTES = Base::CTA_M * 4;   // A's scales of a stage; Bt's BN values follow them
+  static constexpr int SCALE_STAGE_BYTES = SA_WINDOW_BYTES + Base::BN * 4;
+  static constexpr int MAX_STAGES =
+      (kSmemLimit - 1024 - Base::EPI_BYTES - Base::BAR_BYTES) / (Base::STAGE_BYTES + SCALE_STAGE_BYTES);
+  static constexpr int STAGES = Base::STAGES < MAX_STAGES ? Base::STAGES : MAX_STAGES;
+  static constexpr int SMEM_BYTES = Base::SMEM_BYTES + STAGES * SCALE_STAGE_BYTES - (Base::STAGES - STAGES) * Base::STAGE_BYTES;
+  static_assert(STAGES >= 2 && SMEM_BYTES <= kSmemLimit, "1D1D block-scaled ring does not fit");
+  static_assert(SA_WINDOW_BYTES % 16 == 0 && SCALE_STAGE_BYTES % 16 == 0, "bulk copies need 16-byte aligned slices");
+};
+template <class Cfg>
+__host__ __device__ constexpr bool block_1d1d() { return Cfg::BLOCK_1D1D; }
 
 // Batched 16-bit GEMM, C[b] = A[b] Bt[b]^T (libb200_batched.so): A, Bt and C are 3-D tensor maps whose third
 // coordinate is the batch, so a tile's loads are zero-filled and its stores clipped at its own matrix's edge, and a
@@ -310,6 +336,17 @@ template <class Cfg>
 __host__ __device__ constexpr bool bias_act() { return Cfg::BIAS_ACT; }
 __host__ __device__ __forceinline__ const Scales& scales_of(const Scales& s) { return s; }
 __host__ __device__ __forceinline__ const Scales& scales_of(const BiasActArgs& e) { return e.scales; }
+
+// The epilogue arguments of the BlockScaled1D1D<> kernels (hgemm_block_1d1d_kernel): the scales, and the row stride of
+// Bt's (ld_b >= N, ld_b % 4 == 0, `scales.b` 16-byte aligned).
+struct Block1D1DArgs { Scales scales; int ld_b; };
+__host__ __device__ __forceinline__ const Scales& scales_of(const Block1D1DArgs& e) { return e.scales; }
+// ld_b of a kernel's EpiArgs: 0 for the kernels without it
+template <class E>
+__host__ __device__ __forceinline__ int ld_b_of(const E& e) {
+  if constexpr (std::is_same_v<E, Block1D1DArgs>) return e.ld_b;
+  else return 0;
+}
 
 // act(z) in fp32; `act` is warp-uniform. relu: max(z, +0.0) (+0.0 for -0.0 and NaN). gelu_tanh: 0.5 z (1 + tanhf(u)),
 // u = sqrt(2/pi) (z + 0.044715 z^3), torch's tanh approximation (F.gelu(approximate="tanh"), _addmm_activation), each
@@ -872,7 +909,7 @@ hgemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,   // A  [M,K]  box {
                 __half* __restrict__ c_raw,       // C base pointer, used by the split-K reductions' direct stores
                 uint64_t hint_a, uint64_t hint_b, // L2 eviction priority of the A / B loads (ptx::kL2Evict*)
                 Scales scales                     /* e4m3: the per-tensor scales (not read by the 16-bit kernels) */) {
-  static_assert(!bias_act<Cfg>(), "BiasAct<> configurations: hgemm_bias_act_kernel");
+  static_assert(!bias_act<Cfg>() && !block_1d1d<Cfg>(), "BiasAct<> and BlockScaled1D1D<>: kernels of their own");
   const Scales& epi = scales;
 #include "hgemm_tn_kernel_body.inc"
 }
@@ -889,10 +926,24 @@ hgemm_bias_act_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
 #include "hgemm_tn_kernel_body.inc"
 }
 
+// The same with 1 x 128 scales on both operands (BlockScaled1D1D<>): the parameters of hgemm_tn_kernel, Block1D1DArgs
+// last.
+template <class Cfg, int KMODE = kPlain>
+__global__ void __launch_bounds__(kNumThreads, 1)
+hgemm_block_1d1d_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                        const __grid_constant__ CUtensorMap tmap_c, int M, int N, int K, int group_m, int splits_arg,
+                        int aux_arg, float* __restrict__ splitk_ws, unsigned* __restrict__ splitk_ctr,
+                        __half* __restrict__ c_raw, uint64_t hint_a, uint64_t hint_b, Block1D1DArgs epi) {
+  static_assert(block_1d1d<Cfg>(), "a BlockScaled1D1D<> configuration");
+  const Scales& scales = epi.scales;
+#include "hgemm_tn_kernel_body.inc"
+}
+
 // The kernel of (Cfg, KMODE).
 template <class Cfg, int KMODE>
 constexpr auto kernel_of() {
   if constexpr (bias_act<Cfg>()) return &hgemm_bias_act_kernel<Cfg, KMODE>;
+  else if constexpr (block_1d1d<Cfg>()) return &hgemm_block_1d1d_kernel<Cfg, KMODE>;
   else return &hgemm_tn_kernel<Cfg, KMODE>;
 }
 

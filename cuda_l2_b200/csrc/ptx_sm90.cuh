@@ -250,6 +250,12 @@ __device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
   return v;
 }
+// two floats (addr 8-byte aligned), read after an mbarrier wait like ld_shared_f32
+__device__ __forceinline__ float2 ld_shared_v2f(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
 __device__ __forceinline__ void st_shared_v2f(uint32_t addr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }

@@ -618,6 +618,8 @@ def _fp8_gemm_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, *, stream):
     granularity = capi.scale_granularity(m, n, scale_a, scale_b, k=k)
     if granularity == "blockwise":
         scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
+    elif granularity == "blockwise_1d1d":
+        scale_a, scale_b = _m_major(scale_a), _m_major(scale_b)
     elif granularity == "rowwise":
         scale_a, scale_b = _rowwise_scale_arg(scale_a), _rowwise_scale_arg(scale_b)
     else:
@@ -634,13 +636,15 @@ def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, sca
              out_dtype: torch.dtype = torch.float16) -> torch.Tensor:
     """(``a`` [M,K] @ ``b_kmajor`` [N,K]^T), scaled, -> [M,N] ``out_dtype``, e4m3 operands (see the module docstring).
     Per-tensor scales: one element each. Rowwise scales: ``scale_a`` [M,1], ``scale_b`` [1,N]. Blockwise scales:
-    ``scale_a`` [M, ceil(K/128)] in any layout, ``scale_b`` [ceil(N/128), ceil(K/128)]."""
+    ``scale_a`` [M, ceil(K/128)] in any layout, ``scale_b`` [ceil(N/128), ceil(K/128)]. 1 x 128 scales on both
+    operands (the weight gradient of blockwise FP8 training): ``scale_a`` [M, ceil(K/128)] and ``scale_b``
+    [N, ceil(K/128)], each in any layout (the M-major one of :func:`quantize_e4m3_blockwise` is read in place)."""
     return torch.ops.cuda_l2_b200.fp8_gemm(a, b_kmajor, scale_a, scale_b, out_dtype)
 
 
 def _fp8_bias_act_shape(a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype):
     m, n, k = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
-    if capi.scale_granularity(m, n, scale_a, scale_b, k=k) == "blockwise":
+    if capi.scale_granularity(m, n, scale_a, scale_b, k=k) in ("blockwise", "blockwise_1d1d"):
         raise capi.B200HgemmError("fp8_gemm_bias_act: blockwise scales have no bias + activation kernel (per-tensor or "
                                   "rowwise scales only; run fp8_gemm and add the bias)")
     capi.check_bias(bias, n, out_dtype)
@@ -1005,6 +1009,89 @@ def quantize_e4m3_rowwise_dual(x: torch.Tensor) -> tuple[torch.Tensor, torch.Ten
     return quantize_e4m3_rowwise_dual_reference(x)
 
 
+# ------------------------------------------------------------------------------------------ blockwise FP8 training
+#                                                                                            (libb200_quant_block_dual.so)
+# The DeepSeek-V3 recipe: x and dY get one scale per token and 128 channels, W one per 128 x 128 block. A 128 x 128 tile
+# holds complete groups in both orientations, so one launch writes both e4m3 copies of a tensor. These quantisers are
+# plain functions, not operators: the blockwise training path is not traceable by FakeTensor or torch.compile.
+def quantize_e4m3_blockwise_dual_reference(x: torch.Tensor
+                                           ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """:func:`quantize_e4m3_blockwise_dual` as a composition of torch ops: :func:`quantize_e4m3_blockwise_reference`
+    of ``x`` and of ``x^T`` zero-padded to a multiple of 16 columns."""
+    if x.dim() != 2:
+        raise capi.B200HgemmError(f"quantize_e4m3_blockwise_dual takes [rows, cols], got {list(x.shape)}")
+    rows = x.shape[0]
+    q, scale = quantize_e4m3_blockwise_reference(x)
+    q_t, scale_t = quantize_e4m3_blockwise_reference(
+        nn.functional.pad(x.t(), (0, capi.dual_ld_t(rows) - rows)).contiguous())
+    return q, scale, q_t, scale_t
+
+
+def _block_dual_routed(x: torch.Tensor) -> bool:
+    """Whether libb200_quant_block_dual.so runs on ``x``: a non-empty 2-D fp16 / bf16 CUDA tensor."""
+    return x.dim() == 2 and _quant_routed(x, silu_mul=True)
+
+
+def quantize_e4m3_blockwise_dual(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Both 1 x 128 quantisations of a 2-D ``x`` [rows, cols] on its device: ``(q, scale, q_t, scale_t)``, where ``q``
+    [rows, cols] and ``scale`` [rows, ceil(cols/128)] are :func:`quantize_e4m3_blockwise`'s, and ``q_t`` [cols, ld_t]
+    and ``scale_t`` [cols, ceil(rows/128)] are the same for ``x^T`` zero-padded to ``ld_t`` = rows rounded up to 16
+    columns: a K-major FP8 GEMM operand whose reduction runs along x's rows, scaled per 128 of them. Both scales come
+    back in the M-major layout the block-scaled GEMMs read in place. A padding byte is e4m3(0 / s), 0x00 unless the
+    group's scale is NaN. A non-empty CUDA fp16 / bf16 tensor runs one launch of libb200_quant_block_dual.so on the
+    current stream (x read once), anything else :func:`quantize_e4m3_blockwise_dual_reference`, with the same bits. Not
+    an operator: FakeTensor and torch.compile cannot trace it."""
+    if not _block_dual_routed(x):
+        return quantize_e4m3_blockwise_dual_reference(x)
+    rows, cols = x.shape
+    q = x.new_empty((rows, cols), dtype=torch.float8_e4m3fn)
+    q_t = x.new_empty((cols, capi.dual_ld_t(rows)), dtype=torch.float8_e4m3fn)
+    scale = _blockwise_scale((), rows, capi.num_k_blocks(cols), x.device)
+    scale_t = _blockwise_scale((), cols, capi.num_k_blocks(rows), x.device)
+    with torch.cuda.device(x.device):
+        capi.quantize_e4m3_blockwise_dual(x.contiguous(), q, scale, q_t, scale_t,
+                                          stream=torch.cuda.current_stream(x.device).cuda_stream)
+    return q, scale, q_t, scale_t
+
+
+def quantize_e4m3_block128x128_dual_reference(w: torch.Tensor
+                                              ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """:func:`quantize_e4m3_block128x128_dual` as a composition of torch ops: :func:`quantize_e4m3_block128x128` and
+    its transpose."""
+    if w.dim() != 2:
+        raise capi.B200HgemmError(f"quantize_e4m3_block128x128_dual takes [rows, cols], got {list(w.shape)}")
+    q, scale = quantize_e4m3_block128x128(w)
+    return q, scale, q.t().contiguous(), scale.t().contiguous()
+
+
+def quantize_e4m3_block128x128_dual(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Both 128 x 128 block quantisations of a weight ``w`` [N, K] on its device: ``(q, scale, q_t, scale_t)`` with
+    ``q`` [N, K] and ``scale`` [ceil(N/128), ceil(K/128)] those of :func:`quantize_e4m3_block128x128`, ``q_t`` = q^T
+    [K, N] and ``scale_t`` = scale^T (with 128 x 128 blocks, the quantisation of w^T is the transpose of that of w, bit
+    for bit). A non-empty CUDA fp16 / bf16 tensor runs one launch of libb200_quant_block_dual.so on the current stream,
+    anything else :func:`quantize_e4m3_block128x128_dual_reference`, with the same bits. Not an operator."""
+    if not _block_dual_routed(w):
+        return quantize_e4m3_block128x128_dual_reference(w)
+    n, k = w.shape
+    nnb, nkb = -(-n // capi.BLOCK), capi.num_k_blocks(k)
+    q = w.new_empty((n, k), dtype=torch.float8_e4m3fn)
+    q_t = w.new_empty((k, n), dtype=torch.float8_e4m3fn)
+    scale = w.new_empty((nnb, nkb), dtype=torch.float32)
+    scale_t = w.new_empty((nkb, nnb), dtype=torch.float32)
+    with torch.cuda.device(w.device):
+        capi.quantize_e4m3_block128x128_dual(w.contiguous(), q, scale, q_t, scale_t,
+                                             stream=torch.cuda.current_stream(w.device).cuda_stream)
+    return q, scale, q_t, scale_t
+
+
+FP8_TRAIN_GRANULARITIES = ("rowwise", "blockwise")
+
+
+def _check_fp8_train_granularity(granularity: str) -> None:
+    if granularity not in FP8_TRAIN_GRANULARITIES:
+        raise capi.B200HgemmError(f"granularity must be one of {FP8_TRAIN_GRANULARITIES}, got {granularity!r}")
+
+
 def _check_fp8_linear(in_features: int, out_features: int, dtype: torch.dtype, what) -> None:
     """The rules of :func:`fp8_linear`'s three GEMMs: fp16 / bf16, and in_features and out_features multiples of 16
     (each is the reduction of one of them, and e4m3 rows must be 16 bytes)."""
@@ -1067,24 +1154,90 @@ class _Fp8LinearFunction(torch.autograd.Function):
         return grad_x, grad_w
 
 
-def fp8_linear(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+class _Fp8BlockwiseLinearFunction(torch.autograd.Function):
+    """y = x W^T with a gradient in the blockwise recipe: x and dY quantised per token and 128 channels, W per 128 x 128
+    block, every k-block of every product promoted into an fp32 accumulator. The forward saves the transposed e4m3
+    copies its backward reads, not x and W, and only those of the gradients that will be asked for."""
+
+    @staticmethod
+    def forward(ctx, x2, weight):
+        need_x, need_w = ctx.needs_input_grad[:2]
+        ctx.shapes = (x2.shape, weight.shape)
+        ctx.dtypes = (x2.dtype, weight.dtype)
+        if x2.shape[0] == 0:
+            ctx.save_for_backward()
+            return x2.new_empty((0, weight.shape[0]))
+        # dW = q(dY^T) q(X^T)^T needs X transposed; dX = q(dY) q(W^T)^T needs W transposed
+        if need_w:
+            x_q, x_s, x_qt, x_st = quantize_e4m3_blockwise_dual(x2)
+        else:
+            x_q, x_s = quantize_e4m3_blockwise(x2)
+            x_qt = x_st = None
+        if need_x:
+            w_q, w_s, w_qt, w_st = quantize_e4m3_block128x128_dual(weight)
+        else:
+            w_q, w_s = quantize_e4m3_block128x128(weight)
+            w_qt = w_st = None
+        ctx.save_for_backward(x_qt, x_st, w_qt, w_st)
+        return torch.ops.cuda_l2_b200.fp8_gemm(x_q, w_q, x_s, w_s, x2.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        (x_shape, w_shape), (x_dtype, w_dtype) = ctx.shapes, ctx.dtypes
+        need_x, need_w = ctx.needs_input_grad[:2]
+        grad_x = grad_w = None
+        if x_shape[0] == 0:
+            if need_x:
+                grad_x = grad_y.new_empty(x_shape, dtype=x_dtype)
+            if need_w:
+                grad_w = grad_y.new_zeros(w_shape, dtype=w_dtype)
+            return grad_x, grad_w
+        x_qt, x_st, w_qt, w_st = ctx.saved_tensors
+        g = grad_y.contiguous()
+        gemm = torch.ops.cuda_l2_b200.fp8_gemm
+        if need_w:
+            g_q, g_s, g_qt, g_st = quantize_e4m3_blockwise_dual(g)
+            grad_w = gemm(g_qt, x_qt, g_st, x_st, w_dtype)   # [N, ld_t(M)] x [K, ld_t(M)], 1 x 128 scales on both -> [N, K]
+        else:
+            g_q, g_s = quantize_e4m3_blockwise(g)
+        if need_x:
+            grad_x = gemm(g_q, w_qt, g_s, w_st, x_dtype)     # [M, N] x [K, N], 128 x 128 scales of W^T -> [M, K]
+        return grad_x, grad_w
+
+
+def fp8_linear(x: torch.Tensor, weight: torch.Tensor, granularity: str = "rowwise") -> torch.Tensor:
     """``x @ weight^T`` for ``x`` [..., K] and ``weight`` [N, K] of one dtype (fp16 or bf16), K % 16 == 0 and
-    N % 16 == 0, in FP8 with a gradient: x and W are quantised to e4m3 with one fp32 scale per row (per token, per
-    output channel) and multiplied by ``fp8_gemm`` into x's dtype. The backward quantises dY the same way and runs two
-    more ``fp8_gemm`` calls, dX = dY W (scales per token and per input channel) and dW = dY^T X (both operands scaled
-    along the tokens), from the transposed e4m3 copies of W and x that the forward kept. Every product accumulates in
-    the FP8 tensor cores' fast mode. Without a gradient to compute, the forward is ``B200Fp8Linear``'s rowwise one, bit
-    for bit. No host synchronisation: a forward and backward can be captured in one CUDA graph."""
+    N % 16 == 0, in FP8 with a gradient.
+
+    ``granularity="rowwise"``: x and W are quantised to e4m3 with one fp32 scale per row (per token, per output
+    channel) and multiplied by ``fp8_gemm`` into x's dtype. The backward quantises dY the same way and runs two more
+    ``fp8_gemm`` calls, dX = dY W (scales per token and per input channel) and dW = dY^T X (both operands scaled along
+    the tokens), from the transposed e4m3 copies of W and x that the forward kept. Every product accumulates in the FP8
+    tensor cores' fast mode. Without a gradient to compute, the forward is ``B200Fp8Linear``'s rowwise one, bit for
+    bit. No host synchronisation: a forward and backward can be captured in one CUDA graph.
+
+    ``granularity="blockwise"`` (the DeepSeek-V3 recipe): x and dY get one scale per token and 128 channels, W one per
+    128 x 128 block, and every 128-wide k-block of the three products is promoted into an fp32 accumulator. y and dX
+    are block-scaled ``fp8_gemm`` calls; dW = q(dY^T) q(X^T)^T reduces over the tokens with 1 x 128 scales on both
+    operands, so one outlier token squeezes only its own 128-token group. Both orientations of x, dY and W come from
+    one launch each (:func:`quantize_e4m3_blockwise_dual`, :func:`quantize_e4m3_block128x128_dual`). Without a
+    gradient to compute, the forward is ``B200Fp8Linear``'s blockwise one, bit for bit. Also no host synchronisation;
+    its quantisers are not operators, so this path is not traceable by FakeTensor or torch.compile."""
     if x.dim() == 0 or weight.dim() != 2 or x.shape[-1] != weight.shape[1] or x.dtype != weight.dtype:
         raise capi.B200HgemmError(f"fp8_linear: x [..., K] and weight [N, K] of one dtype expected, got "
                                   f"{x.dtype} {tuple(x.shape)} and {weight.dtype} {tuple(weight.shape)}")
+    _check_fp8_train_granularity(granularity)
     n, k = weight.shape
     _check_fp8_linear(k, n, weight.dtype, f"a [{n}, {k}] weight")
     x2 = x.reshape(-1, k)
+    blockwise = granularity == "blockwise"
     if torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad):
-        y = _Fp8LinearFunction.apply(x2, weight)
+        y = (_Fp8BlockwiseLinearFunction if blockwise else _Fp8LinearFunction).apply(x2, weight)
     elif x2.shape[0] == 0:
         y = x2.new_empty((0, n))
+    elif blockwise:
+        (x_q, x_s), (w_q, w_s) = quantize_e4m3_blockwise(x2), quantize_e4m3_block128x128(weight)
+        y = torch.ops.cuda_l2_b200.fp8_gemm(x_q, w_q, x_s, w_s, x.dtype)
     else:
         (x_q, x_s), (w_q, w_s) = quantize_e4m3_rowwise(x2), quantize_e4m3_rowwise(weight)
         y = torch.ops.cuda_l2_b200.fp8_gemm(x_q, w_q, x_s, w_s.reshape(1, n), x.dtype)
@@ -1093,15 +1246,17 @@ def fp8_linear(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
 
 class B200Fp8TrainLinear(nn.Module):
     """``nn.Linear`` trained in FP8: a trainable 16-bit ``weight`` [out_features, in_features] (and optional ``bias``),
-    the product run by :func:`fp8_linear` (rowwise-scaled e4m3 forward and backward), the bias added by torch after it
-    as :class:`B200Linear` does. In eval or no-grad mode the output is :class:`B200Fp8Linear`'s rowwise one, bit for
-    bit. Needs fp16 / bf16 and in_features % 16 == 0, out_features % 16 == 0."""
+    the product run by :func:`fp8_linear` with ``granularity`` ("rowwise", the default, or "blockwise": e4m3 forward and
+    backward with those scales), the bias added by torch after it as :class:`B200Linear` does. In eval or no-grad mode
+    the output is :class:`B200Fp8Linear`'s of the same granularity, bit for bit. Needs fp16 / bf16 and
+    in_features % 16 == 0, out_features % 16 == 0."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True, device=None,
-                 dtype: torch.dtype = torch.bfloat16):
+                 dtype: torch.dtype = torch.bfloat16, granularity: str = "rowwise"):
         super().__init__()
         _check_fp8_linear(in_features, out_features, dtype, "B200Fp8TrainLinear")
-        self.in_features, self.out_features = in_features, out_features
+        _check_fp8_train_granularity(granularity)
+        self.in_features, self.out_features, self.granularity = in_features, out_features, granularity
         self.weight = nn.Parameter(torch.empty((out_features, in_features), device=device, dtype=dtype))
         self.bias = nn.Parameter(torch.empty(out_features, device=device, dtype=dtype)) if bias else None
         self.reset_parameters()
@@ -1109,23 +1264,25 @@ class B200Fp8TrainLinear(nn.Module):
     reset_parameters = B200Linear.reset_parameters
 
     @classmethod
-    def from_linear(cls, lin: nn.Linear) -> "B200Fp8TrainLinear":
+    def from_linear(cls, lin: nn.Linear, granularity: str = "rowwise") -> "B200Fp8TrainLinear":
         """A layer sharing ``lin``'s Parameters (no copy), as :meth:`B200Linear.from_linear`."""
         _check_fp8_linear(lin.in_features, lin.out_features, lin.weight.dtype, lin)
+        _check_fp8_train_granularity(granularity)
         new = cls.__new__(cls)
         nn.Module.__init__(new)
-        new.in_features, new.out_features = lin.in_features, lin.out_features
+        new.in_features, new.out_features, new.granularity = lin.in_features, lin.out_features, granularity
         new.weight, new.bias = lin.weight, lin.bias          # shared storage, no copy
         return new
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        y = fp8_linear(x, self.weight)
+        y = fp8_linear(x, self.weight, self.granularity)
         if self.bias is not None:
             y = y + self.bias
         return y
 
     def extra_repr(self) -> str:
-        return f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}"
+        return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
+                f"granularity={self.granularity}")
 
 
 # ------------------------------------------------------------------------------------------ grouped FP8 (libb200_grouped_fp8.so)
@@ -1330,4 +1487,5 @@ __all__ = ["hgemm", "hgemm_nn", "hgemm_batched", "hgemm_grouped", "hgemm_grouped
            "grouped_linear", "B200GroupedLinear", "B200Linear", "replace_linear_modules", "linear_supported", "fp8_gemm", "quantize_e4m3",
            "quantize_e4m3_rowwise", "quantize_e4m3_blockwise", "quantize_e4m3_block128x128", "B200Fp8Linear",
            "fp8_grouped_gemm", "fp8_batched_gemm", "B200Fp8GroupedLinear", "silu_mul_quantize_e4m3_blockwise",
-           "B200Fp8GroupedMLP", "quantize_e4m3_rowwise_dual", "fp8_linear", "B200Fp8TrainLinear"]
+           "B200Fp8GroupedMLP", "quantize_e4m3_rowwise_dual", "fp8_linear", "B200Fp8TrainLinear",
+           "quantize_e4m3_blockwise_dual", "quantize_e4m3_block128x128_dual"]

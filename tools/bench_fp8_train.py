@@ -21,8 +21,15 @@ graph (replayed):
   fp8_torch  the same step with the torch quantisers (the composition, x.t() padded and quantised): the "before";
   b200_bf16  B200Linear (hgemm with its gradient);
   torch_bf16 nn.Linear (cuBLAS).
-fp8 and fp8_torch are checked bit for bit (y, dX, dW, db) before timing. The card and its power limit are recorded with
-the results. Needs an H100; there is no CPU path.
+  fp8_blockwise  B200Fp8TrainLinear(granularity="blockwise") (dual block quantisers, two block-scaled fp8_gemm calls
+             and one with 1 x 128 scales on both operands);
+fp8 and fp8_torch are checked bit for bit (y, dX, dW, db) before timing.
+
+Blockwise legs: the dual 1 x 128 quantiser (ops.quantize_e4m3_blockwise_dual, one launch, x read once) at the quantiser
+shapes, its kernel time from torch.profiler (b200_quant_block_dual_*) and its bandwidth; and the weight gradient of each
+step shape, dW [out, in] = dY^T [out, T] x X^T [in, T], run by the 1 x 128 x 1 x 128 kernel and by the 128 x 128 kernel
+on the same e4m3 operands (Bt's scales per 128 x 128 block), alternating, as TFLOP/s. The card and its power limit are
+recorded with the results. Needs an H100; there is no CPU path.
 """
 from __future__ import annotations
 
@@ -38,7 +45,7 @@ sys.path.insert(0, str(REPO / "tools"))
 import torch  # noqa: E402
 
 from bench_nn import alternate, card  # noqa: E402
-from cuda_l2_b200 import ops  # noqa: E402
+from cuda_l2_b200 import capi, ops  # noqa: E402
 
 HBM_TBPS = 3.35   # H100 SXM data sheet
 QUANT_SHAPES = [(2048, 4096), (4096, 11008), (11008, 4096), (16384, 7168)]
@@ -52,8 +59,16 @@ def dual_bytes(rows: int, cols: int) -> int:
     return 2 * rows * cols * 2 + rows * cols + cols * ld_t + 4 * (rows + cols)
 
 
-def kernel_us(fn, calls: int) -> float:
-    """Device time of libb200_quant_dual.so's kernels and the workspace memset per call of ``fn`` (torch.profiler)."""
+def block_dual_bytes(rows: int, cols: int) -> int:
+    """Algorithmic bytes of one dual 1 x 128 quantisation of bf16 [rows, cols]: x read once, e4m3 written in both
+    orientations (q_t with its padding), fp32 scales once each."""
+    ld_t = -(-rows // 16) * 16
+    return rows * cols * 2 + rows * cols + cols * ld_t + 4 * (rows * -(-cols // 128) + cols * -(-rows // 128))
+
+
+def kernel_us(fn, calls: int, key: str = "b200_quant_dual_", memset: bool = True) -> float:
+    """Device time of the kernels whose names contain ``key`` (and, with ``memset``, the workspace memsets) per call of
+    ``fn`` (torch.profiler)."""
     from torch.profiler import ProfilerActivity, profile
 
     fn()
@@ -63,7 +78,7 @@ def kernel_us(fn, calls: int) -> float:
             fn()
         torch.cuda.synchronize()
     total = sum(ev.device_time_total for ev in prof.key_averages()
-                if "b200_quant_dual_" in ev.key or ev.key.lower().startswith("memset"))
+                if key in ev.key or (memset and ev.key.lower().startswith("memset")))
     return total / calls
 
 
@@ -90,11 +105,12 @@ def step_legs(t: int, k: int, n: int, seed: int) -> dict:
     g = torch.Generator(device="cuda").manual_seed(seed)
     lin = torch.nn.Linear(k, n, device="cuda", dtype=torch.bfloat16)
     fp8 = ops.B200Fp8TrainLinear.from_linear(lin)
+    fp8_blockwise = ops.B200Fp8TrainLinear.from_linear(lin, granularity="blockwise")
     b200 = ops.B200Linear.from_linear(lin)
     x = torch.randn((t, k), device="cuda", generator=g).bfloat16().requires_grad_()
     gy = torch.randn((t, n), device="cuda", generator=g).bfloat16()
     forwards = {"fp8": fp8, "fp8_torch": lambda a: _TorchQuantFp8Linear.apply(a, lin.weight) + lin.bias,
-                "b200_bf16": b200, "torch_bf16": lin}
+                "fp8_blockwise": fp8_blockwise, "b200_bf16": b200, "torch_bf16": lin}
 
     def eager(fwd):
         def step():
@@ -127,6 +143,24 @@ def step_legs(t: int, k: int, n: int, seed: int) -> dict:
     return legs
 
 
+def wgrad_legs(t: int, k: int, n: int, seed: int) -> tuple[dict, float]:
+    """dW = dY^T X of a step shape on e4m3 operands from the dual 1 x 128 quantiser: the 1 x 128 x 1 x 128 kernel, and
+    the 128 x 128 kernel with X^T's scales taken per 128 x 128 block (their maxima); and the product's FLOPs."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    _, _, gqt, gst = ops.quantize_e4m3_blockwise_dual(torch.randn((t, n), device="cuda", generator=g).bfloat16())
+    _, _, xqt, xst = ops.quantize_e4m3_blockwise_dual(torch.randn((t, k), device="cuda", generator=g).bfloat16())
+    nkb = xst.shape[1]
+    pad = torch.zeros((-(-k // 128) * 128, nkb), device="cuda")
+    pad[:k] = xst
+    xst_block = pad.view(-1, 128, nkb).amax(1).contiguous()
+    one_d = torch.empty((n, k), dtype=torch.bfloat16, device="cuda")
+    block = torch.empty_like(one_d)
+    legs = {"1x128_1x128": lambda: capi.fp8_gemm(gqt, xqt, one_d, gst, xst, stream=torch.cuda.current_stream().cuda_stream),
+            "1x128_128x128": lambda: capi.fp8_gemm(gqt, xqt, block, gst, xst_block,
+                                                   stream=torch.cuda.current_stream().cuda_stream)}
+    return legs, 2.0 * n * k * gqt.shape[1]
+
+
 def main() -> int:
     p = argparse.ArgumentParser()
     p.add_argument("--rounds", type=int, default=7)
@@ -138,7 +172,7 @@ def main() -> int:
         raise SystemExit("bench_fp8_train.py needs an H100 (compute capability 9.0)")
     torch.cuda.set_device(0)
     result = {"card": card(), "rounds": args.rounds, "hbm_tbps_datasheet": HBM_TBPS, "dual_quantiser": {},
-              "step": {}}
+              "block_dual_quantiser": {}, "wgrad": {}, "step": {}}
     g = torch.Generator(device="cuda").manual_seed(1)
     for rows, cols in QUANT_SHAPES:
         x = torch.randn((rows, cols), device="cuda", generator=g).bfloat16()
@@ -160,6 +194,35 @@ def main() -> int:
             times["share_of_hbm"] = nbytes / (us * 1e-6) / (HBM_TBPS * 1e12)
         result["dual_quantiser"][f"{rows}x{cols}"] = times
         del x, fns
+        torch.cuda.empty_cache()
+    for rows, cols in QUANT_SHAPES:
+        x = torch.randn((rows, cols), device="cuda", generator=g).bfloat16()
+        fns = {"kernel": lambda a=x: ops.quantize_e4m3_blockwise_dual(a),
+               "torch": lambda a=x: ops.quantize_e4m3_blockwise_dual_reference(a)}
+        for got, want in zip(fns["kernel"](), fns["torch"]()):
+            dt = torch.uint8 if got.dtype == torch.float8_e4m3fn else torch.int32
+            assert torch.equal(got.view(dt), want.view(dt)), (rows, cols)
+        nbytes = block_dual_bytes(rows, cols)
+        times = alternate(fns, args.rounds, args.ms)
+        for v in times.values():
+            v["us"] = v["ms"] * 1e3
+        times["bytes"] = nbytes
+        if not args.no_profile:
+            us = kernel_us(fns["kernel"], 50, "b200_quant_block_dual_", memset=False)
+            times["kernel_us"] = us
+            times["kernel_gbps"] = nbytes / (us * 1e-6) / 1e9
+            times["share_of_hbm"] = nbytes / (us * 1e-6) / (HBM_TBPS * 1e12)
+        result["block_dual_quantiser"][f"{rows}x{cols}"] = times
+        del x, fns
+        torch.cuda.empty_cache()
+    for t, k, n in STEP_SHAPES:
+        legs, flops = wgrad_legs(t, k, n, seed=t + k + n)
+        times = alternate(legs, args.rounds, args.ms)
+        for v in times.values():
+            v["us"] = v["ms"] * 1e3
+            v["tflops"] = flops / (v["ms"] * 1e-3) * 1e-12
+        result["wgrad"][f"{n}x{k}x{t}"] = times
+        del legs
         torch.cuda.empty_cache()
     for t, k, n in STEP_SHAPES:
         legs = step_legs(t, k, n, seed=t + k + n)
