@@ -76,10 +76,21 @@ LATE_LEG_LISTS = {"nn_fp16": ("grid", "offgrid"), "nn_bf16": ("grid",), "nn_fp16
 EPI_VARIANTS = {"epi_fp16": 0, "epi_bf16": 2, "epi_e4m3_tensor_fp16": 3, "epi_e4m3_rowwise_bf16": 4}   # b200_epilogue.h
 ACTIVATIONS = ("none", "relu", "gelu_tanh")
 
+# The legs of the GEMM with 1 x 128 scales on both operands (the weight gradient of blockwise FP8 training,
+# test_gpu_fp8_train_exact.py), kept apart like NN_LEGS: one output type on the grid, the other off it. Same fields.
+TRAIN_LEGS = {
+    "e4m3_1d1d_fp16": dict(operand="e4m3", out="fp16", acc="fp32", scales="block_1d1d", k_div=2, k_align=16),
+    "e4m3_1d1d_bf16": dict(operand="e4m3", out="bf16", acc="fp32", scales="block_1d1d", k_div=2, k_align=16),
+}
+TRAIN_LEG_LISTS = {"e4m3_1d1d_fp16": ("grid",), "e4m3_1d1d_bf16": ("offgrid",)}
+# weight-gradient samples dW [out_features, in_features] = dY^T X over T tokens: K = dual_ld_t(T), T off 128 and 16
+DW_FEATURES = ((4096, 4096), (11008, 4096), (4096, 11008), (14336, 4096), (768, 3072), (1024, 4096))
+DW_TOKENS = (300, 4104, 16400, 65550)
+
 
 def leg_spec(leg: str) -> dict:
-    """The fields of ``leg``, a key of LEGS or of LATE_LEGS."""
-    return LEGS[leg] if leg in LEGS else LATE_LEGS[leg]
+    """The fields of ``leg``, a key of LEGS, LATE_LEGS or TRAIN_LEGS."""
+    return LEGS[leg] if leg in LEGS else LATE_LEGS[leg] if leg in LATE_LEGS else TRAIN_LEGS[leg]
 
 
 def shape_seed(*dims) -> int:
@@ -133,7 +144,9 @@ def tier(configs: list, acc: str, m: int, n: int, k: int, k_div: int = 1) -> tup
 def choice(leg: str, m: int, n: int, k: int) -> tuple[int, int, int]:
     """(cfg, group_m, splits) the dispatched call of ``leg`` uses for (M, N, K)."""
     from cuda_l2_b200 import capi
-    spec = LEGS[leg]
+    spec = leg_spec(leg)
+    if spec["scales"] == "block_1d1d":
+        return capi.fp8_blockwise_1d1d_select(m, n, k)
     if spec["scales"] == "block":
         return capi.fp8_blockwise_select(m, n, k)
     if spec["scales"]:
@@ -278,9 +291,17 @@ def offgrid_shapes(leg: str) -> list[tuple[int, int, int]]:
 
 def leg_shapes(leg: str) -> list[tuple[int, int, int]]:
     shapes = []
-    for name in (LEG_LISTS[leg] if leg in LEG_LISTS else LATE_LEG_LISTS[leg]):
+    lists = LEG_LISTS if leg in LEG_LISTS else LATE_LEG_LISTS if leg in LATE_LEG_LISTS else TRAIN_LEG_LISTS
+    for name in lists[leg]:
         shapes += grid_shapes() if name == "grid" else offgrid_shapes(leg)
     return shapes
+
+
+def dw_shapes() -> list[tuple[int, int, int]]:
+    """(M, N, K) of the weight-gradient samples: M = out_features, N = in_features, K = dual_ld_t(T), the token count
+    padded to 16 as the dual quantisers pad the transposed copies (the last 128-token block partial)."""
+    from cuda_l2_b200 import capi
+    return [(m, n, capi.dual_ld_t(t)) for m, n in DW_FEATURES for t in DW_TOKENS]
 
 
 @functools.lru_cache(maxsize=None)
@@ -467,8 +488,9 @@ def operands_e4m3(torch, m: int, n: int, k: int, seed: int, device="cuda"):
 
 
 def e4m3_scales(torch, granularity: str, m: int, n: int, k: int, out: str, seed: int, device="cuda"):
-    """(scale_a, scale_b) fp32 tensors as the kernel reads them (block: scale_a M-major with ld_a = M rounded up to 4),
-    and their float64 values as numpy arrays (tensor: scalars; rowwise: [M], [N]; block: [M, nkb], [ceil(N/128), nkb])."""
+    """(scale_a, scale_b) fp32 tensors as the kernel reads them (block: scale_a M-major with ld_a = M rounded up to 4;
+    block_1d1d: scale_b N-major the same way), and their float64 values as numpy arrays (tensor: scalars; rowwise: [M],
+    [N]; block: [M, nkb], [ceil(N/128), nkb]; block_1d1d: [M, nkb], [N, nkb])."""
     if granularity == "tensor":
         pairs = ed.e4m3_tensor_scales(out)
         sa, sb = pairs[seed % len(pairs)]
@@ -478,11 +500,22 @@ def e4m3_scales(torch, granularity: str, m: int, n: int, k: int, out: str, seed:
         sa, sb = ed.e4m3_rowwise_scales(m, n, out)
         return (torch.from_numpy(sa).reshape(m, 1).to(device), torch.from_numpy(sb).reshape(1, n).to(device),
                 sa.astype(np.float64), sb.astype(np.float64))
+    if granularity == "block_1d1d":
+        sa, sb = ed.e4m3_block_1d1d_scales(m, n, k, out)
+        return (m_major(torch, sa, device), m_major(torch, sb, device), sa.astype(np.float64),
+                sb.astype(np.float64))
     sa, sb = ed.e4m3_block_scales(m, n, k, out)
-    nkb, ld = sa.shape[1], -(-m // 4) * 4
+    return m_major(torch, sa, device), torch.from_numpy(sb).to(device), sa.astype(np.float64), sb.astype(np.float64)
+
+
+def m_major(torch, s: np.ndarray, device="cuda", ld: int | None = None):
+    """The (1, ld)-strided view [R, nkb] of scales ``s`` [R, nkb] that the block-scaled kernels read in place, ld = ``ld``
+    or R rounded up to 4, NaN in the padding rows."""
+    r, nkb = s.shape
+    ld = ld or -(-r // 4) * 4
     buf = torch.full((nkb, ld), float("nan"), dtype=torch.float32, device=device)
-    buf[:, :m] = torch.from_numpy(sa).t().to(device)
-    return buf[:, :m].t(), torch.from_numpy(sb).to(device), sa.astype(np.float64), sb.astype(np.float64)
+    buf[:, :r] = torch.from_numpy(np.ascontiguousarray(s, dtype=np.float32)).t().to(device)
+    return buf[:, :r].t()
 
 
 # ------------------------------------------------------------------------------------------------- the reference
@@ -515,17 +548,21 @@ def exact_blocks(torch, ops, scales=None, granularity=None, rows_per_block=None)
     dev = a.device
     b64 = bt.to(torch.float64)
     sa = sb = None
-    if granularity == "block":
+    if granularity in ("block", "block_1d1d"):
         sa = torch.from_numpy(scales[0]).to(dev)
         sb = torch.from_numpy(scales[1]).to(dev)
-        b64 *= _block_factors(sb, k).repeat_interleave(128, dim=0)[:n]
+        if granularity == "block":
+            b64 *= _block_factors(sb, k).repeat_interleave(128, dim=0)[:n]
+        else:                                                   # one scale per row of Bt and 128 k
+            for n0 in range(0, n, 4096):
+                b64[n0:n0 + 4096] *= _block_factors(sb[n0:n0 + 4096], k)
     elif granularity == "rowwise":
         sa, sb = torch.from_numpy(scales[0]).to(dev), torch.from_numpy(scales[1]).to(dev)
     rb = rows_per_block or max(16, (1 << 26) // max(n, k))
     for lo in range(0, m, rb):
         hi = min(m, lo + rb)
         a64 = a[lo:hi].to(torch.float64)
-        if granularity == "block":
+        if granularity in ("block", "block_1d1d"):
             a64 *= _block_factors(sa[lo:hi], k)
         y = a64 @ b64.T
         del a64
@@ -549,6 +586,10 @@ def numpy_rows(torch, ops, rows, cols, out: str, scales=None, granularity=None) 
         sa, sb = scales
         a = a * np.repeat(sa[rows], 128, axis=1)[:, :k]
         b = b * np.repeat(sb[cols // 128], 128, axis=1)[:, :k]
+    elif granularity == "block_1d1d":
+        sa, sb = scales
+        a = a * np.repeat(sa[rows], 128, axis=1)[:, :k]
+        b = b * np.repeat(sb[cols], 128, axis=1)[:, :k]
     y = a @ b.T
     if granularity == "tensor":
         y = y * np.float64(np.float32(np.float32(scales[0]) * np.float32(scales[1])))

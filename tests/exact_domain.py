@@ -234,6 +234,46 @@ def e4m3_block_scales(m: int, n: int, k: int, out: str) -> tuple[np.ndarray, np.
     return np.repeat(sa[:, None], nkb, axis=1).astype(np.float32), sb.astype(np.float32)
 
 
+def e4m3_1d1d_kb_bits(k: int) -> tuple[np.ndarray, np.ndarray]:
+    """The k-block exponents (u, t) of e4m3_block_1d1d_scales: u (A's) only on even k-blocks, t (Bt's) only on odd ones,
+    so u + t <= 1; each an aperiodic-looking pattern of the k-block pair index j = kb // 2 (u: j % 7 in {0, 1, 3}, t:
+    j % 5 in {0, 2}), so that no shift by 1..9 or 32 k-blocks maps either pattern, or their sum, onto itself; 0 on the
+    probe positions' k-blocks."""
+    kb = np.arange(-(-k // 128))
+    j = kb // 2
+    u = ((kb % 2 == 0) & np.isin(j % 7, (0, 1, 3))).astype(np.int64)
+    t = ((kb % 2 == 1) & np.isin(j % 5, (0, 2))).astype(np.int64)
+    probe = [p // 128 for p in probe_positions(k)]
+    u[probe] = t[probe] = 0
+    return u, t
+
+
+def e4m3_block_1d1d_scales(m: int, n: int, k: int, out: str) -> tuple[np.ndarray, np.ndarray]:
+    """Scales of the GEMM with 1 x 128 scales on both operands: scale_a [M, nkb] = Q_m 2^(r_m + u_kb) and scale_b
+    [N, nkb] = 2^(c_n + t_kb), fp32 values (e4m3_1d1d_kb_bits for u, t). c_n cycles E4M3_COL_EXP column by column, so
+    adjacent columns differ and so do columns 8 apart (8 % 3 != 0): a swapped column pair, or a column read from another
+    pair group, changes the result. A scale of either operand read for another k-block changes it too. Every promotion
+    fmaf(p, fp32(sa sb), acc) is exact: u and t never meet, so sum |p| * Q * 2^(u + t) <= 2047 * Q * 2 < 2^24."""
+    u, t = e4m3_1d1d_kb_bits(k)
+    assert (u + t).max(initial=0) <= 1
+    assert E4M3_SUM_BOUND * max(E4M3_Q[out]) * 2 < 2 ** 24
+    r = np.minimum(_cycle(E4M3_ROW_EXP, np.arange(m) // 4), 103)      # 2047 * 4095 * 2^(103 + 1 + 1) < 2^128
+    sa = e4m3_row_q(m, out)[:, None] * np.exp2(r[:, None] + u[None, :])
+    sb = np.exp2(_cycle(E4M3_COL_EXP, np.arange(n))[:, None] + t[None, :])
+    assert np.array_equal(sa.astype(np.float32).astype(np.float64), sa)
+    return sa.astype(np.float32), sb.astype(np.float32)
+
+
+def exact_1d1d(a: np.ndarray, bt: np.ndarray, sa: np.ndarray, sb: np.ndarray) -> np.ndarray:
+    """The exact float64 output of the 1 x 128 x 1 x 128 contract: sum over k-blocks of (A_kb Bt_kb^T) sa[:, kb] sb[:, kb]
+    (every term and partial sum an integer multiple of a power of two below 2^53 units, so float64 is exact)."""
+    y = np.zeros((a.shape[0], bt.shape[0]))
+    for kb in range(sa.shape[1]):
+        part = a[:, kb * 128:(kb + 1) * 128] @ bt[:, kb * 128:(kb + 1) * 128].T
+        y += part * sa[:, kb:kb + 1].astype(np.float64) * sb[None, :, kb].astype(np.float64)
+    return y
+
+
 # ------------------------------------------------------------------------------------------------ the reference
 def round_fp16_bits(x: np.ndarray) -> np.ndarray:
     """float64 -> fp16 bits, one round to nearest even (numpy's cast rounds the double directly)."""

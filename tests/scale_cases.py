@@ -28,7 +28,9 @@ BIG_GROUP = 65536
 GUARD_BYTES = 1 << 20
 BAND_BYTES = 1 << 29          # one float64 working band of the reference (512 MiB)
 REF_SLACK = 1 << 26           # cuBLAS workspace and small tensors of the reference
-SENTINEL = {torch.float16: 0x7D5A, torch.bfloat16: 0x7FA5}   # NaN payloads no kernel produces
+SENTINEL = {torch.float16: 0x7D5A, torch.bfloat16: 0x7FA5,    # NaN payloads no kernel produces
+            torch.float8_e4m3fn: 0xFF}                     # -NaN: the quantisers write NaN as 0x7F
+_BITS = {1: torch.uint8, 2: torch.int16}
 DTYPES = {"16": None, "fp16": torch.float16, "bf16": torch.bfloat16, "e4m3": torch.float8_e4m3fn,
           "fp32": torch.float32, "int32": torch.int32}
 ITEMSIZE = {"16": 2, "fp16": 2, "bf16": 2, "e4m3": 1, "fp32": 4, "int32": 4}
@@ -40,6 +42,13 @@ NN_LONG = (136, 12296, 262216)
 T_GROUPED, N_GROUPED, K_GROUPED = 262216, 12296, 64
 WGRAD = dict(g=NUM_EXPERTS, m=2048, n=9216, t=24576)
 FP8_EXPERTS = dict(g=NUM_EXPERTS, n=2560, k=7168, t=8192, slots=64)
+# The weight gradient of blockwise FP8 training (1 x 128 scales on both operands) over FP8_DW_TOKENS tokens: K is the
+# token count padded to 16 (capi.dual_ld_t), and A [M, K] passes 2^31 bytes along K.
+FP8_DW_TOKENS = 4500007
+FP8_DW = (640, 1152, -(-FP8_DW_TOKENS // 16) * 16)
+# One bf16 activation past 2^31 elements for every quantiser that takes it: rows % 16 != 0 (q_t's padded columns),
+# cols % 128 != 0 and cols / 2 % 128 != 0 (the last 1 x 128 group of x and of the SwiGLU output is partial).
+QUANT = (349203, 8200)
 
 # Long-reduction groups of the K-grouped case: one of 140 001 rows, one holding row 174 648 (dY's crossing) in its
 # middle, a 1-row, an empty one and a short last group.
@@ -106,6 +115,10 @@ def _cases() -> dict:
     t, gn, gk = T_GROUPED, N_GROUPED, K_GROUPED
     w, e = WGRAD, FP8_EXPERTS
     enkb, enb = e["k"] // 128, -(-e["n"] // 128)
+    dm, dn, dk = FP8_DW
+    dnkb = -(-dk // 128)
+    qr, qc = QUANT
+    qld_t = -(-qr // 16) * 16
     i31, i32 = 2 ** 31, 2 ** 32
     out = [
         Case("tn", "2-D TN: dispatcher (fp16 with fp32 and fp16 accumulation, bf16), pinned CTA pair, cluster and "
@@ -144,6 +157,19 @@ def _cases() -> dict:
               _t("ab", (e["g"], e["slots"], e["k"]), "e4m3"), _t("sab", (e["g"], enkb, e["slots"]), "fp32"),
               _t("masked_m", (e["g"],), "int32"), _t("cb", (e["g"], e["slots"], e["n"]), "bf16")),
              ("c", "cb"), "bt", "bytes", ((i31, 117), (i32, 234))),
+        Case("fp8_dw", "1 x 128 x 1 x 128 e4m3 weight gradient, bf16 out, A past 2^31 bytes along K",
+             (_t("a", (dm, dk), "e4m3"), _t("bt", (dn, dk), "e4m3"), _t("sa", (dnkb, -(-dm // 4) * 4), "fp32"),
+              _t("sb", (dnkb, -(-dn // 4) * 4), "fp32"), _t("c", (dm, dn), "bf16")), ("c",), "a", "bytes",
+             ((i31, 477),)),
+        Case("fp8_dw_out", "1 x 128 x 1 x 128 e4m3 2-D, bf16 out",
+             (_t("a", (m, k), "e4m3"), _t("bt", (n, k), "e4m3"), _t("sa", (nkb, -(-m // 4) * 4), "fp32"),
+              _t("sb", (nkb, -(-n // 4) * 4), "fp32"), _t("c", (m, n), "bf16")), ("c",), "c", "elements",
+             ((i31, 16383),)),
+        Case("quant", "every e4m3 quantiser of a bf16 activation, outputs sharing two guarded buffers and two scale "
+             "buffers (each sized for the largest layout it holds)",
+             (_t("x", (qr, qc), "bf16"), _t("q", (qr, qc), "e4m3"), _t("q_t", (qc, qld_t), "e4m3"),
+              _t("scale", (-(-qc // 128), -(-qr // 4) * 4), "fp32"), _t("scale_t", (-(-qr // 128), -(-qc // 4) * 4), "fp32"),
+              _t("workspace", (qr + qc + 1024,), "fp32")), ("q", "q_t"), "x", "elements", ((i31, 261888),)),
     ]
     return {c.name: c for c in out}
 
@@ -168,17 +194,18 @@ def allocate(case: Case, dtype16=torch.float16, device="cuda") -> dict:
 def guarded(shape, dtype, device="cuda"):
     """(buffer, view): the view of ``shape`` lies in the buffer with GUARD_BYTES on each side, all of it holding the
     NaN sentinel of ``dtype``."""
-    g = GUARD_BYTES // torch.empty((), dtype=dtype).element_size()
+    size = torch.empty((), dtype=dtype).element_size()
+    g = GUARD_BYTES // size
     buf = torch.empty((2 * g + math.prod(shape),), dtype=dtype, device=device)
     if device != "meta":
-        buf.view(torch.int16).fill_(SENTINEL[dtype])
+        buf.view(_BITS[size]).fill_(SENTINEL[dtype])
     return buf, buf[g:g + math.prod(shape)].view(shape)
 
 
 def guards_intact(buf) -> bool:
     g = GUARD_BYTES // buf.element_size()
     s = SENTINEL[buf.dtype]
-    bits = buf.view(torch.int16)
+    bits = buf.view(_BITS[buf.element_size()])
     return bool((bits[:g] == s).all()) and bool((bits[-g:] == s).all())
 
 
@@ -420,3 +447,74 @@ def block_expand(s: torch.Tensor, rows: int, cols: int, rb: int = 1) -> torch.Te
     if rb > 1:
         x = x.repeat_interleave(rb, dim=0)
     return x.repeat_interleave(128, dim=1)[:rows, :cols]
+
+
+# ------------------------------------------------------------------------------------------------ quantisers
+QUANTISERS = ("tensor", "rowwise", "blockwise", "silu_mul", "rowwise_dual", "blockwise_dual", "block128x128_dual")
+
+
+def quant_band_rows(cols: int) -> int:
+    """Rows of x per reference band: a multiple of 128 (whole 128-row groups of the transposed and 128 x 128 results)
+    whose float32 copy takes at most a quarter of BAND_BYTES (the reference holds a few of them)."""
+    return max(128, BAND_BYTES // (16 * cols) // 128 * 128)
+
+
+def quant_bands(kind: str, x: torch.Tensor, band_rows: int):
+    """The reference of quantiser ``kind`` (a key of QUANTISERS) on x [rows, cols], band by band: yields (result,
+    index, want) with ``want`` the bits the unbanded ``ops.*_reference`` gives at ``index`` (a tuple of slices) of its
+    ``result`` ("q", "scale", "q_t" or "scale_t", laid out as that reference lays it out). Each band holds ``band_rows``
+    rows of x (a multiple of 128). The global quantities are reduced over all bands first: the per-tensor amax, and the
+    column maxima behind the rowwise dual's scale_t. q_t's band is its columns [lo, hi); its padding columns [rows,
+    ld_t) come with the last band (blockwise dual) or on their own (rowwise dual)."""
+    from cuda_l2_b200 import capi, ops
+    assert band_rows % 128 == 0 and kind in QUANTISERS
+    rows, cols = x.shape
+    e4, big, tiny = torch.float8_e4m3fn, ops.E4M3_MAX, torch.finfo(torch.float32).tiny
+    bands = [(lo, min(rows, lo + band_rows)) for lo in range(0, rows, band_rows)]
+    ld_t = capi.dual_ld_t(rows)
+    every = slice(None)
+    if kind == "tensor":
+        # abs() again: a NaN that reduction returns keeps the sign the unbanded reference's does (+), as in its abs()
+        amax = torch.stack([x[lo:hi].abs().amax() for lo, hi in bands]).amax().abs()
+        scale = (amax.float() / big).clamp_min(tiny).reshape(1)
+        yield "scale", (every,), scale
+        for lo, hi in bands:
+            yield "q", (slice(lo, hi),), (x[lo:hi].float() / scale).clamp(-big, big).to(e4)
+        return
+    if kind == "rowwise_dual":
+        col_max = torch.stack([x[lo:hi].abs().amax(dim=0) for lo, hi in bands]).amax(dim=0).abs()
+        scale_t = (col_max.float() / big).clamp_min(tiny)
+        yield "scale_t", (every,), scale_t
+        pad = torch.zeros((cols, ld_t - rows), dtype=torch.float32, device=x.device)
+        yield "q_t", (every, slice(rows, ld_t)), (pad / scale_t[:, None]).clamp(-big, big).to(e4)
+    for lo, hi in bands:
+        xb, r = x[lo:hi], slice(lo, hi)
+        if kind == "rowwise":
+            q, s = ops.quantize_e4m3_rowwise_reference(xb)
+            yield "q", (r,), q
+            yield "scale", (r,), s
+        elif kind in ("blockwise", "blockwise_dual", "silu_mul"):
+            ref = ops.silu_mul_quantize_e4m3_blockwise_reference if kind == "silu_mul" else \
+                ops.quantize_e4m3_blockwise_reference
+            q, s = ref(xb)
+            yield "q", (r,), q
+            yield "scale", (r,), s
+            if kind == "blockwise_dual":
+                xt = xb.t()
+                if hi == rows:
+                    xt = torch.nn.functional.pad(xt, (0, ld_t - rows))
+                qt, st = ops.quantize_e4m3_blockwise_reference(xt.contiguous())
+                yield "q_t", (every, slice(lo, lo + qt.shape[1])), qt
+                yield "scale_t", (every, slice(lo // 128, lo // 128 + st.shape[1])), st
+        elif kind == "rowwise_dual":
+            q, s = ops.quantize_e4m3_rowwise_reference(xb)
+            yield "q", (r,), q
+            yield "scale", (r,), s.reshape(-1)
+            yield "q_t", (every, r), (xb.t().float() / scale_t[:, None]).clamp(-big, big).to(e4)
+        else:
+            q, s = ops.quantize_e4m3_block128x128(xb)
+            sr = slice(lo // 128, lo // 128 + s.shape[0])
+            yield "q", (r,), q
+            yield "scale", (sr,), s
+            yield "q_t", (every, r), q.t()
+            yield "scale_t", (every, sr), s.t()
