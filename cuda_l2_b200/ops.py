@@ -76,7 +76,11 @@ the nearest grid shape — so deployment is a plain operator:
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernels, so a fine-tuning
 loop works: ``hgemm``'s input gradient reads the weight in place through the row-major B kernels, and its weight
-gradient pays one transposed copy (of the output gradient). The grouped product trains through :func:`grouped_linear`
+gradient pays one transposed copy (of the output gradient). The weight gradient reduces over the tokens M, which the
+forward takes in any number: when M % 8 != 0 that copy would have rows of M % 8 != 0 elements, which no kernel reads,
+so the weight gradients of ``hgemm``, ``hgemm_nn``, ``hgemm_batched`` and ``hgemm_bias_act`` run
+``hgemm_grouped_wgrad`` instead, on both operands in place, with one group (one per batch) whose end it writes on the
+device. The grouped product trains through :func:`grouped_linear`
 (``hgemm_grouped`` itself stays inference only). The FP8 operators have no gradient: a backward through them raises.
 FP8 training goes through :func:`fp8_linear`, whose own backward runs those operators.
 """
@@ -157,6 +161,12 @@ def _hgemm_launch(c, a, b_kmajor, acc="fp32", *, stream):
         capi.gemm_kmajor(a.contiguous(), b_kmajor.contiguous(), c, acc, stream=stream)
 
 
+def _token_ends(m: int, groups: int, device) -> torch.Tensor:
+    """The int32 group ends m, 2m, ..., groups * m of ``groups`` blocks of m tokens, written on the device by one kernel:
+    no host copy, so a backward that passes them to the K-grouped kernel can be captured in a CUDA graph."""
+    return torch.arange(m, m * groups + 1, m, dtype=torch.int32, device=device)
+
+
 def _product_grads(a, b_kmajor, grad_c, need_a: bool, need_b: bool):
     """(dA, dBt) of C = A Bt^T for the output gradient ``grad_c`` (None where not needed)."""
     grad_a = grad_b = None
@@ -167,7 +177,11 @@ def _product_grads(a, b_kmajor, grad_c, need_a: bool, need_b: bool):
     if need_a:
         grad_a = torch.ops.cuda_l2_b200.hgemm_nn(g, b_kmajor, "fp32")
     if need_b:
-        grad_b = torch.ops.cuda_l2_b200.hgemm_nn(g.t().contiguous(), a, "fp32")
+        m = a.shape[0]
+        if m % 8 == 0:
+            grad_b = torch.ops.cuda_l2_b200.hgemm_nn(g.t().contiguous(), a, "fp32")
+        else:   # dC^T would have M % 8 != 0 columns (no 16-byte rows): the K-grouped kernel reduces any M, in place
+            grad_b = torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(g, a, _token_ends(m, 1, g.device), "fp32")[0]
     return grad_a, grad_b
 
 
@@ -210,7 +224,11 @@ def _hgemm_nn_backward(ctx, grad_c):
     if ctx.needs_input_grad[0]:
         grad_a = torch.ops.cuda_l2_b200.hgemm(g, b, "fp32")
     if ctx.needs_input_grad[1]:
-        grad_b = torch.ops.cuda_l2_b200.hgemm_nn(a.t().contiguous(), g, "fp32")
+        m = a.shape[0]
+        if m % 8 == 0:
+            grad_b = torch.ops.cuda_l2_b200.hgemm_nn(a.t().contiguous(), g, "fp32")
+        else:   # A^T would have M % 8 != 0 columns: the K-grouped kernel reads A and dC in place
+            grad_b = torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(a, g, _token_ends(m, 1, g.device), "fp32")[0]
     return grad_a, grad_b, None
 
 
@@ -253,8 +271,15 @@ def _hgemm_batched_backward(ctx, grad_c):
     if ctx.needs_input_grad[0]:
         grad_a = torch.ops.cuda_l2_b200.hgemm_batched(g, b_kmajor.transpose(1, 2).contiguous(), "fp32")
     if ctx.needs_input_grad[1]:
-        grad_b = torch.ops.cuda_l2_b200.hgemm_batched(g.transpose(1, 2).contiguous(), a.transpose(1, 2).contiguous(),
-                                                      "fp32")
+        bsz, m, k = a.shape
+        if m % 8 == 0:
+            grad_b = torch.ops.cuda_l2_b200.hgemm_batched(g.transpose(1, 2).contiguous(),
+                                                          a.transpose(1, 2).contiguous(), "fp32")
+        elif bsz:   # ragged M: the K-grouped kernel, batch b being the group of rows [b M, (b + 1) M), one launch
+            grad_b = torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(g.reshape(bsz * m, -1), a.reshape(bsz * m, k),
+                                                                _token_ends(m, bsz, g.device), "fp32")
+        else:       # no batch: the gradient has no element
+            grad_b = torch.zeros_like(b_kmajor)
     return grad_a, grad_b, None, None
 
 

@@ -126,21 +126,29 @@ def _meta(*shape, dtype):
     return torch.empty(shape, dtype=dtype, device="meta", requires_grad=True)
 
 
+# The token count M is free: the weight gradient reduces over it, at M % 8 != 0 through the K-grouped kernel.
+TOKENS = [40, 41, 1, 193]
+
+
+@pytest.mark.parametrize("m", TOKENS)
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-def test_meta_gradients_of_the_products(dtype):
-    """M = 40 is a multiple of 8: the weight gradient reduces over M."""
-    a, b_kmajor, b = _meta(40, 32, dtype=dtype), _meta(24, 32, dtype=dtype), _meta(32, 24, dtype=dtype)
+def test_meta_gradients_of_the_products(dtype, m):
+    a, b_kmajor, b = _meta(m, 32, dtype=dtype), _meta(24, 32, dtype=dtype), _meta(32, 24, dtype=dtype)
     _grads_match_inputs(ops.hgemm(a, b_kmajor), (a, b_kmajor))
     _grads_match_inputs(ops.hgemm_nn(a, b), (a, b))
-    a3, b3 = _meta(3, 40, 32, dtype=dtype), _meta(3, 24, 32, dtype=dtype)
+    a3, b3 = _meta(3, m, 32, dtype=dtype), _meta(3, 24, 32, dtype=dtype)
     _grads_match_inputs(ops.hgemm_batched(a3, b3), (a3, b3))
+    lin = ops.B200Linear(32, 24, device="meta", dtype=dtype)
+    x = _meta(3, m, 32, dtype=dtype)
+    _grads_match_inputs(lin(x), (x, lin.weight, lin.bias))
 
 
+@pytest.mark.parametrize("m", TOKENS)
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("activation", ["none", "relu", "gelu_tanh"])
 @pytest.mark.parametrize("with_bias", [True, False])
-def test_meta_gradients_of_bias_act(dtype, activation, with_bias):
-    a, b_kmajor = _meta(40, 32, dtype=dtype), _meta(24, 32, dtype=dtype)
+def test_meta_gradients_of_bias_act(dtype, activation, with_bias, m):
+    a, b_kmajor = _meta(m, 32, dtype=dtype), _meta(24, 32, dtype=dtype)
     bias = _meta(24, dtype=dtype) if with_bias else None
     inputs = (a, b_kmajor, bias) if with_bias else (a, b_kmajor)
     _grads_match_inputs(ops.hgemm_bias_act(a, b_kmajor, bias, activation), inputs)
