@@ -345,7 +345,7 @@ def blockwise_ld_a(scale_a) -> int | None:
     are never stepped and do not count. None if the tensor is not laid out that way."""
     *lead, m, nkb = scale_a.shape
     bsz, st = (lead[0] if lead else 1), scale_a.stride()
-    ld = st[-1] if nkb > 1 else -(-m // 4) * 4     # one k-block: the k stride is never stepped
+    ld = st[-1] if nkb > 1 else _m_major_ld(m)     # one k-block: the k stride is never stepped
     if nkb == 1 and bsz > 1:   # the batch stride is the only one stepped: it is nkb * ld_a = ld_a
         ld = st[0]
     if (bsz > 1 and st[0] != nkb * ld) or (m > 1 and st[-2] != 1) or ld < m or ld % 4 or scale_a.data_ptr() % 16:
@@ -354,41 +354,69 @@ def blockwise_ld_a(scale_a) -> int | None:
     return ld if bsz * nkb * ld <= readable else None
 
 
-batched_blockwise_ld_a = blockwise_ld_a   # the batched [B, M, nkb] form, by the name of the batched call
+def _m_major_ld(m: int) -> int:
+    """ld_a of the M-major scales the quantisers write and :func:`m_major` copies into: M rounded up to 4."""
+    return -(-m // 4) * 4
 
 
-def scale_granularity_or_none(m: int, n: int, scale_a, scale_b, k: int | None = None) -> str | None:
-    """:func:`scale_granularity` of a plain product, or None where it raises."""
-    try:
-        return scale_granularity(m, n, scale_a, scale_b, k=k)
-    except B200HgemmError:
-        return None
+def empty_m_major(lead: tuple, m: int, nkb: int, device):
+    """An empty fp32 blockwise scale [*lead, M, nkb] that the block-scaled kernels read in place: the view
+    ``buf[..., :M].transpose(-2, -1)`` of a [*lead, nkb, ld_a] buffer, ld_a = M rounded up to 4."""
+    import torch
+
+    buf = torch.empty((*lead, nkb, _m_major_ld(m)), dtype=torch.float32, device=device)
+    return buf[..., :m].transpose(-2, -1)
+
+
+def m_major(scale):
+    """A blockwise scale [(B,) M, nkb] as the block-scaled kernels read it: ``scale`` itself where
+    :func:`blockwise_ld_a` reads it in place, else a device copy into :func:`empty_m_major`."""
+    if blockwise_ld_a(scale) is not None:
+        return scale
+    *lead, m, nkb = scale.shape
+    return empty_m_major(lead, m, nkb, scale.device).copy_(scale)
 
 
 def _scale_ld_a(scale_a, name: str = "scale_a") -> int:
     """blockwise_ld_a of a ``scale_a`` (or a 1 x 128 ``scale_b``, the same layout) the kernel reads in place;
-    B200HgemmError if it cannot."""
-    ld_a = blockwise_ld_a(scale_a)
+    B200HgemmError if it cannot (a CPU tensor included)."""
+    ld_a = blockwise_ld_a(scale_a) if scale_a.is_cuda else None
     if ld_a is None:
-        raise B200HgemmError(f"blockwise {name} must hold one M-major [ceil(K/128), ld_a] block per matrix (strides "
-                             f"(1, ld_a), batched (ceil(K/128) * ld_a, 1, ld_a)) with ld_a >= M, ld_a % 4 == 0, 16-byte "
-                             f"aligned, every block readable; got strides {tuple(scale_a.stride())}")
+        raise B200HgemmError(f"blockwise {name} must be a CUDA tensor holding one M-major [ceil(K/128), ld_a] block "
+                             f"per matrix (strides (1, ld_a), batched (ceil(K/128) * ld_a, 1, ld_a)) with ld_a >= M, "
+                             f"ld_a % 4 == 0, 16-byte aligned, every block readable; got strides "
+                             f"{tuple(scale_a.stride())} on {scale_a.device}")
     return ld_a
 
 
-def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32", scales: tuple = ()) -> tuple[int, int, int]:
-    """(M, N, K) of a[M,K] @ b_kmajor[N,K]^T -> ``out_dtype``, by the rules of the variant the dtypes and ``acc`` name:
-    2-D operands of one dtype, a shared K, 16-byte rows, two scales exactly for a scaled variant, per tensor or rowwise
-    (:func:`scale_granularity`). Checks shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
+def _scale_args(granularity: str, scale_a, scale_b) -> tuple:
+    """The scale arguments of the e4m3 entry points for scales of ``granularity`` (:func:`scale_granularity`):
+    ``(scale_a, ld_a, scale_b, ld_b)`` for 1 x 128 scales on both operands, both read in place (:func:`_scale_ld_a`);
+    ``(scale_a, ld_a, scale_b)`` for blockwise ones, ``scale_a`` read in place and ``scale_b`` a contiguous CUDA
+    tensor; ``(scale_a, scale_b)`` otherwise, both contiguous CUDA tensors. B200HgemmError if a scale is not so."""
+    if granularity == "blockwise_1d1d":
+        return scale_a.data_ptr(), _scale_ld_a(scale_a), scale_b.data_ptr(), _scale_ld_a(scale_b, "scale_b")
+    if granularity == "blockwise":
+        _contiguous_cuda(scale_b=scale_b)
+        return scale_a.data_ptr(), _scale_ld_a(scale_a), scale_b.data_ptr()
+    _contiguous_cuda(scale_a=scale_a, scale_b=scale_b)
+    return scale_a.data_ptr(), scale_b.data_ptr()
+
+
+def check_operands(a, b_kmajor, out_dtype, acc: str | int = "fp32",
+                   scales: tuple = ()) -> tuple[int, int, int, str | None]:
+    """(M, N, K, granularity) of a[M,K] @ b_kmajor[N,K]^T -> ``out_dtype``, by the rules of the variant the dtypes and
+    ``acc`` name: 2-D operands of one dtype, a shared K, 16-byte rows, two scales exactly for a scaled variant, of the
+    granularity :func:`scale_granularity` returns (None without scales). Checks shapes and dtypes only (meta tensors
+    pass); B200HgemmError otherwise."""
     try:
         (m, k), (n, k2) = a.shape, b_kmajor.shape
     except ValueError:
         raise B200HgemmError(f"2-D operands expected, got {tuple(a.shape)} and {tuple(b_kmajor.shape)}") from None
     t = _operand_type(a, b_kmajor, out_dtype, acc, scales)
-    if scales:
-        scale_granularity(m, n, *scales, k=k)
+    granularity = scale_granularity(m, n, *scales, k=k) if scales else None
     _check_k(a, b_kmajor, t, n, k, k2, "[N, K]")
-    return m, n, k
+    return m, n, k, granularity
 
 
 def _operand_type(a, b_kmajor, out_dtype, acc: str | int, scales: tuple, scaled: bool = True) -> GemmType:
@@ -416,23 +444,21 @@ def _check_k(a, b_kmajor, t: GemmType, n: int, k: int, k2: int, b_layout: str) -
                              f"got N={n}, K={k}")
 
 
-def _contiguous_cuda(in_place=("scale_a",), **tensors) -> None:
-    """B200HgemmError unless every tensor given (None: not passed) is a contiguous CUDA tensor. The tensors named in
-    ``in_place`` (``scale_a``) need not be contiguous: blockwise scales are read M-major, in place
-    (:func:`blockwise_ld_a`)."""
+def _contiguous_cuda(**tensors) -> None:
+    """B200HgemmError unless every tensor given (None: not passed) is a contiguous CUDA tensor."""
     for name, x in tensors.items():
-        if x is not None and (not x.is_cuda or not (x.is_contiguous() or name in in_place)):
+        if x is not None and (not x.is_cuda or not x.is_contiguous()):
             raise B200HgemmError(f"{name} must be a contiguous CUDA tensor")
 
 
-def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = (), in_place=("scale_a",)) -> tuple[int, int, int]:
-    """check_operands for c = a @ b_kmajor^T, all of them (scales included, those in ``in_place`` as
-    :func:`_contiguous_cuda` allows) CUDA tensors, c of shape [M,N]."""
-    _contiguous_cuda(in_place, a=a, b_kmajor=b_kmajor, c=c, **dict(zip(("scale_a", "scale_b"), scales)))
-    m, n, k = check_operands(a, b_kmajor, c.dtype, acc, scales)
+def _kmajor_operands(a, b_kmajor, c, acc: str | int, scales: tuple = ()) -> tuple[int, int, int, str | None]:
+    """check_operands for c = a @ b_kmajor^T, the three contiguous CUDA tensors and c of shape [M,N]. The scales are
+    checked only by shape and dtype here: how they may be laid out depends on the granularity (:func:`_scale_args`)."""
+    _contiguous_cuda(a=a, b_kmajor=b_kmajor, c=c)
+    m, n, k, granularity = check_operands(a, b_kmajor, c.dtype, acc, scales)
     if c.shape != (m, n):
         raise B200HgemmError(f"shape mismatch: a {tuple(a.shape)}, b_kmajor {tuple(b_kmajor.shape)}, c {tuple(c.shape)}")
-    return m, n, k
+    return m, n, k, granularity
 
 
 def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = None, config_id: int | None = None,
@@ -443,7 +469,7 @@ def gemm_kmajor(a, b_kmajor, c, acc: str | int = "fp32", stream: int | None = No
     caps the CTAs of the launch, 0 meaning all SMs, so that each worker runs several tiles."""
     import torch
 
-    m, n, k = _kmajor_operands(a, b_kmajor, c, acc)
+    m, n, k, _ = _kmajor_operands(a, b_kmajor, c, acc)
     lib = hgemm_lib()
     bits = ACC_BITS[acc]
     if config_id is None:
@@ -510,50 +536,23 @@ def fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream: int | None = None, config
     b200_hgemm_run_config; ``max_ctas`` as in :func:`gemm_kmajor`); default is the dispatcher."""
     import torch
 
-    one_d = (a.dim() == 2 and b_kmajor.dim() == 2 and scale_granularity_or_none(
-        a.shape[0], b_kmajor.shape[0], scale_a, scale_b, k=a.shape[1]) == "blockwise_1d1d")
-    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b),
-                               ("scale_a", "scale_b") if one_d else ("scale_a",))
+    m, n, k, granularity = _kmajor_operands(a, b_kmajor, c, "fp32", (scale_a, scale_b))
+    # granularity -> the dispatched and the pinned entry point; their arguments differ only in the scales (_scale_args)
+    dispatched, pinned = {
+        "tensor": ("b200_fp8gemm", "b200_fp8gemm_run_config"),
+        "rowwise": ("b200_fp8gemm_rowwise", "b200_fp8gemm_rowwise_run_config"),
+        "blockwise": ("b200_fp8gemm_blockwise", "b200_fp8gemm_blockwise_run_config"),
+        "blockwise_1d1d": ("cuda_l2_b200_fp8block_1d1d_run", "cuda_l2_b200_fp8block_1d1d_run_config"),
+    }[granularity]
+    ptrs = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), *_scale_args(granularity, scale_a, scale_b))
+    lib = load(_LIBRARY_OF[dispatched])
     out_bf16 = int(c.dtype == torch.bfloat16)
-    granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
-    if granularity == "blockwise_1d1d":
-        ld_a, ld_b = _scale_ld_a(scale_a), _scale_ld_a(scale_b, "scale_b")
-        lib = fp8block_1d1d_lib()
-        if config_id is None:
-            fn = lib.cuda_l2_b200_fp8block_1d1d_run
-            st = fn(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr(), ld_b,
-                    out_bf16, m, n, k, stream)
-        else:
-            fn = lib.cuda_l2_b200_fp8block_1d1d_run_config
-            st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a,
-                    scale_b.data_ptr(), ld_b, m, n, k, group_m, max_ctas, splits, stream)
-        _check(st, fn)
-        return
-    if granularity == "blockwise":
-        ld_a = _scale_ld_a(scale_a)
-        blk = fp8block_lib()
-        if config_id is None:
-            fn = blk.b200_fp8gemm_blockwise
-            st = fn(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a, scale_b.data_ptr(),
-                    out_bf16, m, n, k, stream)
-        else:
-            fn = blk.b200_fp8gemm_blockwise_run_config
-            st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), ld_a,
-                    scale_b.data_ptr(), m, n, k, group_m, max_ctas, splits, stream)
-        _check(st, fn)
-        return
-    if not scale_a.is_contiguous():
-        raise B200HgemmError("scale_a must be a contiguous CUDA tensor")
-    lib = hgemm_lib()
-    rowwise = granularity == "rowwise"
     if config_id is None:
-        fn = lib.b200_fp8gemm_rowwise if rowwise else lib.b200_fp8gemm
-        st = fn(a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(), scale_b.data_ptr(), out_bf16,
-                m, n, k, stream)
+        fn = getattr(lib, dispatched)
+        st = fn(*ptrs, out_bf16, m, n, k, stream)
     else:
-        fn = lib.b200_fp8gemm_rowwise_run_config if rowwise else lib.b200_fp8gemm_run_config
-        st = fn(config_id, out_bf16, a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr(),
-                scale_b.data_ptr(), m, n, k, group_m, max_ctas, splits, stream)
+        fn = getattr(lib, pinned)
+        st = fn(config_id, out_bf16, *ptrs, m, n, k, group_m, max_ctas, splits, stream)
     _check(st, fn)
 
 
@@ -618,11 +617,11 @@ def _tile_list_gemm(kind: str, a, b_kmajor, c, lst, acc: str | int, scales: tupl
     """The call of a tile-list library: ``kind`` "batched" (``lst``: the optional row counts masked_m) or "grouped"
     (``lst``: the group ends offs); with two blockwise ``scales`` the block-scaled FP8 library of that kind, with fp16 /
     bf16 output as ``c``'s dtype. Every tensor is a contiguous CUDA tensor, except that scale_a is read in place
-    (:func:`blockwise_ld_a`). ``config_id`` pins one kernel configuration; default is the dispatcher."""
+    (:func:`_scale_args`). ``config_id`` pins one kernel configuration; default is the dispatcher."""
     import torch
 
     list_name = "masked_m" if kind == "batched" else "offs"
-    _contiguous_cuda(a=a, b_kmajor=b_kmajor, c=c, **dict(zip(("scale_a", "scale_b"), scales)), **{list_name: lst})
+    _contiguous_cuda(a=a, b_kmajor=b_kmajor, c=c, **{list_name: lst})
     out_dtype = c.dtype if scales else None
     if kind == "batched":
         count, rows, n, k = check_batched_operands(a, b_kmajor, acc, lst, out_dtype, scales)
@@ -636,7 +635,7 @@ def _tile_list_gemm(kind: str, a, b_kmajor, c, lst, acc: str | int, scales: tupl
     ptrs = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr())
     if scales:   # the FP8 entry points take the scales after the operands, and the output selector after them
         selector = int(c.dtype == torch.bfloat16)
-        ptrs += (scales[0].data_ptr(), _scale_ld_a(scales[0]), scales[1].data_ptr())
+        ptrs += _scale_args("blockwise", *scales)
     else:        # the 16-bit ones take the variant first
         selector = batched_variant(a.dtype, acc)
     prefix = f"{kind}_fp8" if scales else kind
@@ -926,7 +925,7 @@ def fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=None, config_id:
     """c[b] = the block-scaled product of a[b] and b_kmajor[b]^T for every b, with ``float8_e4m3fn`` operands a [B,M,K]
     and b_kmajor [B,N,K] (contiguous CUDA tensors), c [B,M,N] fp16 or bf16, and block scales read by the kernel when
     it runs (include/b200_batched_fp8.h): ``scale_a`` [B, M, ceil(K/128)] with one M-major block per matrix (strides
-    (nkb * ld_a, 1, ld_a), see :func:`batched_blockwise_ld_a`: what ``ops.quantize_e4m3_blockwise`` of a [B,M,K]
+    (nkb * ld_a, 1, ld_a), see :func:`blockwise_ld_a`: what ``ops.quantize_e4m3_blockwise`` of a [B,M,K]
     tensor returns), ``scale_b`` [B, ceil(N/128), ceil(K/128)] contiguous. ``masked_m``: an optional int32 CUDA tensor
     [B], read by the kernel: only rows [0, clamp(masked_m[b], 0, M)) of c[b] are computed, as for
     :func:`gemm_batched`. ``config_id`` pins one kernel configuration (tests), ``max_ctas`` caps the CTAs (0: all SMs);
@@ -1155,12 +1154,13 @@ def check_bias(bias, n: int, out_dtype) -> None:
                              f"{tuple(bias.shape)}")
 
 
-def _bias_arg(bias):
-    """The bias as the kernels read it: contiguous and 16-byte aligned (a fresh copy if it is not)."""
-    if bias is None:
+def _aligned(t):
+    """``t`` as the kernels read a bias or a vector of scales: contiguous and 16-byte aligned (a fresh copy if it is
+    not). None stays None."""
+    if t is None:
         return None
-    bias = bias.contiguous()
-    return bias if bias.data_ptr() % 16 == 0 else bias.clone()
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
 def gemm_bias_act(a, b_kmajor, c, bias=None, activation: str = "none", scale_a=None, scale_b=None,
@@ -1173,22 +1173,17 @@ def gemm_bias_act(a, b_kmajor, c, bias=None, activation: str = "none", scale_a=N
     "gelu_tanh". ``config_id`` pins one kernel configuration (tests; ``group_m``, ``splits`` and ``max_ctas`` as for
     :func:`gemm_kmajor`); default is the dispatcher's choice for the same variant."""
     scales = () if scale_a is None and scale_b is None else (scale_a, scale_b)
-    m, n, k = _kmajor_operands(a, b_kmajor, c, "fp32", scales)
+    m, n, k, granularity = _kmajor_operands(a, b_kmajor, c, "fp32", scales)
     variant = epilogue_variant(a.dtype, c.dtype)
     act = activation_code(activation)
     _contiguous_cuda(bias=bias)
     check_bias(bias, n, c.dtype)
-    rowwise = 0
-    if scales:
-        granularity = scale_granularity(m, n, scale_a, scale_b, k=k)
-        if granularity in ("blockwise", "blockwise_1d1d"):
-            raise B200HgemmError("blockwise e4m3 scales have no bias + activation kernel (per-tensor or rowwise only)")
-        rowwise = int(granularity == "rowwise")
-        if not scale_a.is_contiguous():
-            raise B200HgemmError("scale_a must be a contiguous CUDA tensor")
-    bias = _bias_arg(bias)
-    args = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), scale_a.data_ptr() if scales else None,
-            scale_b.data_ptr() if scales else None, rowwise, None if bias is None else bias.data_ptr(), act, m, n, k)
+    if granularity in ("blockwise", "blockwise_1d1d"):
+        raise B200HgemmError("blockwise e4m3 scales have no bias + activation kernel (per-tensor or rowwise only)")
+    scale_args = _scale_args(granularity, *scales) if scales else (None, None)
+    bias = _aligned(bias)
+    args = (a.data_ptr(), b_kmajor.data_ptr(), c.data_ptr(), *scale_args, int(granularity == "rowwise"),
+            None if bias is None else bias.data_ptr(), act, m, n, k)
     lib = epilogue_lib()
     if config_id is None:
         fn = lib.cuda_l2_b200_epilogue_run
@@ -1401,15 +1396,16 @@ def quantize_e4m3_blockwise_dual(x, q, scale, q_t, scale_t, stream: int | None =
     """Both 1 x 128 quantisations of a 2-D ``x`` [rows, cols] (fp16 or bf16, contiguous) in one launch: ``q`` (e4m3
     [rows, cols]) with ``scale`` [rows, ceil(cols/128)], and ``q_t`` (e4m3 [cols, dual_ld_t(rows)], x^T zero-padded)
     with ``scale_t`` [cols, ceil(rows/128)], both scales written in place in the M-major layout of
-    :func:`blockwise_ld_a` with ld = rows (cols) rounded up to 4 (csrc/b200_quant_block_dual.h)."""
+    :func:`blockwise_ld_a` with ld = rows (cols) rounded up to 4, as :func:`empty_m_major` allocates them
+    (csrc/b200_quant_block_dual.h)."""
     code, rows, cols = _block_dual_input(x)
     _quant_output(q, x.shape, x)
     _quant_output(q_t, (cols, dual_ld_t(rows)), x)
     for name, s, (m, nkb) in (("scale", scale, (rows, num_k_blocks(cols))),
                               ("scale_t", scale_t, (cols, num_k_blocks(rows)))):
         _fp32_on(s, x, name, (m, nkb))
-        if blockwise_ld_a(s) != -(-m // 4) * 4:
-            raise B200HgemmError(f"{name} must be the M-major view of a [{nkb}, {-(-m // 4) * 4}] buffer")
+        if blockwise_ld_a(s) != _m_major_ld(m):
+            raise B200HgemmError(f"{name} must be the M-major view of a [{nkb}, {_m_major_ld(m)}] buffer")
     fn = quant_block_dual_lib().cuda_l2_b200_quant_block_dual_e4m3_1x128
     _check(fn(code, x.data_ptr(), rows, cols, q.data_ptr(), scale.data_ptr(), q_t.data_ptr(), scale_t.data_ptr(),
               stream), fn)

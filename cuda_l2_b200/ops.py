@@ -99,7 +99,9 @@ def _define_op(name: str, schema: str, shape, launch, why: str = "", outputs=Non
     """Defines the operator cuda_l2_b200::<name> with ``schema``. ``shape(*args)`` checks the arguments by the kernel's
     rules (meta tensors pass) and returns the result's shape and dtype: the fake implementation is an empty tensor of
     those, and the CUDA one allocates the result ``c`` on the operands' device and calls ``launch(c, *args,
-    stream=...)`` there, on torch's current stream, so that it orders with the surrounding torch ops.
+    stream=...)`` there, on torch's current stream, so that it orders with the surrounding torch ops. Whatever more
+    ``shape`` returns (the FP8 operators: the scale granularity it found) is passed to ``launch`` after the arguments,
+    so that the launch does not work it out again.
     An operator with several results passes ``outputs`` instead of ``shape``: ``outputs(*args)`` checks the arguments
     the same way and returns the tuple of empty results, allocated on the device of ``args[0]`` in their final layout;
     the CUDA and the fake implementation both call it, so the fake results have the real ones' shapes and strides, and
@@ -110,15 +112,16 @@ def _define_op(name: str, schema: str, shape, launch, why: str = "", outputs=Non
     torch.library.define(qualname, schema)
 
     def cuda(*args):
+        found = ()
         if outputs is not None:
             c = outputs(*args)
             device = args[0].device
         else:
-            out_shape, dtype = shape(*args)
+            out_shape, dtype, *found = shape(*args)
             c = torch.empty(out_shape, dtype=dtype, device=args[0].device)
             device = c.device
         with torch.cuda.device(device):
-            launch(c, *args, stream=torch.cuda.current_stream(device).cuda_stream)
+            launch(c, *args, *found, stream=torch.cuda.current_stream(device).cuda_stream)
         return c
 
     def cpu(*args):
@@ -127,7 +130,7 @@ def _define_op(name: str, schema: str, shape, launch, why: str = "", outputs=Non
     def fake(*args):
         if outputs is not None:
             return outputs(*args)
-        out_shape, dtype = shape(*args)
+        out_shape, dtype, *_ = shape(*args)
         return args[0].new_empty(out_shape, dtype=dtype)
 
     def no_backward(ctx, *grads):
@@ -152,7 +155,7 @@ def _empty_product(c: torch.Tensor, k: int) -> bool:
 
 
 def _hgemm_shape(a, b_kmajor, acc="fp32"):
-    m, n, _ = capi.check_operands(a, b_kmajor, a.dtype, acc)
+    m, n, _, _ = capi.check_operands(a, b_kmajor, a.dtype, acc)
     return (m, n), a.dtype
 
 
@@ -549,7 +552,7 @@ def _bias_act_empty(c: torch.Tensor, k: int, bias, activation: str) -> bool:
 
 
 def _hgemm_bias_act_shape(a, b_kmajor, bias, activation="none"):
-    m, n, k = capi.check_operands(a, b_kmajor, a.dtype, "fp32")
+    m, n, k, _ = capi.check_operands(a, b_kmajor, a.dtype, "fp32")
     capi.epilogue_variant(a.dtype, a.dtype)
     capi.check_bias(bias, n, a.dtype)
     capi.activation_code(activation)
@@ -612,44 +615,28 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = No
 # ------------------------------------------------------------------------------------------ FP8 (e4m3), inference only
 E4M3_MAX = 448.0   # largest finite float8_e4m3fn value
 
-def _rowwise_scale_arg(s: torch.Tensor) -> torch.Tensor:
-    """A rowwise scale vector as the kernel reads it: contiguous and 16-byte aligned (a fresh copy if it is not)."""
-    s = s.contiguous()
-    return s if s.data_ptr() % 16 == 0 else s.clone()
-
-
-def _m_major(s: torch.Tensor) -> torch.Tensor:
-    """A blockwise ``scale_a`` [M, nkb], or [B, M, nkb], as the kernels read it: one M-major [nkb, ld_a] block per
-    matrix, ld_a = M rounded up to 4 (``buf[..., :M].transpose(-2, -1)`` of an [nkb, ld_a] or [B, nkb, ld_a] buffer), a
-    device copy unless it is already laid out so."""
-    if capi.blockwise_ld_a(s) is not None:
-        return s
-    *lead, m, nkb = s.shape
-    buf = torch.empty((*lead, nkb, -(-m // 4) * 4), dtype=s.dtype, device=s.device)
-    buf[..., :m].copy_(s.transpose(-2, -1))
-    return buf[..., :m].transpose(-2, -1)
+def _kernel_scales(granularity: str, scale_a: torch.Tensor, scale_b: torch.Tensor):
+    """Scales of ``granularity`` (what :func:`capi.scale_granularity` found) as the kernels read them, copied only
+    where they are not laid out so: per-tensor scales one contiguous element each; a blockwise ``scale_a``, and a
+    1 x 128 ``scale_b``, M-major (:func:`capi.m_major`); rowwise vectors and the block scales of Bt contiguous and
+    16-byte aligned."""
+    if granularity == "tensor":
+        return scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous()
+    if granularity == "rowwise":
+        return capi._aligned(scale_a), capi._aligned(scale_b)
+    return capi.m_major(scale_a), (capi.m_major(scale_b) if granularity == "blockwise_1d1d" else
+                                   capi._aligned(scale_b))
 
 
 def _fp8_gemm_shape(a, b_kmajor, scale_a, scale_b, out_dtype):
-    m, n, _ = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
-    return (m, n), out_dtype
+    m, n, _, granularity = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
+    return (m, n), out_dtype, granularity
 
 
-def _fp8_gemm_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, *, stream):
-    (m, n), k = c.shape, a.shape[1]
-    a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
-    if m == 0:
-        return
-    granularity = capi.scale_granularity(m, n, scale_a, scale_b, k=k)
-    if granularity == "blockwise":
-        scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
-    elif granularity == "blockwise_1d1d":
-        scale_a, scale_b = _m_major(scale_a), _m_major(scale_b)
-    elif granularity == "rowwise":
-        scale_a, scale_b = _rowwise_scale_arg(scale_a), _rowwise_scale_arg(scale_b)
-    else:
-        scale_a, scale_b = scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous()
-    capi.fp8_gemm(a, b_kmajor, c, scale_a, scale_b, stream=stream)
+def _fp8_gemm_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, granularity, *, stream):
+    if c.shape[0] > 0:
+        capi.fp8_gemm(a.contiguous(), b_kmajor.contiguous(), c, *_kernel_scales(granularity, scale_a, scale_b),
+                      stream=stream)
 
 
 _define_op("fp8_gemm", "(Tensor a, Tensor b_kmajor, Tensor scale_a, Tensor scale_b, ScalarType out_dtype) -> Tensor",
@@ -668,24 +655,19 @@ def fp8_gemm(a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor, sca
 
 
 def _fp8_bias_act_shape(a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype):
-    m, n, k = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
-    if capi.scale_granularity(m, n, scale_a, scale_b, k=k) in ("blockwise", "blockwise_1d1d"):
+    m, n, _, granularity = capi.check_operands(a, b_kmajor, out_dtype, scales=(scale_a, scale_b))
+    if granularity in ("blockwise", "blockwise_1d1d"):
         raise capi.B200HgemmError("fp8_gemm_bias_act: blockwise scales have no bias + activation kernel (per-tensor or "
                                   "rowwise scales only; run fp8_gemm and add the bias)")
     capi.check_bias(bias, n, out_dtype)
     capi.activation_code(activation)
-    return (m, n), out_dtype
+    return (m, n), out_dtype, granularity
 
 
-def _fp8_bias_act_launch(c, a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype, *, stream):
-    (m, n), k = c.shape, a.shape[1]
-    if _bias_act_empty(c, k, bias, activation):
-        return
-    if capi.scale_granularity(m, n, scale_a, scale_b, k=k) == "rowwise":
-        scale_a, scale_b = _rowwise_scale_arg(scale_a), _rowwise_scale_arg(scale_b)
-    else:
-        scale_a, scale_b = scale_a.reshape(1).contiguous(), scale_b.reshape(1).contiguous()
-    capi.gemm_bias_act(a.contiguous(), b_kmajor.contiguous(), c, bias, activation, scale_a, scale_b, stream=stream)
+def _fp8_bias_act_launch(c, a, b_kmajor, scale_a, scale_b, bias, activation, out_dtype, granularity, *, stream):
+    if not _bias_act_empty(c, a.shape[1], bias, activation):
+        capi.gemm_bias_act(a.contiguous(), b_kmajor.contiguous(), c, bias, activation,
+                           *_kernel_scales(granularity, scale_a, scale_b), stream=stream)
 
 
 _define_op("fp8_gemm_bias_act",
@@ -722,14 +704,6 @@ def quantize_e4m3_rowwise_reference(x: torch.Tensor) -> tuple[torch.Tensor, torc
     return q, scale
 
 
-def _blockwise_scale(lead, m: int, nkb: int, device) -> torch.Tensor:
-    """An empty blockwise scale [(B,) M, nkb] in the layout of the reference's: the view
-    ``buf[..., :M].transpose(-2, -1)`` of a [(B,) nkb, ld_a] buffer, ld_a = M rounded up to 4, which the block-scaled
-    GEMMs read in place."""
-    buf = torch.empty((*lead, nkb, -(-m // 4) * 4), dtype=torch.float32, device=device)
-    return buf[..., :m].transpose(-2, -1)
-
-
 def quantize_e4m3_blockwise_reference(x: torch.Tensor, masked_m: torch.Tensor | None = None
                                       ) -> tuple[torch.Tensor, torch.Tensor]:
     """:func:`quantize_e4m3_blockwise` as a composition of torch ops. ``masked_m`` changes nothing here: every row is
@@ -741,9 +715,7 @@ def quantize_e4m3_blockwise_reference(x: torch.Tensor, masked_m: torch.Tensor | 
     xb = nn.functional.pad(x.float(), (0, nkb * capi.BLOCK - k)).view(*lead, m, nkb, capi.BLOCK)
     scale = (xb.abs().amax(dim=-1) / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny)
     q = (xb / scale[..., None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).view(*lead, m, nkb * capi.BLOCK)
-    buf = torch.empty((*lead, nkb, -(-m // 4) * 4), dtype=torch.float32, device=x.device)
-    buf[..., :m].copy_(scale.transpose(-2, -1))
-    return q[..., :k].contiguous(), buf[..., :m].transpose(-2, -1)
+    return q[..., :k].contiguous(), capi.empty_m_major(lead, m, nkb, x.device).copy_(scale)
 
 
 def silu_mul_quantize_e4m3_blockwise_reference(h: torch.Tensor, masked_m: torch.Tensor | None = None
@@ -804,7 +776,7 @@ def _blockwise_outputs(x, k: int, masked_m):
     *lead, m, _ = x.shape
     _check_masked_m(masked_m, lead[0] if lead else 1)
     return (x.new_empty((*lead, m, k), dtype=torch.float8_e4m3fn),
-            _blockwise_scale(lead, m, capi.num_k_blocks(k), x.device))
+            capi.empty_m_major(lead, m, capi.num_k_blocks(k), x.device))
 
 
 def _quantize_e4m3_blockwise_outputs(x, masked_m=None):
@@ -1071,8 +1043,8 @@ def quantize_e4m3_blockwise_dual(x: torch.Tensor) -> tuple[torch.Tensor, torch.T
     rows, cols = x.shape
     q = x.new_empty((rows, cols), dtype=torch.float8_e4m3fn)
     q_t = x.new_empty((cols, capi.dual_ld_t(rows)), dtype=torch.float8_e4m3fn)
-    scale = _blockwise_scale((), rows, capi.num_k_blocks(cols), x.device)
-    scale_t = _blockwise_scale((), cols, capi.num_k_blocks(rows), x.device)
+    scale = capi.empty_m_major((), rows, capi.num_k_blocks(cols), x.device)
+    scale_t = capi.empty_m_major((), cols, capi.num_k_blocks(rows), x.device)
     with torch.cuda.device(x.device):
         capi.quantize_e4m3_blockwise_dual(x.contiguous(), q, scale, q_t, scale_t,
                                           stream=torch.cuda.current_stream(x.device).cuda_stream)
@@ -1320,7 +1292,7 @@ def _fp8_grouped_launch(c, a, b_kmajor, scale_a, scale_b, offs, out_dtype, *, st
     if b_kmajor.shape[0] == 0 or c.shape[0] == 0:   # no group or no row
         return
     a, b_kmajor, offs = a.contiguous(), b_kmajor.contiguous(), offs.contiguous()
-    scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
+    scale_a, scale_b = _kernel_scales("blockwise", scale_a, scale_b)   # the only form the shape check accepts
     capi.fp8_grouped_gemm(a, b_kmajor, c, scale_a, scale_b, offs, stream=stream)
 
 
@@ -1348,7 +1320,7 @@ def _fp8_batched_launch(c, a, b_kmajor, scale_a, scale_b, out_dtype, masked_m=No
     if c.shape[0] == 0 or c.shape[1] == 0:   # no matrix or no row
         return
     a, b_kmajor = a.contiguous(), b_kmajor.contiguous()
-    scale_a, scale_b = _m_major(scale_a), _rowwise_scale_arg(scale_b)
+    scale_a, scale_b = _kernel_scales("blockwise", scale_a, scale_b)   # the only form the shape check accepts
     if masked_m is not None:
         masked_m = masked_m.contiguous()
     capi.fp8_batched_gemm(a, b_kmajor, c, scale_a, scale_b, masked_m=masked_m, stream=stream)

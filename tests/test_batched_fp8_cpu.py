@@ -264,7 +264,7 @@ def test_batched_quantiser_is_the_2d_quantiser_on_each_matrix_with_in_place_stri
         assert q.dtype == E4 and q.shape == x.shape and q.is_contiguous()
         assert s.shape == (bsz, m, nkb) and s.dtype == torch.float32
         assert s.stride() == (nkb * ld, 1, ld) and s.untyped_storage().nbytes() == 4 * bsz * nkb * ld
-        assert capi.batched_blockwise_ld_a(s) == ld
+        assert capi.blockwise_ld_a(s) == ld
         for b in range(bsz):
             q2, s2 = ops.quantize_e4m3_blockwise(x[b])
             assert torch.equal(q[b].view(torch.uint8), q2.view(torch.uint8)) and torch.equal(s[b], s2), (shape, b)
@@ -276,18 +276,18 @@ def test_batched_quantiser_is_the_2d_quantiser_on_each_matrix_with_in_place_stri
 def test_batched_ld_a_rules():
     buf = torch.zeros(3, 4, 100)                     # [B, nkb, ld_a] with ld_a = 100
     s = buf[:, :, :90].transpose(1, 2)
-    assert capi.batched_blockwise_ld_a(s) == 100
-    assert capi.batched_blockwise_ld_a(torch.zeros(3, 90, 4)) is None                          # row-major
-    assert capi.batched_blockwise_ld_a(torch.zeros(3, 4, 90).transpose(1, 2)) is None          # ld_a = 90: % 4
-    assert capi.batched_blockwise_ld_a(torch.zeros(4, 3, 100)[:, :, :90].transpose(0, 2).transpose(0, 1)) is None
+    assert capi.blockwise_ld_a(s) == 100
+    assert capi.blockwise_ld_a(torch.zeros(3, 90, 4)) is None                          # row-major
+    assert capi.blockwise_ld_a(torch.zeros(3, 4, 90).transpose(1, 2)) is None          # ld_a = 90: % 4
+    assert capi.blockwise_ld_a(torch.zeros(4, 3, 100)[:, :, :90].transpose(0, 2).transpose(0, 1)) is None
     gap = torch.zeros(3, 5, 100)                     # batch stride 500 != nkb * ld_a = 400
-    assert capi.batched_blockwise_ld_a(gap[:, :4, :90].transpose(1, 2)) is None
-    assert capi.batched_blockwise_ld_a(torch.zeros(3, 4, 100)[:2, :, :90].transpose(1, 2)) == 100   # fewer batches
+    assert capi.blockwise_ld_a(gap[:, :4, :90].transpose(1, 2)) is None
+    assert capi.blockwise_ld_a(torch.zeros(3, 4, 100)[:2, :, :90].transpose(1, 2)) == 100   # fewer batches
     short = torch.zeros(1190).as_strided((3, 90, 4), (400, 1, 100))   # B * nkb * ld_a = 1200 floats not readable
-    assert capi.batched_blockwise_ld_a(short) is None
-    assert capi.batched_blockwise_ld_a(torch.zeros(1200).as_strided((3, 90, 4), (400, 1, 100))) == 100
+    assert capi.blockwise_ld_a(short) is None
+    assert capi.blockwise_ld_a(torch.zeros(1200).as_strided((3, 90, 4), (400, 1, 100))) == 100
     one = torch.zeros(3, 1, 92)                      # one k-block: the batch stride is ld_a
-    assert capi.batched_blockwise_ld_a(one[:, :, :90].transpose(1, 2)) == 92
+    assert capi.blockwise_ld_a(one[:, :, :90].transpose(1, 2)) == 92
 
 
 def test_masked_forward_on_meta_tensors():

@@ -205,7 +205,7 @@ def test_row_stride_larger_than_m_and_quantiser_scales_in_place():
     counts = [5, 77, 0, 40, 100]
     rows = rows_of(counts, b, m)
     a, sa, bt, sb = randn_problem(b, m, n, k, 21)
-    assert capi.batched_blockwise_ld_a(sa) == -(-m // 4) * 4               # read in place, as the quantiser returns it
+    assert capi.blockwise_ld_a(sa) == -(-m // 4) * 4               # read in place, as the quantiser returns it
     for out_dtype in OUT:
         want = reference(a, sa, bt, sb, rows, out_dtype, 4)
         for view in (sa, batched_m_major(sa, 96), batched_m_major(sa, 1024)):

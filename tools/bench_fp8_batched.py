@@ -42,7 +42,7 @@ CASES = [(G, m, n, k, fill) for (n, k) in ((4096, 7168), (7168, 2048)) for m in 
 
 
 def operand_sets(g, m, n, k, counts, gen):
-    from cuda_l2_b200 import ops
+    from cuda_l2_b200 import capi, ops
 
     set_bytes = g * m * k + g * n * k + 2 * g * m * n + 2 * (g * m * k + g * n * k)
     nsets = max(2, min(8, -(-4 * L2_BYTES // set_bytes)))
@@ -60,8 +60,8 @@ def operand_sets(g, m, n, k, counts, gen):
                        ).bfloat16()
         # the grouped leg's operands: the valid tokens packed by expert, with their own quantisation's scales
         packed = torch.cat([a[e, :r] for e, r in enumerate(counts)])
-        packed_sa = ops._m_major(torch.cat([sa[e, :r] for e, r in enumerate(counts)]))
-        per_expert = [ops._m_major(sa[e, :r]) if r > 0 else None for e, r in enumerate(counts)]
+        packed_sa = capi.m_major(torch.cat([sa[e, :r] for e, r in enumerate(counts)]))
+        per_expert = [capi.m_major(sa[e, :r]) if r > 0 else None for e, r in enumerate(counts)]
         sets.append(dict(a=a, sa=sa, bt=bt, sb=sb, a16=a16, bt16=bt16, pa=packed, psa=packed_sa, sa_e=per_expert,
                          c=torch.empty((g, m, n), dtype=torch.bfloat16, device="cuda"),
                          pc=torch.empty((max(ends[-1], 1), n), dtype=torch.bfloat16, device="cuda"),

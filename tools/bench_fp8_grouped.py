@@ -43,7 +43,7 @@ RAGGED = (8, 8192, 2056, 2064)
 
 
 def operand_sets(g, t, n, k, starts, ends, gen):
-    from cuda_l2_b200 import ops
+    from cuda_l2_b200 import capi, ops
 
     set_bytes = t * k + g * n * k + 2 * t * n + 2 * (t * k + g * n * k)
     nsets = max(2, min(8, -(-4 * L2_BYTES // set_bytes)))
@@ -58,7 +58,7 @@ def operand_sets(g, t, n, k, starts, ends, gen):
         for e in range(g):
             bt16[e] = (bt[e].float() * sb[e].repeat_interleave(128, dim=0)[:n].repeat_interleave(128, dim=1)[:, :k]
                        ).bfloat16()
-        per_expert = [ops._m_major(sa[r0:r1]) if r1 > r0 else None for r0, r1 in zip(starts, ends)]
+        per_expert = [capi.m_major(sa[r0:r1]) if r1 > r0 else None for r0, r1 in zip(starts, ends)]
         sets.append(dict(a=a, sa=sa, bt=bt, sb=sb, a16=a16, bt16=bt16, sa_e=per_expert, nkb=nkb,
                          c=torch.empty((t, n), dtype=torch.bfloat16, device="cuda")))
     return sets
