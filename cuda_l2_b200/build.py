@@ -16,6 +16,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
   the input gradient and the K-grouped kernels of the weight gradient (csrc/b200_grouped_bwd.h; no public symbol)
 * ``libb200_epilogue.so`` — the 2-D fp16 / bf16 / e4m3 GEMM with a fused bias + ReLU / tanh-GELU epilogue
   (csrc/b200_epilogue.h; no public symbol)
+* ``libb200_wgrad_accum.so`` — weight gradients added into fp32 main-grad buffers by the GEMM epilogue: the 16-bit
+  K-grouped, e4m3 rowwise and e4m3 1 x 128 kernels (csrc/b200_wgrad_accum.h; no public symbol)
 * ``libb200_quant.so``  — the one-pass e4m3 quantisers of FP8 activations: per tensor, rowwise, 1 x 128 blocks and
   SwiGLU + 1 x 128 blocks (csrc/b200_quant.h; no public symbol)
 * ``libb200_quant_dual.so`` — the dual-orientation rowwise e4m3 quantiser of FP8 training: x and x^T quantised from
@@ -103,6 +105,9 @@ BLOCK_VARIANTS = (5, 6)   # block-scaled e4m3 with fp16 / bf16 output (the GemmT
 BWD_VARIANTS = (0, 2)     # the grouped backward: fp16 and bf16, both with fp32 accumulation (the GemmType index)
 EPILOGUE_VARIANTS = (0, 2, 3, 4)   # bias + activation: fp16, bf16, e4m3 to fp16, e4m3 to bf16 (the GemmType index)
 BLOCK_1D1D_VARIANTS = (7, 8)      # 1 x 128 scales on both operands: e4m3 to fp16 / bf16 (the GemmType index)
+# fp32 weight-gradient accumulation: K-grouped fp16 and bf16, e4m3 rowwise, e4m3 1 x 128 (the GemmType index; one
+# object per e4m3 family, whose fp32 output does not depend on the 16-bit flavour)
+WGRAD_ACCUM_VARIANTS = (0, 2, 3, 7)
 
 
 def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, list[str]]]:
@@ -115,8 +120,9 @@ def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, lis
 # compiles its 16-bit kernels (b200_hgemm_capi.cu) and its e4m3 ones (b200_fp8_capi.cu) in parallel; the tile-list
 # libraries compile one source per variant (31 kernels each for the 16-bit variants, 17 for the block-scaled ones), and
 # so does libb200_nn.so (43 kernels per 16-bit variant), libb200_grouped_bwd.so (56 per variant: 28 configurations
-# times two kinds), libb200_epilogue.so (46 per variant: libb200_hgemm.so's (configuration, K-mode) pairs) and
-# libb200_fp8block_1d1d.so (19 per output type, libb200_fp8block.so's configurations and K-modes).
+# times two kinds), libb200_epilogue.so (46 per variant: libb200_hgemm.so's (configuration, K-mode) pairs),
+# libb200_fp8block_1d1d.so (19 per output type, libb200_fp8block.so's configurations and K-modes) and
+# libb200_wgrad_accum.so (28 K-grouped kernels per 16-bit variant, 46 rowwise e4m3 ones and 19 1 x 128 ones).
 LIBRARIES = {
     "capi": ("libb200_hgemm.so", [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], []),
     "fp8block": ("libb200_fp8block.so", [(CSRC / "b200_fp8_block_capi.cu", [])], []),
@@ -128,6 +134,7 @@ LIBRARIES = {
     "nn": ("libb200_nn.so", _per_variant("b200_nn.cu", VARIANTS), []),
     "grouped_bwd": ("libb200_grouped_bwd.so", _per_variant("b200_grouped_bwd.cu", BWD_VARIANTS), []),
     "epilogue": ("libb200_epilogue.so", _per_variant("b200_epilogue.cu", EPILOGUE_VARIANTS), []),
+    "wgrad_accum": ("libb200_wgrad_accum.so", _per_variant("b200_wgrad_accum.cu", WGRAD_ACCUM_VARIANTS), []),
     "quant": ("libb200_quant.so", [(CSRC / "b200_quant.cu", [])], []),
     "quant_dual": ("libb200_quant_dual.so", [(CSRC / "b200_quant_dual.cu", [])], []),
     "quant_block_dual": ("libb200_quant_block_dual.so", [(CSRC / "b200_quant_block_dual.cu", [])], []),

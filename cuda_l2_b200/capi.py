@@ -109,6 +109,7 @@ QUANT_LIB = "libb200_quant.so"               # csrc/b200_quant.h
 QUANT_DUAL_LIB = "libb200_quant_dual.so"     # csrc/b200_quant_dual.h
 FP8BLOCK_1D1D_LIB = "libb200_fp8block_1d1d.so"       # csrc/b200_fp8_block_1d1d.h
 QUANT_BLOCK_DUAL_LIB = "libb200_quant_block_dual.so"  # csrc/b200_quant_block_dual.h
+WGRAD_ACCUM_LIB = "libb200_wgrad_accum.so"   # csrc/b200_wgrad_accum.h
 _QUANT_BLOCK_DUAL = ([_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp], _i)
 _QUANT_BLOCKWISE = ([_i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp], _i)
 INTERNAL_ABI = {
@@ -157,6 +158,16 @@ INTERNAL_ABI = {
         "cuda_l2_b200_quant_block_dual_e4m3_128x128": _QUANT_BLOCK_DUAL,
         "cuda_l2_b200_quant_block_dual_launch_count": ([], ctypes.c_ulonglong),
         "cuda_l2_b200_quant_block_dual_strerror": ([_i], ctypes.c_char_p),
+    },
+    WGRAD_ACCUM_LIB: {
+        "cuda_l2_b200_wgrad_accum_grouped": _BWD_RUN,
+        "cuda_l2_b200_wgrad_accum_fp8": ([_i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_wgrad_accum_grouped_select": _BWD_SELECT,
+        "cuda_l2_b200_wgrad_accum_fp8_select": ([_i, _i, _i, _i, _ip, _ip, _ip], _i),
+        "cuda_l2_b200_wgrad_accum_prewarm": ([_vp], _i),
+        "cuda_l2_b200_wgrad_accum_release": ([], _i),
+        "cuda_l2_b200_wgrad_accum_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_wgrad_accum_strerror": ([_i], ctypes.c_char_p),
     },
 }
 _TABLES = {**ABI, **INTERNAL_ABI}
@@ -1212,6 +1223,97 @@ def epilogue_release() -> None:
 
 def epilogue_launch_count() -> int:
     return int(epilogue_lib().cuda_l2_b200_epilogue_launch_count())
+
+
+# ---------------------------------------------------------------- fp32 weight-gradient accumulation
+#                                                                  (libb200_wgrad_accum.so)
+WGRAD_ACCUM_FORMS = {"rowwise": 1, "blockwise_1d1d": 3}   # the scale forms of cuda_l2_b200_wgrad_accum_fp8
+
+
+def wgrad_accum_lib() -> ctypes.CDLL:
+    """libb200_wgrad_accum.so: weight gradients added into fp32 buffers by the GEMM epilogue (csrc/b200_wgrad_accum.h,
+    no public ABI)."""
+    return load(WGRAD_ACCUM_LIB)
+
+
+def check_main_grad(main_grad, shape: tuple, device, what: str = "main_grad") -> None:
+    """B200HgemmError unless ``main_grad`` is what the accumulating kernels add into: an fp32 tensor of ``shape``,
+    contiguous, on ``device`` (shape, dtype and layout only on the meta device; 16-byte aligned on a real one)."""
+    import torch
+
+    if main_grad is None:
+        raise B200HgemmError(f"{what} is missing: an fp32 tensor of shape {list(shape)} on {device} is needed")
+    if (main_grad.dtype != torch.float32 or tuple(main_grad.shape) != tuple(shape) or main_grad.device != device
+            or not main_grad.is_contiguous()):
+        raise B200HgemmError(f"{what} must be a contiguous fp32 tensor of shape {list(shape)} on {device}, got "
+                             f"{main_grad.dtype} {list(main_grad.shape)} on {main_grad.device}"
+                             f"{'' if main_grad.is_contiguous() else ', not contiguous'}")
+    if main_grad.device.type != "meta" and main_grad.data_ptr() % 16:
+        raise B200HgemmError(f"{what} must be 16-byte aligned")
+
+
+def wgrad_accum_grouped(a, b, c32, offs, config_id: int | None = None, group_m: int = 0, max_ctas: int = 0,
+                        stream: int | None = None) -> None:
+    """c32[g] += a[start_g:end_g]^T @ b[start_g:end_g] for every group g, in fp32 with one rounding per element after
+    the whole sum (csrc/b200_wgrad_accum.h): :func:`gemm_grouped_wgrad`'s product, a [T,M] and b [T,N] fp16 or bf16,
+    offs the int32 group ends [G], c32 [G,M,N] fp32, all contiguous CUDA tensors. An empty group's matrix and, with
+    T == 0, all of c32 stay as they are, and T == 0 launches nothing. ``config_id`` pins one kernel configuration (one
+    with BN >= 64); default is :func:`gemm_grouped_wgrad`'s dispatcher."""
+    _contiguous_cuda(a=a, b=b, offs=offs)
+    g, t, m, n = check_grouped_wgrad_operands(a, b, offs)
+    check_main_grad(c32, (g, m, n), a.device, "c32")
+    fn = wgrad_accum_lib().cuda_l2_b200_wgrad_accum_grouped
+    _check(fn(_bwd_variant(a.dtype, "fp32"), -1 if config_id is None else config_id, a.data_ptr(), b.data_ptr(),
+              c32.data_ptr(), offs.data_ptr(), g, t, m, n, group_m, max_ctas, stream), fn)
+
+
+def wgrad_accum_fp8(a, b_kmajor, c32, scale_a, scale_b, stream: int | None = None, config_id: int | None = None,
+                    group_m: int = 0, splits: int = 1, max_ctas: int = 0) -> None:
+    """c32[M,N] += the e4m3 product of :func:`fp8_gemm` for ``a`` [M,K] and ``b_kmajor`` [N,K], in fp32 with one
+    rounding per element after the whole sum (csrc/b200_wgrad_accum.h): exactly the value fp8_gemm rounds to its output
+    is added. The scales are rowwise (``scale_a`` [M,1], ``scale_b`` [1,N], contiguous) or 1 x 128 on both operands
+    (``scale_a`` [M, ceil(K/128)], ``scale_b`` [N, ceil(K/128)], read in place as for :func:`fp8_gemm`); per-tensor and
+    128 x 128 scales have no accumulating kernel. ``config_id`` pins one kernel configuration (``splits``, ``group_m``
+    and ``max_ctas`` as for :func:`fp8_gemm`); default is :func:`fp8_gemm`'s dispatcher for those scales."""
+    import torch
+
+    _contiguous_cuda(a=a, b_kmajor=b_kmajor)
+    m, n, k, granularity = check_operands(a, b_kmajor, torch.bfloat16, "fp32", (scale_a, scale_b))
+    if granularity not in WGRAD_ACCUM_FORMS:
+        raise B200HgemmError(f"fp32 accumulation takes rowwise or 1 x 128 x 1 x 128 (blockwise_1d1d) scales, got "
+                             f"{granularity} scales")
+    check_main_grad(c32, (m, n), a.device, "c32")
+    args = _scale_args(granularity, scale_a, scale_b)
+    if granularity == "rowwise":
+        args = (args[0], 0, args[1], 0)
+    fn = wgrad_accum_lib().cuda_l2_b200_wgrad_accum_fp8
+    _check(fn(WGRAD_ACCUM_FORMS[granularity], -1 if config_id is None else config_id, a.data_ptr(),
+              b_kmajor.data_ptr(), c32.data_ptr(), *args, m, n, k, group_m, max_ctas, splits, stream), fn)
+
+
+def wgrad_accum_grouped_select(variant: int, g: int, t: int, m: int, n: int) -> tuple[int, int]:
+    """(config id, rasterisation group) of the dispatched :func:`wgrad_accum_grouped` call."""
+    return _select(wgrad_accum_lib().cuda_l2_b200_wgrad_accum_grouped_select, variant, g, t, m, n)
+
+
+def wgrad_accum_fp8_select(granularity: str, m: int, n: int, k: int) -> tuple[int, int, int]:
+    """(config id, rasterisation group, splits code) of the dispatched :func:`wgrad_accum_fp8` call."""
+    return _select(wgrad_accum_lib().cuda_l2_b200_wgrad_accum_fp8_select, WGRAD_ACCUM_FORMS[granularity], m, n, k)
+
+
+def wgrad_accum_prewarm(stream: int | None = None) -> None:
+    """Allocate libb200_wgrad_accum.so's split-K scratch for ``stream`` ahead of a CUDA-graph capture (a first split-K
+    or stream-K call inside a capture runs undivided without it)."""
+    _check(wgrad_accum_lib().cuda_l2_b200_wgrad_accum_prewarm(stream), "cuda_l2_b200_wgrad_accum_prewarm")
+
+
+def wgrad_accum_release() -> None:
+    """Free libb200_wgrad_accum.so's split-K scratch (no launch of it may be in flight)."""
+    _check(wgrad_accum_lib().cuda_l2_b200_wgrad_accum_release(), "cuda_l2_b200_wgrad_accum_release")
+
+
+def wgrad_accum_launch_count() -> int:
+    return int(wgrad_accum_lib().cuda_l2_b200_wgrad_accum_launch_count())
 
 
 # ------------------------------------------------------------------------------------------ e4m3 quantisers

@@ -469,10 +469,13 @@ struct LaunchArgs {
   int act;              // ... and the activation code
 };
 
-// The kernel's last argument: the scales, BiasAct<>'s BiasActArgs or BlockScaled1D1D<>'s Block1D1DArgs.
+// The kernel's last argument: the scales, BiasAct<>'s BiasActArgs, BlockScaled1D1D<>'s Block1D1DArgs, or AccumF32<>'s
+// AccumArgs (the wrapped kernel's argument and C, which is fp32).
 template <class Cfg>
 typename Cfg::EpiArgs epi_args(const LaunchArgs& a) {
-  if constexpr (bias_act<Cfg>()) return BiasActArgs{a.scales, a.bias, a.act};
+  if constexpr (accum_f32<Cfg>())
+    return typename Cfg::EpiArgs{epi_args<typename Cfg::AccumBase>(a), reinterpret_cast<float*>(a.c)};
+  else if constexpr (bias_act<Cfg>()) return BiasActArgs{a.scales, a.bias, a.act};
   else if constexpr (block_1d1d<Cfg>()) return Block1D1DArgs{a.scales, a.ld_b};
   else return a.scales;
 }
@@ -720,7 +723,8 @@ int launch_list(const void* A, const void* Bt, void* C, const int* list, int cou
   if (st != kOk || rows == 0) return st;
   const Elem elem = traits(kType).operand, output = traits(kType).output;
   if constexpr (k_grouped<Cfg>()) {
-    if (K == 0) {   // no row to reduce over: every matrix of C is zero
+    if (K == 0) {   // no row to reduce over: every matrix of C is zero (AccumF32<>: C stays as it is)
+      if constexpr (accum_f32<Cfg>()) return kOk;
       const cudaError_t e = cudaMemsetAsync(C, 0, size_t(count) * size_t(rows) * size_t(N) * elem_bytes(output),
                                             stream);
       return e == cudaSuccess ? kOk : int(e);

@@ -103,9 +103,9 @@ struct Config {
   static constexpr bool STREAM_K = CLUSTER_M_ * CLUSTER_N_ == 1 && BN_ >= 64 && M_REP_ == 1;
   static constexpr bool SPLIT_K = STREAM_K && CTA_GROUP_ == 1;
   // the variant wrappers below (BlockScaled<>, BlockScaled1D1D<>, Batched<>, Grouped<>, RowMajorB<>, GroupedK<>,
-  // BiasAct<>) override these
+  // BiasAct<>, AccumF32<>) override these
   static constexpr bool BLOCK_SCALED = false, BATCHED = false, GROUPED = false, ROW_MAJOR_B = false, K_GROUPED = false,
-                        BIAS_ACT = false, BLOCK_1D1D = false;
+                        BIAS_ACT = false, BLOCK_1D1D = false, ACCUM_F32 = false;
   using Cursor = NoBatches;   // the flat tile list the kernel walks (hgemm_schedule.cuh): none
   using EpiArgs = Scales;     // the kernel's last parameter
   static constexpr int EPI_BYTES = 8 * EPI_ROWS * 64 * 2;    // 8 consumer warps x one staging buffer (sized for EPI_N = 64)
@@ -347,6 +347,39 @@ __host__ __device__ __forceinline__ int ld_b_of(const E& e) {
   if constexpr (std::is_same_v<E, Block1D1DArgs>) return e.ld_b;
   else return 0;
 }
+
+// fp32 accumulation of the finished sum (libb200_wgrad_accum.so, the weight gradient into an fp32 main-grad buffer):
+// C32[m,n] = fp32(C32[m,n] + s(m,n)), one round-to-nearest-even addition per element, where s is exactly the fp32 value
+// the wrapped kernel rounds to its 16-bit output (the fp32 sum; e4m3 rowwise: fp32(fp32(acc * sb[n]) * sa[m]); 1 x 128
+// scales: the promoted sum). Only the finished sum is added, once: split-K partials, DSMEM tiles and stream-K register
+// images are those of the wrapped kernel, summed in their fixed order first. Nothing outside [M, N] (K-grouped:
+// [G, M, N]) is read or written, and an empty group of a K-grouped kernel leaves its matrix untouched. The final
+// writers read and write C32 directly from registers (or the reductions' float4s), 8 bytes per fragment pair: a quad of
+// lanes covers 32 contiguous bytes. Wraps the 16-bit K-grouped kernels (GroupedK<RowMajorB<>>), the 2-D e4m3 kernels
+// (rowwise scales) and the 1 x 128 block-scaled ones (BlockScaled1D1D<>). A wrapper, like BiasAct<>, so that the other
+// kernels and their names stay as they are; the kernel takes AccumArgs as its last parameter (hgemm_accum_kernel).
+template <class E>
+struct AccumArgs { E base; float* c32; };
+template <class Base>
+struct AccumF32 : Base {
+  static constexpr bool ACCUM_F32 = true;
+  using AccumBase = Base;
+  using EpiArgs = AccumArgs<typename Base::EpiArgs>;
+  static_assert(Base::ACC_F32 && !Base::BIAS_ACT && !Base::BATCHED && !Base::GROUPED &&
+                    (Base::K_GROUPED || (Base::E4M3 && !Base::ROW_MAJOR_B)) && (!Base::BLOCK_SCALED || Base::BLOCK_1D1D),
+                "fp32 accumulation: the K-grouped 16-bit kernels, the 2-D e4m3 ones and the 1 x 128 block-scaled ones");
+};
+template <class Cfg>
+__host__ __device__ constexpr bool accum_f32() { return Cfg::ACCUM_F32; }
+template <class E>
+__host__ __device__ __forceinline__ const Scales& scales_of(const AccumArgs<E>& e) { return scales_of(e.base); }
+template <class E>
+__host__ __device__ __forceinline__ int ld_b_of(const AccumArgs<E>& e) { return ld_b_of(e.base); }
+// The fp32 C of a kernel's EpiArgs: null for the kernels without one
+template <class E>
+__host__ __device__ __forceinline__ float* c32_of(const E&) { return nullptr; }
+template <class E>
+__host__ __device__ __forceinline__ float* c32_of(const AccumArgs<E>& e) { return e.c32; }
 
 // act(z) in fp32; `act` is warp-uniform. relu: max(z, +0.0) (+0.0 for -0.0 and NaN). gelu_tanh: 0.5 z (1 + tanhf(u)),
 // u = sqrt(2/pi) (z + 0.044715 z^3), torch's tanh approximation (F.gelu(approximate="tanh"), _addmm_activation), each
@@ -657,6 +690,83 @@ __device__ __forceinline__ void zero_tile_store(__half* __restrict__ c, int batc
   }
 }
 
+// One finished float4 of the split-K reductions added in place into C32 (AccumF32<> kernels), at a 16-byte aligned
+// address.
+__device__ __forceinline__ void accum_quad(float* __restrict__ dst, const float4& v) {
+  float4* p = reinterpret_cast<float4*>(dst);
+  float4 o = *p;
+  o.x = __fadd_rn(o.x, v.x); o.y = __fadd_rn(o.y, v.y);
+  o.z = __fadd_rn(o.z, v.z); o.w = __fadd_rn(o.w, v.w);
+  *p = o;
+}
+
+// One 64-row block of the plain (and stream-K owner) epilogue of an AccumF32<> unit: the finished sums of this warp's
+// rows row0 .. row0 + 15 and columns n0 .., scaled as the wrapped kernel scales them before its rounding (e4m3 rowwise:
+// fp32(fp32(acc * sb[n]) * sa[m]); per tensor: fp32(acc * fp32(sa * sb))), added into c32 [M, N] (the unit's own
+// matrix) straight from the registers. Rows at or past M and columns at or past N are not touched (N % 8 == 0: n < N
+// covers n + 1). The column scales are read where they are used, one float2 per column pair, so that nothing is held
+// across the accumulators. The pairs of a row go in groups of G: the group's G loads of C32 are issued back to back,
+// then its G additions and stores. Pair by pair, every load would wait for the previous pair's store (the compiler
+// cannot prove that they do not alias), one dependent global round trip per pair.
+template <class Cfg, class Reg, int NR>
+__device__ __forceinline__ void accum_block(const Reg (&d)[NR], int lane, int row0, int n0, int M, int N,
+                                           float* __restrict__ c32, const Scales& s, float scale) {
+  constexpr int PAIRS = NR / 4;                  // column pairs of one row
+  // pairs in flight, 2 G registers next to the accumulators; the rowwise e4m3 kernels also hold the column scales
+  constexpr int G_MAX = (Cfg::E4M3 && !block_scaled<Cfg>()) ? 2 : 8;
+  constexpr int G = PAIRS < G_MAX ? PAIRS : G_MAX;
+  static_assert(PAIRS % G == 0, "whole groups");
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {   // pairs 2c + h share row l/4 + 8h
+    const int m = row0 + frag_row(lane, h);
+    if (m >= M) continue;
+    [[maybe_unused]] float sa = 0.f;
+    if constexpr (Cfg::E4M3 && !block_scaled<Cfg>()) {
+      if (s.rowwise) sa = __ldg(s.a + m);
+    }
+    float* row = c32 + size_t(m) * N;
+#pragma unroll
+    for (int c0 = 0; c0 < PAIRS; c0 += G) {
+      float2 old[G];
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        const int n = n0 + frag_col(lane, 2 * (c0 + j) + h);
+        old[j] = n < N ? *reinterpret_cast<const float2*>(row + n) : make_float2(0.f, 0.f);
+      }
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        const int p = 2 * (c0 + j) + h;
+        const int n = n0 + frag_col(lane, p);
+        if (n >= N) continue;
+        float x = d[2 * p], y = d[2 * p + 1];
+        if constexpr (Cfg::E4M3 && !block_scaled<Cfg>()) {
+          if (s.rowwise) {   // warp-uniform
+            const float2 sb = __ldg(reinterpret_cast<const float2*>(s.b + n));
+            x = __fmul_rn(__fmul_rn(x, sb.x), sa);
+            y = __fmul_rn(__fmul_rn(y, sb.y), sa);
+          } else {
+            x = __fmul_rn(x, scale);
+            y = __fmul_rn(y, scale);
+          }
+        }
+        *reinterpret_cast<float2*>(row + n) = make_float2(__fadd_rn(old[j].x, x), __fadd_rn(old[j].y, y));
+      }
+    }
+  }
+}
+
+// The plain (and stream-K owner) epilogue of an AccumF32<> unit: accum_block for each of the warpgroup's MR 64-row blocks
+// (this warp's rows m_row0 + 64 r ..). The blocks are separate calls rather than a loop, which the compiler declines to
+// unroll around a body of this size: a block index that is not a constant would move the accumulators to local memory.
+template <class Cfg, class Reg, int MR, int NR>
+__device__ __forceinline__ void accum_epilogue(const Reg (&d)[MR][NR], int lane, int m_row0, int n0, int M, int N,
+                                               float* __restrict__ c32, const Scales& s) {
+  static_assert(MR == 1 || MR == 2, "one or two 64-row blocks per warpgroup");
+  const float scale = output_scale<Cfg>(s);
+  accum_block<Cfg>(d[0], lane, m_row0, n0, M, N, c32, s, scale);
+  if constexpr (MR == 2) accum_block<Cfg>(d[1], lane, m_row0 + 64, n0, M, N, c32, s, scale);
+}
+
 // Split-K epilogue (CTA_GROUP == 1, one (tile, split) unit per CTA, all units resident at once).
 //   phase 1  every split writes its 128 x BN fp32 partial tile to the workspace slot (tile, split);
 //   barrier  a per-tile arrival counter in global memory (release/acquire at gpu scope);
@@ -721,6 +831,10 @@ __device__ __forceinline__ void splitk_epilogue(const Reg (&d)[NR], int e, int r
       }
       scale_quad<Cfg>(acc, scale, scales, gm, gn);
       bias_act_quad<Cfg>(acc, epi, gn);
+      if constexpr (accum_f32<Cfg>()) {
+        accum_quad(epi.c32 + size_t(gm) * N + gn, acc);
+        continue;
+      }
       uint2 out;
       out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
       out.y = pack_out_x2_rn<Cfg::BF16>(acc.z, acc.w);
@@ -785,6 +899,10 @@ __device__ __forceinline__ void cluster_splitk_reduce(int e, int split, int spli
     }
     scale_quad<Cfg>(acc, scale, scales, gm, gn);
     bias_act_quad<Cfg>(acc, epi, gn);
+    if constexpr (accum_f32<Cfg>()) {
+      accum_quad(epi.c32 + size_t(gm) * N + gn, acc);
+      continue;
+    }
     uint2 out;
     out.x = pack_out_x2_rn<Cfg::BF16>(acc.x, acc.y);
     out.y = pack_out_x2_rn<Cfg::BF16>(acc.z, acc.w);
@@ -939,10 +1057,24 @@ hgemm_block_1d1d_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
 #include "hgemm_tn_kernel_body.inc"
 }
 
+// The same adding into an fp32 C (AccumF32<>): the parameters of hgemm_tn_kernel, AccumArgs (the wrapped kernel's
+// EpiArgs and the fp32 C) last. tmap_c and c_raw are not written.
+template <class Cfg, int KMODE = kPlain>
+__global__ void __launch_bounds__(kNumThreads, 1)
+hgemm_accum_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                   const __grid_constant__ CUtensorMap tmap_c, int M, int N, int K, int group_m, int splits_arg,
+                   int aux_arg, float* __restrict__ splitk_ws, unsigned* __restrict__ splitk_ctr,
+                   __half* __restrict__ c_raw, uint64_t hint_a, uint64_t hint_b, typename Cfg::EpiArgs epi) {
+  static_assert(accum_f32<Cfg>(), "an AccumF32<> configuration");
+  const Scales& scales = scales_of(epi);
+#include "hgemm_tn_kernel_body.inc"
+}
+
 // The kernel of (Cfg, KMODE).
 template <class Cfg, int KMODE>
 constexpr auto kernel_of() {
-  if constexpr (bias_act<Cfg>()) return &hgemm_bias_act_kernel<Cfg, KMODE>;
+  if constexpr (accum_f32<Cfg>()) return &hgemm_accum_kernel<Cfg, KMODE>;
+  else if constexpr (bias_act<Cfg>()) return &hgemm_bias_act_kernel<Cfg, KMODE>;
   else if constexpr (block_1d1d<Cfg>()) return &hgemm_block_1d1d_kernel<Cfg, KMODE>;
   else return &hgemm_tn_kernel<Cfg, KMODE>;
 }

@@ -72,6 +72,11 @@ the nearest grid shape — so deployment is a plain operator:
   csrc/b200_quant_dual.h): the two K-major e4m3 operands FP8 training needs of each tensor. Inference only itself.
 * :func:`fp8_linear` and :class:`B200Fp8TrainLinear`: ``x @ W^T`` trained in FP8, a rowwise-scaled e4m3 forward and
   backward (three ``fp8_gemm`` calls per step) over a trainable 16-bit weight.
+* ``fuse_wgrad_accumulation=True`` on :class:`B200Linear`, :class:`B200Fp8TrainLinear` and :class:`B200GroupedLinear`
+  (and ``fp8_linear(..., main_grad=...)``): the backward adds dW into the weight's fp32 ``main_grad`` in the GEMM
+  epilogue (libb200_wgrad_accum.so, csrc/b200_wgrad_accum.h) and returns no weight gradient. The plain functions
+  :func:`wgrad_accumulate_`, :func:`grouped_wgrad_accumulate_` and :func:`fp8_gemm_accumulate_` are the pieces; they are
+  not operators.
 
 There is no CPU or PyTorch fallback on the forward path: a non-CUDA tensor, a missing library or a non-H100 device
 raises. Backward (training is not what the reference targets) is provided through the same kernels, so a fine-tuning
@@ -382,19 +387,25 @@ def _grouped_linear_shape(x, w, offs, acc="fp32"):
     return _hgemm_grouped_shape(x, w, offs, acc)
 
 
+def _grouped_input_grad(g, x, w, offs, acc):
+    """dX of the grouped product for the contiguous output gradient ``g``: dX[s:e] = dY[s:e] W[g] (W [G, N, K] is a
+    row-major B over the reduced N, read in place), into zeros, so that rows at or past the last end stay zero."""
+    grad_x = torch.zeros_like(x)
+    if x.numel() > 0 and g.shape[1] > 0:   # an empty reduction (N == 0) leaves dX zero
+        with torch.cuda.device(x.device):
+            capi.gemm_grouped_nn(g, w.contiguous(), grad_x, offs.contiguous(), acc,
+                                 stream=torch.cuda.current_stream(x.device).cuda_stream)
+    return grad_x
+
+
 def _grouped_linear_backward(ctx, grad_y):
     x, w, offs = ctx.saved_tensors
     grad_x = grad_w = None
     g = grad_y.contiguous()
-    # Y[s:e] = X[s:e] W[g]^T  =>  dX[s:e] = dY[s:e] W[g] (W [G, N, K] is a row-major B over the reduced N, read in
-    # place), dW[g] = dY[s:e]^T X[s:e] (the K-grouped product). Rows of dY at or past the last end are never read.
+    # Y[s:e] = X[s:e] W[g]^T  =>  dX[s:e] = dY[s:e] W[g], dW[g] = dY[s:e]^T X[s:e] (the K-grouped product). Rows of dY at
+    # or past the last end are never read.
     if ctx.needs_input_grad[0]:
-        # into zeros: rows of dX at or past the last end get no group and stay zero
-        grad_x = torch.zeros_like(x)
-        if x.numel() > 0 and g.shape[1] > 0:   # an empty reduction (N == 0) leaves dX zero
-            with torch.cuda.device(x.device):
-                capi.gemm_grouped_nn(g, w.contiguous(), grad_x, offs.contiguous(), ctx.acc,
-                                     stream=torch.cuda.current_stream(x.device).cuda_stream)
+        grad_x = _grouped_input_grad(g, x, w, offs, ctx.acc)
     if ctx.needs_input_grad[1]:
         grad_w = torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(g, x, offs, ctx.acc)
     return grad_x, grad_w, None, None
@@ -420,18 +431,128 @@ def grouped_linear(x: torch.Tensor, w: torch.Tensor, offs: torch.Tensor, acc: st
     return torch.ops.cuda_l2_b200.grouped_linear(x, w, offs, acc)
 
 
+# ------------------------------------------------------- fp32 weight-gradient accumulation (libb200_wgrad_accum.so)
+def _on_stream(t: torch.Tensor):
+    """(device context, torch's current stream handle) for a launch on ``t``'s device."""
+    return torch.cuda.device(t.device), torch.cuda.current_stream(t.device).cuda_stream
+
+
+def grouped_wgrad_accumulate_(main_grad: torch.Tensor, grad_y: torch.Tensor, x: torch.Tensor,
+                              offs: torch.Tensor) -> torch.Tensor:
+    """``main_grad[g] += grad_y[start_g:end_g]^T @ x[start_g:end_g]`` for every group g, in place, and returns
+    ``main_grad``: the weight gradient of :func:`grouped_linear` added into an fp32 buffer [G, N, K] by the epilogue of
+    its K-grouped kernel (csrc/b200_wgrad_accum.h). ``grad_y`` [T, N] and ``x`` [T, K] fp16 or bf16, ``offs`` the int32
+    group ends [G] on the GPU. Each element gets exactly the fp32 sum that :func:`hgemm_grouped_wgrad` rounds, added
+    with one rounding; an empty group's matrix and, with T == 0, all of ``main_grad`` stay as they are, bits included.
+    Not an operator and not differentiable: it is the fused layers' backward."""
+    g, t, n, k = capi.check_grouped_wgrad_operands(grad_y, x, offs)
+    capi.check_main_grad(main_grad, (g, n, k), grad_y.device)
+    if main_grad.device.type != "meta":
+        ctx, stream = _on_stream(main_grad)
+        with ctx:
+            capi.wgrad_accum_grouped(grad_y.contiguous(), x.contiguous(), main_grad, offs.contiguous(), stream=stream)
+    return main_grad
+
+
+def wgrad_accumulate_(main_grad: torch.Tensor, grad_y: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """``main_grad += grad_y^T @ x`` in place for a 16-bit linear layer, and returns ``main_grad``: ``grad_y`` [T, N]
+    and ``x`` [T, K] fp16 or bf16, ``main_grad`` [N, K] fp32 (the weight's shape). Any token count T; T == 0 changes
+    nothing and launches nothing. :func:`grouped_wgrad_accumulate_` with one group, both operands read in place."""
+    if grad_y.dim() != 2 or x.dim() != 2:
+        raise capi.B200HgemmError(f"wgrad_accumulate_: grad_y [T, N] and x [T, K] expected, got {tuple(grad_y.shape)} "
+                                  f"and {tuple(x.shape)}")
+    t, n = grad_y.shape
+    capi.check_main_grad(main_grad, (n, x.shape[1]), grad_y.device)
+    offs = _token_ends(t, 1, grad_y.device) if t > 0 else grad_y.new_empty((1,), dtype=torch.int32)
+    grouped_wgrad_accumulate_(main_grad.view(1, *main_grad.shape), grad_y, x, offs)
+    return main_grad
+
+
+def fp8_gemm_accumulate_(c32: torch.Tensor, a: torch.Tensor, b_kmajor: torch.Tensor, scale_a: torch.Tensor,
+                         scale_b: torch.Tensor) -> torch.Tensor:
+    """``c32 +=`` the e4m3 product :func:`fp8_gemm` computes for ``a`` [M, K] and ``b_kmajor`` [N, K], in place, and
+    returns ``c32`` ([M, N] fp32): exactly the fp32 value fp8_gemm rounds to its output is added, with one rounding. The
+    scales are rowwise (``scale_a`` [M, 1], ``scale_b`` [1, N]: the weight gradient of rowwise :func:`fp8_linear`) or
+    1 x 128 on both operands (``scale_a`` [M, ceil(K/128)], ``scale_b`` [N, ceil(K/128)], in any layout: the blockwise
+    one); per-tensor and 128 x 128 scales raise. Not an operator and not differentiable."""
+    m, n, k, granularity = capi.check_operands(a, b_kmajor, torch.bfloat16, scales=(scale_a, scale_b))
+    if granularity not in capi.WGRAD_ACCUM_FORMS:
+        raise capi.B200HgemmError(f"fp8_gemm_accumulate_ takes rowwise or 1 x 128 x 1 x 128 scales, got {granularity}")
+    capi.check_main_grad(c32, (m, n), a.device, "c32")
+    if c32.device.type != "meta" and m > 0 and k > 0:
+        ctx, stream = _on_stream(c32)
+        with ctx:
+            capi.wgrad_accum_fp8(a.contiguous(), b_kmajor.contiguous(), c32,
+                                 *_kernel_scales(granularity, scale_a, scale_b), stream=stream)
+    return c32
+
+
+def _fused_main_grad(weight: torch.Tensor) -> torch.Tensor:
+    """``weight.main_grad`` of a layer with ``fuse_wgrad_accumulation``: an fp32 tensor of the weight's shape,
+    contiguous, on its device. B200HgemmError naming the rule otherwise."""
+    main_grad = getattr(weight, "main_grad", None)
+    capi.check_main_grad(main_grad, tuple(weight.shape), weight.device, "weight.main_grad (fuse_wgrad_accumulation)")
+    return main_grad
+
+
+class _LinearWgradAccumFunction(torch.autograd.Function):
+    """``hgemm(x2, weight)`` whose backward adds dW into ``weight.main_grad`` (:func:`wgrad_accumulate_`), read when
+    the backward runs as Megatron-LM reads it, and returns no gradient for the weight; a frozen weight gets nothing
+    added. The forward and dX are the ``hgemm`` operator's, bit for bit."""
+
+    @staticmethod
+    def forward(ctx, x2, weight, acc):
+        ctx.acc, ctx.weight = acc, weight
+        ctx.save_for_backward(x2, weight)
+        return torch.ops.cuda_l2_b200.hgemm(x2, weight, acc)
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        x2, weight = ctx.saved_tensors
+        grad_x, _ = _product_grads(x2, weight, grad_y, ctx.needs_input_grad[0], False)
+        if ctx.needs_input_grad[1]:
+            wgrad_accumulate_(_fused_main_grad(ctx.weight), grad_y.contiguous(), x2)
+        return grad_x, None, None
+
+
+class _GroupedLinearWgradAccumFunction(torch.autograd.Function):
+    """:func:`grouped_linear` whose backward adds dW into ``w.main_grad`` (:func:`grouped_wgrad_accumulate_`), read
+    when the backward runs, and returns no gradient for the weight stack; a frozen stack gets nothing added. The forward
+    and dX are ``grouped_linear``'s, bit for bit."""
+
+    @staticmethod
+    def forward(ctx, x, w, offs, acc):
+        ctx.acc, ctx.weight = acc, w
+        ctx.save_for_backward(x, w, offs)
+        return torch.ops.cuda_l2_b200.hgemm_grouped(x, w, offs, acc)
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        x, w, offs = ctx.saved_tensors
+        g = grad_y.contiguous()
+        grad_x = _grouped_input_grad(g, x, w, offs, ctx.acc) if ctx.needs_input_grad[0] else None
+        if ctx.needs_input_grad[1]:
+            grouped_wgrad_accumulate_(_fused_main_grad(ctx.weight), g, x, offs)
+        return grad_x, None, None, None
+
+
 class B200GroupedLinear(nn.Module):
     """Trainable experts of a mixture-of-experts layer: G ``nn.Linear`` weights [N, K] without bias, stacked as the
     Parameter ``weight`` [G, N, K] (fp16 or bf16). ``forward(x, offs)`` takes the tokens sorted by expert, ``x`` [T, K],
     and the int32 cumulative group ends ``offs`` [G] on the GPU, and runs :func:`grouped_linear`: no host
     synchronisation in either direction. Rows at or past ``offs[-1]`` of the result are unspecified. Needs
-    K % 8 == 0 and N % 8 == 0."""
+    K % 8 == 0 and N % 8 == 0.
+
+    ``fuse_wgrad_accumulation=True``: the weight must carry ``weight.main_grad``, an fp32 tensor of its shape (checked
+    in forward); the backward adds dW into it (:func:`grouped_wgrad_accumulate_`) and leaves ``weight.grad`` None. y
+    and dX are the unfused layer's, bit for bit."""
 
     def __init__(self, num_groups: int, in_features: int, out_features: int, device=None,
-                 dtype: torch.dtype = torch.bfloat16, acc: str = "fp32"):
+                 dtype: torch.dtype = torch.bfloat16, acc: str = "fp32", fuse_wgrad_accumulation: bool = False):
         super().__init__()
         self._check(num_groups, in_features, out_features, dtype, acc)
         self.num_groups, self.in_features, self.out_features, self.acc = num_groups, in_features, out_features, acc
+        self.fuse_wgrad_accumulation = fuse_wgrad_accumulation
         self.weight = nn.Parameter(torch.empty((num_groups, out_features, in_features), device=device, dtype=dtype))
         bound = 1.0 / (in_features ** 0.5)
         with torch.no_grad():
@@ -445,7 +566,8 @@ class B200GroupedLinear(nn.Module):
         capi._bwd_variant(dtype, acc)
 
     @classmethod
-    def from_weights(cls, w: torch.Tensor, acc: str = "fp32") -> "B200GroupedLinear":
+    def from_weights(cls, w: torch.Tensor, acc: str = "fp32",
+                     fuse_wgrad_accumulation: bool = False) -> "B200GroupedLinear":
         """The experts of a weight stack ``w`` [G, N, K] (a Parameter or a tensor), sharing its storage: no copy."""
         if w.dim() != 3:
             raise capi.B200HgemmError(f"from_weights needs a weight stack [G, N, K], got {list(w.shape)}")
@@ -454,15 +576,20 @@ class B200GroupedLinear(nn.Module):
         new = cls.__new__(cls)
         nn.Module.__init__(new)
         new.num_groups, new.in_features, new.out_features, new.acc = g, k, n, acc
+        new.fuse_wgrad_accumulation = fuse_wgrad_accumulation
         new.weight = w if isinstance(w, nn.Parameter) else nn.Parameter(w)
         return new
 
     def forward(self, x: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+        if self.fuse_wgrad_accumulation:
+            _fused_main_grad(self.weight)
+            if torch.is_grad_enabled() and (x.requires_grad or self.weight.requires_grad):
+                return _GroupedLinearWgradAccumFunction.apply(x, self.weight, offs, self.acc)
         return grouped_linear(x, self.weight, offs, self.acc)
 
     def extra_repr(self) -> str:
         return (f"num_groups={self.num_groups}, in_features={self.in_features}, out_features={self.out_features}, "
-                f"acc={self.acc}")
+                f"acc={self.acc}" + (", fuse_wgrad_accumulation=True" if self.fuse_wgrad_accumulation else ""))
 
 
 def linear_supported(in_features: int, out_features: int, dtype: torch.dtype) -> bool:
@@ -472,15 +599,21 @@ def linear_supported(in_features: int, out_features: int, dtype: torch.dtype) ->
 
 class B200Linear(nn.Module):
     """``nn.Linear`` whose matmul runs on the H100 HGEMM kernel. The weight keeps ``nn.Linear``'s layout
-    ``[out_features, in_features]`` — which IS the kernel's K-major B operand — so swapping a layer copies nothing."""
+    ``[out_features, in_features]`` — which IS the kernel's K-major B operand — so swapping a layer copies nothing.
+
+    ``fuse_wgrad_accumulation=True`` (Megatron-LM's gradient-accumulation fusion): the weight must carry
+    ``weight.main_grad``, an fp32 tensor of its shape, contiguous, on its device (checked in forward); the backward adds
+    dW = dY^T X into it with the K-grouped kernel's epilogue (:func:`wgrad_accumulate_`, any token count) and leaves
+    ``weight.grad`` None. y, dX and the bias gradient are the unfused layer's, bit for bit."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True, device=None,
-                 dtype: torch.dtype = torch.float16, acc: str = "fp32"):
+                 dtype: torch.dtype = torch.float16, acc: str = "fp32", fuse_wgrad_accumulation: bool = False):
         super().__init__()
         if not linear_supported(in_features, out_features, dtype):
             raise capi.B200HgemmError(f"B200Linear needs fp16/bf16 and feature counts divisible by 8, got "
                                       f"{in_features}->{out_features} {dtype}")
         self.in_features, self.out_features, self.acc = in_features, out_features, acc
+        self.fuse_wgrad_accumulation = fuse_wgrad_accumulation
         self.weight = nn.Parameter(torch.empty((out_features, in_features), device=device, dtype=dtype))
         self.bias = nn.Parameter(torch.empty(out_features, device=device, dtype=dtype)) if bias else None
         self.reset_parameters()
@@ -493,24 +626,35 @@ class B200Linear(nn.Module):
                 self.bias.uniform_(-bound, bound)
 
     @classmethod
-    def from_linear(cls, lin: nn.Linear, acc: str = "fp32") -> "B200Linear":
+    def from_linear(cls, lin: nn.Linear, acc: str = "fp32", fuse_wgrad_accumulation: bool = False) -> "B200Linear":
         new = cls.__new__(cls)
         nn.Module.__init__(new)
         if not linear_supported(lin.in_features, lin.out_features, lin.weight.dtype):
             raise capi.B200HgemmError(f"cannot convert {lin}: needs fp16/bf16 weights and feature counts divisible by 8")
         new.in_features, new.out_features, new.acc = lin.in_features, lin.out_features, acc
+        new.fuse_wgrad_accumulation = fuse_wgrad_accumulation
         new.weight, new.bias = lin.weight, lin.bias          # shared storage, no copy
         return new
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         lead = x.shape[:-1]
-        y = torch.ops.cuda_l2_b200.hgemm(x.reshape(-1, self.in_features), self.weight, self.acc)
+        x2 = x.reshape(-1, self.in_features)
+        fused = False
+        if self.fuse_wgrad_accumulation:
+            _fused_main_grad(self.weight)
+            fused = torch.is_grad_enabled() and (x.requires_grad or self.weight.requires_grad)
+        if fused:
+            y = _LinearWgradAccumFunction.apply(x2, self.weight, self.acc)
+        else:
+            y = torch.ops.cuda_l2_b200.hgemm(x2, self.weight, self.acc)
         if self.bias is not None:
             y = y + self.bias
         return y.view(*lead, self.out_features)
 
     def extra_repr(self) -> str:
-        return f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, acc={self.acc}"
+        fused = ", fuse_wgrad_accumulation=True" if self.fuse_wgrad_accumulation else ""
+        return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
+                f"acc={self.acc}{fused}")
 
 
 def replace_linear_modules(model: nn.Module, acc: str = "fp32", skip: tuple[str, ...] = ()) -> list[str]:
@@ -1107,10 +1251,11 @@ class _Fp8LinearFunction(torch.autograd.Function):
     copies its backward reads, not x and W, and only those of the gradients that will be asked for."""
 
     @staticmethod
-    def forward(ctx, x2, weight):
+    def forward(ctx, x2, weight, main_grad=None):
         need_x, need_w = ctx.needs_input_grad[:2]
         ctx.shapes = (x2.shape, weight.shape)
         ctx.dtypes = (x2.dtype, weight.dtype)
+        ctx.main_grad = main_grad
         if x2.shape[0] == 0:
             ctx.save_for_backward()
             return x2.new_empty((0, weight.shape[0]))
@@ -1136,19 +1281,22 @@ class _Fp8LinearFunction(torch.autograd.Function):
         if x_shape[0] == 0:
             if need_x:
                 grad_x = grad_y.new_empty(x_shape, dtype=x_dtype)
-            if need_w:
+            if need_w and ctx.main_grad is None:
                 grad_w = grad_y.new_zeros(w_shape, dtype=w_dtype)
-            return grad_x, grad_w
+            return grad_x, grad_w, None
         x_qt, x_st, w_qt, w_st = ctx.saved_tensors
         g = grad_y.contiguous()
         if need_w:
             g_q, g_s, g_qt, g_st = quantize_e4m3_rowwise_dual(g)
-            grad_w = _rowwise_gemm(g_qt, g_st, x_qt, x_st, w_dtype)       # [N, ld_t(M)] x [K, ld_t(M)] -> [N, K]
+            if ctx.main_grad is None:
+                grad_w = _rowwise_gemm(g_qt, g_st, x_qt, x_st, w_dtype)   # [N, ld_t(M)] x [K, ld_t(M)] -> [N, K]
+            else:   # the same product's fp32 value, added into main_grad
+                fp8_gemm_accumulate_(ctx.main_grad, g_qt, x_qt, g_st.reshape(-1, 1), x_st.reshape(1, -1))
         else:
             g_q, g_s = quantize_e4m3_rowwise(g)
         if need_x:
             grad_x = _rowwise_gemm(g_q, g_s, w_qt, w_st, x_dtype)         # [M, N] x [K, N] -> [M, K]
-        return grad_x, grad_w
+        return grad_x, grad_w, None
 
 
 class _Fp8BlockwiseLinearFunction(torch.autograd.Function):
@@ -1157,10 +1305,11 @@ class _Fp8BlockwiseLinearFunction(torch.autograd.Function):
     copies its backward reads, not x and W, and only those of the gradients that will be asked for."""
 
     @staticmethod
-    def forward(ctx, x2, weight):
+    def forward(ctx, x2, weight, main_grad=None):
         need_x, need_w = ctx.needs_input_grad[:2]
         ctx.shapes = (x2.shape, weight.shape)
         ctx.dtypes = (x2.dtype, weight.dtype)
+        ctx.main_grad = main_grad
         if x2.shape[0] == 0:
             ctx.save_for_backward()
             return x2.new_empty((0, weight.shape[0]))
@@ -1186,23 +1335,27 @@ class _Fp8BlockwiseLinearFunction(torch.autograd.Function):
         if x_shape[0] == 0:
             if need_x:
                 grad_x = grad_y.new_empty(x_shape, dtype=x_dtype)
-            if need_w:
+            if need_w and ctx.main_grad is None:
                 grad_w = grad_y.new_zeros(w_shape, dtype=w_dtype)
-            return grad_x, grad_w
+            return grad_x, grad_w, None
         x_qt, x_st, w_qt, w_st = ctx.saved_tensors
         g = grad_y.contiguous()
         gemm = torch.ops.cuda_l2_b200.fp8_gemm
         if need_w:
             g_q, g_s, g_qt, g_st = quantize_e4m3_blockwise_dual(g)
-            grad_w = gemm(g_qt, x_qt, g_st, x_st, w_dtype)   # [N, ld_t(M)] x [K, ld_t(M)], 1 x 128 scales on both -> [N, K]
+            if ctx.main_grad is None:
+                grad_w = gemm(g_qt, x_qt, g_st, x_st, w_dtype)   # [N, ld_t(M)] x [K, ld_t(M)], 1 x 128 scales -> [N, K]
+            else:   # the same product's fp32 value, added into main_grad
+                fp8_gemm_accumulate_(ctx.main_grad, g_qt, x_qt, g_st, x_st)
         else:
             g_q, g_s = quantize_e4m3_blockwise(g)
         if need_x:
             grad_x = gemm(g_q, w_qt, g_s, w_st, x_dtype)     # [M, N] x [K, N], 128 x 128 scales of W^T -> [M, K]
-        return grad_x, grad_w
+        return grad_x, grad_w, None
 
 
-def fp8_linear(x: torch.Tensor, weight: torch.Tensor, granularity: str = "rowwise") -> torch.Tensor:
+def fp8_linear(x: torch.Tensor, weight: torch.Tensor, granularity: str = "rowwise",
+               main_grad: torch.Tensor | None = None) -> torch.Tensor:
     """``x @ weight^T`` for ``x`` [..., K] and ``weight`` [N, K] of one dtype (fp16 or bf16), K % 16 == 0 and
     N % 16 == 0, in FP8 with a gradient.
 
@@ -1219,17 +1372,24 @@ def fp8_linear(x: torch.Tensor, weight: torch.Tensor, granularity: str = "rowwis
     operands, so one outlier token squeezes only its own 128-token group. Both orientations of x, dY and W come from
     one launch each (:func:`quantize_e4m3_blockwise_dual`, :func:`quantize_e4m3_block128x128_dual`). Without a
     gradient to compute, the forward is ``B200Fp8Linear``'s blockwise one, bit for bit. Also no host synchronisation;
-    its quantisers are not operators, so this path is not traceable by FakeTensor or torch.compile."""
+    its quantisers are not operators, so this path is not traceable by FakeTensor or torch.compile.
+
+    ``main_grad``: an fp32 tensor of the weight's shape, contiguous, on its device. The backward then adds dW into it
+    (:func:`fp8_gemm_accumulate_`: exactly the fp32 value the unfused dW rounds, one rounding per element) and returns
+    no gradient for the weight. y and dX are the unfused call's, bit for bit. The backward writes the tensor given here.
+    A frozen weight (``requires_grad=False``) gets nothing added."""
     if x.dim() == 0 or weight.dim() != 2 or x.shape[-1] != weight.shape[1] or x.dtype != weight.dtype:
         raise capi.B200HgemmError(f"fp8_linear: x [..., K] and weight [N, K] of one dtype expected, got "
                                   f"{x.dtype} {tuple(x.shape)} and {weight.dtype} {tuple(weight.shape)}")
     _check_fp8_train_granularity(granularity)
     n, k = weight.shape
     _check_fp8_linear(k, n, weight.dtype, f"a [{n}, {k}] weight")
+    if main_grad is not None:
+        capi.check_main_grad(main_grad, (n, k), weight.device)
     x2 = x.reshape(-1, k)
     blockwise = granularity == "blockwise"
     if torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad):
-        y = (_Fp8BlockwiseLinearFunction if blockwise else _Fp8LinearFunction).apply(x2, weight)
+        y = (_Fp8BlockwiseLinearFunction if blockwise else _Fp8LinearFunction).apply(x2, weight, main_grad)
     elif x2.shape[0] == 0:
         y = x2.new_empty((0, n))
     elif blockwise:
@@ -1246,14 +1406,21 @@ class B200Fp8TrainLinear(nn.Module):
     the product run by :func:`fp8_linear` with ``granularity`` ("rowwise", the default, or "blockwise": e4m3 forward and
     backward with those scales), the bias added by torch after it as :class:`B200Linear` does. In eval or no-grad mode
     the output is :class:`B200Fp8Linear`'s of the same granularity, bit for bit. Needs fp16 / bf16 and
-    in_features % 16 == 0, out_features % 16 == 0."""
+    in_features % 16 == 0, out_features % 16 == 0.
+
+    ``fuse_wgrad_accumulation=True``: the weight must carry ``weight.main_grad``, an fp32 tensor of its shape (checked
+    in forward); the backward adds dW into it (``fp8_linear``'s ``main_grad``) and leaves ``weight.grad`` None. The buffer
+    written is the ``weight.main_grad`` of the forward: replacing it between forward and backward leaves the new one
+    untouched, and a step captured in a CUDA graph keeps writing the buffer it was captured with (zero it in place)."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True, device=None,
-                 dtype: torch.dtype = torch.bfloat16, granularity: str = "rowwise"):
+                 dtype: torch.dtype = torch.bfloat16, granularity: str = "rowwise",
+                 fuse_wgrad_accumulation: bool = False):
         super().__init__()
         _check_fp8_linear(in_features, out_features, dtype, "B200Fp8TrainLinear")
         _check_fp8_train_granularity(granularity)
         self.in_features, self.out_features, self.granularity = in_features, out_features, granularity
+        self.fuse_wgrad_accumulation = fuse_wgrad_accumulation
         self.weight = nn.Parameter(torch.empty((out_features, in_features), device=device, dtype=dtype))
         self.bias = nn.Parameter(torch.empty(out_features, device=device, dtype=dtype)) if bias else None
         self.reset_parameters()
@@ -1261,25 +1428,29 @@ class B200Fp8TrainLinear(nn.Module):
     reset_parameters = B200Linear.reset_parameters
 
     @classmethod
-    def from_linear(cls, lin: nn.Linear, granularity: str = "rowwise") -> "B200Fp8TrainLinear":
+    def from_linear(cls, lin: nn.Linear, granularity: str = "rowwise",
+                    fuse_wgrad_accumulation: bool = False) -> "B200Fp8TrainLinear":
         """A layer sharing ``lin``'s Parameters (no copy), as :meth:`B200Linear.from_linear`."""
         _check_fp8_linear(lin.in_features, lin.out_features, lin.weight.dtype, lin)
         _check_fp8_train_granularity(granularity)
         new = cls.__new__(cls)
         nn.Module.__init__(new)
         new.in_features, new.out_features, new.granularity = lin.in_features, lin.out_features, granularity
+        new.fuse_wgrad_accumulation = fuse_wgrad_accumulation
         new.weight, new.bias = lin.weight, lin.bias          # shared storage, no copy
         return new
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        y = fp8_linear(x, self.weight, self.granularity)
+        main_grad = _fused_main_grad(self.weight) if self.fuse_wgrad_accumulation else None
+        y = fp8_linear(x, self.weight, self.granularity, main_grad)
         if self.bias is not None:
             y = y + self.bias
         return y
 
     def extra_repr(self) -> str:
         return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
-                f"granularity={self.granularity}")
+                f"granularity={self.granularity}" + (", fuse_wgrad_accumulation=True" if self.fuse_wgrad_accumulation
+                                                     else ""))
 
 
 # ------------------------------------------------------------------------------------------ grouped FP8 (libb200_grouped_fp8.so)
