@@ -18,6 +18,8 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
   (csrc/b200_epilogue.h; no public symbol)
 * ``libb200_wgrad_accum.so`` — weight gradients added into fp32 main-grad buffers by the GEMM epilogue: the 16-bit
   K-grouped, e4m3 rowwise and e4m3 1 x 128 kernels (csrc/b200_wgrad_accum.h; no public symbol)
+* ``libb200_swiglu.so`` — the gate / up projection of a SwiGLU MLP with silu(g) * u fused into the GEMM epilogue, and
+  the one-pass SwiGLU backward (csrc/b200_swiglu.h; no public symbol)
 * ``libb200_quant.so``  — the one-pass e4m3 quantisers of FP8 activations: per tensor, rowwise, 1 x 128 blocks and
   SwiGLU + 1 x 128 blocks (csrc/b200_quant.h; no public symbol)
 * ``libb200_quant_dual.so`` — the dual-orientation rowwise e4m3 quantiser of FP8 training: x and x^T quantised from
@@ -108,6 +110,7 @@ BLOCK_1D1D_VARIANTS = (7, 8)      # 1 x 128 scales on both operands: e4m3 to fp1
 # fp32 weight-gradient accumulation: K-grouped fp16 and bf16, e4m3 rowwise, e4m3 1 x 128 (the GemmType index; one
 # object per e4m3 family, whose fp32 output does not depend on the 16-bit flavour)
 WGRAD_ACCUM_VARIANTS = (0, 2, 3, 7)
+SWIGLU_VARIANTS = (0, 2)   # the SwiGLU epilogue: fp16 and bf16, both with fp32 accumulation (the GemmType index)
 
 
 def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, list[str]]]:
@@ -122,7 +125,9 @@ def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, lis
 # so does libb200_nn.so (43 kernels per 16-bit variant), libb200_grouped_bwd.so (56 per variant: 28 configurations
 # times two kinds), libb200_epilogue.so (46 per variant: libb200_hgemm.so's (configuration, K-mode) pairs),
 # libb200_fp8block_1d1d.so (19 per output type, libb200_fp8block.so's configurations and K-modes) and
-# libb200_wgrad_accum.so (28 K-grouped kernels per 16-bit variant, 46 rowwise e4m3 ones and 19 1 x 128 ones).
+# libb200_wgrad_accum.so (28 K-grouped kernels per 16-bit variant, 46 rowwise e4m3 ones and 19 1 x 128 ones) and
+# libb200_swiglu.so (18 gated kernels per variant, the BN = 128 and 256 configurations on the plain schedule, and the
+# backward kernel of each variant in the object of variant 0).
 LIBRARIES = {
     "capi": ("libb200_hgemm.so", [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], []),
     "fp8block": ("libb200_fp8block.so", [(CSRC / "b200_fp8_block_capi.cu", [])], []),
@@ -135,6 +140,7 @@ LIBRARIES = {
     "grouped_bwd": ("libb200_grouped_bwd.so", _per_variant("b200_grouped_bwd.cu", BWD_VARIANTS), []),
     "epilogue": ("libb200_epilogue.so", _per_variant("b200_epilogue.cu", EPILOGUE_VARIANTS), []),
     "wgrad_accum": ("libb200_wgrad_accum.so", _per_variant("b200_wgrad_accum.cu", WGRAD_ACCUM_VARIANTS), []),
+    "swiglu": ("libb200_swiglu.so", _per_variant("b200_swiglu.cu", SWIGLU_VARIANTS), []),
     "quant": ("libb200_quant.so", [(CSRC / "b200_quant.cu", [])], []),
     "quant_dual": ("libb200_quant_dual.so", [(CSRC / "b200_quant_dual.cu", [])], []),
     "quant_block_dual": ("libb200_quant_block_dual.so", [(CSRC / "b200_quant_block_dual.cu", [])], []),

@@ -110,6 +110,7 @@ QUANT_DUAL_LIB = "libb200_quant_dual.so"     # csrc/b200_quant_dual.h
 FP8BLOCK_1D1D_LIB = "libb200_fp8block_1d1d.so"       # csrc/b200_fp8_block_1d1d.h
 QUANT_BLOCK_DUAL_LIB = "libb200_quant_block_dual.so"  # csrc/b200_quant_block_dual.h
 WGRAD_ACCUM_LIB = "libb200_wgrad_accum.so"   # csrc/b200_wgrad_accum.h
+SWIGLU_LIB = "libb200_swiglu.so"             # csrc/b200_swiglu.h
 _QUANT_BLOCK_DUAL = ([_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp], _i)
 _QUANT_BLOCKWISE = ([_i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp], _i)
 INTERNAL_ABI = {
@@ -168,6 +169,14 @@ INTERNAL_ABI = {
         "cuda_l2_b200_wgrad_accum_release": ([], _i),
         "cuda_l2_b200_wgrad_accum_launch_count": ([], ctypes.c_ulonglong),
         "cuda_l2_b200_wgrad_accum_strerror": ([_i], ctypes.c_char_p),
+    },
+    SWIGLU_LIB: {
+        "cuda_l2_b200_swiglu_run": ([_i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_swiglu_run_config": ([_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_swiglu_select": ([_i, _i, _i, _i, _ip, _ip, _ip], _i),
+        "cuda_l2_b200_swiglu_backward": ([_i, _vp, _vp, _vp, _i, _i, _vp], _i),
+        "cuda_l2_b200_swiglu_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_swiglu_strerror": ([_i], ctypes.c_char_p),
     },
 }
 _TABLES = {**ABI, **INTERNAL_ABI}
@@ -1223,6 +1232,91 @@ def epilogue_release() -> None:
 
 def epilogue_launch_count() -> int:
     return int(epilogue_lib().cuda_l2_b200_epilogue_launch_count())
+
+
+# ------------------------------------------------------------------------------------ SwiGLU (libb200_swiglu.so)
+SWIGLU_BLOCK = 64   # gate and up rows of w_gu interleave in blocks of this many (csrc/b200_swiglu.h)
+
+
+def swiglu_lib() -> ctypes.CDLL:
+    """libb200_swiglu.so: the gate / up GEMM with silu(g) * u fused into its epilogue, and the one-pass SwiGLU backward
+    (csrc/b200_swiglu.h, no public ABI)."""
+    return load(SWIGLU_LIB)
+
+
+def swiglu_variant(dtype) -> int:
+    """The GemmType index of the SwiGLU kernels for ``dtype``: 0 fp16, 2 bf16 (fp32 accumulation). B200HgemmError for
+    any other dtype."""
+    import torch
+
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise B200HgemmError(f"SwiGLU kernels take fp16 or bf16 tensors, got {dtype}")
+    return 0 if dtype == torch.float16 else 2
+
+
+def check_swiglu_operands(x, w_gu) -> tuple[int, int, int]:
+    """(M, I, K) of y = swiglu(x [M, K] @ w_gu [2I, K]^T): 2-D operands of one 16-bit dtype, a shared K with K % 8 == 0,
+    and 2I rows with I % 64 == 0 (whole 64-row gate / up blocks). Shapes and dtypes only (meta tensors pass);
+    B200HgemmError otherwise."""
+    try:
+        (m, k), (n, k2) = x.shape, w_gu.shape
+    except ValueError:
+        raise B200HgemmError(f"2-D operands expected, got {tuple(x.shape)} and {tuple(w_gu.shape)}") from None
+    swiglu_variant(x.dtype)
+    if w_gu.dtype != x.dtype:
+        raise B200HgemmError(f"x and w_gu must share a dtype, got {x.dtype} and {w_gu.dtype}")
+    if k2 != k:
+        raise B200HgemmError(f"inner dimensions differ: x {tuple(x.shape)}, w_gu {tuple(w_gu.shape)} ([2I, K])")
+    if n % (2 * SWIGLU_BLOCK) or k % 8:
+        raise B200HgemmError(f"w_gu [2I, K] needs I % {SWIGLU_BLOCK} == 0 and K % 8 == 0, got 2I={n}, K={k}")
+    return m, n // 2, k
+
+
+def swiglu(x, w_gu, y, h=None, stream: int | None = None, config_id: int | None = None, group_m: int = 0,
+           splits: int = 1, max_ctas: int = 0) -> None:
+    """y [M, I] = silu(g) * u of h = x [M, K] @ w_gu [2I, K]^T, whose gate and up columns interleave in blocks of 64
+    (csrc/b200_swiglu.h), with fp32 accumulation: torch's ``F.silu(g) * u`` on the 16-bit h, bit for bit. ``h``
+    [M, 2I] (optional) receives h itself, the bits :func:`gemm_kmajor` writes with the same configuration. All
+    contiguous CUDA tensors of one dtype (fp16 or bf16). ``config_id`` pins one configuration (BN = 128 or 256; tests;
+    ``group_m``, ``max_ctas`` as for :func:`gemm_kmajor`, every ``splits`` runs the plain schedule); default is the
+    dispatcher's TN choice for (M, 2I, K) mapped to its gated sibling."""
+    _contiguous_cuda(x=x, w_gu=w_gu, y=y, h=h)
+    m, i, k = check_swiglu_operands(x, w_gu)
+    if tuple(y.shape) != (m, i) or y.dtype != x.dtype or (h is not None and (tuple(h.shape) != (m, 2 * i) or
+                                                                             h.dtype != x.dtype)):
+        raise B200HgemmError(f"y must be [{m}, {i}] and h [{m}, {2 * i}] of {x.dtype}, got y {y.dtype} "
+                             f"{tuple(y.shape)}" + ("" if h is None else f", h {h.dtype} {tuple(h.shape)}"))
+    args = (x.data_ptr(), w_gu.data_ptr(), None if h is None else h.data_ptr(), y.data_ptr(), m, i, k)
+    lib = swiglu_lib()
+    if config_id is None:
+        fn = lib.cuda_l2_b200_swiglu_run
+        st = fn(swiglu_variant(x.dtype), *args, stream)
+    else:
+        fn = lib.cuda_l2_b200_swiglu_run_config
+        st = fn(swiglu_variant(x.dtype), config_id, *args, group_m, splits, max_ctas, stream)
+    _check(st, fn)
+
+
+def swiglu_backward(dy, h, dh, stream: int | None = None) -> None:
+    """dh [M, 2I] = the gradient of y = silu(g) * u at h [M, 2I] for dy [M, I], in h's interleaved layout: the steps
+    torch's autograd takes through ``F.silu(g) * u`` (csrc/b200_swiglu.h). Contiguous CUDA tensors of one dtype."""
+    _contiguous_cuda(dy=dy, h=h, dh=dh)
+    if dy.dim() != 2 or h.dim() != 2 or tuple(h.shape) != (dy.shape[0], 2 * dy.shape[1]) or dh.shape != h.shape or \
+            not dy.dtype == h.dtype == dh.dtype:
+        raise B200HgemmError(f"dy [M, I], h and dh [M, 2I] of one dtype expected, got dy {dy.dtype} {tuple(dy.shape)}, "
+                             f"h {h.dtype} {tuple(h.shape)}, dh {dh.dtype} {tuple(dh.shape)}")
+    fn = swiglu_lib().cuda_l2_b200_swiglu_backward
+    _check(fn(swiglu_variant(dy.dtype), dy.data_ptr(), h.data_ptr(), dh.data_ptr(), dy.shape[0], dy.shape[1], stream),
+           fn)
+
+
+def swiglu_select(variant: int, m: int, i: int, k: int) -> tuple[int, int, int]:
+    """(config_id, group_m, splits): the dispatched SwiGLU call's choice for variant ``variant`` (0 fp16, 2 bf16)."""
+    return _select(swiglu_lib().cuda_l2_b200_swiglu_select, variant, m, i, k)
+
+
+def swiglu_launch_count() -> int:
+    return int(swiglu_lib().cuda_l2_b200_swiglu_launch_count())
 
 
 # ---------------------------------------------------------------- fp32 weight-gradient accumulation

@@ -4,6 +4,7 @@
 // element arithmetic is in b200_quant_arith.cuh, shared with libb200_quant_dual.so.
 #include "b200_quant.h"
 #include "b200_quant_arith.cuh"
+#include "swiglu_arith.cuh"
 
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -29,15 +30,8 @@ enum Status : int {
 constexpr int kBlock = 128;   // the 1 x 128 scale block
 
 // ------------------------------------------------------------------------------------------------ SwiGLU
-// the SwiGLU product p = RN(fp32(RN(silu(g))) * fp32(u)) of torch's `F.silu(g) * u` on 16-bit tensors
-__device__ __forceinline__ float round_to(float v, __half) { return __half2float(__float2half_rn(v)); }
-__device__ __forceinline__ float round_to(float v, __nv_bfloat16) { return __bfloat162float(__float2bfloat16_rn(v)); }
-
-template <typename T>
-__device__ __forceinline__ float silu_mul(float g, float u) {
-  const float s = round_to(__fdiv_rn(g, 1.0f + expf(-g)), T());
-  return round_to(s * u, T());
-}
+// the SwiGLU product p = RN(fp32(RN(silu(g))) * fp32(u)) of torch's `F.silu(g) * u` on 16-bit tensors: silu_mul of
+// swiglu_arith.cuh, which the gated GEMM epilogue shares
 
 // ------------------------------------------------------------------------------------------------ 1 x 128 blocks
 // One CTA of 128 threads quantises 32 rows of one k-block. A row's 128 columns are spread over LPR = 128 / EPL lanes

@@ -132,16 +132,55 @@ static_assert(every_config_has_a_sibling(), "the configuration table lost a row-
 
 }  // namespace nn
 
+// The SwiGLU configurations (libb200_swiglu.so, Gated<>). Host code: the library maps the dispatcher's TN choice through
+// this rule.
+namespace gated {
+
+// A gate / up pair is two 64-column chunks of one tile: BN = 128 and 256 have a gated kernel.
+constexpr bool has_kernel(int id) { return kConfigs[id].bn == 128 || kConfigs[id].bn == 256; }
+
+// The gated stand-in of configuration `id`: itself if it has a gated kernel; otherwise (BN = 32, 64, 192) the BN = 128
+// configuration with the same CTA group and M_REP and the largest cluster no wider in M or N than its own.
+constexpr int sibling(int id) {
+  const ConfigDesc& c = kConfigs[id];
+  if (has_kernel(id)) return id;
+  int best = -1;
+  for (int j = 0; j < kNumConfigs; ++j) {
+    const ConfigDesc& d = kConfigs[j];
+    if (d.bn == 128 && d.cta_group == c.cta_group && d.m_rep == c.m_rep && d.cluster_m <= c.cluster_m &&
+        d.cluster_n <= c.cluster_n &&
+        (best < 0 || d.cluster_m * d.cluster_n > kConfigs[best].cluster_m * kConfigs[best].cluster_n))
+      best = j;
+  }
+  return best;
+}
+constexpr bool every_config_has_a_sibling() {
+  for (int id = 0; id < kNumConfigs; ++id) {
+    const int s = sibling(id);
+    if (s < 0 || !has_kernel(s) || (has_kernel(id) && s != id)) return false;
+  }
+  return true;
+}
+static_assert(every_config_has_a_sibling(), "the configuration table lost a SwiGLU sibling");
+
+// Only the plain schedule is compiled for the gated kernels: plan() runs split-K and stream-K requests plain.
+constexpr unsigned kModes = 1u << kPlain;
+
+}  // namespace gated
+
 // What the kernels of a configuration wrapper cover, read from Probe, the wrapper's type of configuration 1 (BN = 128,
 // one CTA, no cluster), which every wrapper compiles: block-scaled kernels exist for the block::eligible
-// configurations and carry block::kModes, row-major B ones exist for the nn::has_kernel configurations; every other
-// wrapper has every configuration in every K-mode.
+// configurations and carry block::kModes, row-major B ones exist for the nn::has_kernel configurations, gated ones for
+// the gated::has_kernel configurations with gated::kModes; every other wrapper has every configuration in every K-mode.
 template <class Probe>
 constexpr bool has_kernel(int id) {
-  return block_scaled<Probe>() ? block::eligible(id) : row_major_b<Probe>() ? nn::has_kernel(id) : true;
+  return block_scaled<Probe>() ? block::eligible(id)
+         : row_major_b<Probe>() ? nn::has_kernel(id)
+         : is_gated<Probe>()    ? gated::has_kernel(id)
+                                : true;
 }
 template <class Probe>
-constexpr unsigned k_modes() { return block_scaled<Probe>() ? block::kModes : 0xFu; }
+constexpr unsigned k_modes() { return block_scaled<Probe>() ? block::kModes : is_gated<Probe>() ? gated::kModes : 0xFu; }
 
 // The wrapper of the TN, per-tensor and rowwise configurations: none.
 template <class Cfg>

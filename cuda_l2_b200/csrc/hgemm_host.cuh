@@ -467,13 +467,15 @@ struct LaunchArgs {
   cudaStream_t stream;
   const void* bias;     // BiasAct<> kernels: the bias (or null) ...
   int act;              // ... and the activation code
+  GatedArgs gated;      // Gated<> kernels: y's map, and whether h (C) is stored
 };
 
 // The kernel's last argument: the scales, BiasAct<>'s BiasActArgs, BlockScaled1D1D<>'s Block1D1DArgs, or AccumF32<>'s
 // AccumArgs (the wrapped kernel's argument and C, which is fp32).
 template <class Cfg>
 typename Cfg::EpiArgs epi_args(const LaunchArgs& a) {
-  if constexpr (accum_f32<Cfg>())
+  if constexpr (is_gated<Cfg>()) return a.gated;
+  else if constexpr (accum_f32<Cfg>())
     return typename Cfg::EpiArgs{epi_args<typename Cfg::AccumBase>(a), reinterpret_cast<float*>(a.c)};
   else if constexpr (bias_act<Cfg>()) return BiasActArgs{a.scales, a.bias, a.act};
   else if constexpr (block_1d1d<Cfg>()) return Block1D1DArgs{a.scales, a.ld_b};
@@ -562,12 +564,20 @@ constexpr int default_group_m() { return Cfg::CTA_GROUP == 2 ? 8 : 16; }
 // of a scaled variant (device pointers), unused otherwise; `ld_a`: the row stride of block scales. RowMajorB<>
 // configurations read `Bt` as B [K, N] row-major. `scratch`: where the workspace of split-K and stream-K comes from.
 // BiasAct<> configurations: the bias (null, or N values of the output type) and the activation code. BlockScaled1D1D<>
-// configurations: `ld_b`, the row stride of Bt's 1 x 128 scales.
+// configurations: `ld_b`, the row stride of Bt's 1 x 128 scales. Gated<> configurations: C is h [M, N] (null: not
+// stored) and `y` is y [M, N / 2], 16-byte aligned, with N % 128 == 0 (whole gate / up pairs).
 template <class Cfg, unsigned MODES = 0xFu>
 int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
            int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0,
-           ScratchFn scratch = splitk_scratch, const void* bias = nullptr, int act = kActNone, int ld_b = 0) {
+           ScratchFn scratch = splitk_scratch, const void* bias = nullptr, int act = kActNone, int ld_b = 0,
+           void* y = nullptr) {
   constexpr GemmType kType = gemm_type<Cfg>();
+  [[maybe_unused]] const bool store_h = C != nullptr;
+  if constexpr (is_gated<Cfg>()) {
+    if (!y) return kNullPointer;
+    if (!C) C = y;   // for the argument rules and tmap_c, which is then never written
+    if ((reinterpret_cast<uintptr_t>(y) & 15) || N % 128) return kBadAlignment;
+  }
   int st = validate(kType, A, Bt, C, scales, M, N, K, ld_a);
   if (st != kOk) return st;
   if constexpr (bias_act<Cfg>()) {
@@ -588,7 +598,15 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   } else {
     if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, operand)) != kOk) return st;
   }
-  if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk) return st;
+  if constexpr (is_gated<Cfg>()) {
+    // h's map (y's when h is not stored: never written) and y's, both in 64-column store boxes
+    if ((st = cache.get(store_h ? C : y, M, store_h ? N : N / 2, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk)
+      return st;
+    if ((st = cache.get(y, M, N / 2, Cfg::EPI_ROWS, &a.gated.y_map, Cfg::EPI_N, output)) != kOk) return st;
+    a.gated.store_h = store_h ? 1 : 0;
+  } else {
+    if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk) return st;
+  }
 
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = plan<Cfg, MODES>(M, N, K, splits, max_workers, [&] { return max_resident_clusters<Cfg>(di); });

@@ -38,6 +38,7 @@
 
 #include "hgemm_schedule.cuh"
 #include "ptx_sm90.cuh"
+#include "swiglu_arith.cuh"
 #include "wgmma_sm90.cuh"
 
 
@@ -381,6 +382,28 @@ __host__ __device__ __forceinline__ float* c32_of(const E&) { return nullptr; }
 template <class E>
 __host__ __device__ __forceinline__ float* c32_of(const AccumArgs<E>& e) { return e.c32; }
 
+// Fused SwiGLU epilogue (libb200_swiglu.so): h = A Bt^T over a gate / up weight Bt [2I, K] whose rows are interleaved in
+// 64-row blocks (rows [128 b, 128 b + 64) gate rows [64 b, 64 b + 64), the next 64 the matching up rows), so that h's
+// columns are [g | u] per 128. The epilogue writes y [M, I] = silu_mul(RN(g), RN(u)) (swiglu_arith.cuh), torch's
+// `F.silu(g) * u` on the 16-bit h, and, when `store_h` is set, h [M, 2I] itself through the unchanged store path (the
+// bits of the wrapped kernel's output). Chunk J (even) and chunk J + 1 of a 64-row block are one gate / up pair: in the
+// wgmma accumulator layout the thread that holds column c of chunk J holds column c of chunk J + 1 for the same rows, so
+// every pair is in one thread's registers. y's chunk goes out through the warp's staging buffer with a TMA store of its
+// own map, `y_map` ([M, I], box {64, 16}). The 2-D 16-bit TN kernels with fp32 accumulation and BN = 128 or 256 (whole
+// pairs per tile), plain schedule only. A wrapper, like BiasAct<>, so that the other kernels and their names stay as
+// they are; the kernel takes GatedArgs as its last parameter (hgemm_gated_kernel).
+struct GatedArgs { CUtensorMap y_map; int store_h; };
+template <class Base>
+struct Gated : Base {
+  using EpiArgs = GatedArgs;
+  static_assert(Base::ACC_F32 && !Base::E4M3 && !Base::BLOCK_SCALED && !Base::BATCHED && !Base::GROUPED &&
+                    !Base::ROW_MAJOR_B && !Base::K_GROUPED && !Base::BIAS_ACT && !Base::ACCUM_F32,
+                "SwiGLU: the 2-D 16-bit TN kernels with fp32 accumulation only");
+  static_assert(Base::BN == 128 || Base::BN == 256, "SwiGLU: whole gate / up pairs of 64-column chunks per tile");
+};
+template <class Cfg>
+__host__ __device__ constexpr bool is_gated() { return std::is_same_v<typename Cfg::EpiArgs, GatedArgs>; }
+
 // act(z) in fp32; `act` is warp-uniform. relu: max(z, +0.0) (+0.0 for -0.0 and NaN). gelu_tanh: 0.5 z (1 + tanhf(u)),
 // u = sqrt(2/pi) (z + 0.044715 z^3), torch's tanh approximation (F.gelu(approximate="tanh"), _addmm_activation), each
 // step one IEEE fp32 operation and tanhf CUDA's full-precision one (no tanh.approx.f32). Where tanh(u) nears -1 (z below
@@ -670,6 +693,59 @@ __device__ __forceinline__ void bias_act_epilogue(Reg (&acc)[MR][NR], uint32_t e
       bias_act_epilogue<Cfg, R, J + 1>(acc, epi_buf, lane, tmap_c, m_row0, n0, M, N, epi);
     } else {
       bias_act_epilogue<Cfg, R + 1, 0>(acc, epi_buf, lane, tmap_c, m_row0, n0, M, N, epi);
+    }
+  }
+}
+
+// Gated<> kernels: y of one gate / up pair of store chunks (J = chunk, J + 1) of this warp's 16 rows into the staging
+// buffer, then its TMA store at y's column col0 = (n0 + 64 J) / 2 and row row0. g and u are rounded to the output type
+// as the h store packs them (RN), so y is silu_mul of the 16-bit h. Rows past M are clipped by the map; I % 64 == 0, so
+// a pair is wholly inside or wholly outside y's columns.
+template <class Cfg, class Reg, int NR>
+__device__ __forceinline__ void gated_store_chunk(const Reg (&d)[NR], int chunk, uint32_t epi_buf, int lane,
+                                                  const CUtensorMap* tmap_y, int col0, int row0, int M, int I) {
+  using namespace ptx;
+  using T = std::conditional_t<Cfg::BF16, __nv_bfloat16, __half>;
+  constexpr int EN = Cfg::EPI_N;
+  constexpr int PER_CHUNK = EN / 4;
+  static_assert(EN == 64, "64-column chunks");
+  if (lane == 0) tma_store_wait_read<0>();
+  __syncwarp();
+#pragma unroll
+  for (int q = 0; q < PER_CHUNK; ++q) {
+    uint32_t off = uint32_t(frag_row(lane, q) * (EN * 2) + frag_col(lane, q) * 2);
+    off ^= ((off >> 7) & 7u) << 4;
+    const float2 g = acc_pair<Cfg>(d, chunk * PER_CHUNK + q), u = acc_pair<Cfg>(d, (chunk + 1) * PER_CHUNK + q);
+    const float y0 = silu_mul<T>(round_to(g.x, T()), round_to(u.x, T()));
+    const float y1 = silu_mul<T>(round_to(g.y, T()), round_to(u.y, T()));
+    st_shared_b32(epi_buf + off, pack_out_x2_rn<Cfg::BF16>(y0, y1));   // exact: both are 16-bit values already
+  }
+  fence_proxy_async_smem();
+  __syncwarp();
+  if (lane == 0) {
+    if (row0 < M && col0 < I) tma_store_2d(tmap_y, epi_buf, col0, row0);
+    tma_store_commit();
+  }
+}
+
+// The plain epilogue of a Gated<> unit: for every 64-row block R of the warpgroup (rows m_row0 + 64 R ..) and every
+// gate / up pair of chunks (J, J + 1), h's two chunks when the launch stores h (epilogue_store_chunk, the wrapped
+// kernel's bits), then y's chunk (gated_store_chunk). Unrolled by recursion, as bias_act_epilogue is.
+template <class Cfg, int R = 0, int J = 0, class Reg, int MR, int NR>
+__device__ __forceinline__ void gated_epilogue(const Reg (&acc)[MR][NR], uint32_t epi_buf, int lane,
+                                               const CUtensorMap* tmap_h, const GatedArgs& epi, int m_row0, int n0,
+                                               int M, int N) {
+  if constexpr (R < MR) {
+    const int row0 = m_row0 + R * 64;
+    if constexpr (J < Cfg::EPI_CHUNKS) {
+      if (epi.store_h) {
+        epilogue_store_chunk<Cfg>(acc[R], J, epi_buf, lane, tmap_h, n0 + J * Cfg::EPI_N, row0, M, N);
+        epilogue_store_chunk<Cfg>(acc[R], J + 1, epi_buf, lane, tmap_h, n0 + (J + 1) * Cfg::EPI_N, row0, M, N);
+      }
+      gated_store_chunk<Cfg>(acc[R], J, epi_buf, lane, &epi.y_map, (n0 + J * Cfg::EPI_N) / 2, row0, M, N / 2);
+      gated_epilogue<Cfg, R, J + 2>(acc, epi_buf, lane, tmap_h, epi, m_row0, n0, M, N);
+    } else {
+      gated_epilogue<Cfg, R + 1, 0>(acc, epi_buf, lane, tmap_h, epi, m_row0, n0, M, N);
     }
   }
 }
@@ -1070,10 +1146,24 @@ hgemm_accum_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 #include "hgemm_tn_kernel_body.inc"
 }
 
+// The same with the SwiGLU epilogue (Gated<>): the parameters of hgemm_tn_kernel, GatedArgs (y's map, read in place as
+// tmap_c is) last; tmap_c is h's map, written only when epi.store_h is set. Plain schedule only.
+template <class Cfg, int KMODE = kPlain>
+__global__ void __launch_bounds__(kNumThreads, 1)
+hgemm_gated_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                   const __grid_constant__ CUtensorMap tmap_c, int M, int N, int K, int group_m, int splits_arg,
+                   int aux_arg, float* __restrict__ splitk_ws, unsigned* __restrict__ splitk_ctr,
+                   __half* __restrict__ c_raw, uint64_t hint_a, uint64_t hint_b, const __grid_constant__ GatedArgs epi) {
+  static_assert(is_gated<Cfg>() && KMODE == kPlain, "a Gated<> configuration, plain schedule");
+  const Scales scales{nullptr, nullptr};   // 16-bit operands: no scales
+#include "hgemm_tn_kernel_body.inc"
+}
+
 // The kernel of (Cfg, KMODE).
 template <class Cfg, int KMODE>
 constexpr auto kernel_of() {
-  if constexpr (accum_f32<Cfg>()) return &hgemm_accum_kernel<Cfg, KMODE>;
+  if constexpr (is_gated<Cfg>()) return &hgemm_gated_kernel<Cfg, KMODE>;
+  else if constexpr (accum_f32<Cfg>()) return &hgemm_accum_kernel<Cfg, KMODE>;
   else if constexpr (bias_act<Cfg>()) return &hgemm_bias_act_kernel<Cfg, KMODE>;
   else if constexpr (block_1d1d<Cfg>()) return &hgemm_block_1d1d_kernel<Cfg, KMODE>;
   else return &hgemm_tn_kernel<Cfg, KMODE>;

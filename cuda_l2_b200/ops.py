@@ -72,6 +72,11 @@ the nearest grid shape — so deployment is a plain operator:
   csrc/b200_quant_dual.h): the two K-major e4m3 operands FP8 training needs of each tensor. Inference only itself.
 * :func:`fp8_linear` and :class:`B200Fp8TrainLinear`: ``x @ W^T`` trained in FP8, a rowwise-scaled e4m3 forward and
   backward (three ``fp8_gemm`` calls per step) over a trainable 16-bit weight.
+* :func:`swiglu_linear` and :class:`B200SwiGLULinear`: ``F.silu(x @ W_gate^T) * (x @ W_up^T)``, the gate / up
+  projection of a SwiGLU MLP, as one GEMM whose epilogue applies the activation (libb200_swiglu.so,
+  csrc/b200_swiglu.h), over a fused weight whose gate and up rows interleave in blocks of 64
+  (:func:`interleave_gate_up`, :func:`split_gate_up`). The backward is one element-wise pass for dh, then the
+  product's dX and dW. Plain functions, not operators.
 * ``fuse_wgrad_accumulation=True`` on :class:`B200Linear`, :class:`B200Fp8TrainLinear` and :class:`B200GroupedLinear`
   (and ``fp8_linear(..., main_grad=...)``): the backward adds dW into the weight's fp32 ``main_grad`` in the GEMM
   epilogue (libb200_wgrad_accum.so, csrc/b200_wgrad_accum.h) and returns no weight gradient. The plain functions
@@ -655,6 +660,135 @@ class B200Linear(nn.Module):
         fused = ", fuse_wgrad_accumulation=True" if self.fuse_wgrad_accumulation else ""
         return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
                 f"acc={self.acc}{fused}")
+
+
+# ------------------------------------------------------------------------------------------ SwiGLU (libb200_swiglu.so)
+def interleave_gate_up(w_gate: torch.Tensor, w_up: torch.Tensor) -> torch.Tensor:
+    """The fused gate / up weight ``w_gu`` [2I, H] of a SwiGLU MLP from its gate and up weights [I, H] (a copy): rows
+    [128 b, 128 b + 64) are gate rows [64 b, 64 b + 64), rows [128 b + 64, 128 b + 128) the matching up rows. I must be
+    a multiple of 64."""
+    if w_gate.dim() != 2 or w_gate.shape != w_up.shape or w_gate.shape[0] % capi.SWIGLU_BLOCK:
+        raise capi.B200HgemmError(f"gate and up weights must both be [I, H] with I % {capi.SWIGLU_BLOCK} == 0, got "
+                                  f"{tuple(w_gate.shape)} and {tuple(w_up.shape)}")
+    i, h = w_gate.shape
+    blk = capi.SWIGLU_BLOCK
+    return torch.stack((w_gate.reshape(i // blk, blk, h), w_up.reshape(i // blk, blk, h)), dim=1).reshape(2 * i, h)
+
+
+def split_gate_up(w_gu: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """``(w_gate, w_up)``, each [I, H], of a fused gate / up weight ``w_gu`` [2I, H] (copies): the inverse of
+    :func:`interleave_gate_up`."""
+    blk = capi.SWIGLU_BLOCK
+    if w_gu.dim() != 2 or w_gu.shape[0] % (2 * blk):
+        raise capi.B200HgemmError(f"w_gu must be [2I, H] with I % {blk} == 0, got {tuple(w_gu.shape)}")
+    n, h = w_gu.shape
+    v = w_gu.reshape(n // (2 * blk), 2, blk, h)
+    return tuple(v[:, j].clone(memory_format=torch.contiguous_format).view(n // 2, h) for j in (0, 1))
+
+
+def _swiglu_forward(x2: torch.Tensor, w_gu: torch.Tensor, want_h: bool):
+    """(y [M, I], h [M, 2I] or None) of the fused gate / up product of ``x2`` [M, H]: one launch of libb200_swiglu.so.
+    M == 0 launches nothing, and K == 0 makes y (and h) zero, as :func:`_empty_product` does for the products."""
+    m, i, k = capi.check_swiglu_operands(x2, w_gu)
+    if not x2.is_cuda or not w_gu.is_cuda:
+        raise capi.B200HgemmError("swiglu_linear has no CPU implementation (and no fallback): move the tensors to an H100")
+    y = torch.empty((m, i), dtype=x2.dtype, device=x2.device)
+    h = torch.empty((m, 2 * i), dtype=x2.dtype, device=x2.device) if want_h else None
+    if m == 0:
+        return y, h
+    if k == 0:   # h = 0, so y = silu(0) * 0 = +0
+        y.zero_()
+        if h is not None:
+            h.zero_()
+        return y, h
+    with torch.cuda.device(x2.device):
+        capi.swiglu(x2.contiguous(), w_gu.contiguous(), y, h, stream=torch.cuda.current_stream(x2.device).cuda_stream)
+    return y, h
+
+
+class _SwiGLULinearFunction(torch.autograd.Function):
+    """y = silu(g) * u of h = x2 w_gu^T, saving x2, w_gu and h (not silu(g)). The backward is one pass of
+    libb200_swiglu.so's SwiGLU gradient (dh from dy and h), then dX and dW of the product through
+    :func:`_product_grads` (any token count)."""
+
+    @staticmethod
+    def forward(ctx, x2, w_gu):
+        x2, w_gu = x2.contiguous(), w_gu.contiguous()
+        y, h = _swiglu_forward(x2, w_gu, True)
+        ctx.save_for_backward(x2, w_gu, h)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        x2, w_gu, h = ctx.saved_tensors
+        dh = torch.empty_like(h)
+        if dh.numel():
+            with torch.cuda.device(h.device):
+                capi.swiglu_backward(grad_y.contiguous(), h, dh, stream=torch.cuda.current_stream(h.device).cuda_stream)
+        return _product_grads(x2, w_gu, dh, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+
+
+def swiglu_linear(x: torch.Tensor, w_gu: torch.Tensor) -> torch.Tensor:
+    """``F.silu(x @ W_gate^T) * (x @ W_up^T)`` for ``x`` [..., H] and the fused weight ``w_gu`` [2I, H]
+    (:func:`interleave_gate_up`), as one GEMM whose epilogue applies the SwiGLU: fp16 or bf16 with fp32 accumulation,
+    y [..., I] bit for bit torch's ``F.silu(g) * u`` on the 16-bit gate / up product. Differentiable in ``x`` and
+    ``w_gu``; without a gradient to compute, h is never written. No host synchronisation in either direction, so a
+    training step can be captured in a CUDA graph. I % 64 == 0 and H % 8 == 0."""
+    lead = x.shape[:-1]
+    x2 = x.reshape(lead.numel(), x.shape[-1])   # explicit rows: -1 is ambiguous when H == 0
+    if torch.is_grad_enabled() and (x.requires_grad or w_gu.requires_grad):
+        y = _SwiGLULinearFunction.apply(x2, w_gu)
+    else:
+        y, _ = _swiglu_forward(x2, w_gu, False)
+    return y.view(*lead, y.shape[-1])
+
+
+class B200SwiGLULinear(nn.Module):
+    """The gate and up projections of a SwiGLU MLP (Llama, Mistral, Qwen) with the activation, as one layer:
+    ``forward(x) = F.silu(gate_proj(x)) * up_proj(x)`` through :func:`swiglu_linear`. The Parameter ``weight`` is the
+    fused ``w_gu`` [2I, H], gate and up rows interleaved in blocks of 64 (:func:`interleave_gate_up`,
+    :func:`split_gate_up`). No bias. fp16 or bf16; I % 64 == 0 and H % 8 == 0."""
+
+    def __init__(self, in_features: int, intermediate_features: int, device=None, dtype: torch.dtype = torch.bfloat16):
+        super().__init__()
+        self._check(in_features, intermediate_features, dtype)
+        self.in_features, self.intermediate_features = in_features, intermediate_features
+        self.weight = nn.Parameter(torch.empty((2 * intermediate_features, in_features), device=device, dtype=dtype))
+        bound = 1.0 / (in_features ** 0.5)
+        with torch.no_grad():
+            self.weight.uniform_(-bound, bound)
+
+    @staticmethod
+    def _check(h: int, i: int, dtype: torch.dtype) -> None:
+        if dtype not in (torch.float16, torch.bfloat16) or h <= 0 or h % 8 or i <= 0 or i % capi.SWIGLU_BLOCK:
+            raise capi.B200HgemmError(f"B200SwiGLULinear needs fp16 / bf16, in_features % 8 == 0 and "
+                                      f"intermediate_features % {capi.SWIGLU_BLOCK} == 0, got {h} -> {i} {dtype}")
+
+    @classmethod
+    def from_linears(cls, gate_proj: nn.Linear, up_proj: nn.Linear) -> "B200SwiGLULinear":
+        """The layer of two bias-free ``nn.Linear`` projections H -> I of one dtype and device, their weights
+        interleaved into a new Parameter (a copy)."""
+        if gate_proj.bias is not None or up_proj.bias is not None:
+            raise capi.B200HgemmError("from_linears needs bias-free gate and up projections (a SwiGLU MLP has none)")
+        wg, wu = gate_proj.weight, up_proj.weight
+        if wg.shape != wu.shape or wg.dtype != wu.dtype or wg.device != wu.device:
+            raise capi.B200HgemmError(f"gate and up projections must match in shape, dtype and device, got "
+                                      f"{tuple(wg.shape)} {wg.dtype} {wg.device} and {tuple(wu.shape)} {wu.dtype} "
+                                      f"{wu.device}")
+        i, h = wg.shape
+        cls._check(h, i, wg.dtype)
+        new = cls.__new__(cls)
+        nn.Module.__init__(new)
+        new.in_features, new.intermediate_features = h, i
+        with torch.no_grad():
+            new.weight = nn.Parameter(interleave_gate_up(wg, wu), requires_grad=wg.requires_grad or wu.requires_grad)
+        return new
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return swiglu_linear(x, self.weight)
+
+    def extra_repr(self) -> str:
+        return f"in_features={self.in_features}, intermediate_features={self.intermediate_features}"
 
 
 def replace_linear_modules(model: nn.Module, acc: str = "fp32", skip: tuple[str, ...] = ()) -> list[str]:
