@@ -20,6 +20,9 @@ Artifacts land in ``cuda_l2_b200/lib/`` (git-ignored build products):
   K-grouped, e4m3 rowwise and e4m3 1 x 128 kernels (csrc/b200_wgrad_accum.h; no public symbol)
 * ``libb200_swiglu.so`` — the gate / up projection of a SwiGLU MLP with silu(g) * u fused into the GEMM epilogue, and
   the one-pass SwiGLU backward (csrc/b200_swiglu.h; no public symbol)
+* ``libb200_grouped_swiglu.so`` — the gate / up projection of SwiGLU experts over contiguous row groups with
+  silu(g) * u fused into the GEMM epilogue, and the SwiGLU backward over the groups' rows (csrc/b200_grouped_swiglu.h;
+  no public symbol)
 * ``libb200_quant.so``  — the one-pass e4m3 quantisers of FP8 activations: per tensor, rowwise, 1 x 128 blocks and
   SwiGLU + 1 x 128 blocks (csrc/b200_quant.h; no public symbol)
 * ``libb200_quant_dual.so`` — the dual-orientation rowwise e4m3 quantiser of FP8 training: x and x^T quantised from
@@ -111,6 +114,7 @@ BLOCK_1D1D_VARIANTS = (7, 8)      # 1 x 128 scales on both operands: e4m3 to fp1
 # object per e4m3 family, whose fp32 output does not depend on the 16-bit flavour)
 WGRAD_ACCUM_VARIANTS = (0, 2, 3, 7)
 SWIGLU_VARIANTS = (0, 2)   # the SwiGLU epilogue: fp16 and bf16, both with fp32 accumulation (the GemmType index)
+GROUPED_SWIGLU_VARIANTS = (0, 2)   # the grouped SwiGLU epilogue: the same two variants
 
 
 def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, list[str]]]:
@@ -127,7 +131,8 @@ def _per_variant(source: str, variants: tuple[int, ...]) -> list[tuple[Path, lis
 # libb200_fp8block_1d1d.so (19 per output type, libb200_fp8block.so's configurations and K-modes) and
 # libb200_wgrad_accum.so (28 K-grouped kernels per 16-bit variant, 46 rowwise e4m3 ones and 19 1 x 128 ones) and
 # libb200_swiglu.so (18 gated kernels per variant, the BN = 128 and 256 configurations on the plain schedule, and the
-# backward kernel of each variant in the object of variant 0).
+# backward kernel of each variant in the object of variant 0), and so does libb200_grouped_swiglu.so (the same 18
+# configurations per variant over row groups, and its two backward kernels in the object of variant 0).
 LIBRARIES = {
     "capi": ("libb200_hgemm.so", [(CSRC / "b200_hgemm_capi.cu", []), (CSRC / "b200_fp8_capi.cu", [])], []),
     "fp8block": ("libb200_fp8block.so", [(CSRC / "b200_fp8_block_capi.cu", [])], []),
@@ -141,6 +146,7 @@ LIBRARIES = {
     "epilogue": ("libb200_epilogue.so", _per_variant("b200_epilogue.cu", EPILOGUE_VARIANTS), []),
     "wgrad_accum": ("libb200_wgrad_accum.so", _per_variant("b200_wgrad_accum.cu", WGRAD_ACCUM_VARIANTS), []),
     "swiglu": ("libb200_swiglu.so", _per_variant("b200_swiglu.cu", SWIGLU_VARIANTS), []),
+    "grouped_swiglu": ("libb200_grouped_swiglu.so", _per_variant("b200_grouped_swiglu.cu", GROUPED_SWIGLU_VARIANTS), []),
     "quant": ("libb200_quant.so", [(CSRC / "b200_quant.cu", [])], []),
     "quant_dual": ("libb200_quant_dual.so", [(CSRC / "b200_quant_dual.cu", [])], []),
     "quant_block_dual": ("libb200_quant_block_dual.so", [(CSRC / "b200_quant_block_dual.cu", [])], []),

@@ -111,6 +111,7 @@ FP8BLOCK_1D1D_LIB = "libb200_fp8block_1d1d.so"       # csrc/b200_fp8_block_1d1d.
 QUANT_BLOCK_DUAL_LIB = "libb200_quant_block_dual.so"  # csrc/b200_quant_block_dual.h
 WGRAD_ACCUM_LIB = "libb200_wgrad_accum.so"   # csrc/b200_wgrad_accum.h
 SWIGLU_LIB = "libb200_swiglu.so"             # csrc/b200_swiglu.h
+GROUPED_SWIGLU_LIB = "libb200_grouped_swiglu.so"   # csrc/b200_grouped_swiglu.h
 _QUANT_BLOCK_DUAL = ([_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp], _i)
 _QUANT_BLOCKWISE = ([_i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp], _i)
 INTERNAL_ABI = {
@@ -177,6 +178,14 @@ INTERNAL_ABI = {
         "cuda_l2_b200_swiglu_backward": ([_i, _vp, _vp, _vp, _i, _i, _vp], _i),
         "cuda_l2_b200_swiglu_launch_count": ([], ctypes.c_ulonglong),
         "cuda_l2_b200_swiglu_strerror": ([_i], ctypes.c_char_p),
+    },
+    GROUPED_SWIGLU_LIB: {
+        "cuda_l2_b200_grouped_swiglu_run": ([_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_grouped_swiglu_run_config": ([_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_grouped_swiglu_select": ([_i, _i, _i, _i, _i, _ip, _ip], _i),
+        "cuda_l2_b200_grouped_swiglu_backward": ([_i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp], _i),
+        "cuda_l2_b200_grouped_swiglu_launch_count": ([], ctypes.c_ulonglong),
+        "cuda_l2_b200_grouped_swiglu_strerror": ([_i], ctypes.c_char_p),
     },
 }
 _TABLES = {**ABI, **INTERNAL_ABI}
@@ -1317,6 +1326,90 @@ def swiglu_select(variant: int, m: int, i: int, k: int) -> tuple[int, int, int]:
 
 def swiglu_launch_count() -> int:
     return int(swiglu_lib().cuda_l2_b200_swiglu_launch_count())
+
+
+# ------------------------------------------------------------------ grouped SwiGLU (libb200_grouped_swiglu.so)
+def grouped_swiglu_lib() -> ctypes.CDLL:
+    """libb200_grouped_swiglu.so: the gate / up GEMM of SwiGLU experts over contiguous row groups with silu(g) * u fused
+    into its epilogue, and the SwiGLU backward over the groups' rows (csrc/b200_grouped_swiglu.h, no public ABI)."""
+    return load(GROUPED_SWIGLU_LIB)
+
+
+def check_grouped_swiglu_operands(x, w_gu, offs) -> tuple[int, int, int, int]:
+    """(G, T, I, H) of y = swiglu(h) with h[start_g:end_g] = x[start_g:end_g] @ w_gu[g]^T: x [T, H] and the expert stack
+    w_gu [G, 2I, H] of one 16-bit dtype, H % 8 == 0, I % 64 == 0 (whole 64-row gate / up blocks), and the int32 group
+    ends ``offs`` [G]. Shapes and dtypes only (meta tensors pass); B200HgemmError otherwise."""
+    try:
+        (t, k), (g, n, k2) = x.shape, w_gu.shape
+    except ValueError:
+        raise B200HgemmError(f"x [T, H] and w_gu [G, 2I, H] expected, got {tuple(x.shape)} and "
+                             f"{tuple(w_gu.shape)}") from None
+    swiglu_variant(x.dtype)
+    if w_gu.dtype != x.dtype:
+        raise B200HgemmError(f"x and w_gu must share a dtype, got {x.dtype} and {w_gu.dtype}")
+    if k2 != k:
+        raise B200HgemmError(f"inner dimensions differ: x {tuple(x.shape)}, w_gu {tuple(w_gu.shape)} ([G, 2I, H])")
+    if g < 1:
+        raise B200HgemmError("w_gu must hold at least one expert")
+    if n == 0 or n % (2 * SWIGLU_BLOCK) or k % 8:
+        raise B200HgemmError(f"w_gu [G, 2I, H] needs I % {SWIGLU_BLOCK} == 0 (I > 0) and H % 8 == 0, got 2I={n}, H={k}")
+    _check_offs(offs, g)
+    return g, t, n // 2, k
+
+
+def grouped_swiglu(x, w_gu, offs, y, h=None, stream: int | None = None, config_id: int | None = None,
+                   group_m: int = 0, max_ctas: int = 0) -> None:
+    """y [T, I] = silu(g) * u of the grouped product h[start_g:end_g] = x[start_g:end_g] @ w_gu[g]^T, each expert's
+    gate and up rows interleaved in blocks of 64 (csrc/b200_grouped_swiglu.h), fp32 accumulation: torch's
+    ``F.silu(g) * u`` on the 16-bit h, bit for bit. ``offs``: int32 CUDA tensor [G] of cumulative group ends, read by
+    the kernel and clamped as for :func:`gemm_grouped`. ``h`` [T, 2I] (optional) receives h itself, the bits
+    :func:`gemm_grouped` writes with the same configuration. Rows of y and h at or past the last group's end are not
+    written. Contiguous CUDA tensors of one dtype (fp16 or bf16). ``config_id`` pins one configuration (BN = 128 or
+    256; tests; ``group_m``, ``max_ctas`` as for :func:`gemm_grouped`); default is the grouped dispatcher's choice for
+    (G, T, 2I, H) mapped to its gated sibling."""
+    _contiguous_cuda(x=x, w_gu=w_gu, y=y, h=h, offs=offs)
+    g, t, i, k = check_grouped_swiglu_operands(x, w_gu, offs)
+    if tuple(y.shape) != (t, i) or y.dtype != x.dtype or (h is not None and (tuple(h.shape) != (t, 2 * i) or
+                                                                             h.dtype != x.dtype)):
+        raise B200HgemmError(f"y must be [{t}, {i}] and h [{t}, {2 * i}] of {x.dtype}, got y {y.dtype} "
+                             f"{tuple(y.shape)}" + ("" if h is None else f", h {h.dtype} {tuple(h.shape)}"))
+    args = (x.data_ptr(), w_gu.data_ptr(), None if h is None else h.data_ptr(), y.data_ptr(), offs.data_ptr(), g, t, i,
+            k)
+    lib = grouped_swiglu_lib()
+    if config_id is None:
+        fn = lib.cuda_l2_b200_grouped_swiglu_run
+        st = fn(swiglu_variant(x.dtype), *args, stream)
+    else:
+        fn = lib.cuda_l2_b200_grouped_swiglu_run_config
+        st = fn(swiglu_variant(x.dtype), config_id, *args, group_m, max_ctas, stream)
+    _check(st, fn)
+
+
+def grouped_swiglu_backward(dy, h, dh, offs, stream: int | None = None) -> None:
+    """dh [T, 2I] = the gradient of y = silu(g) * u at h [T, 2I] for dy [T, I], in h's interleaved layout, for the rows
+    below the groups' last end (read on the device from the int32 CUDA tensor ``offs`` [G]): the steps torch's
+    autograd takes through ``F.silu(g) * u`` (csrc/b200_grouped_swiglu.h). Rows of dy and h at or past that end are
+    never read, and rows of dh there never written. Contiguous CUDA tensors of one dtype."""
+    _contiguous_cuda(dy=dy, h=h, dh=dh, offs=offs)
+    if dy.dim() != 2 or h.dim() != 2 or tuple(h.shape) != (dy.shape[0], 2 * dy.shape[1]) or dh.shape != h.shape or \
+            not dy.dtype == h.dtype == dh.dtype:
+        raise B200HgemmError(f"dy [T, I], h and dh [T, 2I] of one dtype expected, got dy {dy.dtype} {tuple(dy.shape)}, "
+                             f"h {h.dtype} {tuple(h.shape)}, dh {dh.dtype} {tuple(dh.shape)}")
+    if offs.dim() != 1:
+        raise B200HgemmError(f"offs must be an int32 tensor [G], got {tuple(offs.shape)}")
+    _check_offs(offs, offs.shape[0])
+    fn = grouped_swiglu_lib().cuda_l2_b200_grouped_swiglu_backward
+    _check(fn(swiglu_variant(dy.dtype), dy.data_ptr(), h.data_ptr(), dh.data_ptr(), offs.data_ptr(), offs.shape[0],
+              dy.shape[0], dy.shape[1], stream), fn)
+
+
+def grouped_swiglu_select(variant: int, g: int, t: int, i: int, h: int) -> tuple[int, int]:
+    """(config_id, group_m): the dispatched grouped SwiGLU call's choice for variant ``variant`` (0 fp16, 2 bf16)."""
+    return _select(grouped_swiglu_lib().cuda_l2_b200_grouped_swiglu_select, variant, g, t, i, h)
+
+
+def grouped_swiglu_launch_count() -> int:
+    return int(grouped_swiglu_lib().cuda_l2_b200_grouped_swiglu_launch_count())
 
 
 # ---------------------------------------------------------------- fp32 weight-gradient accumulation

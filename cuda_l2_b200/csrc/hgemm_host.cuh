@@ -468,13 +468,16 @@ struct LaunchArgs {
   const void* bias;     // BiasAct<> kernels: the bias (or null) ...
   int act;              // ... and the activation code
   GatedArgs gated;      // Gated<> kernels: y's map, and whether h (C) is stored
+  void* y;              // Gated<Grouped<>> kernels: y, for the boxes that straddle a group's end
 };
 
-// The kernel's last argument: the scales, BiasAct<>'s BiasActArgs, BlockScaled1D1D<>'s Block1D1DArgs, or AccumF32<>'s
-// AccumArgs (the wrapped kernel's argument and C, which is fp32).
+// The kernel's last argument: the scales, BiasAct<>'s BiasActArgs, BlockScaled1D1D<>'s Block1D1DArgs, AccumF32<>'s
+// AccumArgs (the wrapped kernel's argument and C, which is fp32), Gated<>'s GatedArgs or Gated<Grouped<>>'s
+// GroupedGatedArgs (GatedArgs and y).
 template <class Cfg>
 typename Cfg::EpiArgs epi_args(const LaunchArgs& a) {
-  if constexpr (is_gated<Cfg>()) return a.gated;
+  if constexpr (is_gated<Cfg>() && grouped<Cfg>()) return GroupedGatedArgs{a.gated, static_cast<__half*>(a.y)};
+  else if constexpr (is_gated<Cfg>()) return a.gated;
   else if constexpr (accum_f32<Cfg>())
     return typename Cfg::EpiArgs{epi_args<typename Cfg::AccumBase>(a), reinterpret_cast<float*>(a.c)};
   else if constexpr (bias_act<Cfg>()) return BiasActArgs{a.scales, a.bias, a.act};
@@ -730,13 +733,21 @@ int validate_list(GemmType type, const void* A, const void* Bt, const void* C, c
 //   GroupedK<> (`rows` is M, `K` is T): C[g] = A[start_g : end_g]^T B[start_g : end_g] for g < count, A [T, M] and
 //   `Bt` as B [T, N] row-major, C [count, M, N], the groups as for Grouped<>. Every matrix of C is written, an empty
 //   group's with +0.0; T == 0 zero-fills C on the stream and launches nothing (a map needs at least one row).
+//   Gated<Grouped<>>: Grouped<>'s product h = C [rows, N] (null: not stored) with the SwiGLU epilogue, y [rows, N / 2]
+//   (`y`, 16-byte aligned, N % 128 == 0): the rows of y below the last group's end are written, each by its own group.
 template <class Cfg>
 int launch_list(const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
                 cudaStream_t stream, int group_m = 0, int max_ctas = 0, Scales scales = Scales{nullptr, nullptr},
-                int ld_a = 0) {
+                int ld_a = 0, void* y = nullptr) {
   static_assert(batched<Cfg>() || grouped<Cfg>() || k_grouped<Cfg>(), "a Batched<>, Grouped<> or GroupedK<> configuration");
   constexpr GemmType kType = gemm_type<Cfg>();
   const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
+  [[maybe_unused]] const bool store_h = C != nullptr;
+  if constexpr (is_gated<Cfg>()) {
+    if (!y) return kNullPointer;
+    if (!C) C = y;   // for the argument rules and tmap_c, which is then never written
+    if ((reinterpret_cast<uintptr_t>(y) & 15) || N % 128) return kBadAlignment;
+  }
   int st = validate_list<Cfg>(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a);
   if (st != kOk || rows == 0) return st;
   const Elem elem = traits(kType).operand, output = traits(kType).output;
@@ -769,7 +780,16 @@ int launch_list(const void* A, const void* Bt, void* C, const int* list, int cou
   } else {
     if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, count)) != kOk) return st;
   }
-  if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, depth)) != kOk) return st;
+  if constexpr (is_gated<Cfg>()) {
+    // h's map (y's when h is not stored: never written) and y's, both in 64-column store boxes
+    if ((st = cache.get(store_h ? C : y, rows, store_h ? N : N / 2, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk)
+      return st;
+    if ((st = cache.get(y, rows, N / 2, Cfg::EPI_ROWS, &a.gated.y_map, Cfg::EPI_N, output)) != kOk) return st;
+    a.gated.store_h = store_h ? 1 : 0;
+    a.y = y;
+  } else {
+    if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, depth)) != kOk) return st;
+  }
   }
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = list_plan<Cfg>(tiles, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });

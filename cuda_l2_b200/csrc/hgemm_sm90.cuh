@@ -401,8 +401,30 @@ struct Gated : Base {
                 "SwiGLU: the 2-D 16-bit TN kernels with fp32 accumulation only");
   static_assert(Base::BN == 128 || Base::BN == 256, "SwiGLU: whole gate / up pairs of 64-column chunks per tile");
 };
+// Gated<Grouped<...>> (libb200_grouped_swiglu.so, the gate / up projection of MoE experts): Grouped<>'s main loop and
+// tile list over w_gu [G, 2I, K], each expert's matrix interleaved as above, with Gated<>'s epilogue. h goes through
+// Grouped<>'s store path (rows from the group's first row, a box that straddles the group's end stored row by row with
+// generic stores), and so does y: a 16-row box of y wholly inside the group is a TMA store of y_map ([T, I]), one that
+// straddles the group's end stores only the group's rows from the staging buffer to `y` [T, I] (the next group's CTA
+// owns the rest). Its own argument type, so that GatedArgs and the 2-D kernels stay as they are; the kernel is
+// hgemm_grouped_gated_kernel.
+struct GroupedGatedArgs : GatedArgs { __half* y; };
+template <class Base>
+struct Gated<Grouped<Base>> : Grouped<Base> {
+  using EpiArgs = GroupedGatedArgs;
+  static_assert(Base::ACC_F32 && !Base::E4M3 && !Base::BLOCK_SCALED && !Base::BATCHED && !Base::GROUPED &&
+                    !Base::ROW_MAJOR_B && !Base::K_GROUPED && !Base::BIAS_ACT && !Base::ACCUM_F32,
+                "grouped SwiGLU: the grouped 16-bit TN kernels with fp32 accumulation only");
+  static_assert(Base::BN == 128 || Base::BN == 256, "SwiGLU: whole gate / up pairs of 64-column chunks per tile");
+};
 template <class Cfg>
-__host__ __device__ constexpr bool is_gated() { return std::is_same_v<typename Cfg::EpiArgs, GatedArgs>; }
+__host__ __device__ constexpr bool is_gated() {
+  return std::is_same_v<typename Cfg::EpiArgs, GatedArgs> || std::is_same_v<typename Cfg::EpiArgs, GroupedGatedArgs>;
+}
+// y's pointer of a kernel's EpiArgs: null for the kernels without one
+template <class E>
+__host__ __device__ __forceinline__ __half* y_of(const E&) { return nullptr; }
+__host__ __device__ __forceinline__ __half* y_of(const GroupedGatedArgs& e) { return e.y; }
 
 // act(z) in fp32; `act` is warp-uniform. relu: max(z, +0.0) (+0.0 for -0.0 and NaN). gelu_tanh: 0.5 z (1 + tanhf(u)),
 // u = sqrt(2/pi) (z + 0.044715 z^3), torch's tanh approximation (F.gelu(approximate="tanh"), _addmm_activation), each
@@ -607,6 +629,10 @@ __device__ __forceinline__ void epilogue_store_chunk(const Reg (&d)[NR], int chu
   using namespace ptx;
   constexpr int EN = Cfg::EPI_N;
   constexpr int PER_CHUNK = EN / 4;   // packed pairs of one chunk per thread
+  // Gated<Grouped<>> kernels: the lane is hidden from the compiler, so that each chunk computes its staging offsets
+  // anew. Otherwise ptxas holds them across the SwiGLU epilogue and, next to the group's cursor, spills them to the
+  // stack in configuration 0. The other kernels are compiled as before.
+  if constexpr (is_gated<Cfg>() && grouped<Cfg>()) asm volatile("" : "+r"(lane));
   // the previous store from this warp's staging buffer must have finished reading it
   if (lane == 0) tma_store_wait_read<0>();
   __syncwarp();
@@ -700,15 +726,18 @@ __device__ __forceinline__ void bias_act_epilogue(Reg (&acc)[MR][NR], uint32_t e
 // Gated<> kernels: y of one gate / up pair of store chunks (J = chunk, J + 1) of this warp's 16 rows into the staging
 // buffer, then its TMA store at y's column col0 = (n0 + 64 J) / 2 and row row0. g and u are rounded to the output type
 // as the h store packs them (RN), so y is silu_mul of the 16-bit h. Rows past M are clipped by the map; I % 64 == 0, so
-// a pair is wholly inside or wholly outside y's columns.
+// a pair is wholly inside or wholly outside y's columns. Grouped kernels: M is the end row of the tile's group, and a
+// box that straddles it is copied out row by row to y_raw [., I] instead, as epilogue_store_chunk does for C.
 template <class Cfg, class Reg, int NR>
 __device__ __forceinline__ void gated_store_chunk(const Reg (&d)[NR], int chunk, uint32_t epi_buf, int lane,
-                                                  const CUtensorMap* tmap_y, int col0, int row0, int M, int I) {
+                                                  const CUtensorMap* tmap_y, int col0, int row0, int M, int I,
+                                                  __half* __restrict__ y_raw = nullptr) {
   using namespace ptx;
   using T = std::conditional_t<Cfg::BF16, __nv_bfloat16, __half>;
   constexpr int EN = Cfg::EPI_N;
   constexpr int PER_CHUNK = EN / 4;
   static_assert(EN == 64, "64-column chunks");
+  if constexpr (grouped<Cfg>()) asm volatile("" : "+r"(lane));   // see epilogue_store_chunk
   if (lane == 0) tma_store_wait_read<0>();
   __syncwarp();
 #pragma unroll
@@ -722,6 +751,22 @@ __device__ __forceinline__ void gated_store_chunk(const Reg (&d)[NR], int chunk,
   }
   fence_proxy_async_smem();
   __syncwarp();
+  if constexpr (grouped<Cfg>()) {
+    // a box that straddles the group's end (warp-uniform): only the rows below M, one 16-byte chunk per lane and step
+    if (row0 + Cfg::EPI_ROWS > M) {
+      constexpr int CPR = EN * 2 / 16;   // 16-byte chunks per staged row
+#pragma unroll 1
+      for (int i = lane; i < Cfg::EPI_ROWS * CPR; i += 32) {
+        const int r = i / CPR, c = i % CPR;
+        if (row0 + r < M && col0 + 8 * c < I) {
+          uint32_t off = uint32_t(r * (EN * 2) + c * 16);
+          off ^= ((off >> 7) & 7u) << 4;
+          *reinterpret_cast<uint4*>(y_raw + size_t(row0 + r) * I + col0 + 8 * c) = ld_shared_v4_b32(epi_buf + off);
+        }
+      }
+      return;
+    }
+  }
   if (lane == 0) {
     if (row0 < M && col0 < I) tma_store_2d(tmap_y, epi_buf, col0, row0);
     tma_store_commit();
@@ -730,22 +775,26 @@ __device__ __forceinline__ void gated_store_chunk(const Reg (&d)[NR], int chunk,
 
 // The plain epilogue of a Gated<> unit: for every 64-row block R of the warpgroup (rows m_row0 + 64 R ..) and every
 // gate / up pair of chunks (J, J + 1), h's two chunks when the launch stores h (epilogue_store_chunk, the wrapped
-// kernel's bits), then y's chunk (gated_store_chunk). Unrolled by recursion, as bias_act_epilogue is.
+// kernel's bits), then y's chunk (gated_store_chunk). Unrolled by recursion, as bias_act_epilogue is. Grouped kernels:
+// m_row0 counts from the group's first row, M is the group's end, and h_raw / y_raw take the rows of a box that
+// straddles it.
 template <class Cfg, int R = 0, int J = 0, class Reg, int MR, int NR>
 __device__ __forceinline__ void gated_epilogue(const Reg (&acc)[MR][NR], uint32_t epi_buf, int lane,
                                                const CUtensorMap* tmap_h, const GatedArgs& epi, int m_row0, int n0,
-                                               int M, int N) {
+                                               int M, int N, __half* __restrict__ h_raw = nullptr,
+                                               __half* __restrict__ y_raw = nullptr) {
   if constexpr (R < MR) {
     const int row0 = m_row0 + R * 64;
     if constexpr (J < Cfg::EPI_CHUNKS) {
       if (epi.store_h) {
-        epilogue_store_chunk<Cfg>(acc[R], J, epi_buf, lane, tmap_h, n0 + J * Cfg::EPI_N, row0, M, N);
-        epilogue_store_chunk<Cfg>(acc[R], J + 1, epi_buf, lane, tmap_h, n0 + (J + 1) * Cfg::EPI_N, row0, M, N);
+        epilogue_store_chunk<Cfg>(acc[R], J, epi_buf, lane, tmap_h, n0 + J * Cfg::EPI_N, row0, M, N, nullptr, 0, h_raw);
+        epilogue_store_chunk<Cfg>(acc[R], J + 1, epi_buf, lane, tmap_h, n0 + (J + 1) * Cfg::EPI_N, row0, M, N, nullptr,
+                                  0, h_raw);
       }
-      gated_store_chunk<Cfg>(acc[R], J, epi_buf, lane, &epi.y_map, (n0 + J * Cfg::EPI_N) / 2, row0, M, N / 2);
-      gated_epilogue<Cfg, R, J + 2>(acc, epi_buf, lane, tmap_h, epi, m_row0, n0, M, N);
+      gated_store_chunk<Cfg>(acc[R], J, epi_buf, lane, &epi.y_map, (n0 + J * Cfg::EPI_N) / 2, row0, M, N / 2, y_raw);
+      gated_epilogue<Cfg, R, J + 2>(acc, epi_buf, lane, tmap_h, epi, m_row0, n0, M, N, h_raw, y_raw);
     } else {
-      gated_epilogue<Cfg, R + 1, 0>(acc, epi_buf, lane, tmap_h, epi, m_row0, n0, M, N);
+      gated_epilogue<Cfg, R + 1, 0>(acc, epi_buf, lane, tmap_h, epi, m_row0, n0, M, N, h_raw, y_raw);
     }
   }
 }
@@ -1159,10 +1208,25 @@ hgemm_gated_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 #include "hgemm_tn_kernel_body.inc"
 }
 
+// The same over contiguous row groups (Gated<Grouped<>>): the parameters of hgemm_tn_kernel with Grouped<>'s meaning
+// (splits_arg G, splitk_ctr the offsets, c_raw h), GroupedGatedArgs (y's map and y itself) last.
+template <class Cfg, int KMODE = kPlain>
+__global__ void __launch_bounds__(kNumThreads, 1)
+hgemm_grouped_gated_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                           const __grid_constant__ CUtensorMap tmap_c, int M, int N, int K, int group_m,
+                           int splits_arg, int aux_arg, float* __restrict__ splitk_ws,
+                           unsigned* __restrict__ splitk_ctr, __half* __restrict__ c_raw, uint64_t hint_a,
+                           uint64_t hint_b, const __grid_constant__ GroupedGatedArgs epi) {
+  static_assert(is_gated<Cfg>() && grouped<Cfg>() && KMODE == kPlain, "a Gated<Grouped<>> configuration, plain schedule");
+  const Scales scales{nullptr, nullptr};   // 16-bit operands: no scales
+#include "hgemm_tn_kernel_body.inc"
+}
+
 // The kernel of (Cfg, KMODE).
 template <class Cfg, int KMODE>
 constexpr auto kernel_of() {
-  if constexpr (is_gated<Cfg>()) return &hgemm_gated_kernel<Cfg, KMODE>;
+  if constexpr (is_gated<Cfg>() && grouped<Cfg>()) return &hgemm_grouped_gated_kernel<Cfg, KMODE>;
+  else if constexpr (is_gated<Cfg>()) return &hgemm_gated_kernel<Cfg, KMODE>;
   else if constexpr (accum_f32<Cfg>()) return &hgemm_accum_kernel<Cfg, KMODE>;
   else if constexpr (bias_act<Cfg>()) return &hgemm_bias_act_kernel<Cfg, KMODE>;
   else if constexpr (block_1d1d<Cfg>()) return &hgemm_block_1d1d_kernel<Cfg, KMODE>;

@@ -666,24 +666,32 @@ class B200Linear(nn.Module):
 def interleave_gate_up(w_gate: torch.Tensor, w_up: torch.Tensor) -> torch.Tensor:
     """The fused gate / up weight ``w_gu`` [2I, H] of a SwiGLU MLP from its gate and up weights [I, H] (a copy): rows
     [128 b, 128 b + 64) are gate rows [64 b, 64 b + 64), rows [128 b + 64, 128 b + 128) the matching up rows. I must be
-    a multiple of 64."""
-    if w_gate.dim() != 2 or w_gate.shape != w_up.shape or w_gate.shape[0] % capi.SWIGLU_BLOCK:
+    a multiple of 64. An expert stack ([G, I, H] each) gives [G, 2I, H], every expert's matrix interleaved so."""
+    if w_gate.dim() == 3:
+        if w_gate.shape != w_up.shape or w_gate.shape[1] % capi.SWIGLU_BLOCK:
+            raise capi.B200HgemmError(f"gate and up expert stacks must both be [G, I, H] with I % {capi.SWIGLU_BLOCK} "
+                                      f"== 0, got {tuple(w_gate.shape)} and {tuple(w_up.shape)}")
+    elif w_gate.dim() != 2 or w_gate.shape != w_up.shape or w_gate.shape[0] % capi.SWIGLU_BLOCK:
         raise capi.B200HgemmError(f"gate and up weights must both be [I, H] with I % {capi.SWIGLU_BLOCK} == 0, got "
                                   f"{tuple(w_gate.shape)} and {tuple(w_up.shape)}")
-    i, h = w_gate.shape
+    lead, (i, h) = w_gate.shape[:-2], w_gate.shape[-2:]
     blk = capi.SWIGLU_BLOCK
-    return torch.stack((w_gate.reshape(i // blk, blk, h), w_up.reshape(i // blk, blk, h)), dim=1).reshape(2 * i, h)
+    return torch.stack((w_gate.reshape(*lead, i // blk, blk, h), w_up.reshape(*lead, i // blk, blk, h)),
+                       dim=-3).reshape(*lead, 2 * i, h)
 
 
 def split_gate_up(w_gu: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
     """``(w_gate, w_up)``, each [I, H], of a fused gate / up weight ``w_gu`` [2I, H] (copies): the inverse of
-    :func:`interleave_gate_up`."""
+    :func:`interleave_gate_up`. An expert stack [G, 2I, H] gives two stacks [G, I, H]."""
     blk = capi.SWIGLU_BLOCK
-    if w_gu.dim() != 2 or w_gu.shape[0] % (2 * blk):
+    if w_gu.dim() == 3:
+        if w_gu.shape[1] % (2 * blk):
+            raise capi.B200HgemmError(f"w_gu expert stack must be [G, 2I, H] with I % {blk} == 0, got {tuple(w_gu.shape)}")
+    elif w_gu.dim() != 2 or w_gu.shape[0] % (2 * blk):
         raise capi.B200HgemmError(f"w_gu must be [2I, H] with I % {blk} == 0, got {tuple(w_gu.shape)}")
-    n, h = w_gu.shape
-    v = w_gu.reshape(n // (2 * blk), 2, blk, h)
-    return tuple(v[:, j].clone(memory_format=torch.contiguous_format).view(n // 2, h) for j in (0, 1))
+    lead, (n, h) = w_gu.shape[:-2], w_gu.shape[-2:]
+    v = w_gu.reshape(*lead, n // (2 * blk), 2, blk, h)
+    return tuple(v.select(-3, j).clone(memory_format=torch.contiguous_format).view(*lead, n // 2, h) for j in (0, 1))
 
 
 def _swiglu_forward(x2: torch.Tensor, w_gu: torch.Tensor, want_h: bool):
@@ -789,6 +797,127 @@ class B200SwiGLULinear(nn.Module):
 
     def extra_repr(self) -> str:
         return f"in_features={self.in_features}, intermediate_features={self.intermediate_features}"
+
+
+# ------------------------------------------------------------------ grouped SwiGLU (libb200_grouped_swiglu.so)
+def _grouped_swiglu_forward(x: torch.Tensor, w_gu: torch.Tensor, offs: torch.Tensor, want_h: bool):
+    """(y [T, I], h [T, 2I] or None) of the fused grouped gate / up product of ``x`` [T, H] by the expert stack ``w_gu``
+    [G, 2I, H]: one launch of libb200_grouped_swiglu.so. T == 0 launches nothing, and H == 0 makes y (and h) zero, as
+    :func:`_swiglu_forward` does."""
+    _, t, i, k = capi.check_grouped_swiglu_operands(x, w_gu, offs)
+    if not x.is_cuda or not w_gu.is_cuda or not offs.is_cuda:
+        raise capi.B200HgemmError("grouped_swiglu_linear has no CPU implementation (and no fallback): move the tensors "
+                                  "to an H100")
+    y = torch.empty((t, i), dtype=x.dtype, device=x.device)
+    h = torch.empty((t, 2 * i), dtype=x.dtype, device=x.device) if want_h else None
+    if t == 0:
+        return y, h
+    if k == 0:   # h = 0, so y = silu(0) * 0 = +0
+        y.zero_()
+        if h is not None:
+            h.zero_()
+        return y, h
+    with torch.cuda.device(x.device):
+        capi.grouped_swiglu(x.contiguous(), w_gu.contiguous(), offs.contiguous(), y, h,
+                            stream=torch.cuda.current_stream(x.device).cuda_stream)
+    return y, h
+
+
+class _GroupedSwiGLULinearFunction(torch.autograd.Function):
+    """y = silu(g) * u of the grouped product h = x w_gu[g]^T per group, saving x, w_gu, offs and h. The backward is one
+    pass of libb200_grouped_swiglu.so's SwiGLU gradient over the groups' rows (dh from dy and h), then dX from
+    :func:`_grouped_input_grad` (zero past the last end) and dW [G, 2I, H] from :func:`hgemm_grouped_wgrad`. Rows of dy
+    at or past the last end are never read. No host synchronisation."""
+
+    @staticmethod
+    def forward(ctx, x, w_gu, offs):
+        x, w_gu, offs = x.contiguous(), w_gu.contiguous(), offs.contiguous()
+        y, h = _grouped_swiglu_forward(x, w_gu, offs, True)
+        ctx.save_for_backward(x, w_gu, offs, h)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        x, w_gu, offs, h = ctx.saved_tensors
+        dh = torch.empty_like(h)
+        if dh.numel():
+            with torch.cuda.device(h.device):
+                capi.grouped_swiglu_backward(grad_y.contiguous(), h, dh, offs,
+                                             stream=torch.cuda.current_stream(h.device).cuda_stream)
+        grad_x = _grouped_input_grad(dh, x, w_gu, offs, "fp32") if ctx.needs_input_grad[0] else None
+        grad_w = None
+        if ctx.needs_input_grad[1]:
+            grad_w = torch.ops.cuda_l2_b200.hgemm_grouped_wgrad(dh, x, offs, "fp32")
+        return grad_x, grad_w, None
+
+
+def grouped_swiglu_linear(x: torch.Tensor, w_gu: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+    """The gate and up projections of SwiGLU experts with the activation: ``x`` [T, H] sorted into contiguous groups by
+    the int32 cumulative ends ``offs`` [G] (on the GPU), ``w_gu`` [G, 2I, H] one fused gate / up weight per expert
+    (:func:`interleave_gate_up` of expert stacks) -> y [T, I], rows [offs[g-1], offs[g]) being ``F.silu(x[rows] @
+    W_gate[g]^T) * (x[rows] @ W_up[g]^T)``, as one grouped GEMM whose epilogue applies the SwiGLU: fp16 or bf16 with
+    fp32 accumulation, bit for bit torch's ``F.silu(g) * u`` on the 16-bit grouped product. Rows at or past
+    ``offs[-1]`` are unspecified. Differentiable in ``x`` and ``w_gu``; without a gradient to compute, h is never
+    written. The backward never reads rows of the output gradient at or past ``offs[-1]`` and gives dX zero there. No
+    host synchronisation in either direction, so a training step can be captured in a CUDA graph with the offsets
+    changing between replays. I % 64 == 0 and H % 8 == 0."""
+    if torch.is_grad_enabled() and (x.requires_grad or w_gu.requires_grad):
+        return _GroupedSwiGLULinearFunction.apply(x, w_gu, offs)
+    y, _ = _grouped_swiglu_forward(x, w_gu, offs, False)
+    return y
+
+
+class B200GroupedSwiGLULinear(nn.Module):
+    """The gate and up projections of the SwiGLU experts of a mixture-of-experts layer (Mixtral, Qwen-MoE, DeepSeek)
+    with the activation, as one layer: ``forward(x, offs)`` takes the tokens sorted by expert, ``x`` [T, H], and the
+    int32 cumulative group ends ``offs`` [G] on the GPU, and runs :func:`grouped_swiglu_linear`. The Parameter
+    ``weight`` is the expert stack ``w_gu`` [G, 2I, H], each expert's gate and up rows interleaved in blocks of 64
+    (:func:`interleave_gate_up`, :func:`split_gate_up`). Rows at or past ``offs[-1]`` of the result are unspecified.
+    No bias. fp16 or bf16; I % 64 == 0 and H % 8 == 0."""
+
+    def __init__(self, num_groups: int, in_features: int, intermediate_features: int, device=None,
+                 dtype: torch.dtype = torch.bfloat16):
+        super().__init__()
+        self._check(num_groups, in_features, intermediate_features, dtype)
+        self.num_groups, self.in_features, self.intermediate_features = num_groups, in_features, intermediate_features
+        self.weight = nn.Parameter(torch.empty((num_groups, 2 * intermediate_features, in_features), device=device,
+                                               dtype=dtype))
+        bound = 1.0 / (in_features ** 0.5)
+        with torch.no_grad():
+            self.weight.uniform_(-bound, bound)
+
+    @staticmethod
+    def _check(g: int, h: int, i: int, dtype: torch.dtype) -> None:
+        if g < 1 or dtype not in (torch.float16, torch.bfloat16) or h <= 0 or h % 8 or i <= 0 or \
+                i % capi.SWIGLU_BLOCK:
+            raise capi.B200HgemmError(f"B200GroupedSwiGLULinear needs G >= 1, fp16 / bf16, in_features % 8 == 0 and "
+                                      f"intermediate_features % {capi.SWIGLU_BLOCK} == 0, got G={g}, {h} -> {i} {dtype}")
+
+    @classmethod
+    def from_weights(cls, w_gate: torch.Tensor, w_up: torch.Tensor) -> "B200GroupedSwiGLULinear":
+        """The layer of the expert stacks ``w_gate`` and ``w_up`` [G, I, H] of one dtype and device, interleaved into a
+        new, trainable Parameter (a copy), as :meth:`B200GroupedLinear.from_weights` makes one. A vLLM-style ``w13``
+        [G, 2I, H] (gate rows first) is ``from_weights(w13[:, :I], w13[:, I:])``."""
+        if w_gate.dim() != 3 or w_gate.shape != w_up.shape or w_gate.dtype != w_up.dtype or \
+                w_gate.device != w_up.device:
+            raise capi.B200HgemmError(f"gate and up stacks must both be [G, I, H] of one dtype and device, got "
+                                      f"{tuple(w_gate.shape)} {w_gate.dtype} {w_gate.device} and {tuple(w_up.shape)} "
+                                      f"{w_up.dtype} {w_up.device}")
+        g, i, h = w_gate.shape
+        cls._check(g, h, i, w_gate.dtype)
+        new = cls.__new__(cls)
+        nn.Module.__init__(new)
+        new.num_groups, new.in_features, new.intermediate_features = g, h, i
+        with torch.no_grad():
+            new.weight = nn.Parameter(interleave_gate_up(w_gate, w_up))
+        return new
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+        return grouped_swiglu_linear(x, self.weight, offs)
+
+    def extra_repr(self) -> str:
+        return (f"num_groups={self.num_groups}, in_features={self.in_features}, "
+                f"intermediate_features={self.intermediate_features}")
 
 
 def replace_linear_modules(model: nn.Module, acc: str = "fp32", skip: tuple[str, ...] = ()) -> list[str]:
