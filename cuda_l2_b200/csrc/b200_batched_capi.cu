@@ -27,16 +27,15 @@ int b200_batched_gemm(int variant, const void* A, const void* B_kmajor, void* C,
                       int N, int K, void* stream) {
   using namespace b200;
   if (!tile_list::holds(tile_list::Library{}, variant)) return host::kBadConfig;
-  return tile_list::gemm(tile_list::Library{}, GemmType(variant), A, B_kmajor, C, Scales{nullptr, nullptr}, 0,
-                         masked_m, B, M, N, K, stream);
+  return tile_list::gemm(tile_list::Library{}, GemmType(variant), A, B_kmajor, C, masked_m, B, M, N, K, stream);
 }
 
 int b200_batched_gemm_run_config(int variant, int config_id, const void* A, const void* B_kmajor, void* C,
                                  const int* masked_m, int B, int M, int N, int K, int group_m, int max_ctas,
                                  void* stream) {
   using namespace b200;
-  return tile_list::run(tile_list::Library{}, GemmType(variant), config_id, A, B_kmajor, C, Scales{nullptr, nullptr}, 0,
-                        masked_m, B, M, N, K, group_m, max_ctas, stream);
+  return tile_list::run(tile_list::Library{}, GemmType(variant), config_id, A, B_kmajor, C, masked_m, B, M, N, K,
+                        group_m, max_ctas, stream);
 }
 
 int b200_batched_select(int variant, int B, int M, int N, int K, int* config_id, int* group_m) {

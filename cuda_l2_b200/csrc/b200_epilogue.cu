@@ -13,15 +13,11 @@
 
 namespace b200 {
 
-#define B200_EPI_RUN(T)                                                                                       \
-  int run_config<T, BiasAct>(int, const void*, const void*, void*, Scales, int, int, int, int, int, int, void*, \
-                             int, host::ScratchFn, const void*, int, int)
-extern template B200_EPI_RUN(host::GemmType::kF16Acc32);
-extern template B200_EPI_RUN(host::GemmType::kBF16);
-extern template B200_EPI_RUN(host::GemmType::kE4M3F16);
-extern template B200_EPI_RUN(host::GemmType::kE4M3BF16);
-template B200_EPI_RUN(host::GemmType(B200_VARIANT));
-#undef B200_EPI_RUN
+extern template B200_RUN(host::GemmType::kF16Acc32, BiasAct);
+extern template B200_RUN(host::GemmType::kBF16, BiasAct);
+extern template B200_RUN(host::GemmType::kE4M3F16, BiasAct);
+extern template B200_RUN(host::GemmType::kE4M3BF16, BiasAct);
+template B200_RUN(host::GemmType(B200_VARIANT), BiasAct);
 
 }  // namespace b200
 
@@ -36,29 +32,32 @@ bool known_variant(int v) {
          v == int(GemmType::kE4M3BF16);
 }
 
-b200::Scales scales_of(int variant, const void* scale_a, const void* scale_b, int rowwise) {
-  if (!b200::host::traits(GemmType(variant)).scaled) return b200::Scales{nullptr, nullptr};
-  return b200::Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b), rowwise != 0};
+// The epilogue operands of a call: the scales of an e4m3 variant, the bias and the activation code.
+b200::host::EpiOperands operands(int variant, const void* scale_a, const void* scale_b, int rowwise, const void* bias,
+                                 int act) {
+  const b200::Scales sc = b200::host::traits(GemmType(variant)).scaled
+      ? b200::Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b), rowwise != 0}
+      : b200::Scales{nullptr, nullptr};
+  return {sc, 0, 0, bias, act};
 }
 
-int run_config(int variant, int config_id, const void* A, const void* Bt, void* C, b200::Scales sc, const void* bias,
-               int act, int M, int N, int K, int group_m, int max_ctas, int splits, void* stream) {
+// Split-K scratch comes from this library's own pool (host::splitk_scratch, run_config's default).
+int run_config(int variant, int config_id, const void* A, const void* Bt, void* C, const b200::host::EpiOperands& op,
+               int M, int N, int K, int group_m, int max_ctas, int splits, void* stream) {
   using b200::BiasAct;
   using b200::run_config;
-  const b200::host::ScratchFn scratch = b200::host::splitk_scratch;   // this library's own pool
   switch (GemmType(variant)) {
     case GemmType::kF16Acc32:
-      return run_config<GemmType::kF16Acc32, BiasAct>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas, splits,
-                                                      stream, 0, scratch, bias, act);
+      return run_config<GemmType::kF16Acc32, BiasAct>(config_id, A, Bt, C, M, N, K, group_m, max_ctas, splits, stream,
+                                                      op);
     case GemmType::kBF16:
-      return run_config<GemmType::kBF16, BiasAct>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas, splits, stream,
-                                                  0, scratch, bias, act);
+      return run_config<GemmType::kBF16, BiasAct>(config_id, A, Bt, C, M, N, K, group_m, max_ctas, splits, stream, op);
     case GemmType::kE4M3F16:
-      return run_config<GemmType::kE4M3F16, BiasAct>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas, splits,
-                                                     stream, 0, scratch, bias, act);
+      return run_config<GemmType::kE4M3F16, BiasAct>(config_id, A, Bt, C, M, N, K, group_m, max_ctas, splits, stream,
+                                                     op);
     case GemmType::kE4M3BF16:
-      return run_config<GemmType::kE4M3BF16, BiasAct>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas, splits,
-                                                      stream, 0, scratch, bias, act);
+      return run_config<GemmType::kE4M3BF16, BiasAct>(config_id, A, Bt, C, M, N, K, group_m, max_ctas, splits, stream,
+                                                      op);
     default:
       return b200::host::kBadConfig;
   }
@@ -74,18 +73,18 @@ int cuda_l2_b200_epilogue_run(int variant, const void* A, const void* B_kmajor, 
   using namespace b200;
   if (!known_variant(variant)) return host::kBadConfig;
   // the argument rules before the lookup, which wants a valid shape
-  const Scales sc = scales_of(variant, scale_a, scale_b, rowwise);
-  if (const int st = host::validate(GemmType(variant), A, B_kmajor, C, sc, M, N, K)) return st;
+  const host::EpiOperands op = operands(variant, scale_a, scale_b, rowwise, bias, act);
+  if (const int st = host::validate(GemmType(variant), A, B_kmajor, C, op, M, N, K)) return st;
   if (const int st = host::validate_bias_act(bias, act)) return st;
   const dispatch::Choice ch = dispatch::select(GemmType(variant), M, N, K);
-  return run_config(variant, ch.config_id, A, B_kmajor, C, sc, bias, act, M, N, K, ch.group_m, 0, ch.splits, stream);
+  return run_config(variant, ch.config_id, A, B_kmajor, C, op, M, N, K, ch.group_m, 0, ch.splits, stream);
 }
 
 int cuda_l2_b200_epilogue_run_config(int variant, int config_id, const void* A, const void* B_kmajor, void* C,
                                      const void* scale_a, const void* scale_b, int rowwise, const void* bias, int act,
                                      int M, int N, int K, int group_m, int max_ctas, int splits, void* stream) {
   if (!known_variant(variant)) return b200::host::kBadConfig;
-  return run_config(variant, config_id, A, B_kmajor, C, scales_of(variant, scale_a, scale_b, rowwise), bias, act, M, N,
+  return run_config(variant, config_id, A, B_kmajor, C, operands(variant, scale_a, scale_b, rowwise, bias, act), M, N,
                     K, group_m, max_ctas, splits, stream);
 }
 

@@ -13,13 +13,9 @@
 
 namespace b200 {
 
-#define B200_1D1D_RUN(T)                                                                                        \
-  int run_config<T, BlockScaled1D1D>(int, const void*, const void*, void*, Scales, int, int, int, int, int, int, \
-                                     void*, int, host::ScratchFn, const void*, int, int)
-extern template B200_1D1D_RUN(host::GemmType::kE4M3F16Block1D1D);
-extern template B200_1D1D_RUN(host::GemmType::kE4M3BF16Block1D1D);
-template B200_1D1D_RUN(host::GemmType(B200_VARIANT));
-#undef B200_1D1D_RUN
+extern template B200_RUN(host::GemmType::kE4M3F16Block1D1D, BlockScaled1D1D);
+extern template B200_RUN(host::GemmType::kE4M3BF16Block1D1D, BlockScaled1D1D);
+template B200_RUN(host::GemmType(B200_VARIANT), BlockScaled1D1D);
 
 }  // namespace b200
 
@@ -29,22 +25,21 @@ namespace {
 
 using b200::host::GemmType;
 
-b200::Scales scales_of(const void* scale_a, const void* scale_b) {
-  return b200::Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
+// The epilogue operands of a call: both operands' 1 x 128 scales and their row strides.
+b200::host::EpiOperands operands(const void* scale_a, int ld_a, const void* scale_b, int ld_b) {
+  return {b200::Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)}, ld_a, ld_b};
 }
 
-int run(int config_id, int out_bf16, const void* A, const void* Bt, void* C, b200::Scales sc, int ld_a, int ld_b, int M,
+int run(int config_id, int out_bf16, const void* A, const void* Bt, void* C, const b200::host::EpiOperands& op, int M,
         int N, int K, int group_m, int max_ctas, int splits, void* stream) {
   using b200::BlockScaled1D1D;
   using b200::run_config;
-  const b200::host::ScratchFn scratch = b200::host::splitk_scratch;   // never called: no workspace mode is compiled
   if (out_bf16 == 0)
-    return run_config<GemmType::kE4M3F16Block1D1D, BlockScaled1D1D>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas,
-                                                                    splits, stream, ld_a, scratch, nullptr, 0, ld_b);
+    return run_config<GemmType::kE4M3F16Block1D1D, BlockScaled1D1D>(config_id, A, Bt, C, M, N, K, group_m, max_ctas,
+                                                                    splits, stream, op);
   if (out_bf16 == 1)
-    return run_config<GemmType::kE4M3BF16Block1D1D, BlockScaled1D1D>(config_id, A, Bt, C, sc, M, N, K, group_m,
-                                                                     max_ctas, splits, stream, ld_a, scratch, nullptr, 0,
-                                                                     ld_b);
+    return run_config<GemmType::kE4M3BF16Block1D1D, BlockScaled1D1D>(config_id, A, Bt, C, M, N, K, group_m, max_ctas,
+                                                                     splits, stream, op);
   return b200::host::kBadConfig;
 }
 
@@ -57,17 +52,17 @@ int cuda_l2_b200_fp8block_1d1d_run(const void* A, const void* B_kmajor, void* C,
   using namespace b200;
   if (out_bf16 != 0 && out_bf16 != 1) return host::kBadConfig;
   // the argument rules before the lookup, which wants a valid shape
-  const Scales sc = scales_of(scale_a, scale_b);
-  if (const int st = host::validate(GemmType::kE4M3F16Block1D1D, A, B_kmajor, C, sc, M, N, K, ld_a)) return st;
+  const host::EpiOperands op = operands(scale_a, ld_a, scale_b, ld_b);
+  if (const int st = host::validate(GemmType::kE4M3F16Block1D1D, A, B_kmajor, C, op, M, N, K)) return st;
   if (ld_b < N || ld_b % 4) return host::kBadScaleLdB;
   const dispatch::Choice ch = block::select(M, N, K);
-  return run(ch.config_id, out_bf16, A, B_kmajor, C, sc, ld_a, ld_b, M, N, K, ch.group_m, 0, ch.splits, stream);
+  return run(ch.config_id, out_bf16, A, B_kmajor, C, op, M, N, K, ch.group_m, 0, ch.splits, stream);
 }
 
 int cuda_l2_b200_fp8block_1d1d_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
                                           const void* scale_a, int ld_a, const void* scale_b, int ld_b, int M, int N,
                                           int K, int group_m, int max_ctas, int splits, void* stream) {
-  return run(config_id, out_bf16, A, B_kmajor, C, scales_of(scale_a, scale_b), ld_a, ld_b, M, N, K, group_m, max_ctas,
+  return run(config_id, out_bf16, A, B_kmajor, C, operands(scale_a, ld_a, scale_b, ld_b), M, N, K, group_m, max_ctas,
              splits, stream);
 }
 

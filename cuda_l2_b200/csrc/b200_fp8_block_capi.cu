@@ -13,18 +13,19 @@ namespace block {
 
 // (eligible(), sibling() and kModes are in hgemm_configs.cuh, select() in hgemm_dispatch.cuh.)
 
-Scales scales_of(const void* scale_a, const void* scale_b) {
-  return Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)};
+// The epilogue operands of a call: the block scales and the row stride of A's.
+host::EpiOperands operands(const void* scale_a, int ld_a, const void* scale_b) {
+  return {Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b)}, ld_a};
 }
 
-int run(int config_id, int out_bf16, const void* A, const void* Bt, void* C, Scales sc, int ld_a, int M, int N, int K,
-        int group_m, int max_ctas, int splits, void* stream) {
+int run(int config_id, int out_bf16, const void* A, const void* Bt, void* C, const host::EpiOperands& op, int M, int N,
+        int K, int group_m, int max_ctas, int splits, void* stream) {
   if (out_bf16 == 0)
-    return run_config<GemmType::kE4M3F16Block, BlockScaled>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas,
-                                                            splits, stream, ld_a);
+    return run_config<GemmType::kE4M3F16Block, BlockScaled>(config_id, A, Bt, C, M, N, K, group_m, max_ctas, splits,
+                                                            stream, op);
   if (out_bf16 == 1)
-    return run_config<GemmType::kE4M3BF16Block, BlockScaled>(config_id, A, Bt, C, sc, M, N, K, group_m, max_ctas,
-                                                             splits, stream, ld_a);
+    return run_config<GemmType::kE4M3BF16Block, BlockScaled>(config_id, A, Bt, C, M, N, K, group_m, max_ctas, splits,
+                                                             stream, op);
   return host::kBadConfig;
 }
 
@@ -37,17 +38,17 @@ int b200_fp8gemm_blockwise(const void* A, const void* B_kmajor, void* C, const v
                            const void* scale_b, int out_bf16, int M, int N, int K, void* stream) {
   using namespace b200;
   if (out_bf16 != 0 && out_bf16 != 1) return host::kBadConfig;
-  const Scales sc = block::scales_of(scale_a, scale_b);
-  if (const int st = host::validate(GemmType::kE4M3F16Block, A, B_kmajor, C, sc, M, N, K, ld_a)) return st;
+  const host::EpiOperands op = block::operands(scale_a, ld_a, scale_b);
+  if (const int st = host::validate(GemmType::kE4M3F16Block, A, B_kmajor, C, op, M, N, K)) return st;
   const dispatch::Choice ch = block::select(M, N, K);
-  return block::run(ch.config_id, out_bf16, A, B_kmajor, C, sc, ld_a, M, N, K, ch.group_m, 0, ch.splits, stream);
+  return block::run(ch.config_id, out_bf16, A, B_kmajor, C, op, M, N, K, ch.group_m, 0, ch.splits, stream);
 }
 
 int b200_fp8gemm_blockwise_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
                                       const void* scale_a, int ld_a, const void* scale_b, int M, int N, int K,
                                       int group_m, int max_ctas, int splits, void* stream) {
-  return b200::block::run(config_id, out_bf16, A, B_kmajor, C, b200::block::scales_of(scale_a, scale_b), ld_a, M,
-                          N, K, group_m, max_ctas, splits, stream);
+  return b200::block::run(config_id, out_bf16, A, B_kmajor, C, b200::block::operands(scale_a, ld_a, scale_b), M, N,
+                          K, group_m, max_ctas, splits, stream);
 }
 
 int b200_fp8gemm_blockwise_select(int M, int N, int K, int* config_id, int* group_m, int* splits) {

@@ -11,23 +11,25 @@ using b200::host::GemmType;
 
 namespace {
 
-b200::Scales scales_of(const void* scale_a, const void* scale_b, bool rowwise) {
-  return b200::Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b), rowwise};
+// The epilogue operands of a call: the per-tensor or rowwise scales.
+b200::host::EpiOperands scales_of(const void* scale_a, const void* scale_b, bool rowwise) {
+  return {b200::Scales{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b), rowwise}};
 }
 
-int fp8_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C, b200::Scales sc, int M,
-                   int N, int K, int group_m, int max_ctas, int splits, void* stream) {
+int fp8_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
+                   const b200::host::EpiOperands& op, int M, int N, int K, int group_m, int max_ctas, int splits,
+                   void* stream) {
   if (out_bf16 == 0)
-    return b200::run_config<GemmType::kE4M3F16>(config_id, A, B_kmajor, C, sc, M, N, K, group_m, max_ctas, splits, stream);
+    return b200::run_config<GemmType::kE4M3F16>(config_id, A, B_kmajor, C, M, N, K, group_m, max_ctas, splits, stream, op);
   if (out_bf16 == 1)
-    return b200::run_config<GemmType::kE4M3BF16>(config_id, A, B_kmajor, C, sc, M, N, K, group_m, max_ctas, splits, stream);
+    return b200::run_config<GemmType::kE4M3BF16>(config_id, A, B_kmajor, C, M, N, K, group_m, max_ctas, splits, stream, op);
   return b200::host::kBadConfig;
 }
 
-int fp8_gemm(const void* A, const void* B_kmajor, void* C, b200::Scales sc, int out_bf16, int M, int N, int K,
-             void* stream) {
-  if (out_bf16 == 0) return b200::dispatch::gemm<GemmType::kE4M3F16>(A, B_kmajor, C, sc, M, N, K, stream);
-  if (out_bf16 == 1) return b200::dispatch::gemm<GemmType::kE4M3BF16>(A, B_kmajor, C, sc, M, N, K, stream);
+int fp8_gemm(const void* A, const void* B_kmajor, void* C, const b200::host::EpiOperands& op, int out_bf16, int M, int N,
+             int K, void* stream) {
+  if (out_bf16 == 0) return b200::dispatch::gemm<GemmType::kE4M3F16>(A, B_kmajor, C, M, N, K, stream, op);
+  if (out_bf16 == 1) return b200::dispatch::gemm<GemmType::kE4M3BF16>(A, B_kmajor, C, M, N, K, stream, op);
   return b200::host::kBadConfig;
 }
 

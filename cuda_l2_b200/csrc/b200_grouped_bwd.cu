@@ -40,11 +40,8 @@ int cuda_l2_b200_grouped_bwd_nn(int variant, int config_id, const void* A, const
   using namespace b200;
   const tile_list::NNLibrary lib;
   if (!tile_list::holds(lib, variant)) return host::kBadConfig;
-  if (config_id < 0)
-    return tile_list::gemm(lib, GemmType(variant), A, B_rowmajor, C, Scales{nullptr, nullptr}, 0, offs, G, T, N, K,
-                           stream);
-  return tile_list::run(lib, GemmType(variant), config_id, A, B_rowmajor, C, Scales{nullptr, nullptr}, 0, offs, G, T, N,
-                        K, group_m, max_ctas, stream);
+  if (config_id < 0) return tile_list::gemm(lib, GemmType(variant), A, B_rowmajor, C, offs, G, T, N, K, stream);
+  return tile_list::run(lib, GemmType(variant), config_id, A, B_rowmajor, C, offs, G, T, N, K, group_m, max_ctas, stream);
 }
 
 // The K-grouped list: `count` = G matrices of `rows` = M rows by N columns, a reduction over K = T rows.
@@ -53,10 +50,8 @@ int cuda_l2_b200_grouped_bwd_wgrad(int variant, int config_id, const void* A, co
   using namespace b200;
   const tile_list::WgradLibrary lib;
   if (!tile_list::holds(lib, variant)) return host::kBadConfig;
-  if (config_id < 0)
-    return tile_list::gemm(lib, GemmType(variant), A, B, C, Scales{nullptr, nullptr}, 0, offs, G, M, N, T, stream);
-  return tile_list::run(lib, GemmType(variant), config_id, A, B, C, Scales{nullptr, nullptr}, 0, offs, G, M, N, T,
-                        group_m, max_ctas, stream);
+  if (config_id < 0) return tile_list::gemm(lib, GemmType(variant), A, B, C, offs, G, M, N, T, stream);
+  return tile_list::run(lib, GemmType(variant), config_id, A, B, C, offs, G, M, N, T, group_m, max_ctas, stream);
 }
 
 int cuda_l2_b200_grouped_bwd_nn_select(int variant, int G, int T, int N, int K, int* config_id, int* group_m) {

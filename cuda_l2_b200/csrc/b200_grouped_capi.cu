@@ -28,15 +28,14 @@ int b200_grouped_gemm(int variant, const void* A, const void* B_kmajor, void* C,
                       int K, void* stream) {
   using namespace b200;
   if (!tile_list::holds(tile_list::Library{}, variant)) return host::kBadConfig;
-  return tile_list::gemm(tile_list::Library{}, GemmType(variant), A, B_kmajor, C, Scales{nullptr, nullptr}, 0, offs, G,
-                         T, N, K, stream);
+  return tile_list::gemm(tile_list::Library{}, GemmType(variant), A, B_kmajor, C, offs, G, T, N, K, stream);
 }
 
 int b200_grouped_gemm_run_config(int variant, int config_id, const void* A, const void* B_kmajor, void* C,
                                  const int* offs, int G, int T, int N, int K, int group_m, int max_ctas, void* stream) {
   using namespace b200;
-  return tile_list::run(tile_list::Library{}, GemmType(variant), config_id, A, B_kmajor, C, Scales{nullptr, nullptr}, 0,
-                        offs, G, T, N, K, group_m, max_ctas, stream);
+  return tile_list::run(tile_list::Library{}, GemmType(variant), config_id, A, B_kmajor, C, offs, G, T, N, K, group_m,
+                        max_ctas, stream);
 }
 
 int b200_grouped_select(int variant, int G, int T, int N, int K, int* config_id, int* group_m) {

@@ -29,8 +29,8 @@ int b200_grouped_fp8_gemm(const void* A, const void* B_kmajor, void* C, const vo
                           const void* scale_b, int out_bf16, const int* offs, int G, int T, int N, int K, void* stream) {
   using namespace b200;
   if (!tile_list::known_out(out_bf16)) return host::kBadConfig;
-  return tile_list::gemm(tile_list::Library{}, tile_list::block_type(out_bf16), A, B_kmajor, C,
-                         tile_list::block_scales(scale_a, scale_b), ld_a, offs, G, T, N, K, stream);
+  return tile_list::gemm(tile_list::Library{}, tile_list::block_type(out_bf16), A, B_kmajor, C, offs, G, T, N, K, stream,
+                         tile_list::block_operands(scale_a, ld_a, scale_b));
 }
 
 int b200_grouped_fp8_gemm_run_config(int config_id, int out_bf16, const void* A, const void* B_kmajor, void* C,
@@ -38,8 +38,8 @@ int b200_grouped_fp8_gemm_run_config(int config_id, int out_bf16, const void* A,
                                      int N, int K, int group_m, int max_ctas, void* stream) {
   using namespace b200;
   if (!tile_list::known_out(out_bf16)) return host::kBadConfig;
-  return tile_list::run(tile_list::Library{}, tile_list::block_type(out_bf16), config_id, A, B_kmajor, C,
-                        tile_list::block_scales(scale_a, scale_b), ld_a, offs, G, T, N, K, group_m, max_ctas, stream);
+  return tile_list::run(tile_list::Library{}, tile_list::block_type(out_bf16), config_id, A, B_kmajor, C, offs, G, T, N,
+                        K, group_m, max_ctas, stream, tile_list::block_operands(scale_a, ld_a, scale_b));
 }
 
 int b200_grouped_fp8_select(int G, int T, int N, int K, int* config_id, int* group_m) {

@@ -7,47 +7,24 @@
 
 #include "hgemm_configs.cuh"
 #include "hgemm_dispatch.cuh"
-#include "swiglu_arith.cuh"
+#include "swiglu_backward.cuh"
 
 #ifndef B200_VARIANT
 #error "compile once per variant with -DB200_VARIANT=0 or 2"
 #endif
 
 namespace b200 {
-namespace grouped_swiglu {
+namespace tile_list {
 
-// Configuration `id` of variant T wrapped in Gated<Grouped<>>: h (C, may be null) and y over the groups of `offs`,
-// N = 2I. A configuration without a gated kernel is kBadConfig; T == 0 launches nothing.
-template <host::GemmType T>
-int run_config(int id, const void* x, const void* w, void* h, void* y, const int* offs, int G, int rows, int N, int K,
-               int group_m, int max_ctas, void* stream) {
-  constexpr host::GemmTypeTraits t = host::traits(T);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int st = host::kBadConfig;
-  switch (id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
-  case ID:                                                                                                     \
-    if constexpr (gated::has_kernel(ID))                                                                       \
-      st = host::launch_list<Gated<Grouped<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16()>>>>(         \
-          x, w, h, offs, G, rows, N, K, s, group_m, max_ctas, Scales{nullptr, nullptr}, 0, y);                 \
-    break;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      break;
-  }
-  if (st == host::kOk && rows > 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return st;
-}
+template <class Cfg>
+using GatedGrouped = Gated<Grouped<Cfg>>;
 
-#define B200_GROUPED_SWIGLU_RUN(T)                                                                           \
-  int run_config<T>(int, const void*, const void*, void*, void*, const int*, int, int, int, int, int, int, void*)
-extern template B200_GROUPED_SWIGLU_RUN(host::GemmType::kF16Acc32);
-extern template B200_GROUPED_SWIGLU_RUN(host::GemmType::kBF16);
-template B200_GROUPED_SWIGLU_RUN(host::GemmType(B200_VARIANT));
-#undef B200_GROUPED_SWIGLU_RUN
+// fp16 and bf16, both with fp32 accumulation
+#define B200_SWIGLU_TYPES(X, W) X(W, host::GemmType::kF16Acc32) X(W, host::GemmType::kBF16)
+B200_LIST_OBJECT(Library, GatedGrouped, B200_SWIGLU_TYPES);
+#undef B200_SWIGLU_TYPES
 
-}  // namespace grouped_swiglu
+}  // namespace tile_list
 }  // namespace b200
 
 #if B200_VARIANT == 0
@@ -55,28 +32,8 @@ template B200_GROUPED_SWIGLU_RUN(host::GemmType(B200_VARIANT));
 namespace b200 {
 namespace grouped_swiglu {
 
-constexpr int kBwdThreads = 256;
-constexpr int kBwdMaxCtas = 132 * 16;   // grid-stride beyond this: enough 16-byte requests in flight to fill HBM
-
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
-__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
-
-// One 16-byte vector of eight 16-bit values as fp32, and back (RN: the values are 16-bit values already)
-template <typename T>
-__device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
-  const T* e = reinterpret_cast<const T*>(&v);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) f[j] = to_f32(e[j]);
-}
-
-template <typename T>
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 v;
-  uint32_t* w = reinterpret_cast<uint32_t*>(&v);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) w[j] = ptx::pack_out_x2_rn<std::is_same_v<T, __nv_bfloat16>>(f[2 * j], f[2 * j + 1]);
-  return v;
-}
+using swiglu::kBwdMaxCtas;
+using swiglu::kBwdThreads;
 
 // The groups' last end as GroupCursor clamps them: end_g = clamp(offs[g], end_{g-1}, T) from end_{-1} = 0 is
 // min(max(0, offs[0], ..., offs[g]), T), so the last one is the largest offset clamped to [0, T]. Warp 0 of the block
@@ -95,48 +52,16 @@ __device__ __forceinline__ int groups_end(const int* __restrict__ offs, int G, i
   return s_end;
 }
 
-// dh = swiglu_grad(dy, h) for the rows below the groups' last end: one thread per eight consecutive columns of y (one
-// 16-byte vector of dy, of g, of u, of dg and of du), grid-stride over those rows' vectors. I % 64 == 0: the eight
-// columns lie in one 64-column gate / up block. The arithmetic is libb200_swiglu.so's backward, element for element.
+// dh = swiglu_grad(dy, h) for the rows below the groups' last end: libb200_swiglu.so's backward over those rows.
 template <typename T>
 __global__ void __launch_bounds__(kBwdThreads)
 grouped_swiglu_backward_kernel(const T* __restrict__ dy, const T* __restrict__ h, T* __restrict__ dh,
                                const int* __restrict__ offs, int G, int rows, int I) {
-  const int per_row = I / 8;
-  const long long vectors = (long long)groups_end(offs, G, rows) * per_row;
-  for (long long i = blockIdx.x * (long long)kBwdThreads + threadIdx.x; i < vectors;
-       i += (long long)gridDim.x * kBwdThreads) {
-    const long long row = i / per_row;
-    const int col = int(i - row * per_row) * 8;                      // y's column
-    const size_t hg = size_t(row) * 2 * I + size_t(col / 64) * 128 + col % 64, hu = hg + 64;
-    float d[8], g[8], u[8], dg[8], du[8];
-    unpack8<T>(__ldg(reinterpret_cast<const uint4*>(dy + size_t(row) * I + col)), d);
-    unpack8<T>(__ldg(reinterpret_cast<const uint4*>(h + hg)), g);
-    unpack8<T>(__ldg(reinterpret_cast<const uint4*>(h + hu)), u);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) swiglu_grad<T>(d[j], g[j], u[j], dg[j], du[j]);
-    *reinterpret_cast<uint4*>(dh + hg) = pack8<T>(dg);
-    *reinterpret_cast<uint4*>(dh + hu) = pack8<T>(du);
-  }
+  swiglu::backward_vectors(dy, h, dh, (long long)groups_end(offs, G, rows) * (I / 8), I);
 }
 
 inline bool known_variant(int variant) {
   return variant == int(host::GemmType::kF16Acc32) || variant == int(host::GemmType::kBF16);
-}
-
-// The shortest worst-case tile list (GroupCursor::max_tiles) of any configuration with a gated kernel: when it passes
-// INT_MAX, every configuration refuses the shape, so the dispatched call refuses it before the lookup. The list is
-// Grouped<>'s of the same configuration.
-inline long long fewest_tiles(int G, int T, int N) {
-  long long fewest = 0x7fffffffffffffffLL;
-#define B200_TILES(ID, BN, STAGES, CG, CM, CN, MR)                                                               \
-  if constexpr (gated::has_kernel(ID)) {                                                                        \
-    using W = Grouped<Config<BN, STAGES, CG, true, CM, CN, MR>>;                                                 \
-    fewest = std::min(fewest, W::Cursor::template max_tiles<W>(G, T, N));                                       \
-  }
-  B200_HGEMM_CONFIGS(B200_TILES)
-#undef B200_TILES
-  return fewest;
 }
 
 // The argument rules of the forward entry points, before any CUDA call.
@@ -150,23 +75,24 @@ int validate(int variant, const void* x, const void* w, const void* h, const voi
                  reinterpret_cast<uintptr_t>(y)) & 15))
     return host::kBadAlignment;
   if (reinterpret_cast<uintptr_t>(offs) & 3) return host::kBadAlignment;
-  if (fewest_tiles(G, T > 0 ? T : 1, 2 * I) > 0x7fffffffLL) return host::kBadShape;
+  // the shortest worst-case tile list of the gated configurations: past INT_MAX every configuration refuses the shape
+  if (tile_list::fewest_tiles<tile_list::GatedGrouped>(G, T > 0 ? T : 1, 2 * I) > 0x7fffffffLL) return host::kBadShape;
   return host::kOk;
 }
 
-// The grouped choice for (G, T, 2I, H) mapped to its gated sibling (the plain schedule is the only one of tile lists).
+// The grouped choice for (G, T, 2I, H) mapped to its gated sibling (tile_list::select).
 dispatch::Choice select(int variant, int G, int T, int I, int H) {
-  dispatch::Choice ch = tile_list::select<Grouped>(host::GemmType(variant), G, T, 2 * I, H);
-  ch.config_id = gated::sibling(ch.config_id);
-  ch.splits = 1;
-  return ch;
+  return tile_list::select<tile_list::GatedGrouped>(host::GemmType(variant), G, T, 2 * I, H);
 }
 
+// Configuration `config_id` of `variant` wrapped in Gated<Grouped<>>: h (may be null) and y over the groups of `offs`,
+// N = 2I. A configuration without a gated kernel is kBadConfig; T == 0 launches nothing.
 int run(int variant, int config_id, const void* x, const void* w, void* h, void* y, const int* offs, int G, int T,
         int I, int H, int group_m, int max_ctas, void* stream) {
-  if (variant == int(host::GemmType::kBF16))
-    return run_config<host::GemmType::kBF16>(config_id, x, w, h, y, offs, G, T, 2 * I, H, group_m, max_ctas, stream);
-  return run_config<host::GemmType::kF16Acc32>(config_id, x, w, h, y, offs, G, T, 2 * I, H, group_m, max_ctas, stream);
+  host::EpiOperands op;
+  op.y = y;
+  return tile_list::run(tile_list::Library{}, host::GemmType(variant), config_id, x, w, h, offs, G, T, 2 * I, H, group_m,
+                        max_ctas, stream, op);
 }
 
 template <typename T>
@@ -232,7 +158,8 @@ int cuda_l2_b200_grouped_swiglu_backward(int variant, const void* dy, const void
 }
 
 unsigned long long cuda_l2_b200_grouped_swiglu_launch_count(void) {
-  return b200::g_launches.load(std::memory_order_relaxed);
+  return b200::g_launches.load(std::memory_order_relaxed) +
+         b200::tile_list::g_list_launches.load(std::memory_order_relaxed);
 }
 
 const char* cuda_l2_b200_grouped_swiglu_strerror(int status) {

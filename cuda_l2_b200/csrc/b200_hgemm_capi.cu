@@ -164,33 +164,33 @@ int b200_hgemm_select(int acc_bits, int M, int N, int K, int* config_id, int* gr
 int b200_hgemm_run_config(int acc_bits, int config_id, const void* A, const void* B_kmajor, void* C, int M,
                           int N, int K, int group_m, int max_ctas, int splits, void* stream) {
   if (acc_bits == 32)
-    return b200::run_config<GemmType::kF16Acc32>(config_id, A, B_kmajor, C, {}, M, N, K, group_m, max_ctas, splits, stream);
+    return b200::run_config<GemmType::kF16Acc32>(config_id, A, B_kmajor, C, M, N, K, group_m, max_ctas, splits, stream);
   if (acc_bits == 16)
-    return b200::run_config<GemmType::kF16Acc16>(config_id, A, B_kmajor, C, {}, M, N, K, group_m, max_ctas, splits, stream);
+    return b200::run_config<GemmType::kF16Acc16>(config_id, A, B_kmajor, C, M, N, K, group_m, max_ctas, splits, stream);
   return b200::host::kBadConfig;
 }
 
 int b200_hgemm_f32acc(const void* A, const void* B_rowmajor, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
   if (!B_kmajor && B_rowmajor) return gemm_rowmajor<GemmType::kF16Acc32>(A, B_rowmajor, C, M, N, K, stream);
-  return b200::dispatch::gemm<GemmType::kF16Acc32>(A, B_kmajor, C, {}, M, N, K, stream);
+  return b200::dispatch::gemm<GemmType::kF16Acc32>(A, B_kmajor, C, M, N, K, stream);
 }
 
 int b200_hgemm_f16acc(const void* A, const void* B_rowmajor, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
   if (!B_kmajor && B_rowmajor) return gemm_rowmajor<GemmType::kF16Acc16>(A, B_rowmajor, C, M, N, K, stream);
-  return b200::dispatch::gemm<GemmType::kF16Acc16>(A, B_kmajor, C, {}, M, N, K, stream);
+  return b200::dispatch::gemm<GemmType::kF16Acc16>(A, B_kmajor, C, M, N, K, stream);
 }
 
 int b200_bgemm_f32acc(const void* A, const void* B_rowmajor, const void* B_kmajor, void* C, int M, int N,
                       int K, void* stream) {
   if (!B_kmajor && B_rowmajor) return gemm_rowmajor<GemmType::kBF16>(A, B_rowmajor, C, M, N, K, stream);
-  return b200::dispatch::gemm<GemmType::kBF16>(A, B_kmajor, C, {}, M, N, K, stream);
+  return b200::dispatch::gemm<GemmType::kBF16>(A, B_kmajor, C, M, N, K, stream);
 }
 
 int b200_bgemm_run_config(int config_id, const void* A, const void* B_kmajor, void* C, int M, int N, int K,
                           int group_m, int max_ctas, int splits, void* stream) {
-  return b200::run_config<GemmType::kBF16>(config_id, A, B_kmajor, C, {}, M, N, K, group_m, max_ctas, splits, stream);
+  return b200::run_config<GemmType::kBF16>(config_id, A, B_kmajor, C, M, N, K, group_m, max_ctas, splits, stream);
 }
 
 int b200_hgemm_host(int acc_bits, const void* hA, const void* hB_kmajor, void* hC, int M, int N, int K) {

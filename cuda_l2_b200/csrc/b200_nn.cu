@@ -11,14 +11,10 @@
 
 namespace b200 {
 
-#define B200_NN_RUN(T)                                                                                          \
-  int run_config<T, RowMajorB>(int, const void*, const void*, void*, Scales, int, int, int, int, int, int, void*, \
-                               int, host::ScratchFn, const void*, int, int)
-extern template B200_NN_RUN(host::GemmType::kF16Acc32);
-extern template B200_NN_RUN(host::GemmType::kF16Acc16);
-extern template B200_NN_RUN(host::GemmType::kBF16);
-template B200_NN_RUN(host::GemmType(B200_VARIANT));
-#undef B200_NN_RUN
+extern template B200_RUN(host::GemmType::kF16Acc32, RowMajorB);
+extern template B200_RUN(host::GemmType::kF16Acc16, RowMajorB);
+extern template B200_RUN(host::GemmType::kBF16, RowMajorB);
+template B200_RUN(host::GemmType(B200_VARIANT), RowMajorB);
 
 }  // namespace b200
 
@@ -30,14 +26,14 @@ extern "C" int cuda_l2_b200_nn_run_config(int variant, int config_id, const void
   using b200::RowMajorB;
   switch (variant) {
     case 0:
-      return b200::run_config<GemmType::kF16Acc32, RowMajorB>(config_id, A, B_rowmajor, C, {}, M, N, K, group_m,
-                                                              max_ctas, splits, stream, 0, scratch);
+      return b200::run_config<GemmType::kF16Acc32, RowMajorB>(config_id, A, B_rowmajor, C, M, N, K, group_m, max_ctas,
+                                                              splits, stream, {}, scratch);
     case 1:
-      return b200::run_config<GemmType::kF16Acc16, RowMajorB>(config_id, A, B_rowmajor, C, {}, M, N, K, group_m,
-                                                              max_ctas, splits, stream, 0, scratch);
+      return b200::run_config<GemmType::kF16Acc16, RowMajorB>(config_id, A, B_rowmajor, C, M, N, K, group_m, max_ctas,
+                                                              splits, stream, {}, scratch);
     case 2:
-      return b200::run_config<GemmType::kBF16, RowMajorB>(config_id, A, B_rowmajor, C, {}, M, N, K, group_m, max_ctas,
-                                                          splits, stream, 0, scratch);
+      return b200::run_config<GemmType::kBF16, RowMajorB>(config_id, A, B_rowmajor, C, M, N, K, group_m, max_ctas,
+                                                          splits, stream, {}, scratch);
     default:
       return b200::host::kBadConfig;
   }

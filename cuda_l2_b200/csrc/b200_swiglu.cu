@@ -6,48 +6,16 @@
 
 #include "hgemm_configs.cuh"
 #include "hgemm_dispatch.cuh"
-#include "swiglu_arith.cuh"
+#include "swiglu_backward.cuh"
 
 #ifndef B200_VARIANT
 #error "compile once per variant with -DB200_VARIANT=0 or 2"
 #endif
 
 namespace b200 {
-namespace swiglu {
-
-// Configuration `id` of variant T wrapped in Gated<>: h (C, may be null) and y, N = 2I. A configuration without a
-// gated kernel is kBadConfig.
-template <host::GemmType T>
-int run_config(int id, const void* x, const void* w, void* h, void* y, int M, int N, int K, int group_m, int max_ctas,
-               int splits, void* stream) {
-  constexpr host::GemmTypeTraits t = host::traits(T);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int st = host::kBadConfig;
-  switch (id) {
-#define B200_CASE(ID, BN, STAGES, CG, CM, CN, MR)                                                                  \
-  case ID:                                                                                                     \
-    if constexpr (gated::has_kernel(ID))                                                                       \
-      st = host::launch<Gated<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16()>>, gated::kModes>(        \
-          x, w, h, M, N, K, s, group_m, max_ctas, splits, Scales{nullptr, nullptr}, 0, host::splitk_scratch,   \
-          nullptr, kActNone, 0, y);                                                                            \
-    break;
-    B200_HGEMM_CONFIGS(B200_CASE)
-#undef B200_CASE
-    default:
-      break;
-  }
-  if (st == host::kOk) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return st;
-}
-
-#define B200_SWIGLU_RUN(T) \
-  int run_config<T>(int, const void*, const void*, void*, void*, int, int, int, int, int, int, void*)
-extern template B200_SWIGLU_RUN(host::GemmType::kF16Acc32);
-extern template B200_SWIGLU_RUN(host::GemmType::kBF16);
-template B200_SWIGLU_RUN(host::GemmType(B200_VARIANT));
-#undef B200_SWIGLU_RUN
-
-}  // namespace swiglu
+extern template B200_RUN(host::GemmType::kF16Acc32, Gated);
+extern template B200_RUN(host::GemmType::kBF16, Gated);
+template B200_RUN(host::GemmType(B200_VARIANT), Gated);
 }  // namespace b200
 
 #if B200_VARIANT == 0
@@ -55,49 +23,11 @@ template B200_SWIGLU_RUN(host::GemmType(B200_VARIANT));
 namespace b200 {
 namespace swiglu {
 
-constexpr int kBwdThreads = 256;
-constexpr int kBwdMaxCtas = 132 * 16;   // grid-stride beyond this: enough 16-byte requests in flight to fill HBM
-
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
-__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
-
-// One 16-byte vector of eight 16-bit values as fp32, and back (RN: the values are 16-bit values already)
-template <typename T>
-__device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
-  const T* e = reinterpret_cast<const T*>(&v);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) f[j] = to_f32(e[j]);
-}
-
-template <typename T>
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 v;
-  uint32_t* w = reinterpret_cast<uint32_t*>(&v);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) w[j] = ptx::pack_out_x2_rn<std::is_same_v<T, __nv_bfloat16>>(f[2 * j], f[2 * j + 1]);
-  return v;
-}
-
-// dh = swiglu_grad(dy, h): one thread per eight consecutive columns of y (one 16-byte vector of dy, of g, of u, of dg and
-// of du), grid-stride over the M * I / 8 vectors. I % 64 == 0: the eight columns lie in one 64-column gate / up block.
+// dh = swiglu_grad(dy, h) over all M rows, M * I / 8 vectors.
 template <typename T>
 __global__ void __launch_bounds__(kBwdThreads) swiglu_backward_kernel(const T* __restrict__ dy, const T* __restrict__ h,
                                                                        T* __restrict__ dh, long long vectors, int I) {
-  const int per_row = I / 8;
-  for (long long i = blockIdx.x * (long long)kBwdThreads + threadIdx.x; i < vectors;
-       i += (long long)gridDim.x * kBwdThreads) {
-    const long long row = i / per_row;
-    const int col = int(i - row * per_row) * 8;                      // y's column
-    const size_t hg = size_t(row) * 2 * I + size_t(col / 64) * 128 + col % 64, hu = hg + 64;
-    float d[8], g[8], u[8], dg[8], du[8];
-    unpack8<T>(__ldg(reinterpret_cast<const uint4*>(dy + size_t(row) * I + col)), d);
-    unpack8<T>(__ldg(reinterpret_cast<const uint4*>(h + hg)), g);
-    unpack8<T>(__ldg(reinterpret_cast<const uint4*>(h + hu)), u);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) swiglu_grad<T>(d[j], g[j], u[j], dg[j], du[j]);
-    *reinterpret_cast<uint4*>(dh + hg) = pack8<T>(dg);
-    *reinterpret_cast<uint4*>(dh + hu) = pack8<T>(du);
-  }
+  backward_vectors(dy, h, dh, vectors, I);
 }
 
 // The argument rules shared by the forward entry points, before any CUDA call.
@@ -121,11 +51,17 @@ dispatch::Choice select(int variant, int M, int I, int K) {
   return ch;
 }
 
+// Configuration `config_id` of `variant` wrapped in Gated<>: h (may be null) and y, N = 2I. A configuration without a
+// gated kernel is kBadConfig.
 int run(int variant, int config_id, const void* x, const void* w, void* h, void* y, int M, int I, int K, int group_m,
         int splits, int max_ctas, void* stream) {
+  host::EpiOperands op;
+  op.y = y;
   if (variant == int(host::GemmType::kBF16))
-    return run_config<host::GemmType::kBF16>(config_id, x, w, h, y, M, 2 * I, K, group_m, max_ctas, splits, stream);
-  return run_config<host::GemmType::kF16Acc32>(config_id, x, w, h, y, M, 2 * I, K, group_m, max_ctas, splits, stream);
+    return run_config<host::GemmType::kBF16, Gated>(config_id, x, w, h, M, 2 * I, K, group_m, max_ctas, splits, stream,
+                                                    op);
+  return run_config<host::GemmType::kF16Acc32, Gated>(config_id, x, w, h, M, 2 * I, K, group_m, max_ctas, splits,
+                                                      stream, op);
 }
 
 template <typename T>

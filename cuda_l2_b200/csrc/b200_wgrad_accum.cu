@@ -20,17 +20,13 @@ namespace b200 {
 template <class Cfg>
 using Accum1D1D = AccumF32<BlockScaled1D1D<Cfg>>;
 
-#define B200_ACCUM_RUN(T, W)                                                                                  \
-  int run_config<T, W>(int, const void*, const void*, void*, Scales, int, int, int, int, int, int, void*, int, \
-                       host::ScratchFn, const void*, int, int)
-extern template B200_ACCUM_RUN(host::GemmType::kE4M3F16, AccumF32);
-extern template B200_ACCUM_RUN(host::GemmType::kE4M3F16Block1D1D, Accum1D1D);
+extern template B200_RUN(host::GemmType::kE4M3F16, AccumF32);
+extern template B200_RUN(host::GemmType::kE4M3F16Block1D1D, Accum1D1D);
 #if B200_VARIANT == 3
-template B200_ACCUM_RUN(host::GemmType::kE4M3F16, AccumF32);
+template B200_RUN(host::GemmType::kE4M3F16, AccumF32);
 #elif B200_VARIANT == 7
-template B200_ACCUM_RUN(host::GemmType::kE4M3F16Block1D1D, Accum1D1D);
+template B200_RUN(host::GemmType::kE4M3F16Block1D1D, Accum1D1D);
 #endif
-#undef B200_ACCUM_RUN
 
 namespace tile_list {
 
@@ -60,17 +56,22 @@ b200::dispatch::Choice fp8_select(int form, int M, int N, int K) {
   return form == kFormRowwise ? b200::dispatch::select(GemmType::kE4M3F16, M, N, K) : b200::block::select(M, N, K);
 }
 
-int run_fp8(int form, int config_id, const void* A, const void* Bt, float* C32, const void* scale_a, int ld_a,
-            const void* scale_b, int ld_b, int M, int N, int K, int group_m, int max_ctas, int splits, void* stream) {
+// The epilogue operands of `form`: rowwise scales, or 1 x 128 scales of both operands with their row strides.
+b200::host::EpiOperands operands(int form, const void* scale_a, int ld_a, const void* scale_b, int ld_b) {
+  const b200::Scales sc{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b), form == kFormRowwise};
+  if (form == kFormRowwise) return {sc};
+  return {sc, ld_a, ld_b};
+}
+
+// Split-K scratch comes from this library's own pool (host::splitk_scratch, run_config's default).
+int run_fp8(int form, int config_id, const void* A, const void* Bt, float* C32, const b200::host::EpiOperands& op,
+            int M, int N, int K, int group_m, int max_ctas, int splits, void* stream) {
   using namespace b200;
-  const host::ScratchFn scratch = host::splitk_scratch;   // this library's own pool
-  const float* sa = static_cast<const float*>(scale_a);
-  const float* sb = static_cast<const float*>(scale_b);
   if (form == kFormRowwise)
-    return run_config<GemmType::kE4M3F16, AccumF32>(config_id, A, Bt, C32, Scales{sa, sb, true}, M, N, K, group_m,
-                                                    max_ctas, splits, stream, 0, scratch);
-  return run_config<GemmType::kE4M3F16Block1D1D, Accum1D1D>(config_id, A, Bt, C32, Scales{sa, sb}, M, N, K, group_m,
-                                                            max_ctas, splits, stream, ld_a, scratch, nullptr, 0, ld_b);
+    return run_config<GemmType::kE4M3F16, AccumF32>(config_id, A, Bt, C32, M, N, K, group_m, max_ctas, splits, stream,
+                                                    op);
+  return run_config<GemmType::kE4M3F16Block1D1D, Accum1D1D>(config_id, A, Bt, C32, M, N, K, group_m, max_ctas, splits,
+                                                            stream, op);
 }
 
 }  // namespace
@@ -83,10 +84,8 @@ int cuda_l2_b200_wgrad_accum_grouped(int variant, int config_id, const void* A, 
   using namespace b200;
   const tile_list::AccumWgradLibrary lib;
   if (!tile_list::holds(lib, variant)) return host::kBadConfig;
-  if (config_id < 0)
-    return tile_list::gemm(lib, GemmType(variant), A, B, C32, Scales{nullptr, nullptr}, 0, offs, G, M, N, T, stream);
-  return tile_list::run(lib, GemmType(variant), config_id, A, B, C32, Scales{nullptr, nullptr}, 0, offs, G, M, N, T,
-                        group_m, max_ctas, stream);
+  if (config_id < 0) return tile_list::gemm(lib, GemmType(variant), A, B, C32, offs, G, M, N, T, stream);
+  return tile_list::run(lib, GemmType(variant), config_id, A, B, C32, offs, G, M, N, T, group_m, max_ctas, stream);
 }
 
 int cuda_l2_b200_wgrad_accum_fp8(int form, int config_id, const void* A, const void* B_kmajor, float* C32,
@@ -94,11 +93,11 @@ int cuda_l2_b200_wgrad_accum_fp8(int form, int config_id, const void* A, const v
                                  int group_m, int max_ctas, int splits, void* stream) {
   using namespace b200;
   if (form != kFormRowwise && form != kForm1D1D) return host::kBadConfig;
+  const host::EpiOperands op = operands(form, scale_a, ld_a, scale_b, ld_b);
   if (config_id < 0) {
     // the argument rules before the lookup, which wants a valid shape
     const GemmType type = form == kFormRowwise ? GemmType::kE4M3F16 : GemmType::kE4M3F16Block1D1D;
-    const Scales sc{static_cast<const float*>(scale_a), static_cast<const float*>(scale_b), form == kFormRowwise};
-    if (const int st = host::validate(type, A, B_kmajor, C32, sc, M, N, K, ld_a)) return st;
+    if (const int st = host::validate(type, A, B_kmajor, C32, op, M, N, K)) return st;
     if (form == kForm1D1D && (ld_b < N || ld_b % 4)) return host::kBadScaleLdB;
     const dispatch::Choice ch = fp8_select(form, M, N, K);
     config_id = ch.config_id;
@@ -106,8 +105,7 @@ int cuda_l2_b200_wgrad_accum_fp8(int form, int config_id, const void* A, const v
     max_ctas = 0;
     splits = ch.splits;
   }
-  return run_fp8(form, config_id, A, B_kmajor, C32, scale_a, ld_a, scale_b, ld_b, M, N, K, group_m, max_ctas, splits,
-                 stream);
+  return run_fp8(form, config_id, A, B_kmajor, C32, op, M, N, K, group_m, max_ctas, splits, stream);
 }
 
 int cuda_l2_b200_wgrad_accum_grouped_select(int variant, int G, int T, int M, int N, int* config_id, int* group_m) {

@@ -190,16 +190,14 @@ using Unwrapped = Cfg;
 // translation unit of the library; hidden, so that no other shared object's copy is bound to it.
 __attribute__((visibility("hidden"))) inline std::atomic<unsigned long long> g_launches{0};
 
-// Launch configuration `id` of variant T in Wrapper (Unwrapped, BlockScaled, BlockScaled1D1D, RowMajorB or BiasAct),
-// with the block scales' ld_a, the split-K scratch source, BiasAct's bias and activation code, and BlockScaled1D1D's
-// ld_b, of host::launch. A configuration
-// without a kernel is kBadConfig. An instantiation
-// compiles the kernels of all configurations for T, so each translation unit of a library instantiates only the
-// variants it exports.
+// Launch configuration `id` of variant T in Wrapper (Unwrapped, BlockScaled, BlockScaled1D1D, RowMajorB, BiasAct,
+// AccumF32 or Gated), with the epilogue operands and the split-K scratch source of host::launch. A configuration
+// without a kernel is kBadConfig. An instantiation compiles the kernels of all configurations for T, so each translation
+// unit of a library instantiates only the variants it exports (B200_RUN).
 template <host::GemmType T, template <class> class Wrapper = Unwrapped>
-int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, int M, int N, int K, int group_m,
-               int max_ctas, int splits, void* stream, int ld_a = 0, host::ScratchFn scratch = host::splitk_scratch,
-               const void* bias = nullptr, int act = kActNone, int ld_b = 0) {
+int run_config(int id, const void* A, const void* Bt, void* C, int M, int N, int K, int group_m, int max_ctas,
+               int splits, void* stream, const host::EpiOperands& op = {},
+               host::ScratchFn scratch = host::splitk_scratch) {
   constexpr host::GemmTypeTraits t = host::traits(T);
   using Probe = Wrapper<Config<128, 6, 1, t.acc_f32, 1, 1, 1, t.bf16(), t.e4m3()>>;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -209,8 +207,7 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
   case ID:                                                                                                     \
     if constexpr (has_kernel<Probe>(ID))                                                                       \
       st = host::launch<Wrapper<Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16(), t.e4m3()>>,            \
-                        k_modes<Probe>()>(A, Bt, C, M, N, K, s, group_m, max_ctas, splits, scales, ld_a, scratch, \
-                                          bias, act, ld_b);                                                    \
+                        k_modes<Probe>()>(A, Bt, C, M, N, K, s, group_m, max_ctas, splits, op, scratch);   \
     break;
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE
@@ -221,19 +218,27 @@ int run_config(int id, const void* A, const void* Bt, void* C, Scales scales, in
   return st;
 }
 
+// The explicit instantiation of run_config<T, W>: a library compiled once per variant declares the other objects'
+// `extern template B200_RUN(T, W);` and instantiates its own with `template B200_RUN(T, W);`.
+#define B200_RUN(T, W)                                                                                        \
+  int run_config<T, W>(int, const void*, const void*, void*, int, int, int, int, int, int, void*,              \
+                       const host::EpiOperands&, host::ScratchFn)
+
 // The tile-list libraries (libb200_batched.so, libb200_grouped.so): the 16-bit variants 0, 1, 2 (the GemmType index) of
 // every configuration, wrapped in Wrapper (Batched or Grouped), launched by host::launch_list. libb200_batched_fp8.so,
 // libb200_grouped_fp8.so: the block-scaled e4m3 variants 5, 6 of the block-scaled configurations,
 // Wrapper<BlockScaled<...>>, with their scales. libb200_grouped_bwd.so: variants 0 and 2 of the configurations with a
-// row-major B kernel, wrapped in Grouped<RowMajorB<>> or GroupedK<RowMajorB<>>.
+// row-major B kernel, wrapped in Grouped<RowMajorB<>> or GroupedK<RowMajorB<>>. libb200_wgrad_accum.so:
+// AccumF32<GroupedK<RowMajorB<>>>. libb200_grouped_swiglu.so: the gated configurations in Gated<Grouped<>>.
 namespace tile_list {
 
 // The C entry points' selectors: a block-scaled library's `out_bf16` (0: fp16, 1: bf16 output) names GemmType
-// 5 + out_bf16, and its scales arrive as untyped pointers; the other libraries' `variant` is the GemmType index.
+// 5 + out_bf16, and its scales arrive as untyped pointers (block_operands: with the row stride of A's); the other
+// libraries' `variant` is the GemmType index.
 inline bool known_out(int out_bf16) { return out_bf16 == 0 || out_bf16 == 1; }
 inline host::GemmType block_type(int out_bf16) { return host::GemmType(int(host::GemmType::kE4M3F16Block) + out_bf16); }
-inline Scales block_scales(const void* a, const void* b) {
-  return Scales{static_cast<const float*>(a), static_cast<const float*>(b)};
+inline host::EpiOperands block_operands(const void* a, int ld_a, const void* b) {
+  return {Scales{static_cast<const float*>(a), static_cast<const float*>(b)}, ld_a};
 }
 
 // Kernel launches of the library that holds it (b200_batched_launch_count, b200_grouped_launch_count,
@@ -248,7 +253,7 @@ using Variant = std::conditional_t<host::traits(T).block, BlockScaled<Cfg>, Cfg>
 // A configuration without a kernel of Wrapper and T (has_kernel) returns kBadConfig.
 template <template <class> class Wrapper, host::GemmType T>
 int run_config(int id, const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
-               int group_m, int max_ctas, cudaStream_t s, Scales scales, int ld_a) {
+               int group_m, int max_ctas, cudaStream_t s, const host::EpiOperands& op) {
   constexpr host::GemmTypeTraits t = host::traits(T);
   static_assert(!t.scaled || t.block, "16-bit or block-scaled variants");
   using Probe = Wrapper<Variant<T, Config<128, 6, 1, t.acc_f32, 1, 1, 1, t.bf16(), t.e4m3()>>>;
@@ -258,7 +263,7 @@ int run_config(int id, const void* A, const void* Bt, void* C, const int* list, 
   case ID:                                                                                                     \
     if constexpr (has_kernel<Probe>(ID))                                                                       \
       st = host::launch_list<Wrapper<Variant<T, Config<BN, STAGES, CG, t.acc_f32, CM, CN, MR, t.bf16(), t.e4m3()>>>>( \
-          A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas, scales, ld_a);                               \
+          A, Bt, C, list, count, rows, N, K, s, group_m, max_ctas, op);                                        \
     break;
     B200_HGEMM_CONFIGS(B200_CASE)
 #undef B200_CASE
@@ -297,7 +302,7 @@ using ListProbe = Wrapper<Config<128, 6, 1, true>>;
 // kernels. The first variant's object also holds the C entry points.
 #define B200_LIST_RUN(W, T)                                                                                    \
   int run_config<W, T>(int, const void*, const void*, void*, const int*, int, int, int, int, int, int, cudaStream_t, \
-                       Scales, int)
+                       const host::EpiOperands&)
 #define B200_LIST_EXTERN(W, T) extern template B200_LIST_RUN(W, T);
 #define B200_LIST_ARG(W, T) , T
 #define B200_LIST_OBJECT(NAME, W, TYPES)                                                                       \
@@ -305,16 +310,16 @@ using ListProbe = Wrapper<Config<128, 6, 1, true>>;
   template B200_LIST_RUN(W, host::GemmType(B200_VARIANT));                                                     \
   using NAME = ListLibrary<W TYPES(B200_LIST_ARG, W)>
 
-// Configuration `config_id` of variant `type`, with the block scales and ld_a of a block-scaled variant (ignored by
-// the 16-bit ones). A variant that is not the library's own is kBadConfig.
+// Configuration `config_id` of variant `type`, with the epilogue operands of host::launch_list (a block-scaled
+// variant's scales and ld_a, Gated<Grouped<>>'s y). A variant that is not the library's own is kBadConfig.
 template <template <class> class Wrapper, host::GemmType... Types>
 int run(ListLibrary<Wrapper, Types...>, host::GemmType type, int config_id, const void* A, const void* Bt, void* C,
-        Scales scales, int ld_a, const int* list, int count, int rows, int N, int K, int group_m, int max_ctas,
-        void* stream) {
+        const int* list, int count, int rows, int N, int K, int group_m, int max_ctas, void* stream,
+        const host::EpiOperands& op = {}) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   int st = host::kBadConfig;
   (void)((type == Types && (st = run_config<Wrapper, Types>(config_id, A, Bt, C, list, count, rows, N, K, group_m,
-                                                            max_ctas, s, scales, ld_a), true)) || ...);
+                                                            max_ctas, s, op), true)) || ...);
   return st;
 }
 

@@ -202,17 +202,30 @@ inline const DeviceInfo& device_info() {
   return info;
 }
 
+// The operands of a launch besides A, Bt and C. Each configuration reads only those of its kind, and `{}` is a plain
+// 16-bit launch. Host code only: the kernels take their own argument types (Cfg::EpiArgs), which epilogue() builds.
+struct EpiOperands {
+  Scales scales{nullptr, nullptr};   // scaled variants: per-tensor or rowwise scales, or block scales (device memory)
+  int ld_a = 0;                      // block scales: the row stride of scales.a
+  int ld_b = 0;                      // BlockScaled1D1D<>: the row stride of Bt's 1 x 128 scales (scales.b)
+  const void* bias = nullptr;        // BiasAct<>: the bias (null, or N values of the output type) ...
+  int act = kActNone;                // ... and the activation code
+  void* y = nullptr;                 // Gated<>: y [rows, N / 2], 16-byte aligned
+};
+
 // The argument rules of a variant, checked before anything touches the device. TMA wants 16-byte row strides: A / Bt
 // rows hold K operand elements (K % 8 == 0 at two bytes, K % 16 == 0 at one byte), C rows N 16-bit elements. The scales
-// of a scaled variant are fp32 values in device memory: 4-byte aligned per tensor, 16-byte aligned vectors (M and N
-// values) rowwise, where the split-K reductions read the column scales as float4. Block scales: `a` 16-byte aligned (one
-// bulk copy per k-block) with ld_a >= M and ld_a % 4 == 0, `b` 4-byte aligned (1 x 128 scales of Bt: 16-byte aligned,
-// one bulk copy per k-block too; launch() checks their ld_b). Tile-list launches (launch_list):
-// batches >= 1 matrices, a tile list of at most INT_MAX `tiles`, and its device array `list` (a batched launch's
-// optional row counts) 4-byte aligned. Grouped launches (validate_grouped) pass their offsets as `list`.
-inline int validate(GemmType type, const void* A, const void* Bt, const void* C, Scales scales, int M, int N, int K,
-                    int ld_a = 0, int batches = 1, long long tiles = 1, const int* list = nullptr) {
+// (`op.scales`) of a scaled variant are fp32 values in device memory: 4-byte aligned per tensor, 16-byte aligned vectors
+// (M and N values) rowwise, where the split-K reductions read the column scales as float4. Block scales: `a` 16-byte
+// aligned (one bulk copy per k-block) with `op.ld_a` >= M and ld_a % 4 == 0, `b` 4-byte aligned (1 x 128 scales of Bt:
+// 16-byte aligned, one bulk copy per k-block too; validate_epilogue() checks their ld_b). Tile-list launches
+// (launch_list): batches >= 1 matrices, a tile list of at most INT_MAX `tiles`, and its device array `list` (a batched
+// launch's optional row counts) 4-byte aligned. Grouped launches (validate_grouped) pass their offsets as `list`.
+inline int validate(GemmType type, const void* A, const void* Bt, const void* C, const EpiOperands& op, int M, int N,
+                    int K, int batches = 1, long long tiles = 1, const int* list = nullptr) {
   const GemmTypeTraits& t = traits(type);
+  const Scales& scales = op.scales;
+  const int ld_a = op.ld_a;
   if (!A || !Bt || !C || (t.scaled && (!scales.a || !scales.b))) return kNullPointer;
   if (M <= 0 || N <= 0 || K <= 0 || batches < 1 || tiles > 0x7fffffffLL) return kBadShape;
   if (reinterpret_cast<uintptr_t>(list) & 3) return kBadAlignment;
@@ -449,44 +462,76 @@ inline bool pdl_enabled() {
   return on;
 }
 
-// One (configuration, K-mode) instance of the kernel: opt into its dynamic shared memory once, then launch.
-// Function attributes are per device AND per copy of the kernel: when two shared objects instantiate this template
-// (libb200_hgemm.so and a JIT-built hgemm_lib.so in one process), a function-local static may be merged across
-// them (STB_GNU_UNIQUE) while each object still launches its own kernel copy. Key on both.
+// The launch of a configuration: the maps, the plan, and the kernel's arguments, its last one (Cfg::EpiArgs) built by
+// epilogue().
+template <class Cfg>
 struct LaunchArgs {
   CUtensorMap ma, mb, mc;
   int M, N, K, group_m;
   Plan plan;
   float* ws; unsigned* ctr; __half* c;
   uint64_t hint_a, hint_b;
-  Scales scales;
-  int ld_a;             // block scales: the row stride of scales.a
-  int ld_b;             // 1 x 128 scales of Bt (BlockScaled1D1D<>): the row stride of scales.b
+  int ld_a;             // block scales: the row stride of scales.a (the kernel's aux_arg)
   int batches;          // batched kernels: the batch count ...
   const int* masked_m;  // ... and the row counts per batch (null: dense); grouped kernels: G and the offsets
   cudaStream_t stream;
-  const void* bias;     // BiasAct<> kernels: the bias (or null) ...
-  int act;              // ... and the activation code
-  GatedArgs gated;      // Gated<> kernels: y's map, and whether h (C) is stored
-  void* y;              // Gated<Grouped<>> kernels: y, for the boxes that straddle a group's end
+  typename Cfg::EpiArgs epi;
 };
 
-// The kernel's last argument: the scales, BiasAct<>'s BiasActArgs, BlockScaled1D1D<>'s Block1D1DArgs, AccumF32<>'s
-// AccumArgs (the wrapped kernel's argument and C, which is fp32), Gated<>'s GatedArgs or Gated<Grouped<>>'s
-// GroupedGatedArgs (GatedArgs and y).
-template <class Cfg>
-typename Cfg::EpiArgs epi_args(const LaunchArgs& a) {
-  if constexpr (is_gated<Cfg>() && grouped<Cfg>()) return GroupedGatedArgs{a.gated, static_cast<__half*>(a.y)};
-  else if constexpr (is_gated<Cfg>()) return a.gated;
-  else if constexpr (accum_f32<Cfg>())
-    return typename Cfg::EpiArgs{epi_args<typename Cfg::AccumBase>(a), reinterpret_cast<float*>(a.c)};
-  else if constexpr (bias_act<Cfg>()) return BiasActArgs{a.scales, a.bias, a.act};
-  else if constexpr (block_1d1d<Cfg>()) return Block1D1DArgs{a.scales, a.ld_b};
-  else return a.scales;
+// The argument rules of Cfg's epilogue operands around `base(C)`, the launch's own rules (validate or validate_list), in
+// this order: Gated<>'s y (non-null, then 16-byte aligned with N % 128 == 0: whole gate / up pairs), where a null h (C)
+// is checked as y; the base rules; BiasAct<>'s bias and activation code (validate_bias_act); BlockScaled1D1D<>'s ld_b.
+template <class Cfg, class BaseRules>
+int validate_epilogue(const EpiOperands& op, const void* C, int N, BaseRules&& base) {
+  if constexpr (is_gated<Cfg>()) {
+    if (!op.y) return kNullPointer;
+    if (!C) C = op.y;
+    if ((reinterpret_cast<uintptr_t>(op.y) & 15) || N % 128) return kBadAlignment;
+  }
+  if (const int st = base(C)) return st;
+  if constexpr (bias_act<Cfg>()) return validate_bias_act(op.bias, op.act);
+  if constexpr (block_1d1d<Cfg>()) {
+    if (op.ld_b < N || op.ld_b % 4) return kBadScaleLdB;
+  }
+  return kOk;
 }
 
+// C's map ([rows, N], `depth` matrices: 0 is a 2-D map), C itself and the kernel's last argument, after
+// validate_epilogue(): the scales, BiasAct<>'s BiasActArgs, BlockScaled1D1D<>'s Block1D1DArgs, AccumF32<>'s AccumArgs
+// (the wrapped kernel's argument and C, which is fp32), Gated<>'s GatedArgs (y's map, and whether h is stored: C is h,
+// and when it is null y stands in for it, whose map is then never written) or Gated<Grouped<>>'s GroupedGatedArgs
+// (GatedArgs and y).
+template <class Cfg>
+int epilogue(const EpiOperands& op, void* C, int rows, int N, int depth, MapCache& cache, LaunchArgs<Cfg>& a) {
+  constexpr Elem output = traits(gemm_type<Cfg>()).output;
+  if constexpr (is_gated<Cfg>()) {
+    const bool store_h = C != nullptr;
+    a.c = static_cast<__half*>(store_h ? C : op.y);
+    // h's map (y's when h is not stored) and y's, both in 64-column store boxes
+    int st = cache.get(a.c, rows, store_h ? N : N / 2, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output);
+    if (st != kOk || (st = cache.get(op.y, rows, N / 2, Cfg::EPI_ROWS, &a.epi.y_map, Cfg::EPI_N, output)) != kOk)
+      return st;
+    a.epi.store_h = store_h ? 1 : 0;
+    if constexpr (grouped<Cfg>()) a.epi.y = static_cast<__half*>(op.y);
+    return kOk;
+  } else {
+    a.c = static_cast<__half*>(C);
+    if constexpr (accum_f32<Cfg>() && block_1d1d<Cfg>())
+      a.epi = {Block1D1DArgs{op.scales, op.ld_b}, static_cast<float*>(C)};
+    else if constexpr (accum_f32<Cfg>()) a.epi = {op.scales, static_cast<float*>(C)};
+    else if constexpr (bias_act<Cfg>()) a.epi = BiasActArgs{op.scales, op.bias, op.act};
+    else if constexpr (block_1d1d<Cfg>()) a.epi = Block1D1DArgs{op.scales, op.ld_b};
+    else a.epi = op.scales;
+    return cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, depth);
+  }
+}
+
+// One (configuration, K-mode) instance of the kernel: opt into its dynamic shared memory once, then launch.
+// Function attributes are per device AND per copy of the kernel: when two shared objects instantiate this template
+// (libb200_hgemm.so and a JIT-built hgemm_lib.so in one process), a function-local static may be merged across
+// them (STB_GNU_UNIQUE) while each object still launches its own kernel copy. Key on both.
 template <class Cfg, int KMODE>
-int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
+int launch_mode(const DeviceInfo& di, const LaunchArgs<Cfg>& a) {
   static thread_local int attr_dev = -1;
   static thread_local const void* attr_fn = nullptr;
   constexpr auto kernel = kernel_of<Cfg, KMODE>();
@@ -545,13 +590,13 @@ int launch_mode(const DeviceInfo& di, const LaunchArgs& a) {
   const int splits_arg = kTileList ? a.batches : a.plan.splits;
   unsigned* ctr = kTileList ? reinterpret_cast<unsigned*>(const_cast<int*>(a.masked_m)) : a.ctr;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m, splits_arg, aux, a.ws,
-                                     ctr, a.c, a.hint_a, a.hint_b, epi_args<Cfg>(a));
+                                     ctr, a.c, a.hint_a, a.hint_b, a.epi);
   if (e != cudaSuccess && coop && pdl && e != cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
     coop_pdl_ok = false;               // the pair of attributes is not accepted here: cooperative only, from now on
     cfg.numAttrs = na - 1;
     e = cudaLaunchKernelEx(&cfg, kernel, a.ma, a.mb, a.mc, a.M, a.N, a.K, a.group_m, splits_arg, aux, a.ws, ctr, a.c,
-                           a.hint_a, a.hint_b, epi_args<Cfg>(a));
+                           a.hint_a, a.hint_b, a.epi);
   }
   return e == cudaSuccess ? kOk : int(e);
 }
@@ -563,53 +608,30 @@ constexpr int default_group_m() { return Cfg::CTA_GROUP == 2 ? 8 : 16; }
 // group_m <= 0 selects the default rasterisation width. max_ctas <= 0 means "all SMs". `splits`: 1 none, > 1 workspace
 // split-K, -2/-4/-8 cluster split-K, kStreamKTail / kStreamKTailPlusWave stream-K, as plan() grants it. MODES: bit
 // mask of the K-modes this call site may need (a per-shape translation unit names its one mode and so compiles two
-// kernels instead of four; the plain mode is always available as fallback). `scales`: the per-tensor or rowwise scales
-// of a scaled variant (device pointers), unused otherwise; `ld_a`: the row stride of block scales. RowMajorB<>
-// configurations read `Bt` as B [K, N] row-major. `scratch`: where the workspace of split-K and stream-K comes from.
-// BiasAct<> configurations: the bias (null, or N values of the output type) and the activation code. BlockScaled1D1D<>
-// configurations: `ld_b`, the row stride of Bt's 1 x 128 scales. Gated<> configurations: C is h [M, N] (null: not
-// stored) and `y` is y [M, N / 2], 16-byte aligned, with N % 128 == 0 (whole gate / up pairs).
+// kernels instead of four; the plain mode is always available as fallback). `op`: the operands the configuration's
+// epilogue reads (EpiOperands; validate_epilogue gives their rules): the scales of a scaled variant, the row stride of
+// block scales (`ld_a`) and of BlockScaled1D1D<>'s 1 x 128 scales of Bt (`ld_b`), BiasAct<>'s bias and activation code,
+// and Gated<>'s y [M, N / 2], for which C is h [M, N] (null: not stored). RowMajorB<> configurations read `Bt` as
+// B [K, N] row-major. `scratch`: where the workspace of split-K and stream-K comes from.
 template <class Cfg, unsigned MODES = 0xFu>
-int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream,
-           int group_m = 0, int max_ctas = 0, int splits = 1, Scales scales = Scales{nullptr, nullptr}, int ld_a = 0,
-           ScratchFn scratch = splitk_scratch, const void* bias = nullptr, int act = kActNone, int ld_b = 0,
-           void* y = nullptr) {
+int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStream_t stream, int group_m = 0,
+           int max_ctas = 0, int splits = 1, const EpiOperands& op = {}, ScratchFn scratch = splitk_scratch) {
   constexpr GemmType kType = gemm_type<Cfg>();
-  [[maybe_unused]] const bool store_h = C != nullptr;
-  if constexpr (is_gated<Cfg>()) {
-    if (!y) return kNullPointer;
-    if (!C) C = y;   // for the argument rules and tmap_c, which is then never written
-    if ((reinterpret_cast<uintptr_t>(y) & 15) || N % 128) return kBadAlignment;
-  }
-  int st = validate(kType, A, Bt, C, scales, M, N, K, ld_a);
+  int st = validate_epilogue<Cfg>(op, C, N, [&](const void* c) { return validate(kType, A, Bt, c, op, M, N, K); });
   if (st != kOk) return st;
-  if constexpr (bias_act<Cfg>()) {
-    if ((st = validate_bias_act(bias, act)) != kOk) return st;
-  }
-  if constexpr (block_1d1d<Cfg>()) {
-    if (ld_b < N || ld_b % 4) return kBadScaleLdB;
-  }
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
 
-  LaunchArgs a{};
+  LaunchArgs<Cfg> a{};
   MapCache& cache = map_cache();
-  const Elem operand = traits(kType).operand, output = traits(kType).output;
+  const Elem operand = traits(kType).operand;
   if ((st = cache.get(A, M, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, operand)) != kOk) return st;
   if constexpr (row_major_b<Cfg>()) {   // B [K, N]: boxes of 64 columns (one atom column) by this CTA's K slice
     if ((st = cache.get(Bt, K, N, Cfg::B_K_ROWS, &a.mb, 64, operand)) != kOk) return st;
   } else {
     if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, operand)) != kOk) return st;
   }
-  if constexpr (is_gated<Cfg>()) {
-    // h's map (y's when h is not stored: never written) and y's, both in 64-column store boxes
-    if ((st = cache.get(store_h ? C : y, M, store_h ? N : N / 2, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk)
-      return st;
-    if ((st = cache.get(y, M, N / 2, Cfg::EPI_ROWS, &a.gated.y_map, Cfg::EPI_N, output)) != kOk) return st;
-    a.gated.store_h = store_h ? 1 : 0;
-  } else {
-    if ((st = cache.get(C, M, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk) return st;
-  }
+  if ((st = epilogue<Cfg>(op, C, M, N, 0, cache, a)) != kOk) return st;
 
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = plan<Cfg, MODES>(M, N, K, splits, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
@@ -624,13 +646,8 @@ int launch(const void* A, const void* Bt, void* C, int M, int N, int K, cudaStre
   }
   a.M = M; a.N = N; a.K = K;
   a.group_m = group_m > 0 ? group_m : default_group_m<Cfg>();
-  a.c = static_cast<__half*>(C);
-  a.scales = scales;
-  a.ld_a = ld_a;
-  a.ld_b = ld_b;
+  a.ld_a = op.ld_a;
   a.stream = stream;
-  a.bias = bias;
-  a.act = act;
   // L2 eviction priorities: when one operand is streamed (about) once while the other is re-read by every tile row
   // or column and is small enough to live in L2, keep the small one and let the streamed one go first.
   a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
@@ -685,11 +702,10 @@ Plan list_plan(long long max_tiles, int K, int max_workers, ResidentClusters&& r
 // list (`worst_tiles`, GroupCursor::max_tiles) of at most INT_MAX tiles. Block-scaled e4m3: the block-scale rules with
 // M = T (at least one row: ld_a >= max(T, 1)).
 inline int validate_grouped(GemmType type, const void* A, const void* Bt, const void* C, const int* offs, int groups,
-                            int T, int N, int K, long long worst_tiles, Scales scales = Scales{nullptr, nullptr},
-                            int ld_a = 0) {
+                            int T, int N, int K, long long worst_tiles, const EpiOperands& op = {}) {
   if (!A || !Bt || !C || !offs) return kNullPointer;
   if (T < 0 || groups < 1) return kBadShape;
-  return validate(type, A, Bt, C, scales, T > 0 ? T : 1, N, K, ld_a, 1, worst_tiles, offs);
+  return validate(type, A, Bt, C, op, T > 0 ? T : 1, N, K, 1, worst_tiles, offs);
 }
 
 // The argument rules of a K-grouped launch (GroupedK<>): A [T, M], B [T, N] and C [G, M, N] with 16-byte rows (M % 8 and
@@ -701,16 +717,16 @@ inline int validate_k_grouped(GemmType type, const void* A, const void* B, const
   if (!C || !offs || (T != 0 && (!A || !B))) return kNullPointer;
   if (T < 0 || groups < 1) return kBadShape;
   if (T == 0) A = B = C;   // not read
-  return validate(type, A, B, C, Scales{nullptr, nullptr}, M, N, M, 0, 1, tiles, offs);
+  return validate(type, A, B, C, {}, M, N, M, 1, tiles, offs);
 }
 
 // The argument rules of a tile-list launch of Cfg's kind, with launch_list's arguments.
 template <class Cfg>
 int validate_list(GemmType type, const void* A, const void* Bt, const void* C, const int* list, int count, int rows,
-                  int N, int K, long long tiles, Scales scales, int ld_a) {
+                  int N, int K, long long tiles, const EpiOperands& op) {
   return k_grouped<Cfg>() ? validate_k_grouped(type, A, Bt, C, list, count, K, rows, N, tiles)
-         : grouped<Cfg>() ? validate_grouped(type, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a)
-                          : validate(type, A, Bt, C, scales, rows, N, K, ld_a, count, tiles, list);
+         : grouped<Cfg>() ? validate_grouped(type, A, Bt, C, list, count, rows, N, K, tiles, op)
+                          : validate(type, A, Bt, C, op, rows, N, K, count, tiles, list);
 }
 
 // One launch of a Batched<>, Grouped<> or GroupedK<> configuration, which walks the flat tile list of its Cfg::Cursor over
@@ -723,32 +739,27 @@ int validate_list(GemmType type, const void* A, const void* Bt, const void* C, c
 //   C [rows, N], contiguous; `list` (device memory, read by the kernel only): the cumulative group ends,
 //   end_g = clamp(list[g], start_g, rows) with start_0 = 0 and start_g = end_{g-1}. Every row of C below
 //   end_{count-1} is written once, by its own group; no other is written.
-//   Grouped<BlockScaled<>> (e4m3 operands): the same, with the block scales of the 2-D call over M = rows (`scales.a`,
-//   `ld_a`) and one [ceil(N/128), ceil(K/128)] matrix of Bt's scales per group (`scales.b`).
+//   Grouped<BlockScaled<>> (e4m3 operands): the same, with the block scales of the 2-D call over M = rows
+//   (`op.scales.a`, `op.ld_a`) and one [ceil(N/128), ceil(K/128)] matrix of Bt's scales per group (`op.scales.b`).
 //   Batched<BlockScaled<>> (e4m3 operands): the batched product, with one [ceil(K/128), ld_a] block of A's scales per
 //   matrix, stacked (value (b, m, kb) at scales.a[(b * ceil(K/128) + kb) * ld_a + m]), and one [ceil(N/128),
-//   ceil(K/128)] matrix of Bt's scales per batch (`scales.b`).
+//   ceil(K/128)] matrix of Bt's scales per batch (`op.scales.b`).
 //   Grouped<RowMajorB<>>: Grouped<>'s product with `Bt` read as B [count, K, N] row-major: C[start_g : end_g] =
 //   A[start_g : end_g] B[g].
 //   GroupedK<> (`rows` is M, `K` is T): C[g] = A[start_g : end_g]^T B[start_g : end_g] for g < count, A [T, M] and
 //   `Bt` as B [T, N] row-major, C [count, M, N], the groups as for Grouped<>. Every matrix of C is written, an empty
 //   group's with +0.0; T == 0 zero-fills C on the stream and launches nothing (a map needs at least one row).
 //   Gated<Grouped<>>: Grouped<>'s product h = C [rows, N] (null: not stored) with the SwiGLU epilogue, y [rows, N / 2]
-//   (`y`, 16-byte aligned, N % 128 == 0): the rows of y below the last group's end are written, each by its own group.
+//   (`op.y`, 16-byte aligned, N % 128 == 0): the rows of y below the last group's end are written, each by its own
+//   group.
 template <class Cfg>
 int launch_list(const void* A, const void* Bt, void* C, const int* list, int count, int rows, int N, int K,
-                cudaStream_t stream, int group_m = 0, int max_ctas = 0, Scales scales = Scales{nullptr, nullptr},
-                int ld_a = 0, void* y = nullptr) {
+                cudaStream_t stream, int group_m = 0, int max_ctas = 0, const EpiOperands& op = {}) {
   static_assert(batched<Cfg>() || grouped<Cfg>() || k_grouped<Cfg>(), "a Batched<>, Grouped<> or GroupedK<> configuration");
   constexpr GemmType kType = gemm_type<Cfg>();
   const long long tiles = Cfg::Cursor::template max_tiles<Cfg>(count, rows, N);
-  [[maybe_unused]] const bool store_h = C != nullptr;
-  if constexpr (is_gated<Cfg>()) {
-    if (!y) return kNullPointer;
-    if (!C) C = y;   // for the argument rules and tmap_c, which is then never written
-    if ((reinterpret_cast<uintptr_t>(y) & 15) || N % 128) return kBadAlignment;
-  }
-  int st = validate_list<Cfg>(kType, A, Bt, C, list, count, rows, N, K, tiles, scales, ld_a);
+  int st = validate_epilogue<Cfg>(
+      op, C, N, [&](const void* c) { return validate_list<Cfg>(kType, A, Bt, c, list, count, rows, N, K, tiles, op); });
   if (st != kOk || rows == 0) return st;
   const Elem elem = traits(kType).operand, output = traits(kType).output;
   if constexpr (k_grouped<Cfg>()) {
@@ -762,43 +773,31 @@ int launch_list(const void* A, const void* Bt, void* C, const int* list, int cou
   const DeviceInfo& di = device_info();
   if (di.cc_major != 9) return kNotHopper;
 
-  LaunchArgs a{};
+  LaunchArgs<Cfg> a{};
   MapCache& cache = map_cache();
   if constexpr (k_grouped<Cfg>()) {
-    // A [T, M] and B [T, N] in boxes of 64 columns (one atom column) by this CTA's K slice; C one M x N matrix per group
+    // A [T, M] and B [T, N] in boxes of 64 columns (one atom column) by this CTA's K slice
     if ((st = cache.get(A, K, rows, Cfg::A_K_ROWS, &a.ma, 64, elem)) != kOk) return st;
     if ((st = cache.get(Bt, K, N, Cfg::B_K_ROWS, &a.mb, 64, elem)) != kOk) return st;
-    if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, count)) != kOk) return st;
   } else {
-  // Bt is one N x K matrix per batch or group (row-major B: one K x N matrix per group, in atom-column boxes); A and C
-  // are one matrix per batch (3-D maps, so that TMA clips each box at its own matrix's edge), or the rows of all groups
-  // (2-D maps)
-  const int depth = batched<Cfg>() ? count : 0;
-  if ((st = cache.get(A, rows, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem, depth)) != kOk) return st;
-  if constexpr (row_major_b<Cfg>()) {
-    if ((st = cache.get(Bt, K, N, Cfg::B_K_ROWS, &a.mb, 64, elem, count)) != kOk) return st;
-  } else {
-    if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, count)) != kOk) return st;
-  }
-  if constexpr (is_gated<Cfg>()) {
-    // h's map (y's when h is not stored: never written) and y's, both in 64-column store boxes
-    if ((st = cache.get(store_h ? C : y, rows, store_h ? N : N / 2, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output)) != kOk)
+    // Bt is one N x K matrix per batch or group (row-major B: one K x N matrix per group, in atom-column boxes); A is
+    // one matrix per batch (a 3-D map, so that TMA clips each box at its own matrix's edge), or the rows of all groups
+    if ((st = cache.get(A, rows, K, Cfg::A_BOX_ROWS, &a.ma, Cfg::BLOCK_K, elem, batched<Cfg>() ? count : 0)) != kOk)
       return st;
-    if ((st = cache.get(y, rows, N / 2, Cfg::EPI_ROWS, &a.gated.y_map, Cfg::EPI_N, output)) != kOk) return st;
-    a.gated.store_h = store_h ? 1 : 0;
-    a.y = y;
-  } else {
-    if ((st = cache.get(C, rows, N, Cfg::EPI_ROWS, &a.mc, Cfg::EPI_N, output, depth)) != kOk) return st;
+    if constexpr (row_major_b<Cfg>()) {
+      if ((st = cache.get(Bt, K, N, Cfg::B_K_ROWS, &a.mb, 64, elem, count)) != kOk) return st;
+    } else {
+      if ((st = cache.get(Bt, N, K, Cfg::B_BOX_ROWS, &a.mb, Cfg::BLOCK_K, elem, count)) != kOk) return st;
+    }
   }
-  }
+  // C: one M x N matrix per group (K-grouped) or per batch, as A, or the rows of all groups
+  if ((st = epilogue<Cfg>(op, C, rows, N, k_grouped<Cfg>() || batched<Cfg>() ? count : 0, cache, a)) != kOk) return st;
   const int max_workers = (max_ctas > 0 ? max_ctas : di.num_sms) / Cfg::CLUSTER_CTAS;
   a.plan = list_plan<Cfg>(tiles, K, max_workers, [&] { return max_resident_clusters<Cfg>(di); });
   a.M = rows; a.N = N; a.K = K;
   a.group_m = group_m > 0 ? group_m : default_group_m<Cfg>();
-  a.c = static_cast<__half*>(C);
   a.hint_a = ptx::kL2EvictNormal; a.hint_b = ptx::kL2EvictNormal;
-  a.scales = scales;
-  a.ld_a = ld_a;
+  a.ld_a = op.ld_a;
   a.batches = count;
   a.masked_m = list;
   a.stream = stream;

@@ -19,8 +19,8 @@ REPO = Path(__file__).resolve().parent.parent
 GOLDEN = REPO / "tests" / "golden" / "gemm_sass_digest.json"
 CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
 # every library of cuda_l2_b200/build.py that holds GEMM kernels (the quantisers of libb200_quant.so are not among them)
-GEMM_LIBRARIES = ("capi", "fp8block", "batched", "grouped", "grouped_fp8", "batched_fp8", "nn", "grouped_bwd",
-                  "epilogue", "baselines")
+GEMM_LIBRARIES = ("capi", "fp8block", "fp8block_1d1d", "batched", "grouped", "grouped_fp8", "batched_fp8", "nn",
+                  "grouped_bwd", "epilogue", "wgrad_accum", "swiglu", "grouped_swiglu", "baselines")
 
 
 def _digest(text: str, marker: str) -> str:
